@@ -1,12 +1,19 @@
 #!/usr/bin/env python
-"""bench.py -- QPS of the Vamana batched search (BASELINE.json metric) on B200, one JSON line.
+"""bench.py -- QPS of the Vamana batched search (BASELINE.json metric) on H100, one JSON line.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 Workload (BASELINE.json configs[1], the configuration the metric is quoted on): synthetic 1M x 96-d
-float32, L2, Vamana search_window=128, batch = 10k queries, k = 10; graph built once per box by the
-reference's own CPU builder (oracle/_ref, R=64, window 128, alpha 1.2) and cached under /tmp.
+float32, L2, Vamana search_window=128, batch = 10k queries, k = 10; graph built by the library's own GPU
+builder (svsb200_build_vamana, R=64, window 128, alpha 1.2), every row's neighbours sorted by id, and cached
+in the temporary directory.  Both arms search that same cached graph; only the reference arm on a machine
+without a GPU falls back to the reference's CPU builder (oracle/_ref), and its `config.graph_builder` says so.
 A "step" = one full pass of the hot path over the 10k-query batch.
+
+--dump-outputs DIR writes what the timed path returned in its last timed step (ids.npy as float64,
+distances.npy as float32): the inputs are seeded and every graph row is sorted, so two builds of the project
+can be compared output for output.  Graphs built apart can differ in rare ties (ids at equal distance may
+change), so the line's `config.graph_sha1` names the graph that was searched.
 
 Lines printed (rank 0 only):
   value     whole-job QPS with queries/results resident in HBM (CUDA events, max over ranks)
@@ -21,6 +28,7 @@ import json
 import os
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -33,8 +41,8 @@ WORKLOADS = {
     # name: n, dim, dtype, metric, nq, k, window, max_degree, build window
     "c2-1Mx96-f32-L2-w128": dict(n=1_000_000, dim=96, dtype="float32", metric="l2", nq=10_000, k=10, window=128,
                                  max_degree=64, build_window=128, alpha=1.2),
-    # reduced-size stand-ins for BASELINE configs[2..4] (the full sizes need a GPU graph builder: the reference's
-    # CPU builder takes ~36 s per million 96-d vectors on the box's 16-core quota)
+    # reduced-size stand-ins for BASELINE configs[2..4]; every workload's graph comes from the GPU builder unless it
+    # names another (the reference's CPU builder needs minutes to hours at the larger sizes)
     "c3s-200kx768-f16-IP-w128": dict(n=200_000, dim=768, dtype="float16", metric="ip", nq=10_000, k=10, window=128,
                                      max_degree=64, build_window=128, alpha=0.95),
     "c4s-1Mx96-lvq8-L2-w128": dict(n=1_000_000, dim=96, dtype="float32", metric="l2", nq=10_000, k=10, window=128,
@@ -42,8 +50,7 @@ WORKLOADS = {
                                    graph_from="c2-1Mx96-f32-L2-w128"),
     "c5s-2Mx96-f16-L2-sharded": dict(n=2_000_000, dim=96, dtype="float16", metric="l2", nq=10_000, k=10, window=128,
                                      max_degree=64, build_window=128, alpha=1.2, sharded=True),
-    # BASELINE configs[2..4] at their stated sizes; graphs from the GPU builder (svsb200_build_vamana: the reference's
-    # CPU builder needs minutes to hours at these sizes) -- both arms then search that same graph
+    # BASELINE configs[2..4] at their stated sizes
     "c3-1Mx768-f16-IP-w128": dict(n=1_000_000, dim=768, dtype="float16", metric="ip", nq=10_000, k=10, window=128,
                                   max_degree=64, build_window=128, alpha=0.95, builder="gpu"),
     "c4-10Mx96-lvq8-L2-w128": dict(n=10_000_000, dim=96, dtype="float32", metric="l2", nq=10_000, k=10, window=128,
@@ -54,8 +61,8 @@ WORKLOADS = {
     "tiny-100kx96-f32-L2-w128": dict(n=100_000, dim=96, dtype="float32", metric="l2", nq=10_000, k=10, window=128,
                                      max_degree=64, build_window=128, alpha=1.2),
 }
-FALLBACK_HBM_GBS = 6650.0   # /opt/skills/guides/B200_PROFILING.md, used only without MEASURED_PEAKS.json
-FALLBACK_BF16_TFLOPS = 2250.0   # nominal dense bf16 (same guide), used only without MEASURED_PEAKS.json
+FALLBACK_HBM_GBS = 3350.0   # NVIDIA H100 SXM data sheet (700 W), used only without MEASURED_PEAKS.json
+FALLBACK_BF16_TFLOPS = 989.0   # same data sheet, dense bf16/fp16, used only without MEASURED_PEAKS.json
 
 
 def log(*a):
@@ -81,35 +88,70 @@ def dist_env():
 
 
 # ------------------------------------------------------------------------------------------------
-# workload: data + graph (cached per box under /tmp, rank 0 builds)
+# workload: data + graph (cached in the temporary directory, rank 0 builds)
 # ------------------------------------------------------------------------------------------------
-def build_graph_cached(tag, w, base, rank_builds, barrier):
-    """Vamana graph from the reference's own CPU builder (oracle/_ref), cached per box under /tmp."""
+def sort_rows(graph, chunk=1 << 20):
+    """Neighbours of every row in id order, in place (zero padding after them): the GPU builder adds reverse edges
+    with atomics, so their order within a row depends on thread timing.  Rows go in chunks, so that a multi-GB shard
+    graph needs no full-size temporaries."""
+    cols = np.arange(graph.shape[1] - 1)
+    for a in range(0, graph.shape[0], chunk):
+        rows = graph[a:a + chunk]
+        pad = cols[None, :] >= rows[:, :1]
+        nb = rows[:, 1:]
+        nb[pad] = 0xFFFFFFFF
+        nb.sort(axis=1)
+        nb[pad] = 0
+    return graph
+
+
+def graph_digest(graph, ep):
+    """Names the searched graph (entry point + rows) in the JSON line."""
+    h = hashlib.sha1(np.uint32(ep).tobytes())
+    h.update(memoryview(np.ascontiguousarray(graph, dtype=np.uint32)))
+    return h.hexdigest()[:16]
+
+
+def gpu_usable():
+    try:
+        from scalablevectorsearch_b200 import _lib
+        return _lib.lib().svsb200_device_count() > 0
+    except Exception:   # noqa: BLE001 -- no library or no driver: no GPU
+        return False
+
+
+def gpu_build(tag, w, base):
+    from scalablevectorsearch_b200 import DistanceType, VamanaBuildParameters, build_graph
+    t1 = time.time()
+    graph, ep = build_graph(base, {"l2": DistanceType.L2, "ip": DistanceType.MIP}[w["metric"]],
+                            VamanaBuildParameters(alpha=w["alpha"], graph_max_degree=w["max_degree"],
+                                                  window_size=w["build_window"]),
+                            device=int(os.environ.get("LOCAL_RANK", 0)))
+    log(f"GPU graph build {tag} n={base.shape[0]} dim={base.shape[1]} R={w['max_degree']}: {time.time() - t1:.1f} s, "
+        f"avg degree {graph[:, 0].mean():.1f}")
+    return sort_rows(np.ascontiguousarray(graph, dtype=np.uint32)), ep
+
+
+def graph_cache_path(tag, w):
     key = hashlib.sha1(json.dumps({k: w.get(k) for k in ("n", "dim", "dtype", "metric", "max_degree", "build_window",
                                                            "alpha", "builder")}, sort_keys=True).encode()).hexdigest()[:12]
-    cache = os.path.join(os.environ.get("SVSB200_CACHE", "/tmp/svsb200_cache"), f"graph_{tag}_{key}.npy")
+    return os.path.join(os.environ.get("SVSB200_CACHE") or os.path.join(tempfile.gettempdir(), "svsb200_cache"),
+                        f"graph_{tag}_{key}.npy")
+
+
+def build_graph_cached(tag, w, base, rank_builds, barrier):
+    """Vamana graph from w["builder"] (default "gpu": the library's GPU builder; "reference": the reference's own CPU
+    builder in oracle/_ref), cached in the temporary directory."""
+    w = dict(w, builder=w.get("builder", "gpu"))
+    cache = graph_cache_path(tag, w)
     if w.get("per_shard_data") and w.get("builder") == "gpu":
         # multi-GB shard graphs: built in place on this rank's GPU, never written to disk
-        from scalablevectorsearch_b200 import DistanceType, VamanaBuildParameters, build_graph
-        t1 = time.time()
-        graph, ep = build_graph(base, {"l2": DistanceType.L2, "ip": DistanceType.MIP}[w["metric"]],
-                                VamanaBuildParameters(alpha=w["alpha"], graph_max_degree=w["max_degree"],
-                                                      window_size=w["build_window"]),
-                                device=int(os.environ.get("LOCAL_RANK", 0)))
-        log(f"GPU graph build {tag} n={base.shape[0]} dim={base.shape[1]} R={w['max_degree']}: {time.time() - t1:.1f} s, "
-            f"avg degree {graph[:, 0].mean():.1f}")
+        graph, ep = gpu_build(tag, w, base)
         barrier()
         return ep, graph
     if rank_builds and not os.path.exists(cache) and w.get("builder") == "gpu":
-        from scalablevectorsearch_b200 import DistanceType, VamanaBuildParameters, build_graph
         os.makedirs(os.path.dirname(cache), exist_ok=True)
-        t1 = time.time()
-        graph, ep = build_graph(base, {"l2": DistanceType.L2, "ip": DistanceType.MIP}[w["metric"]],
-                                VamanaBuildParameters(alpha=w["alpha"], graph_max_degree=w["max_degree"],
-                                                      window_size=w["build_window"]),
-                                device=int(os.environ.get("LOCAL_RANK", 0)))
-        log(f"GPU graph build {tag} n={base.shape[0]} dim={base.shape[1]} R={w['max_degree']}: {time.time() - t1:.1f} s, "
-            f"avg degree {graph[:, 0].mean():.1f}")
+        graph, ep = gpu_build(tag, w, base)
         tmp = cache + f".tmp{os.getpid()}"
         with open(tmp, "wb") as f:
             np.save(f, np.concatenate([np.array([[ep] + [0] * w["max_degree"]], dtype=np.uint32), graph]))
@@ -117,8 +159,8 @@ def build_graph_cached(tag, w, base, rank_builds, barrier):
     if rank_builds and not os.path.exists(cache):
         from oracle.bindings import RefLib   # checker/baseline infrastructure: builds the graph only
         if not RefLib.available():
-            raise SystemExit("oracle/_ref/libsvsref.so is missing: run `python -c 'import __graft_entry__ as g; "
-                             "g.build()'` where /root/reference exists (the graph comes from the reference builder)")
+            raise SystemExit("oracle/_ref/libsvsref.so is missing: `python -c 'import __graft_entry__ as g; g.build()'` "
+                             "builds it where the reference sources are present (the graph comes from the reference builder)")
         os.makedirs(os.path.dirname(cache), exist_ok=True)
         t1 = time.time()
         threads = max(1, effective_cpus() // w.get("build_share", 1))
@@ -135,7 +177,9 @@ def build_graph_cached(tag, w, base, rank_builds, barrier):
     return int(blob[0, 0]), np.ascontiguousarray(blob[1:])
 
 
-def load_workload(name, rank, world, barrier):
+def load_workload(name, rank, world, barrier, reference_arm=False):
+    """Data, queries and the one graph both arms search.  Only the reference arm, on a machine with neither a GPU nor
+    a cached GPU-built graph, takes the reference's CPU builder instead (`config.graph_builder` says which)."""
     from scalablevectorsearch_b200.synthetic import clustered_unit_vectors
     w = WORKLOADS[name]
     t0 = time.time()
@@ -143,13 +187,19 @@ def load_workload(name, rank, world, barrier):
     if w["dtype"] == "float16":
         base = base.astype(np.float16)
     gname = w.get("graph_from", name)
-    ep, graph = build_graph_cached(gname, WORKLOADS[gname], base, rank == 0, barrier)
-    log(f"rank {rank}: workload {name} ready in {time.time() - t0:.1f} s (entry point {ep})")
+    gw = dict(WORKLOADS[gname])
+    gw.setdefault("builder", "gpu")
+    if (reference_arm and gw["builder"] == "gpu" and not os.path.exists(graph_cache_path(gname, gw))
+            and not gpu_usable()):
+        gw["builder"] = "reference"
+    ep, graph = build_graph_cached(gname, gw, base, rank == 0, barrier)
+    w = dict(w, graph_builder=gw["builder"], graph_sha1=graph_digest(graph, ep))
+    log(f"rank {rank}: workload {name} ready in {time.time() - t0:.1f} s (entry point {ep}, graph {w['graph_sha1']})")
     return w, base, queries, graph, ep
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons during the timed region, and the card's name and power limit."""
     FIELDS = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
               "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
               "clocks_event_reasons.sw_power_cap")
@@ -179,13 +229,18 @@ class ClockSampler:
             self.thread.join(timeout=2)
 
     def summary(self):
+        try:
+            card = subprocess.run(["nvidia-smi", f"--id={self.gpu}", "--query-gpu=name,power.limit",
+                                   "--format=csv,noheader"], capture_output=True, text=True, timeout=30).stdout.strip()
+        except (OSError, subprocess.SubprocessError):
+            card = None
         sm = [float(r[0]) for r in self.rows if len(r) >= 7 and r[0].replace(".", "").isdigit()]
         if not sm:
-            return {"sm_mhz": None, "sm_max_mhz": None, "reasons": [], "samples": 0}
+            return {"sm_mhz": None, "sm_max_mhz": None, "reasons": [], "samples": 0, "gpu": card}
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         reasons = [n for i, n in enumerate(names) if any(r[3 + i].startswith("Active") for r in self.rows if len(r) >= 7)]
         return {"sm_mhz": float(np.median(sm)), "sm_max_mhz": float(self.rows[0][1]), "reasons": reasons,
-                "samples": len(sm)}
+                "samples": len(sm), "gpu": card}
 
 
 def algorithmic_bytes(hops, evals, rows_read, w, row_bytes, qbytes):
@@ -220,7 +275,7 @@ def run_reference(args):
     rank, _, world = dist_env()
     if rank != 0:
         return
-    w, base, queries, graph, ep = load_workload(args.workload, 0, 1, lambda: None)
+    w, base, queries, graph, ep = load_workload(args.workload, 0, 1, lambda: None, reference_arm=True)
     if args.window:
         w = dict(w, window=args.window)
     threads = effective_cpus()
@@ -256,8 +311,9 @@ def run_config(name, w, graph, gpus, weak):
 def workload_config(name, w, graph):
     return {"workload": name, "n": w["n"], "dim": w["dim"], "base_dtype": w["dtype"], "distance": w["metric"],
             "batch": w["nq"], "k": w["k"], "search_window": w["window"], "graph_max_degree": w["max_degree"],
-            "graph_avg_degree": round(float(graph[:, 0].mean()), 2),
-            "l2_policy": "index (vectors+graph) is several times larger than the 126 MB L2; no explicit flush"}
+            "graph_avg_degree": round(float(graph[:, 0].mean()), 2), "graph_builder": w["graph_builder"],
+            "graph_sha1": w["graph_sha1"],
+            "l2_policy": "index (vectors+graph) is several times larger than the 50 MB L2; no explicit flush"}
 
 
 # ------------------------------------------------------------------------------------------------
@@ -441,7 +497,7 @@ def run_ours(args):
         if os.path.exists(peaks_path):
             peak, peak_src = float(json.load(open(peaks_path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         else:
-            peak, peak_src = FALLBACK_HBM_GBS, "fallback (B200_PROFILING.md)"
+            peak, peak_src = FALLBACK_HBM_GBS, "fallback (H100 SXM data sheet)"
         achieved = total_bytes / (kern_ms * 1e-3) / 1e9 / world   # per-GPU GB/s of the search kernel
         ref_achieved = total_ref_bytes / (kern_ms * 1e-3) / 1e9 / world
         nofilter_achieved = total_ref_bytes / (nofilter * 1e-3) / 1e9 / world
@@ -476,7 +532,7 @@ def run_ours(args):
             tf_peak = (float(json.load(open(peaks_path)).get("bf16_tflops", FALLBACK_BF16_TFLOPS))
                        if os.path.exists(peaks_path) else FALLBACK_BF16_TFLOPS)
             tflops = 2.0 * sample * w["n"] * w["dim"] / (gt_ms * 1e-3) / 1e12
-            ground_truth = {"kernel": "flat_gemm_topk_kernel (tcgen05 fp16 x fp16 -> fp32, fused top-k) + exact rescore",
+            ground_truth = {"kernel": "flat_gemm_topk_kernel (wgmma fp16 x fp16 -> fp32, fused top-k) + exact rescore",
                             "queries": sample, "ms": gt_ms, "tflops_whole_call": tflops, "peak_tflops": tf_peak,
                             "frac_of_bf16_peak": tflops / tf_peak, "queries_sent_to_exact_scan": int(fb),
                             "note": "whole svsb200_flat_search_device call (GEMM + per-tile top-k + bit-exact rescoring + "
@@ -555,9 +611,18 @@ def run_ours(args):
             "clocks": clocks.summary(),
         }
         print(json.dumps(line), flush=True)
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, ids_all, d_all)
     if world > 1:
         dist.barrier()
         dist.destroy_process_group()
+
+
+def dump_outputs(directory, ids, dists):
+    """What the timed path returned in its last timed step: ids (exact in float64) and distances (float32)."""
+    os.makedirs(directory, exist_ok=True)
+    np.save(os.path.join(directory, "ids.npy"), ids.cpu().numpy().astype(np.float64))
+    np.save(os.path.join(directory, "distances.npy"), dists.cpu().numpy().astype(np.float32))
 
 
 def run_sharded(args):
@@ -650,11 +715,14 @@ def run_sharded(args):
             "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
             "config": {"workload": args.workload, "n": w["n"], "shards": total_shards, "shards_in_this_run": world,
                        "rows_per_shard": hi - lo, "graph_seconds_rank0": round(t_build, 1),
-                       "graph_builder": w.get("builder", "reference cpu"), "dim": w["dim"], "base_dtype": w["dtype"],
+                       "graph_sha1_rank0": graph_digest(graph, ep),
+                       "graph_builder": w.get("builder", "gpu"), "dim": w["dim"], "base_dtype": w["dtype"],
                        "distance": w["metric"], "batch": nq, "k": k, "search_window": w["window"],
                        "parallelism": f"index sharded x{world} (own graph per shard), NCCL all-gather + TotalOrder merge"},
             "matches_reference_per_shard_plus_merge": ok, "checked_queries": ns, "recall_at_10": round(recall, 4)}),
             flush=True)
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, ids, d)
     if world > 1:
         dist.barrier()
         dist.destroy_process_group()
@@ -683,6 +751,8 @@ def main():
                          "result as `value` and the weak one under `weak` in the same line)")
     ap.add_argument("--cpu-sample", dest="cpu_sample", type=int, default=0,
                     help="cpu_baseline: time only the first N queries of the batch (bounded sample for big workloads)")
+    ap.add_argument("--dump-outputs", dest="dump_outputs", default=None, metavar="DIR",
+                    help="write the timed path's results of its last timed step as DIR/<name>.npy")
     args = ap.parse_args()
     if WORKLOADS[args.workload].get("sharded"):
         run_sharded(args)

@@ -1,4 +1,4 @@
-/* svsb200.h -- C ABI of libsvsb200.so: the B200-native Vamana batched-search hot path.
+/* svsb200.h -- C ABI of libsvsb200.so: the H100-native Vamana batched-search hot path.
  *
  * This is the drop-in boundary for the reference's Vamana search (SURVEY.md §8b).  Each
  * entry point names the reference interface it replaces (file:line relative to
@@ -10,7 +10,7 @@
  *   * every function returns 0 on success, non-zero on failure; svsb200_last_error()
  *     gives the message for the calling thread (the C++ adapter rethrows it as
  *     svs::ANNException, matching include/svs/lib/exception.h);
- *   * there is no CPU fallback: if no sm_100-class device is usable, create/search fail;
+ *   * there is no CPU fallback: if no sm_90-class device is usable, create/search fail;
  *   * "host" pointers may be pageable or pinned; "device" pointers must live on the
  *     index's device;
  *   * ids are the reference's internal uint32 ids (core/graph/graph.h:388) widened to
@@ -255,7 +255,7 @@ int svsb200_flat_plan(size_t nq, size_t n, int sm_count, uint32_t* ctas, uint32_
 
 /* Exact exhaustive (flat) search on the tensor cores.  Replaces: svs::Flat / FlatIndex::search
  * (include/svs/index/flat/flat.h:159,421-465): top-k of every query against all `n` base vectors inside `index`.
- * A query-tile x base-tile fp16 GEMM (tcgen05 / TMEM, operands staged by bulk copies) selects candidates, the
+ * A query-tile x base-tile fp16 GEMM (wgmma, operands staged by bulk copies) selects candidates, the
  * candidates are re-scored with the graph search's own bit-exact distance code, and an error bound on the fp16
  * products proves per query that no other vector can belong to the top k; queries that fail the proof are
  * re-run by the exact scan.  The result therefore always equals svsb200_exhaustive_device bit for bit (ids and

@@ -1,4 +1,4 @@
-"""scalablevectorsearch_b200 -- B200-native Vamana batched search behind the SVS interface.
+"""scalablevectorsearch_b200 -- H100-native Vamana batched search behind the SVS interface.
 
 Only the hot path of SURVEY.md §8 lives here: ``csrc/`` (CUDA kernels + C ABI -> ``libsvsb200.so``),
 the host-side mirror of the reference's search interface (:mod:`.vamana`), and the file formats

@@ -1,7 +1,7 @@
 """ctypes binding of ``libsvsb200.so`` (the C ABI in ``include/svsb200.h``).
 
 The library is CUDA-only.  There is deliberately no fallback: if the shared object is
-missing or no sm_100-class device is usable, importing succeeds but every operation raises.
+missing or no sm_90-class device is usable, importing succeeds but every operation raises.
 """
 from __future__ import annotations
 

@@ -5,7 +5,7 @@
 // `search` is the batched GPU search (optionally through an IDFilter evaluated on the device as a bitmap),
 // `range_search` grows the result lists until they leave the radius.  It stands where the reference's
 // libsvs_runtime implementation sits (bindings/cpp/src/vamana_index.cpp, vamana_index_impl.h:60-330): a program
-// written against the runtime header links this object instead and runs on the B200.
+// written against the runtime header links this object instead and runs on the H100.
 //
 // Compiles against the reference's runtime *headers* only (no svs core headers); the few out-of-line members of the
 // header types that live in libsvs_runtime (Status message storage, the VamanaIndex destructor / static factories)

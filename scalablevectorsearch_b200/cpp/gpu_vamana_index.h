@@ -185,7 +185,7 @@ class GpuVamanaIndex : public svs::index::vamana::VamanaIndex<Graph, Data, Dist>
     /// Devices holding a replica ("threadpool -> CUDA streams": every calling thread gets its own stream).
     size_t num_devices() const { return svsb200_index_num_devices(handle_.get()); }
 
-    std::string name() const { return "GpuVamanaIndex (libsvsb200, sm_100a)"; }
+    std::string name() const { return "GpuVamanaIndex (libsvsb200, sm_90a)"; }
     svsb200_index* native_handle() const { return handle_.get(); }
 
   private:

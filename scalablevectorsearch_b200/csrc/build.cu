@@ -185,7 +185,7 @@ extern "C" int svsb200_build_vamana(const void* vectors, int dtype, size_t n, si
     cudaDeviceProp prop;
     if (cudaSetDevice(device) != cudaSuccess || cudaGetDeviceProperties(&prop, device) != cudaSuccess)
         return set_error("svsb200_build_vamana: cannot select the device");
-    if (prop.major != 10 || prop.minor != 0) return set_error("svsb200_build_vamana: device is not sm_100");
+    if (prop.major != 9 || prop.minor != 0) return set_error("svsb200_build_vamana: device is not sm_90");
 
     const size_t es = dtype == SVSB200_F32 ? 4 : 2;
     const size_t row_bytes = dim * es;

@@ -1,4 +1,4 @@
-// common.cuh -- shared definitions for libsvsb200 (sm_100a only).
+// common.cuh -- shared definitions for libsvsb200 (sm_90a only).
 #pragma once
 
 #include <cuda_runtime.h>

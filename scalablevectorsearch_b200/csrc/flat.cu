@@ -1,4 +1,4 @@
-// flat.cu -- exhaustive (flat) search on the 5th-generation tensor cores (SURVEY.md §8 f2).
+// flat.cu -- exhaustive (flat) search on the Hopper tensor cores (SURVEY.md §8 f2).
 //
 // Replaces, for ground truth and re-ranking: svs::Flat / FlatIndex::search
 // (include/svs/index/flat/flat.h:159,421-465) -- the one place on this path where a query block x base block
@@ -6,13 +6,12 @@
 // scan with the search path's distance code, ties by id):
 //
 //   1. flat_gemm_topk_kernel: S = Q . X^T in fp16 with fp32 accumulation.  One CTA per (128-query tile, range of
-//      256-row base tiles); operands are pre-tiled in HBM in the UMMA canonical K-major layout (8x8 core matrices,
-//      no swizzle) so that every k-block of a tile is one contiguous blob moved by ONE `cp.async.bulk`
-//      (SASS UBLKCP) into a 5-stage shared-memory ring signalled through mbarriers; a single elected thread
-//      issues `tcgen05.mma.cta_group::1.kind::f16` (SASS UTCHMMA, M=128 N=256 K=16) into a double-buffered
-//      256-column TMEM accumulator; four epilogue warps read their 32 TMEM lanes with `tcgen05.ld` (SASS LDTM),
-//      turn scores into keys (|x|^2 - 2 q.x for L2, -q.x for inner product) and keep, per query, the KC smallest
-//      keys seen in this CTA's base range.
+//      256-row base tiles); operands are pre-tiled in HBM in the canonical K-major layout of the warpgroup MMA
+//      (8x8 core matrices, no swizzle) so that every k-block of a tile is one contiguous blob moved by ONE
+//      `cp.async.bulk` into a 6-stage shared-memory ring signalled through mbarriers by a producer warp.  Two
+//      consumer warpgroups each issue `wgmma.mma_async.m64n256k16.f32.f16.f16` on 64 of the tile's 128 query rows,
+//      keep the 64 x 256 fp32 accumulator in registers, turn scores into keys (|x|^2 - 2 q.x for L2, -q.x for
+//      inner product) and keep, per query, the KC smallest keys seen in this CTA's base range.
 //   2. flat_rescore_kernel: every candidate of a query (all ranges) is re-scored with the search path's own
 //      bit-exact distance code (eval_pass) and the k best by (key, id) are written out.
 //   3. verification: fp16 rounding moves a key by at most E(q) (derived below); a base row that is NOT a
@@ -70,35 +69,57 @@ __device__ __forceinline__ void bulk_copy_g2s(void* smem_dst, const void* gmem_s
                  "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar))
                  : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving reads of an accumulator register across the wait that completes it
+__device__ __forceinline__ void reg_fence(float& r) { asm volatile("" : "+f"(r)::"memory"); }
+// Warpgroup-MMA shared-memory matrix descriptor, K-major, no swizzle (layout type 0): 8x8-element core matrices of
+// 128 contiguous bytes; LBO = byte distance between the two 8-element k-chunks of one K=16 MMA, SBO = byte distance
+// between 8-row groups.
+__device__ __forceinline__ uint64_t wgmma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+    return uint64_t((smem_addr >> 4) & 0x3FFFu) | (uint64_t((lbo_bytes >> 4) & 0x3FFFu) << 16) |
+           (uint64_t((sbo_bytes >> 4) & 0x3FFFu) << 32);
 }
-__device__ __forceinline__ void tc_mma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+// D (64 x 256, fp32, in registers) [+]= A (64 x 16) . B (256 x 16)^T, both fp16 K-major in shared memory.
+__device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
     asm volatile(
         "{\n\t"
         ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
+        "setp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+        "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+        "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+        "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+        "%128, %129, p, 1, 1, 0, 0;\n\t"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+          "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+          "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+          "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+          "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+          "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+          "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+          "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+          "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-// UMMA shared-memory matrix descriptor, K-major, no swizzle (cute/arch/mma_sm100_desc.hpp SmemDescriptor): 8x8-element
-// core matrices of 128 contiguous bytes; LBO = byte distance between the two 8-element k-chunks of one K=16 MMA,
-// SBO = byte distance between 8-row groups.
-__device__ __forceinline__ uint64_t umma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    return uint64_t((smem_addr >> 4) & 0x3FFFu) | (uint64_t((lbo_bytes >> 4) & 0x3FFFu) << 16) |
-           (uint64_t((sbo_bytes >> 4) & 0x3FFFu) << 32) | (uint64_t(1) << 46);
-}
-// Instruction descriptor (InstrDescriptor): D = F32, A = B = F16, both K-major, N >> 3 at bit 17, M >> 4 at bit 24.
-constexpr uint32_t kFlatIdesc = (1u << 4) | ((FLAT_BN >> 3) << 17) | ((FLAT_BM >> 4) << 24);
-
-// Per-query list of the FLAT_KC smallest keys: shared memory, [query row][FLAT_KC] with FLAT_KC odd, so that both a
-// lane walking its own row and a warp reading one row side by side are bank-conflict free.  Keys are stored as
-// order-preserving unsigned integers (REDUX.MAX works on them); a list starts full of +inf / no-id entries, so there
-// is no fill count -- an update always replaces the current maximum, and the row's threshold is the new maximum.
+// Per-query list of the FLAT_KC smallest keys: shared memory, [query row][FLAT_KC] with FLAT_KC odd, so that a warp
+// reading one row side by side is bank-conflict free.  Keys are stored as order-preserving unsigned integers
+// (REDUX.MAX works on them); a list starts full of +inf / no-id entries, so there is no fill count -- an update always
+// replaces the current maximum, and the row's threshold is the new maximum.
 static_assert(FLAT_KC % 2 == 1 && FLAT_KC > 32 && FLAT_KC <= 64, "list layout");
 __device__ __forceinline__ uint32_t flat_ord(float f) {
     const uint32_t u = __float_as_uint(f);
@@ -107,8 +128,7 @@ __device__ __forceinline__ uint32_t flat_ord(float f) {
 __device__ __forceinline__ float flat_unord(uint32_t o) {
     return __uint_as_float(o ^ ((o >> 31) ? 0x80000000u : 0xFFFFFFFFu));
 }
-// The whole warp updates the list of row `warp_row0 + src` with (key, id) broadcast from lane `src`; returns the row's
-// new threshold (warp-uniform).
+// The whole warp updates the list of row `list_row` with (key, id); returns the row's new threshold (warp-uniform).
 __device__ __forceinline__ float flat_list_replace_max(uint32_t* lkey, uint32_t* lid, uint32_t list_row, uint32_t lane,
                                                       float key, uint32_t id) {
     uint32_t* rk = lkey + list_row * FLAT_KC;
@@ -143,10 +163,10 @@ struct FlatParams {
 // sequence, cut into G = gridDim.x / R contiguous, equal segments -- every SM gets the same number of tiles whatever
 // the batch size.  Segment g is walked by R CTAs (blockIdx g, g + G, ...: all resident at once, started together, doing
 // identical work), one per query tile of the row group: they ask for the same base tile within microseconds of each
-// other, so all but the first request are served by L2 -- without this, 148 CTAs stream 148 different places of a
-// base that is many times the L2 and every operand byte comes from DRAM (measured: 97 GB for 1M x 768).  A segment
-// may run over a row-group boundary (the lists are flushed there), and a query tile is covered by a few consecutive
-// segments ("pieces"); each piece keeps two lists per query, one per half of the 256 tile columns (one per epilogue warp).
+// other, so all but the first request are served by L2 -- without this, one CTA per SM streams as many different
+// places of a base that is many times the L2, and every operand byte comes from DRAM.  A segment may run over a
+// row-group boundary (the lists are flushed there), and a query tile is covered by a few consecutive segments
+// ("pieces"); each piece keeps two lists per query, one per half of the 256 tile columns.
 __host__ __device__ inline uint64_t flat_seg_begin(uint64_t total, uint32_t ctas, uint32_t b) { return total * b / ctas; }
 __host__ __device__ inline uint32_t flat_cta_of_tile(uint64_t t, uint64_t total, uint32_t ctas) {
     uint32_t b = uint32_t(t * ctas / total);
@@ -155,23 +175,20 @@ __host__ __device__ inline uint32_t flat_cta_of_tile(uint64_t t, uint64_t total,
     return b;
 }
 
-// Shared memory: stages | bias[2][256] | list keys [2][128][KC] | list ids [2][128][KC] | barriers | tmem slot
-constexpr uint32_t FLAT_EPI_WARPS = 8, FLAT_THREADS = 64 + 32 * FLAT_EPI_WARPS;
-constexpr size_t kFlatSmem = size_t(FLAT_STAGES) * FLAT_STAGE_BYTES + 2 * FLAT_BN * 4 + 2 * 2 * size_t(FLAT_KC) * FLAT_BM * 4 + 256;
+// Threads: warps 0-7 are the two consumer warpgroups (a warpgroup is four consecutive warps starting at a multiple of
+// four), warp 8 the producer.  Shared memory: stages | list keys [2][128][KC] | list ids [2][128][KC] | barriers.
+constexpr uint32_t FLAT_CONSUMER_WARPS = 8, FLAT_THREADS = 32 * FLAT_CONSUMER_WARPS + 32;
+constexpr size_t kFlatSmem = size_t(FLAT_STAGES) * FLAT_STAGE_BYTES + 2 * 2 * size_t(FLAT_KC) * FLAT_BM * 4 + 128;
+static_assert(kFlatSmem <= 227 * 1024, "flat GEMM shared memory exceeds the 227 KB a block may use");
 
 __global__ void __launch_bounds__(FLAT_THREADS, 1) flat_gemm_topk_kernel(const __grid_constant__ FlatParams fp) {
     extern __shared__ __align__(1024) uint8_t smem[];
     uint8_t* stages = smem;
-    float* bias_s = reinterpret_cast<float*>(smem + size_t(FLAT_STAGES) * FLAT_STAGE_BYTES);   // [2][FLAT_BN]
-    uint32_t* lkey = reinterpret_cast<uint32_t*>(bias_s + 2 * FLAT_BN);                         // [2][128][KC] ordered keys
+    uint32_t* lkey = reinterpret_cast<uint32_t*>(smem + size_t(FLAT_STAGES) * FLAT_STAGE_BYTES);   // [2][128][KC] ordered keys
     uint32_t* lid = lkey + 2 * size_t(FLAT_KC) * FLAT_BM;
     uint64_t* bars = reinterpret_cast<uint64_t*>(lid + 2 * size_t(FLAT_KC) * FLAT_BM);
     uint64_t* full = bars;                       // [STAGES] bytes of a stage have landed
-    uint64_t* empty = bars + FLAT_STAGES;        // [STAGES] the MMAs reading a stage have completed
-    uint64_t* tmem_full = empty + FLAT_STAGES;   // [2] an accumulator is complete
-    uint64_t* tmem_empty = tmem_full + 2;        // [2] the epilogue has drained an accumulator
-    uint64_t* bias_full = tmem_empty + 2;        // [2] the bias tile of an accumulator has landed
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bias_full + 2);
+    uint64_t* empty = bars + FLAT_STAGES;        // [STAGES] the MMAs of every consumer warp reading a stage have completed
 
     const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t nseg = gridDim.x / fp.share, seg = blockIdx.x % nseg, member = blockIdx.x / nseg;
@@ -182,28 +199,16 @@ __global__ void __launch_bounds__(FLAT_THREADS, 1) flat_gemm_topk_kernel(const _
     // by every role alike)
     const uint32_t mtile0 = uint32_t(t_lo / fp.ntiles) * fp.share + member, nt0 = uint32_t(t_lo % fp.ntiles);
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         for (uint32_t i = 0; i < FLAT_STAGES; ++i) {
             mbar_init(full + i, 1);
-            mbar_init(empty + i, 1);
-        }
-        for (uint32_t i = 0; i < 2; ++i) {
-            mbar_init(tmem_full + i, 1);
-            mbar_init(tmem_empty + i, 32 * FLAT_EPI_WARPS);
-            mbar_init(bias_full + i, 1);
+            mbar_init(empty + i, FLAT_CONSUMER_WARPS);
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {   // one warp allocates all 512 TMEM columns (two 256-column accumulators)
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512u));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == FLAT_CONSUMER_WARPS) {
         // ===== producer: one bulk copy per operand blob =====
         if (lane == 0) {
             uint32_t s = 0, ph = 0, mtile = mtile0, nt = nt0;
@@ -251,156 +256,124 @@ __global__ void __launch_bounds__(FLAT_THREADS, 1) flat_gemm_topk_kernel(const _
             }
             if (fp.share > 1) fp.progress[blockIdx.x] = 0xFFFFFFFFu;   // finished: never the slowest again
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer: a single thread =====
-        if (lane == 0) {
-            uint32_t s = 0, ph = 0, acc = 0, aph = 0, nt = nt0, mtile = mtile0;
-            for (uint64_t t = t_lo; t < t_hi; ++t) {
-                if (mtile >= fp.mtiles) {
-                    if (++nt == fp.ntiles) {
-                        nt = 0;
-                        mtile += fp.share;
-                    }
-                    continue;
-                }
-                mbar_wait(tmem_empty + acc, aph ^ 1u);
-                tc_fence_after();
-                mbar_arrive_expect_tx(bias_full + acc, FLAT_BN * 4);
-                bulk_copy_g2s(bias_s + acc * FLAT_BN, fp.b_bias + size_t(nt) * FLAT_BN, FLAT_BN * 4, bias_full + acc);
-                for (uint32_t kb = 0; kb < fp.KB; ++kb) {
-                    mbar_wait(full + s, ph);
-                    tc_fence_after();
-                    const uint32_t a_addr = smem_u32(stages + size_t(s) * FLAT_STAGE_BYTES);
-                    const uint32_t b_addr = a_addr + FLAT_A_BYTES;
+        return;
+    }
+
+    // ===== consumers: warpgroup wg computes query rows 64 wg .. 64 wg + 63 of the tile against all 256 base rows.
+    // Accumulator element d[4c + 2i + e] of a thread is (row 16 (warp % 4) + lane / 4 + 8 i, column 8c + 2 (lane % 4) + e)
+    // of its warpgroup's 64 x 256 block, so the four lanes of a quad share two rows; a row keeps one list per column
+    // half, updated by the whole warp (all lanes of a quad see the new threshold) =====
+    const uint32_t wg = warp >> 2;
+    const uint32_t row0 = wg * 64 + (warp & 3u) * 16 + (lane >> 2);   // the thread's rows: row0, row0 + 8
+    const uint32_t frow = wg * 64 + (warp & 3u) * 16 + (lane >> 1), fhalf = lane & 1u;   // the (row, half) list this lane clears / writes out
+    float d[128];
 #pragma unroll
-                    for (uint32_t j = 0; j < FLAT_BK / 16; ++j) {
-                        // k-chunks 2j and 2j+1 of the blob: [kc][rows/8][8][8] halves
-                        const uint64_t adesc = umma_desc(a_addr + 2 * j * (FLAT_BM * 16), FLAT_BM * 16, 128);
-                        const uint64_t bdesc = umma_desc(b_addr + 2 * j * (FLAT_BN * 16), FLAT_BN * 16, 128);
-                        tc_mma_f16(tmem_base + acc * FLAT_BN, adesc, bdesc, kFlatIdesc, (kb | j) != 0 ? 1u : 0u);
-                    }
-                    tc_commit(empty + s);
-                    if (++s == FLAT_STAGES) {
-                        s = 0;
-                        ph ^= 1u;
-                    }
-                }
-                tc_commit(tmem_full + acc);
-                acc ^= 1u;
-                if (acc == 0) aph ^= 1u;
-                if (++nt == fp.ntiles) {
-                    nt = 0;
-                    mtile += fp.share;
-                }
-            }
-        }
-    } else {
-        // ===== epilogue: warp w reads TMEM lanes 32*(w%4) .. +31 (= query rows of the tile); the two warps of a
-        // lane quarter take one half of the 256 columns each, with a list of their own per row =====
-        const uint32_t quad = warp & 3u, half = (warp - 2u) >> 2;
-        const uint32_t row = quad * 32 + lane;
-        uint32_t* my_key = lkey + size_t(half) * FLAT_BM * FLAT_KC;
-        uint32_t* my_id = lid + size_t(half) * FLAT_BM * FLAT_KC;
-        uint32_t acc = 0, aph = 0, mtile = mtile0, nt = nt0;
-        float thr = INFINITY;   // this row's threshold: the largest key of its list
-        for (uint32_t e = 0; e < FLAT_KC; ++e) {
-            my_key[row * FLAT_KC + e] = flat_ord(INFINITY);
-            my_id[row * FLAT_KC + e] = 0xFFFFFFFFu;
-        }
-        __syncwarp();
-        for (uint64_t t = t_lo; t < t_hi; ++t) {
-            if (mtile >= fp.mtiles) {
-                if (++nt == fp.ntiles) {
-                    nt = 0;
-                    mtile += fp.share;
-                }
-                continue;
-            }
-            mbar_wait(tmem_full + acc, aph);
-            mbar_wait(bias_full + acc, aph);
-            tc_fence_after();
-            const float* bias = bias_s + acc * FLAT_BN;
-#pragma unroll 1
-            for (uint32_t c = half * (FLAT_BN / 64); c < (half + 1) * (FLAT_BN / 64); ++c) {
-                uint32_t v[32];
-                const uint32_t taddr = tmem_base + ((quad * 32u) << 16) + acc * FLAT_BN + c * 32;
-                asm volatile(
-                    "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                    "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-                    : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-                      "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-                      "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-                      "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-                    : "r"(taddr));
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                // keys of the 32 columns, in groups of four with the group minimum; only groups whose minimum beats a
-                // row's threshold (rare once the lists have settled) are looked at key by key
-                float key[32], gmin[8];
-                float best = INFINITY;
+    for (uint32_t i = 0; i < 128; ++i) d[i] = 0.f;
+    float thr[2][2];   // [row i][column half]: the largest key of that list
 #pragma unroll
-                for (uint32_t i4 = 0; i4 < 8; ++i4) {
-                    const float4 b4 = *reinterpret_cast<const float4*>(bias + c * 32 + i4 * 4);
-                    key[4 * i4 + 0] = fmaf(fp.key_scale, __uint_as_float(v[4 * i4 + 0]), b4.x);
-                    key[4 * i4 + 1] = fmaf(fp.key_scale, __uint_as_float(v[4 * i4 + 1]), b4.y);
-                    key[4 * i4 + 2] = fmaf(fp.key_scale, __uint_as_float(v[4 * i4 + 2]), b4.z);
-                    key[4 * i4 + 3] = fmaf(fp.key_scale, __uint_as_float(v[4 * i4 + 3]), b4.w);
-                    gmin[i4] = fminf(fminf(key[4 * i4 + 0], key[4 * i4 + 1]), fminf(key[4 * i4 + 2], key[4 * i4 + 3]));
-                    best = fminf(best, gmin[i4]);
-                }
-                // (warp-uniform branches; inside, one key at a time: the lanes whose key beats their row's threshold
-                // are served in turn by the whole warp)
-                if (__any_sync(0xFFFFFFFFu, best < thr)) {
-#pragma unroll
-                    for (uint32_t i4 = 0; i4 < 8; ++i4) {
-                        if (!__any_sync(0xFFFFFFFFu, gmin[i4] < thr)) continue;
-#pragma unroll
-                        for (uint32_t i = 4 * i4; i < 4 * i4 + 4; ++i) {
-                            uint32_t hits = __ballot_sync(0xFFFFFFFFu, key[i] < thr);
-                            while (hits) {
-                                const uint32_t src = uint32_t(__ffs(int(hits)) - 1);
-                                hits &= hits - 1;
-                                const float k_src = __shfl_sync(0xFFFFFFFFu, key[i], src);
-                                const float tnew = flat_list_replace_max(my_key, my_id, quad * 32 + src, lane, k_src,
-                                                                         nt * FLAT_BN + c * 32 + i);
-                                if (lane == src) thr = tnew;
-                            }
-                        }
-                    }
-                }
-            }
-            tc_fence_before();
-            mbar_arrive(tmem_empty + acc);
-            acc ^= 1u;
-            if (acc == 0) aph ^= 1u;
-            if (++nt == fp.ntiles || t + 1 == t_hi) {
-                // the query tile (or this CTA's part of it) is finished: lists out, lists reset
-                const uint32_t piece = seg - flat_cta_of_tile(uint64_t(mtile / fp.share) * fp.ntiles, total, nseg);
-                const size_t q = size_t(mtile) * FLAT_BM + row;
-                float* ok = fp.cand_key + (q * fp.nlists + piece * 2 + half) * FLAT_KC;
-                uint32_t* oi = fp.cand_id + (q * fp.nlists + piece * 2 + half) * FLAT_KC;
-                __syncwarp();
-                for (uint32_t e = 0; e < FLAT_KC; ++e) {
-                    ok[e] = flat_unord(my_key[row * FLAT_KC + e]);
-                    oi[e] = my_id[row * FLAT_KC + e];
-                    my_key[row * FLAT_KC + e] = flat_ord(INFINITY);
-                    my_id[row * FLAT_KC + e] = 0xFFFFFFFFu;
-                }
-                __syncwarp();
-                thr = INFINITY;
+    for (uint32_t i = 0; i < 4; ++i) thr[i >> 1][i & 1] = INFINITY;
+    for (uint32_t e = 0; e < FLAT_KC; ++e) {
+        lkey[(fhalf * FLAT_BM + frow) * FLAT_KC + e] = flat_ord(INFINITY);
+        lid[(fhalf * FLAT_BM + frow) * FLAT_KC + e] = 0xFFFFFFFFu;
+    }
+    __syncwarp();
+    uint32_t s = 0, ph = 0, mtile = mtile0, nt = nt0;
+    for (uint64_t t = t_lo; t < t_hi; ++t) {
+        if (mtile >= fp.mtiles) {
+            if (++nt == fp.ntiles) {
                 nt = 0;
                 mtile += fp.share;
             }
+            continue;
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u));
+        // ---- mainloop: one k-block per stage, two K=16 MMAs each; a stage is released once the MMAs of the next one
+        // have been issued and its own have completed ----
+        uint32_t prev = 0;
+        for (uint32_t kb = 0; kb < fp.KB; ++kb) {
+            mbar_wait(full + s, ph);
+            const uint32_t a_addr = smem_u32(stages + size_t(s) * FLAT_STAGE_BYTES) + wg * 1024u;   // 8 row groups of 128 B
+            const uint32_t b_addr = smem_u32(stages + size_t(s) * FLAT_STAGE_BYTES + FLAT_A_BYTES);
+            wgmma_fence();
+#pragma unroll
+            for (uint32_t j = 0; j < FLAT_BK / 16; ++j) {
+                // k-chunks 2j and 2j+1 of the blob: [kc][rows/8][8][8] halves
+                const uint64_t adesc = wgmma_desc(a_addr + 2 * j * (FLAT_BM * 16), FLAT_BM * 16, 128);
+                const uint64_t bdesc = wgmma_desc(b_addr + 2 * j * (FLAT_BN * 16), FLAT_BN * 16, 128);
+                wgmma_m64n256k16(d, adesc, bdesc, (kb | j) != 0 ? 1u : 0u);
+            }
+            wgmma_commit();
+            wgmma_wait<1>();
+            if (kb > 0 && lane == 0) mbar_arrive(empty + prev);
+            prev = s;
+            if (++s == FLAT_STAGES) {
+                s = 0;
+                ph ^= 1u;
+            }
+        }
+        wgmma_wait<0>();
+#pragma unroll
+        for (uint32_t i = 0; i < 128; ++i) reg_fence(d[i]);
+        if (lane == 0) mbar_arrive(empty + prev);
+
+        // ---- epilogue: keys of the thread's 128 elements; only columns whose keys beat a row's threshold (rare once
+        // the lists have settled) are looked at key by key, the lanes with such a key served in turn by the whole warp ----
+        const float* bias = fp.b_bias + size_t(nt) * FLAT_BN + 2 * (lane & 3u);
+#pragma unroll
+        for (uint32_t c = 0; c < FLAT_BN / 8; ++c) {
+            const uint32_t h = c / (FLAT_BN / 16);
+            const float2 b2 = __ldg(reinterpret_cast<const float2*>(bias + 8 * c));
+            float key[4];
+            key[0] = fmaf(fp.key_scale, d[4 * c + 0], b2.x);
+            key[1] = fmaf(fp.key_scale, d[4 * c + 1], b2.y);
+            key[2] = fmaf(fp.key_scale, d[4 * c + 2], b2.x);
+            key[3] = fmaf(fp.key_scale, d[4 * c + 3], b2.y);
+            const bool any = fminf(key[0], key[1]) < thr[0][h] || fminf(key[2], key[3]) < thr[1][h];
+            if (!__any_sync(0xFFFFFFFFu, any)) continue;
+            uint32_t* my_key = lkey + size_t(h) * FLAT_BM * FLAT_KC;
+            uint32_t* my_id = lid + size_t(h) * FLAT_BM * FLAT_KC;
+#pragma unroll
+            for (uint32_t v = 0; v < 4; ++v) {
+                const uint32_t i = v >> 1;
+                bool pending = key[v] < thr[i][h];
+                uint32_t hits = __ballot_sync(0xFFFFFFFFu, pending);
+                while (hits) {
+                    const uint32_t src = uint32_t(__ffs(int(hits)) - 1);
+                    const float k_src = __shfl_sync(0xFFFFFFFFu, key[v], src);
+                    const uint32_t id = nt * FLAT_BN + 8 * c + 2 * (src & 3u) + (v & 1u);
+                    const float tnew = flat_list_replace_max(my_key, my_id, row0 - (lane >> 2) + (src >> 2) + 8 * i, lane,
+                                                             k_src, id);
+                    if ((lane >> 2) == (src >> 2)) thr[i][h] = tnew;
+                    // another lane of the quad may hold a key of the same row that no longer beats the new threshold
+                    pending = pending && lane != src && key[v] < thr[i][h];
+                    hits = __ballot_sync(0xFFFFFFFFu, pending);
+                }
+            }
+        }
+        if (++nt == fp.ntiles || t + 1 == t_hi) {
+            // the query tile (or this CTA's part of it) is finished: lists out, lists reset
+            const uint32_t piece = seg - flat_cta_of_tile(uint64_t(mtile / fp.share) * fp.ntiles, total, nseg);
+            const size_t q = size_t(mtile) * FLAT_BM + frow;
+            float* ok = fp.cand_key + (q * fp.nlists + piece * 2 + fhalf) * FLAT_KC;
+            uint32_t* oi = fp.cand_id + (q * fp.nlists + piece * 2 + fhalf) * FLAT_KC;
+            uint32_t* rk = lkey + (fhalf * FLAT_BM + frow) * FLAT_KC;
+            uint32_t* ri = lid + (fhalf * FLAT_BM + frow) * FLAT_KC;
+            __syncwarp();
+            for (uint32_t e = 0; e < FLAT_KC; ++e) {
+                ok[e] = flat_unord(rk[e]);
+                oi[e] = ri[e];
+                rk[e] = flat_ord(INFINITY);
+                ri[e] = 0xFFFFFFFFu;
+            }
+            __syncwarp();
+#pragma unroll
+            for (uint32_t i = 0; i < 4; ++i) thr[i >> 1][i & 1] = INFINITY;
+            nt = 0;
+            mtile += fp.share;
+        }
     }
 }
 
-// ---- operand tiling: rows -> fp16 blobs in the UMMA canonical layout -------------------------------------------
+// ---- operand tiling: rows -> fp16 blobs in the canonical K-major layout of the warpgroup MMA ----------------------
 // element (row r, k e) of tile t = r / TR lives at  ((t*KB + e/32) * 4 + (e%32)/8) * TR*8 + ((r%TR)/8)*64 + (r%8)*8 + e%8
 template <int SRCT>
 __global__ void flat_tile_kernel(const char* __restrict__ src, uint32_t row_stride, uint32_t n, uint32_t dim, uint32_t TR,

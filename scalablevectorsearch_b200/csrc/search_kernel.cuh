@@ -1,4 +1,4 @@
-// search_kernel.cuh -- the Vamana batched greedy search as one persistent sm_100a kernel.
+// search_kernel.cuh -- the Vamana batched greedy search as one persistent sm_90a kernel.
 //
 // Replaces, for a whole query batch (file:line under /root/reference/include/svs):
 //   index/vamana/index.h:564-611        VamanaIndex::search       (thread pool -> grid)
@@ -110,23 +110,12 @@ template <int OP> __device__ __forceinline__ void accumulate(float& s, float& nr
     }
 }
 
-// Blackwell packs two IEEE fp32 operations into one instruction (PTX add/sub/fma.rn.f32x2 ->
-// SASS FADD2 / FFMA2): each half rounds exactly like the scalar _rn form, so the expression
-// tree -- and every bit of the result -- is unchanged while the FP instruction count halves.
-__device__ __forceinline__ float2 fsub2_rn(float2 a, float2 b) {
-    unsigned long long d;
-    asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(*reinterpret_cast<unsigned long long*>(&a)), "l"(*reinterpret_cast<unsigned long long*>(&b)));
-    return *reinterpret_cast<float2*>(&d);
-}
-__device__ __forceinline__ float2 fadd2_rn(float2 a, float2 b) {
-    unsigned long long d;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(*reinterpret_cast<unsigned long long*>(&a)), "l"(*reinterpret_cast<unsigned long long*>(&b)));
-    return *reinterpret_cast<float2*>(&d);
-}
+// Two lanes of fp32 arithmetic side by side (the kernels keep their sums in float2 pairs): each half is the scalar
+// _rn operation, so the expression tree -- and every bit of the result -- is that of `accumulate`.
+__device__ __forceinline__ float2 fsub2_rn(float2 a, float2 b) { return make_float2(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 fadd2_rn(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 __device__ __forceinline__ float2 ffma2_rn(float2 a, float2 b, float2 c) {
-    unsigned long long d;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(*reinterpret_cast<unsigned long long*>(&a)), "l"(*reinterpret_cast<unsigned long long*>(&b)), "l"(*reinterpret_cast<unsigned long long*>(&c)));
-    return *reinterpret_cast<float2*>(&d);
+    return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 }
 template <int OP> __device__ __forceinline__ void accumulate2(float2& s, float2& nrm, float2 x, float2 y) {
     if constexpr (OP == OP_L2F) {

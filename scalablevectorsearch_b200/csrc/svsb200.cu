@@ -1,4 +1,4 @@
-// svsb200.cu -- C ABI (include/svsb200.h) of the B200 Vamana search library: index upload to one or
+// svsb200.cu -- C ABI (include/svsb200.h) of the H100 Vamana search library: index upload to one or
 // several GPUs, query preparation (the device-side maybe_fix_argument), launch plumbing, result gather.
 //
 // Host-side structure (the reference's thread pool -> CUDA streams, index/vamana/index.h:455-470,564-611):
@@ -11,7 +11,7 @@
 //     the reference's TotalOrder (mode B); with NVLink peer access the shards' search kernels write their
 //     rows straight into the merging device's buffer.
 //
-// No CPU fallback lives here: every entry point either runs CUDA kernels on an sm_100 device or fails.
+// No CPU fallback lives here: every entry point either runs CUDA kernels on an sm_90 device or fails.
 #include "common.cuh"
 
 #include <algorithm>
@@ -121,7 +121,7 @@ struct Replica {
     uint16_t* d_ref_degree = nullptr;
     float* d_mean = nullptr;          // LVQ-8: dataset mean
     uint32_t* d_entry = nullptr;      // entry points when there are several
-    // tensor-core flat search: the base vectors as fp16 UMMA tiles + per-row bias, built on first use
+    // tensor-core flat search: the base vectors as fp16 warpgroup-MMA tiles + per-row bias, built on first use
     void* flat_b = nullptr;
     float* flat_bias = nullptr;
     unsigned int* flat_xmax = nullptr;
@@ -724,8 +724,8 @@ int svsb200_index_create_multi(const void* vectors, int dtype, size_t n, size_t 
             if (devices[j] == device) return fail("svsb200_index_create: device listed twice");
         cudaDeviceProp prop;
         CUDA_TRY(cudaGetDeviceProperties(&prop, device));
-        if (prop.major != 10 || prop.minor != 0)
-            return fail("svsb200_index_create: device is not sm_100 (this binary holds sm_100a code only)");
+        if (prop.major != 9 || prop.minor != 0)
+            return fail("svsb200_index_create: device is not sm_90 (this binary holds sm_90a code only)");
         std::unique_ptr<Replica> rep(new Replica());
         rep->device = device;
         rep->sm_count = prop.multiProcessorCount;
@@ -993,8 +993,8 @@ int svsb200_index_assemble(const char* config_path, const char* graph_path, cons
         if (device < 0 || device >= ndev) return fail("svsb200_index_assemble: bad device ordinal");
         cudaDeviceProp prop;
         CUDA_TRY(cudaGetDeviceProperties(&prop, device));
-        if (prop.major != 10 || prop.minor != 0)
-            return fail("svsb200_index_assemble: device is not sm_100 (this binary holds sm_100a code only)");
+        if (prop.major != 9 || prop.minor != 0)
+            return fail("svsb200_index_assemble: device is not sm_90 (this binary holds sm_90a code only)");
         std::unique_ptr<Replica> rep(new Replica());
         rep->device = device;
         rep->sm_count = prop.multiProcessorCount;

@@ -12,9 +12,9 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box via gpurun)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
     # The product library is built in-tree (git-ignored); compile it if this checkout has not been built yet
-    # (nvcc cross-compiles sm_100a without a GPU).  Never a fallback: tests still go through libsvsb200.so.
+    # (nvcc cross-compiles sm_90a without a GPU).  Never a fallback: tests still go through libsvsb200.so.
     lib = os.path.join(ROOT, "scalablevectorsearch_b200", "libsvsb200.so")
     if not os.path.exists(lib) and os.path.exists("/usr/local/cuda/bin/nvcc"):
         import subprocess

@@ -7,8 +7,10 @@ Outputs: test_dataset.npz   compact copy of the fixtures the parity tests need o
          ref_outputs.npz    ids / distances / work counters the *reference itself* produces
          golden_recalls.json the 17 (window, capacity) -> recall@10 goldens of
                             data/test_dataset/reference/vamana_reference.toml (vamana_test_search)
+         ref_builder.json   entry point, mean degree and recall@10 of graphs from the reference's own
+                            builder, for the GPU builder's tests (tests/test_gpu_build.py)
 
-    python tests/golden/make_golden.py
+    python tests/golden/make_golden.py [--builder-only]
 """
 import json
 import os
@@ -45,9 +47,43 @@ def parse_goldens(path):
     return out
 
 
+def recall_at_k(ids, gt, k=10):
+    return sum(len(set(r[:k].tolist()) & set(t[:k].tolist())) for r, t in zip(ids, gt)) / (k * len(ids))
+
+
+def builder_goldens(ref):
+    """The reference builder's side of tests/test_gpu_build.py, searched with the reference's own search (bit-exact
+    with the GPU search, so these are the recalls that test would measure on the reference's graphs)."""
+    from scalablevectorsearch_b200.synthetic import clustered_unit_vectors
+    z = np.load(f"{OUT}/test_dataset.npz")
+    X, Q = z["data"].astype(np.float32), z["queries"].astype(np.float32)
+    out = {"test_dataset": {}}
+    for metric in ("l2", "ip", "cosine"):
+        alpha = 1.2 if metric == "l2" else 0.95
+        g, ep = ref.build(X, metric, 32, 64, alpha=alpha, threads=4)
+        idx = ref.index(X, g, ep, metric, threads=4)
+        out["test_dataset"][metric] = {
+            "max_degree": 32, "window_size": 64, "alpha": alpha, "entry_point": int(ep),
+            "mean_degree": float(g[:, 0].mean()),
+            "recall": {str(w): recall_at_k(idx.search(Q, 10, w, w)[0], z[f"gt_{metric}"]) for w in (10, 30)}}
+    base, queries = clustered_unit_vectors(30_000, 500, 96)
+    base16 = base.astype(np.float16)
+    x = base16.astype(np.float32)
+    d = (queries ** 2).sum(1)[:, None] + (x ** 2).sum(1)[None, :] - 2.0 * queries @ x.T
+    gt = np.argsort(d, axis=1, kind="stable")[:, :10]
+    g, ep = ref.build(base16, "l2", 64, 128, alpha=1.2, threads=8)
+    ids = ref.index(base16, g, ep, "l2", threads=8).search(queries, 10, 64, 64)[0]
+    out["synthetic_30000x96_f16_l2"] = {"max_degree": 64, "window_size": 128, "alpha": 1.2, "search_window": 64,
+                                         "recall": recall_at_k(ids, gt)}
+    json.dump(out, open(f"{OUT}/ref_builder.json", "w"), indent=1)
+
+
 def main():
     ref = RefLib()
     assert ref.avx512(), "goldens must come from the AVX-512 expression tree"
+    if "--builder-only" in sys.argv:
+        builder_goldens(ref)
+        return
     X = io.read_svs(f"{SRC}/data_f32.svs", np.float32)
     G = io.read_graph(f"{SRC}/graph_128.svs")
     Q = io.read_vecs(f"{SRC}/queries_f32.fvecs")
@@ -103,7 +139,8 @@ def main():
                 outs[f"{metric}_sq_{cname}_{qn}_w24_c40_ids"] = ids.astype(np.uint32)
                 outs[f"{metric}_sq_{cname}_{qn}_w24_c40_dists"] = dists
     np.savez_compressed(f"{OUT}/ref_outputs.npz", **outs)
-    for f in ("test_dataset.npz", "ref_outputs.npz", "golden_recalls.json"):
+    builder_goldens(ref)
+    for f in ("test_dataset.npz", "ref_outputs.npz", "golden_recalls.json", "ref_builder.json"):
         print(f, os.path.getsize(f"{OUT}/{f}") // 1024, "KiB")
 
 

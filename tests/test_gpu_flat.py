@@ -2,7 +2,10 @@
 
 The checker is svsb200_exhaustive_device (the search path's distance code over every base vector, itself checked
 against the oracle in test_gpu_parity.py::test_exhaustive_scan_is_exact_topk): ids and distance bits must be equal
-for every query, whether the GEMM candidates verified or the query fell back to the scan."""
+for every query, whether the GEMM candidates verified or the query fell back to the scan.  The fallback keeps the
+result exact even when the GEMM is wrong, so on clustered vectors (where the error bound proves every query) the tests
+also require that no query fell back: a defect in the GEMM or its accumulator layout, even in a single query row of a
+tile, sends that row's queries to the scan and fails them."""
 import numpy as np
 import pytest
 
@@ -38,7 +41,7 @@ def test_flat_equals_exact_scan_on_clustered_vectors(metric, dtype):
     (ei, ed, _), (fi, fd, nfb) = _both(index, queries, 10)
     assert np.array_equal(fi, ei), (metric, dtype)
     assert np.array_equal(bits(fd), bits(ed))
-    assert nfb < queries.shape[0] // 2, f"{nfb} of {queries.shape[0]} queries fell back to the scan"
+    assert nfb == 0, f"{nfb} of {queries.shape[0]} queries fell back to the scan"
     hi, hd = index.flat_search(queries[:50], 10)          # host-buffer form
     assert np.array_equal(hi.astype(np.int64), ei[:50]) and np.array_equal(bits(hd), bits(ed[:50]))
 
@@ -72,4 +75,4 @@ def test_flat_row_groups_and_pacing(n, nq, dim):
         (ei, ed, _), (fi, fd, nfb) = _both(index, queries, 10)
         assert np.array_equal(fi, ei), (metric, n, nq, dim)
         assert np.array_equal(bits(fd), bits(ed))
-        assert nfb < nq // 2
+        assert nfb == 0, f"{nfb} of {nq} queries fell back to the scan"
