@@ -111,23 +111,6 @@ template <int ROWT> cudaError_t launch_search_fast(int op, const SearchParams& p
 // Exhaustive scan with the same distance code (ground truth / flat search).
 template <int ROWT> cudaError_t launch_search_exhaustive(int op, const SearchParams& p, const LaunchConfig& cfg);
 
-// Tensor-core exhaustive search (flat.cu)
-cudaError_t flat_tile_rows(int srct, const void* src, uint32_t row_stride, uint32_t n, uint32_t dim, uint32_t tile_rows,
-                           float scale, int l2, void* dst_tiles, float* bias, float* norms, unsigned int* max_norm_bits,
-                           cudaStream_t stream);
-cudaError_t flat_gemm_topk(const void* a_tiles, const void* b_tiles, const float* b_bias, uint32_t KB, uint32_t ntiles,
-                           uint32_t mtiles, uint32_t ctas, uint32_t share, uint32_t nlists, float key_scale, float* cand_key,
-                           uint32_t* cand_id, uint32_t* progress, cudaStream_t stream);
-struct SearchParams;
-void flat_plan(uint32_t mtiles, uint32_t ntiles, uint32_t sm_count, uint32_t* ctas, uint32_t* share, uint32_t* nlists);
-cudaError_t flat_rescore(int rowt, int op, const SearchParams& p, const float* cand_key, const uint32_t* cand_id, uint32_t nsplit,
-                         uint32_t nq, uint32_t k, const float* qnorm, const unsigned int* xmax_bits, uint64_t* out_ids,
-                         float* out_dists, uint32_t* unverified, uint32_t* n_unverified, cudaStream_t stream);
-cudaError_t flat_move_rows(const void* src, void* dst, const uint32_t* idx, const uint32_t* count, uint32_t max_count,
-                           uint32_t row_bytes, int scatter, cudaStream_t stream);
-uint32_t flat_kc();
-
 void count_launch();
-int set_error(const std::string& msg);   // records the calling thread's svsb200_last_error(); returns 1
 
 }  // namespace svsb200

@@ -26,6 +26,7 @@
 // the products are exact in fp32 and the tensor-core accumulation of `dim` of them adds at most dim 2^-22 ||q|| ||x||;
 // for L2 the bias |x~|^2 differs from |x|^2 by at most 2^-10 ||x||^2 when the data was rounded.  So
 //   E_ip(q) = (r 2^-11 + dim 2^-22) ||q|| Xmax,      E_l2(q) = 2 E_ip(q) + [data rounded] 2^-10 Xmax^2.
+#include "host.cuh"
 #include "search_kernel.cuh"
 
 #include <cuda_fp16.h>
@@ -513,10 +514,10 @@ __global__ void flat_move_rows_kernel(const char* __restrict__ src, char* __rest
     for (uint32_t b = threadIdx.x; b < row_bytes; b += blockDim.x) d[b] = s[b];
 }
 
-// ---- launchers (called from svsb200.cu) ------------------------------------------------------------------------------
-cudaError_t flat_tile_rows(int srct, const void* src, uint32_t row_stride, uint32_t n, uint32_t dim, uint32_t tile_rows,
-                           float scale, int l2, void* dst_tiles, float* bias, float* norms, unsigned int* max_norm_bits,
-                           cudaStream_t stream) {
+// ---- launchers ------------------------------------------------------------------------------------------------------
+static cudaError_t flat_tile_rows(int srct, const void* src, uint32_t row_stride, uint32_t n, uint32_t dim, uint32_t tile_rows,
+                                  float scale, int l2, void* dst_tiles, float* bias, float* norms, unsigned int* max_norm_bits,
+                                  cudaStream_t stream) {
     const uint32_t KB = (dim + FLAT_BK - 1) / FLAT_BK;
     const uint32_t rows_padded = (n + tile_rows - 1) / tile_rows * tile_rows;
     cudaError_t err = cudaMemsetAsync(dst_tiles, 0, size_t(rows_padded) * KB * FLAT_BK * 2, stream);
@@ -542,7 +543,7 @@ __global__ void flat_fill_kernel(float* __restrict__ key, uint32_t* __restrict__
 // Grid size, sharing factor and lists per query for a problem: as many CTAs as SMs in groups of R, fewer segments
 // while a query tile would be cut into more pieces than the rescoring kernel holds candidates for (small batches
 // over a large base).
-void flat_plan(uint32_t mtiles, uint32_t ntiles, uint32_t sm_count, uint32_t* ctas, uint32_t* share, uint32_t* nlists) {
+static void flat_plan(uint32_t mtiles, uint32_t ntiles, uint32_t sm_count, uint32_t* ctas, uint32_t* share, uint32_t* nlists) {
     const uint32_t R = mtiles >= 8 ? 4 : mtiles >= 4 ? 2 : 1;
     const uint32_t ngroups = (mtiles + R - 1) / R;
     const uint64_t total = uint64_t(ngroups) * ntiles;
@@ -561,9 +562,9 @@ void flat_plan(uint32_t mtiles, uint32_t ntiles, uint32_t sm_count, uint32_t* ct
     }
 }
 
-cudaError_t flat_gemm_topk(const void* a_tiles, const void* b_tiles, const float* b_bias, uint32_t KB, uint32_t ntiles,
-                           uint32_t mtiles, uint32_t ctas, uint32_t share, uint32_t nlists, float key_scale, float* cand_key,
-                           uint32_t* cand_id, uint32_t* progress, cudaStream_t stream) {
+static cudaError_t flat_gemm_topk(const void* a_tiles, const void* b_tiles, const float* b_bias, uint32_t KB, uint32_t ntiles,
+                                  uint32_t mtiles, uint32_t ctas, uint32_t share, uint32_t nlists, float key_scale, float* cand_key,
+                                  uint32_t* cand_id, uint32_t* progress, cudaStream_t stream) {
     FlatParams fp{};
     fp.a_tiles = static_cast<const __half*>(a_tiles);
     fp.b_tiles = static_cast<const __half*>(b_tiles);
@@ -596,9 +597,9 @@ template <int ROWT> static cudaError_t rescore_rowt(int op, const SearchParams& 
     return cudaGetLastError();
 }
 
-cudaError_t flat_rescore(int rowt, int op, const SearchParams& p, const float* cand_key, const uint32_t* cand_id, uint32_t nsplit,
-                         uint32_t nq, uint32_t k, const float* qnorm, const unsigned int* xmax_bits, uint64_t* out_ids,
-                         float* out_dists, uint32_t* unverified, uint32_t* n_unverified, cudaStream_t stream) {
+static cudaError_t flat_rescore(int rowt, int op, const SearchParams& p, const float* cand_key, const uint32_t* cand_id, uint32_t nsplit,
+                                uint32_t nq, uint32_t k, const float* qnorm, const unsigned int* xmax_bits, uint64_t* out_ids,
+                                float* out_dists, uint32_t* unverified, uint32_t* n_unverified, cudaStream_t stream) {
     RescoreParams rp{};
     rp.cand_key = cand_key;
     rp.cand_id = cand_id;
@@ -617,8 +618,8 @@ cudaError_t flat_rescore(int rowt, int op, const SearchParams& p, const float* c
     return rowt == SVSB200_F32 ? rescore_rowt<SVSB200_F32>(op, p, rp, stream) : rescore_rowt<SVSB200_F16>(op, p, rp, stream);
 }
 
-cudaError_t flat_move_rows(const void* src, void* dst, const uint32_t* idx, const uint32_t* count, uint32_t max_count,
-                           uint32_t row_bytes, int scatter, cudaStream_t stream) {
+static cudaError_t flat_move_rows(const void* src, void* dst, const uint32_t* idx, const uint32_t* count, uint32_t max_count,
+                                  uint32_t row_bytes, int scatter, cudaStream_t stream) {
     if (max_count == 0) return cudaSuccess;
     flat_move_rows_kernel<<<max_count, 128, 0, stream>>>(static_cast<const char*>(src), static_cast<char*>(dst), idx, count,
                                                         row_bytes, scatter);
@@ -626,18 +627,116 @@ cudaError_t flat_move_rows(const void* src, void* dst, const uint32_t* idx, cons
     return cudaGetLastError();
 }
 
-uint32_t flat_kc() { return FLAT_KC; }
+// Shared body of the tensor-core flat search: device buffers in, device buffers out, enqueued on sc->stream except
+// for one synchronisation (the count of queries that need the exact-scan fallback).
+static int flat_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, const void* d_queries, int qdtype, size_t nq, size_t k,
+                          uint64_t* d_out_ids, float* d_out_dists, uint32_t* fallback_queries) {
+    if (fallback_queries) *fallback_queries = 0;
+    if (nq == 0) return 0;
+    cudaStream_t stream = sc->stream;
+    const bool gemm_ok = ix->storage == SVSB200_PLAIN && (ix->dtype == SVSB200_F32 || ix->dtype == SVSB200_F16) &&
+                         ix->metric != SVSB200_COSINE && (qdtype == SVSB200_F32 || qdtype == SVSB200_F16) &&
+                         k + 8 <= FLAT_KC && ix->n >= 512;
+    if (!gemm_ok) {   // shapes outside the GEMM path: the exact scan
+        if (fallback_queries) *fallback_queries = uint32_t(nq);
+        return search_on_device(ix, rep, sc, d_queries, qdtype, nq, k, k, k, d_out_ids, 8, d_out_dists, stream, true);
+    }
+    const uint32_t n = uint32_t(ix->n), dim = uint32_t(ix->dim);
+    const uint32_t KB = (dim + 31) / 32, ntiles = (n + 255) / 256, mtiles = uint32_t((nq + 127) / 128);
+    const int l2 = ix->metric == SVSB200_L2;
+    {   // base tiles, once per replica
+        std::lock_guard<std::mutex> lock(rep->mu);
+        if (!rep->flat_b.ptr) {
+            CUDA_TRY(rep->flat_b.ensure(size_t(ntiles) * 256 * KB * 32 * 2));
+            CUDA_TRY(rep->flat_bias.ensure(size_t(ntiles) * 256));
+            CUDA_TRY(rep->flat_xmax.ensure(1));
+            CUDA_TRY(cudaMemsetAsync(rep->flat_xmax.ptr, 0, 4, stream));
+            CUDA_TRY(flat_tile_rows(ix->dtype, rep->d_vectors.ptr, ix->row_stride, n, dim, 256, 1.0f, l2, rep->flat_b.ptr,
+                                    rep->flat_bias.ptr, nullptr, rep->flat_xmax.ptr, stream));
+            CUDA_TRY(cudaStreamSynchronize(stream));
+        }
+    }
+    // one CTA per SM over equal runs of output tiles; `nsplit` = candidate lists per query (flat_plan)
+    uint32_t flat_ctas = 1, flat_share = 1, nsplit = 2;
+    flat_plan(mtiles, ntiles, uint32_t(rep->sm_count), &flat_ctas, &flat_share, &nsplit);
+    const size_t qrow = size_t(dim) * esize(qdtype);
+    CUDA_TRY(sc->flat_a.ensure(size_t(mtiles) * 128 * KB * 32 * 2));
+    CUDA_TRY(sc->flat_qnorm.ensure(size_t(mtiles) * 128));
+    CUDA_TRY(sc->flat_ckey.ensure(size_t(mtiles) * 128 * nsplit * FLAT_KC));
+    CUDA_TRY(sc->flat_cid.ensure(size_t(mtiles) * 128 * nsplit * FLAT_KC));
+    CUDA_TRY(sc->flat_unv.ensure(nq + 1));
+    CUDA_TRY(sc->flat_progress.ensure(flat_ctas));
+    CUDA_TRY(cudaMemsetAsync(sc->flat_progress.ptr, 0, size_t(flat_ctas) * 4, stream));
+    CUDA_TRY(flat_tile_rows(qdtype, d_queries, uint32_t(qrow), uint32_t(nq), dim, 128, 1.0f, 0, sc->flat_a.ptr, nullptr,
+                            sc->flat_qnorm.ptr, nullptr, stream));
+    CUDA_TRY(flat_gemm_topk(sc->flat_a.ptr, rep->flat_b.ptr, rep->flat_bias.ptr, KB, ntiles, mtiles, flat_ctas, flat_share, nsplit,
+                            l2 ? -2.0f : -1.0f, sc->flat_ckey.ptr, sc->flat_cid.ptr, sc->flat_progress.ptr, stream));
+    // exact re-scoring with the search path's distance code: prepared queries as for a search
+    if (int rc = prepare_queries(ix, rep, sc, d_queries, qdtype, nq, PREP_FLOAT, stream)) return rc;
+    SearchParams p{};
+    p.vectors = rep->d_vectors.ptr;
+    p.n = n;
+    p.dim = dim;
+    p.row_stride = ix->row_stride;
+    p.greater = !l2;
+    p.qf = sc->q_f32.ptr;
+    p.qaux = sc->q_aux.ptr;
+    p.qstride = query_stride(dim);
+    p.nq = uint32_t(nq);
+    p.k = uint32_t(k);
+    CUDA_TRY(cudaMemsetAsync(sc->flat_unv.ptr, 0, 4, stream));
+    // rounding terms of E(q) (file header): the query is always rounded to fp16, float32 data too
+    p.scale = (qdtype == SVSB200_F32 ? 1.0f : 0.0f) + (ix->dtype == SVSB200_F32 ? 1.0f : 0.0f);   // number of rounded operands
+    CUDA_TRY(flat_rescore(ix->dtype, l2 ? OP_L2F : OP_IPF, p, sc->flat_ckey.ptr, sc->flat_cid.ptr, nsplit, uint32_t(nq), uint32_t(k),
+                          sc->flat_qnorm.ptr, rep->flat_xmax.ptr, d_out_ids, d_out_dists, sc->flat_unv.ptr + 1, sc->flat_unv.ptr, stream));
+    // queries whose bound did not verify: exact scan, results scattered over the rescored rows
+    uint32_t nunv = 0;
+    CUDA_TRY(cudaMemcpyAsync(&nunv, sc->flat_unv.ptr, 4, cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaStreamSynchronize(stream));
+    if (fallback_queries) *fallback_queries = nunv;
+    if (nunv) {
+        CUDA_TRY(sc->flat_q2.ensure(size_t(nunv) * qrow));
+        CUDA_TRY(sc->flat_i2.ensure(size_t(nunv) * k));
+        CUDA_TRY(sc->flat_d2.ensure(size_t(nunv) * k));
+        CUDA_TRY(flat_move_rows(d_queries, sc->flat_q2.ptr, sc->flat_unv.ptr + 1, sc->flat_unv.ptr, nunv, uint32_t(qrow), 0, stream));
+        int rc = search_on_device(ix, rep, sc, sc->flat_q2.ptr, qdtype, nunv, k, k, k, sc->flat_i2.ptr, 8, sc->flat_d2.ptr, stream, true);
+        if (rc) return rc;
+        CUDA_TRY(flat_move_rows(sc->flat_i2.ptr, d_out_ids, sc->flat_unv.ptr + 1, sc->flat_unv.ptr, nunv, uint32_t(k * 8), 1, stream));
+        CUDA_TRY(flat_move_rows(sc->flat_d2.ptr, d_out_dists, sc->flat_unv.ptr + 1, sc->flat_unv.ptr, nunv, uint32_t(k * 4), 1, stream));
+    }
+    return 0;
+}
+
+// Blocking form on host buffers, on a scratch set of the pool.
+static int flat_search_host(svsb200_index* ix, Replica* rep, Scratch* sc, const void* queries, int qdtype, size_t nq, size_t k,
+                            uint64_t* out_ids, float* out_dists) {
+    const size_t qbytes = nq * ix->dim * esize(qdtype);
+    CUDA_TRY(sc->q_raw.ensure(qbytes));
+    CUDA_TRY(sc->ids.ensure(nq * k * 8));
+    CUDA_TRY(sc->dists.ensure(nq * k));
+    CUDA_TRY(cudaMemcpyAsync(sc->q_raw.ptr, queries, qbytes, cudaMemcpyHostToDevice, sc->stream));
+    int rc = flat_on_device(ix, rep, sc, sc->q_raw.ptr, qdtype, nq, k, reinterpret_cast<uint64_t*>(sc->ids.ptr), sc->dists.ptr,
+                            nullptr);
+    if (rc) return rc;
+    CUDA_TRY(cudaMemcpyAsync(out_ids, sc->ids.ptr, nq * k * 8, cudaMemcpyDeviceToHost, sc->stream));
+    CUDA_TRY(cudaMemcpyAsync(out_dists, sc->dists.ptr, nq * k * 4, cudaMemcpyDeviceToHost, sc->stream));
+    CUDA_TRY(cudaStreamSynchronize(sc->stream));
+    return 0;
+}
 
 }  // namespace svsb200
 
+using namespace svsb200;
+
+extern "C" {
+
 // How svsb200_flat_search* splits a problem (include/svsb200.h): host arithmetic only, so that the work split -- which the
 // kernel recomputes from the same inline functions -- can be checked without a device (tests/test_flat_plan.py).
-extern "C" int svsb200_flat_plan(size_t nq, size_t n, int sm_count, uint32_t* ctas, uint32_t* share, uint32_t* lists_per_query,
-                                 uint64_t* segment_begin) {
-    using namespace svsb200;
+int svsb200_flat_plan(size_t nq, size_t n, int sm_count, uint32_t* ctas, uint32_t* share, uint32_t* lists_per_query,
+                      uint64_t* segment_begin) {
     if (nq == 0 || n == 0 || sm_count <= 0 || !ctas || !share || !lists_per_query)
-        return set_error("svsb200_flat_plan: nq, n, sm_count must be positive and the outputs non-NULL");
-    if (nq > (size_t(1) << 31) || n > (size_t(1) << 31)) return set_error("svsb200_flat_plan: problem too large");
+        return fail("svsb200_flat_plan: nq, n, sm_count must be positive and the outputs non-NULL");
+    if (nq > (size_t(1) << 31) || n > (size_t(1) << 31)) return fail("svsb200_flat_plan: problem too large");
     const uint32_t mtiles = uint32_t((nq + FLAT_BM - 1) / FLAT_BM), ntiles = uint32_t((n + FLAT_BN - 1) / FLAT_BN);
     flat_plan(mtiles, ntiles, uint32_t(sm_count), ctas, share, lists_per_query);
     if (segment_begin) {
@@ -647,3 +746,37 @@ extern "C" int svsb200_flat_plan(size_t nq, size_t n, int sm_count, uint32_t* ct
     }
     return 0;
 }
+
+int svsb200_flat_search_device(svsb200_index* ix, const void* d_queries, int qdtype, size_t nq, size_t k, uint64_t* d_out_ids,
+                               float* d_out_dists, void* stream_, uint32_t* fallback_queries) {
+    if (!ix) return fail("svsb200_flat_search_device: NULL index");
+    if (nq && (!d_queries || !d_out_ids || !d_out_dists)) return fail("svsb200_flat_search_device: NULL buffer");
+    if (k == 0 || k > 1024) return fail("svsb200_flat_search_device: k must be in [1, 1024]");
+    if (qdtype < SVSB200_F32 || qdtype > SVSB200_U8) return fail("bad query dtype");
+    if (ix->reps.size() != 1) return fail("svsb200_flat_search_device: the index must live on exactly one device");
+    Replica* rep = ix->reps[0].get();
+    CUDA_TRY(cudaSetDevice(rep->device));
+    std::string err;
+    Scratch* sc = scratch_for_stream(rep, static_cast<cudaStream_t>(stream_), &err);
+    if (!sc) return fail(err);
+    return flat_on_device(ix, rep, sc, d_queries, qdtype, nq, k, d_out_ids, d_out_dists, fallback_queries);
+}
+
+int svsb200_flat_search(svsb200_index* ix, const void* queries, int qdtype, size_t nq, size_t k, uint64_t* out_ids,
+                        float* out_dists) {
+    if (!ix) return fail("svsb200_flat_search: NULL index");
+    if (nq == 0) return 0;
+    if (!queries || !out_ids || !out_dists) return fail("svsb200_flat_search: NULL buffer");
+    if (k == 0 || k > 1024) return fail("svsb200_flat_search: k must be in [1, 1024]");
+    if (qdtype < SVSB200_F32 || qdtype > SVSB200_U8) return fail("bad query dtype");
+    Replica* rep = ix->reps[0].get();
+    CUDA_TRY(cudaSetDevice(rep->device));
+    std::string err;
+    Scratch* sc = acquire(rep, &err);
+    if (!sc) return fail(err);
+    int rc = flat_search_host(ix, rep, sc, queries, qdtype, nq, k, out_ids, out_dists);
+    release(rep, sc);
+    return rc;
+}
+
+}  // extern "C"

@@ -258,6 +258,9 @@ def test_assemble_from_files_like_the_reference_binding(dataset, ref_outputs, tm
     with pytest.raises(Svsb200Error):      # VectorDataLoader(dims=...) is checked against the file
         Vamana(str(tmp_path / "config.toml"), GraphLoader(str(tmp_path / "graph.svs")),
                VectorDataLoader(str(tmp_path / "data.svs"), DataType.float32, dims=96))
+    with pytest.raises(Svsb200Error):      # a device listed twice, as index creation from arrays rejects it
+        Vamana(str(tmp_path / "config.toml"), GraphLoader(str(tmp_path / "graph.svs")),
+               VectorDataLoader(str(tmp_path / "data.svs"), DataType.float32), device=[0, 0])
     with pytest.raises(TypeError):         # declared query type (default float32) is enforced
         index.search(dataset.queries[:4].astype(np.float16), 10)
     # the same data as .fvecs goes through the strided vecs reader
