@@ -277,6 +277,37 @@ int svsb200_exhaustive_device(
     svsb200_index* index, const void* d_queries, int qdtype, size_t nq, size_t k,
     uint64_t* d_out_ids, float* d_out_dists, void* stream);
 
+/* Dynamic index.  Replaces: MutableVamanaIndex(graph, data, entry_point, distance, external_ids, threadpool)
+ * (include/svs/index/vamana/dynamic_index.h:178-202) for float32 / float16 plain storage on one device, adjacency rows
+ * of at most 128 neighbours, L2 / MIP / cosine.  Arguments as svsb200_index_create (dense rows), plus one distinct
+ * external id per row; every slot starts Valid.  The result is an ordinary index handle:
+ *   * svsb200_search / _cancellable / _device run MutableVamanaIndex::search (dynamic_index.h:482-571): the walk goes
+ *     through Deleted slots (ValidBuilder, :93-108) but the MutableBuffer (dynamic_search_buffer.h) never counts or
+ *     returns them; ids are the EXTERNAL ids (id_bytes must be 8).  Short rows are padded with all-ones / +-inf.
+ *     These calls block until the kernels are done (a query whose list outgrows the buffer's room for Deleted entries
+ *     is re-run with more room; the "dynamic_slack" option sets the initial room, "dynamic_reruns" counts re-runs);
+ *     a cancellation predicate is polled while they run;
+ *   * svsb200_search_filtered takes a bitmap over the slots, clears the slots that are not Valid from it and returns
+ *     external ids; svsb200_range_search returns external ids;
+ *   * flat, exhaustive and sharded searches, set_entry_points and set_id_offset fail on it.
+ * External id 2^64 - 1 is reserved (it marks padding).
+ * Mutations must not run concurrently with searches of the same index. */
+int svsb200_dynamic_create(
+    const void* vectors, int dtype, size_t n, size_t dim, const uint32_t* graph_rows, size_t graph_row_len,
+    uint32_t entry_point, int metric, const uint64_t* external_ids, int device, svsb200_index** out);
+/* delete_entries (dynamic_index.h:773-788): soft deletion.  Fails without changing anything unless every id is
+ * present (and listed once); afterwards the slots are Deleted and the ids unknown. */
+int svsb200_dynamic_delete(svsb200_index* index, const uint64_t* ids, size_t count);
+/* all_ids / has_id: the external ids of the Valid slots, in slot order.  *count is the room of out_ids on entry
+ * (out_ids may be NULL to ask for the count) and the number of ids on return. */
+int svsb200_dynamic_ids(const svsb200_index* index, uint64_t* out_ids, size_t* count);
+int svsb200_dynamic_has_id(const svsb200_index* index, uint64_t id, int* out);
+/* The index's state for inspection: graph uint32[n][max_degree + 1] (degree first), status uint8[n]
+ * (0 Empty, 1 Valid, 2 Deleted), external ids uint64[n] and the entry point; n = svsb200_index_size (slots).
+ * Any output may be NULL. */
+int svsb200_dynamic_export(const svsb200_index* index, uint32_t* graph_rows_out, uint8_t* status_out,
+                           uint64_t* ext_ids_out, uint32_t* entry_point_out);
+
 #ifdef __cplusplus
 }
 #endif

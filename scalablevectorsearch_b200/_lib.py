@@ -23,6 +23,8 @@ SYMBOLS = [
     "svsb200_index_create_multi", "svsb200_index_num_devices", "svsb200_search_cancellable", "svsb200_set_id_offset",
     "svsb200_search_sharded", "svsb200_build_vamana", "svsb200_flat_search_device", "svsb200_flat_search", "svsb200_index_assemble", "svsb200_toml_get", "svsb200_search_filtered", "svsb200_range_search", "svsb200_free", "svsb200_set_entry_points",
     "svsb200_flat_plan",
+    "svsb200_dynamic_create", "svsb200_dynamic_delete", "svsb200_dynamic_ids", "svsb200_dynamic_has_id",
+    "svsb200_dynamic_export",
 ]
 
 _lib = None
@@ -83,6 +85,11 @@ def lib() -> C.CDLL:
     l.svsb200_free.restype = None
     l.svsb200_set_entry_points.argtypes = [vp, vp, sz]
     l.svsb200_build_vamana.argtypes = [vp, i32, sz, sz, sz, i32, C.c_float, sz, sz, sz, sz, i32, vp, C.POINTER(u32)]
+    l.svsb200_dynamic_create.argtypes = [vp, i32, sz, sz, vp, sz, u32, i32, vp, i32, C.POINTER(vp)]
+    l.svsb200_dynamic_delete.argtypes = [vp, vp, sz]
+    l.svsb200_dynamic_ids.argtypes = [vp, vp, C.POINTER(sz)]
+    l.svsb200_dynamic_has_id.argtypes = [vp, C.c_uint64, C.POINTER(i32)]
+    l.svsb200_dynamic_export.argtypes = [vp, vp, vp, vp, C.POINTER(u32)]
     _lib = l
     return l
 

@@ -76,7 +76,17 @@ struct SearchParams {
     uint2* hist;
     uint32_t* hist_count;
     uint32_t hist_cap;
+    // dynamic index only (MUT kernels, the reference's MutableBuffer search): per-slot status, external ids, buffer room
+    const uint8_t* status;       // [n] SlotMetadata: a Deleted slot is walked through but never returned
+    const uint64_t* ext_ids;     // [n] external id of every slot (what the copy-out writes; NULL: the slot itself)
+    uint32_t buf_cap;            // entries the buffer may hold: capacity + slack for Deleted entries
+    uint32_t* ovf;               // [1 + nq] count, then the queries whose buffer ran out of slack (not written)
+    const uint32_t* qlist;       // optional: run only these queries (a re-run of overflowed ones)
 };
+
+// SlotMetadata of the reference's MutableVamanaIndex (index/vamana/dynamic_index.h:60-79).
+enum SlotStatus : uint8_t { SLOT_EMPTY = 0, SLOT_VALID = 1, SLOT_DELETED = 2 };
+constexpr uint32_t kInvalidBit = 0x40000000u;   // MUT kernels: PredicatedSearchNeighbor::valid() == false, packed into the id
 
 struct LaunchConfig {
     int grid;
@@ -108,6 +118,8 @@ constexpr int kFastMaxGW = 4;   // adjacency rows up to 128 neighbours (4 x 32) 
 template <int ROWT> cudaError_t launch_search(int op, const SearchParams& p, const LaunchConfig& cfg, int rows_in_flight);
 // The lean one-warp-per-CTA form of the same search (search_fast.cuh); defined in fast_<type>.cu.
 template <int ROWT> cudaError_t launch_search_fast(int op, const SearchParams& p, const LaunchConfig& cfg);
+// The same kernel in its MutableBuffer mode (dynamic indexes, f32 / f16 rows); defined in fast_dynamic.cu.
+cudaError_t launch_search_dynamic(int rowt, int op, const SearchParams& p, const LaunchConfig& cfg);
 // Exhaustive scan with the same distance code (ground truth / flat search).
 template <int ROWT> cudaError_t launch_search_exhaustive(int op, const SearchParams& p, const LaunchConfig& cfg);
 

@@ -754,6 +754,7 @@ int svsb200_flat_search_device(svsb200_index* ix, const void* d_queries, int qdt
     if (k == 0 || k > 1024) return fail("svsb200_flat_search_device: k must be in [1, 1024]");
     if (qdtype < SVSB200_F32 || qdtype > SVSB200_U8) return fail("bad query dtype");
     if (ix->reps.size() != 1) return fail("svsb200_flat_search_device: the index must live on exactly one device");
+    if (ix->dynamic) return fail("svsb200_flat_search_device: flat search is not available on a dynamic index");
     Replica* rep = ix->reps[0].get();
     CUDA_TRY(cudaSetDevice(rep->device));
     std::string err;
@@ -769,6 +770,7 @@ int svsb200_flat_search(svsb200_index* ix, const void* queries, int qdtype, size
     if (!queries || !out_ids || !out_dists) return fail("svsb200_flat_search: NULL buffer");
     if (k == 0 || k > 1024) return fail("svsb200_flat_search: k must be in [1, 1024]");
     if (qdtype < SVSB200_F32 || qdtype > SVSB200_U8) return fail("bad query dtype");
+    if (ix->dynamic) return fail("svsb200_flat_search: flat search is not available on a dynamic index");
     Replica* rep = ix->reps[0].get();
     CUDA_TRY(cudaSetDevice(rep->device));
     std::string err;

@@ -15,10 +15,12 @@
 
 #include "common.cuh"
 
+#include <atomic>
 #include <map>
 #include <memory>
 #include <mutex>
 #include <string>
+#include <unordered_map>
 #include <vector>
 
 namespace svsb200 {
@@ -115,6 +117,10 @@ struct Scratch {
     DeviceBuffer<uint32_t> flat_cid, flat_unv;         // candidates, unverified list (+ its counter in slot 0)
     DeviceBuffer<uint32_t> flat_progress;              // per CTA of the flat GEMM: tiles started (keeps row groups in step)
     DeviceBuffer<uint64_t> flat_i2;
+    DeviceBuffer<uint32_t> dyn_ovf, dyn_qlist;         // dynamic search: overflowed queries, the list being re-run
+    bool dyn_slot_ids = false;                         // dynamic search: write slots, not external ids (filtered / range)
+    int (*cancel_fn)(void*) = nullptr;                 // the caller's cancellation predicate while a search runs
+    void* cancel_arg = nullptr;
     DeviceBuffer<uint64_t> gather_ids, merged_ids;     // sharded search (on the merging device)
     DeviceBuffer<float> gather_dists, merged_dists;
     DeviceBuffer<unsigned int> d_counter;
@@ -143,6 +149,8 @@ struct Replica {
     DeviceBuffer<uint16_t> d_ref_degree;
     DeviceBuffer<float> d_mean;          // LVQ-8: dataset mean
     DeviceBuffer<uint32_t> d_entry;      // entry points when there are several
+    DeviceBuffer<uint8_t> d_status;      // dynamic index: SlotStatus per slot
+    DeviceBuffer<uint64_t> d_ext_ids;    // dynamic index: external id per slot
     // tensor-core flat search: the base vectors as fp16 warpgroup-MMA tiles + per-row bias, built on first use
     DeviceBuffer<unsigned char> flat_b;
     DeviceBuffer<float> flat_bias;
@@ -225,6 +233,14 @@ struct svsb200_index {
     long host_chunks = 0;             // host-buffer searches: pieces per device whose copies overlap the kernels (0 = auto)
     std::mutex mu;
     svsb200::Scratch* last = nullptr; // scratch of the most recent search: counters, kernel time, kernel kind
+    // dynamic index (svsb200_dynamic_*, MutableVamanaIndex): slot status and external ids live on the device
+    // (Replica::d_status / d_ext_ids) and are mirrored here with the external -> slot translator.
+    bool dynamic = false;
+    std::vector<uint8_t> status;
+    std::vector<uint64_t> ext_ids;
+    std::unordered_map<uint64_t, uint32_t> translator;
+    long dyn_slack = -1;              // option "dynamic_slack"
+    std::atomic<long> dyn_reruns{0};  // queries re-run with a larger buffer so far
 };
 
 namespace svsb200 {

@@ -546,6 +546,8 @@ int svsb200_set_counting(svsb200_index* ix, int enabled) {
 int svsb200_set_entry_points(svsb200_index* ix, const uint32_t* entry_points, size_t count) {
     if (!ix || !entry_points) return fail("svsb200_set_entry_points: NULL argument");
     if (count == 0 || count > 32) return fail("svsb200_set_entry_points: 1..32 entry points");
+    // MutableVamanaIndex keeps exactly one entry point (dynamic_index.h:790-793)
+    if (ix->dynamic) return fail("svsb200_set_entry_points: a dynamic index has a single entry point");
     for (size_t i = 0; i < count; ++i)
         if (entry_points[i] >= ix->n) return fail("svsb200_set_entry_points: entry point out of range");
     for (auto& rep : ix->reps) {
@@ -561,6 +563,7 @@ int svsb200_set_entry_points(svsb200_index* ix, const uint32_t* entry_points, si
 
 int svsb200_set_id_offset(svsb200_index* ix, uint64_t offset) {
     if (!ix) return fail("svsb200_set_id_offset: NULL index");
+    if (ix->dynamic) return fail("svsb200_set_id_offset: a dynamic index cannot be a shard");
     ix->id_offset = offset;
     return 0;
 }
@@ -593,6 +596,11 @@ int svsb200_set_option(svsb200_index* ix, const char* name, long value) {
         if (value > 0 && value < 8) return fail("visited_filter_slots must be 0 (off) or at least 8");
         if (value > 16384) return fail("visited_filter_slots must be <= 16384");
         ix->filter_slots = value;
+    } else if (key == "dynamic_slack") {
+        // dynamic index: buffer entries held beyond the capacity for Deleted ones (-1 = default); results never change,
+        // a query that needs more is re-run with more room
+        if (value < -1 || value > (1 << 20)) return fail("dynamic_slack must be in [-1, 2^20]");
+        ix->dyn_slack = value;
     } else {
         return fail("svsb200_set_option: unknown option " + key);
     }
@@ -615,6 +623,8 @@ int svsb200_get_option(svsb200_index* ix, const char* name, long* value) {
     else if (key == "config_search_buffer_capacity") *value = ix->cfg_capacity;
     else if (key == "config_search_buffer_visited_set") *value = ix->cfg_visited;
     else if (key == "entry_point") *value = long(ix->entry_point);
+    else if (key == "dynamic_slack") *value = ix->dyn_slack;
+    else if (key == "dynamic_reruns") *value = long(ix->dyn_reruns);
     else if (key == "streams") {         // scratch sets (= streams) created so far over all replicas
         long c = 0;
         for (auto& rep : ix->reps) {

@@ -246,6 +246,21 @@ __global__ void range_count_kernel(const float* __restrict__ dists, const uint64
     if (c == kk && !exhausted) atomicAdd(unfinished, 1u);
 }
 
+// Dynamic index, filtered search: members whose slot is not Valid are cleared from the bitmap (one thread per word).
+__global__ void keep_valid_kernel(uint32_t* __restrict__ bitmap, const uint8_t* __restrict__ status, size_t n) {
+    const size_t w = size_t(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (w * 32 >= n) return;
+    uint32_t keep = 0;
+    for (uint32_t b = 0; b < 32 && w * 32 + b < n; ++b) keep |= (status[w * 32 + b] == SLOT_VALID ? 1u : 0u) << b;
+    bitmap[w] &= keep;
+}
+
+// Dynamic index: slots -> external ids in place (padding ids stay all-ones).
+__global__ void slots_to_external_kernel(uint64_t* __restrict__ ids, size_t count, const uint64_t* __restrict__ ext_ids) {
+    const size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (i < count && ids[i] != ~uint64_t(0)) ids[i] = ext_ids[ids[i]];
+}
+
 // ---------------------------------------------------------------------------------------
 // Host side
 // ---------------------------------------------------------------------------------------
@@ -408,11 +423,100 @@ template <typename F> static cudaError_t with_row_type(int rowt, F f) {
     }
 }
 
+// Waits for the event `ev` of a dynamic search's launch.  With a cancellation predicate in the scratch it polls it
+// meanwhile and, once it returns non-zero, raises the device flag the kernel polls per query and per hop, waits for the
+// kernel to drain and lowers the flag again.  *cancelled tells whether that happened.
+static int wait_dynamic(Scratch* sc, cudaEvent_t ev, bool* cancelled) {
+    *cancelled = false;
+    if (!sc->cancel_fn) {
+        CUDA_TRY(cudaEventSynchronize(ev));
+        return 0;
+    }
+    for (;;) {
+        const cudaError_t q = cudaEventQuery(ev);
+        if (q == cudaSuccess) break;
+        if (q != cudaErrorNotReady) return fail(std::string("cudaEventQuery: ") + cudaGetErrorString(q));
+        if (!*cancelled && sc->cancel_fn(sc->cancel_arg)) {
+            *cancelled = true;
+            CUDA_TRY(cudaMemsetAsync(sc->d_cancel.ptr, 1, sizeof(int), sc->ctl));
+        }
+        std::this_thread::sleep_for(std::chrono::microseconds(20));
+    }
+    if (*cancelled) {
+        CUDA_TRY(cudaMemsetAsync(sc->d_cancel.ptr, 0, sizeof(int), sc->ctl));
+        CUDA_TRY(cudaStreamSynchronize(sc->ctl));
+    }
+    return 0;
+}
+
+// Search of a dynamic index (MutableVamanaIndex::search, dynamic_index.h:482-571) on the lean kernel's MUT form.  The
+// buffer holds `capacity + slack` entries; queries whose list outgrows it are listed by the kernel and re-run here with
+// four times the room until none is left, so the answer never depends on the slack.  Blocking on `stream`; a
+// cancellation predicate in the scratch is polled while the kernels run (the rows of a cancelled search are unspecified,
+// as in the reference).  The ids written are external ids, or slots when the scratch asks for them (dyn_slot_ids).
+static int search_dynamic(svsb200_index* ix, Replica* rep, Scratch* sc, SearchParams p, LaunchConfig cfg, int op, bool use_fast,
+                          cudaStream_t stream) {
+    const int rowt = ix->dtype;
+    if (ix->storage != SVSB200_PLAIN || (rowt != SVSB200_F32 && rowt != SVSB200_F16))
+        return fail("dynamic index: float32 / float16 plain storage only");
+    if (!use_fast || op > OP_COSF)
+        return fail("dynamic index: the search needs the lean kernel (visited filter on, generic_kernel off, float queries)");
+    const size_t smem_limit = 227 * 1024;
+    const size_t fixed = fast_smem_bytes(p.qstride, 0, p.deg_pad, p.filter_slots * 2u);
+    const size_t max_cap = std::min<size_t>((smem_limit - fixed) / 8 / 32 * 32, size_t(1) << 24);
+    const size_t C = p.capacity;
+    size_t slack = ix->dyn_slack >= 0 ? size_t(ix->dyn_slack) : 3 * C + 32;
+    // a list never holds more than n distinct slots, so n entries of room can never overflow
+    size_t bcap = std::min(std::max(C + slack, C), std::max<size_t>(ix->n, C));
+    if (C > max_cap) return fail("search buffer capacity too large for shared memory");
+    bcap = std::min(bcap, max_cap);
+    p.status = rep->d_status.ptr;
+    p.ext_ids = sc->dyn_slot_ids ? nullptr : rep->d_ext_ids.ptr;
+    CUDA_TRY(sc->dyn_ovf.ensure(1 + size_t(p.nq)));
+    CUDA_TRY(sc->dyn_qlist.ensure(size_t(p.nq)));
+    p.ovf = sc->dyn_ovf.ptr;
+    p.qlist = nullptr;
+    CUDA_TRY(cudaEventRecord(sc->ev_start, stream));
+    for (;;) {
+        p.buf_cap = uint32_t(bcap);
+        p.cap_pad = uint32_t(round_up(bcap, 32));
+        cfg.smem_bytes = fast_smem_bytes(p.qstride, p.cap_pad, p.deg_pad, p.filter_slots * 2u);
+        CUDA_TRY(cudaMemsetAsync(sc->d_counter.ptr, 0, sizeof(unsigned int), stream));
+        CUDA_TRY(cudaMemsetAsync(p.ovf, 0, sizeof(uint32_t), stream));
+        CUDA_TRY(launch_search_dynamic(rowt, op, p, cfg));
+        CUDA_TRY(cudaEventRecord(sc->ev_done, stream));
+        bool cancelled = false;
+        if (int rc = wait_dynamic(sc, sc->ev_done, &cancelled)) return rc;
+        if (cancelled) break;
+        uint32_t over = 0;
+        CUDA_TRY(cudaMemcpyAsync(&over, p.ovf, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
+        CUDA_TRY(cudaStreamSynchronize(stream));
+        if (over == 0) break;
+        if (bcap >= std::max<size_t>(ix->n, C) || bcap >= max_cap)
+            return fail("dynamic index: the search buffer cannot hold the Deleted entries of this query in shared memory");
+        ix->dyn_reruns += long(over);
+        CUDA_TRY(cudaMemcpyAsync(sc->dyn_qlist.ptr, p.ovf + 1, size_t(over) * sizeof(uint32_t), cudaMemcpyDeviceToDevice,
+                                 stream));
+        p.qlist = sc->dyn_qlist.ptr;
+        p.nq = over;
+        bcap = std::min(std::min(4 * bcap + 32, std::max<size_t>(ix->n, C)), max_cap);
+    }
+    CUDA_TRY(cudaEventRecord(sc->ev_stop, stream));
+    sc->timed = true;
+    {
+        std::lock_guard<std::mutex> lock(ix->mu);
+        ix->last = sc;
+    }
+    return 0;
+}
+
 int search_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, const void* d_queries, int qdtype, size_t nq, size_t k,
                      size_t window, size_t capacity, void* d_out_ids, int id_bytes, float* d_out_dists, cudaStream_t stream,
                      bool exhaustive) {
     if (id_bytes != 4 && id_bytes != 8) return fail("id_bytes must be 4 or 8");
     if (qdtype < SVSB200_F32 || qdtype > SVSB200_U8) return fail("bad query dtype");
+    if (ix->dynamic && id_bytes != 8) return fail("a dynamic index returns 64-bit external ids: id_bytes must be 8");
+    if (ix->dynamic && exhaustive) return fail("exhaustive search is not available on a dynamic index");
     if (window > capacity) {
         // SearchBufferConfig::check_invariants (search_buffer.h:87-96)
         return fail("Improper configuration for search buffer! search window size cannot exceed capacity");
@@ -439,6 +543,7 @@ int search_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, const void* d
     bool use_fast = false;
     if (int rc = choose_launch(ix, rep, &p, exhaustive, stream, &cfg, &use_fast)) return rc;
     sc->last_kernel = use_fast ? 1 : 0;
+    if (ix->dynamic) return search_dynamic(ix, rep, sc, p, cfg, op, use_fast, stream);
     const int nrows = ix->rows_in_flight ? int(ix->rows_in_flight) : 2;
     uint32_t split = 1;
     if (exhaustive) {
@@ -570,6 +675,13 @@ static int search_filtered(svsb200_index* ix, Replica* rep, Scratch* sc, const v
     CUDA_TRY(cudaMemcpyAsync(d_bitmap.ptr, id_bitmap, words * 4, cudaMemcpyHostToDevice, sc->stream));
     CUDA_TRY(cudaMemcpyAsync(sc->q_raw.ptr, queries, qbytes, cudaMemcpyHostToDevice, sc->stream));
     CUDA_TRY(cudaMemsetAsync(d_oi.ptr, 0xFF, nq * k * 8, sc->stream));
+    if (ix->dynamic) {
+        // the bitmap is over slots: only Valid slots may be returned; the search lists slots, translated at the end
+        keep_valid_kernel<<<unsigned((words + 255) / 256), 256, 0, sc->stream>>>(d_bitmap.ptr, rep->d_status.ptr, ix->n);
+        count_launch();
+        CUDA_TRY(cudaGetLastError());
+        sc->dyn_slot_ids = true;
+    }
     // lists grow until every query has k members or its search is exhausted
     size_t kk = std::max(k, window);
     int rc = grow_until_done(ix, rep, sc, qdtype, nq, window, &kk, d_found.ptr + nq, [&](size_t len) {
@@ -577,7 +689,13 @@ static int search_filtered(svsb200_index* ix, Replica* rep, Scratch* sc, const v
             reinterpret_cast<const uint64_t*>(sc->ids.ptr), sc->dists.ptr, uint32_t(nq), uint32_t(len), uint32_t(k),
             d_bitmap.ptr, d_oi.ptr, d_od.ptr, d_found.ptr, d_found.ptr + nq);
     });
+    sc->dyn_slot_ids = false;
     if (rc) return rc;
+    if (ix->dynamic) {
+        slots_to_external_kernel<<<unsigned((nq * k + 255) / 256), 256, 0, sc->stream>>>(d_oi.ptr, nq * k, rep->d_ext_ids.ptr);
+        count_launch();
+        CUDA_TRY(cudaGetLastError());
+    }
     std::vector<uint32_t> found(nq);
     CUDA_TRY(cudaMemcpyAsync(found.data(), d_found.ptr, nq * 4, cudaMemcpyDeviceToHost, sc->stream));
     CUDA_TRY(cudaMemcpyAsync(out_ids, d_oi.ptr, nq * k * 8, cudaMemcpyDeviceToHost, sc->stream));
@@ -607,7 +725,7 @@ static int range_search(svsb200_index* ix, Replica* rep, Scratch* sc, const void
             sc->dists.ptr, reinterpret_cast<const uint64_t*>(sc->ids.ptr), uint32_t(nq), uint32_t(len), radius,
             ix->metric != SVSB200_L2, d_counts.ptr, d_counts.ptr + nq);
     });
-    if (rc) return rc;
+    if (rc) return rc;   // (on a dynamic index the list holds no Deleted slot and its ids are already external)
     CUDA_TRY(cudaMemcpyAsync(out_counts, d_counts.ptr, nq * 4, cudaMemcpyDeviceToHost, sc->stream));
     std::vector<uint64_t> ids(nq * kk);
     std::vector<float> dd(nq * kk);
@@ -783,6 +901,8 @@ int svsb200_search_cancellable(svsb200_index* ix, const void* queries, int qdtyp
         used_m.push_back(m);
         sc->timed = false;
         sc->poll_cancel = cancel != nullptr;
+        sc->cancel_fn = ix->dynamic ? cancel : nullptr;   // a dynamic search waits for its kernels itself
+        sc->cancel_arg = cancel_arg;
         auto step = [&]() -> int {
             CUDA_TRY(sc->q_raw.ensure(m * qrow));
             CUDA_TRY(sc->ids.ensure(m * k * size_t(id_bytes)));
@@ -815,6 +935,7 @@ int svsb200_search_cancellable(svsb200_index* ix, const void* queries, int qdtyp
     if (rc_wait == 0) rc_wait = wait_all(used);
     for (size_t i = 0; i < used.size(); ++i) {
         used[i]->poll_cancel = false;
+        used[i]->cancel_fn = nullptr;
         if (used_rep[i]) release(used_rep[i], used[i]);
     }
     if (rc) return fail(first_error);
@@ -873,6 +994,7 @@ int svsb200_search_sharded(svsb200_index* const* shards, size_t nshards, const v
     if (qdtype < SVSB200_F32 || qdtype > SVSB200_U8) return fail("bad query dtype");
     for (size_t s = 0; s < nshards; ++s) {
         if (!shards[s] || shards[s]->reps.size() != 1) return fail("svsb200_search_sharded: every shard is a single-device index");
+        if (shards[s]->dynamic) return fail("svsb200_search_sharded: a dynamic index cannot be a shard");
         if (shards[s]->dim != shards[0]->dim || shards[s]->metric != shards[0]->metric)
             return fail("svsb200_search_sharded: shards disagree on dimension or metric");
     }

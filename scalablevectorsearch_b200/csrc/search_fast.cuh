@@ -48,7 +48,21 @@ static __device__ unsigned long long g_phase_clocks[8];   // (one copy per trans
 
 // HIST = true is the graph builder's form (build.cu): every expanded node is appended, with its key, to the
 // query's search history -- the reference's `use_full_search_history` candidate pool (vamana_build.h:344-352).
-template <int ROWT, int OP, int DS, int KS, bool HIST = false>
+//
+// MUT = true is the search of a dynamic index: MutableVamanaIndex::search (dynamic_index.h:482-571), i.e. the
+// MutableBuffer (dynamic_search_buffer.h:41-617) filled through ValidBuilder (dynamic_index.h:93-108).  A candidate
+// whose slot is Deleted is inserted with the invalid bit set: the walk goes through it, but it does not count
+// towards the window or the capacity.  With V = the number of valid entries the buffer holds:
+//   * full() is V == capacity, and can_skip compares with the last entry, the capacity-th valid one once full;
+//   * every entry behind the capacity-th valid one is dropped (the no-split resize to roi_end_ and the split
+//     buffer's walk_back truncation both amount to this);
+//   * next() / done() look at [0, roi_end), roi_end = one past the window-th valid entry, or the size while
+//     V < window.
+// These are functions of the merged list alone, so the group-of-32 merge stays equal to one-by-one inserts
+// (tests/test_mutable_buffer.py).  Invalid entries make the list longer than `capacity`: it is held in `buf_cap`
+// entries, and a query whose cut point would lie beyond them stops, lists itself in `ovf` and is re-run by the host
+// with more room.  The copy-out is cleanup() + the first k valid entries, as external ids.
+template <int ROWT, int OP, int DS, int KS, bool HIST = false, bool MUT = false>
 __global__ void __launch_bounds__(32, fast_min_blocks<ROWT, OP, DS, KS>()) vamana_search_fast_kernel(const __grid_constant__ SearchParams p) {
     constexpr int NROWS = 2;
     constexpr bool kInt = (OP >= OP_L2I);
@@ -56,6 +70,8 @@ __global__ void __launch_bounds__(32, fast_min_blocks<ROWT, OP, DS, KS>()) vaman
     constexpr int GROUPS = 32 / G;                            // rows per slot of a pass
     constexpr unsigned FULL = 0xFFFFFFFFu;
     constexpr uint32_t NONE = 0xFFFFFFFFu;
+    constexpr uint32_t idmask = MUT ? (kIdMask & ~kInvalidBit) : kIdMask;
+    static_assert(!(HIST && MUT), "the builder searches a static graph");
 
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int lane = threadIdx.x;
@@ -82,6 +98,9 @@ __global__ void __launch_bounds__(32, fast_min_blocks<ROWT, OP, DS, KS>()) vaman
         if (lane == 0) q = atomicAdd(p.work_counter, 1u);
         q = __shfl_sync(FULL, q, 0);
         if (q >= p.nq) break;
+        if constexpr (MUT) {
+            if (p.qlist) q = p.qlist[q];
+        }
         // cancellation between queries (extensions.h:579)
         if (p.cancel && *reinterpret_cast<const volatile int*>(p.cancel)) break;
 
@@ -105,6 +124,8 @@ __global__ void __launch_bounds__(32, fast_min_blocks<ROWT, OP, DS, KS>()) vaman
         const uint32_t E = p.n_entry > 1 ? min(p.n_entry, 32u) : 1u;   // entry points (index/vamana/index.h:304-312)
         uint32_t size = 0, cursor = 0, n_hops = 0, n_evals = E, n_fetched = E;
         uint32_t n_hist = 0;
+        uint32_t nvalid = 0, roi_end = 0;     // MUT: valid entries, one past the window-th valid one
+        bool overflow = false;                // MUT: the list outgrew buf_cap before its cut point
         uint32_t staged_node = NONE;          // node whose adjacency row sits in nxt[]
         uint32_t nxt[kFastMaxGW];
 #pragma unroll
@@ -127,8 +148,8 @@ __global__ void __launch_bounds__(32, fast_min_blocks<ROWT, OP, DS, KS>()) vaman
                 ncand = E;
                 __syncwarp();
             } else {
-            // buffer.next(): first unvisited entry inside min(size, window)
-            const uint32_t upper = min(size, W);
+            // buffer.next(): first unvisited entry inside min(size, window)  (MUT: inside roi_end)
+            const uint32_t upper = MUT ? roi_end : min(size, W);
             uint32_t pos = cursor, pred_pos = NONE;
             bool found = false;
 #pragma unroll 1
@@ -150,7 +171,7 @@ __global__ void __launch_bounds__(32, fast_min_blocks<ROWT, OP, DS, KS>()) vaman
             if (!found) break;   // done()
             // (masked: lane 0 sets the visited bit of this entry below, and nothing orders that store behind the other
             // lanes' read of it -- compute-sanitizer racecheck, round 2)
-            const uint32_t node = buf[pos].y & kIdMask;
+            const uint32_t node = buf[pos].y & idmask;
             // graph.get_node(node): staged in registers by the previous hop if the prediction held; a miss
             // loads into the same registers.  nb[] is copied out BEFORE the next prefetch is issued into nxt[]:
             // the write-after-read dependence keeps the prefetch loads behind every wait on this hop's row, so
@@ -166,13 +187,17 @@ __global__ void __launch_bounds__(32, fast_min_blocks<ROWT, OP, DS, KS>()) vaman
             for (int w = 0; w < kFastMaxGW; ++w) nb[w] = nxt[w];
             staged_node = NONE;
             if (pred_pos != NONE) {
-                staged_node = buf[pred_pos].y & kIdMask;
+                staged_node = buf[pred_pos].y & idmask;
                 const uint32_t* prow = p.graph + size_t(staged_node) * p.gstride;
 #pragma unroll
                 for (int w = 0; w < kFastMaxGW; ++w)
                     if (w * 32u < p.gstride) nxt[w] = __ldg(prow + w * 32u + lane);
             }
-            if (lane == 0) buf[pos].y = node | kVisitedBit;
+            if constexpr (MUT) {
+                if (lane == 0) buf[pos].y = (buf[pos].y & kInvalidBit) | node | kVisitedBit;
+            } else {
+                if (lane == 0) buf[pos].y = node | kVisitedBit;
+            }
             if constexpr (HIST) {
                 if (lane == 0 && n_hist < p.hist_cap) p.hist[size_t(q) * p.hist_cap + n_hist] = make_uint2(buf[pos].x, node);
                 n_hist += (n_hist < p.hist_cap) ? 1u : 0u;
@@ -249,8 +274,8 @@ __global__ void __launch_bounds__(32, fast_min_blocks<ROWT, OP, DS, KS>()) vaman
                 const bool valid = r < ncand;
                 const float d = valid ? ckey[r] : 0.0f;
                 const uint32_t id = valid ? cid[r] : 0u;
-                // can_skip (search_buffer.h:342-344): full && cmp(back, d)
-                const bool full = (size == C);
+                // can_skip (search_buffer.h:342-344): full && cmp(back, d)   (MUT: dynamic_search_buffer.h:413-417)
+                const bool full = MUT ? (nvalid == C) : (size == C);
                 const float backkey = full ? __uint_as_float(buf[size - 1].x) : 0.0f;   // C >= 1, so full implies size >= 1
                 bool surv = valid && !(full && backkey < d);
                 if (!__any_sync(FULL, surv)) continue;
@@ -268,7 +293,7 @@ __global__ void __launch_bounds__(32, fast_min_blocks<ROWT, OP, DS, KS>()) vaman
                     while (j > 0) {
                         const uint2 e = buf[--j];
                         if (__uint_as_float(e.x) < d) break;
-                        if ((e.y & kIdMask) == id) {
+                        if ((e.y & idmask) == id) {
                             surv = false;
                             break;
                         }
@@ -304,9 +329,14 @@ __global__ void __launch_bounds__(32, fast_min_blocks<ROWT, OP, DS, KS>()) vaman
                 __syncwarp();   // every lane is done reading the compacted keys
                 if (surv) {
                     skc[rank] = d;
-                    sid[rank] = id;
+                    if constexpr (MUT) {   // ValidBuilder: invalid iff the slot is Deleted
+                        sid[rank] = id | (p.status[id] == SLOT_DELETED ? kInvalidBit : 0u);
+                    } else {
+                        sid[rank] = id;
+                    }
                 }
-                const uint32_t newsize = min(size + S, C);
+                const uint32_t newsize = min(size + S, MUT ? p.buf_cap : C);
+                const uint32_t merged = size + S;   // MUT: length of the merged list before any cut
                 const int top = int((newsize - 1) >> 5), lo = int(minpos >> 5);
                 // Final slot f holds either the survivor with fp == f or the old entry f - #{fp < f}.  Done in
                 // place, top-down, 128 entries (4 x 32) at a time: a block only reads the old buffer inside itself
@@ -342,6 +372,34 @@ __global__ void __launch_bounds__(32, fast_min_blocks<ROWT, OP, DS, KS>()) vaman
                 size = newsize;
                 cursor = min(cursor, minpos);   // best_unvisited = min(best_unvisited, i) (:401)
                 __syncwarp();
+                if constexpr (MUT) {
+                    // cut behind the capacity-th valid entry; roi_end behind the window-th (dynamic_search_buffer.h:295-411)
+                    uint32_t v = 0, cut = NONE, roiw = NONE;
+#pragma unroll 1
+                    for (uint32_t j0 = 0; j0 < size && cut == NONE; j0 += 32) {
+                        const uint32_t j = j0 + lane;
+                        const bool ok = j < size && !(buf[j].y & kInvalidBit);
+                        const unsigned mv = __ballot_sync(FULL, ok);
+                        const uint32_t nth = v + __popc(mv & lt_mask) + 1;   // this entry is the nth valid one
+                        const unsigned mw = __ballot_sync(FULL, ok && nth == W);
+                        const unsigned mc = __ballot_sync(FULL, ok && nth == C);
+                        if (mw) roiw = j0 + __ffs(mw) - 1;
+                        if (mc) cut = j0 + __ffs(mc) - 1;
+                        v += __popc(mv);
+                    }
+                    if (cut != NONE) {
+                        size = cut + 1;
+                        nvalid = C;
+                    } else {
+                        nvalid = v;
+                        overflow = merged > size;   // entries behind buf_cap were lost before the cut
+                    }
+                    roi_end = nvalid >= W ? roiw + 1 : size;
+                    if (overflow) break;
+                }
+            }
+            if constexpr (MUT) {
+                if (overflow) break;
             }
 #ifdef SVSB200_PHASE_CLOCKS
             if (lane == 0) {
@@ -356,6 +414,44 @@ __global__ void __launch_bounds__(32, fast_min_blocks<ROWT, OP, DS, KS>()) vaman
             if (cancelled) break;
         }
 
+        if constexpr (MUT) {
+            if (overflow) {   // not written: the host re-runs this query with more room
+                if (lane == 0) p.ovf[1 + atomicAdd(p.ovf, 1u)] = q;
+                __syncwarp();
+                continue;
+            }
+            // buffer.cleanup() (dynamic_search_buffer.h:521-525), then the first k valid entries as external ids
+            // (translate_to_external, dynamic_index.h:566-570); the tail is padded like the static copy-out
+            uint32_t cnt = 0;
+#pragma unroll 1
+            for (uint32_t j0 = 0; j0 < size && cnt < p.k; j0 += 32) {
+                const uint32_t j = j0 + lane;
+                const uint2 e = j < size ? buf[j] : make_uint2(0u, kInvalidBit);
+                const bool ok = !(e.y & kInvalidBit);
+                const unsigned m = __ballot_sync(FULL, ok);
+                const uint32_t o = cnt + __popc(m & lt_mask);
+                if (ok && o < p.k) {
+                    const size_t oo = size_t(q) * p.k + o;
+                    const uint32_t slot = e.y & idmask;
+                    reinterpret_cast<uint64_t*>(p.out_ids)[oo] = p.ext_ids ? p.ext_ids[slot] : uint64_t(slot);
+                    p.out_dists[oo] = __fmul_rn(__uint_as_float(e.x), ksign);
+                }
+                cnt += __popc(m);
+            }
+#pragma unroll 1
+            for (uint32_t j = cnt + lane; j < p.k; j += 32) {
+                const size_t oo = size_t(q) * p.k + j;
+                reinterpret_cast<uint64_t*>(p.out_ids)[oo] = ~uint64_t(0);
+                p.out_dists[oo] = p.greater ? -INFINITY : INFINITY;
+            }
+            if (p.hops && lane == 0) {
+                p.hops[q] = n_hops;
+                p.evals[q] = n_evals;
+                p.fetched[q] = n_fetched;
+            }
+            __syncwarp();
+            continue;
+        }
         // ---- copy the first k entries out (extensions.h:588-590) ----
 #pragma unroll 1
         for (uint32_t j = lane; j < p.k; j += 32) {
@@ -382,9 +478,9 @@ __global__ void __launch_bounds__(32, fast_min_blocks<ROWT, OP, DS, KS>()) vaman
     }
 }
 
-template <int ROWT, int OP, int DS, int KS = 1, bool HIST = false>
+template <int ROWT, int OP, int DS, int KS = 1, bool HIST = false, bool MUT = false>
 cudaError_t launch_fast(const SearchParams& p, const LaunchConfig& cfg) {
-    auto kernel = vamana_search_fast_kernel<ROWT, OP, DS, KS, HIST>;
+    auto kernel = vamana_search_fast_kernel<ROWT, OP, DS, KS, HIST, MUT>;
     cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(cfg.smem_bytes));
     if (err != cudaSuccess) return err;
     int grid = cfg.grid;
@@ -410,6 +506,14 @@ template <int ROWT, int OP, bool HIST = false> cudaError_t launch_fast_dims(cons
         if (p.dim >= 256 && !p.no_split) return launch_fast<ROWT, OP, 0, 4, HIST>(p, cfg);
     }
     return launch_fast<ROWT, OP, 0, 1, HIST>(p, cfg);
+}
+
+// Dimension dispatch of the MUT kernels: the same shapes as the static search.
+template <int ROWT, int OP> cudaError_t launch_fast_dims_mut(const SearchParams& p, const LaunchConfig& cfg) {
+    if (p.dim == 96) return launch_fast<ROWT, OP, 96, 1, false, true>(p, cfg);
+    if (p.dim == 128) return launch_fast<ROWT, OP, 128, 1, false, true>(p, cfg);
+    if (p.dim >= 256 && !p.no_split) return launch_fast<ROWT, OP, 0, 4, false, true>(p, cfg);
+    return launch_fast<ROWT, OP, 0, 1, false, true>(p, cfg);
 }
 
 }  // namespace svsb200

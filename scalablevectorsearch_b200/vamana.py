@@ -365,7 +365,7 @@ class Vamana:
         Returns (ids uint64, distances, found per query); short rows are padded with all-ones / +inf."""
         q = np.ascontiguousarray(queries)
         mask = np.ascontiguousarray(allowed, dtype=bool)
-        if mask.shape != (self.size,):
+        if mask.shape != (self._lib.svsb200_index_size(self._h),):
             raise ValueError("allowed must hold one boolean per indexed vector")
         bitmap = np.packbits(mask, bitorder="little")
         bitmap = np.concatenate([bitmap, np.zeros((-len(bitmap)) % 4, dtype=np.uint8)]).view(np.uint32)
@@ -484,3 +484,90 @@ class ShardedVamana:
                                                     cfg.search_window_size, cfg.search_buffer_capacity,
                                                     ids.ctypes.data, dists.ctypes.data))
         return ids, dists
+
+
+class DynamicVamana(Vamana):
+    """GPU-backed dynamic Vamana index: the reference's ``svs.DynamicVamana`` / ``MutableVamanaIndex``
+    (bindings/python/src/dynamic_vamana.cpp, include/svs/index/vamana/dynamic_index.h) assembled from a graph, its
+    data and one external id per row, with soft deletion.  Searches return external ids and never return a deleted
+    one, while the walk still goes through deleted rows, exactly as ``MutableVamanaIndex::search`` does.  Mutations
+    must not run concurrently with searches of the same index.  float32 / float16 data, one device."""
+
+    @classmethod
+    def from_arrays(cls, data: np.ndarray, graph: np.ndarray, entry_point: int, ids=None,
+                    distance: DistanceType = DistanceType.L2, device: int = 0, num_threads: int = 1) -> "DynamicVamana":
+        """``MutableVamanaIndex(graph, data, entry_point, distance, external_ids, threadpool)``
+        (dynamic_index.h:178-202); ``ids`` defaults to ``0 .. n-1``."""
+        data = np.ascontiguousarray(data)
+        graph = np.ascontiguousarray(graph, dtype=np.uint32)
+        if data.ndim != 2 or graph.ndim != 2:
+            raise ValueError("data and graph must be 2-D")
+        if data.dtype not in (np.float32, np.float16):
+            raise TypeError("a dynamic index takes float32 / float16 data")
+        if graph.shape[0] != data.shape[0]:
+            raise ValueError("Wrong sizes!")
+        n = data.shape[0]
+        ids = np.arange(n, dtype=np.uint64) if ids is None else np.ascontiguousarray(ids, dtype=np.uint64)
+        if ids.shape != (n,):
+            raise ValueError("one external id per row")
+        self = cls.__new__(cls)
+        self._lib = _lib.lib()
+        self._distance = DistanceType(distance)
+        self._dtype = data.dtype
+        self._params = VamanaSearchParameters()
+        self._num_threads = int(num_threads)
+        handle = C.c_void_p()
+        _lib.check(self._lib.svsb200_dynamic_create(
+            data.ctypes.data, _DTYPE_CODE[data.dtype], n, data.shape[1], graph.ctypes.data, graph.shape[1],
+            int(entry_point), int(self._distance), ids.ctypes.data, int(device), C.byref(handle)))
+        self._h = handle
+        return self
+
+    @property
+    def size(self) -> int:
+        """Number of valid (searchable) entries (``MutableVamanaIndex::size``)."""
+        n = C.c_size_t(0)
+        _lib.check(self._lib.svsb200_dynamic_ids(self._h, None, C.byref(n)))
+        return int(n.value)
+
+    @property
+    def num_slots(self) -> int:
+        """Rows held on the device, deleted ones included."""
+        return self._lib.svsb200_index_size(self._h)
+
+    def all_ids(self) -> np.ndarray:
+        """External ids of every valid entry (``all_ids``), in slot order."""
+        n = C.c_size_t(self.size)
+        out = np.empty(n.value, dtype=np.uint64)
+        _lib.check(self._lib.svsb200_dynamic_ids(self._h, out.ctypes.data, C.byref(n)))
+        return out[: n.value]
+
+    def has_id(self, id: int) -> bool:
+        out = C.c_int()
+        _lib.check(self._lib.svsb200_dynamic_has_id(self._h, int(id), C.byref(out)))
+        return bool(out.value)
+
+    def delete(self, ids) -> int:
+        """Soft deletion (``delete_entries``, dynamic_index.h:773-788): fails without changing anything unless every
+        id is present.  Returns the number of deleted entries."""
+        ids = np.ascontiguousarray(np.atleast_1d(ids), dtype=np.uint64)
+        _lib.check(self._lib.svsb200_dynamic_delete(self._h, ids.ctypes.data, len(ids)))
+        return len(ids)
+
+    def search_filtered(self, queries: np.ndarray, n_neighbors: int, allowed: np.ndarray):
+        """Filtered search: ``allowed`` is a boolean mask over the SLOTS (``num_slots`` entries, in the order of
+        :meth:`export`); entries that are not valid are never returned.  Returns external ids, distances and the
+        number found per query."""
+        return super().search_filtered(queries, n_neighbors, allowed)
+
+    def export(self):
+        """(graph uint32[n][R+1] degree first, status uint8[n] (0 Empty, 1 Valid, 2 Deleted), external ids, entry
+        point) over every slot."""
+        n, R = self.num_slots, self.graph_max_degree
+        graph = np.empty((n, R + 1), dtype=np.uint32)
+        status = np.empty(n, dtype=np.uint8)
+        ids = np.empty(n, dtype=np.uint64)
+        ep = C.c_uint32()
+        _lib.check(self._lib.svsb200_dynamic_export(self._h, graph.ctypes.data, status.ctypes.data, ids.ctypes.data,
+                                                    C.byref(ep)))
+        return graph, status, ids, int(ep.value)
