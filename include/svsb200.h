@@ -308,6 +308,44 @@ int svsb200_dynamic_has_id(const svsb200_index* index, uint64_t id, int* out);
 int svsb200_dynamic_export(const svsb200_index* index, uint32_t* graph_rows_out, uint8_t* status_out,
                            uint64_t* ext_ids_out, uint32_t* entry_point_out);
 
+/* Mutation parameters: alpha_, construction_window_size_, max_candidates_ and prune_to_ of MutableVamanaIndex
+ * (dynamic_index.h:316-371), used by svsb200_dynamic_add and svsb200_dynamic_consolidate.  0 selects the default:
+ * alpha 1.2 (L2) / 0.95 (MIP, cosine), window 2 * max_degree, max_candidates 3 * window clamped to 512, prune_to
+ * max_degree - 4 (max_degree when below 16).  The GPU builder's candidate pool holds 512 entries, so max_candidates
+ * above 512 is an error, as are an alpha on the wrong side of 1, prune_to > max_degree and a window that leaves the
+ * pool no room.  An index starts with the defaults (svsb200_dynamic_build: with its build parameters).  The search
+ * history is always kept in full (use_full_search_history = true). */
+int svsb200_dynamic_set_build_parameters(svsb200_index* index, float alpha, size_t window_size, size_t max_candidates,
+                                         size_t prune_to);
+/* Any output may be NULL. */
+int svsb200_dynamic_get_build_parameters(const svsb200_index* index, float* alpha, size_t* window_size,
+                                         size_t* max_candidates, size_t* prune_to);
+/* add_points (dynamic_index.h:657-749): `count` rows of the index's dtype (dense, HOST) with one new external id
+ * each.  Slots are chosen as the reference chooses them: Empty slots from first_empty (from slot 0 when reuse_empty
+ * is non-zero), then new slots past the end; first_empty becomes max(first_empty, last slot + 1).  The rows are
+ * linked in by one pass of the graph builder over the slots (VamanaBuilder::construct with alpha), whose search walks
+ * Deleted slots too; the slots become Valid afterwards.  Everything (dtype, repeated, present or reserved ids) is
+ * checked before anything changes.  `slots_out` (optional, `count` entries) receives the slots used.  The device
+ * arrays grow geometrically; svsb200_index_size then reports the new number of slots. */
+int svsb200_dynamic_add(svsb200_index* index, const void* vectors, int dtype, size_t count, const uint64_t* ids,
+                        int reuse_empty, uint64_t* slots_out);
+/* consolidate (dynamic_index.h:976-1013, consolidate.h): a Deleted entry point is replaced by the medoid of the Valid
+ * rows (fails, changing nothing, when none is left); every Valid node with a neighbour that is not Valid gets its
+ * row rebuilt from its Valid neighbours and the rows of the others, truncated to max_candidates and pruned to
+ * prune_to with alpha; then every Deleted slot becomes Empty.  Ties among exactly equal distances are broken by id
+ * (the reference leaves their order unspecified). */
+int svsb200_dynamic_consolidate(svsb200_index* index);
+/* compact (dynamic_index.h:817-916): the Valid slots move, in ascending order, to [0, size): rows, adjacency rows
+ * (ids remapped), status, external ids and entry point; the allocations shrink to fit.  Fails without changing
+ * anything while a Deleted slot is present (consolidate first). */
+int svsb200_dynamic_compact(svsb200_index* index);
+/* MutableVamanaIndex(parameters, data, external_ids, distance) (dynamic_index.h:208-261): svsb200_build_vamana's
+ * two passes, then svsb200_dynamic_create; the build parameters (defaults as for svsb200_dynamic_set_build_parameters)
+ * become the mutation parameters. */
+int svsb200_dynamic_build(const void* vectors, int dtype, size_t n, size_t dim, int metric, float alpha,
+                          size_t graph_max_degree, size_t window_size, size_t max_candidates, size_t prune_to,
+                          const uint64_t* external_ids, int device, svsb200_index** out);
+
 #ifdef __cplusplus
 }
 #endif

@@ -24,7 +24,8 @@ SYMBOLS = [
     "svsb200_search_sharded", "svsb200_build_vamana", "svsb200_flat_search_device", "svsb200_flat_search", "svsb200_index_assemble", "svsb200_toml_get", "svsb200_search_filtered", "svsb200_range_search", "svsb200_free", "svsb200_set_entry_points",
     "svsb200_flat_plan",
     "svsb200_dynamic_create", "svsb200_dynamic_delete", "svsb200_dynamic_ids", "svsb200_dynamic_has_id",
-    "svsb200_dynamic_export",
+    "svsb200_dynamic_export", "svsb200_dynamic_set_build_parameters", "svsb200_dynamic_get_build_parameters",
+    "svsb200_dynamic_add", "svsb200_dynamic_consolidate", "svsb200_dynamic_compact", "svsb200_dynamic_build",
 ]
 
 _lib = None
@@ -90,6 +91,12 @@ def lib() -> C.CDLL:
     l.svsb200_dynamic_ids.argtypes = [vp, vp, C.POINTER(sz)]
     l.svsb200_dynamic_has_id.argtypes = [vp, C.c_uint64, C.POINTER(i32)]
     l.svsb200_dynamic_export.argtypes = [vp, vp, vp, vp, C.POINTER(u32)]
+    l.svsb200_dynamic_set_build_parameters.argtypes = [vp, C.c_float, sz, sz, sz]
+    l.svsb200_dynamic_get_build_parameters.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(sz), C.POINTER(sz), C.POINTER(sz)]
+    l.svsb200_dynamic_add.argtypes = [vp, vp, i32, sz, vp, i32, vp]
+    l.svsb200_dynamic_consolidate.argtypes = [vp]
+    l.svsb200_dynamic_compact.argtypes = [vp]
+    l.svsb200_dynamic_build.argtypes = [vp, i32, sz, sz, i32, C.c_float, sz, sz, sz, sz, vp, i32, C.POINTER(vp)]
     _lib = l
     return l
 

@@ -21,4 +21,14 @@ template <> cudaError_t launch_build_prune_op<SVSB200_F32>(int op, const SearchP
     }
 }
 
+template <> cudaError_t launch_consolidate_pool_op<SVSB200_F32>(int op, const SearchParams& p, const BuildParams& bp, int grid,
+                                                                cudaStream_t stream) {
+    switch (op) {
+        case OP_L2F: return launch_consolidate_pool<SVSB200_F32, OP_L2F>(p, bp, grid, stream);
+        case OP_IPF: return launch_consolidate_pool<SVSB200_F32, OP_IPF>(p, bp, grid, stream);
+        case OP_COSF: return launch_consolidate_pool<SVSB200_F32, OP_COSF>(p, bp, grid, stream);
+        default: return cudaErrorInvalidValue;
+    }
+}
+
 }  // namespace svsb200

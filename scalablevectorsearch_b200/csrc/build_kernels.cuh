@@ -16,6 +16,10 @@
 // The reference's result depends on thread timing (vertex locks, bucket order), so the parity bar is the
 // reference's own: recall equivalence of the built index (tests/integration/vamana/index_build.cpp:96,139).
 // Distances inside the builder use the search path's bit-exact code (eval_pass), keys = sign * distance.
+//
+// The dynamic index reuses these kernels: add_points runs `construct` over a list of slots (BuildParams::slots),
+// and consolidate (consolidate.h) selects each node's candidate pool with `consolidate_pool_kernel` and prunes it
+// with `build_prune_kernel` in mode CONSOLIDATE.
 #pragma once
 
 #include "search_fast.cuh"
@@ -26,14 +30,20 @@ namespace svsb200 {
 
 constexpr uint32_t kPoolMax = 512;   // candidate pool entries per node held in shared memory
 
+enum BuildPruneMode : int {
+    PRUNE_FORWARD = 0,       // pool = search history + adjacency
+    PRUNE_REVERSE = 1,       // pool = overflow edges + adjacency
+    PRUNE_CONSOLIDATE = 2,   // pool = hist[w] as given (consolidate_pool_kernel's selection)
+};
+
 struct BuildParams {
-    int reverse;                 // 0: forward (pool = search history + adjacency), 1: reverse (overflow + adjacency)
-    uint32_t first;              // forward: first node of the batch (node = first + i, query row i)
-    uint32_t count;              // forward: batch size
+    int reverse;                 // BuildPruneMode
+    uint32_t first;              // forward: first entry of the batch (node = first + i, or slots[first + i]; query row i)
+    uint32_t count;              // forward / consolidate: batch size
     const uint32_t* count_ptr;   // reverse: number of touched vertices (device)
-    const uint32_t* nodes;       // reverse: the touched vertices
-    const uint2* hist;           // forward: [count][hist_cap] {key bits, id}
-    const uint32_t* hist_count;
+    const uint32_t* nodes;       // reverse: the touched vertices; consolidate: the batch's nodes
+    uint2* hist;                 // forward, consolidate: [count][hist_cap] {key bits, id}
+    uint32_t* hist_count;
     uint32_t hist_cap;
     const int* head;             // reverse: overflow linked lists (head per vertex, -1 = empty)
     const int* next;
@@ -47,6 +57,11 @@ struct BuildParams {
     float alpha;
     int iterative;               // prune strategy: 0 = Progressive (L2), 1 = Iterative (inner product, cosine)
     unsigned int* work_counter;
+    const uint32_t* slots;       // forward: the batch's nodes are slots[first + i] (NULL: first + i)
+    const uint8_t* status;       // consolidate_pool_kernel: SlotStatus per slot
+    uint32_t* scratch_ids;       // consolidate_pool_kernel: [grid][scratch_len] per warp
+    float* scratch_keys;
+    uint32_t scratch_len;        // a power of two >= max_degree^2
 };
 
 // Per-CTA (one warp) shared memory of build_prune_kernel.
@@ -75,6 +90,35 @@ __device__ __forceinline__ float stage_row(const SearchParams& p, uint32_t id, f
     return sqrtf(sq);
 }
 
+// Sorts the first `count` (key, id) pairs by TotalOrder (key, then id), one warp: bitonic over the next power of two
+// >= 32, the tail padded with (+inf, 0xFFFFFFFF).  The arrays (shared or global) need room for that power of two.
+__device__ __forceinline__ void warp_sort_pairs(float* key, uint32_t* id, uint32_t count, int lane) {
+    uint32_t N = 32;
+    while (N < count) N <<= 1;
+    for (uint32_t i = count + lane; i < N; i += 32) {
+        key[i] = INFINITY;
+        id[i] = 0xFFFFFFFFu;
+    }
+    __syncwarp();
+    for (uint32_t k = 2; k <= N; k <<= 1) {
+        for (uint32_t j = k >> 1; j > 0; j >>= 1) {
+            for (uint32_t i = lane; i < N / 2; i += 32) {
+                const uint32_t a = ((i & ~(j - 1)) << 1) | (i & (j - 1));
+                const uint32_t b = a | j;
+                const bool up = (a & k) == 0;
+                const float ka = key[a], kb = key[b];
+                const uint32_t ia = id[a], ib = id[b];
+                const bool a_gt_b = (kb < ka) || (!(ka < kb) && ib < ia);
+                if (a_gt_b == up) {
+                    key[a] = kb; key[b] = ka;
+                    id[a] = ib; id[b] = ia;
+                }
+            }
+            __syncwarp();
+        }
+    }
+}
+
 template <int ROWT, int OP, int DS, int KS>
 __global__ void __launch_bounds__(32, 16) build_prune_kernel(const __grid_constant__ SearchParams p,
                                                             const __grid_constant__ BuildParams bp) {
@@ -95,14 +139,14 @@ __global__ void __launch_bounds__(32, 16) build_prune_kernel(const __grid_consta
     uint32_t* res = lpos + kPoolMax;                                  // [256] result
     const char* vectors = reinterpret_cast<const char*>(p.vectors);
     const float ksign = p.greater ? -1.0f : 1.0f;
-    const uint32_t total = bp.reverse ? *bp.count_ptr : bp.count;
+    const uint32_t total = bp.reverse == PRUNE_REVERSE ? *bp.count_ptr : bp.count;
 
     for (;;) {
         uint32_t w = 0;
         if (lane == 0) w = atomicAdd(bp.work_counter, 1u);
         w = __shfl_sync(FULL, w, 0);
         if (w >= total) break;
-        const uint32_t node = bp.reverse ? bp.nodes[w] : bp.first + w;
+        const uint32_t node = bp.reverse ? bp.nodes[w] : bp.slots ? bp.slots[bp.first + w] : bp.first + w;
         const uint32_t deg0 = min(bp.deg[node], bp.max_degree);
         uint32_t* row = bp.graph + size_t(node) * bp.gstride;
 
@@ -110,7 +154,16 @@ __global__ void __launch_bounds__(32, 16) build_prune_kernel(const __grid_consta
         uint32_t P = 0;       // entries whose key is known
         uint32_t M = 0;       // entries of lid[] whose distance to `node` still has to be computed
         float qnorm = 1.0f;   // cosine: norm of the vector currently staged as the query
-        if (!bp.reverse) {
+        if (bp.reverse == PRUNE_CONSOLIDATE) {
+            // the whole pool, keys included, as consolidate_pool_kernel selected it
+            qnorm = stage_row<ROWT>(p, node, q_s, lane);
+            P = min(bp.hist_count[w], min(bp.hist_cap, kPoolMax));
+            for (uint32_t i = lane; i < P; i += 32) {
+                const uint2 e = bp.hist[size_t(w) * bp.hist_cap + i];
+                ckey[i] = __uint_as_float(e.x);
+                cid[i] = e.y;
+            }
+        } else if (!bp.reverse) {
             // the node as a query: prepared by the search launch of this round
             for (uint32_t i = lane; i < p.qstride; i += 32) q_s[i] = p.qf[size_t(w) * p.qstride + i];
             qnorm = p.qaux[2 * size_t(w)];
@@ -171,31 +224,7 @@ __global__ void __launch_bounds__(32, 16) build_prune_kernel(const __grid_consta
         P += M;
         __syncwarp();
 
-        // ---- sort by TotalOrder (key, id): bitonic over the next power of two ----
-        uint32_t N = 32;
-        while (N < P) N <<= 1;
-        for (uint32_t i = P + lane; i < N; i += 32) {
-            ckey[i] = INFINITY;
-            cid[i] = 0xFFFFFFFFu;
-        }
-        __syncwarp();
-        for (uint32_t k = 2; k <= N; k <<= 1) {
-            for (uint32_t j = k >> 1; j > 0; j >>= 1) {
-                for (uint32_t i = lane; i < N / 2; i += 32) {
-                    const uint32_t a = ((i & ~(j - 1)) << 1) | (i & (j - 1));
-                    const uint32_t b = a | j;
-                    const bool up = (a & k) == 0;
-                    const float ka = ckey[a], kb = ckey[b];
-                    const uint32_t ia = cid[a], ib = cid[b];
-                    const bool a_gt_b = (kb < ka) || (!(ka < kb) && ib < ia);
-                    if (a_gt_b == up) {
-                        ckey[a] = kb; ckey[b] = ka;
-                        cid[a] = ib; cid[b] = ia;
-                    }
-                }
-                __syncwarp();
-            }
-        }
+        warp_sort_pairs(ckey, cid, P, lane);
         P = min(P, bp.max_candidates);
 
         // ---- heuristic_prune_neighbors (prune.h): state[] is the Progressive strategy's `pruned` ratio
@@ -283,6 +312,93 @@ __global__ void __launch_bounds__(32, 16) build_prune_kernel(const __grid_consta
     }
 }
 
+// Candidate pools of consolidation (GraphConsolidator::generate_updates, consolidate.h:191-288), one warp per Valid
+// node that has a neighbour which is not Valid, persistent over bp.nodes[0 .. bp.count):
+//   populate_candidates: the node's Valid neighbours and the adjacency rows of the others;
+//   filter_candidates: repeats and ids that are not Valid dropped, distances from the node (cosine: fix_argument on the
+//   node), sorted;  the first max_candidate_pool_size are kept.
+// The whole set (up to max_degree^2 ids) lives in this warp's slice of global scratch; it is sorted by id to drop the
+// repeats, then by TotalOrder (key, id) -- the reference sorts by distance alone, so its order among exactly equal
+// distances is unspecified -- and the best max_candidates go to hist[w] for build_prune_kernel (PRUNE_CONSOLIDATE).
+// The node itself stays in the pool when a deleted neighbour links back to it, as in the reference; the prune skips
+// it.  The kernel reads the node's own row and the rows of slots that are not Valid only.
+template <int ROWT, int OP, int DS, int KS>
+__global__ void __launch_bounds__(32, 16) consolidate_pool_kernel(const __grid_constant__ SearchParams p,
+                                                                 const __grid_constant__ BuildParams bp) {
+    constexpr int G = KS * 16 / Row<ROWT>::LPT;
+    constexpr int GROUPS = 32 / G;
+    constexpr unsigned FULL = 0xFFFFFFFFu;
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    float* q_s = reinterpret_cast<float*>(smem_raw);
+    const int lane = threadIdx.x;
+    const int g = lane / G, t = lane % G;
+    const unsigned lt_mask = (1u << lane) - 1u;
+    uint32_t* sid = bp.scratch_ids + size_t(blockIdx.x) * bp.scratch_len;
+    float* skey = bp.scratch_keys + size_t(blockIdx.x) * bp.scratch_len;
+    const char* vectors = reinterpret_cast<const char*>(p.vectors);
+    const float ksign = p.greater ? -1.0f : 1.0f;
+
+    for (;;) {
+        uint32_t w = 0;
+        if (lane == 0) w = atomicAdd(bp.work_counter, 1u);
+        w = __shfl_sync(FULL, w, 0);
+        if (w >= bp.count) break;
+        const uint32_t node = bp.nodes[w];
+        const uint32_t* row = bp.graph + size_t(node) * bp.gstride;
+        const uint32_t deg0 = min(bp.deg[node], bp.max_degree);
+        // ---- populate_candidates + the Valid filter ----
+        uint32_t M = 0;
+        for (uint32_t j = 0; j < deg0; ++j) {
+            const uint32_t dst = row[j];
+            if (bp.status[dst] == SLOT_VALID) {
+                if (lane == 0) sid[M] = dst;
+                ++M;
+                continue;
+            }
+            const uint32_t* orow = bp.graph + size_t(dst) * bp.gstride;
+            const uint32_t od = min(bp.deg[dst], bp.max_degree);
+            for (uint32_t j0 = 0; j0 < od; j0 += 32) {
+                const uint32_t jj = j0 + lane;
+                const uint32_t id = jj < od ? orow[jj] : kNoNeighbor;
+                const bool keep = id != kNoNeighbor && bp.status[id] == SLOT_VALID;
+                const unsigned m = __ballot_sync(FULL, keep);
+                if (keep) sid[M + __popc(m & lt_mask)] = id;
+                M += __popc(m);
+            }
+        }
+        __syncwarp();
+        // ---- repeats: sort by id, keep the first of every run ----
+        for (uint32_t i = lane; i < M; i += 32) skey[i] = 0.0f;
+        warp_sort_pairs(skey, sid, M, lane);
+        uint32_t U = 0, carry = 0xFFFFFFFFu;
+        for (uint32_t i0 = 0; i0 < M; i0 += 32) {
+            const uint32_t i = i0 + lane;
+            const uint32_t id = i < M ? sid[i] : 0xFFFFFFFFu;
+            uint32_t prev = __shfl_up_sync(FULL, id, 1);
+            if (lane == 0) prev = carry;
+            carry = __shfl_sync(FULL, id, 31);
+            const bool keep = i < M && id != prev;
+            const unsigned m = __ballot_sync(FULL, keep);
+            __syncwarp();
+            if (keep) sid[U + __popc(m & lt_mask)] = id;
+            U += __popc(m);
+        }
+        __syncwarp();
+        // ---- filter_candidates: distances from the node, TotalOrder ----
+        const float qnorm = stage_row<ROWT>(p, node, q_s, lane);
+        __syncwarp();
+        for (uint32_t base = 0; base < U; base += 2 * GROUPS)
+            eval_pass<ROWT, OP, DS, 2, KS, true>(p, q_s, vectors, sid, skey, base, U, g, t, qnorm, 0.f, ksign);
+        __syncwarp();
+        warp_sort_pairs(skey, sid, U, lane);
+        const uint32_t P = min(U, bp.max_candidates);
+        for (uint32_t i = lane; i < P; i += 32)
+            bp.hist[size_t(w) * bp.hist_cap + i] = make_uint2(__float_as_uint(skey[i]), sid[i]);
+        if (lane == 0) bp.hist_count[w] = P;
+        __syncwarp();
+    }
+}
+
 template <int ROWT, int OP> cudaError_t launch_build_prune(const SearchParams& p, const BuildParams& bp, int grid, cudaStream_t stream) {
     const size_t smem = build_smem_bytes(p.qstride);
     auto go = [&](auto kernel) -> cudaError_t {
@@ -297,8 +413,24 @@ template <int ROWT, int OP> cudaError_t launch_build_prune(const SearchParams& p
     return go(build_prune_kernel<ROWT, OP, 0, 1>);
 }
 
+// `grid` warps, each with its own scratch slice (bp.scratch_len entries).
+template <int ROWT, int OP>
+cudaError_t launch_consolidate_pool(const SearchParams& p, const BuildParams& bp, int grid, cudaStream_t stream) {
+    const size_t smem = size_t(p.qstride) * 4;
+    auto go = [&](auto kernel) -> cudaError_t {
+        kernel<<<grid, 32, smem, stream>>>(p, bp);
+        count_launch();
+        return cudaGetLastError();
+    };
+    if (p.dim == 96) return go(consolidate_pool_kernel<ROWT, OP, 96, 1>);
+    if (p.dim >= 256) return go(consolidate_pool_kernel<ROWT, OP, 0, 4>);
+    return go(consolidate_pool_kernel<ROWT, OP, 0, 1>);
+}
+
 // Defined in build_f32.cu / build_f16.cu.
 template <int ROWT> cudaError_t launch_build_search(int op, const SearchParams& p, const LaunchConfig& cfg);
 template <int ROWT> cudaError_t launch_build_prune_op(int op, const SearchParams& p, const BuildParams& bp, int grid, cudaStream_t stream);
+template <int ROWT>
+cudaError_t launch_consolidate_pool_op(int op, const SearchParams& p, const BuildParams& bp, int grid, cudaStream_t stream);
 
 }  // namespace svsb200

@@ -1,11 +1,14 @@
 // dynamic.cu -- the dynamic (mutable) Vamana index of the C ABI: MutableVamanaIndex
-// (index/vamana/dynamic_index.h) assembled from a graph, data and external ids, with soft deletion.  Every slot has
-// a status (Valid / Deleted / Empty) and an external id in HBM; the external -> slot translator
-// (core/translation.h) lives on the host.  Searches go through svsb200_search* and run the lean kernel's
-// MutableBuffer form (search_fast.cuh, MUT = true).
+// (index/vamana/dynamic_index.h) built or assembled from a graph, data and external ids, with insertion, soft
+// deletion, consolidation and compaction.  Every slot has a status (Valid / Deleted / Empty) and an external id in
+// HBM; the external -> slot translator (core/translation.h) lives on the host.  Searches go through svsb200_search*
+// and run the lean kernel's MutableBuffer form (search_fast.cuh, MUT = true); insertion runs the graph builder over
+// the new slots (build.cu), consolidation its prune kernel over pools selected by consolidate_pool_kernel.
+#include "build_kernels.cuh"
 #include "host.cuh"
 
 #include <algorithm>
+#include <cmath>
 #include <unordered_set>
 
 namespace svsb200 {
@@ -20,6 +23,139 @@ static int check_dynamic(const svsb200_index* ix, const char* who) {
     if (!ix) return fail(std::string(who) + ": NULL index");
     if (!ix->dynamic) return fail(std::string(who) + ": not a dynamic index (create it with svsb200_dynamic_create)");
     return 0;
+}
+
+// Row slots[i] of the data <- row i of `src` (row_stride bytes, a multiple of 16); adjacency row slots[i] emptied
+// (copy_points + clear_lists, dynamic_index.h:714-716).  One warp per row.
+__global__ void place_rows_kernel(const uint4* __restrict__ src, const uint32_t* __restrict__ slots, uint32_t count,
+                                  uint32_t row_stride, uint4* __restrict__ vectors, uint32_t* __restrict__ graph,
+                                  uint32_t gstride) {
+    const uint32_t i = blockIdx.x * (blockDim.x / 32) + threadIdx.x / 32;
+    const uint32_t lane = threadIdx.x & 31;
+    if (i >= count) return;
+    const size_t s = slots[i], words = row_stride / 16;
+    for (size_t j = lane; j < words; j += 32) vectors[s * words + j] = src[i * words + j];
+    for (uint32_t j = lane; j < gstride; j += 32) graph[s * gstride + j] = kNoNeighbor;
+}
+
+// status[slots[i]] = Valid, ext_ids[slots[i]] = ids[i]
+__global__ void mark_added_kernel(const uint32_t* __restrict__ slots, const uint64_t* __restrict__ ids, uint32_t count,
+                                  uint8_t* __restrict__ status, uint64_t* __restrict__ ext_ids) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= count) return;
+    status[slots[i]] = SLOT_VALID;
+    ext_ids[slots[i]] = ids[i];
+}
+
+__global__ void deleted_to_empty_kernel(uint8_t* __restrict__ status, uint32_t n) {
+    const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
+    if (v < n && status[v] == SLOT_DELETED) status[v] = SLOT_EMPTY;
+}
+
+// The rows consolidation rewrites: Valid nodes with at least one neighbour that is not Valid (is_deleted is
+// status != Valid, so Empty counts; consolidate.h:249-257).  Listed in no particular order.
+__global__ void consolidation_nodes_kernel(const uint32_t* __restrict__ graph, const uint32_t* __restrict__ deg,
+                                           const uint8_t* __restrict__ status, uint32_t n, uint32_t gstride,
+                                           uint32_t* __restrict__ list, uint32_t* __restrict__ count) {
+    const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= n || status[v] != SLOT_VALID) return;
+    const uint32_t* row = graph + size_t(v) * gstride;
+    for (uint32_t j = 0; j < deg[v]; ++j)
+        if (status[row[j]] != SLOT_VALID) {
+            list[atomicAdd(count, 1u)] = v;
+            return;
+        }
+}
+
+// ref_degree[v] = deg[v]: rows written by a mutation hold no repeats, so their stored length is the reference's degree
+__global__ void ref_degree_kernel(const uint32_t* __restrict__ deg, uint32_t n, uint16_t* __restrict__ ref_degree) {
+    const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
+    if (v < n) ref_degree[v] = uint16_t(deg[v]);
+}
+
+// compact (dynamic_index.h:817-916): new slot i <- old slot new_to_old[i]; data row, adjacency row with every id mapped
+// through old_to_new, stored degree.  One warp per new slot.
+__global__ void compact_kernel(const uint32_t* __restrict__ new_to_old, const uint32_t* __restrict__ old_to_new, uint32_t m,
+                               uint32_t row_stride, uint32_t gstride, const uint4* __restrict__ vec_in,
+                               const uint32_t* __restrict__ graph_in, const uint16_t* __restrict__ refdeg_in,
+                               uint4* __restrict__ vec_out, uint32_t* __restrict__ graph_out, uint16_t* __restrict__ refdeg_out) {
+    const uint32_t i = blockIdx.x * (blockDim.x / 32) + threadIdx.x / 32;
+    const uint32_t lane = threadIdx.x & 31;
+    if (i >= m) return;
+    const size_t o = new_to_old[i], words = row_stride / 16;
+    for (size_t j = lane; j < words; j += 32) vec_out[i * words + j] = vec_in[o * words + j];
+    for (uint32_t j = lane; j < gstride; j += 32) {
+        const uint32_t id = graph_in[o * gstride + j];
+        graph_out[size_t(i) * gstride + j] = id == kNoNeighbor ? kNoNeighbor : old_to_new[id];
+    }
+    if (lane == 0) refdeg_out[i] = refdeg_in[o];
+}
+
+// A copy of `buf` with room for `want` elements whose first `used` elements are the old ones (no-op if it fits).
+template <typename T> static cudaError_t grow(DeviceBuffer<T>& buf, size_t used, size_t want) {
+    if (want <= buf.count) return cudaSuccess;
+    DeviceBuffer<T> bigger;
+    cudaError_t e = bigger.ensure(want);
+    if (e == cudaSuccess && used) e = cudaMemcpy(bigger.ptr, buf.ptr, used * sizeof(T), cudaMemcpyDeviceToDevice);
+    if (e == cudaSuccess) buf = std::move(bigger);   // (the old block goes with `bigger`)
+    return e;
+}
+
+// Bytes of device memory a dynamic index with room for `slots` slots holds.
+static size_t dynamic_bytes(const svsb200_index* ix, size_t slots) {
+    return slots * (size_t(ix->row_stride) + size_t(ix->gstride) * sizeof(uint32_t) + sizeof(uint16_t) + 1 + sizeof(uint64_t));
+}
+
+// Mutation parameters, 0 selecting the default (verify_and_set_default_index_parameters, index.h:1079-1110, and the
+// from-graph constructor's window 2R, dynamic_index.h:198).  Rejects what the GPU builder cannot honour exactly: its
+// candidate pool holds kPoolMax entries, so max_candidates <= 512 (the default 3 * window is clamped to 512).
+static int resolve_mutation_parameters(const char* who, int metric, size_t R, float* alpha, size_t* window,
+                                       size_t* max_candidates, size_t* prune_to) {
+    const std::string w(who);
+    if (*alpha == 0.f) *alpha = metric == SVSB200_L2 ? 1.2f : 0.95f;
+    if (!(*alpha > 0.f) || !std::isfinite(*alpha) || (metric == SVSB200_L2 ? *alpha < 1.0f : *alpha > 1.0f))
+        return fail(w + ": alpha on the wrong side of 1 for this metric");
+    if (*window == 0) *window = 2 * R;
+    if (*window + 32 > kPoolMax - graph_stride(R)) return fail(w + ": window_size too large for the candidate pool");
+    if (*max_candidates == 0) *max_candidates = std::min<size_t>(3 * *window, kPoolMax);
+    if (*max_candidates > kPoolMax) return fail(w + ": max_candidates above 512, the GPU builder's candidate pool");
+    if (*prune_to == 0) *prune_to = R >= 16 ? R - 4 : R;
+    if (*prune_to > R) return fail(w + ": prune_to must be <= graph_max_degree");
+    return 0;
+}
+
+// The graph of a dynamic index as the builder sees it (deg = the caller's [n] scratch), on rep's device.
+static GraphBuild graph_build(const svsb200_index* ix, Replica* rep, uint32_t* deg, cudaStream_t stream) {
+    GraphBuild b;
+    b.dtype = ix->dtype;
+    b.metric = ix->metric;
+    b.n = ix->n;
+    b.dim = ix->dim;
+    b.R = uint32_t(ix->max_degree);
+    b.gstride = ix->gstride;
+    b.row_stride = ix->row_stride;
+    b.vectors = rep->d_vectors.ptr;
+    b.graph = rep->d_graph.ptr;
+    b.deg = deg;
+    b.window = ix->dyn_window;
+    b.max_candidates = ix->dyn_max_candidates;
+    b.prune_to = ix->dyn_prune_to;
+    b.alpha = ix->dyn_alpha;
+    b.sm_count = rep->sm_count;
+    b.stream = stream;
+    return b;
+}
+
+// Runs `body(stream)` on a scratch stream of the index's device.
+template <typename F> static int on_stream(svsb200_index* ix, F body) {
+    Replica* rep = ix->reps[0].get();
+    CUDA_TRY(cudaSetDevice(rep->device));
+    std::string err;
+    Scratch* sc = acquire(rep, &err);
+    if (!sc) return fail(err);
+    const int rc = body(rep, sc->stream);
+    release(rep, sc);
+    return rc;
 }
 
 }  // namespace svsb200
@@ -62,6 +198,10 @@ int svsb200_dynamic_create(const void* vectors, int dtype, size_t n, size_t dim,
     CUDA_TRY(cudaMemcpy(rep->d_ext_ids.ptr, ix->ext_ids.data(), n * sizeof(uint64_t), cudaMemcpyHostToDevice));
     ix->device_bytes += n * (1 + sizeof(uint64_t));
     ix->dynamic = true;
+    ix->first_empty = n;
+    if (int rc = resolve_mutation_parameters("svsb200_dynamic_create", metric, ix->max_degree, &ix->dyn_alpha, &ix->dyn_window,
+                                             &ix->dyn_max_candidates, &ix->dyn_prune_to))
+        return rc;
     *out = owner.release();
     return 0;
 }
@@ -151,6 +291,311 @@ int svsb200_dynamic_export(const svsb200_index* ix, uint32_t* graph_rows_out, ui
     if (status_out) std::copy(ix->status.begin(), ix->status.end(), status_out);
     if (ext_ids_out) std::copy(ix->ext_ids.begin(), ix->ext_ids.end(), ext_ids_out);
     if (entry_point_out) *entry_point_out = ix->entry_point;
+    return 0;
+}
+
+int svsb200_dynamic_set_build_parameters(svsb200_index* ix, float alpha, size_t window_size, size_t max_candidates,
+                                         size_t prune_to) {
+    const char* who = "svsb200_dynamic_set_build_parameters";
+    if (int rc = check_dynamic(ix, who)) return rc;
+    if (int rc = resolve_mutation_parameters(who, ix->metric, ix->max_degree, &alpha, &window_size, &max_candidates, &prune_to))
+        return rc;
+    ix->dyn_alpha = alpha;
+    ix->dyn_window = window_size;
+    ix->dyn_max_candidates = max_candidates;
+    ix->dyn_prune_to = prune_to;
+    return 0;
+}
+
+int svsb200_dynamic_get_build_parameters(const svsb200_index* ix, float* alpha, size_t* window_size, size_t* max_candidates,
+                                         size_t* prune_to) {
+    if (int rc = check_dynamic(ix, "svsb200_dynamic_get_build_parameters")) return rc;
+    if (alpha) *alpha = ix->dyn_alpha;
+    if (window_size) *window_size = ix->dyn_window;
+    if (max_candidates) *max_candidates = ix->dyn_max_candidates;
+    if (prune_to) *prune_to = ix->dyn_prune_to;
+    return 0;
+}
+
+int svsb200_dynamic_add(svsb200_index* ix, const void* vectors, int dtype, size_t count, const uint64_t* ids, int reuse_empty,
+                        uint64_t* slots_out) {
+    const char* who = "svsb200_dynamic_add";
+    if (int rc = check_dynamic(ix, who)) return rc;
+    if (count == 0) return 0;
+    if (!vectors || !ids) return fail("svsb200_dynamic_add: NULL argument");
+    if (dtype != ix->dtype) return fail("svsb200_dynamic_add: the points' dtype differs from the index's");
+    // translator_.insert (core/translation.h:105-127), checked before anything changes
+    {
+        std::unordered_set<uint64_t> seen;
+        seen.reserve(count);
+        for (size_t i = 0; i < count; ++i) {
+            if (ids[i] == ~uint64_t(0)) return fail("svsb200_dynamic_add: external id 2^64 - 1 is reserved");
+            if (!seen.insert(ids[i]).second) return fail("svsb200_dynamic_add: External IDs contain repeat elements!");
+            if (ix->translator.count(ids[i]))
+                return fail("svsb200_dynamic_add: External ID " + std::to_string(ids[i]) + " already exists!");
+        }
+    }
+    // slots (add_points, dynamic_index.h:670-706): Empty ones from first_empty_ (from 0 with reuse_empty), then appended
+    std::vector<uint32_t> slots;
+    slots.reserve(count);
+    for (size_t s = reuse_empty ? 0 : ix->first_empty; s < ix->status.size() && slots.size() < count; ++s)
+        if (ix->status[s] == SLOT_EMPTY) slots.push_back(uint32_t(s));
+    const size_t old_n = ix->n, new_n = old_n + (count - slots.size());
+    if (new_n >= (size_t(1) << 30)) return fail("svsb200_dynamic_add: at most 2^30 - 1 slots");
+    for (size_t s = old_n; s < new_n; ++s) slots.push_back(uint32_t(s));
+    {
+        GraphBuild b;
+        b = graph_build(ix, ix->reps[0].get(), nullptr, nullptr);
+        b.n = new_n;
+        if (int rc = check_construct(who, b)) return rc;
+    }
+    int rc = on_stream(ix, [&](Replica* rep, cudaStream_t stream) -> int {
+        // geometric growth: many small calls do not copy the index each time
+        const size_t cap = rep->d_status.count;
+        if (new_n > cap) {
+            const size_t want = std::max(new_n, 2 * cap);
+            CUDA_TRY(cudaStreamSynchronize(stream));
+            CUDA_TRY(grow(rep->d_vectors, old_n * ix->row_stride, want * ix->row_stride));
+            CUDA_TRY(grow(rep->d_graph, old_n * ix->gstride, want * ix->gstride));
+            CUDA_TRY(grow(rep->d_ref_degree, old_n, want));
+            CUDA_TRY(grow(rep->d_status, old_n, want));
+            CUDA_TRY(grow(rep->d_ext_ids, old_n, want));
+            ix->device_bytes = dynamic_bytes(ix, want);
+        }
+        ix->n = new_n;
+        ix->status.resize(new_n, SLOT_EMPTY);
+        ix->ext_ids.resize(new_n, 0);
+        DeviceBuffer<unsigned char> d_src;
+        DeviceBuffer<uint32_t> d_slots, d_deg;
+        DeviceBuffer<uint64_t> d_ids;
+        CUDA_TRY(d_src.ensure(count * ix->row_stride));
+        CUDA_TRY(d_slots.ensure(count));
+        CUDA_TRY(d_ids.ensure(count));
+        CUDA_TRY(d_deg.ensure(new_n));
+        CUDA_TRY(cudaMemsetAsync(d_src.ptr, 0, count * ix->row_stride, stream));
+        const size_t row_bytes = ix->dim * esize(ix->dtype);
+        CUDA_TRY(cudaMemcpy2DAsync(d_src.ptr, ix->row_stride, vectors, row_bytes, row_bytes, count, cudaMemcpyHostToDevice, stream));
+        CUDA_TRY(cudaMemcpyAsync(d_slots.ptr, slots.data(), count * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
+        CUDA_TRY(cudaMemcpyAsync(d_ids.ptr, ids, count * sizeof(uint64_t), cudaMemcpyHostToDevice, stream));
+        place_rows_kernel<<<unsigned((count + 7) / 8), 256, 0, stream>>>(
+            reinterpret_cast<const uint4*>(d_src.ptr), d_slots.ptr, uint32_t(count), ix->row_stride,
+            reinterpret_cast<uint4*>(rep->d_vectors.ptr), rep->d_graph.ptr, ix->gstride);
+        count_launch();
+        CUDA_TRY(cudaGetLastError());
+        const GraphBuild b = graph_build(ix, rep, d_deg.ptr, stream);
+        if (int rc2 = row_degrees(b)) return rc2;
+        // builder.construct(alpha_, entry_point(), slots) (dynamic_index.h:719-739): its greedy search ignores the slot
+        // status, so Deleted slots are walked and may become neighbours of the new points, as in the reference
+        if (int rc2 = construct_graph(who, b, ix->dyn_alpha, ix->entry_point, d_slots.ptr, count)) return rc2;
+        ref_degree_kernel<<<unsigned((new_n + 255) / 256), 256, 0, stream>>>(d_deg.ptr, uint32_t(new_n), rep->d_ref_degree.ptr);
+        count_launch();
+        mark_added_kernel<<<unsigned((count + 255) / 256), 256, 0, stream>>>(d_slots.ptr, d_ids.ptr, uint32_t(count),
+                                                                            rep->d_status.ptr, rep->d_ext_ids.ptr);
+        count_launch();
+        CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(cudaStreamSynchronize(stream));
+        return 0;
+    });
+    if (rc) return rc;
+    for (size_t i = 0; i < count; ++i) {
+        ix->status[slots[i]] = SLOT_VALID;
+        ix->ext_ids[slots[i]] = ids[i];
+        ix->translator.emplace(ids[i], slots[i]);
+        if (slots_out) slots_out[i] = slots[i];
+    }
+    ix->first_empty = std::max<size_t>(ix->first_empty, size_t(slots.back()) + 1);
+    return 0;
+}
+
+int svsb200_dynamic_consolidate(svsb200_index* ix) {
+    const char* who = "svsb200_dynamic_consolidate";
+    if (int rc = check_dynamic(ix, who)) return rc;
+    const size_t n = ix->n, R = ix->max_degree;
+    const size_t valid = ix->translator.size();
+    const bool replace_entry = ix->status[ix->entry_point] == SLOT_DELETED;
+    // (the reference would silently pick slot 0)
+    if (replace_entry && valid == 0) return fail("svsb200_dynamic_consolidate: no Valid slot left for the entry point");
+    uint32_t entry_point = ix->entry_point;
+    int rc = on_stream(ix, [&](Replica* rep, cudaStream_t stream) -> int {
+        DeviceBuffer<uint32_t> d_deg, d_nodes, d_count;
+        CUDA_TRY(d_deg.ensure(n));
+        CUDA_TRY(d_nodes.ensure(n));
+        CUDA_TRY(d_count.ensure(1));
+        const GraphBuild b = graph_build(ix, rep, d_deg.ptr, stream);
+        // the entry point: compute_entry_point(data_, threadpool_, valid) (dynamic_index.h:982-993)
+        if (replace_entry)
+            if (int rc2 = medoid(b, rep->d_status.ptr, valid, &entry_point)) return rc2;
+        if (int rc2 = row_degrees(b)) return rc2;
+        CUDA_TRY(cudaMemsetAsync(d_count.ptr, 0, sizeof(uint32_t), stream));
+        consolidation_nodes_kernel<<<unsigned((n + 255) / 256), 256, 0, stream>>>(rep->d_graph.ptr, d_deg.ptr, rep->d_status.ptr,
+                                                                                 uint32_t(n), ix->gstride, d_nodes.ptr, d_count.ptr);
+        count_launch();
+        CUDA_TRY(cudaGetLastError());
+        uint32_t total = 0;
+        CUDA_TRY(cudaMemcpyAsync(&total, d_count.ptr, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
+        CUDA_TRY(cudaStreamSynchronize(stream));
+        if (total) {
+            // A node's new row depends only on its own row and on the rows of slots that are not Valid; neither changes
+            // while consolidation runs (only Valid rows are rewritten, each by its own node).  So one pass over all
+            // nodes, rows rewritten in place batch by batch, equals the reference's batches of 200 000 with updates
+            // applied after each batch (consolidate.h).
+            const size_t chunk = std::min<size_t>(total, 32768);
+            const int grid = int(std::min<size_t>(size_t(rep->sm_count) * 16, chunk));
+            uint32_t scratch_len = 32;
+            while (scratch_len < R * R) scratch_len <<= 1;
+            DeviceBuffer<uint2> d_hist;
+            DeviceBuffer<uint32_t> d_hist_count, d_sid;
+            DeviceBuffer<float> d_skey;
+            DeviceBuffer<unsigned int> d_work;
+            CUDA_TRY(d_hist.ensure(chunk * kPoolMax));
+            CUDA_TRY(d_hist_count.ensure(chunk));
+            CUDA_TRY(d_sid.ensure(size_t(grid) * scratch_len));
+            CUDA_TRY(d_skey.ensure(size_t(grid) * scratch_len));
+            CUDA_TRY(d_work.ensure(1));
+            SearchParams p{};
+            p.vectors = rep->d_vectors.ptr;
+            p.graph = rep->d_graph.ptr;
+            p.n = uint32_t(n);
+            p.dim = uint32_t(ix->dim);
+            p.row_stride = ix->row_stride;
+            p.gstride = ix->gstride;
+            p.greater = ix->metric != SVSB200_L2;
+            p.scale = 1.f;
+            p.qstride = query_stride(ix->dim);
+            BuildParams bp{};
+            bp.hist = d_hist.ptr;
+            bp.hist_count = d_hist_count.ptr;
+            bp.hist_cap = kPoolMax;
+            bp.graph = rep->d_graph.ptr;
+            bp.deg = d_deg.ptr;
+            bp.gstride = ix->gstride;
+            bp.max_degree = uint32_t(R);
+            bp.limit = uint32_t(ix->dyn_prune_to);
+            bp.max_candidates = uint32_t(ix->dyn_max_candidates);
+            bp.alpha = ix->dyn_alpha;
+            bp.iterative = ix->metric != SVSB200_L2;
+            bp.work_counter = d_work.ptr;
+            bp.status = rep->d_status.ptr;
+            bp.scratch_ids = d_sid.ptr;
+            bp.scratch_keys = d_skey.ptr;
+            bp.scratch_len = scratch_len;
+            const int op = ix->metric == SVSB200_L2 ? OP_L2F : ix->metric == SVSB200_IP ? OP_IPF : OP_COSF;
+            const bool f32 = ix->dtype == SVSB200_F32;
+            for (size_t start = 0; start < total; start += chunk) {
+                bp.nodes = d_nodes.ptr + start;
+                bp.count = uint32_t(std::min<size_t>(chunk, total - start));
+                CUDA_TRY(cudaMemsetAsync(d_work.ptr, 0, 4, stream));
+                CUDA_TRY(f32 ? launch_consolidate_pool_op<SVSB200_F32>(op, p, bp, grid, stream)
+                             : launch_consolidate_pool_op<SVSB200_F16>(op, p, bp, grid, stream));
+                CUDA_TRY(cudaMemsetAsync(d_work.ptr, 0, 4, stream));
+                bp.reverse = PRUNE_CONSOLIDATE;
+                const int prune_grid = int(std::min<size_t>(size_t(rep->sm_count) * 16, bp.count));
+                CUDA_TRY(f32 ? launch_build_prune_op<SVSB200_F32>(op, p, bp, prune_grid, stream)
+                             : launch_build_prune_op<SVSB200_F16>(op, p, bp, prune_grid, stream));
+            }
+            ref_degree_kernel<<<unsigned((n + 255) / 256), 256, 0, stream>>>(d_deg.ptr, uint32_t(n), rep->d_ref_degree.ptr);
+            count_launch();
+        }
+        deleted_to_empty_kernel<<<unsigned((n + 255) / 256), 256, 0, stream>>>(rep->d_status.ptr, uint32_t(n));
+        count_launch();
+        CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(cudaStreamSynchronize(stream));
+        return 0;
+    });
+    if (rc) return rc;
+    ix->entry_point = entry_point;
+    for (auto& st : ix->status)
+        if (st == SLOT_DELETED) st = SLOT_EMPTY;
+    return 0;
+}
+
+int svsb200_dynamic_compact(svsb200_index* ix) {
+    const char* who = "svsb200_dynamic_compact";
+    if (int rc = check_dynamic(ix, who)) return rc;
+    // (the reference throws from robin_map::at after it has already moved the data)
+    if (std::find(ix->status.begin(), ix->status.end(), uint8_t(SLOT_DELETED)) != ix->status.end())
+        return fail("svsb200_dynamic_compact: the index holds Deleted slots; consolidate first");
+    // nonmissing_indices (dynamic_index.h:800-809): the Valid slots, ascending
+    const size_t n = ix->n;
+    std::vector<uint32_t> new_to_old, old_to_new(n, kNoNeighbor);
+    new_to_old.reserve(ix->translator.size());
+    for (size_t s = 0; s < n; ++s)
+        if (ix->status[s] == SLOT_VALID) {
+            old_to_new[s] = uint32_t(new_to_old.size());
+            new_to_old.push_back(uint32_t(s));
+        }
+    const size_t m = new_to_old.size();
+    if (m == 0 || old_to_new[ix->entry_point] == kNoNeighbor)
+        return fail("svsb200_dynamic_compact: the entry point is not Valid; consolidate first");
+    std::vector<uint64_t> ext(m);
+    for (size_t i = 0; i < m; ++i) ext[i] = ix->ext_ids[new_to_old[i]];
+    int rc = on_stream(ix, [&](Replica* rep, cudaStream_t stream) -> int {
+        DeviceBuffer<uint32_t> d_n2o, d_o2n, graph;
+        DeviceBuffer<unsigned char> vectors;
+        DeviceBuffer<uint16_t> refdeg;
+        DeviceBuffer<uint8_t> status;
+        DeviceBuffer<uint64_t> ext_ids;
+        CUDA_TRY(d_n2o.ensure(m));
+        CUDA_TRY(d_o2n.ensure(n));
+        CUDA_TRY(vectors.ensure(m * ix->row_stride));
+        CUDA_TRY(graph.ensure(m * ix->gstride));
+        CUDA_TRY(refdeg.ensure(m));
+        CUDA_TRY(status.ensure(m));
+        CUDA_TRY(ext_ids.ensure(m));
+        CUDA_TRY(cudaMemcpyAsync(d_n2o.ptr, new_to_old.data(), m * 4, cudaMemcpyHostToDevice, stream));
+        CUDA_TRY(cudaMemcpyAsync(d_o2n.ptr, old_to_new.data(), n * 4, cudaMemcpyHostToDevice, stream));
+        CUDA_TRY(cudaMemcpyAsync(ext_ids.ptr, ext.data(), m * 8, cudaMemcpyHostToDevice, stream));
+        CUDA_TRY(cudaMemsetAsync(status.ptr, SLOT_VALID, m, stream));
+        compact_kernel<<<unsigned((m + 7) / 8), 256, 0, stream>>>(
+            d_n2o.ptr, d_o2n.ptr, uint32_t(m), ix->row_stride, ix->gstride, reinterpret_cast<const uint4*>(rep->d_vectors.ptr),
+            rep->d_graph.ptr, rep->d_ref_degree.ptr, reinterpret_cast<uint4*>(vectors.ptr), graph.ptr, refdeg.ptr);
+        count_launch();
+        CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(cudaStreamSynchronize(stream));
+        rep->d_vectors = std::move(vectors);   // (the old blocks are freed with the locals)
+        rep->d_graph = std::move(graph);
+        rep->d_ref_degree = std::move(refdeg);
+        rep->d_status = std::move(status);
+        rep->d_ext_ids = std::move(ext_ids);
+        return 0;
+    });
+    if (rc) return rc;
+    ix->n = m;
+    ix->device_bytes = dynamic_bytes(ix, m);
+    ix->status.assign(m, SLOT_VALID);
+    ix->ext_ids = std::move(ext);
+    for (size_t i = 0; i < m; ++i) ix->translator[ix->ext_ids[i]] = uint32_t(i);
+    ix->entry_point = old_to_new[ix->entry_point];
+    ix->first_empty = m;
+    return 0;
+}
+
+int svsb200_dynamic_build(const void* vectors, int dtype, size_t n, size_t dim, int metric, float alpha,
+                          size_t graph_max_degree, size_t window_size, size_t max_candidates, size_t prune_to,
+                          const uint64_t* external_ids, int device, svsb200_index** out) {
+    const char* who = "svsb200_dynamic_build";
+    if (!out) return fail("svsb200_dynamic_build: NULL output");
+    *out = nullptr;
+    if (metric < SVSB200_L2 || metric > SVSB200_COSINE) return fail("svsb200_dynamic_build: bad metric");
+    if (graph_max_degree == 0 || graph_max_degree > 32u * kFastMaxGW)
+        return fail("svsb200_dynamic_build: graph_max_degree must be in [1, 128]");
+    if (window_size == 0) return fail("svsb200_dynamic_build: window_size must be positive");
+    if (int rc = resolve_mutation_parameters(who, metric, graph_max_degree, &alpha, &window_size, &max_candidates, &prune_to))
+        return rc;
+    std::vector<uint32_t> graph(n * (graph_max_degree + 1));
+    uint32_t entry_point = 0;
+    if (int rc = svsb200_build_vamana(vectors, dtype, n, dim, 0, metric, alpha, graph_max_degree, window_size, max_candidates,
+                                      prune_to, device, graph.data(), &entry_point))
+        return rc;
+    svsb200_index* ix = nullptr;
+    if (int rc = svsb200_dynamic_create(vectors, dtype, n, dim, graph.data(), graph_max_degree + 1, entry_point, metric,
+                                        external_ids, device, &ix))
+        return rc;
+    ix->dyn_alpha = alpha;
+    ix->dyn_window = window_size;
+    ix->dyn_max_candidates = max_candidates;
+    ix->dyn_prune_to = prune_to;
+    *out = ix;
     return 0;
 }
 

@@ -241,6 +241,10 @@ struct svsb200_index {
     std::unordered_map<uint64_t, uint32_t> translator;
     long dyn_slack = -1;              // option "dynamic_slack"
     std::atomic<long> dyn_reruns{0};  // queries re-run with a larger buffer so far
+    size_t first_empty = 0;           // first_empty_: where add_points looks for Empty slots unless told to reuse
+    // mutation parameters (alpha_, construction_window_size_, max_candidates_, prune_to_)
+    float dyn_alpha = 0.f;
+    size_t dyn_window = 0, dyn_max_candidates = 0, dyn_prune_to = 0;
 };
 
 namespace svsb200 {
@@ -266,5 +270,31 @@ int prepare_queries(const svsb200_index* ix, const Replica* rep, Scratch* sc, co
 int search_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, const void* d_queries, int qdtype, size_t nq, size_t k,
                      size_t window, size_t capacity, void* d_out_ids, int id_bytes, float* d_out_dists, cudaStream_t stream,
                      bool exhaustive = false);
+
+// ---- graph construction (build.cu), shared by svsb200_build_vamana and the dynamic index ----
+// A float32 / float16 graph on the current device: n rows (row_stride apart), adjacency rows (gstride apart, neighbours
+// first, kNoNeighbor padding) and the row lengths, with VamanaBuildParameters.
+struct GraphBuild {
+    int dtype = 0, metric = 0;
+    size_t n = 0, dim = 0;
+    uint32_t R = 0, gstride = 0, row_stride = 0;
+    const void* vectors = nullptr;
+    uint32_t* graph = nullptr;
+    uint32_t* deg = nullptr;
+    size_t window = 0, max_candidates = 0, prune_to = 0;
+    float alpha = 1.f;                // forward pruning
+    int sm_count = 0;
+    cudaStream_t stream = nullptr;
+};
+// Fails ("<who>: ...") when the builder's search cannot run with these parameters on n rows.
+int check_construct(const char* who, const GraphBuild& b);
+// VamanaBuilder::construct(reverse_alpha, entry_point, nodes) (vamana_build.h:221-318): one pass over the nodes
+// d_slots[0 .. count) (device list; NULL: nodes 0 .. count), in max(40, count / 4096) batches.  Blocking on b.stream.
+int construct_graph(const char* who, const GraphBuild& b, float reverse_alpha, uint32_t entry_point, const uint32_t* d_slots,
+                    size_t count);
+// find_medioid (core/medioid.h:292-350) over the `count` rows whose status is Valid (d_status NULL: all n rows).
+int medoid(const GraphBuild& b, const uint8_t* d_status, size_t count, uint32_t* out);
+// b.deg[v] = length of adjacency row v, for every row (enqueued on b.stream).
+int row_degrees(const GraphBuild& b);
 
 }  // namespace svsb200

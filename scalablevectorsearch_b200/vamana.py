@@ -488,10 +488,42 @@ class ShardedVamana:
 
 class DynamicVamana(Vamana):
     """GPU-backed dynamic Vamana index: the reference's ``svs.DynamicVamana`` / ``MutableVamanaIndex``
-    (bindings/python/src/dynamic_vamana.cpp, include/svs/index/vamana/dynamic_index.h) assembled from a graph, its
-    data and one external id per row, with soft deletion.  Searches return external ids and never return a deleted
-    one, while the walk still goes through deleted rows, exactly as ``MutableVamanaIndex::search`` does.  Mutations
-    must not run concurrently with searches of the same index.  float32 / float16 data, one device."""
+    (bindings/python/src/dynamic_vamana.cpp, include/svs/index/vamana/dynamic_index.h) built on the GPU or assembled
+    from a graph, its data and one external id per row, with ``add``, soft ``delete``, ``consolidate`` and
+    ``compact``.  Searches return external ids and never return a deleted one, while the walk still goes through
+    deleted rows, exactly as ``MutableVamanaIndex::search`` does.  Mutations must not run concurrently with searches
+    of the same index.  float32 / float16 data, one device."""
+
+    @classmethod
+    def build(cls, parameters: VamanaBuildParameters, data: np.ndarray, ids=None, distance: "DistanceType" = None,
+              device: int = 0, num_threads: int = 1) -> "DynamicVamana":
+        """``svs.DynamicVamana.build(parameters, data, ids, distance)`` (``MutableVamanaIndex(parameters, data,
+        external_ids, distance)``, dynamic_index.h:208-261): the GPU builder's graph, with ``parameters`` kept as the
+        mutation parameters.  ``ids`` defaults to ``0 .. n-1``."""
+        distance = DistanceType.L2 if distance is None else DistanceType(distance)
+        data = np.ascontiguousarray(data)
+        if data.ndim != 2 or data.dtype not in (np.float32, np.float16):
+            raise TypeError("DynamicVamana.build takes a 2-D float32 / float16 array")
+        if not parameters.use_full_search_history:
+            raise ValueError("the GPU builder always keeps the full search history (the reference's default)")
+        n = data.shape[0]
+        ids = np.arange(n, dtype=np.uint64) if ids is None else np.ascontiguousarray(ids, dtype=np.uint64)
+        if ids.shape != (n,):
+            raise ValueError("one external id per row")
+        self = cls.__new__(cls)
+        self._lib = _lib.lib()
+        self._distance = distance
+        self._dtype = data.dtype
+        self._params = VamanaSearchParameters()
+        self._num_threads = int(num_threads)
+        handle = C.c_void_p()
+        _lib.check(self._lib.svsb200_dynamic_build(
+            data.ctypes.data, _DTYPE_CODE[data.dtype], n, data.shape[1], int(distance), float(parameters.alpha),
+            int(parameters.graph_max_degree), int(parameters.window_size), int(parameters.max_candidate_pool_size),
+            int(parameters.prune_to), ids.ctypes.data, int(device), C.byref(handle)))
+        self._h = handle
+        self.build_parameters = parameters
+        return self
 
     @classmethod
     def from_arrays(cls, data: np.ndarray, graph: np.ndarray, entry_point: int, ids=None,
@@ -553,6 +585,56 @@ class DynamicVamana(Vamana):
         ids = np.ascontiguousarray(np.atleast_1d(ids), dtype=np.uint64)
         _lib.check(self._lib.svsb200_dynamic_delete(self._h, ids.ctypes.data, len(ids)))
         return len(ids)
+
+    def add(self, points: np.ndarray, ids, reuse_empty: bool = False) -> np.ndarray:
+        """``add_points`` (dynamic_index.h:657-749): insert rows of the index's dtype with new external ids.  Empty
+        slots are used first (from the start with ``reuse_empty``), then the index grows.  Fails without changing
+        anything on a repeated, present or reserved id.  Returns the slots used."""
+        pts = np.ascontiguousarray(points)
+        ids = np.ascontiguousarray(np.atleast_1d(ids), dtype=np.uint64)
+        if pts.ndim != 2 or pts.shape[1] != self.dimensions:
+            raise ValueError(f"points must be [count, {self.dimensions}]")
+        if pts.shape[0] != len(ids):
+            raise ValueError(f"Number of points ({pts.shape[0]}) not equal to the number of external ids ({len(ids)})!")
+        if pts.dtype not in _DTYPE_CODE:
+            raise TypeError(f"unsupported data type {pts.dtype}")
+        slots = np.empty(len(ids), dtype=np.uint64)
+        _lib.check(self._lib.svsb200_dynamic_add(self._h, pts.ctypes.data, _DTYPE_CODE[pts.dtype], len(ids), ids.ctypes.data,
+                                                 int(bool(reuse_empty)), slots.ctypes.data))
+        return slots
+
+    def consolidate(self):
+        """``consolidate`` (dynamic_index.h:976-1013): unlink the deleted entries from the graph; their slots become
+        empty.  A deleted entry point is replaced by the medoid of the valid rows."""
+        _lib.check(self._lib.svsb200_dynamic_consolidate(self._h))
+
+    def compact(self):
+        """``compact`` (dynamic_index.h:817-916): move the valid entries to slots ``0 .. size-1``, in slot order.
+        Fails without changing anything while deleted entries are present (call :meth:`consolidate` first)."""
+        _lib.check(self._lib.svsb200_dynamic_compact(self._h))
+
+    def _build_parameters(self):
+        a, w, m, p = C.c_float(), C.c_size_t(), C.c_size_t(), C.c_size_t()
+        _lib.check(self._lib.svsb200_dynamic_get_build_parameters(self._h, C.byref(a), C.byref(w), C.byref(m), C.byref(p)))
+        return {"alpha": float(a.value), "construction_window_size": int(w.value), "max_candidates": int(m.value),
+                "prune_to": int(p.value)}
+
+    def _set_build_parameter(self, name, value):
+        cur = self._build_parameters()
+        cur[name] = value
+        _lib.check(self._lib.svsb200_dynamic_set_build_parameters(
+            self._h, float(cur["alpha"]), int(cur["construction_window_size"]), int(cur["max_candidates"]),
+            int(cur["prune_to"])))
+
+    # mutation parameters (dynamic_vamana.cpp; 0 restores the default)
+    alpha = property(lambda self: self._build_parameters()["alpha"],
+                     lambda self, v: self._set_build_parameter("alpha", v))
+    construction_window_size = property(lambda self: self._build_parameters()["construction_window_size"],
+                                        lambda self, v: self._set_build_parameter("construction_window_size", v))
+    max_candidates = property(lambda self: self._build_parameters()["max_candidates"],
+                              lambda self, v: self._set_build_parameter("max_candidates", v))
+    prune_to = property(lambda self: self._build_parameters()["prune_to"],
+                        lambda self, v: self._set_build_parameter("prune_to", v))
 
     def search_filtered(self, queries: np.ndarray, n_neighbors: int, allowed: np.ndarray):
         """Filtered search: ``allowed`` is a boolean mask over the SLOTS (``num_slots`` entries, in the order of
