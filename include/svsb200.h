@@ -234,11 +234,14 @@ int svsb200_lvq8_compress(const float* data, size_t n, size_t dim, const float* 
  * batches of max(40, n/4096) rounds, greedy search with full search history + alpha-robust pruning
  * (prune.h: Progressive strategy for L2, Iterative for MIP and cosine), reverse edges with overflow re-pruning to
  * `prune_to`.  Arguments are VamanaBuildParameters (index/vamana/build_params.h): 0 selects the reference's
- * default (alpha 1.2 / 0.95, max_candidate_pool_size = 3 * window_size, prune_to = max_degree - 4).
+ * default (alpha 1.2 / 0.95, max_candidate_pool_size = 3 * window_size clamped to 512, prune_to = max_degree - 4).
+ * The candidate pool holds 512 entries, so max_candidate_pool_size > 512 is refused.  A construction search that
+ * expands more than 4096 nodes fails the build rather than prune from an incomplete history.
  *   vectors     n x dim float32 / float16 rows in HOST memory (row_stride_bytes apart, 0 = dense);
  *   graph_rows_out  uint32[n][graph_max_degree + 1], the reference's in-memory layout (degree first), HOST;
- * The reference's result depends on thread timing, so parity is its own bar: recall equivalence of the
- * built index (tests/integration/vamana/index_build.cpp:96,139-140). */
+ * The reference's result depends on thread timing in rounds of several nodes.  Where every round holds one node
+ * (n <= 40) the rows equal the reference's; larger builds are held to recall equivalence, the reference's own bar
+ * (tests/integration/vamana/index_build.cpp:96,139-140). */
 int svsb200_build_vamana(
     const void* vectors, int dtype, size_t n, size_t dim, size_t row_stride_bytes, int metric,
     float alpha, size_t graph_max_degree, size_t window_size, size_t max_candidate_pool_size,

@@ -24,16 +24,22 @@ __global__ void reverse_insert_kernel(uint32_t first, uint32_t count, const uint
     const uint32_t u = graph[size_t(v) * gstride + j];
     if (u == kNoNeighbor || u == v) return;
     // graph.add_edge(u, v) keeps rows free of repeats (core/graph/graph.h:211-260)
+    // The reference tests the degree first (vamana_build.h:494-500): a full row takes the edge into the overflow even
+    // when it already holds v, so that row is pruned again.
     uint32_t* urow = graph + size_t(u) * gstride;
     const uint32_t du = min(deg[u], max_degree);
-    for (uint32_t z = 0; z < du; ++z)
-        if (urow[z] == v) return;
-    const uint32_t slot = atomicAdd(deg + u, 1u);
-    if (slot < max_degree) {
-        urow[slot] = v;
-        return;
+    bool present = false;
+    for (uint32_t z = 0; z < du && !present; ++z) present = urow[z] == v;
+    if (present) {
+        if (du < max_degree) return;
+    } else {
+        const uint32_t slot = atomicAdd(deg + u, 1u);
+        if (slot < max_degree) {
+            urow[slot] = v;
+            return;
+        }
+        atomicSub(deg + u, 1u);
     }
-    atomicSub(deg + u, 1u);
     const uint32_t e = atomicAdd(pair_count, 1u);
     if (e >= pair_cap) return;
     pair_v[e] = v;
@@ -207,9 +213,8 @@ int medoid(const GraphBuild& b, const uint8_t* d_status, size_t count, uint32_t*
 // The lean search kernel in HIST mode over this graph: parameters and launch configuration (visited filter sized for
 // b.n).  Errors read "<who>: ...".
 static int build_search_config(const char* who, const GraphBuild& b, SearchParams* p, LaunchConfig* cfg) {
-    const uint32_t hist_cap = kPoolMax - b.gstride;
     if (b.window == 0) return fail(std::string(who) + ": window_size must be positive");
-    if (b.window + 32 > hist_cap) return fail(std::string(who) + ": window_size too large for the candidate pool");
+    if (b.window + 32 > kPoolMax - b.gstride) return fail(std::string(who) + ": window_size too large for the candidate pool");
     *p = SearchParams{};
     p->vectors = b.vectors;
     p->graph = b.graph;
@@ -228,7 +233,8 @@ static int build_search_config(const char* who, const GraphBuild& b, SearchParam
     p->cap_pad = uint32_t((b.window + 31) / 32 * 32);
     p->deg_pad = b.gstride;
     p->id_bytes = 4;
-    p->hist_cap = hist_cap;
+    // the whole history is kept; build_prune_kernel selects the pool from it in chunks when it outgrows shared memory
+    p->hist_cap = kHistMax;
     // visited filter of the lean kernel, at its default size
     const LeanFilter lean = lean_filter(b.n, 2048);
     p->filter_slots = lean.slots;
@@ -274,7 +280,8 @@ int construct_graph(const char* who, const GraphBuild& b, float reverse_alpha, u
     CUDA_TRY(d_next.ensure(pair_cap));
     CUDA_TRY(d_pair_v.ensure(pair_cap));
     CUDA_TRY(d_touched.ensure(pair_cap));
-    CUDA_TRY(d_counts.ensure(2));
+    CUDA_TRY(d_counts.ensure(3));   // pair count, touched count, history overflow flag
+    CUDA_TRY(cudaMemsetAsync(d_counts.ptr + 2, 0, 4, stream));
     CUDA_TRY(d_hist.ensure(batchsize * size_t(p.hist_cap)));
     CUDA_TRY(d_hist_count.ensure(batchsize));
     CUDA_TRY(d_qf.ensure(batchsize * size_t(qstride)));
@@ -300,7 +307,8 @@ int construct_graph(const char* who, const GraphBuild& b, float reverse_alpha, u
     bp.deg = b.deg;
     bp.gstride = b.gstride;
     bp.max_degree = R;
-    bp.max_candidates = uint32_t(std::min<size_t>(b.max_candidates, kPoolMax));
+    bp.max_candidates = uint32_t(b.max_candidates);
+    bp.hist_overflow = d_counts.ptr + 2;
     bp.iterative = b.metric != SVSB200_L2;
     bp.work_counter = d_work.ptr;
     bp.count_ptr = d_counts.ptr + 1;
@@ -347,7 +355,12 @@ int construct_graph(const char* who, const GraphBuild& b, float reverse_alpha, u
         count_launch();
         CUDA_TRY(cudaGetLastError());
     }
+    uint32_t hist_overflow = 0;
+    CUDA_TRY(cudaMemcpyAsync(&hist_overflow, d_counts.ptr + 2, 4, cudaMemcpyDeviceToHost, stream));
     CUDA_TRY(cudaStreamSynchronize(stream));
+    if (hist_overflow)
+        return fail(std::string(who) + ": a construction search expanded more than " + std::to_string(kHistMax) +
+                    " nodes; its history would be incomplete");
     return 0;
 }
 
@@ -367,7 +380,10 @@ extern "C" int svsb200_build_vamana(const void* vectors, int dtype, size_t n, si
     if (graph_max_degree == 0 || graph_max_degree > 32u * kFastMaxGW) return fail("svsb200_build_vamana: graph_max_degree must be in [1, 128]");
     if (window_size == 0) return fail("svsb200_build_vamana: window_size must be positive");
     // verify_and_set_default_index_parameters (index/vamana/index.h:1079-1110)
-    if (max_candidate_pool_size == 0) max_candidate_pool_size = 3 * window_size;
+    // The candidate pool holds kPoolMax entries: the default is clamped to it, a larger value refused.
+    if (max_candidate_pool_size == 0) max_candidate_pool_size = std::min<size_t>(3 * window_size, kPoolMax);
+    if (max_candidate_pool_size > kPoolMax)
+        return fail("svsb200_build_vamana: max_candidate_pool_size above 512, the GPU builder's candidate pool");
     if (prune_to == 0) prune_to = graph_max_degree >= 16 ? graph_max_degree - 4 : graph_max_degree;
     if (prune_to > graph_max_degree) return fail("svsb200_build_vamana: prune_to must be <= graph_max_degree");
     if (alpha == 0.f) alpha = metric == SVSB200_L2 ? 1.2f : 0.95f;
