@@ -237,7 +237,10 @@ int svsb200_lvq8_compress(const float* data, size_t n, size_t dim, const float* 
  * default (alpha 1.2 / 0.95, max_candidate_pool_size = 3 * window_size clamped to 512, prune_to = max_degree - 4).
  * The candidate pool holds 512 entries, so max_candidate_pool_size > 512 is refused.  A construction search that
  * expands more than 4096 nodes fails the build rather than prune from an incomplete history.
- *   vectors     n x dim float32 / float16 rows in HOST memory (row_stride_bytes apart, 0 = dense);
+ *   vectors     n x dim float32 / float16 / int8 / uint8 rows in HOST memory (row_stride_bytes apart, 0 = dense).
+ *               int8 / uint8 rows are built with exact int x int distances throughout, as the reference builds
+ *               SimpleData<int8_t / uint8_t> (the datum is its own query); the cosine norm is distance::norm's
+ *               sequential fp32 sum;
  *   graph_rows_out  uint32[n][graph_max_degree + 1], the reference's in-memory layout (degree first), HOST;
  * The reference's result depends on thread timing in rounds of several nodes.  Where every round holds one node
  * (n <= 40) the rows equal the reference's; larger builds are held to recall equivalence, the reference's own bar

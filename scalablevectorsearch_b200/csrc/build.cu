@@ -1,9 +1,11 @@
 // build.cu -- host side of the GPU Vamana graph builder (SURVEY.md §8 f1) + its small helper kernels.
 // Replaces index::vamana::auto_build / VamanaBuilder::construct (index/vamana/index.h:404-440,968-994,
-// vamana_build.h:221-310) for float32 / float16 data with L2 or inner-product distance.
+// vamana_build.h:221-310) for float32 / float16 / int8 / uint8 data with L2, inner-product or cosine distance.  Integer
+// rows are built with exact int x int distances, float rows with the fp32 expression tree of the search.
 #include "build_kernels.cuh"
 #include "host.cuh"
 
+#include <type_traits>
 #include <vector>
 
 namespace svsb200 {
@@ -67,7 +69,9 @@ __global__ void column_sum_kernel(const char* __restrict__ vectors, uint32_t n, 
             if (status && status[r] != SLOT_VALID) continue;
             const char* row = vectors + size_t(r) * row_stride;
             if constexpr (ROWT == SVSB200_F32) acc += double(reinterpret_cast<const float*>(row)[d]);
-            else acc += double(__half2float(reinterpret_cast<const __half*>(row)[d]));
+            else if constexpr (ROWT == SVSB200_F16) acc += double(__half2float(reinterpret_cast<const __half*>(row)[d]));
+            else if constexpr (ROWT == SVSB200_I8) acc += double(reinterpret_cast<const int8_t*>(row)[d]);
+            else acc += double(reinterpret_cast<const uint8_t*>(row)[d]);
         }
         atomicAdd(sums + d, acc);
     }
@@ -92,7 +96,9 @@ __global__ void medoid_distance_kernel(const char* __restrict__ vectors, uint32_
         for (uint32_t d = lane; d < dim; d += 32) {
             double x;
             if constexpr (ROWT == SVSB200_F32) x = double(reinterpret_cast<const float*>(row)[d]);
-            else x = double(__half2float(reinterpret_cast<const __half*>(row)[d]));
+            else if constexpr (ROWT == SVSB200_F16) x = double(__half2float(reinterpret_cast<const __half*>(row)[d]));
+            else if constexpr (ROWT == SVSB200_I8) x = double(reinterpret_cast<const int8_t*>(row)[d]);
+            else x = double(reinterpret_cast<const uint8_t*>(row)[d]);
             const double diff = sums[d] / count - x;
             acc += diff * diff;
         }
@@ -154,6 +160,37 @@ __global__ void batch_queries_kernel(const char* __restrict__ vectors, uint32_t 
     }
 }
 
+// int8 / uint8 batch rows as prepared integer queries (prepare_queries_kernel's PREP_INT mode): the raw codes
+// zero-padded to qstride bytes, {a_norm in distance::norm's order, int32 bits of sum x*x}
+template <int ROWT>
+__global__ void batch_codes_kernel(const char* __restrict__ vectors, uint32_t row_stride, uint32_t dim, uint32_t qstride,
+                                   uint32_t first, uint32_t count, const uint32_t* __restrict__ slots,
+                                   uint8_t* __restrict__ qcodes, float* __restrict__ qaux) {
+    const uint32_t q = blockIdx.x * (blockDim.x / 32) + threadIdx.x / 32;
+    const int lane = threadIdx.x & 31;
+    if (q >= count) return;
+    const char* row = vectors + size_t(slots ? slots[first + q] : first + q) * row_stride;
+    const int xx = stage_codes<ROWT>(row, dim, qstride, reinterpret_cast<uint32_t*>(qcodes + size_t(q) * qstride), lane);
+    const float a_norm = codes_norm<ROWT>(row, dim, xx, lane);
+    if (lane == 0) {
+        qaux[2 * size_t(q)] = a_norm;
+        qaux[2 * size_t(q) + 1] = __int_as_float(xx);
+    }
+}
+
+// f(std::integral_constant<int, T>{}) for the builder's element type T = dtype.
+template <typename F> static cudaError_t with_rowt(int dtype, F&& f) {
+    switch (dtype) {
+        case SVSB200_F32: return f(std::integral_constant<int, SVSB200_F32>{});
+        case SVSB200_F16: return f(std::integral_constant<int, SVSB200_F16>{});
+        case SVSB200_I8: return f(std::integral_constant<int, SVSB200_I8>{});
+        case SVSB200_U8: return f(std::integral_constant<int, SVSB200_U8>{});
+        default: return cudaErrorInvalidValue;
+    }
+}
+
+static bool int_dtype(int dtype) { return dtype == SVSB200_I8 || dtype == SVSB200_U8; }
+
 __global__ void fill_u32_kernel(uint32_t* p, size_t n, uint32_t v) {
     const size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x;
     if (i < n) p[i] = v;
@@ -188,13 +225,12 @@ int medoid(const GraphBuild& b, const uint8_t* d_status, size_t count, uint32_t*
     CUDA_TRY(cudaMemsetAsync(d_sums.ptr, 0, dim * 8, b.stream));
     const char* v = static_cast<const char*>(b.vectors);
     const int narrow = d_status ? 1 : 0;
-    if (b.dtype == SVSB200_F32) {
-        column_sum_kernel<SVSB200_F32><<<unsigned((n + 255) / 256), 128, 0, b.stream>>>(v, uint32_t(n), uint32_t(dim), b.row_stride, d_status, d_sums.ptr);
-        medoid_distance_kernel<SVSB200_F32><<<nblk, 256, 0, b.stream>>>(v, uint32_t(n), uint32_t(dim), b.row_stride, d_status, double(count), narrow, d_sums.ptr, d_best_d.ptr, d_best_i.ptr);
-    } else {
-        column_sum_kernel<SVSB200_F16><<<unsigned((n + 255) / 256), 128, 0, b.stream>>>(v, uint32_t(n), uint32_t(dim), b.row_stride, d_status, d_sums.ptr);
-        medoid_distance_kernel<SVSB200_F16><<<nblk, 256, 0, b.stream>>>(v, uint32_t(n), uint32_t(dim), b.row_stride, d_status, double(count), narrow, d_sums.ptr, d_best_d.ptr, d_best_i.ptr);
-    }
+    CUDA_TRY(with_rowt(b.dtype, [&](auto t) {
+        constexpr int T = decltype(t)::value;
+        column_sum_kernel<T><<<unsigned((n + 255) / 256), 128, 0, b.stream>>>(v, uint32_t(n), uint32_t(dim), b.row_stride, d_status, d_sums.ptr);
+        medoid_distance_kernel<T><<<nblk, 256, 0, b.stream>>>(v, uint32_t(n), uint32_t(dim), b.row_stride, d_status, double(count), narrow, d_sums.ptr, d_best_d.ptr, d_best_i.ptr);
+        return cudaSuccess;
+    }));
     count_launch();
     count_launch();
     CUDA_TRY(cudaGetLastError());
@@ -274,6 +310,7 @@ int construct_graph(const char* who, const GraphBuild& b, float reverse_alpha, u
     DeviceBuffer<int> d_head, d_next;
     DeviceBuffer<uint2> d_hist;
     DeviceBuffer<float> d_qf, d_qaux;
+    DeviceBuffer<uint8_t> d_qcodes;
     DeviceBuffer<unsigned int> d_work;
     CUDA_TRY(d_head.ensure(b.n));
     CUDA_TRY(cudaMemsetAsync(d_head.ptr, 0xFF, b.n * 4, stream));
@@ -284,17 +321,23 @@ int construct_graph(const char* who, const GraphBuild& b, float reverse_alpha, u
     CUDA_TRY(cudaMemsetAsync(d_counts.ptr + 2, 0, 4, stream));
     CUDA_TRY(d_hist.ensure(batchsize * size_t(p.hist_cap)));
     CUDA_TRY(d_hist_count.ensure(batchsize));
-    CUDA_TRY(d_qf.ensure(batchsize * size_t(qstride)));
+    const bool ints = int_dtype(dtype);
+    if (ints) CUDA_TRY(d_qcodes.ensure(batchsize * size_t(qstride)));
+    else CUDA_TRY(d_qf.ensure(batchsize * size_t(qstride)));
     CUDA_TRY(d_qaux.ensure(batchsize * 2));
     CUDA_TRY(cudaMemsetAsync(d_qaux.ptr, 0, batchsize * 2 * 4, stream));
     CUDA_TRY(d_work.ensure(1));
     p.entry_point = entry_point;
     p.qf = d_qf.ptr;
+    p.qcodes = d_qcodes.ptr;
     p.qaux = d_qaux.ptr;
     p.work_counter = d_work.ptr;
     p.hist = d_hist.ptr;
     p.hist_count = d_hist_count.ptr;
-    const int op = b.metric == SVSB200_L2 ? OP_L2F : b.metric == SVSB200_IP ? OP_IPF : OP_COSF;
+    // integer rows: int x int distances throughout, as the reference's default build adaptor uses the datum itself as
+    // the query (extensions.h:114-282)
+    const int op = ints ? (b.metric == SVSB200_L2 ? OP_L2I : b.metric == SVSB200_IP ? OP_IPI : OP_COSI)
+                        : (b.metric == SVSB200_L2 ? OP_L2F : b.metric == SVSB200_IP ? OP_IPF : OP_COSF);
 
     BuildParams bp{};
     bp.hist = d_hist.ptr;
@@ -322,14 +365,18 @@ int construct_graph(const char* who, const GraphBuild& b, float reverse_alpha, u
         if (stop == start) continue;
         const uint32_t B = uint32_t(stop - start);
         // 1. generate_neighbors: search ...
-        if (dtype == SVSB200_F32)
-            batch_queries_kernel<SVSB200_F32><<<(B + 7) / 8, 256, 0, stream>>>(vectors, row_stride, uint32_t(b.dim), qstride, uint32_t(start), B, d_slots, d_qf.ptr, d_qaux.ptr);
-        else
-            batch_queries_kernel<SVSB200_F16><<<(B + 7) / 8, 256, 0, stream>>>(vectors, row_stride, uint32_t(b.dim), qstride, uint32_t(start), B, d_slots, d_qf.ptr, d_qaux.ptr);
+        CUDA_TRY(with_rowt(dtype, [&](auto t) {
+            constexpr int T = decltype(t)::value;
+            if constexpr (T == SVSB200_I8 || T == SVSB200_U8)
+                batch_codes_kernel<T><<<(B + 7) / 8, 256, 0, stream>>>(vectors, row_stride, uint32_t(b.dim), qstride, uint32_t(start), B, d_slots, d_qcodes.ptr, d_qaux.ptr);
+            else
+                batch_queries_kernel<T><<<(B + 7) / 8, 256, 0, stream>>>(vectors, row_stride, uint32_t(b.dim), qstride, uint32_t(start), B, d_slots, d_qf.ptr, d_qaux.ptr);
+            return cudaSuccess;
+        }));
         count_launch();
         CUDA_TRY(cudaMemsetAsync(d_work.ptr, 0, 4, stream));
         p.nq = B;
-        CUDA_TRY(dtype == SVSB200_F32 ? launch_build_search<SVSB200_F32>(op, p, cfg) : launch_build_search<SVSB200_F16>(op, p, cfg));
+        CUDA_TRY(with_rowt(dtype, [&](auto t) { return launch_build_search<decltype(t)::value>(op, p, cfg); }));
         // ... pool + prune (always with the configured alpha, vamana_build.h:268-272)
         CUDA_TRY(cudaMemsetAsync(d_work.ptr, 0, 4, stream));
         bp.reverse = PRUNE_FORWARD;
@@ -337,8 +384,9 @@ int construct_graph(const char* who, const GraphBuild& b, float reverse_alpha, u
         bp.count = B;
         bp.limit = R;
         bp.alpha = b.alpha;
-        CUDA_TRY(dtype == SVSB200_F32 ? launch_build_prune_op<SVSB200_F32>(op, p, bp, std::min<int>(prune_grid, int(B)), stream)
-                                      : launch_build_prune_op<SVSB200_F16>(op, p, bp, std::min<int>(prune_grid, int(B)), stream));
+        CUDA_TRY(with_rowt(dtype, [&](auto t) {
+            return launch_build_prune_op<decltype(t)::value>(op, p, bp, std::min<int>(prune_grid, int(B)), stream);
+        }));
         // 2. add_reverse_edges
         CUDA_TRY(cudaMemsetAsync(d_counts.ptr, 0, 8, stream));
         reverse_insert_kernel<<<unsigned((size_t(B) * R + 255) / 256), 256, 0, stream>>>(
@@ -349,8 +397,7 @@ int construct_graph(const char* who, const GraphBuild& b, float reverse_alpha, u
         bp.reverse = PRUNE_REVERSE;
         bp.limit = uint32_t(b.prune_to);
         bp.alpha = reverse_alpha;
-        CUDA_TRY(dtype == SVSB200_F32 ? launch_build_prune_op<SVSB200_F32>(op, p, bp, prune_grid, stream)
-                                      : launch_build_prune_op<SVSB200_F16>(op, p, bp, prune_grid, stream));
+        CUDA_TRY(with_rowt(dtype, [&](auto t) { return launch_build_prune_op<decltype(t)::value>(op, p, bp, prune_grid, stream); }));
         reset_heads_kernel<<<unsigned((pair_cap + 255) / 256), 256, 0, stream>>>(d_touched.ptr, d_counts.ptr + 1, d_head.ptr);
         count_launch();
         CUDA_TRY(cudaGetLastError());
@@ -374,7 +421,7 @@ extern "C" int svsb200_build_vamana(const void* vectors, int dtype, size_t n, si
                                     uint32_t* entry_point_out) {
     const char* who = "svsb200_build_vamana";
     if (!vectors || !graph_rows_out || !entry_point_out) return fail("svsb200_build_vamana: NULL argument");
-    if (dtype != SVSB200_F32 && dtype != SVSB200_F16) return fail("svsb200_build_vamana: float32 / float16 data only");
+    if (dtype < SVSB200_F32 || dtype > SVSB200_U8) return fail("svsb200_build_vamana: bad dtype");
     if (metric < SVSB200_L2 || metric > SVSB200_COSINE) return fail("svsb200_build_vamana: bad metric");
     if (n < 2 || dim == 0 || n >= (size_t(1) << 31)) return fail("svsb200_build_vamana: bad shape");
     if (graph_max_degree == 0 || graph_max_degree > 32u * kFastMaxGW) return fail("svsb200_build_vamana: graph_max_degree must be in [1, 128]");

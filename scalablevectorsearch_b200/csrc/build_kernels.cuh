@@ -21,7 +21,8 @@
 // every round holds one node (static builds of n <= 40, dynamic adds of at most 40 points); equal neighbour sets
 // for large adds into an existing graph; recall equivalence of whole static builds, the reference's own bar
 // (tests/integration/vamana/index_build.cpp:96,139).
-// Distances inside the builder use the search path's bit-exact code (eval_pass), keys = sign * distance.
+// Distances inside the builder use the search path's bit-exact code (eval_pass), keys = sign * distance: the float tree
+// for float32 / float16 rows, the exact integer ops (OP_*I) for int8 / uint8 rows, whose datum is its own query.
 //
 // The dynamic index reuses these kernels: add_points runs `construct` over a list of slots (BuildParams::slots),
 // and consolidate (consolidate.h) selects each node's candidate pool with `consolidate_pool_kernel` and prunes it
@@ -78,24 +79,70 @@ __host__ __device__ inline size_t build_smem_bytes(uint32_t qstride) {
     return size_t(qstride) * 4 + size_t(kPoolMax) * 4 * 6 + 256 * 4;
 }
 
-// Row `id` of the dataset as the fp32 operand the distance code expects in q_s (what prepare_queries_kernel
-// does for a query: exact conversion, zero padding).
-// Returns the row's Euclidean norm (the `a_norm` of CosineSimilarity::fix_argument, cosine.h:117-119).
+// An int8 / uint8 row's codes as the integer distance code expects its operand (what prepare_queries_kernel writes in
+// PREP_INT mode): the raw bytes, zero-padded to qstride (a multiple of 16) bytes, to `dst`.  Returns the exact sum x*x.
 template <int ROWT>
-__device__ __forceinline__ float stage_row(const SearchParams& p, uint32_t id, float* q_s, int lane) {
-    const char* row = reinterpret_cast<const char*>(p.vectors) + size_t(id) * p.row_stride;
-    float sq = 0.f;
-    for (uint32_t i = lane; i < p.qstride; i += 32) {
-        float v = 0.f;
-        if (i < p.dim) {
-            if constexpr (ROWT == SVSB200_F32) v = reinterpret_cast<const float*>(row)[i];
-            else v = __half2float(reinterpret_cast<const __half*>(row)[i]);
+__device__ __forceinline__ int stage_codes(const char* row, uint32_t dim, uint32_t qstride, uint32_t* dst, int lane) {
+    int xx = 0;
+    for (uint32_t i = lane; i < qstride / 4; i += 32) {
+        uint32_t w = 0;
+        if (4 * i < dim) {
+            w = reinterpret_cast<const uint32_t*>(row)[i];
+            if (4 * i + 4 > dim) w &= (1u << (8 * (dim - 4 * i))) - 1u;
         }
-        q_s[i] = v;
-        sq = fmaf(v, v, sq);
+        dst[i] = w;
+        if constexpr (ROWT == SVSB200_I8) xx = __dp4a(int(w), int(w), xx);
+        else xx = int(__dp4a(w, w, unsigned(xx)));
     }
-    for (int o = 16; o; o >>= 1) sq += __shfl_xor_sync(0xFFFFFFFFu, sq, o);
-    return sqrtf(sq);
+    for (int o = 16; o; o >>= 1) xx += __shfl_xor_sync(0xFFFFFFFFu, xx, o);
+    return xx;
+}
+
+// The cosine `a_norm` of an int8 / uint8 row (CosineSimilarity::fix_argument -> distance::norm, distance_core.h:45-66):
+// sqrt of a sequential fp32 `accum += x*x`.  Every partial sum is a non-negative integer no larger than xx, so while
+// xx <= 2^24 they are all exact and the result is float(xx); above that the order rounds, and lane 0 repeats the sum in
+// the reference's order.
+template <int ROWT>
+__device__ __forceinline__ float codes_norm(const char* row, uint32_t dim, int xx, int lane) {
+    float acc = float(xx);
+    if (xx > (1 << 24)) {
+        if (lane == 0) {
+            acc = 0.f;
+            for (uint32_t i = 0; i < dim; ++i) {
+                const int v = ROWT == SVSB200_I8 ? int(int8_t(row[i])) : int(uint8_t(row[i]));
+                acc = __fadd_rn(acc, float(v * v));
+            }
+        }
+        acc = __shfl_sync(0xFFFFFFFFu, acc, 0);
+    }
+    return __fsqrt_rn(acc);
+}
+
+// Row `id` of the dataset as the operand the distance code expects in q_s (what prepare_queries_kernel does for a
+// query): for the float ops the exact fp32 conversion, zero padding; for the integer ops the raw codes (stage_codes),
+// with `aux1` = the int32 bits of sum x*x that OP_L2I needs.
+// Returns the row's Euclidean norm (the `a_norm` of CosineSimilarity::fix_argument, cosine.h:117-119).
+template <int ROWT, int OP>
+__device__ __forceinline__ float stage_row(const SearchParams& p, uint32_t id, float* q_s, int lane, float& aux1) {
+    const char* row = reinterpret_cast<const char*>(p.vectors) + size_t(id) * p.row_stride;
+    if constexpr (OP >= OP_L2I) {
+        const int xx = stage_codes<ROWT>(row, p.dim, p.qstride, reinterpret_cast<uint32_t*>(q_s), lane);
+        aux1 = __int_as_float(xx);
+        return codes_norm<ROWT>(row, p.dim, xx, lane);
+    } else {
+        float sq = 0.f;
+        for (uint32_t i = lane; i < p.qstride; i += 32) {
+            float v = 0.f;
+            if (i < p.dim) {
+                if constexpr (ROWT == SVSB200_F32) v = reinterpret_cast<const float*>(row)[i];
+                else v = __half2float(reinterpret_cast<const __half*>(row)[i]);
+            }
+            q_s[i] = v;
+            sq = fmaf(v, v, sq);
+        }
+        for (int o = 16; o; o >>= 1) sq += __shfl_xor_sync(0xFFFFFFFFu, sq, o);
+        return sqrtf(sq);
+    }
 }
 
 // Sorts the first `count` (key, id) pairs by TotalOrder (key, then id), one warp: bitonic over the next power of two
@@ -161,7 +208,7 @@ __device__ __forceinline__ uint32_t merge_into_pool(float* ckey, uint32_t* cid, 
 template <int ROWT, int OP, int DS, int KS>
 __global__ void __launch_bounds__(32, 16) build_prune_kernel(const __grid_constant__ SearchParams p,
                                                             const __grid_constant__ BuildParams bp) {
-    constexpr int G = KS * 16 / Row<ROWT>::LPT;
+    constexpr int G = OP >= OP_L2I ? 4 : KS * 16 / Row<ROWT>::LPT;   // threads per row, as in eval_pass
     constexpr int GROUPS = 32 / G;
     constexpr unsigned FULL = 0xFFFFFFFFu;
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -193,9 +240,10 @@ __global__ void __launch_bounds__(32, 16) build_prune_kernel(const __grid_consta
         uint32_t P = 0;       // entries whose key is known
         uint32_t M = 0;       // entries of lid[] whose distance to `node` still has to be computed
         float qnorm = 1.0f;   // cosine: norm of the vector currently staged as the query
+        float qaux1 = 0.f;    // OP_L2I: int32 bits of sum x*x of the vector currently staged as the query
         if (bp.reverse == PRUNE_CONSOLIDATE) {
             // the whole pool, keys included, as consolidate_pool_kernel selected it
-            qnorm = stage_row<ROWT>(p, node, q_s, lane);
+            qnorm = stage_row<ROWT, OP>(p, node, q_s, lane, qaux1);
             P = min(bp.hist_count[w], min(bp.hist_cap, kPoolMax));
             for (uint32_t i = lane; i < P; i += 32) {
                 const uint2 e = bp.hist[size_t(w) * bp.hist_cap + i];
@@ -204,7 +252,13 @@ __global__ void __launch_bounds__(32, 16) build_prune_kernel(const __grid_consta
             }
         } else if (!bp.reverse) {
             // the node as a query: prepared by the search launch of this round
-            for (uint32_t i = lane; i < p.qstride; i += 32) q_s[i] = p.qf[size_t(w) * p.qstride + i];
+            if constexpr (OP >= OP_L2I) {
+                const uint32_t* src = reinterpret_cast<const uint32_t*>(p.qcodes + size_t(w) * p.qstride);
+                for (uint32_t i = lane; i < p.qstride / 4; i += 32) reinterpret_cast<uint32_t*>(q_s)[i] = src[i];
+                qaux1 = p.qaux[2 * size_t(w) + 1];
+            } else {
+                for (uint32_t i = lane; i < p.qstride; i += 32) q_s[i] = p.qf[size_t(w) * p.qstride + i];
+            }
             qnorm = p.qaux[2 * size_t(w)];
             const uint32_t H = bp.hist_count[w];
             // the search stops recording at hist_cap entries: the history may be incomplete, so the build fails
@@ -225,7 +279,7 @@ __global__ void __launch_bounds__(32, 16) build_prune_kernel(const __grid_consta
                 }
                 __syncwarp();
                 for (uint32_t base = 0; base < Q; base += 2 * GROUPS)
-                    eval_pass<ROWT, OP, DS, 2, KS, true>(p, q_s, vectors, lid, lkey, base, Q, g, t, qnorm, 0.f, ksign);
+                    eval_pass<ROWT, OP, DS, 2, KS, true>(p, q_s, vectors, lid, lkey, base, Q, g, t, qnorm, qaux1, ksign);
                 __syncwarp();
                 warp_sort_pairs(lkey, lid, Q, lane);
                 P = merge_into_pool(ckey, cid, 0, lkey, lid, Q, bp.max_candidates, state, lpos, lane);
@@ -260,7 +314,7 @@ __global__ void __launch_bounds__(32, 16) build_prune_kernel(const __grid_consta
                 }
             }
         } else {
-            qnorm = stage_row<ROWT>(p, node, q_s, lane);
+            qnorm = stage_row<ROWT, OP>(p, node, q_s, lane, qaux1);
             // overflow edges of this round (vamana_build.h:528-531): one per node of the round that links here, so
             // they are distinct and none is the node itself
             uint32_t nover = 0;
@@ -282,7 +336,7 @@ __global__ void __launch_bounds__(32, 16) build_prune_kernel(const __grid_consta
                 const uint32_t nrow = Q;
                 __syncwarp();
                 for (uint32_t base = 0; base < Q; base += 2 * GROUPS)
-                    eval_pass<ROWT, OP, DS, 2, KS, true>(p, q_s, vectors, lid, lkey, base, Q, g, t, qnorm, 0.f, ksign);
+                    eval_pass<ROWT, OP, DS, 2, KS, true>(p, q_s, vectors, lid, lkey, base, Q, g, t, qnorm, qaux1, ksign);
                 __syncwarp();
                 warp_sort_pairs(lkey, lid, Q, lane);
                 P = merge_into_pool(ckey, cid, 0, lkey, lid, Q, bp.max_candidates, state, lpos, lane);
@@ -305,7 +359,7 @@ __global__ void __launch_bounds__(32, 16) build_prune_kernel(const __grid_consta
                     }
                     __syncwarp();
                     for (uint32_t base = 0; base < U; base += 2 * GROUPS)
-                        eval_pass<ROWT, OP, DS, 2, KS, true>(p, q_s, vectors, lid, lkey, base, U, g, t, qnorm, 0.f, ksign);
+                        eval_pass<ROWT, OP, DS, 2, KS, true>(p, q_s, vectors, lid, lkey, base, U, g, t, qnorm, qaux1, ksign);
                     __syncwarp();
                     warp_sort_pairs(lkey, lid, U, lane);
                     P = merge_into_pool(ckey, cid, P, lkey, lid, U, bp.max_candidates, state, lpos, lane);
@@ -332,7 +386,7 @@ __global__ void __launch_bounds__(32, 16) build_prune_kernel(const __grid_consta
         __syncwarp();
         // distances node -> lid[0..M), appended to the pool
         for (uint32_t base = 0; base < M; base += 2 * GROUPS)
-            eval_pass<ROWT, OP, DS, 2, KS, true>(p, q_s, vectors, lid, lkey, base, M, g, t, qnorm, 0.f, ksign);
+            eval_pass<ROWT, OP, DS, 2, KS, true>(p, q_s, vectors, lid, lkey, base, M, g, t, qnorm, qaux1, ksign);
         __syncwarp();
         for (uint32_t i = lane; i < M; i += 32) {
             cid[P + i] = lid[i];
@@ -374,7 +428,7 @@ __global__ void __launch_bounds__(32, 16) build_prune_kernel(const __grid_consta
                     res[nres] = cid[j];
                 }
                 ++nres;
-                qnorm = stage_row<ROWT>(p, cid[j], q_s, lane);
+                qnorm = stage_row<ROWT, OP>(p, cid[j], q_s, lane, qaux1);
                 __syncwarp();
                 // the later entries still available at this level, compacted
                 uint32_t L = 0;
@@ -396,7 +450,7 @@ __global__ void __launch_bounds__(32, 16) build_prune_kernel(const __grid_consta
                 if (L == 0) continue;
                 // djk for every listed entry: key(selected, candidate)
                 for (uint32_t base = 0; base < L; base += 2 * GROUPS)
-                    eval_pass<ROWT, OP, DS, 2, KS, true>(p, q_s, vectors, lid, lkey, base, L, g, t, qnorm, 0.f, ksign);
+                    eval_pass<ROWT, OP, DS, 2, KS, true>(p, q_s, vectors, lid, lkey, base, L, g, t, qnorm, qaux1, ksign);
                 __syncwarp();
                 for (uint32_t i = lane; i < L; i += 32) {
                     const uint32_t tt = lpos[i];
@@ -502,10 +556,11 @@ __global__ void __launch_bounds__(32, 16) consolidate_pool_kernel(const __grid_c
         }
         __syncwarp();
         // ---- filter_candidates: distances from the node, TotalOrder ----
-        const float qnorm = stage_row<ROWT>(p, node, q_s, lane);
+        float qaux1 = 0.f;
+        const float qnorm = stage_row<ROWT, OP>(p, node, q_s, lane, qaux1);
         __syncwarp();
         for (uint32_t base = 0; base < U; base += 2 * GROUPS)
-            eval_pass<ROWT, OP, DS, 2, KS, true>(p, q_s, vectors, sid, skey, base, U, g, t, qnorm, 0.f, ksign);
+            eval_pass<ROWT, OP, DS, 2, KS, true>(p, q_s, vectors, sid, skey, base, U, g, t, qnorm, qaux1, ksign);
         __syncwarp();
         warp_sort_pairs(skey, sid, U, lane);
         const uint32_t P = min(U, bp.max_candidates);
@@ -525,8 +580,10 @@ template <int ROWT, int OP> cudaError_t launch_build_prune(const SearchParams& p
         count_launch();
         return cudaGetLastError();
     };
-    if (p.dim == 96) return go(build_prune_kernel<ROWT, OP, 96, 1>);
-    if (p.dim >= 256) return go(build_prune_kernel<ROWT, OP, 0, 4>);
+    if constexpr (OP < OP_L2I) {   // the integer distance code has one shape for every dimension
+        if (p.dim == 96) return go(build_prune_kernel<ROWT, OP, 96, 1>);
+        if (p.dim >= 256) return go(build_prune_kernel<ROWT, OP, 0, 4>);
+    }
     return go(build_prune_kernel<ROWT, OP, 0, 1>);
 }
 
@@ -544,9 +601,10 @@ cudaError_t launch_consolidate_pool(const SearchParams& p, const BuildParams& bp
     return go(consolidate_pool_kernel<ROWT, OP, 0, 1>);
 }
 
-// Defined in build_f32.cu / build_f16.cu.
+// Defined in build_f32.cu / build_f16.cu / build_i8.cu / build_u8.cu; the int8 / uint8 forms take the integer ops.
 template <int ROWT> cudaError_t launch_build_search(int op, const SearchParams& p, const LaunchConfig& cfg);
 template <int ROWT> cudaError_t launch_build_prune_op(int op, const SearchParams& p, const BuildParams& bp, int grid, cudaStream_t stream);
+// Float32 / float16 only: the dynamic index takes no integer data.
 template <int ROWT>
 cudaError_t launch_consolidate_pool_op(int op, const SearchParams& p, const BuildParams& bp, int grid, cudaStream_t stream);
 

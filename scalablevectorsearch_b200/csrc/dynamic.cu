@@ -576,6 +576,7 @@ int svsb200_dynamic_build(const void* vectors, int dtype, size_t n, size_t dim, 
     const char* who = "svsb200_dynamic_build";
     if (!out) return fail("svsb200_dynamic_build: NULL output");
     *out = nullptr;
+    if (dtype != SVSB200_F32 && dtype != SVSB200_F16) return fail("svsb200_dynamic_build: float32 / float16 data only");
     if (metric < SVSB200_L2 || metric > SVSB200_COSINE) return fail("svsb200_dynamic_build: bad metric");
     if (graph_max_degree == 0 || graph_max_degree > 32u * kFastMaxGW)
         return fail("svsb200_dynamic_build: graph_max_degree must be in [1, 128]");

@@ -272,8 +272,9 @@ int search_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, const void* d
                      bool exhaustive = false);
 
 // ---- graph construction (build.cu), shared by svsb200_build_vamana and the dynamic index ----
-// A float32 / float16 graph on the current device: n rows (row_stride apart), adjacency rows (gstride apart, neighbours
-// first, kNoNeighbor padding) and the row lengths, with VamanaBuildParameters.
+// A float32 / float16 / int8 / uint8 graph (the dynamic index: float32 / float16) on the current device: n rows
+// (row_stride apart), adjacency rows (gstride apart, neighbours first, kNoNeighbor padding) and the row lengths, with
+// VamanaBuildParameters.
 struct GraphBuild {
     int dtype = 0, metric = 0;
     size_t n = 0, dim = 0;

@@ -147,10 +147,11 @@ class VamanaBuildParameters:
 def build_graph(data: np.ndarray, distance: "DistanceType", parameters: VamanaBuildParameters, device: int = 0):
     """Vamana graph construction on the GPU (``svsb200_build_vamana``; stands where ``svs.Vamana.build`` /
     ``index::vamana::auto_build`` runs the reference's CPU builder).  Returns ``(graph uint32[n][R+1] in the
-    reference's degree-first layout, entry_point)``."""
+    reference's degree-first layout, entry_point)``.  int8 / uint8 rows are built with exact integer distances, as the
+    reference builds ``SimpleData<int8_t / uint8_t>``."""
     data = np.ascontiguousarray(data)
-    if data.dtype not in (np.float32, np.float16) or data.ndim != 2:
-        raise TypeError("build_graph takes a 2-D float32 / float16 array")
+    if data.dtype not in _DTYPE_CODE or data.ndim != 2:
+        raise TypeError("build_graph takes a 2-D float32 / float16 / int8 / uint8 array")
     if not parameters.use_full_search_history:
         raise ValueError("the GPU builder always keeps the full search history (the reference's default)")
     lib = _lib.lib()
