@@ -23,11 +23,15 @@ import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
 
-def uint8_rows(n, dim):
+def uint8_rows(n, dim, nq=0):
+    """n base rows; with nq > 0, also nq queries of the same law through the same mapping (clipped to 0..255)."""
     from scalablevectorsearch_b200.synthetic import clustered_unit_vectors
-    base, _ = clustered_unit_vectors(n, 1, dim)
+    base, queries = clustered_unit_vectors(n, max(nq, 1), dim)
     lo, hi = float(base.min()), float(base.max())
-    return np.rint((base - lo) * (255.0 / (hi - lo))).astype(np.uint8)
+    rows = np.rint((base - lo) * (255.0 / (hi - lo))).astype(np.uint8)
+    if nq == 0:
+        return rows
+    return rows, np.rint(np.clip((queries - lo) * (255.0 / (hi - lo)), 0.0, 255.0)).astype(np.uint8)
 
 
 def main():

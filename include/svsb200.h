@@ -265,7 +265,12 @@ int svsb200_flat_plan(size_t nq, size_t n, int sm_count, uint32_t* ctas, uint32_
  * candidates are re-scored with the graph search's own bit-exact distance code, and an error bound on the fp16
  * products proves per query that no other vector can belong to the top k; queries that fail the proof are
  * re-run by the exact scan.  The result therefore always equals svsb200_exhaustive_device bit for bit (ids and
- * distances; ties by id).  float32/float16 data and queries, L2 and MIP, k <= 25; other shapes take the scan.
+ * distances; ties by id).  GEMM shapes, all with L2 or MIP, plain storage, k <= 25 and n >= 512:
+ *   - float32/float16 data with float32/float16 queries, and int8/uint8 data with float32 queries: the fp16 GEMM;
+ *   - (int8, int8) and (uint8, uint8) up to dim 32768: an exact int8/uint8 GEMM (wgmma s32.s8.s8 / s32.u8.u8) whose
+ *     candidate lists are exact in (distance, id) order, so no query needs the scan while distances stay below 2^24.
+ * Other shapes (cosine, SQ, LVQ-8, integer rows wider than 32768, float rows wider than about 55000, ...) take
+ * the scan.
  * `fallback_queries` (optional) receives how many queries needed the scan. */
 int svsb200_flat_search_device(
     svsb200_index* index, const void* d_queries, int qdtype, size_t nq, size_t k,

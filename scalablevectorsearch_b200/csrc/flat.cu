@@ -26,10 +26,36 @@
 // the products are exact in fp32 and the tensor-core accumulation of `dim` of them adds at most dim 2^-22 ||q|| ||x||;
 // for L2 the bias |x~|^2 differs from |x|^2 by at most 2^-10 ||x||^2 when the data was rounded.  So
 //   E_ip(q) = (r 2^-11 + dim 2^-22) ||q|| Xmax,      E_l2(q) = 2 E_ip(q) + [data rounded] 2^-10 Xmax^2.
+// int8 / uint8 data with float32 queries takes this path too: integers up to 255 are exact in fp16, so only the query
+// is rounded (r = 1).  The bias is the exact integer |x|^2 converted once (at most 2^-24 Xmax^2 off), and the fp32 key
+// bias - 2 s~ is itself rounded once (2^-24 of |x|^2 + 2 |q| |x|), so integer data adds an explicit [integer data]
+// 2^-23 Xmax^2 to E_l2.  The 2^-23 |q| |x| part is NOT inside r 2^-11, which the query's rounding uses up: it is
+// covered by the accumulation term, whose dim 2^-22 (doubled in E_l2) is twice the dim 2^-23 that a truncating fp32
+// accumulator can lose (four times round-to-nearest's); the spare dim 2^-22 >= 2^-23 holds it.  Tightening the dim
+// term below 2x would have to add 2^-23 |q| Xmax explicitly.  (The same margin holds the key rounding of float data.)
+//
+// Integer path: (int8, int8) and (uint8, uint8) with dim <= 32768 run `wgmma.mma_async.m64n256k32.s32.{s8.s8,u8.u8}`
+// instead, over tiles of the raw codes (64-element k-blocks: one blob has the bytes of an fp16 blob, so the ring, the
+// producer and the work split are the same).  Every sum is exact in int32 (32768 * 255^2 < 2^31), and so is the key
+// K = |x|^2 - 2 s (L2) or -s (inner product).  The lists hold the KC smallest (K, id) PAIRS of their range, so each
+// is exact, ties included.  The reported distance is a monotone function F of K: float(|q|^2 + K) for L2, float(K) for
+// the key of inner product (-float(s)); call v(K) the integer inside the float.  Every row outside the candidates has
+// a pair above T, the smallest list-maximum pair, and the k-th result has the pair (K_k, id_k).  The result is exact iff
+// every excluded row ranks after the k-th result by (F, id), which holds when either
+//   (a) F(T.K) > F(K_k): then F(K) >= F(T.K) > F(K_k) for every excluded row, or
+//   (b) |v(T.K)| < 2^24 and T > (K_k, id_k): v(T.K) - 1, v(T.K) and v(T.K) + 1 are exact floats, so
+//       F(T.K - 1) < F(T.K) < F(T.K + 1).  An excluded row has K >= T.K >= K_k.  If K_k < T.K, then
+//       F(K_k) <= F(T.K - 1) < F(T.K) <= F(K).  If K_k = T.K, a row with K > T.K has F(K) >= F(T.K + 1) > F(K_k), and
+//       one with K = T.K has an id above T.id > id_k.  (At |v| = 2^24 the bound fails: 2^24 + 1 rounds to 2^24.)
+// Below 2^24 (b) always holds, so no query falls back.  The GEMM key is also checked against the rescored distance,
+// F(K) == the exact distance for every candidate: a wrong integer GEMM shows as a fallback, not a wrong answer.
 #include "host.cuh"
 #include "search_kernel.cuh"
 
 #include <cuda_fp16.h>
+
+#include <climits>
+#include <type_traits>
 
 namespace svsb200 {
 
@@ -40,6 +66,10 @@ constexpr uint32_t FLAT_STAGES = 6;
 constexpr uint32_t FLAT_KC = 33;                                     // list entries per (query, base range)
 constexpr uint32_t FLAT_LEAD = 4;                                    // tiles a CTA may run ahead of its segment's slowest CTA
 constexpr uint32_t FLAT_CMAX = 1024;                                 // candidates per query the rescoring kernel holds
+constexpr uint32_t FLAT_BK8 = 64;                                    // k elements per blob of 8-bit operands (same bytes)
+constexpr uint32_t FLAT_INT_MAX_DIM = 32768;                         // integer GEMM: every int32 sum and key is exact
+// Operand kind of the GEMM: fp16 (float data, or integer data with float32 queries) or the raw int8 / uint8 codes.
+enum FlatKind : int { FLAT_F16 = 0, FLAT_S8 = 1, FLAT_U8 = 2 };
 
 // ---- PTX helpers -------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
@@ -117,6 +147,49 @@ __device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t adesc
           "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
         : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
+// D (64 x 256, int32, in registers) [+]= A (64 x 32) . B (256 x 32)^T, both int8 (KIND FLAT_S8) or uint8 (FLAT_U8)
+// K-major in shared memory: the same descriptors as the fp16 MMA, a core matrix being 8 rows x 16 one-byte elements.
+#define FLAT_WGMMA_INT(TYPE)                                                                                          \
+    asm volatile(                                                                                                     \
+        "{\n\t"                                                                                                       \
+        ".reg .pred p;\n\t"                                                                                           \
+        "setp.ne.b32 p, %130, 0;\n\t"                                                                                 \
+        "wgmma.mma_async.sync.aligned.m64n256k32.s32." TYPE "." TYPE " "                                              \
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "                                     \
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "                            \
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "                            \
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "                            \
+        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "                            \
+        "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "                            \
+        "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "                 \
+        "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "           \
+        "%128, %129, p;\n\t"                                                                                          \
+        "}\n"                                                                                                         \
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),             \
+          "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),       \
+          "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),     \
+          "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]),     \
+          "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]),     \
+          "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]),     \
+          "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]),     \
+          "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63]),     \
+          "+r"(d[64]), "+r"(d[65]), "+r"(d[66]), "+r"(d[67]), "+r"(d[68]), "+r"(d[69]), "+r"(d[70]), "+r"(d[71]),     \
+          "+r"(d[72]), "+r"(d[73]), "+r"(d[74]), "+r"(d[75]), "+r"(d[76]), "+r"(d[77]), "+r"(d[78]), "+r"(d[79]),     \
+          "+r"(d[80]), "+r"(d[81]), "+r"(d[82]), "+r"(d[83]), "+r"(d[84]), "+r"(d[85]), "+r"(d[86]), "+r"(d[87]),     \
+          "+r"(d[88]), "+r"(d[89]), "+r"(d[90]), "+r"(d[91]), "+r"(d[92]), "+r"(d[93]), "+r"(d[94]), "+r"(d[95]),     \
+          "+r"(d[96]), "+r"(d[97]), "+r"(d[98]), "+r"(d[99]), "+r"(d[100]), "+r"(d[101]), "+r"(d[102]), "+r"(d[103]), \
+          "+r"(d[104]), "+r"(d[105]), "+r"(d[106]), "+r"(d[107]), "+r"(d[108]), "+r"(d[109]), "+r"(d[110]),           \
+          "+r"(d[111]), "+r"(d[112]), "+r"(d[113]), "+r"(d[114]), "+r"(d[115]), "+r"(d[116]), "+r"(d[117]),           \
+          "+r"(d[118]), "+r"(d[119]), "+r"(d[120]), "+r"(d[121]), "+r"(d[122]), "+r"(d[123]), "+r"(d[124]),           \
+          "+r"(d[125]), "+r"(d[126]), "+r"(d[127])                                                                    \
+        : "l"(adesc), "l"(bdesc), "r"(accumulate))
+template <int KIND>
+__device__ __forceinline__ void wgmma_m64n256k32(int (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    if constexpr (KIND == FLAT_S8) FLAT_WGMMA_INT("s8");
+    else FLAT_WGMMA_INT("u8");
+}
+#undef FLAT_WGMMA_INT
+__device__ __forceinline__ void reg_fence(int& r) { asm volatile("" : "+r"(r)::"memory"); }
 // Per-query list of the FLAT_KC smallest keys: shared memory, [query row][FLAT_KC] with FLAT_KC odd, so that a warp
 // reading one row side by side is bank-conflict free.  Keys are stored as order-preserving unsigned integers
 // (REDUX.MAX works on them); a list starts full of +inf / no-id entries, so there is no fill count -- an update always
@@ -147,16 +220,47 @@ __device__ __forceinline__ float flat_list_replace_max(uint32_t* lkey, uint32_t*
     }
     return flat_unord(__reduce_max_sync(0xFFFFFFFFu, max(v0, v1)));
 }
+// Integer lists are ordered by the pair (key, id).  The whole warp offers (okey, id) to the list of row `list_row`: it
+// replaces the list's largest pair if it is below it.  Returns the ordered key of the new largest pair -- the row's
+// threshold, warp-uniform: a pair can only be below the largest pair if its key does not exceed that key.  Keys are
+// uint32(K) ^ 0x80000000; an empty entry is (0xFFFFFFFF, 0xFFFFFFFF), above every real pair.
+__device__ __forceinline__ uint64_t flat_pair_max(uint64_t v) {
+    const uint32_t hi = __reduce_max_sync(0xFFFFFFFFu, uint32_t(v >> 32));
+    const uint32_t lo = __reduce_max_sync(0xFFFFFFFFu, uint32_t(v >> 32) == hi ? uint32_t(v) : 0u);
+    return (uint64_t(hi) << 32) | lo;
+}
+__device__ __forceinline__ uint32_t flat_pair_offer(uint32_t* lkey, uint32_t* lid, uint32_t list_row, uint32_t lane,
+                                                    uint32_t okey, uint32_t id) {
+    uint32_t* rk = lkey + list_row * FLAT_KC;
+    uint32_t* ri = lid + list_row * FLAT_KC;
+    const bool has1 = lane + 32 < FLAT_KC;
+    uint64_t v0 = (uint64_t(rk[lane]) << 32) | ri[lane];
+    uint64_t v1 = has1 ? (uint64_t(rk[lane + 32]) << 32) | ri[lane + 32] : 0u;
+    const uint64_t mx = flat_pair_max(max(v0, v1));
+    const uint64_t nv = (uint64_t(okey) << 32) | id;
+    if (nv >= mx) return uint32_t(mx >> 32);   // an equal key with a larger id
+    const uint32_t in0 = __ballot_sync(0xFFFFFFFFu, v0 == mx);
+    const uint32_t in1 = __ballot_sync(0xFFFFFFFFu, v1 == mx && has1);
+    const uint32_t slot = in0 ? uint32_t(__ffs(int(in0)) - 1) : uint32_t(__ffs(int(in1)) + 31);
+    if (lane == (slot & 31u)) {
+        rk[slot] = okey;
+        ri[slot] = id;
+        if (slot < 32) v0 = nv; else v1 = nv;
+    }
+    return __reduce_max_sync(0xFFFFFFFFu, uint32_t(max(v0, v1) >> 32));
+}
 
 struct FlatParams {
     const __half* a_tiles;    // [mtiles][KB] blobs of FLAT_A_BYTES
     const __half* b_tiles;    // [ntiles][KB] blobs of FLAT_B_BYTES
     const float* b_bias;      // [ntiles * FLAT_BN]: |x~|^2 (L2) / 0 (inner product), +inf for padding rows
+                              // (integer kinds: int32 |x|^2 / 0, INT32_MAX for padding rows)
     uint32_t KB, ntiles, mtiles, nlists;
     uint32_t share;           // R: CTAs that walk the same base tiles at the same time, on R consecutive query tiles
     uint32_t* progress;       // [gridDim.x] tiles started by each CTA (zeroed before the launch)
-    float key_scale;          // key = bias + key_scale * s
+    float key_scale;          // key = bias + key_scale * s (-2 or -1)
     float* cand_key;          // [mtiles * FLAT_BM][nlists][FLAT_KC], pre-filled with (+inf, no id)
+                              // (integer kinds: ordered int32 keys, pre-filled with 0xFFFFFFFF)
     uint32_t* cand_id;
 };
 
@@ -182,7 +286,19 @@ constexpr uint32_t FLAT_CONSUMER_WARPS = 8, FLAT_THREADS = 32 * FLAT_CONSUMER_WA
 constexpr size_t kFlatSmem = size_t(FLAT_STAGES) * FLAT_STAGE_BYTES + 2 * 2 * size_t(FLAT_KC) * FLAT_BM * 4 + 128;
 static_assert(kFlatSmem <= 227 * 1024, "flat GEMM shared memory exceeds the 227 KB a block may use");
 
+// Ordered key of an empty list entry, and the threshold of an empty list.
+template <int KIND> __device__ __forceinline__ uint32_t flat_empty_key() {
+    if constexpr (KIND == FLAT_F16) return flat_ord(INFINITY);
+    else return 0xFFFFFFFFu;
+}
+template <int KIND> __device__ __forceinline__ auto flat_no_threshold() {
+    if constexpr (KIND == FLAT_F16) return INFINITY;
+    else return 0xFFFFFFFFu;
+}
+
+template <int KIND>
 __global__ void __launch_bounds__(FLAT_THREADS, 1) flat_gemm_topk_kernel(const __grid_constant__ FlatParams fp) {
+    using acc_t = std::conditional_t<KIND == FLAT_F16, float, int>;
     extern __shared__ __align__(1024) uint8_t smem[];
     uint8_t* stages = smem;
     uint32_t* lkey = reinterpret_cast<uint32_t*>(smem + size_t(FLAT_STAGES) * FLAT_STAGE_BYTES);   // [2][128][KC] ordered keys
@@ -267,14 +383,15 @@ __global__ void __launch_bounds__(FLAT_THREADS, 1) flat_gemm_topk_kernel(const _
     const uint32_t wg = warp >> 2;
     const uint32_t row0 = wg * 64 + (warp & 3u) * 16 + (lane >> 2);   // the thread's rows: row0, row0 + 8
     const uint32_t frow = wg * 64 + (warp & 3u) * 16 + (lane >> 1), fhalf = lane & 1u;   // the (row, half) list this lane clears / writes out
-    float d[128];
+    acc_t d[128];
 #pragma unroll
-    for (uint32_t i = 0; i < 128; ++i) d[i] = 0.f;
-    float thr[2][2];   // [row i][column half]: the largest key of that list
+    for (uint32_t i = 0; i < 128; ++i) d[i] = acc_t(0);
+    // [row i][column half]: the largest key of that list (integer kinds: the ordered key of its largest (key, id) pair)
+    std::conditional_t<KIND == FLAT_F16, float, uint32_t> thr[2][2];
 #pragma unroll
-    for (uint32_t i = 0; i < 4; ++i) thr[i >> 1][i & 1] = INFINITY;
+    for (uint32_t i = 0; i < 4; ++i) thr[i >> 1][i & 1] = flat_no_threshold<KIND>();
     for (uint32_t e = 0; e < FLAT_KC; ++e) {
-        lkey[(fhalf * FLAT_BM + frow) * FLAT_KC + e] = flat_ord(INFINITY);
+        lkey[(fhalf * FLAT_BM + frow) * FLAT_KC + e] = flat_empty_key<KIND>();
         lid[(fhalf * FLAT_BM + frow) * FLAT_KC + e] = 0xFFFFFFFFu;
     }
     __syncwarp();
@@ -287,8 +404,8 @@ __global__ void __launch_bounds__(FLAT_THREADS, 1) flat_gemm_topk_kernel(const _
             }
             continue;
         }
-        // ---- mainloop: one k-block per stage, two K=16 MMAs each; a stage is released once the MMAs of the next one
-        // have been issued and its own have completed ----
+        // ---- mainloop: one k-block per stage, two MMAs each (K = 16 fp16 / K = 32 8-bit elements); a stage is released
+        // once the MMAs of the next one have been issued and its own have completed ----
         uint32_t prev = 0;
         for (uint32_t kb = 0; kb < fp.KB; ++kb) {
             mbar_wait(full + s, ph);
@@ -297,10 +414,11 @@ __global__ void __launch_bounds__(FLAT_THREADS, 1) flat_gemm_topk_kernel(const _
             wgmma_fence();
 #pragma unroll
             for (uint32_t j = 0; j < FLAT_BK / 16; ++j) {
-                // k-chunks 2j and 2j+1 of the blob: [kc][rows/8][8][8] halves
+                // k-chunks 2j and 2j+1 of the blob: [kc][rows/8][8][16 bytes]
                 const uint64_t adesc = wgmma_desc(a_addr + 2 * j * (FLAT_BM * 16), FLAT_BM * 16, 128);
                 const uint64_t bdesc = wgmma_desc(b_addr + 2 * j * (FLAT_BN * 16), FLAT_BN * 16, 128);
-                wgmma_m64n256k16(d, adesc, bdesc, (kb | j) != 0 ? 1u : 0u);
+                if constexpr (KIND == FLAT_F16) wgmma_m64n256k16(d, adesc, bdesc, (kb | j) != 0 ? 1u : 0u);
+                else wgmma_m64n256k32<KIND>(d, adesc, bdesc, (kb | j) != 0 ? 1u : 0u);
             }
             wgmma_commit();
             wgmma_wait<1>();
@@ -318,35 +436,74 @@ __global__ void __launch_bounds__(FLAT_THREADS, 1) flat_gemm_topk_kernel(const _
 
         // ---- epilogue: keys of the thread's 128 elements; only columns whose keys beat a row's threshold (rare once
         // the lists have settled) are looked at key by key, the lanes with such a key served in turn by the whole warp ----
-        const float* bias = fp.b_bias + size_t(nt) * FLAT_BN + 2 * (lane & 3u);
+        if constexpr (KIND == FLAT_F16) {
+            const float* bias = fp.b_bias + size_t(nt) * FLAT_BN + 2 * (lane & 3u);
 #pragma unroll
-        for (uint32_t c = 0; c < FLAT_BN / 8; ++c) {
-            const uint32_t h = c / (FLAT_BN / 16);
-            const float2 b2 = __ldg(reinterpret_cast<const float2*>(bias + 8 * c));
-            float key[4];
-            key[0] = fmaf(fp.key_scale, d[4 * c + 0], b2.x);
-            key[1] = fmaf(fp.key_scale, d[4 * c + 1], b2.y);
-            key[2] = fmaf(fp.key_scale, d[4 * c + 2], b2.x);
-            key[3] = fmaf(fp.key_scale, d[4 * c + 3], b2.y);
-            const bool any = fminf(key[0], key[1]) < thr[0][h] || fminf(key[2], key[3]) < thr[1][h];
-            if (!__any_sync(0xFFFFFFFFu, any)) continue;
-            uint32_t* my_key = lkey + size_t(h) * FLAT_BM * FLAT_KC;
-            uint32_t* my_id = lid + size_t(h) * FLAT_BM * FLAT_KC;
+            for (uint32_t c = 0; c < FLAT_BN / 8; ++c) {
+                const uint32_t h = c / (FLAT_BN / 16);
+                const float2 b2 = __ldg(reinterpret_cast<const float2*>(bias + 8 * c));
+                float key[4];
+                key[0] = fmaf(fp.key_scale, d[4 * c + 0], b2.x);
+                key[1] = fmaf(fp.key_scale, d[4 * c + 1], b2.y);
+                key[2] = fmaf(fp.key_scale, d[4 * c + 2], b2.x);
+                key[3] = fmaf(fp.key_scale, d[4 * c + 3], b2.y);
+                const bool any = fminf(key[0], key[1]) < thr[0][h] || fminf(key[2], key[3]) < thr[1][h];
+                if (!__any_sync(0xFFFFFFFFu, any)) continue;
+                uint32_t* my_key = lkey + size_t(h) * FLAT_BM * FLAT_KC;
+                uint32_t* my_id = lid + size_t(h) * FLAT_BM * FLAT_KC;
 #pragma unroll
-            for (uint32_t v = 0; v < 4; ++v) {
-                const uint32_t i = v >> 1;
-                bool pending = key[v] < thr[i][h];
-                uint32_t hits = __ballot_sync(0xFFFFFFFFu, pending);
-                while (hits) {
-                    const uint32_t src = uint32_t(__ffs(int(hits)) - 1);
-                    const float k_src = __shfl_sync(0xFFFFFFFFu, key[v], src);
-                    const uint32_t id = nt * FLAT_BN + 8 * c + 2 * (src & 3u) + (v & 1u);
-                    const float tnew = flat_list_replace_max(my_key, my_id, row0 - (lane >> 2) + (src >> 2) + 8 * i, lane,
-                                                             k_src, id);
-                    if ((lane >> 2) == (src >> 2)) thr[i][h] = tnew;
-                    // another lane of the quad may hold a key of the same row that no longer beats the new threshold
-                    pending = pending && lane != src && key[v] < thr[i][h];
-                    hits = __ballot_sync(0xFFFFFFFFu, pending);
+                for (uint32_t v = 0; v < 4; ++v) {
+                    const uint32_t i = v >> 1;
+                    bool pending = key[v] < thr[i][h];
+                    uint32_t hits = __ballot_sync(0xFFFFFFFFu, pending);
+                    while (hits) {
+                        const uint32_t src = uint32_t(__ffs(int(hits)) - 1);
+                        const float k_src = __shfl_sync(0xFFFFFFFFu, key[v], src);
+                        const uint32_t id = nt * FLAT_BN + 8 * c + 2 * (src & 3u) + (v & 1u);
+                        const float tnew = flat_list_replace_max(my_key, my_id, row0 - (lane >> 2) + (src >> 2) + 8 * i, lane,
+                                                                 k_src, id);
+                        if ((lane >> 2) == (src >> 2)) thr[i][h] = tnew;
+                        // another lane of the quad may hold a key of the same row that no longer beats the new threshold
+                        pending = pending && lane != src && key[v] < thr[i][h];
+                        hits = __ballot_sync(0xFFFFFFFFu, pending);
+                    }
+                }
+            }
+        } else {
+            // exact int32 keys (wrapping arithmetic: the true key always fits), ordered as uint32; a column enters a list
+            // iff its (key, id) pair is below the list's largest pair.  Only the key of that pair is kept in registers:
+            // a column whose key equals it is offered, and the list compares the ids.  Padding rows (key INT32_MAX, above
+            // every real key) are never offered.
+            const uint32_t* bias = reinterpret_cast<const uint32_t*>(fp.b_bias) + size_t(nt) * FLAT_BN + 2 * (lane & 3u);
+            const uint32_t ks = uint32_t(int(fp.key_scale));
+#pragma unroll
+            for (uint32_t c = 0; c < FLAT_BN / 8; ++c) {
+                const uint32_t h = c / (FLAT_BN / 16);
+                const uint2 b2 = __ldg(reinterpret_cast<const uint2*>(bias + 8 * c));
+                uint32_t key[4];
+                key[0] = (b2.x + ks * uint32_t(d[4 * c + 0])) ^ 0x80000000u;
+                key[1] = (b2.y + ks * uint32_t(d[4 * c + 1])) ^ 0x80000000u;
+                key[2] = (b2.x + ks * uint32_t(d[4 * c + 2])) ^ 0x80000000u;
+                key[3] = (b2.y + ks * uint32_t(d[4 * c + 3])) ^ 0x80000000u;
+                const bool any = min(key[0], key[1]) <= thr[0][h] || min(key[2], key[3]) <= thr[1][h];
+                if (!__any_sync(0xFFFFFFFFu, any)) continue;
+                uint32_t* my_key = lkey + size_t(h) * FLAT_BM * FLAT_KC;
+                uint32_t* my_id = lid + size_t(h) * FLAT_BM * FLAT_KC;
+#pragma unroll
+                for (uint32_t v = 0; v < 4; ++v) {
+                    const uint32_t i = v >> 1;
+                    bool pending = key[v] != 0xFFFFFFFFu && key[v] <= thr[i][h];
+                    uint32_t hits = __ballot_sync(0xFFFFFFFFu, pending);
+                    while (hits) {
+                        const uint32_t src = uint32_t(__ffs(int(hits)) - 1);
+                        const uint32_t k_src = __shfl_sync(0xFFFFFFFFu, key[v], src);
+                        const uint32_t id = nt * FLAT_BN + 8 * c + 2 * (src & 3u) + (v & 1u);
+                        const uint32_t tnew = flat_pair_offer(my_key, my_id, row0 - (lane >> 2) + (src >> 2) + 8 * i, lane,
+                                                              k_src, id);
+                        if ((lane >> 2) == (src >> 2)) thr[i][h] = tnew;
+                        pending = pending && lane != src && key[v] <= thr[i][h];
+                        hits = __ballot_sync(0xFFFFFFFFu, pending);
+                    }
                 }
             }
         }
@@ -360,14 +517,15 @@ __global__ void __launch_bounds__(FLAT_THREADS, 1) flat_gemm_topk_kernel(const _
             uint32_t* ri = lid + (fhalf * FLAT_BM + frow) * FLAT_KC;
             __syncwarp();
             for (uint32_t e = 0; e < FLAT_KC; ++e) {
-                ok[e] = flat_unord(rk[e]);
+                if constexpr (KIND == FLAT_F16) ok[e] = flat_unord(rk[e]);
+                else reinterpret_cast<uint32_t*>(ok)[e] = rk[e];
                 oi[e] = ri[e];
-                rk[e] = flat_ord(INFINITY);
+                rk[e] = flat_empty_key<KIND>();
                 ri[e] = 0xFFFFFFFFu;
             }
             __syncwarp();
 #pragma unroll
-            for (uint32_t i = 0; i < 4; ++i) thr[i >> 1][i & 1] = INFINITY;
+            for (uint32_t i = 0; i < 4; ++i) thr[i >> 1][i & 1] = flat_no_threshold<KIND>();
             nt = 0;
             mtile += fp.share;
         }
@@ -391,10 +549,18 @@ __global__ void flat_tile_kernel(const char* __restrict__ src, uint32_t row_stri
     const char* row = src + size_t(r) * row_stride;
     const uint32_t t = r / TR, rr = r % TR;
     float sq_rounded = 0.f, sq_exact = 0.f;
+    int sq_int = 0;   // integer rows: |x|^2, exact
     for (uint32_t e = lane; e < dim; e += 32) {
         float x;
-        if constexpr (SRCT == SVSB200_F32) x = reinterpret_cast<const float*>(row)[e];
-        else x = __half2float(reinterpret_cast<const __half*>(row)[e]);
+        if constexpr (SRCT == SVSB200_F32) {
+            x = reinterpret_cast<const float*>(row)[e];
+        } else if constexpr (SRCT == SVSB200_F16) {
+            x = __half2float(reinterpret_cast<const __half*>(row)[e]);
+        } else {
+            const int v = SRCT == SVSB200_I8 ? int(reinterpret_cast<const int8_t*>(row)[e]) : int(reinterpret_cast<const uint8_t*>(row)[e]);
+            sq_int += v * v;
+            x = float(v);   // exact in fp16
+        }
         const __half h = __float2half_rn(x * scale);
         const float xr = __half2float(h) / scale;
         sq_rounded = fmaf(xr, xr, sq_rounded);
@@ -402,9 +568,14 @@ __global__ void flat_tile_kernel(const char* __restrict__ src, uint32_t row_stri
         const size_t o = ((size_t(t) * KB + e / 32) * 4 + (e % 32) / 8) * (size_t(TR) * 8) + (rr / 8) * 64 + (rr % 8) * 8 + e % 8;
         dst[o] = h;
     }
-    for (int o = 16; o; o >>= 1) {
-        sq_rounded += __shfl_xor_sync(0xFFFFFFFFu, sq_rounded, o);
-        sq_exact += __shfl_xor_sync(0xFFFFFFFFu, sq_exact, o);
+    if constexpr (SRCT == SVSB200_I8 || SRCT == SVSB200_U8) {
+        for (int o = 16; o; o >>= 1) sq_int += __shfl_xor_sync(0xFFFFFFFFu, sq_int, o);
+        sq_rounded = sq_exact = float(sq_int);   // one rounding, 2^-24 |x|^2 at most (E_l2 in the header)
+    } else {
+        for (int o = 16; o; o >>= 1) {
+            sq_rounded += __shfl_xor_sync(0xFFFFFFFFu, sq_rounded, o);
+            sq_exact += __shfl_xor_sync(0xFFFFFFFFu, sq_exact, o);
+        }
     }
     if (lane == 0) {
         if (bias) bias[r] = l2 ? sq_rounded : 0.f;
@@ -412,6 +583,34 @@ __global__ void flat_tile_kernel(const char* __restrict__ src, uint32_t row_stri
         if (norms) norms[r] = nrm;
         if (max_norm_bits) atomicMax(max_norm_bits, __float_as_uint(nrm));
     }
+}
+
+// ---- operand tiling, 8-bit: int8 / uint8 rows -> blobs of their raw codes, 64-element k-blocks --------------------
+// element (row r, k e) of tile t = r / TR lives at  ((t*KB + e/64) * 4 + (e%64)/16) * TR*16 + ((r%TR)/8)*128 + (r%8)*16 + e%16
+// (a blob is as many bytes as an fp16 blob); zero padding adds nothing to any integer sum.  bias: |x|^2 (L2) / 0,
+// INT32_MAX for padding rows (above every real key, so they never enter a list).
+template <int SRCT>
+__global__ void flat_tile8_kernel(const char* __restrict__ src, uint32_t row_stride, uint32_t n, uint32_t dim, uint32_t TR,
+                                  uint32_t KB, int l2, uint8_t* __restrict__ dst, int* __restrict__ bias) {
+    const uint32_t r = blockIdx.x * (blockDim.x / 32) + threadIdx.x / 32;
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t rows_padded = (n + TR - 1) / TR * TR;
+    if (r >= rows_padded) return;
+    if (r >= n) {
+        if (bias && lane == 0) bias[r] = INT_MAX;
+        return;
+    }
+    const uint8_t* row = reinterpret_cast<const uint8_t*>(src + size_t(r) * row_stride);
+    const uint32_t t = r / TR, rr = r % TR;
+    int sq = 0;
+    for (uint32_t e = lane; e < dim; e += 32) {
+        const uint8_t c = row[e];
+        const int v = SRCT == SVSB200_I8 ? int(int8_t(c)) : int(c);
+        sq += v * v;
+        dst[((size_t(t) * KB + e / 64) * 4 + (e % 64) / 16) * (size_t(TR) * 16) + (rr / 8) * 128 + (rr % 8) * 16 + e % 16] = c;
+    }
+    for (int o = 16; o; o >>= 1) sq += __shfl_xor_sync(0xFFFFFFFFu, sq, o);
+    if (bias && lane == 0) bias[r] = l2 ? sq : 0;
 }
 
 // ---- exact re-scoring + verification: one warp per query ----------------------------------------------------------
@@ -427,32 +626,56 @@ struct RescoreParams {
     uint32_t* n_unverified;
     float ksign;
     int data_rounded;         // the base vectors were float32 (rounded to fp16 for the GEMM)
+    int data_int;             // the base vectors are int8 / uint8 (exact in fp16; the bias |x|^2 is rounded once)
 };
+
+// Shared memory of the rescoring kernel: the staged query, then candidate ids, approximate and exact keys.
+template <int OP> __host__ __device__ inline size_t flat_rescore_qbytes(uint32_t qstride) {
+    return OP >= OP_L2I ? qstride : size_t(qstride) * 4;   // (qstride is a multiple of 16)
+}
+template <int OP> inline size_t flat_rescore_smem(uint32_t qstride) {
+    return flat_rescore_qbytes<OP>(qstride) + size_t(FLAT_CMAX) * 4 * 3;
+}
+constexpr size_t kFlatRescoreSmemMax = 227 * 1024;   // what a block may opt in to on sm_90
 
 template <int ROWT, int OP>
 __global__ void __launch_bounds__(32, 16) flat_rescore_kernel(const __grid_constant__ SearchParams p,
                                                              const __grid_constant__ RescoreParams rp) {
-    constexpr int G = 16 / Row<ROWT>::LPT;
+    constexpr bool kInt = (OP >= OP_L2I);   // the integer GEMM's candidates: exact keys, (key, id) lists
+    constexpr int G = kInt ? 4 : 16 / Row<ROWT>::LPT;
     constexpr int GROUPS = 32 / G;
+    // rows per group and pass: two, but one for integer rows under the float operators (no spills in 128 registers)
+    constexpr int NR = (ROWT == SVSB200_I8 || ROWT == SVSB200_U8) && !kInt ? 1 : 2;
     constexpr unsigned FULL = 0xFFFFFFFFu;
     constexpr uint32_t CMAX = FLAT_CMAX;
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    float* q_s = reinterpret_cast<float*>(smem_raw);
-    uint32_t* cid = reinterpret_cast<uint32_t*>(q_s + p.qstride);   // [CMAX]
-    float* akey = reinterpret_cast<float*>(cid + CMAX);               // [CMAX] approximate keys
+    float* q_s = reinterpret_cast<float*>(smem_raw);                   // qstride floats (integer: qstride codes)
+    uint32_t* cid = reinterpret_cast<uint32_t*>(smem_raw + flat_rescore_qbytes<OP>(p.qstride));   // [CMAX]
+    float* akey = reinterpret_cast<float*>(cid + CMAX);               // [CMAX] approximate keys (integer: ordered keys)
     float* ekey = akey + CMAX;                                        // [CMAX] exact keys
     const int lane = threadIdx.x;
     const int g = lane / G, t = lane % G;
     const uint32_t q = blockIdx.x;
     if (q >= rp.nq) return;
     const uint32_t total = rp.nsplit * FLAT_KC;
+    const uint32_t* okey = reinterpret_cast<const uint32_t*>(rp.cand_key);
     // candidates of every base range; T = the smallest per-range list maximum (every excluded row is >= it)
     float T = INFINITY;
+    uint64_t Tp = ~uint64_t(0);   // integer: the smallest list-maximum (key, id) pair
     for (uint32_t s = 0; s < rp.nsplit; ++s) {
-        float mx = -INFINITY;
-        for (uint32_t e = lane; e < FLAT_KC; e += 32) mx = fmaxf(mx, rp.cand_key[(size_t(q) * rp.nsplit + s) * FLAT_KC + e]);
-        for (int o = 16; o; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(FULL, mx, o));
-        T = fminf(T, mx);
+        if constexpr (kInt) {
+            uint64_t mx = 0;
+            for (uint32_t e = lane; e < FLAT_KC; e += 32) {
+                const size_t o = (size_t(q) * rp.nsplit + s) * FLAT_KC + e;
+                mx = max(mx, (uint64_t(okey[o]) << 32) | rp.cand_id[o]);
+            }
+            Tp = min(Tp, flat_pair_max(mx));
+        } else {
+            float mx = -INFINITY;
+            for (uint32_t e = lane; e < FLAT_KC; e += 32) mx = fmaxf(mx, rp.cand_key[(size_t(q) * rp.nsplit + s) * FLAT_KC + e]);
+            for (int o = 16; o; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(FULL, mx, o));
+            T = fminf(T, mx);
+        }
     }
     uint32_t C = 0;   // valid candidates, compacted
     for (uint32_t i0 = 0; i0 < total; i0 += 32) {
@@ -463,18 +686,58 @@ __global__ void __launch_bounds__(32, 16) flat_rescore_kernel(const __grid_const
         if (ok) {
             const uint32_t o = C + __popc(m & ((1u << lane) - 1u));
             cid[o] = id;
-            akey[o] = rp.cand_key[size_t(q) * total + i];
+            if constexpr (kInt) reinterpret_cast<uint32_t*>(akey)[o] = okey[size_t(q) * total + i];
+            else akey[o] = rp.cand_key[size_t(q) * total + i];
         }
         C += __popc(m);
     }
     __syncwarp();
-    for (uint32_t i = lane; i < p.qstride; i += 32) q_s[i] = p.qf[size_t(q) * p.qstride + i];
+    if constexpr (kInt) {
+        const uint32_t* src = reinterpret_cast<const uint32_t*>(p.qcodes + size_t(q) * p.qstride);
+        for (uint32_t i = lane; i < p.qstride / 4; i += 32) reinterpret_cast<uint32_t*>(q_s)[i] = src[i];
+    } else {
+        for (uint32_t i = lane; i < p.qstride; i += 32) q_s[i] = p.qf[size_t(q) * p.qstride + i];
+    }
     __syncwarp();
     const float aux0 = p.qaux[2 * size_t(q)], aux1 = p.qaux[2 * size_t(q) + 1];
-    for (uint32_t base = 0; base < C; base += 2 * GROUPS)
-        eval_pass<ROWT, OP, 0, 2, 1, true>(p, q_s, reinterpret_cast<const char*>(p.vectors), cid, ekey, base, C, g, t, aux0, aux1,
+    for (uint32_t base = 0; base < C; base += NR * GROUPS)
+        eval_pass<ROWT, OP, 0, NR, 1, true>(p, q_s, reinterpret_cast<const char*>(p.vectors), cid, ekey, base, C, g, t, aux0, aux1,
                                            rp.ksign);
     __syncwarp();
+    if constexpr (kInt) {
+        // rank of every candidate by (exact key, id); F(K) = float(v(K)), v(K) = |q|^2 + K (L2) or K (header)
+        const int64_t qq = OP == OP_L2I ? int64_t(__float_as_int(aux1)) : 0;
+        bool mismatch = false;
+        float kth_key = -INFINITY;
+        uint64_t kth_pair = 0;
+        for (uint32_t i = lane; i < C; i += 32) {
+            const float ke = ekey[i];
+            const uint32_t id = cid[i], ok_i = reinterpret_cast<const uint32_t*>(akey)[i];
+            uint32_t re = 0;
+            for (uint32_t j = 0; j < C; ++j) {
+                const float kj = ekey[j];
+                re += (kj < ke) || (kj == ke && cid[j] < id);
+            }
+            if (re < rp.k) {
+                rp.out_ids[size_t(q) * rp.k + re] = id;
+                rp.out_dists[size_t(q) * rp.k + re] = ke * rp.ksign;
+            }
+            // the GEMM's key must give the rescored distance
+            mismatch |= __ll2float_rn(qq + int32_t(ok_i ^ 0x80000000u)) != ke;
+            if (re == rp.k - 1) {
+                kth_key = ke;
+                kth_pair = (uint64_t(ok_i) << 32) | id;
+            }
+        }
+        mismatch = __any_sync(FULL, mismatch);
+        for (int o = 16; o; o >>= 1) kth_key = fmaxf(kth_key, __shfl_xor_sync(FULL, kth_key, o));
+        kth_pair = flat_pair_max(kth_pair);
+        const int64_t vT = qq + int32_t(uint32_t(Tp >> 32) ^ 0x80000000u);
+        const bool exact_at_T = vT < (int64_t(1) << 24) && vT > -(int64_t(1) << 24);
+        const bool verified = C >= rp.k && !mismatch && (__ll2float_rn(vT) > kth_key || (exact_at_T && Tp > kth_pair));
+        if (lane == 0 && !verified) rp.unverified[atomicAdd(rp.n_unverified, 1u)] = q;
+        return;
+    }
     // rank of every candidate by (exact key, id) and by approximate key: k is small, C <= 512
     float kth_approx = INFINITY;
     for (uint32_t i = lane; i < C; i += 32) {
@@ -498,7 +761,10 @@ __global__ void __launch_bounds__(32, 16) flat_rescore_kernel(const __grid_const
     const float qn = rp.qnorm[q], xm = __uint_as_float(*rp.xmax_bits);
     const float rounded = p.scale;   // operands that were rounded to fp16 (0, 1 or 2)
     const float e_ip = (rounded * 4.8828125e-4f + float(p.dim) * 2.384185791015625e-7f) * qn * xm * 1.0001f;   // 2^-11 each, dim 2^-22
-    const float E = p.greater ? e_ip : 2.0f * e_ip + (rounded > 1.5f || rp.data_rounded ? 9.765625e-4f * xm * xm : 0.0f);
+    const float E = p.greater ? e_ip
+                              : 2.0f * e_ip + (rounded > 1.5f || rp.data_rounded ? 9.765625e-4f * xm * xm
+                                               : rp.data_int                      ? 1.1920929e-7f * xm * xm   // 2^-23 (header)
+                                                                                  : 0.0f);
     const bool verified = C >= rp.k && T > kth_approx + 2.0f * E;
     if (lane == 0 && !verified) rp.unverified[atomicAdd(rp.n_unverified, 1u)] = q;
 }
@@ -523,19 +789,35 @@ static cudaError_t flat_tile_rows(int srct, const void* src, uint32_t row_stride
     cudaError_t err = cudaMemsetAsync(dst_tiles, 0, size_t(rows_padded) * KB * FLAT_BK * 2, stream);
     if (err != cudaSuccess) return err;
     const unsigned grid = (rows_padded + 7) / 8;
-    if (srct == SVSB200_F32)
-        flat_tile_kernel<SVSB200_F32><<<grid, 256, 0, stream>>>(static_cast<const char*>(src), row_stride, n, dim, tile_rows, KB, scale,
-                                                               l2, static_cast<__half*>(dst_tiles), bias, norms, max_norm_bits);
-    else
-        flat_tile_kernel<SVSB200_F16><<<grid, 256, 0, stream>>>(static_cast<const char*>(src), row_stride, n, dim, tile_rows, KB, scale,
-                                                               l2, static_cast<__half*>(dst_tiles), bias, norms, max_norm_bits);
+    auto kernel = srct == SVSB200_F32 ? flat_tile_kernel<SVSB200_F32>
+                  : srct == SVSB200_F16 ? flat_tile_kernel<SVSB200_F16>
+                  : srct == SVSB200_I8  ? flat_tile_kernel<SVSB200_I8>
+                                        : flat_tile_kernel<SVSB200_U8>;
+    kernel<<<grid, 256, 0, stream>>>(static_cast<const char*>(src), row_stride, n, dim, tile_rows, KB, scale, l2,
+                                     static_cast<__half*>(dst_tiles), bias, norms, max_norm_bits);
     count_launch();
     return cudaGetLastError();
 }
 
-__global__ void flat_fill_kernel(float* __restrict__ key, uint32_t* __restrict__ id, size_t count) {
+// int8 / uint8 rows -> 8-bit blobs (flat_tile8_kernel); `bias` may be NULL (query tiles).
+static cudaError_t flat_tile_rows8(int srct, const void* src, uint32_t row_stride, uint32_t n, uint32_t dim, uint32_t tile_rows,
+                                   int l2, void* dst_tiles, int* bias, cudaStream_t stream) {
+    const uint32_t KB = (dim + FLAT_BK8 - 1) / FLAT_BK8;
+    const uint32_t rows_padded = (n + tile_rows - 1) / tile_rows * tile_rows;
+    cudaError_t err = cudaMemsetAsync(dst_tiles, 0, size_t(rows_padded) * KB * FLAT_BK8, stream);
+    if (err != cudaSuccess) return err;
+    const unsigned grid = (rows_padded + 7) / 8;
+    auto kernel = srct == SVSB200_I8 ? flat_tile8_kernel<SVSB200_I8> : flat_tile8_kernel<SVSB200_U8>;
+    kernel<<<grid, 256, 0, stream>>>(static_cast<const char*>(src), row_stride, n, dim, tile_rows, KB, l2,
+                                     static_cast<uint8_t*>(dst_tiles), bias);
+    count_launch();
+    return cudaGetLastError();
+}
+
+// Lists of absent pieces: (empty key, no id).  `key_bits`: +inf (fp16 lists) or 0xFFFFFFFF (integer lists).
+__global__ void flat_fill_kernel(uint32_t* __restrict__ key, uint32_t key_bits, uint32_t* __restrict__ id, size_t count) {
     for (size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x; i < count; i += size_t(gridDim.x) * blockDim.x) {
-        key[i] = INFINITY;
+        key[i] = key_bits;
         id[i] = 0xFFFFFFFFu;
     }
 }
@@ -562,13 +844,13 @@ static void flat_plan(uint32_t mtiles, uint32_t ntiles, uint32_t sm_count, uint3
     }
 }
 
-static cudaError_t flat_gemm_topk(const void* a_tiles, const void* b_tiles, const float* b_bias, uint32_t KB, uint32_t ntiles,
+static cudaError_t flat_gemm_topk(int kind, const void* a_tiles, const void* b_tiles, const void* b_bias, uint32_t KB, uint32_t ntiles,
                                   uint32_t mtiles, uint32_t ctas, uint32_t share, uint32_t nlists, float key_scale, float* cand_key,
                                   uint32_t* cand_id, uint32_t* progress, cudaStream_t stream) {
     FlatParams fp{};
     fp.a_tiles = static_cast<const __half*>(a_tiles);
     fp.b_tiles = static_cast<const __half*>(b_tiles);
-    fp.b_bias = b_bias;
+    fp.b_bias = static_cast<const float*>(b_bias);
     fp.KB = KB;
     fp.ntiles = ntiles;
     fp.mtiles = mtiles;
@@ -578,23 +860,40 @@ static cudaError_t flat_gemm_topk(const void* a_tiles, const void* b_tiles, cons
     fp.key_scale = key_scale;
     fp.cand_key = cand_key;
     fp.cand_id = cand_id;
-    cudaError_t err = cudaFuncSetAttribute(flat_gemm_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(kFlatSmem));
+    auto kernel = kind == FLAT_S8 ? flat_gemm_topk_kernel<FLAT_S8>
+                  : kind == FLAT_U8 ? flat_gemm_topk_kernel<FLAT_U8>
+                                    : flat_gemm_topk_kernel<FLAT_F16>;
+    cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(kFlatSmem));
     if (err != cudaSuccess) return err;
     const size_t entries = size_t(mtiles) * FLAT_BM * nlists * FLAT_KC;
-    flat_fill_kernel<<<unsigned(std::min<size_t>(4096, (entries + 255) / 256)), 256, 0, stream>>>(cand_key, cand_id, entries);
+    const uint32_t empty_key = kind == FLAT_F16 ? 0x7F800000u : 0xFFFFFFFFu;
+    flat_fill_kernel<<<unsigned(std::min<size_t>(4096, (entries + 255) / 256)), 256, 0, stream>>>(
+        reinterpret_cast<uint32_t*>(cand_key), empty_key, cand_id, entries);
     count_launch();
-    flat_gemm_topk_kernel<<<ctas, FLAT_THREADS, kFlatSmem, stream>>>(fp);
+    kernel<<<ctas, FLAT_THREADS, kFlatSmem, stream>>>(fp);
     count_launch();
     return cudaGetLastError();
 }
 
-template <int ROWT> static cudaError_t rescore_rowt(int op, const SearchParams& p, const RescoreParams& rp, cudaStream_t stream) {
-    const size_t smem = size_t(p.qstride) * 4 + size_t(FLAT_CMAX) * 4 * 3;
-    if (op == OP_L2F) flat_rescore_kernel<ROWT, OP_L2F><<<rp.nq, 32, smem, stream>>>(p, rp);
-    else if (op == OP_IPF) flat_rescore_kernel<ROWT, OP_IPF><<<rp.nq, 32, smem, stream>>>(p, rp);
-    else return cudaErrorInvalidValue;
+// Rows wider than about 9 000 elements need more than the default 48 KB of shared memory: the kernel opts in.
+template <int ROWT, int OP> static cudaError_t rescore_launch(const SearchParams& p, const RescoreParams& rp, cudaStream_t stream) {
+    const size_t smem = flat_rescore_smem<OP>(p.qstride);
+    if (smem > 48 * 1024) {
+        cudaError_t err = cudaFuncSetAttribute(flat_rescore_kernel<ROWT, OP>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
+        if (err != cudaSuccess) return err;
+    }
+    flat_rescore_kernel<ROWT, OP><<<rp.nq, 32, smem, stream>>>(p, rp);
     count_launch();
     return cudaGetLastError();
+}
+template <int ROWT> static cudaError_t rescore_rowt(int op, const SearchParams& p, const RescoreParams& rp, cudaStream_t stream) {
+    if (op == OP_L2F) return rescore_launch<ROWT, OP_L2F>(p, rp, stream);
+    if (op == OP_IPF) return rescore_launch<ROWT, OP_IPF>(p, rp, stream);
+    if constexpr (ROWT == SVSB200_I8 || ROWT == SVSB200_U8) {
+        if (op == OP_L2I) return rescore_launch<ROWT, OP_L2I>(p, rp, stream);
+        if (op == OP_IPI) return rescore_launch<ROWT, OP_IPI>(p, rp, stream);
+    }
+    return cudaErrorInvalidValue;
 }
 
 static cudaError_t flat_rescore(int rowt, int op, const SearchParams& p, const float* cand_key, const uint32_t* cand_id, uint32_t nsplit,
@@ -615,7 +914,13 @@ static cudaError_t flat_rescore(int rowt, int op, const SearchParams& p, const f
     rp.n_unverified = n_unverified;
     rp.ksign = p.greater ? -1.0f : 1.0f;
     rp.data_rounded = rowt == SVSB200_F32;
-    return rowt == SVSB200_F32 ? rescore_rowt<SVSB200_F32>(op, p, rp, stream) : rescore_rowt<SVSB200_F16>(op, p, rp, stream);
+    rp.data_int = rowt == SVSB200_I8 || rowt == SVSB200_U8;
+    switch (rowt) {
+        case SVSB200_F32: return rescore_rowt<SVSB200_F32>(op, p, rp, stream);
+        case SVSB200_F16: return rescore_rowt<SVSB200_F16>(op, p, rp, stream);
+        case SVSB200_I8: return rescore_rowt<SVSB200_I8>(op, p, rp, stream);
+        default: return rescore_rowt<SVSB200_U8>(op, p, rp, stream);
+    }
 }
 
 static cudaError_t flat_move_rows(const void* src, void* dst, const uint32_t* idx, const uint32_t* count, uint32_t max_count,
@@ -634,19 +939,34 @@ static int flat_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, const vo
     if (fallback_queries) *fallback_queries = 0;
     if (nq == 0) return 0;
     cudaStream_t stream = sc->stream;
-    const bool gemm_ok = ix->storage == SVSB200_PLAIN && (ix->dtype == SVSB200_F32 || ix->dtype == SVSB200_F16) &&
-                         ix->metric != SVSB200_COSINE && (qdtype == SVSB200_F32 || qdtype == SVSB200_F16) &&
-                         k + 8 <= FLAT_KC && ix->n >= 512;
-    if (!gemm_ok) {   // shapes outside the GEMM path: the exact scan
+    const bool int_data = ix->dtype == SVSB200_I8 || ix->dtype == SVSB200_U8;
+    const bool shape_ok = ix->storage == SVSB200_PLAIN && ix->metric != SVSB200_COSINE && k + 8 <= FLAT_KC && ix->n >= 512;
+    // the integer GEMM: (int8, int8) / (uint8, uint8), every int32 sum exact
+    const bool int_gemm = shape_ok && int_data && qdtype == ix->dtype && ix->dim <= FLAT_INT_MAX_DIM &&
+                          flat_rescore_smem<OP_L2I>(query_stride(ix->dim)) <= kFlatRescoreSmemMax;
+    // the fp16 GEMM: float32 / float16 data with float32 / float16 queries, integer data with float32 queries; rows
+    // whose staged float query does not fit the rescoring kernel's shared memory keep the scan
+    const bool f16_gemm = shape_ok && (int_data ? qdtype == SVSB200_F32 : (qdtype == SVSB200_F32 || qdtype == SVSB200_F16)) &&
+                          flat_rescore_smem<OP_L2F>(query_stride(ix->dim)) <= kFlatRescoreSmemMax;
+    if (!int_gemm && !f16_gemm) {   // shapes outside the GEMM paths: the exact scan
         if (fallback_queries) *fallback_queries = uint32_t(nq);
         return search_on_device(ix, rep, sc, d_queries, qdtype, nq, k, k, k, d_out_ids, 8, d_out_dists, stream, true);
     }
     const uint32_t n = uint32_t(ix->n), dim = uint32_t(ix->dim);
-    const uint32_t KB = (dim + 31) / 32, ntiles = (n + 255) / 256, mtiles = uint32_t((nq + 127) / 128);
+    // k-blocks per row; a blob holds FLAT_BK fp16 or FLAT_BK8 8-bit elements, FLAT_BK * 2 bytes of a row either way
+    const uint32_t KB = int_gemm ? (dim + FLAT_BK8 - 1) / FLAT_BK8 : (dim + 31) / 32;
+    const uint32_t ntiles = (n + 255) / 256, mtiles = uint32_t((nq + 127) / 128);
     const int l2 = ix->metric == SVSB200_L2;
-    {   // base tiles, once per replica
+    {   // base tiles, once per replica and kind
         std::lock_guard<std::mutex> lock(rep->mu);
-        if (!rep->flat_b.ptr) {
+        if (int_gemm && !rep->flat_b8.ptr) {
+            CUDA_TRY(rep->flat_b8.ensure(size_t(ntiles) * 256 * KB * FLAT_BK8));
+            CUDA_TRY(rep->flat_bias8.ensure(size_t(ntiles) * 256));
+            CUDA_TRY(flat_tile_rows8(ix->dtype, rep->d_vectors.ptr, ix->row_stride, n, dim, 256, l2, rep->flat_b8.ptr,
+                                     rep->flat_bias8.ptr, stream));
+            CUDA_TRY(cudaStreamSynchronize(stream));
+        }
+        if (!int_gemm && !rep->flat_b.ptr) {
             CUDA_TRY(rep->flat_b.ensure(size_t(ntiles) * 256 * KB * 32 * 2));
             CUDA_TRY(rep->flat_bias.ensure(size_t(ntiles) * 256));
             CUDA_TRY(rep->flat_xmax.ensure(1));
@@ -667,12 +987,19 @@ static int flat_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, const vo
     CUDA_TRY(sc->flat_unv.ensure(nq + 1));
     CUDA_TRY(sc->flat_progress.ensure(flat_ctas));
     CUDA_TRY(cudaMemsetAsync(sc->flat_progress.ptr, 0, size_t(flat_ctas) * 4, stream));
-    CUDA_TRY(flat_tile_rows(qdtype, d_queries, uint32_t(qrow), uint32_t(nq), dim, 128, 1.0f, 0, sc->flat_a.ptr, nullptr,
-                            sc->flat_qnorm.ptr, nullptr, stream));
-    CUDA_TRY(flat_gemm_topk(sc->flat_a.ptr, rep->flat_b.ptr, rep->flat_bias.ptr, KB, ntiles, mtiles, flat_ctas, flat_share, nsplit,
-                            l2 ? -2.0f : -1.0f, sc->flat_ckey.ptr, sc->flat_cid.ptr, sc->flat_progress.ptr, stream));
+    if (int_gemm) {
+        CUDA_TRY(flat_tile_rows8(qdtype, d_queries, uint32_t(qrow), uint32_t(nq), dim, 128, 0, sc->flat_a.ptr, nullptr, stream));
+        CUDA_TRY(flat_gemm_topk(ix->dtype == SVSB200_I8 ? FLAT_S8 : FLAT_U8, sc->flat_a.ptr, rep->flat_b8.ptr, rep->flat_bias8.ptr, KB,
+                                ntiles, mtiles, flat_ctas, flat_share, nsplit, l2 ? -2.0f : -1.0f, sc->flat_ckey.ptr, sc->flat_cid.ptr,
+                                sc->flat_progress.ptr, stream));
+    } else {
+        CUDA_TRY(flat_tile_rows(qdtype, d_queries, uint32_t(qrow), uint32_t(nq), dim, 128, 1.0f, 0, sc->flat_a.ptr, nullptr,
+                                sc->flat_qnorm.ptr, nullptr, stream));
+        CUDA_TRY(flat_gemm_topk(FLAT_F16, sc->flat_a.ptr, rep->flat_b.ptr, rep->flat_bias.ptr, KB, ntiles, mtiles, flat_ctas, flat_share,
+                                nsplit, l2 ? -2.0f : -1.0f, sc->flat_ckey.ptr, sc->flat_cid.ptr, sc->flat_progress.ptr, stream));
+    }
     // exact re-scoring with the search path's distance code: prepared queries as for a search
-    if (int rc = prepare_queries(ix, rep, sc, d_queries, qdtype, nq, PREP_FLOAT, stream)) return rc;
+    if (int rc = prepare_queries(ix, rep, sc, d_queries, qdtype, nq, int_gemm ? PREP_INT : PREP_FLOAT, stream)) return rc;
     SearchParams p{};
     p.vectors = rep->d_vectors.ptr;
     p.n = n;
@@ -680,14 +1007,16 @@ static int flat_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, const vo
     p.row_stride = ix->row_stride;
     p.greater = !l2;
     p.qf = sc->q_f32.ptr;
+    p.qcodes = sc->q_codes.ptr;
     p.qaux = sc->q_aux.ptr;
     p.qstride = query_stride(dim);
     p.nq = uint32_t(nq);
     p.k = uint32_t(k);
     CUDA_TRY(cudaMemsetAsync(sc->flat_unv.ptr, 0, 4, stream));
-    // rounding terms of E(q) (file header): the query is always rounded to fp16, float32 data too
+    // rounding terms of E(q) (file header, fp16 path): float32 queries and float32 data are rounded to fp16
     p.scale = (qdtype == SVSB200_F32 ? 1.0f : 0.0f) + (ix->dtype == SVSB200_F32 ? 1.0f : 0.0f);   // number of rounded operands
-    CUDA_TRY(flat_rescore(ix->dtype, l2 ? OP_L2F : OP_IPF, p, sc->flat_ckey.ptr, sc->flat_cid.ptr, nsplit, uint32_t(nq), uint32_t(k),
+    const int op = int_gemm ? (l2 ? OP_L2I : OP_IPI) : (l2 ? OP_L2F : OP_IPF);
+    CUDA_TRY(flat_rescore(ix->dtype, op, p, sc->flat_ckey.ptr, sc->flat_cid.ptr, nsplit, uint32_t(nq), uint32_t(k),
                           sc->flat_qnorm.ptr, rep->flat_xmax.ptr, d_out_ids, d_out_dists, sc->flat_unv.ptr + 1, sc->flat_unv.ptr, stream));
     // queries whose bound did not verify: exact scan, results scattered over the rescored rows
     uint32_t nunv = 0;

@@ -155,6 +155,10 @@ struct Replica {
     DeviceBuffer<unsigned char> flat_b;
     DeviceBuffer<float> flat_bias;
     DeviceBuffer<unsigned int> flat_xmax;
+    // ... and int8 / uint8 base vectors as 8-bit tiles for the integer GEMM + int32 bias (kept apart: one index can be
+    // searched with integer queries and with float32 queries)
+    DeviceBuffer<unsigned char> flat_b8;
+    DeviceBuffer<int> flat_bias8;
     std::mutex mu;
     std::vector<Scratch*> idle;                      // pool for the blocking API
     std::map<cudaStream_t, Scratch*> by_stream;      // one per caller stream for the enqueue-only API
