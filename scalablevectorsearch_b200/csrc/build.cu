@@ -178,17 +178,6 @@ __global__ void batch_codes_kernel(const char* __restrict__ vectors, uint32_t ro
     }
 }
 
-// f(std::integral_constant<int, T>{}) for the builder's element type T = dtype.
-template <typename F> static cudaError_t with_rowt(int dtype, F&& f) {
-    switch (dtype) {
-        case SVSB200_F32: return f(std::integral_constant<int, SVSB200_F32>{});
-        case SVSB200_F16: return f(std::integral_constant<int, SVSB200_F16>{});
-        case SVSB200_I8: return f(std::integral_constant<int, SVSB200_I8>{});
-        case SVSB200_U8: return f(std::integral_constant<int, SVSB200_U8>{});
-        default: return cudaErrorInvalidValue;
-    }
-}
-
 static bool int_dtype(int dtype) { return dtype == SVSB200_I8 || dtype == SVSB200_U8; }
 
 __global__ void fill_u32_kernel(uint32_t* p, size_t n, uint32_t v) {
@@ -225,7 +214,7 @@ int medoid(const GraphBuild& b, const uint8_t* d_status, size_t count, uint32_t*
     CUDA_TRY(cudaMemsetAsync(d_sums.ptr, 0, dim * 8, b.stream));
     const char* v = static_cast<const char*>(b.vectors);
     const int narrow = d_status ? 1 : 0;
-    CUDA_TRY(with_rowt(b.dtype, [&](auto t) {
+    CUDA_TRY(dispatch(DataRows{}, b.dtype, [&](auto t) {
         constexpr int T = decltype(t)::value;
         column_sum_kernel<T><<<unsigned((n + 255) / 256), 128, 0, b.stream>>>(v, uint32_t(n), uint32_t(dim), b.row_stride, d_status, d_sums.ptr);
         medoid_distance_kernel<T><<<nblk, 256, 0, b.stream>>>(v, uint32_t(n), uint32_t(dim), b.row_stride, d_status, double(count), narrow, d_sums.ptr, d_best_d.ptr, d_best_i.ptr);
@@ -281,7 +270,7 @@ static int build_search_config(const char* who, const GraphBuild& b, SearchParam
     cfg->smem_bytes = fast_smem_bytes(p->qstride, p->cap_pad, p->deg_pad, lean.slots * 2u);
     cfg->stream = b.stream;
     cfg->grid = -b.sm_count;
-    if (cfg->smem_bytes > 227 * 1024) return fail(std::string(who) + ": window_size too large for shared memory");
+    if (cfg->smem_bytes > kSmemOptInMax) return fail(std::string(who) + ": window_size too large for shared memory");
     return 0;
 }
 
@@ -365,7 +354,7 @@ int construct_graph(const char* who, const GraphBuild& b, float reverse_alpha, u
         if (stop == start) continue;
         const uint32_t B = uint32_t(stop - start);
         // 1. generate_neighbors: search ...
-        CUDA_TRY(with_rowt(dtype, [&](auto t) {
+        CUDA_TRY(dispatch(DataRows{}, dtype, [&](auto t) {
             constexpr int T = decltype(t)::value;
             if constexpr (T == SVSB200_I8 || T == SVSB200_U8)
                 batch_codes_kernel<T><<<(B + 7) / 8, 256, 0, stream>>>(vectors, row_stride, uint32_t(b.dim), qstride, uint32_t(start), B, d_slots, d_qcodes.ptr, d_qaux.ptr);
@@ -376,7 +365,7 @@ int construct_graph(const char* who, const GraphBuild& b, float reverse_alpha, u
         count_launch();
         CUDA_TRY(cudaMemsetAsync(d_work.ptr, 0, 4, stream));
         p.nq = B;
-        CUDA_TRY(with_rowt(dtype, [&](auto t) { return launch_build_search<decltype(t)::value>(op, p, cfg); }));
+        CUDA_TRY(dispatch(DataRows{}, dtype, [&](auto t) { return launch_build_search<decltype(t)::value>(op, p, cfg); }));
         // ... pool + prune (always with the configured alpha, vamana_build.h:268-272)
         CUDA_TRY(cudaMemsetAsync(d_work.ptr, 0, 4, stream));
         bp.reverse = PRUNE_FORWARD;
@@ -384,7 +373,7 @@ int construct_graph(const char* who, const GraphBuild& b, float reverse_alpha, u
         bp.count = B;
         bp.limit = R;
         bp.alpha = b.alpha;
-        CUDA_TRY(with_rowt(dtype, [&](auto t) {
+        CUDA_TRY(dispatch(DataRows{}, dtype, [&](auto t) {
             return launch_build_prune_op<decltype(t)::value>(op, p, bp, std::min<int>(prune_grid, int(B)), stream);
         }));
         // 2. add_reverse_edges
@@ -397,7 +386,9 @@ int construct_graph(const char* who, const GraphBuild& b, float reverse_alpha, u
         bp.reverse = PRUNE_REVERSE;
         bp.limit = uint32_t(b.prune_to);
         bp.alpha = reverse_alpha;
-        CUDA_TRY(with_rowt(dtype, [&](auto t) { return launch_build_prune_op<decltype(t)::value>(op, p, bp, prune_grid, stream); }));
+        CUDA_TRY(dispatch(DataRows{}, dtype, [&](auto t) {
+            return launch_build_prune_op<decltype(t)::value>(op, p, bp, prune_grid, stream);
+        }));
         reset_heads_kernel<<<unsigned((pair_cap + 255) / 256), 256, 0, stream>>>(d_touched.ptr, d_counts.ptr + 1, d_head.ptr);
         count_launch();
         CUDA_TRY(cudaGetLastError());

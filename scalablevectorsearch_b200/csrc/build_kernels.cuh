@@ -571,41 +571,44 @@ __global__ void __launch_bounds__(32, 16) consolidate_pool_kernel(const __grid_c
     }
 }
 
-template <int ROWT, int OP> cudaError_t launch_build_prune(const SearchParams& p, const BuildParams& bp, int grid, cudaStream_t stream) {
-    const size_t smem = build_smem_bytes(p.qstride);
-    auto go = [&](auto kernel) -> cudaError_t {
-        cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
-        if (err != cudaSuccess) return err;
-        kernel<<<grid, 32, smem, stream>>>(p, bp);
-        count_launch();
-        return cudaGetLastError();
-    };
-    if constexpr (OP < OP_L2I) {   // the integer distance code has one shape for every dimension
-        if (p.dim == 96) return go(build_prune_kernel<ROWT, OP, 96, 1>);
-        if (p.dim >= 256) return go(build_prune_kernel<ROWT, OP, 0, 4>);
-    }
-    return go(build_prune_kernel<ROWT, OP, 0, 1>);
+// The builder's launchers, instantiated once per row type in build_<type>.cu.  Its lean search (HIST) and prune take
+// BuildOps; consolidation's candidate pools are for DynamicRows only.  The prune and the pool run on the caller's grid:
+// `grid` warps, for the pool each with its own scratch slice (bp.scratch_len entries).
+template <int ROWT> cudaError_t launch_build_search(int op, const SearchParams& p, const LaunchConfig& cfg) {
+    return dispatch(BuildOps<ROWT>{}, op, [&](auto o) { return launch_fast<ROWT, decltype(o)::value, true, false>(p, cfg); });
 }
-
-// `grid` warps, each with its own scratch slice (bp.scratch_len entries).
-template <int ROWT, int OP>
-cudaError_t launch_consolidate_pool(const SearchParams& p, const BuildParams& bp, int grid, cudaStream_t stream) {
-    const size_t smem = size_t(p.qstride) * 4;
-    auto go = [&](auto kernel) -> cudaError_t {
-        kernel<<<grid, 32, smem, stream>>>(p, bp);
-        count_launch();
-        return cudaGetLastError();
-    };
-    if (p.dim == 96) return go(consolidate_pool_kernel<ROWT, OP, 96, 1>);
-    if (p.dim >= 256) return go(consolidate_pool_kernel<ROWT, OP, 0, 4>);
-    return go(consolidate_pool_kernel<ROWT, OP, 0, 1>);
-}
-
-// Defined in build_f32.cu / build_f16.cu / build_i8.cu / build_u8.cu; the int8 / uint8 forms take the integer ops.
-template <int ROWT> cudaError_t launch_build_search(int op, const SearchParams& p, const LaunchConfig& cfg);
-template <int ROWT> cudaError_t launch_build_prune_op(int op, const SearchParams& p, const BuildParams& bp, int grid, cudaStream_t stream);
-// Float32 / float16 only: the dynamic index takes no integer data.
 template <int ROWT>
-cudaError_t launch_consolidate_pool_op(int op, const SearchParams& p, const BuildParams& bp, int grid, cudaStream_t stream);
+cudaError_t launch_build_prune_op(int op, const SearchParams& p, const BuildParams& bp, int grid, cudaStream_t stream) {
+    const LaunchConfig cfg{grid, 1, build_smem_bytes(p.qstride), stream};
+    return dispatch(BuildOps<ROWT>{}, op, [&](auto o) {
+        constexpr int OP = decltype(o)::value;
+        return with_shape<OP, false>(p.dim, true, [&](auto ds, auto ks) {
+            return launch_kernel(build_prune_kernel<ROWT, OP, decltype(ds)::value, decltype(ks)::value>, cfg, grid, true,
+                                 p, bp);
+        });
+    });
+}
+template <int ROWT>
+cudaError_t launch_consolidate_pool_op(int op, const SearchParams& p, const BuildParams& bp, int grid, cudaStream_t stream) {
+    const LaunchConfig cfg{grid, 1, size_t(p.qstride) * 4, stream};
+    return dispatch(DynamicOps{}, op, [&](auto o) {
+        constexpr int OP = decltype(o)::value;
+        return with_shape<OP, false>(p.dim, true, [&](auto ds, auto ks) {
+            return launch_kernel(consolidate_pool_kernel<ROWT, OP, decltype(ds)::value, decltype(ks)::value>, cfg, grid, false,
+                                 p, bp);
+        });
+    });
+}
+
+extern template cudaError_t launch_build_search<SVSB200_F32>(int, const SearchParams&, const LaunchConfig&);
+extern template cudaError_t launch_build_search<SVSB200_F16>(int, const SearchParams&, const LaunchConfig&);
+extern template cudaError_t launch_build_search<SVSB200_I8>(int, const SearchParams&, const LaunchConfig&);
+extern template cudaError_t launch_build_search<SVSB200_U8>(int, const SearchParams&, const LaunchConfig&);
+extern template cudaError_t launch_build_prune_op<SVSB200_F32>(int, const SearchParams&, const BuildParams&, int, cudaStream_t);
+extern template cudaError_t launch_build_prune_op<SVSB200_F16>(int, const SearchParams&, const BuildParams&, int, cudaStream_t);
+extern template cudaError_t launch_build_prune_op<SVSB200_I8>(int, const SearchParams&, const BuildParams&, int, cudaStream_t);
+extern template cudaError_t launch_build_prune_op<SVSB200_U8>(int, const SearchParams&, const BuildParams&, int, cudaStream_t);
+extern template cudaError_t launch_consolidate_pool_op<SVSB200_F32>(int, const SearchParams&, const BuildParams&, int, cudaStream_t);
+extern template cudaError_t launch_consolidate_pool_op<SVSB200_F16>(int, const SearchParams&, const BuildParams&, int, cudaStream_t);
 
 }  // namespace svsb200

@@ -8,6 +8,7 @@
 #include <cstdint>
 #include <cstdio>
 #include <string>
+#include <type_traits>
 
 #include "../../include/svsb200.h"
 
@@ -114,15 +115,90 @@ __host__ __device__ inline size_t fast_smem_bytes(uint32_t qstride, uint32_t cap
 
 constexpr int kFastMaxGW = 4;   // adjacency rows up to 128 neighbours (4 x 32) are register-staged
 
-// One launcher per (row type, op); defined in search_<type>.cu.
-template <int ROWT> cudaError_t launch_search(int op, const SearchParams& p, const LaunchConfig& cfg, int rows_in_flight);
-// The lean one-warp-per-CTA form of the same search (search_fast.cuh); defined in fast_<type>.cu.
-template <int ROWT> cudaError_t launch_search_fast(int op, const SearchParams& p, const LaunchConfig& cfg);
-// The same kernel in its MutableBuffer mode (dynamic indexes, f32 / f16 rows); defined in fast_dynamic.cu.
-cudaError_t launch_search_dynamic(int rowt, int op, const SearchParams& p, const LaunchConfig& cfg);
-// Exhaustive scan with the same distance code (ground truth / flat search).
-template <int ROWT> cudaError_t launch_search_exhaustive(int op, const SearchParams& p, const LaunchConfig& cfg);
+constexpr size_t kSmemOptInMax = 227 * 1024;   // dynamic shared memory a block may opt in to on sm_90
+
+// ---- Which (row type, distance operator) pairs every kernel family has ----------------------------------------------
+//   family                                        rows      F32, F16       I8, U8            LVQ8
+//   generic search, exhaustive scan, lean search  SearchRows  L2F IPF COSF   all six           L2F IPF
+//   builder search (HIST), builder prune          DataRows    L2F IPF COSF   L2I IPI COSI      -
+//   consolidate pool, dynamic search (MUT)        DynamicRows L2F IPF COSF   -                 -
+//   flat rescore                                  DataRows    L2F IPF        L2F IPF L2I IPI   -
+// int8 / uint8 rows take float and integer queries in a search; the builder's datum is its own query.
+template <int... V> struct IntList {};
+template <int ROWT> constexpr bool kIntRow = ROWT == SVSB200_I8 || ROWT == SVSB200_U8;
+using FloatOps = IntList<OP_L2F, OP_IPF, OP_COSF>;
+using IntOps = IntList<OP_L2I, OP_IPI, OP_COSI>;
+
+using SearchRows = IntList<SVSB200_F32, SVSB200_F16, SVSB200_I8, SVSB200_U8, ROW_LVQ8>;
+using DataRows = IntList<SVSB200_F32, SVSB200_F16, SVSB200_I8, SVSB200_U8>;   // the four element types of the ABI
+using DynamicRows = IntList<SVSB200_F32, SVSB200_F16>;
+template <int ROWT>
+using SearchOps = std::conditional_t<ROWT == ROW_LVQ8, IntList<OP_L2F, OP_IPF>,
+                                     std::conditional_t<kIntRow<ROWT>, IntList<OP_L2F, OP_IPF, OP_COSF, OP_L2I, OP_IPI, OP_COSI>,
+                                                        FloatOps>>;
+template <int ROWT> using BuildOps = std::conditional_t<kIntRow<ROWT>, IntOps, FloatOps>;
+using DynamicOps = FloatOps;
+template <int ROWT>
+using RescoreOps = std::conditional_t<kIntRow<ROWT>, IntList<OP_L2F, OP_IPF, OP_L2I, OP_IPI>, IntList<OP_L2F, OP_IPF>>;
+
+// f(std::integral_constant<int, V>{}) for the V of the list equal to `v`; cudaErrorInvalidValue when the list lacks it.
+template <int... V, typename F> cudaError_t dispatch(IntList<V...>, int v, F&& f) {
+    cudaError_t err = cudaErrorInvalidValue;
+    (void)((v == V && (err = f(std::integral_constant<int, V>{}), true)) || ...);
+    return err;
+}
+
+// The compile-time shape of a distance pass for rows of `dim` elements: f(DS, KS), DS the static dimension (0: any) and
+// KS the factor by which a float row's accumulators are split over more threads.  Static dimensions get fully unrolled
+// loads (all of a row's loads in flight at once), like the reference's static-N vs Dynamic kernels
+// (distance_core.h:31-42); rows of 256 and more split (float_rows_split) when `split` allows it.  The integer distance
+// code has one shape for every dimension.  The families differ in two ways only: DIM128 (no static 128 for the builder's
+// kernels) and `split` (the searches take it from SearchParams::no_split, the builder and consolidation always split).
+template <int OP, bool DIM128, typename F> cudaError_t with_shape(uint32_t dim, bool split, F&& f) {
+    using One = std::integral_constant<int, 1>;
+    if constexpr (OP < OP_L2I) {
+        if (dim == 96) return f(std::integral_constant<int, 96>{}, One{});
+        if constexpr (DIM128) {
+            if (dim == 128) return f(std::integral_constant<int, 128>{}, One{});
+        }
+        if (dim >= 256 && split) return f(std::integral_constant<int, 0>{}, std::integral_constant<int, 4>{});
+    }
+    return f(std::integral_constant<int, 0>{}, One{});
+}
 
 void count_launch();
+
+// kernel<<<grid, cfg.warps_per_cta * 32, cfg.smem_bytes, cfg.stream>>>(args...), counted, returning the launch error.
+// cfg.grid > 0 is the grid; cfg.grid < 0 asks for a persistent one, -cfg.grid SMs x the CTAs of `kernel` resident per
+// SM.  Either way at most `max_ctas` CTAs.  With `opt_in` the kernel first opts in to cfg.smem_bytes of shared memory.
+template <typename K, typename... Args>
+cudaError_t launch_kernel(K kernel, const LaunchConfig& cfg, size_t max_ctas, bool opt_in, const Args&... args) {
+    const int block = cfg.warps_per_cta * 32;
+    if (opt_in) {
+        cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(cfg.smem_bytes));
+        if (err != cudaSuccess) return err;
+    }
+    int grid = cfg.grid;
+    if (grid < 0) {
+        int resident = 0;
+        cudaError_t err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, kernel, block, cfg.smem_bytes);
+        if (err != cudaSuccess) return err;
+        grid = -grid * (resident > 0 ? resident : 1);
+    }
+    if (size_t(grid) > max_ctas) grid = int(max_ctas);
+    kernel<<<grid, block, cfg.smem_bytes, cfg.stream>>>(args...);
+    count_launch();
+    return cudaGetLastError();
+}
+
+// The search launchers, one per (family, row type), dispatching on the operator.  Defined in search_kernel.cuh and
+// search_fast.cuh, instantiated in search_<type>.cu / fast_<type>.cu / fast_dynamic.cu.
+template <int ROWT> cudaError_t launch_search(int op, const SearchParams& p, const LaunchConfig& cfg, int rows_in_flight);
+// Exhaustive scan with the same distance code (ground truth / flat search).
+template <int ROWT> cudaError_t launch_search_exhaustive(int op, const SearchParams& p, const LaunchConfig& cfg);
+// The lean one-warp-per-CTA form of the same search.
+template <int ROWT> cudaError_t launch_search_fast(int op, const SearchParams& p, const LaunchConfig& cfg);
+// The lean kernel in its MutableBuffer mode (dynamic indexes, DynamicRows).
+template <int ROWT> cudaError_t launch_search_dynamic(int op, const SearchParams& p, const LaunchConfig& cfg);
 
 }  // namespace svsb200

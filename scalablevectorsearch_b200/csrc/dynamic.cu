@@ -480,18 +480,19 @@ int svsb200_dynamic_consolidate(svsb200_index* ix) {
             bp.scratch_keys = d_skey.ptr;
             bp.scratch_len = scratch_len;
             const int op = ix->metric == SVSB200_L2 ? OP_L2F : ix->metric == SVSB200_IP ? OP_IPF : OP_COSF;
-            const bool f32 = ix->dtype == SVSB200_F32;
             for (size_t start = 0; start < total; start += chunk) {
                 bp.nodes = d_nodes.ptr + start;
                 bp.count = uint32_t(std::min<size_t>(chunk, total - start));
                 CUDA_TRY(cudaMemsetAsync(d_work.ptr, 0, 4, stream));
-                CUDA_TRY(f32 ? launch_consolidate_pool_op<SVSB200_F32>(op, p, bp, grid, stream)
-                             : launch_consolidate_pool_op<SVSB200_F16>(op, p, bp, grid, stream));
+                CUDA_TRY(dispatch(DynamicRows{}, ix->dtype, [&](auto t) {
+                    return launch_consolidate_pool_op<decltype(t)::value>(op, p, bp, grid, stream);
+                }));
                 CUDA_TRY(cudaMemsetAsync(d_work.ptr, 0, 4, stream));
                 bp.reverse = PRUNE_CONSOLIDATE;
                 const int prune_grid = int(std::min<size_t>(size_t(rep->sm_count) * 16, bp.count));
-                CUDA_TRY(f32 ? launch_build_prune_op<SVSB200_F32>(op, p, bp, prune_grid, stream)
-                             : launch_build_prune_op<SVSB200_F16>(op, p, bp, prune_grid, stream));
+                CUDA_TRY(dispatch(DynamicRows{}, ix->dtype, [&](auto t) {
+                    return launch_build_prune_op<decltype(t)::value>(op, p, bp, prune_grid, stream);
+                }));
             }
             ref_degree_kernel<<<unsigned((n + 255) / 256), 256, 0, stream>>>(d_deg.ptr, uint32_t(n), rep->d_ref_degree.ptr);
             count_launch();

@@ -3,13 +3,6 @@
 
 namespace svsb200 {
 
-template <> cudaError_t launch_search_fast<SVSB200_F16>(int op, const SearchParams& p, const LaunchConfig& cfg) {
-    switch (op) {
-        case OP_L2F: return launch_fast_dims<SVSB200_F16, OP_L2F>(p, cfg);
-        case OP_IPF: return launch_fast_dims<SVSB200_F16, OP_IPF>(p, cfg);
-        case OP_COSF: return launch_fast_dims<SVSB200_F16, OP_COSF>(p, cfg);
-        default: return cudaErrorInvalidValue;
-    }
-}
+template cudaError_t launch_search_fast<SVSB200_F16>(int, const SearchParams&, const LaunchConfig&);
 
 }  // namespace svsb200

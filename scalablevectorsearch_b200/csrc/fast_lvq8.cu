@@ -3,12 +3,6 @@
 
 namespace svsb200 {
 
-template <> cudaError_t launch_search_fast<ROW_LVQ8>(int op, const SearchParams& p, const LaunchConfig& cfg) {
-    switch (op) {
-        case OP_L2F: return launch_fast_dims<ROW_LVQ8, OP_L2F>(p, cfg);
-        case OP_IPF: return launch_fast_dims<ROW_LVQ8, OP_IPF>(p, cfg);
-        default: return cudaErrorInvalidValue;
-    }
-}
+template cudaError_t launch_search_fast<ROW_LVQ8>(int, const SearchParams&, const LaunchConfig&);
 
 }  // namespace svsb200

@@ -284,7 +284,7 @@ __host__ __device__ inline uint32_t flat_cta_of_tile(uint64_t t, uint64_t total,
 // four), warp 8 the producer.  Shared memory: stages | list keys [2][128][KC] | list ids [2][128][KC] | barriers.
 constexpr uint32_t FLAT_CONSUMER_WARPS = 8, FLAT_THREADS = 32 * FLAT_CONSUMER_WARPS + 32;
 constexpr size_t kFlatSmem = size_t(FLAT_STAGES) * FLAT_STAGE_BYTES + 2 * 2 * size_t(FLAT_KC) * FLAT_BM * 4 + 128;
-static_assert(kFlatSmem <= 227 * 1024, "flat GEMM shared memory exceeds the 227 KB a block may use");
+static_assert(kFlatSmem <= kSmemOptInMax, "flat GEMM shared memory exceeds the 227 KB a block may use");
 
 // Ordered key of an empty list entry, and the threshold of an empty list.
 template <int KIND> __device__ __forceinline__ uint32_t flat_empty_key() {
@@ -636,7 +636,6 @@ template <int OP> __host__ __device__ inline size_t flat_rescore_qbytes(uint32_t
 template <int OP> inline size_t flat_rescore_smem(uint32_t qstride) {
     return flat_rescore_qbytes<OP>(qstride) + size_t(FLAT_CMAX) * 4 * 3;
 }
-constexpr size_t kFlatRescoreSmemMax = 227 * 1024;   // what a block may opt in to on sm_90
 
 template <int ROWT, int OP>
 __global__ void __launch_bounds__(32, 16) flat_rescore_kernel(const __grid_constant__ SearchParams p,
@@ -788,15 +787,12 @@ static cudaError_t flat_tile_rows(int srct, const void* src, uint32_t row_stride
     const uint32_t rows_padded = (n + tile_rows - 1) / tile_rows * tile_rows;
     cudaError_t err = cudaMemsetAsync(dst_tiles, 0, size_t(rows_padded) * KB * FLAT_BK * 2, stream);
     if (err != cudaSuccess) return err;
-    const unsigned grid = (rows_padded + 7) / 8;
-    auto kernel = srct == SVSB200_F32 ? flat_tile_kernel<SVSB200_F32>
-                  : srct == SVSB200_F16 ? flat_tile_kernel<SVSB200_F16>
-                  : srct == SVSB200_I8  ? flat_tile_kernel<SVSB200_I8>
-                                        : flat_tile_kernel<SVSB200_U8>;
-    kernel<<<grid, 256, 0, stream>>>(static_cast<const char*>(src), row_stride, n, dim, tile_rows, KB, scale, l2,
-                                     static_cast<__half*>(dst_tiles), bias, norms, max_norm_bits);
-    count_launch();
-    return cudaGetLastError();
+    const LaunchConfig cfg{int((rows_padded + 7) / 8), 8, 0, stream};
+    return dispatch(DataRows{}, srct, [&](auto t) {
+        return launch_kernel(flat_tile_kernel<decltype(t)::value>, cfg, cfg.grid, false, static_cast<const char*>(src),
+                             row_stride, n, dim, tile_rows, KB, scale, l2, static_cast<__half*>(dst_tiles), bias, norms,
+                             max_norm_bits);
+    });
 }
 
 // int8 / uint8 rows -> 8-bit blobs (flat_tile8_kernel); `bias` may be NULL (query tiles).
@@ -806,12 +802,11 @@ static cudaError_t flat_tile_rows8(int srct, const void* src, uint32_t row_strid
     const uint32_t rows_padded = (n + tile_rows - 1) / tile_rows * tile_rows;
     cudaError_t err = cudaMemsetAsync(dst_tiles, 0, size_t(rows_padded) * KB * FLAT_BK8, stream);
     if (err != cudaSuccess) return err;
-    const unsigned grid = (rows_padded + 7) / 8;
-    auto kernel = srct == SVSB200_I8 ? flat_tile8_kernel<SVSB200_I8> : flat_tile8_kernel<SVSB200_U8>;
-    kernel<<<grid, 256, 0, stream>>>(static_cast<const char*>(src), row_stride, n, dim, tile_rows, KB, l2,
-                                     static_cast<uint8_t*>(dst_tiles), bias);
-    count_launch();
-    return cudaGetLastError();
+    const LaunchConfig cfg{int((rows_padded + 7) / 8), 8, 0, stream};
+    return dispatch(IntList<SVSB200_I8, SVSB200_U8>{}, srct, [&](auto t) {
+        return launch_kernel(flat_tile8_kernel<decltype(t)::value>, cfg, cfg.grid, false, static_cast<const char*>(src),
+                             row_stride, n, dim, tile_rows, KB, l2, static_cast<uint8_t*>(dst_tiles), bias);
+    });
 }
 
 // Lists of absent pieces: (empty key, no id).  `key_bits`: +inf (fp16 lists) or 0xFFFFFFFF (integer lists).
@@ -860,40 +855,15 @@ static cudaError_t flat_gemm_topk(int kind, const void* a_tiles, const void* b_t
     fp.key_scale = key_scale;
     fp.cand_key = cand_key;
     fp.cand_id = cand_id;
-    auto kernel = kind == FLAT_S8 ? flat_gemm_topk_kernel<FLAT_S8>
-                  : kind == FLAT_U8 ? flat_gemm_topk_kernel<FLAT_U8>
-                                    : flat_gemm_topk_kernel<FLAT_F16>;
-    cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(kFlatSmem));
-    if (err != cudaSuccess) return err;
     const size_t entries = size_t(mtiles) * FLAT_BM * nlists * FLAT_KC;
     const uint32_t empty_key = kind == FLAT_F16 ? 0x7F800000u : 0xFFFFFFFFu;
     flat_fill_kernel<<<unsigned(std::min<size_t>(4096, (entries + 255) / 256)), 256, 0, stream>>>(
         reinterpret_cast<uint32_t*>(cand_key), empty_key, cand_id, entries);
     count_launch();
-    kernel<<<ctas, FLAT_THREADS, kFlatSmem, stream>>>(fp);
-    count_launch();
-    return cudaGetLastError();
-}
-
-// Rows wider than about 9 000 elements need more than the default 48 KB of shared memory: the kernel opts in.
-template <int ROWT, int OP> static cudaError_t rescore_launch(const SearchParams& p, const RescoreParams& rp, cudaStream_t stream) {
-    const size_t smem = flat_rescore_smem<OP>(p.qstride);
-    if (smem > 48 * 1024) {
-        cudaError_t err = cudaFuncSetAttribute(flat_rescore_kernel<ROWT, OP>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
-        if (err != cudaSuccess) return err;
-    }
-    flat_rescore_kernel<ROWT, OP><<<rp.nq, 32, smem, stream>>>(p, rp);
-    count_launch();
-    return cudaGetLastError();
-}
-template <int ROWT> static cudaError_t rescore_rowt(int op, const SearchParams& p, const RescoreParams& rp, cudaStream_t stream) {
-    if (op == OP_L2F) return rescore_launch<ROWT, OP_L2F>(p, rp, stream);
-    if (op == OP_IPF) return rescore_launch<ROWT, OP_IPF>(p, rp, stream);
-    if constexpr (ROWT == SVSB200_I8 || ROWT == SVSB200_U8) {
-        if (op == OP_L2I) return rescore_launch<ROWT, OP_L2I>(p, rp, stream);
-        if (op == OP_IPI) return rescore_launch<ROWT, OP_IPI>(p, rp, stream);
-    }
-    return cudaErrorInvalidValue;
+    const LaunchConfig cfg{int(ctas), int(FLAT_THREADS / 32), kFlatSmem, stream};
+    return dispatch(IntList<FLAT_F16, FLAT_S8, FLAT_U8>{}, kind, [&](auto k) {
+        return launch_kernel(flat_gemm_topk_kernel<decltype(k)::value>, cfg, ctas, true, fp);
+    });
 }
 
 static cudaError_t flat_rescore(int rowt, int op, const SearchParams& p, const float* cand_key, const uint32_t* cand_id, uint32_t nsplit,
@@ -915,12 +885,14 @@ static cudaError_t flat_rescore(int rowt, int op, const SearchParams& p, const f
     rp.ksign = p.greater ? -1.0f : 1.0f;
     rp.data_rounded = rowt == SVSB200_F32;
     rp.data_int = rowt == SVSB200_I8 || rowt == SVSB200_U8;
-    switch (rowt) {
-        case SVSB200_F32: return rescore_rowt<SVSB200_F32>(op, p, rp, stream);
-        case SVSB200_F16: return rescore_rowt<SVSB200_F16>(op, p, rp, stream);
-        case SVSB200_I8: return rescore_rowt<SVSB200_I8>(op, p, rp, stream);
-        default: return rescore_rowt<SVSB200_U8>(op, p, rp, stream);
-    }
+    // rows wider than about 9 000 elements need more than the default 48 KB of shared memory: the kernel opts in
+    return dispatch(DataRows{}, rowt, [&](auto t) {
+        return dispatch(RescoreOps<decltype(t)::value>{}, op, [&](auto o) {
+            const LaunchConfig cfg{int(nq), 1, flat_rescore_smem<decltype(o)::value>(p.qstride), stream};
+            return launch_kernel(flat_rescore_kernel<decltype(t)::value, decltype(o)::value>, cfg, nq,
+                                 cfg.smem_bytes > 48 * 1024, p, rp);
+        });
+    });
 }
 
 static cudaError_t flat_move_rows(const void* src, void* dst, const uint32_t* idx, const uint32_t* count, uint32_t max_count,
@@ -943,11 +915,11 @@ static int flat_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, const vo
     const bool shape_ok = ix->storage == SVSB200_PLAIN && ix->metric != SVSB200_COSINE && k + 8 <= FLAT_KC && ix->n >= 512;
     // the integer GEMM: (int8, int8) / (uint8, uint8), every int32 sum exact
     const bool int_gemm = shape_ok && int_data && qdtype == ix->dtype && ix->dim <= FLAT_INT_MAX_DIM &&
-                          flat_rescore_smem<OP_L2I>(query_stride(ix->dim)) <= kFlatRescoreSmemMax;
+                          flat_rescore_smem<OP_L2I>(query_stride(ix->dim)) <= kSmemOptInMax;
     // the fp16 GEMM: float32 / float16 data with float32 / float16 queries, integer data with float32 queries; rows
     // whose staged float query does not fit the rescoring kernel's shared memory keep the scan
     const bool f16_gemm = shape_ok && (int_data ? qdtype == SVSB200_F32 : (qdtype == SVSB200_F32 || qdtype == SVSB200_F16)) &&
-                          flat_rescore_smem<OP_L2F>(query_stride(ix->dim)) <= kFlatRescoreSmemMax;
+                          flat_rescore_smem<OP_L2F>(query_stride(ix->dim)) <= kSmemOptInMax;
     if (!int_gemm && !f16_gemm) {   // shapes outside the GEMM paths: the exact scan
         if (fallback_queries) *fallback_queries = uint32_t(nq);
         return search_on_device(ix, rep, sc, d_queries, qdtype, nq, k, k, k, d_out_ids, 8, d_out_dists, stream, true);

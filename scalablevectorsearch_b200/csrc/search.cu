@@ -271,16 +271,13 @@ int prepare_queries(const svsb200_index* ix, const Replica* rep, Scratch* sc, co
     CUDA_TRY(sc->q_f32.ensure(nq * qstride));
     CUDA_TRY(sc->q_codes.ensure(nq * qstride));
     CUDA_TRY(sc->q_aux.ensure(nq * 2));
-    auto kernel = qdtype == SVSB200_F32   ? prepare_queries_kernel<SVSB200_F32>
-                  : qdtype == SVSB200_F16 ? prepare_queries_kernel<SVSB200_F16>
-                  : qdtype == SVSB200_I8  ? prepare_queries_kernel<SVSB200_I8>
-                                          : prepare_queries_kernel<SVSB200_U8>;
     const int warps = 8;
-    kernel<<<unsigned((nq + warps - 1) / warps), warps * 32, 0, stream>>>(
-        d_queries, uint32_t(nq), uint32_t(ix->dim), qstride, mode, ix->metric, ix->dtype, ix->scale, ix->bias,
-        rep->d_mean.ptr, sc->q_f32.ptr, sc->q_codes.ptr, sc->q_aux.ptr);
-    count_launch();
-    CUDA_TRY(cudaGetLastError());
+    const LaunchConfig cfg{int((nq + warps - 1) / warps), warps, 0, stream};
+    CUDA_TRY(dispatch(DataRows{}, qdtype, [&](auto qt) {
+        return launch_kernel(prepare_queries_kernel<decltype(qt)::value>, cfg, cfg.grid, false, d_queries, uint32_t(nq),
+                             uint32_t(ix->dim), qstride, mode, ix->metric, ix->dtype, ix->scale, ix->bias, rep->d_mean.ptr,
+                             sc->q_f32.ptr, sc->q_codes.ptr, sc->q_aux.ptr);
+    }));
     return 0;
 }
 
@@ -379,7 +376,6 @@ static SearchParams search_params(const svsb200_index* ix, const Replica* rep, c
 // and visited filter in `p`.
 static int choose_launch(const svsb200_index* ix, const Replica* rep, SearchParams* p, bool exhaustive, cudaStream_t stream,
                          LaunchConfig* cfg, bool* use_fast) {
-    const size_t smem_limit = 227 * 1024;
     // The lean kernel (search_fast.cuh) covers the common shape: 16-bit-tag filter on, adjacency rows of up to
     // 128 neighbours; anything else (and the exhaustive scan) runs on the generic kernel.  Its filter: default 256
     // sets (4 KB), more when n needs it for exactness.
@@ -387,7 +383,7 @@ static int choose_launch(const svsb200_index* ix, const Replica* rep, SearchPara
     const LeanFilter lean = lean_filter(ix->n, ix->filter_slots < 0 ? 2048u : uint32_t(ix->filter_slots));
     const size_t fast_bytes = fast_smem_bytes(p->qstride, fast_cap_pad, p->deg_pad, lean.slots * 2u);
     *use_fast = !exhaustive && !ix->generic_kernel && lean.slots >= 64 && ix->filter_tag16 &&
-                p->deg_pad <= 32u * kFastMaxGW && p->gstride % 32u == 0 && fast_bytes <= smem_limit;
+                p->deg_pad <= 32u * kFastMaxGW && p->gstride % 32u == 0 && fast_bytes <= kSmemOptInMax;
     cfg->stream = stream;
     if (*use_fast) {
         p->cap_pad = fast_cap_pad;
@@ -401,8 +397,8 @@ static int choose_launch(const svsb200_index* ix, const Replica* rep, SearchPara
     }
     const size_t per_warp = warp_smem_bytes(p->qstride, p->cap_pad, p->deg_pad, p->filter_slots * (p->filter_tag16 ? 2u : 4u));
     int warps = ix->warps_per_cta ? int(ix->warps_per_cta) : 4;
-    while (warps > 1 && per_warp * warps > smem_limit) warps >>= 1;
-    if (per_warp * warps > smem_limit) return fail("search buffer capacity too large for shared memory");
+    while (warps > 1 && per_warp * warps > kSmemOptInMax) warps >>= 1;
+    if (per_warp * warps > kSmemOptInMax) return fail("search buffer capacity too large for shared memory");
     cfg->warps_per_cta = warps;
     cfg->smem_bytes = per_warp * warps;
     // grid: persistent CTAs; the launcher clamps to what is resident.  ctas_per_sm == 0
@@ -410,17 +406,6 @@ static int choose_launch(const svsb200_index* ix, const Replica* rep, SearchPara
     cfg->grid = rep->sm_count * (ix->ctas_per_sm ? int(ix->ctas_per_sm) : 0);
     if (cfg->grid == 0 || exhaustive) cfg->grid = -rep->sm_count;   // negative: launcher multiplies by occupancy
     return 0;
-}
-
-// Calls f(std::integral_constant<int, ROWT>) for the search kernels' row type `rowt`.
-template <typename F> static cudaError_t with_row_type(int rowt, F f) {
-    switch (rowt) {
-        case ROW_LVQ8: return f(std::integral_constant<int, ROW_LVQ8>{});
-        case SVSB200_F32: return f(std::integral_constant<int, SVSB200_F32>{});
-        case SVSB200_F16: return f(std::integral_constant<int, SVSB200_F16>{});
-        case SVSB200_I8: return f(std::integral_constant<int, SVSB200_I8>{});
-        default: return f(std::integral_constant<int, SVSB200_U8>{});
-    }
 }
 
 // Waits for the event `ev` of a dynamic search's launch.  With a cancellation predicate in the scratch it polls it
@@ -461,9 +446,8 @@ static int search_dynamic(svsb200_index* ix, Replica* rep, Scratch* sc, SearchPa
         return fail("dynamic index: float32 / float16 plain storage only");
     if (!use_fast || op > OP_COSF)
         return fail("dynamic index: the search needs the lean kernel (visited filter on, generic_kernel off, float queries)");
-    const size_t smem_limit = 227 * 1024;
     const size_t fixed = fast_smem_bytes(p.qstride, 0, p.deg_pad, p.filter_slots * 2u);
-    const size_t max_cap = std::min<size_t>((smem_limit - fixed) / 8 / 32 * 32, size_t(1) << 24);
+    const size_t max_cap = std::min<size_t>((kSmemOptInMax - fixed) / 8 / 32 * 32, size_t(1) << 24);
     const size_t C = p.capacity;
     size_t slack = ix->dyn_slack >= 0 ? size_t(ix->dyn_slack) : 3 * C + 32;
     // a list never holds more than n distinct slots, so n entries of room can never overflow
@@ -483,7 +467,7 @@ static int search_dynamic(svsb200_index* ix, Replica* rep, Scratch* sc, SearchPa
         cfg.smem_bytes = fast_smem_bytes(p.qstride, p.cap_pad, p.deg_pad, p.filter_slots * 2u);
         CUDA_TRY(cudaMemsetAsync(sc->d_counter.ptr, 0, sizeof(unsigned int), stream));
         CUDA_TRY(cudaMemsetAsync(p.ovf, 0, sizeof(uint32_t), stream));
-        CUDA_TRY(launch_search_dynamic(rowt, op, p, cfg));
+        CUDA_TRY(dispatch(DynamicRows{}, rowt, [&](auto t) { return launch_search_dynamic<decltype(t)::value>(op, p, cfg); }));
         CUDA_TRY(cudaEventRecord(sc->ev_done, stream));
         bool cancelled = false;
         if (int rc = wait_dynamic(sc, sc->ev_done, &cancelled)) return rc;
@@ -563,7 +547,7 @@ int search_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, const void* d
 
     CUDA_TRY(cudaEventRecord(sc->ev_start, stream));
     const int rowt = ix->storage == SVSB200_LVQ8 ? ROW_LVQ8 : ix->dtype;
-    CUDA_TRY(with_row_type(rowt, [&](auto row) {
+    CUDA_TRY(dispatch(SearchRows{}, rowt, [&](auto row) {
         constexpr int ROWT = decltype(row)::value;
         if (exhaustive) return launch_search_exhaustive<ROWT>(op, p, cfg);
         if (use_fast) return launch_search_fast<ROWT>(op, p, cfg);

@@ -3,22 +3,7 @@
 
 namespace svsb200 {
 
-template <> cudaError_t launch_search<SVSB200_F16>(int op, const SearchParams& p, const LaunchConfig& cfg, int nrows) {
-    switch (op) {
-        case OP_L2F: return launch_dims<SVSB200_F16, OP_L2F>(p, cfg, nrows);
-        case OP_IPF: return launch_dims<SVSB200_F16, OP_IPF>(p, cfg, nrows);
-        case OP_COSF: return launch_dims<SVSB200_F16, OP_COSF>(p, cfg, nrows);
-        default: return cudaErrorInvalidValue;
-    }
-}
-
-template <> cudaError_t launch_search_exhaustive<SVSB200_F16>(int op, const SearchParams& p, const LaunchConfig& cfg) {
-    switch (op) {
-        case OP_L2F: return launch_exhaustive<SVSB200_F16, OP_L2F>(p, cfg);
-        case OP_IPF: return launch_exhaustive<SVSB200_F16, OP_IPF>(p, cfg);
-        case OP_COSF: return launch_exhaustive<SVSB200_F16, OP_COSF>(p, cfg);
-        default: return cudaErrorInvalidValue;
-    }
-}
+template cudaError_t launch_search<SVSB200_F16>(int, const SearchParams&, const LaunchConfig&, int);
+template cudaError_t launch_search_exhaustive<SVSB200_F16>(int, const SearchParams&, const LaunchConfig&);
 
 }  // namespace svsb200

@@ -478,42 +478,28 @@ __global__ void __launch_bounds__(32, fast_min_blocks<ROWT, OP, DS, KS>()) vaman
     }
 }
 
-template <int ROWT, int OP, int DS, int KS = 1, bool HIST = false, bool MUT = false>
-cudaError_t launch_fast(const SearchParams& p, const LaunchConfig& cfg) {
-    auto kernel = vamana_search_fast_kernel<ROWT, OP, DS, KS, HIST, MUT>;
-    cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(cfg.smem_bytes));
-    if (err != cudaSuccess) return err;
-    int grid = cfg.grid;
-    if (grid < 0) {
-        // persistent grid: SM count x resident CTAs of this instantiation
-        int resident = 0;
-        err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, kernel, 32, cfg.smem_bytes);
-        if (err != cudaSuccess) return err;
-        grid = -grid * (resident > 0 ? resident : 1);
-    }
-    if (uint32_t(grid) > p.nq) grid = int(p.nq);
-    kernel<<<grid, 32, cfg.smem_bytes, cfg.stream>>>(p);
-    count_launch();
-    return cudaGetLastError();
+// One lean kernel per query and CTA: at most nq CTAs.  The graph builder (HIST) has no static 128 shape.
+template <int ROWT, int OP, bool HIST, bool MUT> cudaError_t launch_fast(const SearchParams& p, const LaunchConfig& cfg) {
+    return with_shape<OP, !HIST>(p.dim, !p.no_split, [&](auto ds, auto ks) {
+        return launch_kernel(vamana_search_fast_kernel<ROWT, OP, decltype(ds)::value, decltype(ks)::value, HIST, MUT>, cfg,
+                             p.nq, true, p);
+    });
 }
 
-template <int ROWT, int OP, bool HIST = false> cudaError_t launch_fast_dims(const SearchParams& p, const LaunchConfig& cfg) {
-    // Static dimensions get fully unrolled loads; everything else takes the dynamic-length path.  Same
-    // expression tree either way, like the reference's static-N vs Dynamic kernels (distance_core.h:31-42).
-    if constexpr (OP < OP_L2I) {
-        if (p.dim == 96) return launch_fast<ROWT, OP, 96, 1, HIST>(p, cfg);
-        if (p.dim == 128 && !HIST) return launch_fast<ROWT, OP, 128, 1, HIST>(p, cfg);
-        if (p.dim >= 256 && !p.no_split) return launch_fast<ROWT, OP, 0, 4, HIST>(p, cfg);
-    }
-    return launch_fast<ROWT, OP, 0, 1, HIST>(p, cfg);
+// Instantiated once per row type in fast_<type>.cu and fast_dynamic.cu.
+template <int ROWT> cudaError_t launch_search_fast(int op, const SearchParams& p, const LaunchConfig& cfg) {
+    return dispatch(SearchOps<ROWT>{}, op, [&](auto o) { return launch_fast<ROWT, decltype(o)::value, false, false>(p, cfg); });
+}
+template <int ROWT> cudaError_t launch_search_dynamic(int op, const SearchParams& p, const LaunchConfig& cfg) {
+    return dispatch(DynamicOps{}, op, [&](auto o) { return launch_fast<ROWT, decltype(o)::value, false, true>(p, cfg); });
 }
 
-// Dimension dispatch of the MUT kernels: the same shapes as the static search.
-template <int ROWT, int OP> cudaError_t launch_fast_dims_mut(const SearchParams& p, const LaunchConfig& cfg) {
-    if (p.dim == 96) return launch_fast<ROWT, OP, 96, 1, false, true>(p, cfg);
-    if (p.dim == 128) return launch_fast<ROWT, OP, 128, 1, false, true>(p, cfg);
-    if (p.dim >= 256 && !p.no_split) return launch_fast<ROWT, OP, 0, 4, false, true>(p, cfg);
-    return launch_fast<ROWT, OP, 0, 1, false, true>(p, cfg);
-}
+extern template cudaError_t launch_search_fast<SVSB200_F32>(int, const SearchParams&, const LaunchConfig&);
+extern template cudaError_t launch_search_fast<SVSB200_F16>(int, const SearchParams&, const LaunchConfig&);
+extern template cudaError_t launch_search_fast<SVSB200_I8>(int, const SearchParams&, const LaunchConfig&);
+extern template cudaError_t launch_search_fast<SVSB200_U8>(int, const SearchParams&, const LaunchConfig&);
+extern template cudaError_t launch_search_fast<ROW_LVQ8>(int, const SearchParams&, const LaunchConfig&);
+extern template cudaError_t launch_search_dynamic<SVSB200_F32>(int, const SearchParams&, const LaunchConfig&);
+extern template cudaError_t launch_search_dynamic<SVSB200_F16>(int, const SearchParams&, const LaunchConfig&);
 
 }  // namespace svsb200

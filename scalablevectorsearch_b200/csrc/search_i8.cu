@@ -3,28 +3,7 @@
 
 namespace svsb200 {
 
-template <> cudaError_t launch_search<SVSB200_I8>(int op, const SearchParams& p, const LaunchConfig& cfg, int nrows) {
-    switch (op) {
-        case OP_L2F: return launch_dims<SVSB200_I8, OP_L2F>(p, cfg, nrows);
-        case OP_IPF: return launch_dims<SVSB200_I8, OP_IPF>(p, cfg, nrows);
-        case OP_COSF: return launch_dims<SVSB200_I8, OP_COSF>(p, cfg, nrows);
-        case OP_L2I: return launch_dims<SVSB200_I8, OP_L2I>(p, cfg, nrows);
-        case OP_IPI: return launch_dims<SVSB200_I8, OP_IPI>(p, cfg, nrows);
-        case OP_COSI: return launch_dims<SVSB200_I8, OP_COSI>(p, cfg, nrows);
-        default: return cudaErrorInvalidValue;
-    }
-}
-
-template <> cudaError_t launch_search_exhaustive<SVSB200_I8>(int op, const SearchParams& p, const LaunchConfig& cfg) {
-    switch (op) {
-        case OP_L2F: return launch_exhaustive<SVSB200_I8, OP_L2F>(p, cfg);
-        case OP_IPF: return launch_exhaustive<SVSB200_I8, OP_IPF>(p, cfg);
-        case OP_COSF: return launch_exhaustive<SVSB200_I8, OP_COSF>(p, cfg);
-        case OP_L2I: return launch_exhaustive<SVSB200_I8, OP_L2I>(p, cfg);
-        case OP_IPI: return launch_exhaustive<SVSB200_I8, OP_IPI>(p, cfg);
-        case OP_COSI: return launch_exhaustive<SVSB200_I8, OP_COSI>(p, cfg);
-        default: return cudaErrorInvalidValue;
-    }
-}
+template cudaError_t launch_search<SVSB200_I8>(int, const SearchParams&, const LaunchConfig&, int);
+template cudaError_t launch_search_exhaustive<SVSB200_I8>(int, const SearchParams&, const LaunchConfig&);
 
 }  // namespace svsb200

@@ -878,53 +878,40 @@ __global__ void __launch_bounds__(256, SVSB200_MIN_BLOCKS) vamana_search_kernel(
     }
 }
 
-// Host-side launch helper shared by the per-type translation units.
-template <int ROWT, int OP, int DS, int NROWS, int KS = 1>
-cudaError_t launch_one(const SearchParams& p, const LaunchConfig& cfg) {
-    auto kernel = vamana_search_kernel<ROWT, OP, DS, NROWS, false, KS>;
-    cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(cfg.smem_bytes));
-    if (err != cudaSuccess) return err;
-    int grid = cfg.grid;
-    if (grid < 0) {
-        // persistent grid: SM count x resident CTAs of this instantiation
-        int resident = 0;
-        err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, kernel, cfg.warps_per_cta * 32, cfg.smem_bytes);
-        if (err != cudaSuccess) return err;
-        grid = -grid * (resident > 0 ? resident : 1);
-    }
-    const int needed = int((p.nq + cfg.warps_per_cta - 1) / cfg.warps_per_cta);
-    if (grid > needed) grid = needed;
-    kernel<<<grid, cfg.warps_per_cta * 32, cfg.smem_bytes, cfg.stream>>>(p);
-    count_launch();
-    return cudaGetLastError();
+// Host-side launchers, instantiated once per row type in search_<type>.cu.  The generic kernel runs
+// cfg.warps_per_cta queries per CTA with `rows_in_flight` (1 or 2) rows per group and pass; the split shape runs two.
+template <int ROWT>
+cudaError_t launch_search(int op, const SearchParams& p, const LaunchConfig& cfg, int rows_in_flight) {
+    const size_t ctas = (p.nq + cfg.warps_per_cta - 1) / cfg.warps_per_cta;
+    return dispatch(SearchOps<ROWT>{}, op, [&](auto o) {
+        constexpr int OP = decltype(o)::value;
+        return with_shape<OP, true>(p.dim, !p.no_split, [&](auto ds, auto ks) {
+            constexpr int DS = decltype(ds)::value, KS = decltype(ks)::value;
+            if constexpr (KS == 1) {
+                if (rows_in_flight == 1) return launch_kernel(vamana_search_kernel<ROWT, OP, DS, 1>, cfg, ctas, true, p);
+            }
+            return launch_kernel(vamana_search_kernel<ROWT, OP, DS, 2, false, KS>, cfg, ctas, true, p);
+        });
+    });
 }
 
-template <int ROWT, int OP> cudaError_t launch_exhaustive(const SearchParams& p, const LaunchConfig& cfg) {
-    auto kernel = vamana_search_kernel<ROWT, OP, 0, 2, true>;
-    cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(cfg.smem_bytes));
-    if (err != cudaSuccess) return err;
-    int resident = 0;
-    err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, kernel, cfg.warps_per_cta * 32, cfg.smem_bytes);
-    if (err != cudaSuccess) return err;
-    int grid = -cfg.grid * (resident > 0 ? resident : 1);
-    const int needed = int((size_t(p.nq) * (p.exh_split ? p.exh_split : 1u) + cfg.warps_per_cta - 1) / cfg.warps_per_cta);
-    if (grid > needed) grid = needed;
-    kernel<<<grid, cfg.warps_per_cta * 32, cfg.smem_bytes, cfg.stream>>>(p);
-    count_launch();
-    return cudaGetLastError();
+// The exhaustive scan: one work item per (query, range of base rows), on a persistent grid.
+template <int ROWT> cudaError_t launch_search_exhaustive(int op, const SearchParams& p, const LaunchConfig& cfg) {
+    const size_t ctas = (size_t(p.nq) * (p.exh_split ? p.exh_split : 1u) + cfg.warps_per_cta - 1) / cfg.warps_per_cta;
+    return dispatch(SearchOps<ROWT>{}, op, [&](auto o) {
+        return launch_kernel(vamana_search_kernel<ROWT, decltype(o)::value, 0, 2, true>, cfg, ctas, true, p);
+    });
 }
 
-template <int ROWT, int OP> cudaError_t launch_dims(const SearchParams& p, const LaunchConfig& cfg, int nrows) {
-    // Static dimensions get fully unrolled loads (all of a row's loads in flight at once);
-    // everything else takes the dynamic-length path.  Same expression tree either way,
-    // like the reference's static-N vs Dynamic kernels (distance_core.h:31-42).
-    if constexpr (OP < OP_L2I) {
-        if (p.dim == 96) return nrows == 1 ? launch_one<ROWT, OP, 96, 1>(p, cfg) : launch_one<ROWT, OP, 96, 2>(p, cfg);
-        if (p.dim == 128) return nrows == 1 ? launch_one<ROWT, OP, 128, 1>(p, cfg) : launch_one<ROWT, OP, 128, 2>(p, cfg);
-        // wide rows: accumulators split over 4x the threads (float_rows_split)
-        if (p.dim >= 256 && !p.no_split) return launch_one<ROWT, OP, 0, 2, 4>(p, cfg);
-    }
-    return nrows == 1 ? launch_one<ROWT, OP, 0, 1>(p, cfg) : launch_one<ROWT, OP, 0, 2>(p, cfg);
-}
+extern template cudaError_t launch_search<SVSB200_F32>(int, const SearchParams&, const LaunchConfig&, int);
+extern template cudaError_t launch_search<SVSB200_F16>(int, const SearchParams&, const LaunchConfig&, int);
+extern template cudaError_t launch_search<SVSB200_I8>(int, const SearchParams&, const LaunchConfig&, int);
+extern template cudaError_t launch_search<SVSB200_U8>(int, const SearchParams&, const LaunchConfig&, int);
+extern template cudaError_t launch_search<ROW_LVQ8>(int, const SearchParams&, const LaunchConfig&, int);
+extern template cudaError_t launch_search_exhaustive<SVSB200_F32>(int, const SearchParams&, const LaunchConfig&);
+extern template cudaError_t launch_search_exhaustive<SVSB200_F16>(int, const SearchParams&, const LaunchConfig&);
+extern template cudaError_t launch_search_exhaustive<SVSB200_I8>(int, const SearchParams&, const LaunchConfig&);
+extern template cudaError_t launch_search_exhaustive<SVSB200_U8>(int, const SearchParams&, const LaunchConfig&);
+extern template cudaError_t launch_search_exhaustive<ROW_LVQ8>(int, const SearchParams&, const LaunchConfig&);
 
 }  // namespace svsb200

@@ -3,20 +3,7 @@
 
 namespace svsb200 {
 
-template <> cudaError_t launch_search<ROW_LVQ8>(int op, const SearchParams& p, const LaunchConfig& cfg, int nrows) {
-    switch (op) {
-        case OP_L2F: return launch_dims<ROW_LVQ8, OP_L2F>(p, cfg, nrows);
-        case OP_IPF: return launch_dims<ROW_LVQ8, OP_IPF>(p, cfg, nrows);
-        default: return cudaErrorInvalidValue;
-    }
-}
-
-template <> cudaError_t launch_search_exhaustive<ROW_LVQ8>(int op, const SearchParams& p, const LaunchConfig& cfg) {
-    switch (op) {
-        case OP_L2F: return launch_exhaustive<ROW_LVQ8, OP_L2F>(p, cfg);
-        case OP_IPF: return launch_exhaustive<ROW_LVQ8, OP_IPF>(p, cfg);
-        default: return cudaErrorInvalidValue;
-    }
-}
+template cudaError_t launch_search<ROW_LVQ8>(int, const SearchParams&, const LaunchConfig&, int);
+template cudaError_t launch_search_exhaustive<ROW_LVQ8>(int, const SearchParams&, const LaunchConfig&);
 
 }  // namespace svsb200
