@@ -288,6 +288,46 @@ int svsb200_exhaustive_device(
     svsb200_index* index, const void* d_queries, int qdtype, size_t nq, size_t k,
     uint64_t* d_out_ids, float* d_out_dists, void* stream);
 
+/* The svsb200_flat_search* split for a given k (host arithmetic only, like svsb200_flat_plan): for k <= 25 exactly what
+ * svsb200_flat_plan returns, with `list_entries` = 33; for 26 <= k <= 121 and nq > 256 the deep lists of a flat index
+ * (svsb200_flat_index_search*): `list_entries` = 129, one list per query and piece, lists_per_query x 129 <= 1024.
+ * For 26 <= k <= 121 and nq <= 256 that search runs the exact scan: every output is 0 (segment_begin is untouched).
+ * Fails for k = 0 and k > 121 (those searches do not use the GEMM). */
+int svsb200_flat_plan_k(size_t nq, size_t n, size_t k, int sm_count, uint32_t* ctas, uint32_t* share,
+                        uint32_t* lists_per_query, uint32_t* list_entries, uint64_t* segment_begin);
+
+/* Flat index: rows only, no graph.  Replaces: svs::Flat (include/svs/index/flat/flat.h:159) and the runtime's
+ * FlatIndex (bindings/cpp/include/svs/runtime/flat_index.h).  A distinct handle type, so that no graph call can be
+ * made on it. */
+typedef struct svsb200_flat svsb200_flat;
+
+/* Uploads n x dim float32 / float16 / int8 / uint8 rows from HOST memory (row_stride_bytes apart, 0 = dense) to
+ * `device` for `metric` (L2, IP or cosine).  Nothing for a graph is allocated. */
+int svsb200_flat_index_create(const void* vectors, int dtype, size_t n, size_t dim, size_t row_stride_bytes, int metric,
+                              int device, svsb200_flat** out);
+/* Frees the handle and its device memory (NULL is ignored). */
+int svsb200_flat_index_destroy(svsb200_flat* index);
+/* Number of rows, their dimension, and the device memory the rows hold (the GEMM's operand tiles, built on the first
+ * search, are not counted); 0 for NULL. */
+size_t svsb200_flat_index_size(const svsb200_flat* index);
+size_t svsb200_flat_index_dimensions(const svsb200_flat* index);
+size_t svsb200_flat_index_device_bytes(const svsb200_flat* index);
+
+/* FlatIndex::search / svs::Flat::search (index/flat/flat.h:421-465): the exact top k (1 <= k <= 1024) of every query
+ * over all rows, ids as uint64, ties by id; the result equals svsb200_exhaustive_device over the same rows bit for bit.
+ * Routing: k <= 25 runs the GEMM of svsb200_flat_search; 26 <= k <= 121 with nq > 256 the same GEMM with deep
+ * candidate lists (129 entries per query and base range; one 128-query tile keeps at most 7 SMs busy with them, and
+ * batches of one or two tiles run faster on the scan); larger k, cosine, n < 512 and the shapes svsb200_flat_search
+ * leaves to the scan run the exact scan.  Queries: float32 / float16 over float rows, float32 or the rows' own type over int8 /
+ * uint8 rows.  If k > n the rows are padded with all-ones ids and +-inf distances, as the scan pads them.
+ * `fallback_queries` (optional) receives how many queries ran on the scan.  The device form is enqueued on `stream`
+ * apart from one synchronisation (the fallback count). */
+int svsb200_flat_index_search_device(svsb200_flat* index, const void* d_queries, int qdtype, size_t nq, size_t k,
+                                     uint64_t* d_out_ids, float* d_out_dists, void* stream, uint32_t* fallback_queries);
+/* The same with HOST buffers (blocking). */
+int svsb200_flat_index_search(svsb200_flat* index, const void* queries, int qdtype, size_t nq, size_t k, uint64_t* out_ids,
+                              float* out_dists);
+
 /* Dynamic index.  Replaces: MutableVamanaIndex(graph, data, entry_point, distance, external_ids, threadpool)
  * (include/svs/index/vamana/dynamic_index.h:178-202) for float32 / float16 plain storage on one device, adjacency rows
  * of at most 128 neighbours, L2 / MIP / cosine.  Arguments as svsb200_index_create (dense rows), plus one distinct

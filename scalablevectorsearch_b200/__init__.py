@@ -6,8 +6,9 @@ around it (:mod:`.io`).
 """
 from .vamana import (DataType, DistanceType, DynamicVamana, GraphLoader, SearchBufferConfig, ShardedVamana, Vamana,
                      VamanaBuildParameters, VamanaSearchParameters, VectorDataLoader, build_graph, lvq8_compress)
+from .flat import Flat
 from ._lib import Svsb200Error
 
 __all__ = ["DataType", "DistanceType", "GraphLoader", "SearchBufferConfig", "Vamana", "VamanaSearchParameters",
            "VectorDataLoader", "Svsb200Error", "lvq8_compress", "ShardedVamana", "VamanaBuildParameters", "build_graph",
-           "DynamicVamana"]
+           "DynamicVamana", "Flat"]

@@ -22,7 +22,9 @@ SYMBOLS = [
     "svsb200_merge_topk_device", "svsb200_exhaustive_device", "svsb200_lvq8_row_stride", "svsb200_lvq8_compress",
     "svsb200_index_create_multi", "svsb200_index_num_devices", "svsb200_search_cancellable", "svsb200_set_id_offset",
     "svsb200_search_sharded", "svsb200_build_vamana", "svsb200_flat_search_device", "svsb200_flat_search", "svsb200_index_assemble", "svsb200_toml_get", "svsb200_search_filtered", "svsb200_range_search", "svsb200_free", "svsb200_set_entry_points",
-    "svsb200_flat_plan",
+    "svsb200_flat_plan", "svsb200_flat_plan_k",
+    "svsb200_flat_index_create", "svsb200_flat_index_destroy", "svsb200_flat_index_size", "svsb200_flat_index_dimensions",
+    "svsb200_flat_index_device_bytes", "svsb200_flat_index_search", "svsb200_flat_index_search_device",
     "svsb200_dynamic_create", "svsb200_dynamic_delete", "svsb200_dynamic_ids", "svsb200_dynamic_has_id",
     "svsb200_dynamic_export", "svsb200_dynamic_set_build_parameters", "svsb200_dynamic_get_build_parameters",
     "svsb200_dynamic_add", "svsb200_dynamic_consolidate", "svsb200_dynamic_compact", "svsb200_dynamic_build",
@@ -52,6 +54,14 @@ def lib() -> C.CDLL:
     l.svsb200_device_sm.argtypes = [i32, C.POINTER(i32)]
     l.svsb200_flat_plan.argtypes = [C.c_size_t, C.c_size_t, i32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32),
                                     C.POINTER(C.c_uint32), C.c_void_p]
+    l.svsb200_flat_plan_k.argtypes = [sz, sz, sz, i32, C.POINTER(u32), C.POINTER(u32), C.POINTER(u32), C.POINTER(u32), vp]
+    l.svsb200_flat_index_create.argtypes = [vp, i32, sz, sz, sz, i32, i32, C.POINTER(vp)]
+    l.svsb200_flat_index_destroy.argtypes = [vp]
+    for name in ("size", "dimensions", "device_bytes"):
+        fn = getattr(l, f"svsb200_flat_index_{name}")
+        fn.restype, fn.argtypes = sz, [vp]
+    l.svsb200_flat_index_search.argtypes = [vp, vp, i32, sz, sz, vp, vp]
+    l.svsb200_flat_index_search_device.argtypes = [vp, vp, i32, sz, sz, vp, vp, vp, C.POINTER(u32)]
     l.svsb200_index_create.argtypes = [vp, i32, sz, sz, sz, vp, sz, u32, i32, i32, vp, i32, C.POINTER(vp)]
     l.svsb200_index_destroy.argtypes = [vp]
     for name in ("size", "dimensions", "max_degree", "device_bytes"):

@@ -10,6 +10,13 @@
 // Compiles against the reference's runtime *headers* only (no svs core headers); the few out-of-line members of the
 // header types that live in libsvs_runtime (Status message storage, the VamanaIndex destructor / static factories)
 // are defined here.  save / load / LeanVec are the reference's CPU territory: NOT_IMPLEMENTED.
+//
+// It also implements `svs::runtime::v0::FlatIndex` (bindings/cpp/include/svs/runtime/flat_index.h) on the graph-free
+// flat index of libsvsb200 (svsb200_flat_index_*), with the behaviour of the reference's FlatIndexImpl
+// (bindings/cpp/src/flat_index_impl.h, flat_index.cpp): FP32 storage only, the first `add` creates the index and a
+// second one is NOT_IMPLEMENTED, a search before it is NOT_INITIALIZED with labels -1 and distances +inf, k = 0 is
+// INVALID_ARGUMENT.  Divergence: k > 1024 is INVALID_ARGUMENT (the GPU search returns at most 1024 neighbours).
+#include "svs/runtime/flat_index.h"
 #include "svs/runtime/vamana_index.h"
 
 #include "svsb200.h"
@@ -36,6 +43,7 @@ void Status::destroy_message() noexcept {
 }
 
 VamanaIndex::~VamanaIndex() = default;
+FlatIndex::~FlatIndex() = default;
 
 namespace {
 
@@ -288,6 +296,90 @@ Status VamanaIndex::map_to_file(VamanaIndex** index, const char*, MetricType, St
 }
 Status VamanaIndex::map_to_memory(VamanaIndex** index, void*, size_t, MetricType, StorageKind, size_t*) noexcept {
     if (index) *index = nullptr;
+    return Status(ErrorCode::NOT_IMPLEMENTED, "map_to_memory stays on the reference's CPU library");
+}
+
+// ---- FlatIndex ----
+namespace {
+
+class GpuFlatIndex final : public FlatIndex {
+  public:
+    GpuFlatIndex(size_t dim, MetricType metric) : dim_(dim), metric_(metric) {}
+    ~GpuFlatIndex() override { svsb200_flat_index_destroy(index_); }
+
+    // flat_index_impl.h: the first `add` creates the index, later ones are rejected
+    Status add(size_t n, const float* x) noexcept override {
+        if (index_) return Status(ErrorCode::NOT_IMPLEMENTED, "Flat index does not support adding points after initialization");
+        if (n == 0 || !x) return Status(ErrorCode::INVALID_ARGUMENT, "no data");
+        const int metric = metric_ == MetricType::L2 ? SVSB200_L2 : SVSB200_IP;
+        if (svsb200_flat_index_create(x, SVSB200_F32, n, dim_, 0, metric, 0, &index_)) return gpu_error();
+        return Status_Ok;
+    }
+
+    Status search(size_t n, const float* x, size_t k, float* distances, size_t* labels) const noexcept override {
+        if (!index_) {
+            for (size_t i = 0; i < n * k; ++i) {
+                distances[i] = INFINITY;
+                labels[i] = static_cast<size_t>(-1);
+            }
+            return Status(ErrorCode::NOT_INITIALIZED, "Index not initialized");
+        }
+        if (k == 0) return Status(ErrorCode::INVALID_ARGUMENT, "k must be greater than 0");
+        if (k > 1024) return Status(ErrorCode::INVALID_ARGUMENT, "k must be at most 1024 on the GPU");
+        if (n == 0) return Status_Ok;
+        static_assert(sizeof(size_t) == 8, "labels are 64-bit");
+        if (svsb200_flat_index_search(index_, x, SVSB200_F32, n, k, reinterpret_cast<uint64_t*>(labels), distances))
+            return gpu_error();
+        return Status_Ok;
+    }
+
+    Status reset() noexcept override {
+        svsb200_flat_index_destroy(index_);
+        index_ = nullptr;
+        return Status_Ok;
+    }
+
+    Status save(std::ostream&) const noexcept override {
+        return Status(ErrorCode::NOT_IMPLEMENTED, "save stays on the reference's CPU index (index/flat/flat.h)");
+    }
+
+  private:
+    size_t dim_;
+    MetricType metric_;
+    svsb200_flat* index_ = nullptr;
+};
+
+}  // namespace
+
+Status FlatIndex::check_storage_kind(StorageKind kind) noexcept {
+    return kind == StorageKind::FP32 ? Status_Ok
+                                     : Status(ErrorCode::INVALID_ARGUMENT, "FlatIndex only supports FP32 storage kind");
+}
+
+Status FlatIndex::build(FlatIndex** index, size_t dim, MetricType metric) noexcept {
+    if (!index) return Status(ErrorCode::INVALID_ARGUMENT, "null output");
+    *index = nullptr;
+    if (dim == 0) return Status(ErrorCode::INVALID_ARGUMENT, "dim must be positive");
+    *index = new (std::nothrow) GpuFlatIndex(dim, metric);
+    return *index ? Status_Ok : Status(ErrorCode::RUNTIME_ERROR, "out of memory");
+}
+
+Status FlatIndex::destroy(FlatIndex* index) noexcept {
+    delete index;
+    return Status_Ok;
+}
+
+Status FlatIndex::load(FlatIndex** index, std::istream&, MetricType) noexcept {
+    if (index) *index = nullptr;
+    return Status(ErrorCode::NOT_IMPLEMENTED, "load stays on the reference's CPU library");
+}
+Status FlatIndex::map_to_file(FlatIndex** index, const char*, MetricType) noexcept {
+    if (index) *index = nullptr;
+    return Status(ErrorCode::NOT_IMPLEMENTED, "map_to_file stays on the reference's CPU library");
+}
+Status FlatIndex::map_to_memory(FlatIndex** index, void*, size_t, MetricType, size_t* read_bytes) noexcept {
+    if (index) *index = nullptr;
+    if (read_bytes) *read_bytes = 0;
     return Status(ErrorCode::NOT_IMPLEMENTED, "map_to_memory stays on the reference's CPU library");
 }
 

@@ -11,7 +11,9 @@
 //      `cp.async.bulk` into a 6-stage shared-memory ring signalled through mbarriers by a producer warp.  Two
 //      consumer warpgroups each issue `wgmma.mma_async.m64n256k16.f32.f16.f16` on 64 of the tile's 128 query rows,
 //      keep the 64 x 256 fp32 accumulator in registers, turn scores into keys (|x|^2 - 2 q.x for L2, -q.x for
-//      inner product) and keep, per query, the KC smallest keys seen in this CTA's base range.
+//      inner product) and keep, per query, the KC smallest keys seen in this CTA's base range: KC = 33 in one list per
+//      column half (k <= 25), or KC = 129 in one list per query row (k <= 121, the flat index's deep lists).  Either
+//      way a list covers one (row, base range) pair and the ranges of a query are disjoint.
 //   2. flat_rescore_kernel: every candidate of a query (all ranges) is re-scored with the search path's own
 //      bit-exact distance code (eval_pass) and the k best by (key, id) are written out.
 //   3. verification: fp16 rounding moves a key by at most E(q) (derived below); a base row that is NOT a
@@ -64,7 +66,8 @@ constexpr uint32_t FLAT_A_BYTES = FLAT_BM * FLAT_BK * 2, FLAT_B_BYTES = FLAT_BN 
 constexpr uint32_t FLAT_STAGE_BYTES = FLAT_A_BYTES + FLAT_B_BYTES;
 constexpr uint32_t FLAT_STAGES = 6;
 constexpr uint32_t FLAT_KC = 33;                                     // list entries per (query, base range)
-constexpr uint32_t FLAT_LEAD = 4;                                    // tiles a CTA may run ahead of its segment's slowest CTA
+constexpr uint32_t FLAT_KC_DEEP = 129;                               // ... of the deep lists (Flat handle, k <= 121)
+constexpr uint32_t FLAT_LEAD = 4;                                   // tiles a CTA may run ahead of its segment's slowest CTA
 constexpr uint32_t FLAT_CMAX = 1024;                                 // candidates per query the rescoring kernel holds
 constexpr uint32_t FLAT_BK8 = 64;                                    // k elements per blob of 8-bit operands (same bytes)
 constexpr uint32_t FLAT_INT_MAX_DIM = 32768;                         // integer GEMM: every int32 sum and key is exact
@@ -190,11 +193,13 @@ __device__ __forceinline__ void wgmma_m64n256k32(int (&d)[128], uint64_t adesc, 
 }
 #undef FLAT_WGMMA_INT
 __device__ __forceinline__ void reg_fence(int& r) { asm volatile("" : "+r"(r)::"memory"); }
-// Per-query list of the FLAT_KC smallest keys: shared memory, [query row][FLAT_KC] with FLAT_KC odd, so that a warp
-// reading one row side by side is bank-conflict free.  Keys are stored as order-preserving unsigned integers
-// (REDUX.MAX works on them); a list starts full of +inf / no-id entries, so there is no fill count -- an update always
-// replaces the current maximum, and the row's threshold is the new maximum.
+// Per-query list of the KC smallest keys: shared memory, [query row][KC] with KC odd, so that a warp reading one row
+// side by side is bank-conflict free.  Keys are stored as order-preserving unsigned integers (REDUX.MAX works on them);
+// a list starts full of +inf / no-id entries, so there is no fill count -- an update always replaces the current
+// maximum, and the row's threshold is the new maximum.  A lane holds ceil(KC / 32) entries of the row: two for
+// KC = FLAT_KC, five for FLAT_KC_DEEP.
 static_assert(FLAT_KC % 2 == 1 && FLAT_KC > 32 && FLAT_KC <= 64, "list layout");
+static_assert(FLAT_KC_DEEP % 2 == 1 && FLAT_KC_DEEP > 64, "list layout");
 __device__ __forceinline__ uint32_t flat_ord(float f) {
     const uint32_t u = __float_as_uint(f);
     return u ^ (uint32_t(int32_t(u) >> 31) | 0x80000000u);
@@ -203,22 +208,50 @@ __device__ __forceinline__ float flat_unord(uint32_t o) {
     return __uint_as_float(o ^ ((o >> 31) ? 0x80000000u : 0xFFFFFFFFu));
 }
 // The whole warp updates the list of row `list_row` with (key, id); returns the row's new threshold (warp-uniform).
+template <uint32_t KC>
 __device__ __forceinline__ float flat_list_replace_max(uint32_t* lkey, uint32_t* lid, uint32_t list_row, uint32_t lane,
                                                       float key, uint32_t id) {
-    uint32_t* rk = lkey + list_row * FLAT_KC;
-    uint32_t v0 = rk[lane];
-    uint32_t v1 = lane + 32 < FLAT_KC ? rk[lane + 32] : 0u;
-    const uint32_t mx = __reduce_max_sync(0xFFFFFFFFu, max(v0, v1));
-    const uint32_t in0 = __ballot_sync(0xFFFFFFFFu, v0 == mx);
-    const uint32_t in1 = __ballot_sync(0xFFFFFFFFu, v1 == mx && lane + 32 < FLAT_KC);
-    const uint32_t slot = in0 ? uint32_t(__ffs(int(in0)) - 1) : uint32_t(__ffs(int(in1)) + 31);
-    const uint32_t nk = flat_ord(key);
-    if (lane == (slot & 31u)) {
-        rk[slot] = nk;
-        lid[list_row * FLAT_KC + slot] = id;
-        if (slot < 32) v0 = nk; else v1 = nk;
+    uint32_t* rk = lkey + list_row * KC;
+    if constexpr (KC <= 64) {
+        uint32_t v0 = rk[lane];
+        uint32_t v1 = lane + 32 < KC ? rk[lane + 32] : 0u;
+        const uint32_t mx = __reduce_max_sync(0xFFFFFFFFu, max(v0, v1));
+        const uint32_t in0 = __ballot_sync(0xFFFFFFFFu, v0 == mx);
+        const uint32_t in1 = __ballot_sync(0xFFFFFFFFu, v1 == mx && lane + 32 < KC);
+        const uint32_t slot = in0 ? uint32_t(__ffs(int(in0)) - 1) : uint32_t(__ffs(int(in1)) + 31);
+        const uint32_t nk = flat_ord(key);
+        if (lane == (slot & 31u)) {
+            rk[slot] = nk;
+            lid[list_row * KC + slot] = id;
+            if (slot < 32) v0 = nk; else v1 = nk;
+        }
+        return flat_unord(__reduce_max_sync(0xFFFFFFFFu, max(v0, v1)));
+    } else {
+        constexpr uint32_t NW = (KC + 31) / 32;
+        uint32_t v[NW], m = 0;
+#pragma unroll
+        for (uint32_t w = 0; w < NW; ++w) {
+            v[w] = lane + 32 * w < KC ? rk[lane + 32 * w] : 0u;
+            m = max(m, v[w]);
+        }
+        const uint32_t mx = __reduce_max_sync(0xFFFFFFFFu, m);
+        uint32_t slot = 0;   // the first entry holding the maximum
+#pragma unroll
+        for (int w = int(NW) - 1; w >= 0; --w) {
+            const uint32_t in = __ballot_sync(0xFFFFFFFFu, v[w] == mx && lane + 32 * w < KC);
+            if (in) slot = 32 * w + uint32_t(__ffs(int(in)) - 1);
+        }
+        const uint32_t nk = flat_ord(key);
+        const bool mine = lane == (slot & 31u);
+        if (mine) {
+            rk[slot] = nk;
+            lid[list_row * KC + slot] = id;
+        }
+        m = 0;
+#pragma unroll
+        for (uint32_t w = 0; w < NW; ++w) m = max(m, mine && w == slot / 32 ? nk : v[w]);
+        return flat_unord(__reduce_max_sync(0xFFFFFFFFu, m));
     }
-    return flat_unord(__reduce_max_sync(0xFFFFFFFFu, max(v0, v1)));
 }
 // Integer lists are ordered by the pair (key, id).  The whole warp offers (okey, id) to the list of row `list_row`: it
 // replaces the list's largest pair if it is below it.  Returns the ordered key of the new largest pair -- the row's
@@ -229,25 +262,60 @@ __device__ __forceinline__ uint64_t flat_pair_max(uint64_t v) {
     const uint32_t lo = __reduce_max_sync(0xFFFFFFFFu, uint32_t(v >> 32) == hi ? uint32_t(v) : 0u);
     return (uint64_t(hi) << 32) | lo;
 }
+template <uint32_t KC>
 __device__ __forceinline__ uint32_t flat_pair_offer(uint32_t* lkey, uint32_t* lid, uint32_t list_row, uint32_t lane,
                                                     uint32_t okey, uint32_t id) {
-    uint32_t* rk = lkey + list_row * FLAT_KC;
-    uint32_t* ri = lid + list_row * FLAT_KC;
-    const bool has1 = lane + 32 < FLAT_KC;
-    uint64_t v0 = (uint64_t(rk[lane]) << 32) | ri[lane];
-    uint64_t v1 = has1 ? (uint64_t(rk[lane + 32]) << 32) | ri[lane + 32] : 0u;
-    const uint64_t mx = flat_pair_max(max(v0, v1));
-    const uint64_t nv = (uint64_t(okey) << 32) | id;
-    if (nv >= mx) return uint32_t(mx >> 32);   // an equal key with a larger id
-    const uint32_t in0 = __ballot_sync(0xFFFFFFFFu, v0 == mx);
-    const uint32_t in1 = __ballot_sync(0xFFFFFFFFu, v1 == mx && has1);
-    const uint32_t slot = in0 ? uint32_t(__ffs(int(in0)) - 1) : uint32_t(__ffs(int(in1)) + 31);
-    if (lane == (slot & 31u)) {
-        rk[slot] = okey;
-        ri[slot] = id;
-        if (slot < 32) v0 = nv; else v1 = nv;
+    uint32_t* rk = lkey + list_row * KC;
+    uint32_t* ri = lid + list_row * KC;
+    if constexpr (KC <= 64) {
+        const bool has1 = lane + 32 < KC;
+        uint64_t v0 = (uint64_t(rk[lane]) << 32) | ri[lane];
+        uint64_t v1 = has1 ? (uint64_t(rk[lane + 32]) << 32) | ri[lane + 32] : 0u;
+        const uint64_t mx = flat_pair_max(max(v0, v1));
+        const uint64_t nv = (uint64_t(okey) << 32) | id;
+        if (nv >= mx) return uint32_t(mx >> 32);   // an equal key with a larger id
+        const uint32_t in0 = __ballot_sync(0xFFFFFFFFu, v0 == mx);
+        const uint32_t in1 = __ballot_sync(0xFFFFFFFFu, v1 == mx && has1);
+        const uint32_t slot = in0 ? uint32_t(__ffs(int(in0)) - 1) : uint32_t(__ffs(int(in1)) + 31);
+        if (lane == (slot & 31u)) {
+            rk[slot] = okey;
+            ri[slot] = id;
+            if (slot < 32) v0 = nv; else v1 = nv;
+        }
+        return __reduce_max_sync(0xFFFFFFFFu, uint32_t(max(v0, v1) >> 32));
+    } else {
+        // only the keys stay in registers (the ids are read again where a key equals the largest one)
+        constexpr uint32_t NW = (KC + 31) / 32;
+        uint32_t v[NW], m = 0;
+#pragma unroll
+        for (uint32_t w = 0; w < NW; ++w) {
+            v[w] = lane + 32 * w < KC ? rk[lane + 32 * w] : 0u;
+            m = max(m, v[w]);
+        }
+        const uint32_t hi = __reduce_max_sync(0xFFFFFFFFu, m);
+        uint32_t lo = 0;
+#pragma unroll
+        for (uint32_t w = 0; w < NW; ++w)
+            if (lane + 32 * w < KC && v[w] == hi) lo = max(lo, ri[lane + 32 * w]);
+        lo = __reduce_max_sync(0xFFFFFFFFu, lo);
+        const uint64_t mx = (uint64_t(hi) << 32) | lo;
+        if (((uint64_t(okey) << 32) | id) >= mx) return hi;   // an equal key with a larger id
+        uint32_t slot = 0;   // the first entry holding the largest pair
+#pragma unroll
+        for (int w = int(NW) - 1; w >= 0; --w) {
+            const uint32_t in = __ballot_sync(0xFFFFFFFFu, lane + 32 * w < KC && v[w] == hi && ri[lane + 32 * w] == lo);
+            if (in) slot = 32 * w + uint32_t(__ffs(int(in)) - 1);
+        }
+        const bool mine = lane == (slot & 31u);
+        if (mine) {
+            rk[slot] = okey;
+            ri[slot] = id;
+        }
+        m = 0;
+#pragma unroll
+        for (uint32_t w = 0; w < NW; ++w) m = max(m, mine && w == slot / 32 ? okey : v[w]);
+        return __reduce_max_sync(0xFFFFFFFFu, m);
     }
-    return __reduce_max_sync(0xFFFFFFFFu, uint32_t(max(v0, v1) >> 32));
 }
 
 struct FlatParams {
@@ -259,7 +327,7 @@ struct FlatParams {
     uint32_t share;           // R: CTAs that walk the same base tiles at the same time, on R consecutive query tiles
     uint32_t* progress;       // [gridDim.x] tiles started by each CTA (zeroed before the launch)
     float key_scale;          // key = bias + key_scale * s (-2 or -1)
-    float* cand_key;          // [mtiles * FLAT_BM][nlists][FLAT_KC], pre-filled with (+inf, no id)
+    float* cand_key;          // [mtiles * FLAT_BM][nlists][KC], pre-filled with (+inf, no id)
                               // (integer kinds: ordered int32 keys, pre-filled with 0xFFFFFFFF)
     uint32_t* cand_id;
 };
@@ -271,7 +339,8 @@ struct FlatParams {
 // other, so all but the first request are served by L2 -- without this, one CTA per SM streams as many different
 // places of a base that is many times the L2, and every operand byte comes from DRAM.  A segment may run over a
 // row-group boundary (the lists are flushed there), and a query tile is covered by a few consecutive segments
-// ("pieces"); each piece keeps two lists per query, one per half of the 256 tile columns.
+// ("pieces"); each piece keeps two lists per query, one per half of the 256 tile columns -- or, with the deep lists
+// (KC = FLAT_KC_DEEP), one list per query that both halves share.
 __host__ __device__ inline uint64_t flat_seg_begin(uint64_t total, uint32_t ctas, uint32_t b) { return total * b / ctas; }
 __host__ __device__ inline uint32_t flat_cta_of_tile(uint64_t t, uint64_t total, uint32_t ctas) {
     uint32_t b = uint32_t(t * ctas / total);
@@ -281,10 +350,18 @@ __host__ __device__ inline uint32_t flat_cta_of_tile(uint64_t t, uint64_t total,
 }
 
 // Threads: warps 0-7 are the two consumer warpgroups (a warpgroup is four consecutive warps starting at a multiple of
-// four), warp 8 the producer.  Shared memory: stages | list keys [2][128][KC] | list ids [2][128][KC] | barriers.
+// four), warp 8 the producer.  Shared memory: stages | list keys [H][128][KC] | list ids [H][128][KC] | barriers, with
+// H lists per query row: two (one per column half) with FLAT_KC entries and a 6-stage ring, one with FLAT_KC_DEEP
+// entries and a 4-stage ring (4 x 24 576 + 128 x 129 x 8 + 128 = 230 528 bytes).
 constexpr uint32_t FLAT_CONSUMER_WARPS = 8, FLAT_THREADS = 32 * FLAT_CONSUMER_WARPS + 32;
-constexpr size_t kFlatSmem = size_t(FLAT_STAGES) * FLAT_STAGE_BYTES + 2 * 2 * size_t(FLAT_KC) * FLAT_BM * 4 + 128;
-static_assert(kFlatSmem <= kSmemOptInMax, "flat GEMM shared memory exceeds the 227 KB a block may use");
+template <uint32_t KC> struct FlatShape {
+    static constexpr uint32_t HALVES = KC == FLAT_KC ? 2 : 1;   // lists per query row and piece
+    static constexpr uint32_t STAGES = KC == FLAT_KC ? FLAT_STAGES : 4;
+    static constexpr size_t SMEM = size_t(STAGES) * FLAT_STAGE_BYTES + 2 * HALVES * size_t(KC) * FLAT_BM * 4 + 128;
+    static_assert(SMEM <= kSmemOptInMax, "flat GEMM shared memory exceeds the 227 KB a block may use");
+};
+template struct FlatShape<FLAT_KC>;
+template struct FlatShape<FLAT_KC_DEEP>;
 
 // Ordered key of an empty list entry, and the threshold of an empty list.
 template <int KIND> __device__ __forceinline__ uint32_t flat_empty_key() {
@@ -296,16 +373,19 @@ template <int KIND> __device__ __forceinline__ auto flat_no_threshold() {
     else return 0xFFFFFFFFu;
 }
 
-template <int KIND>
+// (The shape is named through the type alias `Shape` only: a kernel-local constant would make the compiler order the
+// main loop's stage counters differently and change the FLAT_KC instantiations' code.)
+template <int KIND, uint32_t KC>
 __global__ void __launch_bounds__(FLAT_THREADS, 1) flat_gemm_topk_kernel(const __grid_constant__ FlatParams fp) {
     using acc_t = std::conditional_t<KIND == FLAT_F16, float, int>;
+    using Shape = FlatShape<KC>;
     extern __shared__ __align__(1024) uint8_t smem[];
     uint8_t* stages = smem;
-    uint32_t* lkey = reinterpret_cast<uint32_t*>(smem + size_t(FLAT_STAGES) * FLAT_STAGE_BYTES);   // [2][128][KC] ordered keys
-    uint32_t* lid = lkey + 2 * size_t(FLAT_KC) * FLAT_BM;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(lid + 2 * size_t(FLAT_KC) * FLAT_BM);
+    uint32_t* lkey = reinterpret_cast<uint32_t*>(smem + size_t(Shape::STAGES) * FLAT_STAGE_BYTES);   // [H][128][KC] ordered keys
+    uint32_t* lid = lkey + Shape::HALVES * size_t(KC) * FLAT_BM;
+    uint64_t* bars = reinterpret_cast<uint64_t*>(lid + Shape::HALVES * size_t(KC) * FLAT_BM);
     uint64_t* full = bars;                       // [STAGES] bytes of a stage have landed
-    uint64_t* empty = bars + FLAT_STAGES;        // [STAGES] the MMAs of every consumer warp reading a stage have completed
+    uint64_t* empty = bars + Shape::STAGES;      // [STAGES] the MMAs of every consumer warp reading a stage have completed
 
     const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t nseg = gridDim.x / fp.share, seg = blockIdx.x % nseg, member = blockIdx.x / nseg;
@@ -317,7 +397,7 @@ __global__ void __launch_bounds__(FLAT_THREADS, 1) flat_gemm_topk_kernel(const _
     const uint32_t mtile0 = uint32_t(t_lo / fp.ntiles) * fp.share + member, nt0 = uint32_t(t_lo % fp.ntiles);
 
     if (threadIdx.x == 0) {
-        for (uint32_t i = 0; i < FLAT_STAGES; ++i) {
+        for (uint32_t i = 0; i < Shape::STAGES; ++i) {
             mbar_init(full + i, 1);
             mbar_init(empty + i, FLAT_CONSUMER_WARPS);
         }
@@ -361,7 +441,7 @@ __global__ void __launch_bounds__(FLAT_THREADS, 1) flat_gemm_topk_kernel(const _
                     bulk_copy_g2s(st + FLAT_A_BYTES,
                                   reinterpret_cast<const uint8_t*>(fp.b_tiles) + (size_t(nt) * fp.KB + kb) * FLAT_B_BYTES,
                                   FLAT_B_BYTES, full + s);
-                    if (++s == FLAT_STAGES) {
+                    if (++s == Shape::STAGES) {
                         s = 0;
                         ph ^= 1u;
                     }
@@ -379,20 +459,21 @@ __global__ void __launch_bounds__(FLAT_THREADS, 1) flat_gemm_topk_kernel(const _
     // ===== consumers: warpgroup wg computes query rows 64 wg .. 64 wg + 63 of the tile against all 256 base rows.
     // Accumulator element d[4c + 2i + e] of a thread is (row 16 (warp % 4) + lane / 4 + 8 i, column 8c + 2 (lane % 4) + e)
     // of its warpgroup's 64 x 256 block, so the four lanes of a quad share two rows; a row keeps one list per column
-    // half, updated by the whole warp (all lanes of a quad see the new threshold) =====
+    // half (deep lists: one list), updated by the whole warp (all lanes of a quad see the new threshold) =====
     const uint32_t wg = warp >> 2;
     const uint32_t row0 = wg * 64 + (warp & 3u) * 16 + (lane >> 2);   // the thread's rows: row0, row0 + 8
     const uint32_t frow = wg * 64 + (warp & 3u) * 16 + (lane >> 1), fhalf = lane & 1u;   // the (row, half) list this lane clears / writes out
     acc_t d[128];
 #pragma unroll
     for (uint32_t i = 0; i < 128; ++i) d[i] = acc_t(0);
-    // [row i][column half]: the largest key of that list (integer kinds: the ordered key of its largest (key, id) pair)
-    std::conditional_t<KIND == FLAT_F16, float, uint32_t> thr[2][2];
+    // [row i][list]: the largest key of that list (integer kinds: the ordered key of its largest (key, id) pair)
+    std::conditional_t<KIND == FLAT_F16, float, uint32_t> thr[2][Shape::HALVES];
 #pragma unroll
-    for (uint32_t i = 0; i < 4; ++i) thr[i >> 1][i & 1] = flat_no_threshold<KIND>();
-    for (uint32_t e = 0; e < FLAT_KC; ++e) {
-        lkey[(fhalf * FLAT_BM + frow) * FLAT_KC + e] = flat_empty_key<KIND>();
-        lid[(fhalf * FLAT_BM + frow) * FLAT_KC + e] = 0xFFFFFFFFu;
+    for (uint32_t i = 0; i < 2 * Shape::HALVES; ++i) thr[i / Shape::HALVES][i % Shape::HALVES] = flat_no_threshold<KIND>();
+    // (deep lists: the two lanes of a row clear / write out alternate entries of its one list)
+    for (uint32_t e = Shape::HALVES == 2 ? 0u : fhalf; e < KC; e += 3 - Shape::HALVES) {
+        lkey[(Shape::HALVES == 2 ? fhalf * FLAT_BM + frow : frow) * KC + e] = flat_empty_key<KIND>();
+        lid[(Shape::HALVES == 2 ? fhalf * FLAT_BM + frow : frow) * KC + e] = 0xFFFFFFFFu;
     }
     __syncwarp();
     uint32_t s = 0, ph = 0, mtile = mtile0, nt = nt0;
@@ -424,7 +505,7 @@ __global__ void __launch_bounds__(FLAT_THREADS, 1) flat_gemm_topk_kernel(const _
             wgmma_wait<1>();
             if (kb > 0 && lane == 0) mbar_arrive(empty + prev);
             prev = s;
-            if (++s == FLAT_STAGES) {
+            if (++s == Shape::STAGES) {
                 s = 0;
                 ph ^= 1u;
             }
@@ -440,7 +521,7 @@ __global__ void __launch_bounds__(FLAT_THREADS, 1) flat_gemm_topk_kernel(const _
             const float* bias = fp.b_bias + size_t(nt) * FLAT_BN + 2 * (lane & 3u);
 #pragma unroll
             for (uint32_t c = 0; c < FLAT_BN / 8; ++c) {
-                const uint32_t h = c / (FLAT_BN / 16);
+                const uint32_t h = Shape::HALVES == 2 ? c / (FLAT_BN / 16) : 0u;   // the list of this column
                 const float2 b2 = __ldg(reinterpret_cast<const float2*>(bias + 8 * c));
                 float key[4];
                 key[0] = fmaf(fp.key_scale, d[4 * c + 0], b2.x);
@@ -449,8 +530,8 @@ __global__ void __launch_bounds__(FLAT_THREADS, 1) flat_gemm_topk_kernel(const _
                 key[3] = fmaf(fp.key_scale, d[4 * c + 3], b2.y);
                 const bool any = fminf(key[0], key[1]) < thr[0][h] || fminf(key[2], key[3]) < thr[1][h];
                 if (!__any_sync(0xFFFFFFFFu, any)) continue;
-                uint32_t* my_key = lkey + size_t(h) * FLAT_BM * FLAT_KC;
-                uint32_t* my_id = lid + size_t(h) * FLAT_BM * FLAT_KC;
+                uint32_t* my_key = lkey + size_t(h) * FLAT_BM * KC;
+                uint32_t* my_id = lid + size_t(h) * FLAT_BM * KC;
 #pragma unroll
                 for (uint32_t v = 0; v < 4; ++v) {
                     const uint32_t i = v >> 1;
@@ -460,8 +541,8 @@ __global__ void __launch_bounds__(FLAT_THREADS, 1) flat_gemm_topk_kernel(const _
                         const uint32_t src = uint32_t(__ffs(int(hits)) - 1);
                         const float k_src = __shfl_sync(0xFFFFFFFFu, key[v], src);
                         const uint32_t id = nt * FLAT_BN + 8 * c + 2 * (src & 3u) + (v & 1u);
-                        const float tnew = flat_list_replace_max(my_key, my_id, row0 - (lane >> 2) + (src >> 2) + 8 * i, lane,
-                                                                 k_src, id);
+                        const float tnew = flat_list_replace_max<KC>(my_key, my_id, row0 - (lane >> 2) + (src >> 2) + 8 * i,
+                                                                     lane, k_src, id);
                         if ((lane >> 2) == (src >> 2)) thr[i][h] = tnew;
                         // another lane of the quad may hold a key of the same row that no longer beats the new threshold
                         pending = pending && lane != src && key[v] < thr[i][h];
@@ -478,7 +559,7 @@ __global__ void __launch_bounds__(FLAT_THREADS, 1) flat_gemm_topk_kernel(const _
             const uint32_t ks = uint32_t(int(fp.key_scale));
 #pragma unroll
             for (uint32_t c = 0; c < FLAT_BN / 8; ++c) {
-                const uint32_t h = c / (FLAT_BN / 16);
+                const uint32_t h = Shape::HALVES == 2 ? c / (FLAT_BN / 16) : 0u;
                 const uint2 b2 = __ldg(reinterpret_cast<const uint2*>(bias + 8 * c));
                 uint32_t key[4];
                 key[0] = (b2.x + ks * uint32_t(d[4 * c + 0])) ^ 0x80000000u;
@@ -487,8 +568,8 @@ __global__ void __launch_bounds__(FLAT_THREADS, 1) flat_gemm_topk_kernel(const _
                 key[3] = (b2.y + ks * uint32_t(d[4 * c + 3])) ^ 0x80000000u;
                 const bool any = min(key[0], key[1]) <= thr[0][h] || min(key[2], key[3]) <= thr[1][h];
                 if (!__any_sync(0xFFFFFFFFu, any)) continue;
-                uint32_t* my_key = lkey + size_t(h) * FLAT_BM * FLAT_KC;
-                uint32_t* my_id = lid + size_t(h) * FLAT_BM * FLAT_KC;
+                uint32_t* my_key = lkey + size_t(h) * FLAT_BM * KC;
+                uint32_t* my_id = lid + size_t(h) * FLAT_BM * KC;
 #pragma unroll
                 for (uint32_t v = 0; v < 4; ++v) {
                     const uint32_t i = v >> 1;
@@ -498,8 +579,8 @@ __global__ void __launch_bounds__(FLAT_THREADS, 1) flat_gemm_topk_kernel(const _
                         const uint32_t src = uint32_t(__ffs(int(hits)) - 1);
                         const uint32_t k_src = __shfl_sync(0xFFFFFFFFu, key[v], src);
                         const uint32_t id = nt * FLAT_BN + 8 * c + 2 * (src & 3u) + (v & 1u);
-                        const uint32_t tnew = flat_pair_offer(my_key, my_id, row0 - (lane >> 2) + (src >> 2) + 8 * i, lane,
-                                                              k_src, id);
+                        const uint32_t tnew = flat_pair_offer<KC>(my_key, my_id, row0 - (lane >> 2) + (src >> 2) + 8 * i, lane,
+                                                                  k_src, id);
                         if ((lane >> 2) == (src >> 2)) thr[i][h] = tnew;
                         pending = pending && lane != src && key[v] <= thr[i][h];
                         hits = __ballot_sync(0xFFFFFFFFu, pending);
@@ -511,12 +592,13 @@ __global__ void __launch_bounds__(FLAT_THREADS, 1) flat_gemm_topk_kernel(const _
             // the query tile (or this CTA's part of it) is finished: lists out, lists reset
             const uint32_t piece = seg - flat_cta_of_tile(uint64_t(mtile / fp.share) * fp.ntiles, total, nseg);
             const size_t q = size_t(mtile) * FLAT_BM + frow;
-            float* ok = fp.cand_key + (q * fp.nlists + piece * 2 + fhalf) * FLAT_KC;
-            uint32_t* oi = fp.cand_id + (q * fp.nlists + piece * 2 + fhalf) * FLAT_KC;
-            uint32_t* rk = lkey + (fhalf * FLAT_BM + frow) * FLAT_KC;
-            uint32_t* ri = lid + (fhalf * FLAT_BM + frow) * FLAT_KC;
+            const size_t list = q * fp.nlists + piece * Shape::HALVES + (Shape::HALVES == 2 ? fhalf : 0u);
+            float* ok = fp.cand_key + list * KC;
+            uint32_t* oi = fp.cand_id + list * KC;
+            uint32_t* rk = lkey + (Shape::HALVES == 2 ? fhalf * FLAT_BM + frow : frow) * KC;
+            uint32_t* ri = lid + (Shape::HALVES == 2 ? fhalf * FLAT_BM + frow : frow) * KC;
             __syncwarp();
-            for (uint32_t e = 0; e < FLAT_KC; ++e) {
+            for (uint32_t e = Shape::HALVES == 2 ? 0u : fhalf; e < KC; e += 3 - Shape::HALVES) {
                 if constexpr (KIND == FLAT_F16) ok[e] = flat_unord(rk[e]);
                 else reinterpret_cast<uint32_t*>(ok)[e] = rk[e];
                 oi[e] = ri[e];
@@ -525,7 +607,7 @@ __global__ void __launch_bounds__(FLAT_THREADS, 1) flat_gemm_topk_kernel(const _
             }
             __syncwarp();
 #pragma unroll
-            for (uint32_t i = 0; i < 4; ++i) thr[i >> 1][i & 1] = flat_no_threshold<KIND>();
+            for (uint32_t i = 0; i < 2 * Shape::HALVES; ++i) thr[i / Shape::HALVES][i % Shape::HALVES] = flat_no_threshold<KIND>();
             nt = 0;
             mtile += fp.share;
         }
@@ -615,7 +697,7 @@ __global__ void flat_tile8_kernel(const char* __restrict__ src, uint32_t row_str
 
 // ---- exact re-scoring + verification: one warp per query ----------------------------------------------------------
 struct RescoreParams {
-    const float* cand_key;    // [nq_padded][nsplit][KC]
+    const float* cand_key;    // [nq_padded][nsplit][KC], nsplit * KC <= FLAT_CMAX
     const uint32_t* cand_id;
     uint32_t nsplit, nq, k, n;
     const float* qnorm;       // [nq] ||q||
@@ -637,7 +719,7 @@ template <int OP> inline size_t flat_rescore_smem(uint32_t qstride) {
     return flat_rescore_qbytes<OP>(qstride) + size_t(FLAT_CMAX) * 4 * 3;
 }
 
-template <int ROWT, int OP>
+template <int ROWT, int OP, int KC>
 __global__ void __launch_bounds__(32, 16) flat_rescore_kernel(const __grid_constant__ SearchParams p,
                                                              const __grid_constant__ RescoreParams rp) {
     constexpr bool kInt = (OP >= OP_L2I);   // the integer GEMM's candidates: exact keys, (key, id) lists
@@ -656,7 +738,7 @@ __global__ void __launch_bounds__(32, 16) flat_rescore_kernel(const __grid_const
     const int g = lane / G, t = lane % G;
     const uint32_t q = blockIdx.x;
     if (q >= rp.nq) return;
-    const uint32_t total = rp.nsplit * FLAT_KC;
+    const uint32_t total = rp.nsplit * uint32_t(KC);
     const uint32_t* okey = reinterpret_cast<const uint32_t*>(rp.cand_key);
     // candidates of every base range; T = the smallest per-range list maximum (every excluded row is >= it)
     float T = INFINITY;
@@ -664,14 +746,14 @@ __global__ void __launch_bounds__(32, 16) flat_rescore_kernel(const __grid_const
     for (uint32_t s = 0; s < rp.nsplit; ++s) {
         if constexpr (kInt) {
             uint64_t mx = 0;
-            for (uint32_t e = lane; e < FLAT_KC; e += 32) {
-                const size_t o = (size_t(q) * rp.nsplit + s) * FLAT_KC + e;
+            for (uint32_t e = lane; e < uint32_t(KC); e += 32) {
+                const size_t o = (size_t(q) * rp.nsplit + s) * uint32_t(KC) + e;
                 mx = max(mx, (uint64_t(okey[o]) << 32) | rp.cand_id[o]);
             }
             Tp = min(Tp, flat_pair_max(mx));
         } else {
             float mx = -INFINITY;
-            for (uint32_t e = lane; e < FLAT_KC; e += 32) mx = fmaxf(mx, rp.cand_key[(size_t(q) * rp.nsplit + s) * FLAT_KC + e]);
+            for (uint32_t e = lane; e < uint32_t(KC); e += 32) mx = fmaxf(mx, rp.cand_key[(size_t(q) * rp.nsplit + s) * uint32_t(KC) + e]);
             for (int o = 16; o; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(FULL, mx, o));
             T = fminf(T, mx);
         }
@@ -737,7 +819,7 @@ __global__ void __launch_bounds__(32, 16) flat_rescore_kernel(const __grid_const
         if (lane == 0 && !verified) rp.unverified[atomicAdd(rp.n_unverified, 1u)] = q;
         return;
     }
-    // rank of every candidate by (exact key, id) and by approximate key: k is small, C <= 512
+    // rank of every candidate by (exact key, id) and by approximate key: C <= FLAT_CMAX
     float kth_approx = INFINITY;
     for (uint32_t i = lane; i < C; i += 32) {
         const float ke = ekey[i], ka = akey[i];
@@ -817,10 +899,12 @@ __global__ void flat_fill_kernel(uint32_t* __restrict__ key, uint32_t key_bits, 
     }
 }
 
-// Grid size, sharing factor and lists per query for a problem: as many CTAs as SMs in groups of R, fewer segments
-// while a query tile would be cut into more pieces than the rescoring kernel holds candidates for (small batches
-// over a large base).
-static void flat_plan(uint32_t mtiles, uint32_t ntiles, uint32_t sm_count, uint32_t* ctas, uint32_t* share, uint32_t* nlists) {
+// Grid size, sharing factor and lists per query for a problem with lists of `kc` entries (FLAT_KC: two per piece,
+// FLAT_KC_DEEP: one): as many CTAs as SMs in groups of R, fewer segments while a query tile would be cut into more
+// pieces than the rescoring kernel holds candidates for (small batches over a large base).
+static void flat_plan(uint32_t mtiles, uint32_t ntiles, uint32_t sm_count, uint32_t kc, uint32_t* ctas, uint32_t* share,
+                      uint32_t* nlists) {
+    const uint32_t per_piece = kc == FLAT_KC ? 2 : 1;
     const uint32_t R = mtiles >= 8 ? 4 : mtiles >= 4 ? 2 : 1;
     const uint32_t ngroups = (mtiles + R - 1) / R;
     const uint64_t total = uint64_t(ngroups) * ntiles;
@@ -830,16 +914,16 @@ static void flat_plan(uint32_t mtiles, uint32_t ntiles, uint32_t sm_count, uint3
         for (uint32_t m = 0; m < ngroups; ++m)
             pieces = std::max(pieces, flat_cta_of_tile(uint64_t(m + 1) * ntiles - 1, total, g) -
                                           flat_cta_of_tile(uint64_t(m) * ntiles, total, g) + 1);
-        if (2 * pieces * FLAT_KC <= FLAT_CMAX || g == 1) {
+        if (per_piece * pieces * kc <= FLAT_CMAX || g == 1) {
             *ctas = g * R;
             *share = R;
-            *nlists = 2 * pieces;
+            *nlists = per_piece * pieces;
             return;
         }
     }
 }
 
-static cudaError_t flat_gemm_topk(int kind, const void* a_tiles, const void* b_tiles, const void* b_bias, uint32_t KB, uint32_t ntiles,
+static cudaError_t flat_gemm_topk(int kind, int kc, const void* a_tiles, const void* b_tiles, const void* b_bias, uint32_t KB, uint32_t ntiles,
                                   uint32_t mtiles, uint32_t ctas, uint32_t share, uint32_t nlists, float key_scale, float* cand_key,
                                   uint32_t* cand_id, uint32_t* progress, cudaStream_t stream) {
     FlatParams fp{};
@@ -855,18 +939,21 @@ static cudaError_t flat_gemm_topk(int kind, const void* a_tiles, const void* b_t
     fp.key_scale = key_scale;
     fp.cand_key = cand_key;
     fp.cand_id = cand_id;
-    const size_t entries = size_t(mtiles) * FLAT_BM * nlists * FLAT_KC;
+    const size_t entries = size_t(mtiles) * FLAT_BM * nlists * kc;
     const uint32_t empty_key = kind == FLAT_F16 ? 0x7F800000u : 0xFFFFFFFFu;
     flat_fill_kernel<<<unsigned(std::min<size_t>(4096, (entries + 255) / 256)), 256, 0, stream>>>(
         reinterpret_cast<uint32_t*>(cand_key), empty_key, cand_id, entries);
     count_launch();
-    const LaunchConfig cfg{int(ctas), int(FLAT_THREADS / 32), kFlatSmem, stream};
-    return dispatch(IntList<FLAT_F16, FLAT_S8, FLAT_U8>{}, kind, [&](auto k) {
-        return launch_kernel(flat_gemm_topk_kernel<decltype(k)::value>, cfg, ctas, true, fp);
+    return dispatch(IntList<FLAT_KC, FLAT_KC_DEEP>{}, kc, [&](auto c) {
+        constexpr int KC = decltype(c)::value;
+        const LaunchConfig cfg{int(ctas), int(FLAT_THREADS / 32), FlatShape<KC>::SMEM, stream};
+        return dispatch(IntList<FLAT_F16, FLAT_S8, FLAT_U8>{}, kind, [&](auto k) {
+            return launch_kernel(flat_gemm_topk_kernel<decltype(k)::value, uint32_t(KC)>, cfg, ctas, true, fp);
+        });
     });
 }
 
-static cudaError_t flat_rescore(int rowt, int op, const SearchParams& p, const float* cand_key, const uint32_t* cand_id, uint32_t nsplit,
+static cudaError_t flat_rescore(int rowt, int op, int kc, const SearchParams& p, const float* cand_key, const uint32_t* cand_id, uint32_t nsplit,
                                 uint32_t nq, uint32_t k, const float* qnorm, const unsigned int* xmax_bits, uint64_t* out_ids,
                                 float* out_dists, uint32_t* unverified, uint32_t* n_unverified, cudaStream_t stream) {
     RescoreParams rp{};
@@ -886,11 +973,13 @@ static cudaError_t flat_rescore(int rowt, int op, const SearchParams& p, const f
     rp.data_rounded = rowt == SVSB200_F32;
     rp.data_int = rowt == SVSB200_I8 || rowt == SVSB200_U8;
     // rows wider than about 9 000 elements need more than the default 48 KB of shared memory: the kernel opts in
-    return dispatch(DataRows{}, rowt, [&](auto t) {
-        return dispatch(RescoreOps<decltype(t)::value>{}, op, [&](auto o) {
-            const LaunchConfig cfg{int(nq), 1, flat_rescore_smem<decltype(o)::value>(p.qstride), stream};
-            return launch_kernel(flat_rescore_kernel<decltype(t)::value, decltype(o)::value>, cfg, nq,
-                                 cfg.smem_bytes > 48 * 1024, p, rp);
+    return dispatch(IntList<FLAT_KC, FLAT_KC_DEEP>{}, kc, [&](auto c) {
+        return dispatch(DataRows{}, rowt, [&](auto t) {
+            return dispatch(RescoreOps<decltype(t)::value>{}, op, [&](auto o) {
+                const LaunchConfig cfg{int(nq), 1, flat_rescore_smem<decltype(o)::value>(p.qstride), stream};
+                return launch_kernel(flat_rescore_kernel<decltype(t)::value, decltype(o)::value, decltype(c)::value>, cfg,
+                                     nq, cfg.smem_bytes > 48 * 1024, p, rp);
+            });
         });
     });
 }
@@ -904,15 +993,22 @@ static cudaError_t flat_move_rows(const void* src, void* dst, const uint32_t* id
     return cudaGetLastError();
 }
 
+// The deep lists of one query tile keep at most FLAT_CMAX / FLAT_KC_DEEP = 7 CTAs busy: batches of one or two tiles
+// run faster on the scan (DESIGN.md §9b), so the deep lists need more than 2 FLAT_BM queries.
+static bool flat_deep_batch(size_t nq) { return nq > 2 * FLAT_BM; }
+
 // Shared body of the tensor-core flat search: device buffers in, device buffers out, enqueued on sc->stream except
-// for one synchronisation (the count of queries that need the exact-scan fallback).
+// for one synchronisation (the count of queries that need the exact-scan fallback).  `max_kc` is the deepest list the
+// caller allows: k + 8 <= FLAT_KC runs the FLAT_KC lists, k + 8 <= FLAT_KC_DEEP (Flat handle only) the deep ones.
 static int flat_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, const void* d_queries, int qdtype, size_t nq, size_t k,
-                          uint64_t* d_out_ids, float* d_out_dists, uint32_t* fallback_queries) {
+                          uint64_t* d_out_ids, float* d_out_dists, uint32_t* fallback_queries, uint32_t max_kc) {
     if (fallback_queries) *fallback_queries = 0;
     if (nq == 0) return 0;
     cudaStream_t stream = sc->stream;
     const bool int_data = ix->dtype == SVSB200_I8 || ix->dtype == SVSB200_U8;
-    const bool shape_ok = ix->storage == SVSB200_PLAIN && ix->metric != SVSB200_COSINE && k + 8 <= FLAT_KC && ix->n >= 512;
+    const uint32_t kc = k + 8 <= FLAT_KC ? FLAT_KC : FLAT_KC_DEEP;
+    const bool shape_ok = ix->storage == SVSB200_PLAIN && ix->metric != SVSB200_COSINE && k + 8 <= max_kc && ix->n >= 512 &&
+                          (kc == FLAT_KC || flat_deep_batch(nq));
     // the integer GEMM: (int8, int8) / (uint8, uint8), every int32 sum exact
     const bool int_gemm = shape_ok && int_data && qdtype == ix->dtype && ix->dim <= FLAT_INT_MAX_DIM &&
                           flat_rescore_smem<OP_L2I>(query_stride(ix->dim)) <= kSmemOptInMax;
@@ -950,24 +1046,24 @@ static int flat_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, const vo
     }
     // one CTA per SM over equal runs of output tiles; `nsplit` = candidate lists per query (flat_plan)
     uint32_t flat_ctas = 1, flat_share = 1, nsplit = 2;
-    flat_plan(mtiles, ntiles, uint32_t(rep->sm_count), &flat_ctas, &flat_share, &nsplit);
+    flat_plan(mtiles, ntiles, uint32_t(rep->sm_count), kc, &flat_ctas, &flat_share, &nsplit);
     const size_t qrow = size_t(dim) * esize(qdtype);
     CUDA_TRY(sc->flat_a.ensure(size_t(mtiles) * 128 * KB * 32 * 2));
     CUDA_TRY(sc->flat_qnorm.ensure(size_t(mtiles) * 128));
-    CUDA_TRY(sc->flat_ckey.ensure(size_t(mtiles) * 128 * nsplit * FLAT_KC));
-    CUDA_TRY(sc->flat_cid.ensure(size_t(mtiles) * 128 * nsplit * FLAT_KC));
+    CUDA_TRY(sc->flat_ckey.ensure(size_t(mtiles) * 128 * nsplit * kc));
+    CUDA_TRY(sc->flat_cid.ensure(size_t(mtiles) * 128 * nsplit * kc));
     CUDA_TRY(sc->flat_unv.ensure(nq + 1));
     CUDA_TRY(sc->flat_progress.ensure(flat_ctas));
     CUDA_TRY(cudaMemsetAsync(sc->flat_progress.ptr, 0, size_t(flat_ctas) * 4, stream));
     if (int_gemm) {
         CUDA_TRY(flat_tile_rows8(qdtype, d_queries, uint32_t(qrow), uint32_t(nq), dim, 128, 0, sc->flat_a.ptr, nullptr, stream));
-        CUDA_TRY(flat_gemm_topk(ix->dtype == SVSB200_I8 ? FLAT_S8 : FLAT_U8, sc->flat_a.ptr, rep->flat_b8.ptr, rep->flat_bias8.ptr, KB,
+        CUDA_TRY(flat_gemm_topk(ix->dtype == SVSB200_I8 ? FLAT_S8 : FLAT_U8, kc, sc->flat_a.ptr, rep->flat_b8.ptr, rep->flat_bias8.ptr, KB,
                                 ntiles, mtiles, flat_ctas, flat_share, nsplit, l2 ? -2.0f : -1.0f, sc->flat_ckey.ptr, sc->flat_cid.ptr,
                                 sc->flat_progress.ptr, stream));
     } else {
         CUDA_TRY(flat_tile_rows(qdtype, d_queries, uint32_t(qrow), uint32_t(nq), dim, 128, 1.0f, 0, sc->flat_a.ptr, nullptr,
                                 sc->flat_qnorm.ptr, nullptr, stream));
-        CUDA_TRY(flat_gemm_topk(FLAT_F16, sc->flat_a.ptr, rep->flat_b.ptr, rep->flat_bias.ptr, KB, ntiles, mtiles, flat_ctas, flat_share,
+        CUDA_TRY(flat_gemm_topk(FLAT_F16, kc, sc->flat_a.ptr, rep->flat_b.ptr, rep->flat_bias.ptr, KB, ntiles, mtiles, flat_ctas, flat_share,
                                 nsplit, l2 ? -2.0f : -1.0f, sc->flat_ckey.ptr, sc->flat_cid.ptr, sc->flat_progress.ptr, stream));
     }
     // exact re-scoring with the search path's distance code: prepared queries as for a search
@@ -988,7 +1084,7 @@ static int flat_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, const vo
     // rounding terms of E(q) (file header, fp16 path): float32 queries and float32 data are rounded to fp16
     p.scale = (qdtype == SVSB200_F32 ? 1.0f : 0.0f) + (ix->dtype == SVSB200_F32 ? 1.0f : 0.0f);   // number of rounded operands
     const int op = int_gemm ? (l2 ? OP_L2I : OP_IPI) : (l2 ? OP_L2F : OP_IPF);
-    CUDA_TRY(flat_rescore(ix->dtype, op, p, sc->flat_ckey.ptr, sc->flat_cid.ptr, nsplit, uint32_t(nq), uint32_t(k),
+    CUDA_TRY(flat_rescore(ix->dtype, op, kc, p, sc->flat_ckey.ptr, sc->flat_cid.ptr, nsplit, uint32_t(nq), uint32_t(k),
                           sc->flat_qnorm.ptr, rep->flat_xmax.ptr, d_out_ids, d_out_dists, sc->flat_unv.ptr + 1, sc->flat_unv.ptr, stream));
     // queries whose bound did not verify: exact scan, results scattered over the rescored rows
     uint32_t nunv = 0;
@@ -1010,14 +1106,14 @@ static int flat_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, const vo
 
 // Blocking form on host buffers, on a scratch set of the pool.
 static int flat_search_host(svsb200_index* ix, Replica* rep, Scratch* sc, const void* queries, int qdtype, size_t nq, size_t k,
-                            uint64_t* out_ids, float* out_dists) {
+                            uint64_t* out_ids, float* out_dists, uint32_t max_kc) {
     const size_t qbytes = nq * ix->dim * esize(qdtype);
     CUDA_TRY(sc->q_raw.ensure(qbytes));
     CUDA_TRY(sc->ids.ensure(nq * k * 8));
     CUDA_TRY(sc->dists.ensure(nq * k));
     CUDA_TRY(cudaMemcpyAsync(sc->q_raw.ptr, queries, qbytes, cudaMemcpyHostToDevice, sc->stream));
     int rc = flat_on_device(ix, rep, sc, sc->q_raw.ptr, qdtype, nq, k, reinterpret_cast<uint64_t*>(sc->ids.ptr), sc->dists.ptr,
-                            nullptr);
+                            nullptr, max_kc);
     if (rc) return rc;
     CUDA_TRY(cudaMemcpyAsync(out_ids, sc->ids.ptr, nq * k * 8, cudaMemcpyDeviceToHost, sc->stream));
     CUDA_TRY(cudaMemcpyAsync(out_dists, sc->dists.ptr, nq * k * 4, cudaMemcpyDeviceToHost, sc->stream));
@@ -1025,7 +1121,26 @@ static int flat_search_host(svsb200_index* ix, Replica* rep, Scratch* sc, const 
     return 0;
 }
 
+// The plan of flat_on_device for k and a device of `sm_count` SMs (svsb200_flat_plan / svsb200_flat_plan_k).
+static void flat_plan_rows(size_t nq, size_t n, uint32_t kc, int sm_count, uint32_t* ctas, uint32_t* share,
+                           uint32_t* lists_per_query, uint64_t* segment_begin) {
+    const uint32_t mtiles = uint32_t((nq + FLAT_BM - 1) / FLAT_BM), ntiles = uint32_t((n + FLAT_BN - 1) / FLAT_BN);
+    flat_plan(mtiles, ntiles, uint32_t(sm_count), kc, ctas, share, lists_per_query);
+    if (segment_begin) {
+        const uint32_t nseg = *ctas / *share, ngroups = (mtiles + *share - 1) / *share;
+        const uint64_t total = uint64_t(ngroups) * ntiles;
+        for (uint32_t b = 0; b <= nseg; ++b) segment_begin[b] = flat_seg_begin(total, nseg, b);
+    }
+}
+
 }  // namespace svsb200
+
+// A flat index: the rows of an svsb200_index on one device, with no adjacency.  The exact scan walks the rows in blocks
+// of deg_pad = round_up(gstride, 32) candidates and reads nothing else of the graph (search_kernel.cuh, EXH); the
+// block is 32 rows, as for a Vamana index of degree <= 32.
+struct svsb200_flat {
+    std::unique_ptr<svsb200_index> ix;
+};
 
 using namespace svsb200;
 
@@ -1038,13 +1153,22 @@ int svsb200_flat_plan(size_t nq, size_t n, int sm_count, uint32_t* ctas, uint32_
     if (nq == 0 || n == 0 || sm_count <= 0 || !ctas || !share || !lists_per_query)
         return fail("svsb200_flat_plan: nq, n, sm_count must be positive and the outputs non-NULL");
     if (nq > (size_t(1) << 31) || n > (size_t(1) << 31)) return fail("svsb200_flat_plan: problem too large");
-    const uint32_t mtiles = uint32_t((nq + FLAT_BM - 1) / FLAT_BM), ntiles = uint32_t((n + FLAT_BN - 1) / FLAT_BN);
-    flat_plan(mtiles, ntiles, uint32_t(sm_count), ctas, share, lists_per_query);
-    if (segment_begin) {
-        const uint32_t nseg = *ctas / *share, ngroups = (mtiles + *share - 1) / *share;
-        const uint64_t total = uint64_t(ngroups) * ntiles;
-        for (uint32_t b = 0; b <= nseg; ++b) segment_begin[b] = flat_seg_begin(total, nseg, b);
+    flat_plan_rows(nq, n, FLAT_KC, sm_count, ctas, share, lists_per_query, segment_begin);
+    return 0;
+}
+
+int svsb200_flat_plan_k(size_t nq, size_t n, size_t k, int sm_count, uint32_t* ctas, uint32_t* share, uint32_t* lists_per_query,
+                        uint32_t* list_entries, uint64_t* segment_begin) {
+    if (nq == 0 || n == 0 || sm_count <= 0 || !ctas || !share || !lists_per_query || !list_entries)
+        return fail("svsb200_flat_plan_k: nq, n, sm_count must be positive and the outputs non-NULL");
+    if (k == 0 || k + 8 > FLAT_KC_DEEP) return fail("svsb200_flat_plan_k: k must be in [1, 121]");
+    if (nq > (size_t(1) << 31) || n > (size_t(1) << 31)) return fail("svsb200_flat_plan_k: problem too large");
+    *list_entries = k + 8 <= FLAT_KC ? FLAT_KC : FLAT_KC_DEEP;
+    if (*list_entries == FLAT_KC_DEEP && !flat_deep_batch(nq)) {   // the scan route: no GEMM
+        *ctas = *share = *lists_per_query = *list_entries = 0;
+        return 0;
     }
+    flat_plan_rows(nq, n, *list_entries, sm_count, ctas, share, lists_per_query, segment_begin);
     return 0;
 }
 
@@ -1061,7 +1185,7 @@ int svsb200_flat_search_device(svsb200_index* ix, const void* d_queries, int qdt
     std::string err;
     Scratch* sc = scratch_for_stream(rep, static_cast<cudaStream_t>(stream_), &err);
     if (!sc) return fail(err);
-    return flat_on_device(ix, rep, sc, d_queries, qdtype, nq, k, d_out_ids, d_out_dists, fallback_queries);
+    return flat_on_device(ix, rep, sc, d_queries, qdtype, nq, k, d_out_ids, d_out_dists, fallback_queries, FLAT_KC);
 }
 
 int svsb200_flat_search(svsb200_index* ix, const void* queries, int qdtype, size_t nq, size_t k, uint64_t* out_ids,
@@ -1077,7 +1201,88 @@ int svsb200_flat_search(svsb200_index* ix, const void* queries, int qdtype, size
     std::string err;
     Scratch* sc = acquire(rep, &err);
     if (!sc) return fail(err);
-    int rc = flat_search_host(ix, rep, sc, queries, qdtype, nq, k, out_ids, out_dists);
+    int rc = flat_search_host(ix, rep, sc, queries, qdtype, nq, k, out_ids, out_dists, FLAT_KC);
+    release(rep, sc);
+    return rc;
+}
+
+int svsb200_flat_index_create(const void* vectors, int dtype, size_t n, size_t dim, size_t row_stride_bytes, int metric,
+                              int device, svsb200_flat** out) {
+    const char* who = "svsb200_flat_index_create";
+    if (!out) return fail("svsb200_flat_index_create: out is NULL");
+    *out = nullptr;
+    if (!vectors) return fail("svsb200_flat_index_create: NULL input");
+    if (dtype < SVSB200_F32 || dtype > SVSB200_U8) return fail("svsb200_flat_index_create: bad dtype");
+    if (metric < SVSB200_L2 || metric > SVSB200_COSINE) return fail("svsb200_flat_index_create: bad metric");
+    if (n == 0 || dim == 0) return fail("svsb200_flat_index_create: empty dataset");
+    if (n >= (size_t(1) << 31)) return fail("svsb200_flat_index_create: more than 2^31-1 vectors per index");
+    const size_t row_bytes = dim * esize(dtype);
+    if (row_stride_bytes && row_stride_bytes < row_bytes) return fail("svsb200_flat_index_create: row stride below the row size");
+    cudaDeviceProp prop;
+    if (int rc = check_device(who, device, &prop)) return rc;
+    auto flat = std::make_unique<svsb200_flat>();
+    flat->ix = std::make_unique<svsb200_index>();
+    svsb200_index* ix = flat->ix.get();
+    ix->dtype = dtype;
+    ix->metric = metric;
+    ix->storage = SVSB200_PLAIN;
+    ix->n = n;
+    ix->dim = dim;
+    ix->row_stride = data_row_stride(SVSB200_PLAIN, dtype, dim);
+    ix->gstride = 32;   // the scan's block of rows (struct svsb200_flat); there is no adjacency
+    ix->reps.push_back(std::make_unique<Replica>());
+    Replica* rep = ix->reps.back().get();
+    rep->device = device;
+    rep->sm_count = prop.multiProcessorCount;
+    CUDA_TRY(cudaSetDevice(device));
+    const size_t vbytes = n * size_t(ix->row_stride);
+    CUDA_TRY(rep->d_vectors.ensure(vbytes));
+    CUDA_TRY(cudaMemset(rep->d_vectors.ptr, 0, vbytes));
+    CUDA_TRY(cudaMemcpy2D(rep->d_vectors.ptr, ix->row_stride, vectors, row_stride_bytes ? row_stride_bytes : row_bytes, row_bytes,
+                          n, cudaMemcpyHostToDevice));
+    ix->device_bytes = vbytes;
+    *out = flat.release();
+    return 0;
+}
+
+int svsb200_flat_index_destroy(svsb200_flat* index) {
+    delete index;   // Replica / Scratch destructors release the device memory
+    return 0;
+}
+
+size_t svsb200_flat_index_size(const svsb200_flat* index) { return index ? index->ix->n : 0; }
+size_t svsb200_flat_index_dimensions(const svsb200_flat* index) { return index ? index->ix->dim : 0; }
+size_t svsb200_flat_index_device_bytes(const svsb200_flat* index) { return index ? index->ix->device_bytes : 0; }
+
+int svsb200_flat_index_search_device(svsb200_flat* index, const void* d_queries, int qdtype, size_t nq, size_t k,
+                                     uint64_t* d_out_ids, float* d_out_dists, void* stream_, uint32_t* fallback_queries) {
+    if (!index) return fail("svsb200_flat_index_search_device: NULL index");
+    if (nq && (!d_queries || !d_out_ids || !d_out_dists)) return fail("svsb200_flat_index_search_device: NULL buffer");
+    if (k == 0 || k > 1024) return fail("svsb200_flat_index_search_device: k must be in [1, 1024]");
+    if (qdtype < SVSB200_F32 || qdtype > SVSB200_U8) return fail("bad query dtype");
+    svsb200_index* ix = index->ix.get();
+    Replica* rep = ix->reps[0].get();
+    CUDA_TRY(cudaSetDevice(rep->device));
+    std::string err;
+    Scratch* sc = scratch_for_stream(rep, static_cast<cudaStream_t>(stream_), &err);
+    if (!sc) return fail(err);
+    return flat_on_device(ix, rep, sc, d_queries, qdtype, nq, k, d_out_ids, d_out_dists, fallback_queries, FLAT_KC_DEEP);
+}
+
+int svsb200_flat_index_search(svsb200_flat* index, const void* queries, int qdtype, size_t nq, size_t k, uint64_t* out_ids,
+                              float* out_dists) {
+    if (!index) return fail("svsb200_flat_index_search: NULL index");
+    if (k == 0 || k > 1024) return fail("svsb200_flat_index_search: k must be in [1, 1024]");
+    if (nq == 0) return 0;
+    if (!queries || !out_ids || !out_dists) return fail("svsb200_flat_index_search: NULL buffer");
+    if (qdtype < SVSB200_F32 || qdtype > SVSB200_U8) return fail("bad query dtype");
+    svsb200_index* ix = index->ix.get();
+    Replica* rep = ix->reps[0].get();
+    CUDA_TRY(cudaSetDevice(rep->device));
+    std::string err;
+    Scratch* sc = acquire(rep, &err);
+    if (!sc) return fail(err);
+    int rc = flat_search_host(ix, rep, sc, queries, qdtype, nq, k, out_ids, out_dists, FLAT_KC_DEEP);
     release(rep, sc);
     return rc;
 }
