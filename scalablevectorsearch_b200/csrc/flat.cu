@@ -106,8 +106,6 @@ __device__ __forceinline__ void bulk_copy_g2s(void* smem_dst, const void* gmem_s
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
-// keeps the compiler from moving reads of an accumulator register across the wait that completes it
-__device__ __forceinline__ void reg_fence(float& r) { asm volatile("" : "+f"(r)::"memory"); }
 // Warpgroup-MMA shared-memory matrix descriptor, K-major, no swizzle (layout type 0): 8x8-element core matrices of
 // 128 contiguous bytes; LBO = byte distance between the two 8-element k-chunks of one K=16 MMA, SBO = byte distance
 // between 8-row groups.
@@ -115,49 +113,17 @@ __device__ __forceinline__ uint64_t wgmma_desc(uint32_t smem_addr, uint32_t lbo_
     return uint64_t((smem_addr >> 4) & 0x3FFFu) | (uint64_t((lbo_bytes >> 4) & 0x3FFFu) << 16) |
            (uint64_t((sbo_bytes >> 4) & 0x3FFFu) << 32);
 }
-// D (64 x 256, fp32, in registers) [+]= A (64 x 16) . B (256 x 16)^T, both fp16 K-major in shared memory.
-__device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %130, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
-        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
-        "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
-        "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
-        "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
-        "%128, %129, p, 1, 1, 0, 0;\n\t"
-        "}\n"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
-          "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
-          "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
-          "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
-          "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
-          "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
-          "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
-          "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
-          "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
-        : "l"(adesc), "l"(bdesc), "r"(accumulate));
-}
-// D (64 x 256, int32, in registers) [+]= A (64 x 32) . B (256 x 32)^T, both int8 (KIND FLAT_S8) or uint8 (FLAT_U8)
-// K-major in shared memory: the same descriptors as the fp16 MMA, a core matrix being 8 rows x 16 one-byte elements.
-#define FLAT_WGMMA_INT(TYPE)                                                                                          \
+// D (64 x 256, in registers) [+]= A (64 x K) . B (256 x K)^T, both K-major in shared memory: fp16 with fp32
+// accumulation (m64n256k16), or int8 (KIND FLAT_S8) / uint8 (FLAT_U8) with int32 accumulation (m64n256k32) under the
+// same descriptors, a core matrix being 8 rows x 16 one-byte elements.  `C` is the accumulator's register constraint;
+// the fp16 form adds its scale and transpose operands.
+#define FLAT_D8(C, i) C(d[i]), C(d[i + 1]), C(d[i + 2]), C(d[i + 3]), C(d[i + 4]), C(d[i + 5]), C(d[i + 6]), C(d[i + 7])
+#define FLAT_WGMMA(SHAPE, C, TAIL)                                                                                    \
     asm volatile(                                                                                                     \
         "{\n\t"                                                                                                       \
         ".reg .pred p;\n\t"                                                                                           \
         "setp.ne.b32 p, %130, 0;\n\t"                                                                                 \
-        "wgmma.mma_async.sync.aligned.m64n256k32.s32." TYPE "." TYPE " "                                              \
+        "wgmma.mma_async.sync.aligned." SHAPE " "                                                                     \
         "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "                                     \
         "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "                            \
         "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "                            \
@@ -166,32 +132,22 @@ __device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t adesc
         "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "                            \
         "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "                 \
         "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "           \
-        "%128, %129, p;\n\t"                                                                                          \
+        "%128, %129, p" TAIL ";\n\t"                                                                                  \
         "}\n"                                                                                                         \
-        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),             \
-          "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),       \
-          "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),     \
-          "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]),     \
-          "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]),     \
-          "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]),     \
-          "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]),     \
-          "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63]),     \
-          "+r"(d[64]), "+r"(d[65]), "+r"(d[66]), "+r"(d[67]), "+r"(d[68]), "+r"(d[69]), "+r"(d[70]), "+r"(d[71]),     \
-          "+r"(d[72]), "+r"(d[73]), "+r"(d[74]), "+r"(d[75]), "+r"(d[76]), "+r"(d[77]), "+r"(d[78]), "+r"(d[79]),     \
-          "+r"(d[80]), "+r"(d[81]), "+r"(d[82]), "+r"(d[83]), "+r"(d[84]), "+r"(d[85]), "+r"(d[86]), "+r"(d[87]),     \
-          "+r"(d[88]), "+r"(d[89]), "+r"(d[90]), "+r"(d[91]), "+r"(d[92]), "+r"(d[93]), "+r"(d[94]), "+r"(d[95]),     \
-          "+r"(d[96]), "+r"(d[97]), "+r"(d[98]), "+r"(d[99]), "+r"(d[100]), "+r"(d[101]), "+r"(d[102]), "+r"(d[103]), \
-          "+r"(d[104]), "+r"(d[105]), "+r"(d[106]), "+r"(d[107]), "+r"(d[108]), "+r"(d[109]), "+r"(d[110]),           \
-          "+r"(d[111]), "+r"(d[112]), "+r"(d[113]), "+r"(d[114]), "+r"(d[115]), "+r"(d[116]), "+r"(d[117]),           \
-          "+r"(d[118]), "+r"(d[119]), "+r"(d[120]), "+r"(d[121]), "+r"(d[122]), "+r"(d[123]), "+r"(d[124]),           \
-          "+r"(d[125]), "+r"(d[126]), "+r"(d[127])                                                                    \
+        : FLAT_D8(C, 0), FLAT_D8(C, 8), FLAT_D8(C, 16), FLAT_D8(C, 24), FLAT_D8(C, 32), FLAT_D8(C, 40),               \
+          FLAT_D8(C, 48), FLAT_D8(C, 56), FLAT_D8(C, 64), FLAT_D8(C, 72), FLAT_D8(C, 80), FLAT_D8(C, 88),             \
+          FLAT_D8(C, 96), FLAT_D8(C, 104), FLAT_D8(C, 112), FLAT_D8(C, 120)                                           \
         : "l"(adesc), "l"(bdesc), "r"(accumulate))
-template <int KIND>
-__device__ __forceinline__ void wgmma_m64n256k32(int (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
-    if constexpr (KIND == FLAT_S8) FLAT_WGMMA_INT("s8");
-    else FLAT_WGMMA_INT("u8");
+template <int KIND, typename T>
+__device__ __forceinline__ void wgmma_m64n256(T (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    if constexpr (KIND == FLAT_F16) FLAT_WGMMA("m64n256k16.f32.f16.f16", "+f", ", 1, 1, 0, 0");
+    else if constexpr (KIND == FLAT_S8) FLAT_WGMMA("m64n256k32.s32.s8.s8", "+r", "");
+    else FLAT_WGMMA("m64n256k32.s32.u8.u8", "+r", "");
 }
-#undef FLAT_WGMMA_INT
+#undef FLAT_WGMMA
+#undef FLAT_D8
+// keeps the compiler from moving reads of an accumulator register across the wait that completes it
+__device__ __forceinline__ void reg_fence(float& r) { asm volatile("" : "+f"(r)::"memory"); }
 __device__ __forceinline__ void reg_fence(int& r) { asm volatile("" : "+r"(r)::"memory"); }
 // Per-query list of the KC smallest keys: shared memory, [query row][KC] with KC odd, so that a warp reading one row
 // side by side is bank-conflict free.  Keys are stored as order-preserving unsigned integers (REDUX.MAX works on them);
@@ -207,115 +163,58 @@ __device__ __forceinline__ uint32_t flat_ord(float f) {
 __device__ __forceinline__ float flat_unord(uint32_t o) {
     return __uint_as_float(o ^ ((o >> 31) ? 0x80000000u : 0xFFFFFFFFu));
 }
-// The whole warp updates the list of row `list_row` with (key, id); returns the row's new threshold (warp-uniform).
-template <uint32_t KC>
-__device__ __forceinline__ float flat_list_replace_max(uint32_t* lkey, uint32_t* lid, uint32_t list_row, uint32_t lane,
-                                                      float key, uint32_t id) {
-    uint32_t* rk = lkey + list_row * KC;
-    if constexpr (KC <= 64) {
-        uint32_t v0 = rk[lane];
-        uint32_t v1 = lane + 32 < KC ? rk[lane + 32] : 0u;
-        const uint32_t mx = __reduce_max_sync(0xFFFFFFFFu, max(v0, v1));
-        const uint32_t in0 = __ballot_sync(0xFFFFFFFFu, v0 == mx);
-        const uint32_t in1 = __ballot_sync(0xFFFFFFFFu, v1 == mx && lane + 32 < KC);
-        const uint32_t slot = in0 ? uint32_t(__ffs(int(in0)) - 1) : uint32_t(__ffs(int(in1)) + 31);
-        const uint32_t nk = flat_ord(key);
-        if (lane == (slot & 31u)) {
-            rk[slot] = nk;
-            lid[list_row * KC + slot] = id;
-            if (slot < 32) v0 = nk; else v1 = nk;
-        }
-        return flat_unord(__reduce_max_sync(0xFFFFFFFFu, max(v0, v1)));
-    } else {
-        constexpr uint32_t NW = (KC + 31) / 32;
-        uint32_t v[NW], m = 0;
-#pragma unroll
-        for (uint32_t w = 0; w < NW; ++w) {
-            v[w] = lane + 32 * w < KC ? rk[lane + 32 * w] : 0u;
-            m = max(m, v[w]);
-        }
-        const uint32_t mx = __reduce_max_sync(0xFFFFFFFFu, m);
-        uint32_t slot = 0;   // the first entry holding the maximum
-#pragma unroll
-        for (int w = int(NW) - 1; w >= 0; --w) {
-            const uint32_t in = __ballot_sync(0xFFFFFFFFu, v[w] == mx && lane + 32 * w < KC);
-            if (in) slot = 32 * w + uint32_t(__ffs(int(in)) - 1);
-        }
-        const uint32_t nk = flat_ord(key);
-        const bool mine = lane == (slot & 31u);
-        if (mine) {
-            rk[slot] = nk;
-            lid[list_row * KC + slot] = id;
-        }
-        m = 0;
-#pragma unroll
-        for (uint32_t w = 0; w < NW; ++w) m = max(m, mine && w == slot / 32 ? nk : v[w]);
-        return flat_unord(__reduce_max_sync(0xFFFFFFFFu, m));
-    }
-}
-// Integer lists are ordered by the pair (key, id).  The whole warp offers (okey, id) to the list of row `list_row`: it
-// replaces the list's largest pair if it is below it.  Returns the ordered key of the new largest pair -- the row's
-// threshold, warp-uniform: a pair can only be below the largest pair if its key does not exceed that key.  Keys are
-// uint32(K) ^ 0x80000000; an empty entry is (0xFFFFFFFF, 0xFFFFFFFF), above every real pair.
+// Integer lists are ordered by the pair (key, id); their keys are uint32(K) ^ 0x80000000 and an empty entry is
+// (0xFFFFFFFF, 0xFFFFFFFF), above every real pair.  flat_pair_max: the largest pair over the warp.
 __device__ __forceinline__ uint64_t flat_pair_max(uint64_t v) {
     const uint32_t hi = __reduce_max_sync(0xFFFFFFFFu, uint32_t(v >> 32));
     const uint32_t lo = __reduce_max_sync(0xFFFFFFFFu, uint32_t(v >> 32) == hi ? uint32_t(v) : 0u);
     return (uint64_t(hi) << 32) | lo;
 }
-template <uint32_t KC>
-__device__ __forceinline__ uint32_t flat_pair_offer(uint32_t* lkey, uint32_t* lid, uint32_t list_row, uint32_t lane,
+// The whole warp offers the ordered key `okey` with `id` to the list of row `list_row`; returns the ordered key of the
+// row's new largest entry -- its threshold, warp-uniform.  By key (fp16 lists, BY_PAIR = false): the caller offers only
+// keys below the threshold, and the key replaces the first entry holding the largest key.  By (key, id) pair (integer
+// lists): a pair not below the largest pair is rejected (an equal key with a larger id), otherwise it replaces the first
+// entry holding the largest pair; a pair can only be below the largest pair if its key does not exceed that key, so the
+// largest key is still the threshold.  Only the keys stay in registers: the ids are read where a key equals the largest.
+template <uint32_t KC, bool BY_PAIR>
+__device__ __forceinline__ uint32_t flat_list_offer(uint32_t* lkey, uint32_t* lid, uint32_t list_row, uint32_t lane,
                                                     uint32_t okey, uint32_t id) {
+    constexpr uint32_t NW = (KC + 31) / 32;
     uint32_t* rk = lkey + list_row * KC;
     uint32_t* ri = lid + list_row * KC;
-    if constexpr (KC <= 64) {
-        const bool has1 = lane + 32 < KC;
-        uint64_t v0 = (uint64_t(rk[lane]) << 32) | ri[lane];
-        uint64_t v1 = has1 ? (uint64_t(rk[lane + 32]) << 32) | ri[lane + 32] : 0u;
-        const uint64_t mx = flat_pair_max(max(v0, v1));
-        const uint64_t nv = (uint64_t(okey) << 32) | id;
-        if (nv >= mx) return uint32_t(mx >> 32);   // an equal key with a larger id
-        const uint32_t in0 = __ballot_sync(0xFFFFFFFFu, v0 == mx);
-        const uint32_t in1 = __ballot_sync(0xFFFFFFFFu, v1 == mx && has1);
-        const uint32_t slot = in0 ? uint32_t(__ffs(int(in0)) - 1) : uint32_t(__ffs(int(in1)) + 31);
-        if (lane == (slot & 31u)) {
-            rk[slot] = okey;
-            ri[slot] = id;
-            if (slot < 32) v0 = nv; else v1 = nv;
-        }
-        return __reduce_max_sync(0xFFFFFFFFu, uint32_t(max(v0, v1) >> 32));
-    } else {
-        // only the keys stay in registers (the ids are read again where a key equals the largest one)
-        constexpr uint32_t NW = (KC + 31) / 32;
-        uint32_t v[NW], m = 0;
+    uint32_t v[NW], m = 0;
 #pragma unroll
-        for (uint32_t w = 0; w < NW; ++w) {
-            v[w] = lane + 32 * w < KC ? rk[lane + 32 * w] : 0u;
-            m = max(m, v[w]);
-        }
-        const uint32_t hi = __reduce_max_sync(0xFFFFFFFFu, m);
-        uint32_t lo = 0;
+    for (uint32_t w = 0; w < NW; ++w) {
+        v[w] = lane + 32 * w < KC ? rk[lane + 32 * w] : 0u;
+        m = max(m, v[w]);
+    }
+    const uint32_t hi = __reduce_max_sync(0xFFFFFFFFu, m);
+    uint32_t lo = 0;   // (by pair) the largest id among the entries holding the largest key
+    bool take = true;  // (warp-uniform; a rejected pair leaves the list as it is -- no early return, which would make the
+                       // compiler guard every collective below against a divergent warp)
+    if constexpr (BY_PAIR) {
 #pragma unroll
         for (uint32_t w = 0; w < NW; ++w)
             if (lane + 32 * w < KC && v[w] == hi) lo = max(lo, ri[lane + 32 * w]);
         lo = __reduce_max_sync(0xFFFFFFFFu, lo);
-        const uint64_t mx = (uint64_t(hi) << 32) | lo;
-        if (((uint64_t(okey) << 32) | id) >= mx) return hi;   // an equal key with a larger id
-        uint32_t slot = 0;   // the first entry holding the largest pair
-#pragma unroll
-        for (int w = int(NW) - 1; w >= 0; --w) {
-            const uint32_t in = __ballot_sync(0xFFFFFFFFu, lane + 32 * w < KC && v[w] == hi && ri[lane + 32 * w] == lo);
-            if (in) slot = 32 * w + uint32_t(__ffs(int(in)) - 1);
-        }
-        const bool mine = lane == (slot & 31u);
-        if (mine) {
-            rk[slot] = okey;
-            ri[slot] = id;
-        }
-        m = 0;
-#pragma unroll
-        for (uint32_t w = 0; w < NW; ++w) m = max(m, mine && w == slot / 32 ? okey : v[w]);
-        return __reduce_max_sync(0xFFFFFFFFu, m);
+        take = ((uint64_t(okey) << 32) | id) < ((uint64_t(hi) << 32) | lo);
     }
+    uint32_t slot = 0;   // the first entry holding the largest key (pair)
+#pragma unroll
+    for (int w = int(NW) - 1; w >= 0; --w) {
+        const uint32_t in =
+            __ballot_sync(0xFFFFFFFFu, lane + 32 * w < KC && v[w] == hi && (!BY_PAIR || ri[lane + 32 * w] == lo));
+        if (in) slot = 32 * w + uint32_t(__ffs(int(in)) - 1);
+    }
+    const bool mine = take && lane == (slot & 31u);
+    if (mine) {
+        rk[slot] = okey;
+        ri[slot] = id;
+    }
+    m = 0;
+#pragma unroll
+    for (uint32_t w = 0; w < NW; ++w) m = max(m, mine && w == slot / 32 ? okey : v[w]);
+    return __reduce_max_sync(0xFFFFFFFFu, m);
 }
 
 struct FlatParams {
@@ -359,18 +258,36 @@ template <uint32_t KC> struct FlatShape {
     static constexpr uint32_t STAGES = KC == FLAT_KC ? FLAT_STAGES : 4;
     static constexpr size_t SMEM = size_t(STAGES) * FLAT_STAGE_BYTES + 2 * HALVES * size_t(KC) * FLAT_BM * 4 + 128;
     static_assert(SMEM <= kSmemOptInMax, "flat GEMM shared memory exceeds the 227 KB a block may use");
+    // index of the list of query row `row` for column half `half` (the deep lists: of `row`, both halves sharing it)
+    static __device__ __forceinline__ uint32_t list_row(uint32_t row, uint32_t half) {
+        return HALVES == 2 ? half * FLAT_BM + row : row;
+    }
 };
 template struct FlatShape<FLAT_KC>;
 template struct FlatShape<FLAT_KC_DEEP>;
 
-// Ordered key of an empty list entry, and the threshold of an empty list.
+// A key of the epilogue: float (fp16 GEMM) or the ordered key itself (integer GEMM), and its conversions to and from
+// the ordered keys the lists store.
+template <int KIND> using flat_key_t = std::conditional_t<KIND == FLAT_F16, float, uint32_t>;
+template <int KIND> __device__ __forceinline__ uint32_t flat_to_ord(flat_key_t<KIND> key) {
+    if constexpr (KIND == FLAT_F16) return flat_ord(key);
+    else return key;
+}
+template <int KIND> __device__ __forceinline__ flat_key_t<KIND> flat_from_ord(uint32_t o) {
+    if constexpr (KIND == FLAT_F16) return flat_unord(o);
+    else return o;
+}
+// Ordered key of an empty list entry (its flat_from_ord is the threshold of an empty list).
 template <int KIND> __device__ __forceinline__ uint32_t flat_empty_key() {
     if constexpr (KIND == FLAT_F16) return flat_ord(INFINITY);
     else return 0xFFFFFFFFu;
 }
-template <int KIND> __device__ __forceinline__ auto flat_no_threshold() {
-    if constexpr (KIND == FLAT_F16) return INFINITY;
-    else return 0xFFFFFFFFu;
+// Whether a key is offered to a list of threshold `thr`.  fp16: strictly below it, compared as float (the ordered
+// integers would order -0 / +0 and negative NaNs differently).  Integer: at or below it, the list comparing the ids --
+// but never the empty key, which padding rows (bias INT32_MAX, above every real key) have.
+template <int KIND> __device__ __forceinline__ bool flat_beats(flat_key_t<KIND> key, flat_key_t<KIND> thr) {
+    if constexpr (KIND == FLAT_F16) return key < thr;
+    else return key != 0xFFFFFFFFu && key <= thr;
 }
 
 // (The shape is named through the type alias `Shape` only: a kernel-local constant would make the compiler order the
@@ -467,15 +384,26 @@ __global__ void __launch_bounds__(FLAT_THREADS, 1) flat_gemm_topk_kernel(const _
 #pragma unroll
     for (uint32_t i = 0; i < 128; ++i) d[i] = acc_t(0);
     // [row i][list]: the largest key of that list (integer kinds: the ordered key of its largest (key, id) pair)
-    std::conditional_t<KIND == FLAT_F16, float, uint32_t> thr[2][Shape::HALVES];
-#pragma unroll
-    for (uint32_t i = 0; i < 2 * Shape::HALVES; ++i) thr[i / Shape::HALVES][i % Shape::HALVES] = flat_no_threshold<KIND>();
+    flat_key_t<KIND> thr[2][Shape::HALVES];
+    // Writes the lane's list out to (ok, oi) unless ok is NULL, and empties every list of the warp and its thresholds.
     // (deep lists: the two lanes of a row clear / write out alternate entries of its one list)
-    for (uint32_t e = Shape::HALVES == 2 ? 0u : fhalf; e < KC; e += 3 - Shape::HALVES) {
-        lkey[(Shape::HALVES == 2 ? fhalf * FLAT_BM + frow : frow) * KC + e] = flat_empty_key<KIND>();
-        lid[(Shape::HALVES == 2 ? fhalf * FLAT_BM + frow : frow) * KC + e] = 0xFFFFFFFFu;
-    }
-    __syncwarp();
+    auto reset_lists = [&](flat_key_t<KIND>* ok, uint32_t* oi) {
+        uint32_t* rk = lkey + Shape::list_row(frow, fhalf) * KC;
+        uint32_t* ri = lid + Shape::list_row(frow, fhalf) * KC;
+        for (uint32_t e = Shape::HALVES == 2 ? 0u : fhalf; e < KC; e += 3 - Shape::HALVES) {
+            if (ok) {
+                ok[e] = flat_from_ord<KIND>(rk[e]);
+                oi[e] = ri[e];
+            }
+            rk[e] = flat_empty_key<KIND>();
+            ri[e] = 0xFFFFFFFFu;
+        }
+        __syncwarp();
+#pragma unroll
+        for (uint32_t i = 0; i < 2 * Shape::HALVES; ++i)
+            thr[i / Shape::HALVES][i % Shape::HALVES] = flat_from_ord<KIND>(flat_empty_key<KIND>());
+    };
+    reset_lists(nullptr, nullptr);
     uint32_t s = 0, ph = 0, mtile = mtile0, nt = nt0;
     for (uint64_t t = t_lo; t < t_hi; ++t) {
         if (mtile >= fp.mtiles) {
@@ -498,8 +426,7 @@ __global__ void __launch_bounds__(FLAT_THREADS, 1) flat_gemm_topk_kernel(const _
                 // k-chunks 2j and 2j+1 of the blob: [kc][rows/8][8][16 bytes]
                 const uint64_t adesc = wgmma_desc(a_addr + 2 * j * (FLAT_BM * 16), FLAT_BM * 16, 128);
                 const uint64_t bdesc = wgmma_desc(b_addr + 2 * j * (FLAT_BN * 16), FLAT_BN * 16, 128);
-                if constexpr (KIND == FLAT_F16) wgmma_m64n256k16(d, adesc, bdesc, (kb | j) != 0 ? 1u : 0u);
-                else wgmma_m64n256k32<KIND>(d, adesc, bdesc, (kb | j) != 0 ? 1u : 0u);
+                wgmma_m64n256<KIND>(d, adesc, bdesc, (kb | j) != 0 ? 1u : 0u);
             }
             wgmma_commit();
             wgmma_wait<1>();
@@ -516,75 +443,37 @@ __global__ void __launch_bounds__(FLAT_THREADS, 1) flat_gemm_topk_kernel(const _
         if (lane == 0) mbar_arrive(empty + prev);
 
         // ---- epilogue: keys of the thread's 128 elements; only columns whose keys beat a row's threshold (rare once
-        // the lists have settled) are looked at key by key, the lanes with such a key served in turn by the whole warp ----
-        if constexpr (KIND == FLAT_F16) {
-            const float* bias = fp.b_bias + size_t(nt) * FLAT_BN + 2 * (lane & 3u);
+        // the lists have settled) are looked at key by key, the lanes with such a key served in turn by the whole warp.
+        // Integer kinds: exact int32 keys (wrapping arithmetic: the true key always fits), ordered as uint32 ----
+        const uint32_t* bias = reinterpret_cast<const uint32_t*>(fp.b_bias) + size_t(nt) * FLAT_BN + 2 * (lane & 3u);
 #pragma unroll
-            for (uint32_t c = 0; c < FLAT_BN / 8; ++c) {
-                const uint32_t h = Shape::HALVES == 2 ? c / (FLAT_BN / 16) : 0u;   // the list of this column
-                const float2 b2 = __ldg(reinterpret_cast<const float2*>(bias + 8 * c));
-                float key[4];
-                key[0] = fmaf(fp.key_scale, d[4 * c + 0], b2.x);
-                key[1] = fmaf(fp.key_scale, d[4 * c + 1], b2.y);
-                key[2] = fmaf(fp.key_scale, d[4 * c + 2], b2.x);
-                key[3] = fmaf(fp.key_scale, d[4 * c + 3], b2.y);
-                const bool any = fminf(key[0], key[1]) < thr[0][h] || fminf(key[2], key[3]) < thr[1][h];
-                if (!__any_sync(0xFFFFFFFFu, any)) continue;
-                uint32_t* my_key = lkey + size_t(h) * FLAT_BM * KC;
-                uint32_t* my_id = lid + size_t(h) * FLAT_BM * KC;
+        for (uint32_t c = 0; c < FLAT_BN / 8; ++c) {
+            const uint32_t h = Shape::HALVES == 2 ? c / (FLAT_BN / 16) : 0u;   // the list of this column
+            const uint2 b2 = __ldg(reinterpret_cast<const uint2*>(bias + 8 * c));
+            flat_key_t<KIND> key[4];
 #pragma unroll
-                for (uint32_t v = 0; v < 4; ++v) {
-                    const uint32_t i = v >> 1;
-                    bool pending = key[v] < thr[i][h];
-                    uint32_t hits = __ballot_sync(0xFFFFFFFFu, pending);
-                    while (hits) {
-                        const uint32_t src = uint32_t(__ffs(int(hits)) - 1);
-                        const float k_src = __shfl_sync(0xFFFFFFFFu, key[v], src);
-                        const uint32_t id = nt * FLAT_BN + 8 * c + 2 * (src & 3u) + (v & 1u);
-                        const float tnew = flat_list_replace_max<KC>(my_key, my_id, row0 - (lane >> 2) + (src >> 2) + 8 * i,
-                                                                     lane, k_src, id);
-                        if ((lane >> 2) == (src >> 2)) thr[i][h] = tnew;
-                        // another lane of the quad may hold a key of the same row that no longer beats the new threshold
-                        pending = pending && lane != src && key[v] < thr[i][h];
-                        hits = __ballot_sync(0xFFFFFFFFu, pending);
-                    }
-                }
+            for (uint32_t v = 0; v < 4; ++v) {
+                const uint32_t b = v & 1u ? b2.y : b2.x;
+                if constexpr (KIND == FLAT_F16) key[v] = fmaf(fp.key_scale, d[4 * c + v], __uint_as_float(b));
+                else key[v] = (b + uint32_t(int(fp.key_scale)) * uint32_t(d[4 * c + v])) ^ 0x80000000u;
             }
-        } else {
-            // exact int32 keys (wrapping arithmetic: the true key always fits), ordered as uint32; a column enters a list
-            // iff its (key, id) pair is below the list's largest pair.  Only the key of that pair is kept in registers:
-            // a column whose key equals it is offered, and the list compares the ids.  Padding rows (key INT32_MAX, above
-            // every real key) are never offered.
-            const uint32_t* bias = reinterpret_cast<const uint32_t*>(fp.b_bias) + size_t(nt) * FLAT_BN + 2 * (lane & 3u);
-            const uint32_t ks = uint32_t(int(fp.key_scale));
+            const bool any = flat_beats<KIND>(min(key[0], key[1]), thr[0][h]) || flat_beats<KIND>(min(key[2], key[3]), thr[1][h]);
+            if (!__any_sync(0xFFFFFFFFu, any)) continue;
 #pragma unroll
-            for (uint32_t c = 0; c < FLAT_BN / 8; ++c) {
-                const uint32_t h = Shape::HALVES == 2 ? c / (FLAT_BN / 16) : 0u;
-                const uint2 b2 = __ldg(reinterpret_cast<const uint2*>(bias + 8 * c));
-                uint32_t key[4];
-                key[0] = (b2.x + ks * uint32_t(d[4 * c + 0])) ^ 0x80000000u;
-                key[1] = (b2.y + ks * uint32_t(d[4 * c + 1])) ^ 0x80000000u;
-                key[2] = (b2.x + ks * uint32_t(d[4 * c + 2])) ^ 0x80000000u;
-                key[3] = (b2.y + ks * uint32_t(d[4 * c + 3])) ^ 0x80000000u;
-                const bool any = min(key[0], key[1]) <= thr[0][h] || min(key[2], key[3]) <= thr[1][h];
-                if (!__any_sync(0xFFFFFFFFu, any)) continue;
-                uint32_t* my_key = lkey + size_t(h) * FLAT_BM * KC;
-                uint32_t* my_id = lid + size_t(h) * FLAT_BM * KC;
-#pragma unroll
-                for (uint32_t v = 0; v < 4; ++v) {
-                    const uint32_t i = v >> 1;
-                    bool pending = key[v] != 0xFFFFFFFFu && key[v] <= thr[i][h];
-                    uint32_t hits = __ballot_sync(0xFFFFFFFFu, pending);
-                    while (hits) {
-                        const uint32_t src = uint32_t(__ffs(int(hits)) - 1);
-                        const uint32_t k_src = __shfl_sync(0xFFFFFFFFu, key[v], src);
-                        const uint32_t id = nt * FLAT_BN + 8 * c + 2 * (src & 3u) + (v & 1u);
-                        const uint32_t tnew = flat_pair_offer<KC>(my_key, my_id, row0 - (lane >> 2) + (src >> 2) + 8 * i, lane,
-                                                                  k_src, id);
-                        if ((lane >> 2) == (src >> 2)) thr[i][h] = tnew;
-                        pending = pending && lane != src && key[v] <= thr[i][h];
-                        hits = __ballot_sync(0xFFFFFFFFu, pending);
-                    }
+            for (uint32_t v = 0; v < 4; ++v) {
+                const uint32_t i = v >> 1;
+                bool pending = flat_beats<KIND>(key[v], thr[i][h]);
+                uint32_t hits = __ballot_sync(0xFFFFFFFFu, pending);
+                while (hits) {
+                    const uint32_t src = uint32_t(__ffs(int(hits)) - 1);
+                    const uint32_t o_src = flat_to_ord<KIND>(__shfl_sync(0xFFFFFFFFu, key[v], src));
+                    const uint32_t id = nt * FLAT_BN + 8 * c + 2 * (src & 3u) + (v & 1u);
+                    const uint32_t tnew = flat_list_offer<KC, KIND != FLAT_F16>(
+                        lkey, lid, Shape::list_row(row0 - (lane >> 2) + (src >> 2) + 8 * i, h), lane, o_src, id);
+                    if ((lane >> 2) == (src >> 2)) thr[i][h] = flat_from_ord<KIND>(tnew);
+                    // another lane of the quad may hold a key of the same row that no longer beats the new threshold
+                    pending = pending && lane != src && flat_beats<KIND>(key[v], thr[i][h]);
+                    hits = __ballot_sync(0xFFFFFFFFu, pending);
                 }
             }
         }
@@ -593,29 +482,28 @@ __global__ void __launch_bounds__(FLAT_THREADS, 1) flat_gemm_topk_kernel(const _
             const uint32_t piece = seg - flat_cta_of_tile(uint64_t(mtile / fp.share) * fp.ntiles, total, nseg);
             const size_t q = size_t(mtile) * FLAT_BM + frow;
             const size_t list = q * fp.nlists + piece * Shape::HALVES + (Shape::HALVES == 2 ? fhalf : 0u);
-            float* ok = fp.cand_key + list * KC;
-            uint32_t* oi = fp.cand_id + list * KC;
-            uint32_t* rk = lkey + (Shape::HALVES == 2 ? fhalf * FLAT_BM + frow : frow) * KC;
-            uint32_t* ri = lid + (Shape::HALVES == 2 ? fhalf * FLAT_BM + frow : frow) * KC;
+            // (the sync before a write-out is not in reset_lists: one ahead of the first reset makes the compiler stop
+            // proving the consumer warps converged, and the main loop loses the uniform datapath)
             __syncwarp();
-            for (uint32_t e = Shape::HALVES == 2 ? 0u : fhalf; e < KC; e += 3 - Shape::HALVES) {
-                if constexpr (KIND == FLAT_F16) ok[e] = flat_unord(rk[e]);
-                else reinterpret_cast<uint32_t*>(ok)[e] = rk[e];
-                oi[e] = ri[e];
-                rk[e] = flat_empty_key<KIND>();
-                ri[e] = 0xFFFFFFFFu;
-            }
-            __syncwarp();
-#pragma unroll
-            for (uint32_t i = 0; i < 2 * Shape::HALVES; ++i) thr[i / Shape::HALVES][i % Shape::HALVES] = flat_no_threshold<KIND>();
+            reset_lists(reinterpret_cast<flat_key_t<KIND>*>(fp.cand_key) + list * KC, fp.cand_id + list * KC);
             nt = 0;
             mtile += fp.share;
         }
     }
 }
 
-// ---- operand tiling: rows -> fp16 blobs in the canonical K-major layout of the warpgroup MMA ----------------------
-// element (row r, k e) of tile t = r / TR lives at  ((t*KB + e/32) * 4 + (e%32)/8) * TR*8 + ((r%TR)/8)*64 + (r%8)*8 + e%8
+// ---- operand tiling: rows -> blobs in the canonical K-major layout of the warpgroup MMA ---------------------------
+// K-blocks of a row: a blob holds FLAT_BK fp16 or FLAT_BK8 8-bit elements, FLAT_BK * 2 bytes of a row either way.
+__host__ __device__ inline uint32_t flat_kblocks(int kind, uint32_t dim) {
+    return kind == FLAT_F16 ? (dim + FLAT_BK - 1) / FLAT_BK : (dim + FLAT_BK8 - 1) / FLAT_BK8;
+}
+// Element (row r, k e) -- row rr = r % TR of tile t = r / TR of TR rows -- with E elements per 16 bytes (8 fp16, 16
+// 8-bit) and so 4E per blob: blob t*KB + e/(4E), 16-byte k-chunk (e%(4E))/E of it, 8-row group rr/8, row rr%8, element e%E.
+template <uint32_t E> __host__ __device__ inline size_t flat_blob_offset(uint32_t t, uint32_t rr, uint32_t e, uint32_t TR, uint32_t KB) {
+    return ((size_t(t) * KB + e / (4 * E)) * 4 + (e % (4 * E)) / E) * (size_t(TR) * E) + (rr / 8) * (8 * E) + (rr % 8) * E + e % E;
+}
+
+// rows -> fp16 blobs, with the bias, the row norms and their maximum (the error bound's ||q|| and Xmax)
 template <int SRCT>
 __global__ void flat_tile_kernel(const char* __restrict__ src, uint32_t row_stride, uint32_t n, uint32_t dim, uint32_t TR,
                                  uint32_t KB, float scale, int l2, __half* __restrict__ dst, float* __restrict__ bias,
@@ -647,8 +535,7 @@ __global__ void flat_tile_kernel(const char* __restrict__ src, uint32_t row_stri
         const float xr = __half2float(h) / scale;
         sq_rounded = fmaf(xr, xr, sq_rounded);
         sq_exact = fmaf(x, x, sq_exact);
-        const size_t o = ((size_t(t) * KB + e / 32) * 4 + (e % 32) / 8) * (size_t(TR) * 8) + (rr / 8) * 64 + (rr % 8) * 8 + e % 8;
-        dst[o] = h;
+        dst[flat_blob_offset<8>(t, rr, e, TR, KB)] = h;
     }
     if constexpr (SRCT == SVSB200_I8 || SRCT == SVSB200_U8) {
         for (int o = 16; o; o >>= 1) sq_int += __shfl_xor_sync(0xFFFFFFFFu, sq_int, o);
@@ -667,9 +554,7 @@ __global__ void flat_tile_kernel(const char* __restrict__ src, uint32_t row_stri
     }
 }
 
-// ---- operand tiling, 8-bit: int8 / uint8 rows -> blobs of their raw codes, 64-element k-blocks --------------------
-// element (row r, k e) of tile t = r / TR lives at  ((t*KB + e/64) * 4 + (e%64)/16) * TR*16 + ((r%TR)/8)*128 + (r%8)*16 + e%16
-// (a blob is as many bytes as an fp16 blob); zero padding adds nothing to any integer sum.  bias: |x|^2 (L2) / 0,
+// int8 / uint8 rows -> blobs of their raw codes; zero padding adds nothing to any integer sum.  bias: |x|^2 (L2) / 0,
 // INT32_MAX for padding rows (above every real key, so they never enter a list).
 template <int SRCT>
 __global__ void flat_tile8_kernel(const char* __restrict__ src, uint32_t row_stride, uint32_t n, uint32_t dim, uint32_t TR,
@@ -689,7 +574,7 @@ __global__ void flat_tile8_kernel(const char* __restrict__ src, uint32_t row_str
         const uint8_t c = row[e];
         const int v = SRCT == SVSB200_I8 ? int(int8_t(c)) : int(c);
         sq += v * v;
-        dst[((size_t(t) * KB + e / 64) * 4 + (e % 64) / 16) * (size_t(TR) * 16) + (rr / 8) * 128 + (rr % 8) * 16 + e % 16] = c;
+        dst[flat_blob_offset<16>(t, rr, e, TR, KB)] = c;
     }
     for (int o = 16; o; o >>= 1) sq += __shfl_xor_sync(0xFFFFFFFFu, sq, o);
     if (bias && lane == 0) bias[r] = l2 ? sq : 0;
@@ -862,32 +747,26 @@ __global__ void flat_move_rows_kernel(const char* __restrict__ src, char* __rest
 }
 
 // ---- launchers ------------------------------------------------------------------------------------------------------
-static cudaError_t flat_tile_rows(int srct, const void* src, uint32_t row_stride, uint32_t n, uint32_t dim, uint32_t tile_rows,
-                                  float scale, int l2, void* dst_tiles, float* bias, float* norms, unsigned int* max_norm_bits,
-                                  cudaStream_t stream) {
-    const uint32_t KB = (dim + FLAT_BK - 1) / FLAT_BK;
+// Rows -> the operand blobs of `kind`: flat_tile_kernel (fp16) or flat_tile8_kernel (8-bit, which has no norms).
+// `bias` (float, or int32 for 8-bit blobs), `norms` and `max_norm_bits` may be NULL.
+static cudaError_t flat_tile_rows(int kind, int srct, const void* src, uint32_t row_stride, uint32_t n, uint32_t dim,
+                                  uint32_t tile_rows, int l2, void* dst_tiles, void* bias, float* norms,
+                                  unsigned int* max_norm_bits, cudaStream_t stream) {
+    const uint32_t KB = flat_kblocks(kind, dim);
     const uint32_t rows_padded = (n + tile_rows - 1) / tile_rows * tile_rows;
     cudaError_t err = cudaMemsetAsync(dst_tiles, 0, size_t(rows_padded) * KB * FLAT_BK * 2, stream);
     if (err != cudaSuccess) return err;
     const LaunchConfig cfg{int((rows_padded + 7) / 8), 8, 0, stream};
-    return dispatch(DataRows{}, srct, [&](auto t) {
-        return launch_kernel(flat_tile_kernel<decltype(t)::value>, cfg, cfg.grid, false, static_cast<const char*>(src),
-                             row_stride, n, dim, tile_rows, KB, scale, l2, static_cast<__half*>(dst_tiles), bias, norms,
-                             max_norm_bits);
-    });
-}
-
-// int8 / uint8 rows -> 8-bit blobs (flat_tile8_kernel); `bias` may be NULL (query tiles).
-static cudaError_t flat_tile_rows8(int srct, const void* src, uint32_t row_stride, uint32_t n, uint32_t dim, uint32_t tile_rows,
-                                   int l2, void* dst_tiles, int* bias, cudaStream_t stream) {
-    const uint32_t KB = (dim + FLAT_BK8 - 1) / FLAT_BK8;
-    const uint32_t rows_padded = (n + tile_rows - 1) / tile_rows * tile_rows;
-    cudaError_t err = cudaMemsetAsync(dst_tiles, 0, size_t(rows_padded) * KB * FLAT_BK8, stream);
-    if (err != cudaSuccess) return err;
-    const LaunchConfig cfg{int((rows_padded + 7) / 8), 8, 0, stream};
+    const char* s = static_cast<const char*>(src);
+    if (kind == FLAT_F16)
+        return dispatch(DataRows{}, srct, [&](auto t) {
+            return launch_kernel(flat_tile_kernel<decltype(t)::value>, cfg, cfg.grid, false, s, row_stride, n, dim, tile_rows,
+                                 KB, 1.0f, l2, static_cast<__half*>(dst_tiles), static_cast<float*>(bias), norms,
+                                 max_norm_bits);
+        });
     return dispatch(IntList<SVSB200_I8, SVSB200_U8>{}, srct, [&](auto t) {
-        return launch_kernel(flat_tile8_kernel<decltype(t)::value>, cfg, cfg.grid, false, static_cast<const char*>(src),
-                             row_stride, n, dim, tile_rows, KB, l2, static_cast<uint8_t*>(dst_tiles), bias);
+        return launch_kernel(flat_tile8_kernel<decltype(t)::value>, cfg, cfg.grid, false, s, row_stride, n, dim, tile_rows, KB,
+                             l2, static_cast<uint8_t*>(dst_tiles), static_cast<int*>(bias));
     });
 }
 
@@ -997,6 +876,24 @@ static cudaError_t flat_move_rows(const void* src, void* dst, const uint32_t* id
 // run faster on the scan (DESIGN.md §9b), so the deep lists need more than 2 FLAT_BM queries.
 static bool flat_deep_batch(size_t nq) { return nq > 2 * FLAT_BM; }
 
+// The base tiles and bias of operand kind `kind` (and, for fp16 tiles, flat_xmax), built once per replica.
+static int ensure_flat_base(svsb200_index* ix, Replica* rep, int kind, cudaStream_t stream) {
+    Replica::FlatBase& base = kind == FLAT_F16 ? rep->flat_f16 : rep->flat_int;
+    std::lock_guard<std::mutex> lock(rep->mu);
+    if (base.tiles.ptr) return 0;
+    const uint32_t n = uint32_t(ix->n), dim = uint32_t(ix->dim), ntiles = (n + FLAT_BN - 1) / FLAT_BN;
+    CUDA_TRY(base.tiles.ensure(size_t(ntiles) * FLAT_BN * flat_kblocks(kind, dim) * FLAT_BK * 2));
+    CUDA_TRY(base.bias.ensure(size_t(ntiles) * FLAT_BN));
+    if (kind == FLAT_F16) {
+        CUDA_TRY(rep->flat_xmax.ensure(1));
+        CUDA_TRY(cudaMemsetAsync(rep->flat_xmax.ptr, 0, 4, stream));
+    }
+    CUDA_TRY(flat_tile_rows(kind, ix->dtype, rep->d_vectors.ptr, ix->row_stride, n, dim, FLAT_BN, ix->metric == SVSB200_L2,
+                            base.tiles.ptr, base.bias.ptr, nullptr, kind == FLAT_F16 ? rep->flat_xmax.ptr : nullptr, stream));
+    CUDA_TRY(cudaStreamSynchronize(stream));
+    return 0;
+}
+
 // Shared body of the tensor-core flat search: device buffers in, device buffers out, enqueued on sc->stream except
 // for one synchronisation (the count of queries that need the exact-scan fallback).  `max_kc` is the deepest list the
 // caller allows: k + 8 <= FLAT_KC runs the FLAT_KC lists, k + 8 <= FLAT_KC_DEEP (Flat handle only) the deep ones.
@@ -1021,29 +918,12 @@ static int flat_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, const vo
         return search_on_device(ix, rep, sc, d_queries, qdtype, nq, k, k, k, d_out_ids, 8, d_out_dists, stream, true);
     }
     const uint32_t n = uint32_t(ix->n), dim = uint32_t(ix->dim);
-    // k-blocks per row; a blob holds FLAT_BK fp16 or FLAT_BK8 8-bit elements, FLAT_BK * 2 bytes of a row either way
-    const uint32_t KB = int_gemm ? (dim + FLAT_BK8 - 1) / FLAT_BK8 : (dim + 31) / 32;
+    const int kind = !int_gemm ? FLAT_F16 : ix->dtype == SVSB200_I8 ? FLAT_S8 : FLAT_U8;
+    const uint32_t KB = flat_kblocks(kind, dim);
     const uint32_t ntiles = (n + 255) / 256, mtiles = uint32_t((nq + 127) / 128);
     const int l2 = ix->metric == SVSB200_L2;
-    {   // base tiles, once per replica and kind
-        std::lock_guard<std::mutex> lock(rep->mu);
-        if (int_gemm && !rep->flat_b8.ptr) {
-            CUDA_TRY(rep->flat_b8.ensure(size_t(ntiles) * 256 * KB * FLAT_BK8));
-            CUDA_TRY(rep->flat_bias8.ensure(size_t(ntiles) * 256));
-            CUDA_TRY(flat_tile_rows8(ix->dtype, rep->d_vectors.ptr, ix->row_stride, n, dim, 256, l2, rep->flat_b8.ptr,
-                                     rep->flat_bias8.ptr, stream));
-            CUDA_TRY(cudaStreamSynchronize(stream));
-        }
-        if (!int_gemm && !rep->flat_b.ptr) {
-            CUDA_TRY(rep->flat_b.ensure(size_t(ntiles) * 256 * KB * 32 * 2));
-            CUDA_TRY(rep->flat_bias.ensure(size_t(ntiles) * 256));
-            CUDA_TRY(rep->flat_xmax.ensure(1));
-            CUDA_TRY(cudaMemsetAsync(rep->flat_xmax.ptr, 0, 4, stream));
-            CUDA_TRY(flat_tile_rows(ix->dtype, rep->d_vectors.ptr, ix->row_stride, n, dim, 256, 1.0f, l2, rep->flat_b.ptr,
-                                    rep->flat_bias.ptr, nullptr, rep->flat_xmax.ptr, stream));
-            CUDA_TRY(cudaStreamSynchronize(stream));
-        }
-    }
+    if (int rc = ensure_flat_base(ix, rep, kind, stream)) return rc;
+    const Replica::FlatBase& base = kind == FLAT_F16 ? rep->flat_f16 : rep->flat_int;
     // one CTA per SM over equal runs of output tiles; `nsplit` = candidate lists per query (flat_plan)
     uint32_t flat_ctas = 1, flat_share = 1, nsplit = 2;
     flat_plan(mtiles, ntiles, uint32_t(rep->sm_count), kc, &flat_ctas, &flat_share, &nsplit);
@@ -1055,17 +935,11 @@ static int flat_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, const vo
     CUDA_TRY(sc->flat_unv.ensure(nq + 1));
     CUDA_TRY(sc->flat_progress.ensure(flat_ctas));
     CUDA_TRY(cudaMemsetAsync(sc->flat_progress.ptr, 0, size_t(flat_ctas) * 4, stream));
-    if (int_gemm) {
-        CUDA_TRY(flat_tile_rows8(qdtype, d_queries, uint32_t(qrow), uint32_t(nq), dim, 128, 0, sc->flat_a.ptr, nullptr, stream));
-        CUDA_TRY(flat_gemm_topk(ix->dtype == SVSB200_I8 ? FLAT_S8 : FLAT_U8, kc, sc->flat_a.ptr, rep->flat_b8.ptr, rep->flat_bias8.ptr, KB,
-                                ntiles, mtiles, flat_ctas, flat_share, nsplit, l2 ? -2.0f : -1.0f, sc->flat_ckey.ptr, sc->flat_cid.ptr,
-                                sc->flat_progress.ptr, stream));
-    } else {
-        CUDA_TRY(flat_tile_rows(qdtype, d_queries, uint32_t(qrow), uint32_t(nq), dim, 128, 1.0f, 0, sc->flat_a.ptr, nullptr,
-                                sc->flat_qnorm.ptr, nullptr, stream));
-        CUDA_TRY(flat_gemm_topk(FLAT_F16, kc, sc->flat_a.ptr, rep->flat_b.ptr, rep->flat_bias.ptr, KB, ntiles, mtiles, flat_ctas, flat_share,
-                                nsplit, l2 ? -2.0f : -1.0f, sc->flat_ckey.ptr, sc->flat_cid.ptr, sc->flat_progress.ptr, stream));
-    }
+    // (query norms: the fp16 path's error bound only)
+    CUDA_TRY(flat_tile_rows(kind, qdtype, d_queries, uint32_t(qrow), uint32_t(nq), dim, 128, 0, sc->flat_a.ptr, nullptr,
+                            kind == FLAT_F16 ? sc->flat_qnorm.ptr : nullptr, nullptr, stream));
+    CUDA_TRY(flat_gemm_topk(kind, kc, sc->flat_a.ptr, base.tiles.ptr, base.bias.ptr, KB, ntiles, mtiles, flat_ctas, flat_share, nsplit,
+                            l2 ? -2.0f : -1.0f, sc->flat_ckey.ptr, sc->flat_cid.ptr, sc->flat_progress.ptr, stream));
     // exact re-scoring with the search path's distance code: prepared queries as for a search
     if (int rc = prepare_queries(ix, rep, sc, d_queries, qdtype, nq, int_gemm ? PREP_INT : PREP_FLOAT, stream)) return rc;
     SearchParams p{};
@@ -1104,23 +978,6 @@ static int flat_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, const vo
     return 0;
 }
 
-// Blocking form on host buffers, on a scratch set of the pool.
-static int flat_search_host(svsb200_index* ix, Replica* rep, Scratch* sc, const void* queries, int qdtype, size_t nq, size_t k,
-                            uint64_t* out_ids, float* out_dists, uint32_t max_kc) {
-    const size_t qbytes = nq * ix->dim * esize(qdtype);
-    CUDA_TRY(sc->q_raw.ensure(qbytes));
-    CUDA_TRY(sc->ids.ensure(nq * k * 8));
-    CUDA_TRY(sc->dists.ensure(nq * k));
-    CUDA_TRY(cudaMemcpyAsync(sc->q_raw.ptr, queries, qbytes, cudaMemcpyHostToDevice, sc->stream));
-    int rc = flat_on_device(ix, rep, sc, sc->q_raw.ptr, qdtype, nq, k, reinterpret_cast<uint64_t*>(sc->ids.ptr), sc->dists.ptr,
-                            nullptr, max_kc);
-    if (rc) return rc;
-    CUDA_TRY(cudaMemcpyAsync(out_ids, sc->ids.ptr, nq * k * 8, cudaMemcpyDeviceToHost, sc->stream));
-    CUDA_TRY(cudaMemcpyAsync(out_dists, sc->dists.ptr, nq * k * 4, cudaMemcpyDeviceToHost, sc->stream));
-    CUDA_TRY(cudaStreamSynchronize(sc->stream));
-    return 0;
-}
-
 // The plan of flat_on_device for k and a device of `sm_count` SMs (svsb200_flat_plan / svsb200_flat_plan_k).
 static void flat_plan_rows(size_t nq, size_t n, uint32_t kc, int sm_count, uint32_t* ctas, uint32_t* share,
                            uint32_t* lists_per_query, uint64_t* segment_begin) {
@@ -1143,6 +1000,61 @@ struct svsb200_flat {
 };
 
 using namespace svsb200;
+
+// The two search bodies behind the four entry points: `who` names the entry point in errors, `max_kc` is its deepest
+// list (flat_on_device).  A Flat handle is never dynamic and lives on one device.
+
+// Enqueue-only form on device buffers, on the scratch bound to the caller's stream.
+static int flat_search_device(const char* who, svsb200_index* ix, const void* d_queries, int qdtype, size_t nq, size_t k,
+                              uint64_t* d_out_ids, float* d_out_dists, void* stream_, uint32_t* fallback_queries,
+                              uint32_t max_kc) {
+    const std::string w(who);
+    if (!ix) return fail(w + ": NULL index");
+    if (nq && (!d_queries || !d_out_ids || !d_out_dists)) return fail(w + ": NULL buffer");
+    if (k == 0 || k > 1024) return fail(w + ": k must be in [1, 1024]");
+    if (qdtype < SVSB200_F32 || qdtype > SVSB200_U8) return fail("bad query dtype");
+    if (ix->reps.size() != 1) return fail(w + ": the index must live on exactly one device");
+    if (ix->dynamic) return fail(w + ": flat search is not available on a dynamic index");
+    Replica* rep = ix->reps[0].get();
+    CUDA_TRY(cudaSetDevice(rep->device));
+    std::string err;
+    Scratch* sc = scratch_for_stream(rep, static_cast<cudaStream_t>(stream_), &err);
+    if (!sc) return fail(err);
+    return flat_on_device(ix, rep, sc, d_queries, qdtype, nq, k, d_out_ids, d_out_dists, fallback_queries, max_kc);
+}
+
+// Blocking form on host buffers, on a scratch set of the pool (the first replica's).
+static int flat_search_host(const char* who, svsb200_index* ix, const void* queries, int qdtype, size_t nq, size_t k,
+                            uint64_t* out_ids, float* out_dists, uint32_t max_kc) {
+    const std::string w(who);
+    if (!ix) return fail(w + ": NULL index");
+    if (k == 0 || k > 1024) return fail(w + ": k must be in [1, 1024]");
+    if (nq == 0) return 0;
+    if (!queries || !out_ids || !out_dists) return fail(w + ": NULL buffer");
+    if (qdtype < SVSB200_F32 || qdtype > SVSB200_U8) return fail("bad query dtype");
+    if (ix->dynamic) return fail(w + ": flat search is not available on a dynamic index");
+    Replica* rep = ix->reps[0].get();
+    CUDA_TRY(cudaSetDevice(rep->device));
+    std::string err;
+    Scratch* sc = acquire(rep, &err);
+    if (!sc) return fail(err);
+    const int rc = [&]() -> int {
+        const size_t qbytes = nq * ix->dim * esize(qdtype);
+        CUDA_TRY(sc->q_raw.ensure(qbytes));
+        CUDA_TRY(sc->ids.ensure(nq * k * 8));
+        CUDA_TRY(sc->dists.ensure(nq * k));
+        CUDA_TRY(cudaMemcpyAsync(sc->q_raw.ptr, queries, qbytes, cudaMemcpyHostToDevice, sc->stream));
+        if (int rc = flat_on_device(ix, rep, sc, sc->q_raw.ptr, qdtype, nq, k, reinterpret_cast<uint64_t*>(sc->ids.ptr),
+                                    sc->dists.ptr, nullptr, max_kc))
+            return rc;
+        CUDA_TRY(cudaMemcpyAsync(out_ids, sc->ids.ptr, nq * k * 8, cudaMemcpyDeviceToHost, sc->stream));
+        CUDA_TRY(cudaMemcpyAsync(out_dists, sc->dists.ptr, nq * k * 4, cudaMemcpyDeviceToHost, sc->stream));
+        CUDA_TRY(cudaStreamSynchronize(sc->stream));
+        return 0;
+    }();
+    release(rep, sc);
+    return rc;
+}
 
 extern "C" {
 
@@ -1174,36 +1086,14 @@ int svsb200_flat_plan_k(size_t nq, size_t n, size_t k, int sm_count, uint32_t* c
 
 int svsb200_flat_search_device(svsb200_index* ix, const void* d_queries, int qdtype, size_t nq, size_t k, uint64_t* d_out_ids,
                                float* d_out_dists, void* stream_, uint32_t* fallback_queries) {
-    if (!ix) return fail("svsb200_flat_search_device: NULL index");
-    if (nq && (!d_queries || !d_out_ids || !d_out_dists)) return fail("svsb200_flat_search_device: NULL buffer");
-    if (k == 0 || k > 1024) return fail("svsb200_flat_search_device: k must be in [1, 1024]");
-    if (qdtype < SVSB200_F32 || qdtype > SVSB200_U8) return fail("bad query dtype");
-    if (ix->reps.size() != 1) return fail("svsb200_flat_search_device: the index must live on exactly one device");
-    if (ix->dynamic) return fail("svsb200_flat_search_device: flat search is not available on a dynamic index");
-    Replica* rep = ix->reps[0].get();
-    CUDA_TRY(cudaSetDevice(rep->device));
-    std::string err;
-    Scratch* sc = scratch_for_stream(rep, static_cast<cudaStream_t>(stream_), &err);
-    if (!sc) return fail(err);
-    return flat_on_device(ix, rep, sc, d_queries, qdtype, nq, k, d_out_ids, d_out_dists, fallback_queries, FLAT_KC);
+    return flat_search_device("svsb200_flat_search_device", ix, d_queries, qdtype, nq, k, d_out_ids, d_out_dists, stream_,
+                              fallback_queries, FLAT_KC);
 }
 
 int svsb200_flat_search(svsb200_index* ix, const void* queries, int qdtype, size_t nq, size_t k, uint64_t* out_ids,
                         float* out_dists) {
-    if (!ix) return fail("svsb200_flat_search: NULL index");
-    if (nq == 0) return 0;
-    if (!queries || !out_ids || !out_dists) return fail("svsb200_flat_search: NULL buffer");
-    if (k == 0 || k > 1024) return fail("svsb200_flat_search: k must be in [1, 1024]");
-    if (qdtype < SVSB200_F32 || qdtype > SVSB200_U8) return fail("bad query dtype");
-    if (ix->dynamic) return fail("svsb200_flat_search: flat search is not available on a dynamic index");
-    Replica* rep = ix->reps[0].get();
-    CUDA_TRY(cudaSetDevice(rep->device));
-    std::string err;
-    Scratch* sc = acquire(rep, &err);
-    if (!sc) return fail(err);
-    int rc = flat_search_host(ix, rep, sc, queries, qdtype, nq, k, out_ids, out_dists, FLAT_KC);
-    release(rep, sc);
-    return rc;
+    if (ix && nq == 0) return 0;   // an empty batch succeeds whatever k (the Flat handle checks k first)
+    return flat_search_host("svsb200_flat_search", ix, queries, qdtype, nq, k, out_ids, out_dists, FLAT_KC);
 }
 
 int svsb200_flat_index_create(const void* vectors, int dtype, size_t n, size_t dim, size_t row_stride_bytes, int metric,
@@ -1256,35 +1146,14 @@ size_t svsb200_flat_index_device_bytes(const svsb200_flat* index) { return index
 
 int svsb200_flat_index_search_device(svsb200_flat* index, const void* d_queries, int qdtype, size_t nq, size_t k,
                                      uint64_t* d_out_ids, float* d_out_dists, void* stream_, uint32_t* fallback_queries) {
-    if (!index) return fail("svsb200_flat_index_search_device: NULL index");
-    if (nq && (!d_queries || !d_out_ids || !d_out_dists)) return fail("svsb200_flat_index_search_device: NULL buffer");
-    if (k == 0 || k > 1024) return fail("svsb200_flat_index_search_device: k must be in [1, 1024]");
-    if (qdtype < SVSB200_F32 || qdtype > SVSB200_U8) return fail("bad query dtype");
-    svsb200_index* ix = index->ix.get();
-    Replica* rep = ix->reps[0].get();
-    CUDA_TRY(cudaSetDevice(rep->device));
-    std::string err;
-    Scratch* sc = scratch_for_stream(rep, static_cast<cudaStream_t>(stream_), &err);
-    if (!sc) return fail(err);
-    return flat_on_device(ix, rep, sc, d_queries, qdtype, nq, k, d_out_ids, d_out_dists, fallback_queries, FLAT_KC_DEEP);
+    return flat_search_device("svsb200_flat_index_search_device", index ? index->ix.get() : nullptr, d_queries, qdtype, nq, k,
+                              d_out_ids, d_out_dists, stream_, fallback_queries, FLAT_KC_DEEP);
 }
 
 int svsb200_flat_index_search(svsb200_flat* index, const void* queries, int qdtype, size_t nq, size_t k, uint64_t* out_ids,
                               float* out_dists) {
-    if (!index) return fail("svsb200_flat_index_search: NULL index");
-    if (k == 0 || k > 1024) return fail("svsb200_flat_index_search: k must be in [1, 1024]");
-    if (nq == 0) return 0;
-    if (!queries || !out_ids || !out_dists) return fail("svsb200_flat_index_search: NULL buffer");
-    if (qdtype < SVSB200_F32 || qdtype > SVSB200_U8) return fail("bad query dtype");
-    svsb200_index* ix = index->ix.get();
-    Replica* rep = ix->reps[0].get();
-    CUDA_TRY(cudaSetDevice(rep->device));
-    std::string err;
-    Scratch* sc = acquire(rep, &err);
-    if (!sc) return fail(err);
-    int rc = flat_search_host(ix, rep, sc, queries, qdtype, nq, k, out_ids, out_dists, FLAT_KC_DEEP);
-    release(rep, sc);
-    return rc;
+    return flat_search_host("svsb200_flat_index_search", index ? index->ix.get() : nullptr, queries, qdtype, nq, k, out_ids,
+                            out_dists, FLAT_KC_DEEP);
 }
 
 }  // extern "C"

@@ -151,14 +151,15 @@ struct Replica {
     DeviceBuffer<uint32_t> d_entry;      // entry points when there are several
     DeviceBuffer<uint8_t> d_status;      // dynamic index: SlotStatus per slot
     DeviceBuffer<uint64_t> d_ext_ids;    // dynamic index: external id per slot
-    // tensor-core flat search: the base vectors as fp16 warpgroup-MMA tiles + per-row bias, built on first use
-    DeviceBuffer<unsigned char> flat_b;
-    DeviceBuffer<float> flat_bias;
-    DeviceBuffer<unsigned int> flat_xmax;
-    // ... and int8 / uint8 base vectors as 8-bit tiles for the integer GEMM + int32 bias (kept apart: one index can be
-    // searched with integer queries and with float32 queries)
-    DeviceBuffer<unsigned char> flat_b8;
-    DeviceBuffer<int> flat_bias8;
+    // tensor-core flat search: the base vectors as warpgroup-MMA tiles + per-row bias, built on first use, one set per
+    // operand kind (kept apart: one int8 / uint8 index can be searched with integer queries and with float32 queries)
+    struct FlatBase {
+        DeviceBuffer<unsigned char> tiles;
+        DeviceBuffer<float> bias;            // 8-bit tiles: int32 |x|^2
+    };
+    FlatBase flat_f16;                       // fp16 tiles
+    DeviceBuffer<unsigned int> flat_xmax;    // ... and the largest norm of their rows
+    FlatBase flat_int;                       // int8 / uint8 tiles of the integer GEMM
     std::mutex mu;
     std::vector<Scratch*> idle;                      // pool for the blocking API
     std::map<cudaStream_t, Scratch*> by_stream;      // one per caller stream for the enqueue-only API
