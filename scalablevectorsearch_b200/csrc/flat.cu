@@ -22,16 +22,29 @@
 //      Queries that fail the test (rare) are searched again with the exact scan kernel -- the result is exact
 //      in every case.
 //
-// Error bound: with q~, x~ the fp16-rounded operands (relative rounding 2^-11 per element; float16 inputs are
-// not rounded at all), r = the number of rounded operands (0..2):
-//   |q~.x~ - q.x| <= ||q~ - q|| ||x~|| + ||q|| ||x~ - x|| <= r 2^-11 ||q|| ||x|| (1 + 2^-11),
-// the products are exact in fp32 and the tensor-core accumulation of `dim` of them adds at most dim 2^-22 ||q|| ||x||;
-// for L2 the bias |x~|^2 differs from |x|^2 by at most 2^-10 ||x||^2 when the data was rounded.  So
-//   E_ip(q) = (r 2^-11 + dim 2^-22) ||q|| Xmax,      E_l2(q) = 2 E_ip(q) + [data rounded] 2^-10 Xmax^2.
+// Error bound, over the whole float32 range: q~, x~ are the fp16-rounded operands (float16 and integer inputs are not
+// rounded at all).  Per element, |fl16(v) - v| <= 2^-11 |v| + 2^-25: relative in fp16's normal range, absolute (half
+// the subnormal spacing 2^-24) below 2^-14.  So a rounded operand moves by
+//   dq = ||q~ - q|| <= 2^-11 ||q|| + 2^-25 sqrt(dim),   dx = ||x~ - x|| <= 2^-11 Xmax + 2^-25 sqrt(dim)
+// (0 for an operand that is not rounded), and ||q~|| <= ||q|| + dq, ||x~|| <= Xmax + dx.  Then
+//   |q~.x~ - q.x| <= ||q~ - q|| ||x~|| + ||q|| ||x~ - x|| <= dq (Xmax + dx) + ||q|| dx;
+// the products are exact in fp32 (fp16 x fp16, down to 2^-48) and the tensor-core accumulation of `dim` of them adds
+// at most dim 2^-22 ||q~|| ||x~||; for L2 the bias |x~|^2 differs from |x|^2 by at most ||x~ - x|| ||x~ + x|| <=
+// dx (2 Xmax + dx).  So
+//   E_ip(q) = dq (Xmax + dx) + ||q|| dx + dim 2^-22 (||q|| + dq)(Xmax + dx),
+//   E_l2(q) = 2 E_ip(q) + dx (2 Xmax + dx)   (+ the integer term below),
+// both times 1.0001 for the float32 norms.  The rescoring kernel rounds every operation of E and of kth + 2E upward, so
+// neither underflows nor falls below the true bound.  In fp16's normal range this is the relative bound
+// (r 2^-11 + dim 2^-22) ||q|| Xmax, r the number of rounded operands; for unit vectors at dim 96 the absolute term
+// 2^-25 sqrt(96) ~ 3e-7 is about 6e-4 of the 2^-11 one.  An element of magnitude >= 65520 rounds to +-inf: its
+// row's key becomes +-inf or NaN (NaN and +inf keys are never offered to a list), which no finite bound covers.  The
+// tile kernel gives such a row -- query or base -- the norm +inf (so Xmax = +inf), and a query whose ||q||, Xmax or E
+// is not finite is never verified: it runs on the exact scan.  tests/test_flat_bound_model.py checks the formula on a
+// numpy model of the lists and the certificate.
 // int8 / uint8 data with float32 queries takes this path too: integers up to 255 are exact in fp16, so only the query
-// is rounded (r = 1).  The bias is the exact integer |x|^2 converted once (at most 2^-24 Xmax^2 off), and the fp32 key
+// is rounded (dx = 0).  The bias is the exact integer |x|^2 converted once (at most 2^-24 Xmax^2 off), and the fp32 key
 // bias - 2 s~ is itself rounded once (2^-24 of |x|^2 + 2 |q| |x|), so integer data adds an explicit [integer data]
-// 2^-23 Xmax^2 to E_l2.  The 2^-23 |q| |x| part is NOT inside r 2^-11, which the query's rounding uses up: it is
+// 2^-23 Xmax^2 to E_l2.  The 2^-23 |q| |x| part is NOT inside dq Xmax, which the query's rounding uses up: it is
 // covered by the accumulation term, whose dim 2^-22 (doubled in E_l2) is twice the dim 2^-23 that a truncating fp32
 // accumulator can lose (four times round-to-nearest's); the spare dim 2^-22 >= 2^-23 holds it.  Tightening the dim
 // term below 2x would have to add 2^-23 |q| Xmax explicitly.  (The same margin holds the key rounding of float data.)
@@ -519,7 +532,8 @@ __global__ void flat_tile_kernel(const char* __restrict__ src, uint32_t row_stri
     const char* row = src + size_t(r) * row_stride;
     const uint32_t t = r / TR, rr = r % TR;
     float sq_rounded = 0.f, sq_exact = 0.f;
-    int sq_int = 0;   // integer rows: |x|^2, exact
+    int sq_int = 0;           // integer rows: |x|^2, exact
+    bool overflow = false;    // an element rounded to +-inf in fp16 (float rows only)
     for (uint32_t e = lane; e < dim; e += 32) {
         float x;
         if constexpr (SRCT == SVSB200_F32) {
@@ -532,6 +546,7 @@ __global__ void flat_tile_kernel(const char* __restrict__ src, uint32_t row_stri
             x = float(v);   // exact in fp16
         }
         const __half h = __float2half_rn(x * scale);
+        if constexpr (SRCT == SVSB200_F32) overflow |= bool(__hisinf(h));
         const float xr = __half2float(h) / scale;
         sq_rounded = fmaf(xr, xr, sq_rounded);
         sq_exact = fmaf(x, x, sq_exact);
@@ -546,9 +561,11 @@ __global__ void flat_tile_kernel(const char* __restrict__ src, uint32_t row_stri
             sq_exact += __shfl_xor_sync(0xFFFFFFFFu, sq_exact, o);
         }
     }
+    if constexpr (SRCT == SVSB200_F32) overflow = __any_sync(0xFFFFFFFFu, overflow);
     if (lane == 0) {
         if (bias) bias[r] = l2 ? sq_rounded : 0.f;
-        const float nrm = sqrtf(sq_exact) * 1.000001f;
+        // a row with an infinite fp16 element gets the norm +inf (and so Xmax = +inf): its queries never verify
+        const float nrm = overflow ? INFINITY : sqrtf(sq_exact) * 1.000001f;
         if (norms) norms[r] = nrm;
         if (max_norm_bits) atomicMax(max_norm_bits, __float_as_uint(nrm));
     }
@@ -724,14 +741,22 @@ __global__ void __launch_bounds__(32, 16) flat_rescore_kernel(const __grid_const
     }
     for (int o = 16; o; o >>= 1) kth_approx = fminf(kth_approx, __shfl_xor_sync(FULL, kth_approx, o));
     // |approximate key - key| <= E(q) (header): excluded rows are provably outside the exact top k iff T > kth + 2E
+    // Every operation of E and of kth + 2E rounds up, so neither can underflow or fall below the true bound.  A query or
+    // base with an element that overflowed fp16 has a norm of +inf (flat_tile_kernel) and is never verified.
     const float qn = rp.qnorm[q], xm = __uint_as_float(*rp.xmax_bits);
-    const float rounded = p.scale;   // operands that were rounded to fp16 (0, 1 or 2)
-    const float e_ip = (rounded * 4.8828125e-4f + float(p.dim) * 2.384185791015625e-7f) * qn * xm * 1.0001f;   // 2^-11 each, dim 2^-22
-    const float E = p.greater ? e_ip
-                              : 2.0f * e_ip + (rounded > 1.5f || rp.data_rounded ? 9.765625e-4f * xm * xm
-                                               : rp.data_int                      ? 1.1920929e-7f * xm * xm   // 2^-23 (header)
-                                                                                  : 0.0f);
-    const bool verified = C >= rp.k && T > kth_approx + 2.0f * E;
+    const int q_rounded = int(p.scale) - rp.data_rounded;   // p.scale: operands that were rounded to fp16 (0, 1 or 2)
+    const float sd = __fmul_ru(2.98023223876953125e-8f, __fsqrt_ru(float(p.dim)));            // 2^-25 sqrt(dim)
+    const float dq = q_rounded ? __fadd_ru(__fmul_ru(4.8828125e-4f, qn), sd) : 0.0f;          // ||q~ - q||
+    const float dx = rp.data_rounded ? __fadd_ru(__fmul_ru(4.8828125e-4f, xm), sd) : 0.0f;    // ||x~ - x||
+    const float qh = __fadd_ru(qn, dq), xh = __fadd_ru(xm, dx);                                // >= ||q~||, ||x~||
+    float E = __fadd_ru(__fadd_ru(__fmul_ru(dq, xh), __fmul_ru(qn, dx)),
+                        __fmul_ru(__fmul_ru(float(p.dim) * 2.384185791015625e-7f, qh), xh));   // E_ip, dim 2^-22
+    if (!p.greater)
+        E = __fadd_ru(__fadd_ru(__fmul_ru(2.0f, E), __fmul_ru(dx, __fadd_ru(xm, xh))),        // + ||x~|^2 - |x|^2|
+                      rp.data_int ? __fmul_ru(__fmul_ru(1.1920928955078125e-7f, xm), xm) : 0.0f);   // 2^-23 (header)
+    E = __fmul_ru(E, 1.0001f);
+    const bool finite = isfinite(qn) && isfinite(xm) && isfinite(E);
+    const bool verified = C >= rp.k && finite && T > __fadd_ru(kth_approx, __fmul_ru(2.0f, E));
     if (lane == 0 && !verified) rp.unverified[atomicAdd(rp.n_unverified, 1u)] = q;
 }
 
