@@ -7,8 +7,9 @@ Workload: bench.py's C2 data (synthetic 1M x 96 float32, L2, 10k queries, k = 10
 alpha 1.2).  DynamicVamana.build over the first 90 % of the rows, `add` of the last 10 % in calls of 10 000, deletion
 of a random 10 %, `consolidate`, `compact`.  Reported: points inserted per second (host clock around the blocking
 `add` calls), consolidate and compact milliseconds (host clock around each blocking call), recall@10 at window 128
-after every stage against exact ground truth over the live rows (the library's exact flat search), and the card's
-name and power limit read in the same run.  Nothing is written to disk.
+after every stage against exact ground truth over the live rows (a DynamicFlat, the library's exact flat index, mutated
+in step with the graph index, outside the timed calls), and the card's name and power limit read in the same run.
+Nothing is written to disk.
 """
 import json
 import os
@@ -25,19 +26,17 @@ C2 = dict(n=1_000_000, dim=96, nq=10_000, k=10, window=128, max_degree=64, build
 
 
 def main():
-    from scalablevectorsearch_b200 import DistanceType, DynamicVamana, SearchBufferConfig, Vamana, VamanaBuildParameters
+    from scalablevectorsearch_b200 import DistanceType, DynamicFlat, DynamicVamana, SearchBufferConfig, VamanaBuildParameters
     from scalablevectorsearch_b200.synthetic import clustered_unit_vectors
     w = C2
     base, queries = clustered_unit_vectors(w["n"], w["nq"], w["dim"])
     n, n0, k = w["n"], int(0.9 * w["n"]), w["k"]
-    live = np.zeros(n, dtype=bool)
+    # ground truth: the exact top k over the live rows, from a dynamic flat index given the same mutations
+    exact = DynamicFlat.build(base[:n0], np.arange(n0), DistanceType.L2)
 
     def recall(index):
-        """recall@k at window 128 against the exact top k over the live rows (the library's exact flat search)."""
-        rows = np.flatnonzero(live)
-        exact = Vamana.from_arrays(base[rows], np.zeros((len(rows), 2), dtype=np.uint32), 0, DistanceType.L2)
-        gt = rows[exact.flat_search(queries, k)[0].astype(np.int64)]
-        del exact
+        """recall@k at window 128 against the exact top k over the live rows."""
+        gt = exact.search(queries, k)[0].astype(np.int64)
         index.search_parameters.buffer_config = SearchBufferConfig(w["window"], w["window"])
         ids = index.search(queries, k)[0].astype(np.int64)
         return float(np.mean([len(set(a.tolist()) & set(b.tolist())) for a, b in zip(ids, gt)]) / k)
@@ -47,7 +46,6 @@ def main():
                                                       window_size=w["build_window"]), base[:n0], np.arange(n0),
                                 DistanceType.L2)
     build_s = time.time() - t0
-    live[:n0] = True
     rec = {"build": recall(index)}
     add_s = 0.0
     for lo in range(n0, n, 10_000):
@@ -55,19 +53,21 @@ def main():
         t0 = time.time()
         index.add(base[lo:hi], np.arange(lo, hi))
         add_s += time.time() - t0
-        live[lo:hi] = True
+        exact.add(base[lo:hi], np.arange(lo, hi))
     rec["add"] = recall(index)
     gone = np.random.default_rng(0).choice(n, n // 10, replace=False)
     index.delete(gone)
-    live[gone] = False
+    exact.delete(gone)
     rec["delete"] = recall(index)
     t0 = time.time()
     index.consolidate()
     consolidate_ms = (time.time() - t0) * 1e3
+    exact.consolidate()
     rec["consolidate"] = recall(index)
     t0 = time.time()
     index.compact()
     compact_ms = (time.time() - t0) * 1e3
+    exact.compact()
     rec["compact"] = recall(index)
     card = subprocess.run(["nvidia-smi", "--id=0", "--query-gpu=name,power.limit", "--format=csv,noheader"],
                           capture_output=True, text=True, timeout=30).stdout.strip() or None

@@ -397,6 +397,63 @@ int svsb200_dynamic_build(const void* vectors, int dtype, size_t n, size_t dim, 
                           size_t graph_max_degree, size_t window_size, size_t max_candidates, size_t prune_to,
                           const uint64_t* external_ids, int device, svsb200_index** out);
 
+/* Dynamic flat index.  Replaces: DynamicFlatIndex (include/svs/index/flat/dynamic_flat.h:65) with svs::DynamicFlat
+ * (orchestrators/dynamic_flat.h): an exact index over a mutable set of float32 / float16 / int8 / uint8 rows on one
+ * device, L2 / MIP / cosine, addressed by external ids.  A distinct handle type: neither the graph calls nor the
+ * svsb200_flat_index_* calls accept it.  Every slot is Valid or Empty; deleting a slot empties it at once (there is no
+ * Deleted state and nothing to consolidate).  External id 2^64 - 1 is reserved (it marks padding).  Searches may run
+ * concurrently with each other; mutations must not run concurrently with searches of the same index.  A mutation
+ * (add, delete, compact) first waits for every search of the index enqueued so far, including the work that
+ * svsb200_dynamic_flat_search_device leaves queued on the caller's stream, so it may follow such a call without a
+ * synchronisation; a search enqueued while a mutation runs is the caller's error. */
+typedef struct svsb200_dynamic_flat svsb200_dynamic_flat;
+
+/* DynamicFlatIndex(data, external_ids, distance, threadpool) (dynamic_flat.h:94-113): n x dim dense rows from HOST
+ * memory, one distinct external id each; every slot starts Valid.  n = 0 makes an empty index to be filled by
+ * svsb200_dynamic_flat_add. */
+int svsb200_dynamic_flat_create(const void* vectors, int dtype, size_t n, size_t dim, int metric, const uint64_t* external_ids,
+                                int device, svsb200_dynamic_flat** out);
+/* Frees the handle and its device memory (NULL is ignored). */
+int svsb200_dynamic_flat_destroy(svsb200_dynamic_flat* index);
+/* size() (dynamic_flat.h:146-150): Valid rows; the number of slots; dimensions() (:153); the device memory held by the
+ * rows, statuses and external ids of the allocated slots (the GEMM's operand tiles are not counted).  0 for NULL. */
+size_t svsb200_dynamic_flat_size(const svsb200_dynamic_flat* index);
+size_t svsb200_dynamic_flat_num_slots(const svsb200_dynamic_flat* index);
+size_t svsb200_dynamic_flat_dimensions(const svsb200_dynamic_flat* index);
+size_t svsb200_dynamic_flat_device_bytes(const svsb200_dynamic_flat* index);
+/* add_points (dynamic_flat.h:214-276): `count` rows of the index's dtype (dense, HOST) with one new external id each.
+ * Empty slots are taken in ascending order from first_empty (from slot 0 when reuse_empty is non-zero), then new slots
+ * past the end; first_empty becomes max(first_empty, last slot + 1).  Everything (dtype, repeated, present or reserved
+ * ids) is checked before anything changes.  `slots_out` (optional, `count` entries) receives the slots used.  The
+ * device arrays grow geometrically. */
+int svsb200_dynamic_flat_add(svsb200_dynamic_flat* index, const void* vectors, int dtype, size_t count, const uint64_t* ids,
+                             int reuse_empty, uint64_t* slots_out);
+/* delete_entries (dynamic_flat.h:292-307): the slots become Empty and first_empty = min(first_empty, slot).  Fails
+ * without changing anything unless every id is present and listed once. */
+int svsb200_dynamic_flat_delete(svsb200_dynamic_flat* index, const uint64_t* ids, size_t count);
+/* compact (dynamic_flat.h:335-367): the Valid slots move, in ascending order, to [0, size); first_empty = size; the
+ * allocations shrink to fit.  (The reference's batch size only tunes its copy; there is none here.)  consolidate
+ * (:376-378) is a no-op and has no function here. */
+int svsb200_dynamic_flat_compact(svsb200_dynamic_flat* index);
+/* external_ids / has_id (dynamic_flat.h:174,182-197): the external ids of the Valid slots, in slot order.  *count is
+ * the room of out_ids on entry (out_ids may be NULL to ask for the count) and the number of ids on return. */
+int svsb200_dynamic_flat_ids(const svsb200_dynamic_flat* index, uint64_t* out_ids, size_t* count);
+int svsb200_dynamic_flat_has_id(const svsb200_dynamic_flat* index, uint64_t id, int* out);
+/* The slot state for inspection: status uint8[slots] (0 Empty, 1 Valid) and external ids uint64[slots] (2^64 - 1 for
+ * an Empty slot); slots = svsb200_dynamic_flat_num_slots.  Either output may be NULL. */
+int svsb200_dynamic_flat_export(const svsb200_dynamic_flat* index, uint8_t* status_out, uint64_t* ext_ids_out);
+/* search (dynamic_flat.h:513-573): the exact top k (1 <= k <= 1024) of every query over the Valid slots, as EXTERNAL
+ * ids, with the routing, query types, distances and fallback count of svsb200_flat_index_search_device; ties are
+ * broken by slot (the reference leaves their order unspecified).  The result equals svsb200_flat_index_search over the
+ * Valid rows in slot order, its ids mapped to the external ids, bit for bit.  Rows are padded with all-ones ids and
+ * +-inf distances when fewer than k slots are Valid.  The device form is enqueued on `stream` apart from the
+ * fallback count's synchronisation (and, on the first search after a mutation, the maximum norm over the Valid rows). */
+int svsb200_dynamic_flat_search_device(svsb200_dynamic_flat* index, const void* d_queries, int qdtype, size_t nq, size_t k,
+                                       uint64_t* d_out_ids, float* d_out_dists, void* stream, uint32_t* fallback_queries);
+/* The same with HOST buffers (blocking). */
+int svsb200_dynamic_flat_search(svsb200_dynamic_flat* index, const void* queries, int qdtype, size_t nq, size_t k,
+                                uint64_t* out_ids, float* out_dists);
+
 #ifdef __cplusplus
 }
 #endif

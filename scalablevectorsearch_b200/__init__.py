@@ -7,8 +7,9 @@ around it (:mod:`.io`).
 from .vamana import (DataType, DistanceType, DynamicVamana, GraphLoader, SearchBufferConfig, ShardedVamana, Vamana,
                      VamanaBuildParameters, VamanaSearchParameters, VectorDataLoader, build_graph, lvq8_compress)
 from .flat import Flat
+from .dynamic_flat import DynamicFlat
 from ._lib import Svsb200Error
 
 __all__ = ["DataType", "DistanceType", "GraphLoader", "SearchBufferConfig", "Vamana", "VamanaSearchParameters",
            "VectorDataLoader", "Svsb200Error", "lvq8_compress", "ShardedVamana", "VamanaBuildParameters", "build_graph",
-           "DynamicVamana", "Flat"]
+           "DynamicVamana", "Flat", "DynamicFlat"]

@@ -28,6 +28,11 @@ SYMBOLS = [
     "svsb200_dynamic_create", "svsb200_dynamic_delete", "svsb200_dynamic_ids", "svsb200_dynamic_has_id",
     "svsb200_dynamic_export", "svsb200_dynamic_set_build_parameters", "svsb200_dynamic_get_build_parameters",
     "svsb200_dynamic_add", "svsb200_dynamic_consolidate", "svsb200_dynamic_compact", "svsb200_dynamic_build",
+    "svsb200_dynamic_flat_create", "svsb200_dynamic_flat_destroy", "svsb200_dynamic_flat_size",
+    "svsb200_dynamic_flat_num_slots", "svsb200_dynamic_flat_dimensions", "svsb200_dynamic_flat_device_bytes",
+    "svsb200_dynamic_flat_add", "svsb200_dynamic_flat_delete", "svsb200_dynamic_flat_compact", "svsb200_dynamic_flat_ids",
+    "svsb200_dynamic_flat_has_id", "svsb200_dynamic_flat_export", "svsb200_dynamic_flat_search",
+    "svsb200_dynamic_flat_search_device",
 ]
 
 _lib = None
@@ -107,6 +112,19 @@ def lib() -> C.CDLL:
     l.svsb200_dynamic_consolidate.argtypes = [vp]
     l.svsb200_dynamic_compact.argtypes = [vp]
     l.svsb200_dynamic_build.argtypes = [vp, i32, sz, sz, i32, C.c_float, sz, sz, sz, sz, vp, i32, C.POINTER(vp)]
+    l.svsb200_dynamic_flat_create.argtypes = [vp, i32, sz, sz, i32, vp, i32, C.POINTER(vp)]
+    l.svsb200_dynamic_flat_destroy.argtypes = [vp]
+    for name in ("size", "num_slots", "dimensions", "device_bytes"):
+        fn = getattr(l, f"svsb200_dynamic_flat_{name}")
+        fn.restype, fn.argtypes = sz, [vp]
+    l.svsb200_dynamic_flat_add.argtypes = [vp, vp, i32, sz, vp, i32, vp]
+    l.svsb200_dynamic_flat_delete.argtypes = [vp, vp, sz]
+    l.svsb200_dynamic_flat_compact.argtypes = [vp]
+    l.svsb200_dynamic_flat_ids.argtypes = [vp, vp, C.POINTER(sz)]
+    l.svsb200_dynamic_flat_has_id.argtypes = [vp, C.c_uint64, C.POINTER(i32)]
+    l.svsb200_dynamic_flat_export.argtypes = [vp, vp, vp]
+    l.svsb200_dynamic_flat_search.argtypes = [vp, vp, i32, sz, sz, vp, vp]
+    l.svsb200_dynamic_flat_search_device.argtypes = [vp, vp, i32, sz, sz, vp, vp, vp, C.POINTER(u32)]
     _lib = l
     return l
 

@@ -91,16 +91,6 @@ __global__ void compact_kernel(const uint32_t* __restrict__ new_to_old, const ui
     if (lane == 0) refdeg_out[i] = refdeg_in[o];
 }
 
-// A copy of `buf` with room for `want` elements whose first `used` elements are the old ones (no-op if it fits).
-template <typename T> static cudaError_t grow(DeviceBuffer<T>& buf, size_t used, size_t want) {
-    if (want <= buf.count) return cudaSuccess;
-    DeviceBuffer<T> bigger;
-    cudaError_t e = bigger.ensure(want);
-    if (e == cudaSuccess && used) e = cudaMemcpy(bigger.ptr, buf.ptr, used * sizeof(T), cudaMemcpyDeviceToDevice);
-    if (e == cudaSuccess) buf = std::move(bigger);   // (the old block goes with `bigger`)
-    return e;
-}
-
 // Bytes of device memory a dynamic index with room for `slots` slots holds.
 static size_t dynamic_bytes(const svsb200_index* ix, size_t slots) {
     return slots * (size_t(ix->row_stride) + size_t(ix->gstride) * sizeof(uint32_t) + sizeof(uint16_t) + 1 + sizeof(uint64_t));

@@ -771,6 +771,40 @@ __global__ void flat_move_rows_kernel(const char* __restrict__ src, char* __rest
     for (uint32_t b = threadIdx.x; b < row_bytes; b += blockDim.x) d[b] = s[b];
 }
 
+// ---- dynamic flat index: upkeep of the base tiles -----------------------------------------------------------------
+// Rows i < count of blobs tiled 8 rows to a tile (flat_tile_rows with tile_rows = 8), with their bias and norms, ->
+// slots slots[i] (slots NULL: first + i) of base blobs tiled FLAT_BN rows to a tile.  `src` NULL turns the slots into
+// padding rows: zero blobs (so that an integer key stays the empty key) and the bias `empty_bias`.  A row is KB blobs
+// of four 16-byte chunks in either operand kind; one warp per row.
+__global__ void flat_place_rows_kernel(const uint4* __restrict__ src, const uint32_t* __restrict__ src_bias,
+                                       const float* __restrict__ src_norms, const uint32_t* __restrict__ slots, uint32_t first,
+                                       uint32_t count, uint32_t KB, uint32_t empty_bias, uint4* __restrict__ dst,
+                                       uint32_t* __restrict__ bias, float* __restrict__ norms) {
+    const uint32_t i = blockIdx.x * (blockDim.x / 32) + threadIdx.x / 32;
+    const uint32_t lane = threadIdx.x & 31;
+    if (i >= count) return;
+    const uint32_t s = slots ? slots[i] : first + i;
+    for (uint32_t j = lane; j < 4 * KB; j += 32) {
+        const uint4 v = src ? src[flat_blob_offset<16>(i / 8, i % 8, 16 * j, 8, KB) / 16] : make_uint4(0u, 0u, 0u, 0u);
+        dst[flat_blob_offset<16>(s / FLAT_BN, s % FLAT_BN, 16 * j, FLAT_BN, KB) / 16] = v;
+    }
+    if (lane == 0) {
+        bias[s] = src ? src_bias[i] : empty_bias;
+        if (norms) norms[s] = src ? src_norms[i] : 0.f;
+    }
+}
+
+// Xmax of a dynamic flat index: the largest norm over its Valid slots (norms are >= 0 or +inf, so their bits order as
+// unsigned integers).  *xmax_bits is 0 before the launch.
+__global__ void flat_masked_xmax_kernel(const float* __restrict__ norms, const uint8_t* __restrict__ status, uint32_t n,
+                                        unsigned int* __restrict__ xmax_bits) {
+    unsigned int m = 0;
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+        if (status[i] == SLOT_VALID) m = max(m, __float_as_uint(norms[i]));
+    m = __reduce_max_sync(0xFFFFFFFFu, m);
+    if ((threadIdx.x & 31) == 0 && m) atomicMax(xmax_bits, m);
+}
+
 // ---- launchers ------------------------------------------------------------------------------------------------------
 // Rows -> the operand blobs of `kind`: flat_tile_kernel (fp16) or flat_tile8_kernel (8-bit, which has no norms).
 // `bias` (float, or int32 for 8-bit blobs), `norms` and `max_norm_bits` may be NULL.
@@ -897,6 +931,22 @@ static cudaError_t flat_move_rows(const void* src, void* dst, const uint32_t* id
     return cudaGetLastError();
 }
 
+// The bias of a padding row: +inf (fp16 keys) or INT32_MAX (integer keys).
+static uint32_t flat_empty_bias(int kind) { return kind == FLAT_F16 ? 0x7F800000u : 0x7FFFFFFFu; }
+
+// flat_place_rows_kernel into `base` (tiles of operand kind `kind`); src NULL makes the slots padding rows.
+static cudaError_t flat_place_rows(int kind, uint32_t dim, const void* src, const void* src_bias, const float* src_norms,
+                                   const uint32_t* slots, uint32_t first, uint32_t count, Replica::FlatBase& base,
+                                   cudaStream_t stream) {
+    if (count == 0) return cudaSuccess;
+    flat_place_rows_kernel<<<(count + 7) / 8, 256, 0, stream>>>(
+        static_cast<const uint4*>(src), static_cast<const uint32_t*>(src_bias), src_norms, slots, first, count,
+        flat_kblocks(kind, dim), flat_empty_bias(kind), reinterpret_cast<uint4*>(base.tiles.ptr),
+        reinterpret_cast<uint32_t*>(base.bias.ptr), base.norms.ptr);
+    count_launch();
+    return cudaGetLastError();
+}
+
 // The deep lists of one query tile keep at most FLAT_CMAX / FLAT_KC_DEEP = 7 CTAs busy: batches of one or two tiles
 // run faster on the scan (DESIGN.md §9b), so the deep lists need more than 2 FLAT_BM queries.
 static bool flat_deep_batch(size_t nq) { return nq > 2 * FLAT_BM; }
@@ -913,17 +963,53 @@ static int ensure_flat_base(svsb200_index* ix, Replica* rep, int kind, cudaStrea
         CUDA_TRY(rep->flat_xmax.ensure(1));
         CUDA_TRY(cudaMemsetAsync(rep->flat_xmax.ptr, 0, 4, stream));
     }
+    // dynamic flat index: the norm of every slot, flat_xmax being taken over the Valid ones (ensure_slots_xmax)
+    float* norms = nullptr;
+    if (ix->slot_mask && kind == FLAT_F16) {
+        CUDA_TRY(base.norms.ensure(size_t(ntiles) * FLAT_BN));
+        norms = base.norms.ptr;
+        rep->flat_xmax_stale = true;
+    }
     CUDA_TRY(flat_tile_rows(kind, ix->dtype, rep->d_vectors.ptr, ix->row_stride, n, dim, FLAT_BN, ix->metric == SVSB200_L2,
-                            base.tiles.ptr, base.bias.ptr, nullptr, kind == FLAT_F16 ? rep->flat_xmax.ptr : nullptr, stream));
+                            base.tiles.ptr, base.bias.ptr, norms, kind == FLAT_F16 && !norms ? rep->flat_xmax.ptr : nullptr,
+                            stream));
+    if (ix->slot_mask) {   // slots that are not Valid become padding rows
+        std::vector<uint32_t> empty;
+        for (uint32_t s = 0; s < n; ++s)
+            if (ix->status[s] != SLOT_VALID) empty.push_back(s);
+        DeviceBuffer<uint32_t> d_empty;
+        CUDA_TRY(d_empty.ensure(std::max<size_t>(empty.size(), 1)));
+        CUDA_TRY(cudaMemcpyAsync(d_empty.ptr, empty.data(), empty.size() * 4, cudaMemcpyHostToDevice, stream));
+        CUDA_TRY(flat_place_rows(kind, dim, nullptr, nullptr, nullptr, d_empty.ptr, 0, uint32_t(empty.size()), base, stream));
+        CUDA_TRY(cudaStreamSynchronize(stream));   // (before d_empty goes)
+    }
     CUDA_TRY(cudaStreamSynchronize(stream));
+    return 0;
+}
+
+// flat_xmax of a dynamic flat index, retaken over the Valid slots when they changed since it was last taken (a stale
+// maximum would still be sound, but it could keep sending every query to the scan after the row that set it is gone).
+static int ensure_slots_xmax(svsb200_index* ix, Replica* rep, cudaStream_t stream) {
+    std::lock_guard<std::mutex> lock(rep->mu);
+    if (!rep->flat_xmax_stale) return 0;
+    const uint32_t n = uint32_t(ix->n);
+    CUDA_TRY(cudaMemsetAsync(rep->flat_xmax.ptr, 0, 4, stream));
+    const unsigned grid = unsigned(std::max<size_t>(1, std::min<size_t>((n + 255) / 256, size_t(rep->sm_count) * 4)));
+    flat_masked_xmax_kernel<<<grid, 256, 0, stream>>>(rep->flat_f16.norms.ptr, rep->d_status.ptr, n, rep->flat_xmax.ptr);
+    count_launch();
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaStreamSynchronize(stream));
+    rep->flat_xmax_stale = false;
     return 0;
 }
 
 // Shared body of the tensor-core flat search: device buffers in, device buffers out, enqueued on sc->stream except
 // for one synchronisation (the count of queries that need the exact-scan fallback).  `max_kc` is the deepest list the
-// caller allows: k + 8 <= FLAT_KC runs the FLAT_KC lists, k + 8 <= FLAT_KC_DEEP (Flat handle only) the deep ones.
-static int flat_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, const void* d_queries, int qdtype, size_t nq, size_t k,
-                          uint64_t* d_out_ids, float* d_out_dists, uint32_t* fallback_queries, uint32_t max_kc) {
+// caller allows: k + 8 <= FLAT_KC runs the FLAT_KC lists, k + 8 <= FLAT_KC_DEEP (Flat handles only) the deep ones.
+// Ids are row numbers (dynamic flat index: slots; flat_on_device maps them to external ids).
+static int flat_rows_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, const void* d_queries, int qdtype, size_t nq,
+                               size_t k, uint64_t* d_out_ids, float* d_out_dists, uint32_t* fallback_queries,
+                               uint32_t max_kc) {
     if (fallback_queries) *fallback_queries = 0;
     if (nq == 0) return 0;
     cudaStream_t stream = sc->stream;
@@ -948,6 +1034,8 @@ static int flat_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, const vo
     const uint32_t ntiles = (n + 255) / 256, mtiles = uint32_t((nq + 127) / 128);
     const int l2 = ix->metric == SVSB200_L2;
     if (int rc = ensure_flat_base(ix, rep, kind, stream)) return rc;
+    if (ix->slot_mask && kind == FLAT_F16)
+        if (int rc = ensure_slots_xmax(ix, rep, stream)) return rc;
     const Replica::FlatBase& base = kind == FLAT_F16 ? rep->flat_f16 : rep->flat_int;
     // one CTA per SM over equal runs of output tiles; `nsplit` = candidate lists per query (flat_plan)
     uint32_t flat_ctas = 1, flat_share = 1, nsplit = 2;
@@ -1003,6 +1091,81 @@ static int flat_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, const vo
     return 0;
 }
 
+// flat_rows_on_device, with a dynamic flat index's slots mapped to external ids on every route (GEMM, fallback, scan).
+static int flat_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, const void* d_queries, int qdtype, size_t nq, size_t k,
+                          uint64_t* d_out_ids, float* d_out_dists, uint32_t* fallback_queries, uint32_t max_kc) {
+    if (int rc = flat_rows_on_device(ix, rep, sc, d_queries, qdtype, nq, k, d_out_ids, d_out_dists, fallback_queries, max_kc))
+        return rc;
+    if (ix->slot_mask) {
+        CUDA_TRY(slots_to_external(d_out_ids, nq * k, rep->d_ext_ids.ptr, sc->stream));
+        CUDA_TRY(cudaEventRecord(sc->ev_done, sc->stream));   // (a mutation waits for it: dynamic_flat.cu, on_stream)
+    }
+    return 0;
+}
+
+// ---- dynamic flat index: the tiles follow every mutation (host.cuh) ----
+// Each built operand kind of the index's rows: fp16 tiles, and the integer tiles of int8 / uint8 rows.
+template <typename F> static int for_each_flat_base(svsb200_index* ix, Replica* rep, F body) {
+    if (rep->flat_f16.tiles.ptr)
+        if (int rc = body(FLAT_F16, rep->flat_f16)) return rc;
+    if (rep->flat_int.tiles.ptr)
+        if (int rc = body(ix->dtype == SVSB200_I8 ? FLAT_S8 : FLAT_U8, rep->flat_int)) return rc;
+    return 0;
+}
+
+uint32_t flat_max_kc_deep() { return FLAT_KC_DEEP; }
+
+int flat_slots_grow(svsb200_index* ix, Replica* rep, size_t old_n, size_t new_n, cudaStream_t stream) {
+    const uint32_t dim = uint32_t(ix->dim);
+    const size_t old_t = (old_n + FLAT_BN - 1) / FLAT_BN, new_t = (new_n + FLAT_BN - 1) / FLAT_BN;
+    const size_t cap_t = (rep->d_status.count + FLAT_BN - 1) / FLAT_BN;   // geometric, with the slot arrays
+    if (new_t <= old_t) return 0;
+    return for_each_flat_base(ix, rep, [&](int kind, Replica::FlatBase& base) -> int {
+        const size_t tile_bytes = size_t(FLAT_BN) * flat_kblocks(kind, dim) * FLAT_BK * 2;
+        CUDA_TRY(cudaStreamSynchronize(stream));
+        CUDA_TRY(grow(base.tiles, old_t * tile_bytes, cap_t * tile_bytes));
+        CUDA_TRY(grow(base.bias, old_t * FLAT_BN, cap_t * FLAT_BN));
+        if (base.norms.ptr) CUDA_TRY(grow(base.norms, old_t * FLAT_BN, cap_t * FLAT_BN));
+        CUDA_TRY(flat_place_rows(kind, dim, nullptr, nullptr, nullptr, nullptr, uint32_t(old_t * FLAT_BN),
+                                 uint32_t((new_t - old_t) * FLAT_BN), base, stream));
+        return 0;
+    });
+}
+
+int flat_slots_place(svsb200_index* ix, Replica* rep, const void* d_rows, const uint32_t* d_slots, uint32_t count,
+                     cudaStream_t stream) {
+    rep->flat_xmax_stale = true;
+    if (count == 0) return 0;
+    const uint32_t dim = uint32_t(ix->dim), rows8 = (count + 7) / 8 * 8;
+    Replica::SlotStaging& st = rep->staging;
+    return for_each_flat_base(ix, rep, [&](int kind, Replica::FlatBase& base) -> int {
+        // the full tiling's kernels, 8 rows to a tile, then every row moved to its slot (the kinds run one after the
+        // other on `stream`, so they share the staging)
+        CUDA_TRY(st.tiles.ensure(size_t(rows8) * flat_kblocks(kind, dim) * FLAT_BK * 2));
+        CUDA_TRY(st.bias.ensure(rows8));
+        if (base.norms.ptr) CUDA_TRY(st.norms.ensure(rows8));
+        float* norms = base.norms.ptr ? st.norms.ptr : nullptr;
+        CUDA_TRY(flat_tile_rows(kind, ix->dtype, d_rows, ix->row_stride, count, dim, 8, ix->metric == SVSB200_L2,
+                                st.tiles.ptr, st.bias.ptr, norms, nullptr, stream));
+        CUDA_TRY(flat_place_rows(kind, dim, st.tiles.ptr, st.bias.ptr, norms, d_slots, 0, count, base, stream));
+        return 0;
+    });
+}
+
+int flat_slots_clear(svsb200_index* ix, Replica* rep, const uint32_t* d_slots, uint32_t count, cudaStream_t stream) {
+    rep->flat_xmax_stale = true;
+    return for_each_flat_base(ix, rep, [&](int kind, Replica::FlatBase& base) -> int {
+        CUDA_TRY(flat_place_rows(kind, uint32_t(ix->dim), nullptr, nullptr, nullptr, d_slots, 0, count, base, stream));
+        return 0;
+    });
+}
+
+void flat_slots_reset(Replica* rep) {
+    rep->flat_f16 = Replica::FlatBase{};
+    rep->flat_int = Replica::FlatBase{};
+    rep->flat_xmax_stale = true;
+}
+
 // The plan of flat_on_device for k and a device of `sm_count` SMs (svsb200_flat_plan / svsb200_flat_plan_k).
 static void flat_plan_rows(size_t nq, size_t n, uint32_t kc, int sm_count, uint32_t* ctas, uint32_t* share,
                            uint32_t* lists_per_query, uint64_t* segment_begin) {
@@ -1026,13 +1189,14 @@ struct svsb200_flat {
 
 using namespace svsb200;
 
-// The two search bodies behind the four entry points: `who` names the entry point in errors, `max_kc` is its deepest
-// list (flat_on_device).  A Flat handle is never dynamic and lives on one device.
+// The two search bodies behind the four entry points here and the dynamic flat index's two (dynamic_flat.cu): `who`
+// names the entry point in errors, `max_kc` is its deepest list (flat_on_device).  A flat handle is never dynamic and
+// lives on one device.
 
 // Enqueue-only form on device buffers, on the scratch bound to the caller's stream.
-static int flat_search_device(const char* who, svsb200_index* ix, const void* d_queries, int qdtype, size_t nq, size_t k,
-                              uint64_t* d_out_ids, float* d_out_dists, void* stream_, uint32_t* fallback_queries,
-                              uint32_t max_kc) {
+int svsb200::flat_search_device(const char* who, svsb200_index* ix, const void* d_queries, int qdtype, size_t nq, size_t k,
+                                uint64_t* d_out_ids, float* d_out_dists, void* stream_, uint32_t* fallback_queries,
+                                uint32_t max_kc) {
     const std::string w(who);
     if (!ix) return fail(w + ": NULL index");
     if (nq && (!d_queries || !d_out_ids || !d_out_dists)) return fail(w + ": NULL buffer");
@@ -1049,8 +1213,8 @@ static int flat_search_device(const char* who, svsb200_index* ix, const void* d_
 }
 
 // Blocking form on host buffers, on a scratch set of the pool (the first replica's).
-static int flat_search_host(const char* who, svsb200_index* ix, const void* queries, int qdtype, size_t nq, size_t k,
-                            uint64_t* out_ids, float* out_dists, uint32_t max_kc) {
+int svsb200::flat_search_host(const char* who, svsb200_index* ix, const void* queries, int qdtype, size_t nq, size_t k,
+                                uint64_t* out_ids, float* out_dists, uint32_t max_kc) {
     const std::string w(who);
     if (!ix) return fail(w + ": NULL index");
     if (k == 0 || k > 1024) return fail(w + ": k must be in [1, 1024]");

@@ -100,6 +100,16 @@ template <typename T> struct DeviceBuffer {
     }
 };
 
+// A copy of `buf` with room for `want` elements whose first `used` elements are the old ones (no-op if it fits).
+template <typename T> cudaError_t grow(DeviceBuffer<T>& buf, size_t used, size_t want) {
+    if (want <= buf.count) return cudaSuccess;
+    DeviceBuffer<T> bigger;
+    cudaError_t e = bigger.ensure(want);
+    if (e == cudaSuccess && used) e = cudaMemcpy(bigger.ptr, buf.ptr, used * sizeof(T), cudaMemcpyDeviceToDevice);
+    if (e == cudaSuccess) buf = std::move(bigger);   // (the old block goes with `bigger`)
+    return e;
+}
+
 // Everything one in-flight search needs on one device: the analogue of the reference's per-thread scratch
 // space (index/vamana/index.h:455-470).
 struct Scratch {
@@ -156,9 +166,20 @@ struct Replica {
     struct FlatBase {
         DeviceBuffer<unsigned char> tiles;
         DeviceBuffer<float> bias;            // 8-bit tiles: int32 |x|^2
+        DeviceBuffer<float> norms;           // dynamic flat index, fp16 tiles: the norm of every slot's row
     };
     FlatBase flat_f16;                       // fp16 tiles
     DeviceBuffer<unsigned int> flat_xmax;    // ... and the largest norm of their rows
+    bool flat_xmax_stale = false;            // dynamic flat index: the Valid slots changed since flat_xmax was taken
+    // dynamic flat index: staging of a mutation (the added rows, their slots and ids, and the rows tiled 8 to a tile),
+    // kept between calls so that an add or delete allocates -- and synchronises the device -- only when it outgrows them
+    struct SlotStaging {
+        DeviceBuffer<unsigned char> rows, tiles;
+        DeviceBuffer<uint32_t> slots;
+        DeviceBuffer<uint64_t> ids;
+        DeviceBuffer<float> bias, norms;
+    };
+    SlotStaging staging;
     FlatBase flat_int;                       // int8 / uint8 tiles of the integer GEMM
     std::mutex mu;
     std::vector<Scratch*> idle;                      // pool for the blocking API
@@ -247,6 +268,9 @@ struct svsb200_index {
     long dyn_slack = -1;              // option "dynamic_slack"
     std::atomic<long> dyn_reruns{0};  // queries re-run with a larger buffer so far
     size_t first_empty = 0;           // first_empty_: where add_points looks for Empty slots unless told to reuse
+    // dynamic flat index (svsb200_dynamic_flat_*, DynamicFlatIndex): the same slot fields, statuses Valid / Empty only,
+    // and every flat search skips the slots that are not Valid and returns external ids.  `dynamic` stays false.
+    bool slot_mask = false;
     // mutation parameters (alpha_, construction_window_size_, max_candidates_, prune_to_)
     float dyn_alpha = 0.f;
     size_t dyn_window = 0, dyn_max_candidates = 0, dyn_prune_to = 0;
@@ -302,5 +326,30 @@ int construct_graph(const char* who, const GraphBuild& b, float reverse_alpha, u
 int medoid(const GraphBuild& b, const uint8_t* d_status, size_t count, uint32_t* out);
 // b.deg[v] = length of adjacency row v, for every row (enqueued on b.stream).
 int row_degrees(const GraphBuild& b);
+
+// Slots -> external ids in place, `count` ids (padding ids stay all-ones; search.cu), enqueued on `stream`.
+cudaError_t slots_to_external(uint64_t* d_ids, size_t count, const uint64_t* d_ext_ids, cudaStream_t stream);
+
+// ---- flat search (flat.cu), shared by the Flat handle and the dynamic flat index ----
+// The two search bodies: `who` names the entry point in errors, `max_kc` is the deepest candidate list allowed.  The
+// device form is enqueued on the caller's stream, the host form blocks.
+int flat_search_device(const char* who, svsb200_index* ix, const void* d_queries, int qdtype, size_t nq, size_t k,
+                       uint64_t* d_out_ids, float* d_out_dists, void* stream, uint32_t* fallback_queries, uint32_t max_kc);
+int flat_search_host(const char* who, svsb200_index* ix, const void* queries, int qdtype, size_t nq, size_t k,
+                     uint64_t* out_ids, float* out_dists, uint32_t max_kc);
+// Deepest list of the Flat handles' searches (k <= 121 on the GEMM).
+uint32_t flat_max_kc_deep();
+// Incremental upkeep of a dynamic flat index's GEMM operands, for every operand kind already built (nothing before the
+// first search builds them), enqueued on `stream`.  Invariant afterwards: every Valid slot's blobs, bias and norm are
+// what the full tiling writes for its row; every other row is a padding row (zero blobs, the empty bias).
+//   flat_slots_grow:  the slots grow from old_n to new_n: whole 256-row tiles of padding rows behind the kept prefix;
+//   flat_slots_place: rows i of the dense `d_rows` (ix->row_stride apart) are now Valid in slots d_slots[i];
+//   flat_slots_clear: slots d_slots[i] are no longer Valid;
+//   flat_slots_reset: the slots were renumbered (compaction): the tiles are dropped and rebuilt by the next search.
+int flat_slots_grow(svsb200_index* ix, Replica* rep, size_t old_n, size_t new_n, cudaStream_t stream);
+int flat_slots_place(svsb200_index* ix, Replica* rep, const void* d_rows, const uint32_t* d_slots, uint32_t count,
+                     cudaStream_t stream);
+int flat_slots_clear(svsb200_index* ix, Replica* rep, const uint32_t* d_slots, uint32_t count, cudaStream_t stream);
+void flat_slots_reset(Replica* rep);
 
 }  // namespace svsb200

@@ -261,6 +261,13 @@ __global__ void slots_to_external_kernel(uint64_t* __restrict__ ids, size_t coun
     if (i < count && ids[i] != ~uint64_t(0)) ids[i] = ext_ids[ids[i]];
 }
 
+cudaError_t slots_to_external(uint64_t* d_ids, size_t count, const uint64_t* d_ext_ids, cudaStream_t stream) {
+    if (count == 0) return cudaSuccess;
+    slots_to_external_kernel<<<unsigned((count + 255) / 256), 256, 0, stream>>>(d_ids, count, d_ext_ids);
+    count_launch();
+    return cudaGetLastError();
+}
+
 // ---------------------------------------------------------------------------------------
 // Host side
 // ---------------------------------------------------------------------------------------
@@ -523,6 +530,7 @@ int search_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, const void* d
     // (sc->d_cancel is zero here: only wait_kernels raises it, and lowers it again once the kernels have finished)
 
     SearchParams p = search_params(ix, rep, sc, nq, k, window, capacity, d_out_ids, id_bytes, d_out_dists, exhaustive);
+    if (exhaustive && ix->slot_mask) p.status = rep->d_status.ptr;   // dynamic flat index: the Valid slots only
     LaunchConfig cfg{};
     bool use_fast = false;
     if (int rc = choose_launch(ix, rep, &p, exhaustive, stream, &cfg, &use_fast)) return rc;

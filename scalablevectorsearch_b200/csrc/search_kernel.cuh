@@ -561,7 +561,9 @@ __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wai
 // index/flat/flat.h:159,421-465, used here for ground truth): the "neighbours" of every step
 // are the next block of consecutive ids, there is no visited filter and no expansion order;
 // the sorted buffer (window = capacity = k) ends up holding the exact top-k, ties by id.
-template <int ROWT, int OP, int DS, int NROWS, bool EXH = false, int KS = 1>
+// MASK = true (with EXH; the dynamic flat index) keeps only the rows whose p.status is Valid: each block's ids are
+// compacted through the status before the distances, so the survivors stay in ascending order and ties stay by id.
+template <int ROWT, int OP, int DS, int NROWS, bool EXH = false, int KS = 1, bool MASK = false>
 __global__ void __launch_bounds__(256, SVSB200_MIN_BLOCKS) vamana_search_kernel(const __grid_constant__ SearchParams p) {
     constexpr bool kInt = (OP >= OP_L2I);
     constexpr int G = kInt ? 4 : KS * 16 / Row<ROWT>::LPT;     // threads per row
@@ -675,9 +677,21 @@ __global__ void __launch_bounds__(256, SVSB200_MIN_BLOCKS) vamana_search_kernel(
             uint32_t deg = 0;
             if constexpr (EXH) {
                 if (scan_base >= exh_hi) break;
-                deg = min(p.deg_pad, exh_hi - scan_base);
-                for (uint32_t i = lane; i < deg; i += 32) cid[i] = scan_base + i;
-                scan_base += deg;
+                if constexpr (MASK) {
+                    const uint32_t span = min(p.deg_pad, exh_hi - scan_base);
+                    for (uint32_t i0 = 0; i0 < span; i0 += 32) {
+                        const uint32_t i = i0 + lane;
+                        const bool live = i < span && p.status[scan_base + i] == SLOT_VALID;
+                        const unsigned m = __ballot_sync(FULL, live);
+                        if (live) cid[deg + __popc(m & ((1u << lane) - 1u))] = scan_base + i;
+                        deg += __popc(m);
+                    }
+                    scan_base += span;
+                } else {
+                    deg = min(p.deg_pad, exh_hi - scan_base);
+                    for (uint32_t i = lane; i < deg; i += 32) cid[i] = scan_base + i;
+                    scan_base += deg;
+                }
                 __syncwarp();
             } else {
                 // buffer.next(): first unvisited entry inside min(size, window)
@@ -895,10 +909,18 @@ cudaError_t launch_search(int op, const SearchParams& p, const LaunchConfig& cfg
     });
 }
 
-// The exhaustive scan: one work item per (query, range of base rows), on a persistent grid.
+// The exhaustive scan: one work item per (query, range of base rows), on a persistent grid.  With p.status set (the
+// dynamic flat index; plain rows only) it scans the Valid rows alone.  Its rows per group and pass: two, but one for
+// float16 rows and for cosine, where the two-row pass spills under the 128-register bound (as the unmasked scan does);
+// the one-row pass spills nowhere, and the two-row one is faster where it fits.
 template <int ROWT> cudaError_t launch_search_exhaustive(int op, const SearchParams& p, const LaunchConfig& cfg) {
     const size_t ctas = (size_t(p.nq) * (p.exh_split ? p.exh_split : 1u) + cfg.warps_per_cta - 1) / cfg.warps_per_cta;
     return dispatch(SearchOps<ROWT>{}, op, [&](auto o) {
+        constexpr int OP = decltype(o)::value;
+        if constexpr (ROWT != ROW_LVQ8) {
+            constexpr int NR = ROWT == SVSB200_F16 || OP == OP_COSF ? 1 : 2;
+            if (p.status) return launch_kernel(vamana_search_kernel<ROWT, OP, 0, NR, true, 1, true>, cfg, ctas, true, p);
+        }
         return launch_kernel(vamana_search_kernel<ROWT, decltype(o)::value, 0, 2, true>, cfg, ctas, true, p);
     });
 }
