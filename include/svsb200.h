@@ -454,6 +454,60 @@ int svsb200_dynamic_flat_search_device(svsb200_dynamic_flat* index, const void* 
 int svsb200_dynamic_flat_search(svsb200_dynamic_flat* index, const void* queries, int qdtype, size_t nq, size_t k,
                                 uint64_t* out_ids, float* out_dists);
 
+/* IVF index.  Replaces: IVFIndex (include/svs/index/ivf/index.h) with svs::IVF and svs::Clustering
+ * (index/ivf/kmeans.h, common.h): float32 / float16 rows on one device, L2 / MIP / cosine, grouped into C clusters
+ * around float32 centroids.  A search probes, per query, the n_probes centroids nearest under the metric (the flat
+ * search's exact distances over the centroids, ties to the lower centroid; the reference ranks them from an sgemm whose
+ * rounding is the BLAS's) and returns the exact top k (1 <= k <= 1024) over the union of the probed clusters' rows:
+ * the search path's bit-exact distances, ordered by distance, then original row id, padded with all-ones ids and
+ * +-inf distances when the probed clusters hold fewer than k rows.  With n_probes = C the result equals
+ * svsb200_exhaustive_device over the same rows bit for bit.  Integer, SQ and LVQ rows are refused. */
+typedef struct svsb200_ivf svsb200_ivf;
+
+/* The random sequence of svsb200_ivf_cluster: the first `count` outputs of splitmix64 seeded with `seed` (state +=
+ * 0x9E3779B97F4A7C15, then the two xor-shift-multiply rounds).  An own sequence, documented so that a model can
+ * reproduce the clustering bit for bit. */
+int svsb200_ivf_random(uint64_t seed, size_t count, uint64_t* out);
+/* Clustering.build / kmeans_clustering (ivf/kmeans.h:40-131, common.h:446-634) over n x dim dense rows in HOST memory,
+ * the flat (non-hierarchical) k-means, deterministic: is_hierarchical must be 0 (hierarchical k-means is refused).
+ *   1. m = min(n, max(min(2 C, n), ceil(float(n) * training_fraction))) training rows, refused when m < C: the first m
+ *      of a Fisher-Yates shuffle of [0, n) (draw i swaps position i with i + r % (n - i)), taken in ascending order;
+ *   2. centroid c = training row p[c], p the first C of the same shuffle of [0, m) (continuing the sequence);
+ *   3. num_iterations rounds of: assign every training row to its exact nearest centroid (the flat search, k = 1, in
+ *      batches of minibatch_size rows, which changes no result); add every member, in ascending row order, in float32
+ *      onto its old centroid and multiply a centroid with members by float(1.0 / (count + 1)); split every empty
+ *      cluster i in ascending order as the reference does (j cycles from 0 over the populated clusters until a draw
+ *      r = (x >> 40) 2^-24 < float(count_j) / float(m); i copies j; even coordinates of i and odd ones of j times
+ *      1 + 2^-10, the others times 1 - 2^-10, rounded from double; count_i = count_j / 2, count_j -= count_i); for MIP
+ *      and cosine, normalise every centroid (x * (1 / sqrt(sequential float32 sum of squares)), zero rows untouched),
+ *      as also done once after step 2;
+ *   4. assign all n rows to their exact nearest final centroid.
+ * out_centroids: float32 [C][dim]; out_assignments: uint32 [n]. */
+int svsb200_ivf_cluster(const void* vectors, int dtype, size_t n, size_t dim, int metric, size_t num_centroids,
+                        size_t minibatch_size, size_t num_iterations, int is_hierarchical, float training_fraction,
+                        uint64_t seed, int device, float* out_centroids, uint32_t* out_assignments);
+/* IVFIndex::assemble_from_clustering: n x dim rows (HOST) grouped by `assignments` (uint32 [n], each < C; NULL:
+ * every row goes to its exact nearest centroid, computed on the device) around C float32 centroids [C][dim]. */
+int svsb200_ivf_create(const void* vectors, int dtype, size_t n, size_t dim, int metric, const float* centroids,
+                       size_t num_centroids, const uint32_t* assignments, int device, svsb200_ivf** out);
+/* Frees the handle and its device memory (NULL is ignored). */
+int svsb200_ivf_destroy(svsb200_ivf* index);
+/* Rows, dimensions, clusters, device memory held (rows, ids, centroids); 0 for NULL. */
+size_t svsb200_ivf_size(const svsb200_ivf* index);
+size_t svsb200_ivf_dimensions(const svsb200_ivf* index);
+size_t svsb200_ivf_num_clusters(const svsb200_ivf* index);
+size_t svsb200_ivf_device_bytes(const svsb200_ivf* index);
+/* Rows per cluster (uint32 [C]) and the centroids (float32 [C][dim]), HOST buffers. */
+int svsb200_ivf_cluster_sizes(const svsb200_ivf* index, uint32_t* out);
+int svsb200_ivf_centroids(const svsb200_ivf* index, float* out);
+/* search: float32 / float16 queries (DEVICE buffers), 1 <= k <= 1024, 1 <= n_probes <= min(C, 1024); ids uint64
+ * [nq][k], distances float32 [nq][k].  Enqueued on `stream` apart from the synchronisations of the centroid search. */
+int svsb200_ivf_search_device(svsb200_ivf* index, const void* d_queries, int qdtype, size_t nq, size_t k, size_t n_probes,
+                              uint64_t* d_out_ids, float* d_out_dists, void* stream);
+/* The same with HOST buffers (blocking). */
+int svsb200_ivf_search(svsb200_ivf* index, const void* queries, int qdtype, size_t nq, size_t k, size_t n_probes,
+                       uint64_t* out_ids, float* out_dists);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1,0 +1,14 @@
+# oracle/ivf.mk -- the reference's IVF index façade.  TEST INFRASTRUCTURE ONLY (see README.md).
+#
+#   make -f ivf.mk ivf -> _ref/libsvsref_ivf.so   ref/ivf_capi.cpp over the UNMODIFIED reference headers (with the
+#                                                 own ref/shims/mkl.h standing in for the BLAS), linked with the same
+#                                                 distance-kernel objects as _ref/libsvsref.so (flags and rules from Makefile)
+include Makefile
+
+.PHONY: ivf
+ivf: $(OUT)/libsvsref_ivf.so
+
+$(OUT)/ivf_capi.o: ref/ivf_capi.cpp ref/shims/mkl.h ref/shims/toml++/toml.h | $(OUT)/inc/fmt
+	$(CXX) $(REF_CXX) -march=x86-64 -mtune=generic -c $< -o $@
+$(OUT)/libsvsref_ivf.so: $(OUT)/ivf_capi.o $(OUT)/avx512.o $(OUT)/avx2.o
+	$(CXX) -shared -o $@ $^ -lpthread

@@ -33,6 +33,9 @@ SYMBOLS = [
     "svsb200_dynamic_flat_add", "svsb200_dynamic_flat_delete", "svsb200_dynamic_flat_compact", "svsb200_dynamic_flat_ids",
     "svsb200_dynamic_flat_has_id", "svsb200_dynamic_flat_export", "svsb200_dynamic_flat_search",
     "svsb200_dynamic_flat_search_device",
+    "svsb200_ivf_random", "svsb200_ivf_cluster", "svsb200_ivf_create", "svsb200_ivf_destroy", "svsb200_ivf_size",
+    "svsb200_ivf_dimensions", "svsb200_ivf_num_clusters", "svsb200_ivf_device_bytes", "svsb200_ivf_cluster_sizes",
+    "svsb200_ivf_centroids", "svsb200_ivf_search", "svsb200_ivf_search_device",
 ]
 
 _lib = None
@@ -125,6 +128,17 @@ def lib() -> C.CDLL:
     l.svsb200_dynamic_flat_export.argtypes = [vp, vp, vp]
     l.svsb200_dynamic_flat_search.argtypes = [vp, vp, i32, sz, sz, vp, vp]
     l.svsb200_dynamic_flat_search_device.argtypes = [vp, vp, i32, sz, sz, vp, vp, vp, C.POINTER(u32)]
+    l.svsb200_ivf_random.argtypes = [C.c_uint64, sz, vp]
+    l.svsb200_ivf_cluster.argtypes = [vp, i32, sz, sz, i32, sz, sz, sz, i32, C.c_float, C.c_uint64, i32, vp, vp]
+    l.svsb200_ivf_create.argtypes = [vp, i32, sz, sz, i32, vp, sz, vp, i32, C.POINTER(vp)]
+    l.svsb200_ivf_destroy.argtypes = [vp]
+    for name in ("size", "dimensions", "num_clusters", "device_bytes"):
+        fn = getattr(l, f"svsb200_ivf_{name}")
+        fn.restype, fn.argtypes = sz, [vp]
+    l.svsb200_ivf_cluster_sizes.argtypes = [vp, vp]
+    l.svsb200_ivf_centroids.argtypes = [vp, vp]
+    l.svsb200_ivf_search.argtypes = [vp, vp, i32, sz, sz, sz, vp, vp]
+    l.svsb200_ivf_search_device.argtypes = [vp, vp, i32, sz, sz, sz, vp, vp, vp]
     _lib = l
     return l
 

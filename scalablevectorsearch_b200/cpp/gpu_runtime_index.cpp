@@ -16,7 +16,14 @@
 // (bindings/cpp/src/flat_index_impl.h, flat_index.cpp): FP32 storage only, the first `add` creates the index and a
 // second one is NOT_IMPLEMENTED, a search before it is NOT_INITIALIZED with labels -1 and distances +inf, k = 0 is
 // INVALID_ARGUMENT.  Divergence: k > 1024 is INVALID_ARGUMENT (the GPU search returns at most 1024 neighbours).
+//
+// And `svs::runtime::v0::IVFIndex` (bindings/cpp/include/svs/runtime/ivf_index.h) on the IVF index of libsvsb200
+// (svsb200_ivf_*) for FP32 and FP16 storage: `build` clusters (svsb200_ivf_cluster) and assembles the index, `search`
+// probes n_probes clusters (the build's default search parameters, overridden per call).  A non-null IDFilter, save /
+// load, LeanVec and the other storage kinds are NOT_IMPLEMENTED; is_hierarchical must be false (the GPU k-means is
+// flat), and unspecified build parameters take the Python IVFBuildParameters' defaults.
 #include "svs/runtime/flat_index.h"
+#include "svs/runtime/ivf_index.h"
 #include "svs/runtime/vamana_index.h"
 
 #include "svsb200.h"
@@ -44,6 +51,7 @@ void Status::destroy_message() noexcept {
 
 VamanaIndex::~VamanaIndex() = default;
 FlatIndex::~FlatIndex() = default;
+IVFIndex::~IVFIndex() = default;
 
 namespace {
 
@@ -381,6 +389,151 @@ Status FlatIndex::map_to_memory(FlatIndex** index, void*, size_t, MetricType, si
     if (index) *index = nullptr;
     if (read_bytes) *read_bytes = 0;
     return Status(ErrorCode::NOT_IMPLEMENTED, "map_to_memory stays on the reference's CPU library");
+}
+
+// ---- IVFIndex ----
+namespace {
+
+class GpuIVFIndex final : public IVFIndex {
+  public:
+    GpuIVFIndex(svsb200_ivf* index, const SearchParams& sp, size_t threads, size_t intra)
+        : index_(index), sp_(sp), threads_(threads), intra_(intra) {}
+    ~GpuIVFIndex() override { svsb200_ivf_destroy(index_); }
+
+    Status search(size_t n, const float* x, size_t k, float* distances, size_t* labels, const SearchParams* params,
+                  IDFilter* filter) const noexcept override {
+        if (filter) return Status(ErrorCode::NOT_IMPLEMENTED, "filtered IVF search is not available on the GPU");
+        if (k == 0) return Status(ErrorCode::INVALID_ARGUMENT, "k must be greater than 0");
+        if (n == 0) return Status_Ok;
+        size_t n_probes = is_specified(sp_.n_probes) ? sp_.n_probes : 1;
+        float k_reorder = is_specified(sp_.k_reorder) ? sp_.k_reorder : 1.0f;
+        if (params && is_specified(params->n_probes)) n_probes = params->n_probes;
+        if (params && is_specified(params->k_reorder)) k_reorder = params->k_reorder;
+        if (!(k_reorder >= 1.0f)) return Status(ErrorCode::INVALID_ARGUMENT, "k_reorder must be at least 1");
+        static_assert(sizeof(size_t) == 8, "labels are 64-bit");
+        if (svsb200_ivf_search(index_, x, SVSB200_F32, n, k, n_probes, reinterpret_cast<uint64_t*>(labels), distances))
+            return gpu_error();
+        return Status_Ok;
+    }
+    Status save(std::ostream&) const noexcept override {
+        return Status(ErrorCode::NOT_IMPLEMENTED, "save stays on the reference's CPU index");
+    }
+    Status set_num_threads(size_t n) noexcept override {
+        threads_ = n;
+        return Status_Ok;
+    }
+    Status get_num_threads(size_t* n) const noexcept override {
+        if (n) *n = threads_;
+        return Status_Ok;
+    }
+    Status set_intra_query_threads(size_t n) noexcept override {
+        intra_ = n;
+        return Status_Ok;
+    }
+    Status get_intra_query_threads(size_t* n) const noexcept override {
+        if (n) *n = intra_;
+        return Status_Ok;
+    }
+
+  private:
+    svsb200_ivf* index_;
+    SearchParams sp_;
+    size_t threads_, intra_;
+};
+
+// float -> IEEE binary16, round to nearest even (FP16 storage)
+uint16_t to_half(float f) {
+    uint32_t x;
+    std::memcpy(&x, &f, 4);
+    const uint32_t sign = (x >> 16) & 0x8000u, ax = x & 0x7FFFFFFFu;
+    if (ax >= 0x7F800000u) return uint16_t(sign | 0x7C00u | (ax > 0x7F800000u ? 0x200u : 0u));
+    if (ax >= 0x477FF000u) return uint16_t(sign | 0x7C00u);   // rounds to >= 65520: inf
+    if (ax < 0x38800000u) {                                    // below 2^-14: subnormal half
+        const float v = std::fabs(f) * 16777216.0f;            // exact scaling by 2^24
+        return uint16_t(sign | uint32_t(std::nearbyint(v)));
+    }
+    const uint32_t mant = ax & 0x7FFFFFu, exp = (ax >> 23) - 112;
+    uint32_t h = (exp << 10) | (mant >> 13);
+    const uint32_t rest = mant & 0x1FFFu;
+    if (rest > 0x1000u || (rest == 0x1000u && (h & 1u))) ++h;
+    return uint16_t(sign | h);
+}
+
+}  // namespace
+
+Status IVFIndex::check_storage_kind(StorageKind kind) noexcept {
+    return kind == StorageKind::FP32 || kind == StorageKind::FP16
+               ? Status_Ok
+               : Status(ErrorCode::NOT_IMPLEMENTED, "IVFIndex on the GPU supports FP32 and FP16 storage only");
+}
+
+Status IVFIndex::build(IVFIndex** index, size_t dim, MetricType metric, StorageKind storage_kind, size_t n, const float* data,
+                       const BuildParams& params, const SearchParams& default_search_params, size_t num_threads,
+                       size_t intra_query_threads) noexcept {
+    if (!index) return Status(ErrorCode::INVALID_ARGUMENT, "null output");
+    *index = nullptr;
+    if (Status st = check_storage_kind(storage_kind); !st.ok()) return st;
+    if (dim == 0 || n == 0 || !data) return Status(ErrorCode::INVALID_ARGUMENT, "no data");
+    try {
+        const size_t C = is_specified(params.num_centroids) ? params.num_centroids : 1000;
+        const size_t minibatch = is_specified(params.minibatch_size) ? params.minibatch_size : 10000;
+        const size_t iters = is_specified(params.num_iterations) ? params.num_iterations : 10;
+        const int hier = params.is_hierarchical.is_enabled() ? 1 : 0;
+        const float frac = is_specified(params.training_fraction) ? params.training_fraction : 0.1f;
+        const size_t seed = is_specified(params.seed) ? params.seed : 0xC0FFEE;
+        const int m = metric == MetricType::L2 ? SVSB200_L2 : SVSB200_IP;
+        const void* rows = data;
+        int dtype = SVSB200_F32;
+        std::vector<uint16_t> half;
+        if (storage_kind == StorageKind::FP16) {
+            half.resize(n * dim);
+            for (size_t i = 0; i < n * dim; ++i) half[i] = to_half(data[i]);
+            rows = half.data();
+            dtype = SVSB200_F16;
+        }
+        std::vector<float> centroids(C * dim);
+        std::vector<uint32_t> assignments(n);
+        if (svsb200_ivf_cluster(rows, dtype, n, dim, m, C, minibatch, iters, hier, frac, seed, 0, centroids.data(),
+                                assignments.data()))
+            return gpu_error();
+        svsb200_ivf* h = nullptr;
+        if (svsb200_ivf_create(rows, dtype, n, dim, m, centroids.data(), C, assignments.data(), 0, &h)) return gpu_error();
+        *index = new (std::nothrow) GpuIVFIndex(h, default_search_params, num_threads, intra_query_threads);
+        if (!*index) {
+            svsb200_ivf_destroy(h);
+            return Status(ErrorCode::RUNTIME_ERROR, "out of memory");
+        }
+        return Status_Ok;
+    } catch (...) {
+        return Status(ErrorCode::RUNTIME_ERROR, "out of memory");
+    }
+}
+
+Status IVFIndex::build(IVFIndex** index, size_t dim, MetricType metric, StorageKind storage_kind, size_t n, const float* data,
+                       const BuildParams& params, size_t num_threads, size_t intra_query_threads) noexcept {
+    return build(index, dim, metric, storage_kind, n, data, params, SearchParams{}, num_threads, intra_query_threads);
+}
+
+Status IVFIndex::destroy(IVFIndex* index) noexcept {
+    delete index;
+    return Status_Ok;
+}
+
+Status IVFIndex::load(IVFIndex** index, std::istream&, MetricType, StorageKind, size_t, size_t) noexcept {
+    if (index) *index = nullptr;
+    return Status(ErrorCode::NOT_IMPLEMENTED, "load stays on the reference's CPU library");
+}
+
+Status IVFIndexLeanVec::build(IVFIndex** index, size_t, MetricType, StorageKind, size_t, const float*, size_t,
+                              const IVFIndex::BuildParams&, const IVFIndex::SearchParams&, size_t, size_t) noexcept {
+    if (index) *index = nullptr;
+    return Status(ErrorCode::NOT_IMPLEMENTED, "LeanVec storage is not available on the GPU");
+}
+Status IVFIndexLeanVec::build(IVFIndex** index, size_t, MetricType, StorageKind, size_t, const float*,
+                              const LeanVecTrainingData*, const IVFIndex::BuildParams&, const IVFIndex::SearchParams&, size_t,
+                              size_t) noexcept {
+    if (index) *index = nullptr;
+    return Status(ErrorCode::NOT_IMPLEMENTED, "LeanVec storage is not available on the GPU");
 }
 
 }  // SVS_DECLARE_NAMESPACE_VERSION(0)

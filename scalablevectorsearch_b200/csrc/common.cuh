@@ -123,6 +123,7 @@ constexpr size_t kSmemOptInMax = 227 * 1024;   // dynamic shared memory a block 
 //   builder search (HIST), builder prune          DataRows    L2F IPF COSF   L2I IPI COSI      -
 //   consolidate pool, dynamic search (MUT)        DynamicRows L2F IPF COSF   -                 -
 //   flat rescore                                  DataRows    L2F IPF        L2F IPF L2I IPI   -
+//   IVF leaf scan (ivf_kernel.cuh)                IvfRows     L2F IPF COSF   -                 -
 // int8 / uint8 rows take float and integer queries in a search; the builder's datum is its own query.
 template <int... V> struct IntList {};
 template <int ROWT> constexpr bool kIntRow = ROWT == SVSB200_I8 || ROWT == SVSB200_U8;
@@ -138,6 +139,8 @@ using SearchOps = std::conditional_t<ROWT == ROW_LVQ8, IntList<OP_L2F, OP_IPF>,
                                                         FloatOps>>;
 template <int ROWT> using BuildOps = std::conditional_t<kIntRow<ROWT>, IntOps, FloatOps>;
 using DynamicOps = FloatOps;
+using IvfRows = IntList<SVSB200_F32, SVSB200_F16>;
+using IvfOps = FloatOps;
 template <int ROWT>
 using RescoreOps = std::conditional_t<kIntRow<ROWT>, IntList<OP_L2F, OP_IPF, OP_L2I, OP_IPI>, IntList<OP_L2F, OP_IPF>>;
 

@@ -1180,13 +1180,6 @@ static void flat_plan_rows(size_t nq, size_t n, uint32_t kc, int sm_count, uint3
 
 }  // namespace svsb200
 
-// A flat index: the rows of an svsb200_index on one device, with no adjacency.  The exact scan walks the rows in blocks
-// of deg_pad = round_up(gstride, 32) candidates and reads nothing else of the graph (search_kernel.cuh, EXH); the
-// block is 32 rows, as for a Vamana index of degree <= 32.
-struct svsb200_flat {
-    std::unique_ptr<svsb200_index> ix;
-};
-
 using namespace svsb200;
 
 // The two search bodies behind the four entry points here and the dynamic flat index's two (dynamic_flat.cu): `who`

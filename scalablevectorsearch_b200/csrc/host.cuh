@@ -276,6 +276,13 @@ struct svsb200_index {
     size_t dyn_window = 0, dyn_max_candidates = 0, dyn_prune_to = 0;
 };
 
+// A flat index: the rows of an svsb200_index on one device, with no adjacency.  The exact scan walks the rows in blocks
+// of deg_pad = round_up(gstride, 32) candidates and reads nothing else of the graph (search_kernel.cuh, EXH); the
+// block is 32 rows, as for a Vamana index of degree <= 32.  (flat.cu; the IVF index holds its centroids in one.)
+struct svsb200_flat {
+    std::unique_ptr<svsb200_index> ix;
+};
+
 namespace svsb200 {
 
 // Query preparation == distance::maybe_fix_argument for the whole batch (concepts/distance.h:90-130).

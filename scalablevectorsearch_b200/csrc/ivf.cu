@@ -1,0 +1,526 @@
+// ivf.cu -- the IVF index of the C ABI (include/svsb200.h, svsb200_ivf_*): k-means clustering, the cluster-major
+// layout and the search (DESIGN.md §15).
+//
+// Search, per chunk of queries:
+//   1. probe: the flat search (flat.cu) over the centroids with k = n_probes -- exact distances of the search path,
+//      ties to the lower centroid (the reference ranks centroids from an sgemm, ivf/common.h:641-684, 854-888);
+//   2. the queries prepared as for the scan (prepare_queries);
+//   3. inversion: the probes [nq][P] become per-cluster lists of (query, probe), ascending (count, scan, fill, sort);
+//   4. ivf_scan_kernel (ivf_kernel.cuh): one work item per (cluster, chunk of up to Q queries), writing the top k of
+//      every (query, probe) as [P][nq][k];
+//   5. merge_topk_kernel (search.cu) merges the P lists of a query with TotalOrder into [nq][k].
+// The per-(query, probe) lists are kept under IVF_LIST_BUDGET bytes by cutting the batch into query chunks.
+#include "host.cuh"
+#include "ivf_kernel.cuh"
+
+#include <algorithm>
+#include <cmath>
+#include <map>
+#include <numeric>
+#include <vector>
+
+namespace svsb200 {
+
+constexpr size_t IVF_LIST_BUDGET = size_t(256) << 20;   // bytes of per-(query, probe) lists per query chunk
+constexpr size_t IVF_MAX_CHUNK = 8192;                  // queries per chunk (a cluster's list is sorted in shared memory)
+constexpr size_t IVF_MIN_TRAINING_SAMPLE_MULTIPLIER = 2;   // common.h:66
+constexpr double IVF_EPSILON = 1.0 / 1024.0;               // common.h:59
+
+// ---- the documented random sequence (splitmix64) ----
+static uint64_t ivf_next(uint64_t& s) {
+    uint64_t z = (s += 0x9E3779B97F4A7C15ull);
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    return z ^ (z >> 31);
+}
+static float ivf_uniform(uint64_t& s) { return float(ivf_next(s) >> 40) * 0x1p-24f; }
+// The first m of a Fisher-Yates shuffle of [0, n).
+static std::vector<uint32_t> ivf_shuffle_prefix(uint64_t& s, size_t n, size_t m) {
+    std::vector<uint32_t> perm(n);
+    std::iota(perm.begin(), perm.end(), 0u);
+    for (size_t i = 0; i < m; ++i) std::swap(perm[i], perm[i + ivf_next(s) % (n - i)]);
+    perm.resize(m);
+    return perm;
+}
+
+// normalize_centroids (common.h:342-363): x * (1 / norm), the norm a sequential float32 sum of squares.
+static void ivf_normalize(std::vector<float>& cent, size_t C, size_t dim) {
+    for (size_t c = 0; c < C; ++c) {
+        float* x = cent.data() + c * dim;
+        float acc = 0.0f;
+        for (size_t d = 0; d < dim; ++d) {
+            const float sq = x[d] * x[d];
+            acc = acc + sq;
+        }
+        const float norm = std::sqrt(acc);
+        if (norm != 0.0f) {
+            const float inv = 1.0f / norm;
+            for (size_t d = 0; d < dim; ++d) x[d] = x[d] * inv;
+        }
+    }
+}
+
+// centroid_split (common.h:493-537) with the documented sequence.
+static void ivf_split(std::vector<float>& cent, std::vector<uint32_t>& counts, size_t dim, size_t m, uint64_t& s) {
+    const size_t C = counts.size();
+    for (size_t i = 0; i < C; ++i) {
+        if (counts[i] != 0) continue;
+        size_t j = 0;
+        for (;; j = (j + 1) % C) {
+            if (counts[j] == 0) continue;
+            const float p = float(counts[j]) / float(m);
+            if (ivf_uniform(s) < p) break;
+        }
+        float* ci = cent.data() + i * dim;
+        float* cj = cent.data() + j * dim;
+        std::copy(cj, cj + dim, ci);
+        for (size_t d = 0; d < dim; ++d) {
+            const double up = 1.0 + IVF_EPSILON, down = 1.0 - IVF_EPSILON;
+            ci[d] = float(double(ci[d]) * (d % 2 == 0 ? up : down));
+            cj[d] = float(double(cj[d]) * (d % 2 == 0 ? down : up));
+        }
+        counts[i] = counts[j] / 2;
+        counts[j] -= counts[i];
+    }
+}
+
+// An own stream for the blocking entry points, destroyed on scope exit.
+struct OwnStream {
+    cudaStream_t s = nullptr;
+    ~OwnStream() {
+        if (s) cudaStreamDestroy(s);
+    }
+};
+
+// The centroids as a graph-free flat index (float32 rows), so that probing and assignment are one flat search.
+static int ivf_centroid_index(const float* centroids, size_t C, size_t dim, int metric, int device,
+                              std::unique_ptr<svsb200_flat>* out) {
+    svsb200_flat* f = nullptr;
+    if (int rc = svsb200_flat_index_create(centroids, SVSB200_F32, C, dim, 0, metric, device, &f)) return rc;
+    out->reset(f);
+    return 0;
+}
+
+// Nearest centroid of `count` dense rows (device, row_bytes apart) in batches of `batch`, written to d_assign (uint32).
+static int ivf_assign(svsb200_flat* cent, const char* d_rows, int dtype, size_t count, size_t row_bytes, size_t batch,
+                      uint32_t* d_assign, cudaStream_t stream) {
+    DeviceBuffer<uint64_t> ids;
+    DeviceBuffer<float> dists;
+    const size_t b = std::min(batch, count);
+    CUDA_TRY(ids.ensure(std::max<size_t>(b, 1)));
+    CUDA_TRY(dists.ensure(std::max<size_t>(b, 1)));
+    for (size_t lo = 0; lo < count; lo += b) {
+        const size_t nb = std::min(b, count - lo);
+        if (int rc = flat_search_device("svsb200_ivf: assignment", cent->ix.get(), d_rows + lo * row_bytes, dtype, nb, 1,
+                                        ids.ptr, dists.ptr, stream, nullptr, flat_max_kc_deep()))
+            return rc;
+        ivf_narrow_ids_kernel<<<unsigned((nb + 255) / 256), 256, 0, stream>>>(ids.ptr, nb, d_assign + lo);
+        count_launch();
+        CUDA_TRY(cudaGetLastError());
+    }
+    CUDA_TRY(cudaStreamSynchronize(stream));   // (before ids and dists go)
+    return 0;
+}
+
+struct IvfScratch {
+    DeviceBuffer<uint64_t> probe_ids, list_ids;
+    DeviceBuffer<float> probe_dists, list_dists;
+    DeviceBuffer<uint32_t> counts, list_off, item_off, cursor, list;
+};
+
+}  // namespace svsb200
+
+using namespace svsb200;
+
+struct svsb200_ivf {
+    std::unique_ptr<svsb200_index> ix;      // the cluster-major rows (each cluster from a 32-row boundary, zero padding)
+    std::unique_ptr<svsb200_flat> cent;     // the centroids
+    size_t n = 0, C = 0;
+    std::vector<uint32_t> sizes;
+    std::vector<float> centroids;
+    DeviceBuffer<uint32_t> d_row_ids, d_start, d_count;
+    std::mutex mu;
+    std::map<Scratch*, std::unique_ptr<IvfScratch>> scratch;   // per search scratch of ix's replica
+    ~svsb200_ivf() {
+        if (ix) cudaSetDevice(ix->reps[0]->device);
+    }
+};
+
+namespace svsb200 {
+
+template <int ROWT> static cudaError_t launch_ivf_scan(int op, const IvfScanParams& ip, const LaunchConfig& cfg) {
+    return dispatch(IvfOps{}, op, [&](auto o) {
+        constexpr int OP = decltype(o)::value;
+        // rows per group and pass: two where they fit the register bound without spilling, one for float16 rows and
+        // cosine (as for the masked scan)
+        constexpr int NR = ROWT == SVSB200_F16 || OP == OP_COSF ? 1 : 2;
+        return with_shape<OP, true>(ip.p.dim, false, [&](auto ds, auto) {
+            return launch_kernel(ivf_scan_kernel<ROWT, OP, decltype(ds)::value, NR>, cfg, size_t(1) << 20, true, ip);
+        });
+    });
+}
+
+// Queries per chunk: the per-(query, probe) lists under IVF_LIST_BUDGET.
+static size_t ivf_chunk(size_t P, size_t k) {
+    return std::max<size_t>(1, std::min(IVF_MAX_CHUNK, IVF_LIST_BUDGET / (P * k * 12)));
+}
+
+// The search body on device buffers, enqueued on sc->stream (the centroid search synchronises it).
+static int ivf_search_on_device(svsb200_ivf* iv, Scratch* sc, const void* d_queries, int qdtype, size_t nq, size_t k,
+                                size_t P, uint64_t* d_out_ids, float* d_out_dists) {
+    svsb200_index* ix = iv->ix.get();
+    Replica* rep = ix->reps[0].get();
+    cudaStream_t stream = sc->stream;
+    IvfScratch* is = nullptr;
+    {
+        std::lock_guard<std::mutex> lock(iv->mu);
+        auto& slot = iv->scratch[sc];
+        if (!slot) slot = std::make_unique<IvfScratch>();
+        is = slot.get();
+    }
+    const uint32_t C = uint32_t(iv->C), dim = uint32_t(ix->dim), qstride = query_stride(dim);
+    // ring tiles: 32 rows, fewer for rows so wide that two tiles would pass 96 KB
+    uint32_t tile_rows = IVF_TILE_ROWS;
+    while (tile_rows > 1 && 2 * size_t(tile_rows) * ix->row_stride > (size_t(96) << 10)) tile_rows >>= 1;
+    // queries per work item: two CTAs per SM where they fit, else one
+    const size_t fixed = ivf_smem_bytes(ix->row_stride, tile_rows, qstride, uint32_t(k), 0);
+    const size_t slot = ivf_slot_bytes(qstride, uint32_t(k));
+    const size_t limit = kSmemOptInMax - 1024;   // (the kernel's static shared memory)
+    size_t Q = fixed < limit / 2 ? std::min<size_t>(IVF_QMAX, (limit / 2 - fixed) / slot) : 0;
+    if (Q == 0 && fixed < limit) Q = std::min<size_t>(IVF_QMAX, (limit - fixed) / slot);
+    if (Q == 0) return fail("svsb200_ivf_search: k and the row size need more shared memory than a CTA has");
+    const size_t chunk = ivf_chunk(P, k);
+    const size_t qrow = size_t(dim) * esize(qdtype);
+    const size_t cmax = std::min(chunk, nq);
+    CUDA_TRY(is->probe_ids.ensure(cmax * P));
+    CUDA_TRY(is->probe_dists.ensure(cmax * P));
+    CUDA_TRY(is->list_ids.ensure(cmax * P * k));
+    CUDA_TRY(is->list_dists.ensure(cmax * P * k));
+    CUDA_TRY(is->counts.ensure(C));
+    CUDA_TRY(is->list_off.ensure(C + 1));
+    CUDA_TRY(is->item_off.ensure(C + 1));
+    CUDA_TRY(is->cursor.ensure(C));
+    CUDA_TRY(is->list.ensure(cmax * P));
+    int op = ix->metric == SVSB200_L2 ? OP_L2F : ix->metric == SVSB200_IP ? OP_IPF : OP_COSF;
+    for (size_t q0 = 0; q0 < nq; q0 += chunk) {
+        const size_t nqc = std::min(chunk, nq - q0);
+        const char* qp = static_cast<const char*>(d_queries) + q0 * qrow;
+        // 1. probe
+        if (int rc = flat_search_device("svsb200_ivf_search: probe", iv->cent->ix.get(), qp, qdtype, nqc, P,
+                                        is->probe_ids.ptr, is->probe_dists.ptr, stream, nullptr, flat_max_kc_deep()))
+            return rc;
+        // 2. the scan's query operands
+        if (int rc = prepare_queries(ix, rep, sc, qp, qdtype, nqc, PREP_FLOAT, stream)) return rc;
+        // 3. inversion
+        const size_t total = nqc * P;
+        const unsigned tb = unsigned((total + 255) / 256);
+        CUDA_TRY(cudaMemsetAsync(is->counts.ptr, 0, size_t(C) * 4, stream));
+        ivf_count_kernel<<<tb, 256, 0, stream>>>(is->probe_ids.ptr, total, is->counts.ptr);
+        ivf_scan_offsets_kernel<<<1, 1024, 0, stream>>>(is->counts.ptr, C, uint32_t(Q), is->list_off.ptr, is->item_off.ptr,
+                                                         is->cursor.ptr);
+        ivf_fill_kernel<<<tb, 256, 0, stream>>>(is->probe_ids.ptr, total, is->cursor.ptr, is->list.ptr);
+        size_t n2 = 1;
+        while (n2 < nqc) n2 <<= 1;
+        ivf_sort_lists_kernel<<<C, 512, n2 * 4, stream>>>(is->list_off.ptr, is->list.ptr);
+        for (int i = 0; i < 4; ++i) count_launch();
+        CUDA_TRY(cudaGetLastError());
+        // 4. the cluster-major scan
+        IvfScanParams ip{};
+        ip.p.dim = dim;
+        ip.p.row_stride = ix->row_stride;
+        ip.p.greater = ix->metric != SVSB200_L2;
+        ip.p.scale = 1.0f;
+        ip.p.qf = sc->q_f32.ptr;
+        ip.p.qaux = sc->q_aux.ptr;
+        ip.p.qstride = qstride;
+        ip.p.nq = uint32_t(nqc);
+        ip.p.k = uint32_t(k);
+        ip.rows = reinterpret_cast<const char*>(rep->d_vectors.ptr);
+        ip.row_ids = iv->d_row_ids.ptr;
+        ip.cl_start = iv->d_start.ptr;
+        ip.cl_count = iv->d_count.ptr;
+        ip.list_off = is->list_off.ptr;
+        ip.list = is->list.ptr;
+        ip.item_off = is->item_off.ptr;
+        ip.C = C;
+        ip.P = uint32_t(P);
+        ip.nq = uint32_t(nqc);
+        ip.k = uint32_t(k);
+        ip.Q = uint32_t(Q);
+        ip.tile_rows = tile_rows;
+        ip.out_ids = is->list_ids.ptr;
+        ip.out_dists = is->list_dists.ptr;
+        ip.work_counter = sc->d_counter.ptr;
+        CUDA_TRY(cudaMemsetAsync(sc->d_counter.ptr, 0, sizeof(unsigned int), stream));
+        const LaunchConfig cfg{-rep->sm_count, IVF_WARPS, ivf_smem_bytes(ix->row_stride, tile_rows, qstride, uint32_t(k), uint32_t(Q)),
+                               stream};
+        CUDA_TRY(dispatch(IvfRows{}, ix->dtype, [&](auto row) { return launch_ivf_scan<decltype(row)::value>(op, ip, cfg); }));
+        // 5. merge
+        if (int rc = svsb200_merge_topk_device(is->list_ids.ptr, is->list_dists.ptr, P, nqc, k, ix->metric, d_out_ids + q0 * k,
+                                               d_out_dists + q0 * k, rep->device, stream))
+            return rc;
+    }
+    return 0;
+}
+
+static int ivf_check_search(const char* who, const svsb200_ivf* iv, int qdtype, size_t k, size_t n_probes) {
+    const std::string w(who);
+    if (!iv) return fail(w + ": NULL index");
+    if (k == 0 || k > 1024) return fail(w + ": k must be in [1, 1024]");
+    if (n_probes == 0 || n_probes > std::min<size_t>(iv->C, 1024))
+        return fail(w + ": n_probes must be in [1, min(num_clusters, 1024)] = [1, " +
+                    std::to_string(std::min<size_t>(iv->C, 1024)) + "]");
+    if (qdtype != SVSB200_F32 && qdtype != SVSB200_F16) return fail(w + ": queries must be float32 or float16");
+    return 0;
+}
+
+static int ivf_check_rows(const char* who, const void* vectors, int dtype, size_t n, size_t dim, int metric) {
+    const std::string w(who);
+    if (!vectors) return fail(w + ": NULL input");
+    if (dtype != SVSB200_F32 && dtype != SVSB200_F16)
+        return fail(w + ": rows must be float32 or float16 (integer, SQ and LVQ rows are not supported)");
+    if (metric < SVSB200_L2 || metric > SVSB200_COSINE) return fail(w + ": bad metric");
+    if (n == 0 || dim == 0) return fail(w + ": empty dataset");
+    if (n >= (size_t(1) << 31)) return fail(w + ": more than 2^31-1 vectors");
+    return 0;
+}
+
+}  // namespace svsb200
+
+extern "C" {
+
+int svsb200_ivf_random(uint64_t seed, size_t count, uint64_t* out) {
+    if (count && !out) return fail("svsb200_ivf_random: NULL output");
+    for (size_t i = 0; i < count; ++i) out[i] = ivf_next(seed);
+    return 0;
+}
+
+int svsb200_ivf_cluster(const void* vectors, int dtype, size_t n, size_t dim, int metric, size_t num_centroids,
+                        size_t minibatch_size, size_t num_iterations, int is_hierarchical, float training_fraction,
+                        uint64_t seed, int device, float* out_centroids, uint32_t* out_assignments) {
+    const char* who = "svsb200_ivf_cluster";
+    if (int rc = ivf_check_rows(who, vectors, dtype, n, dim, metric)) return rc;
+    if (is_hierarchical)
+        return fail("svsb200_ivf_cluster: is_hierarchical = true: hierarchical k-means is not supported (flat k-means only)");
+    if (!out_centroids || !out_assignments) return fail("svsb200_ivf_cluster: NULL output");
+    const size_t C = num_centroids;
+    if (C == 0) return fail("svsb200_ivf_cluster: num_centroids must be positive");
+    if (minibatch_size == 0) return fail("svsb200_ivf_cluster: minibatch_size must be positive");
+    if (!(training_fraction >= 0.0f) || !std::isfinite(training_fraction))
+        return fail("svsb200_ivf_cluster: training_fraction must be a finite non-negative number");
+    // kmeans.h:54-66
+    const size_t min_training = std::min(C * IVF_MIN_TRAINING_SAMPLE_MULTIPLIER, n);
+    const size_t m = std::min(n, std::max(min_training, size_t(std::ceil(float(n) * training_fraction))));
+    if (m < C)
+        return fail("svsb200_ivf_cluster: insufficient data for clustering: " + std::to_string(m) + " training rows, " +
+                    std::to_string(C) + " centroids required");
+    cudaDeviceProp prop;
+    if (int rc = check_device(who, device, &prop)) return rc;
+    CUDA_TRY(cudaSetDevice(device));
+    const size_t row_bytes = dim * esize(dtype);
+    const char* src = static_cast<const char*>(vectors);
+    // 1-2. training sample and initial centroids
+    uint64_t s = seed;
+    std::vector<uint32_t> sample = ivf_shuffle_prefix(s, n, m);
+    std::sort(sample.begin(), sample.end());
+    const std::vector<uint32_t> init = ivf_shuffle_prefix(s, m, C);
+    std::vector<char> train(m * row_bytes);
+    for (size_t i = 0; i < m; ++i) std::copy(src + size_t(sample[i]) * row_bytes, src + size_t(sample[i] + 1) * row_bytes,
+                                             train.data() + i * row_bytes);
+    std::vector<float> cent(C * dim);
+    for (size_t c = 0; c < C; ++c)
+        for (size_t d = 0; d < dim; ++d) {
+            const char* x = train.data() + size_t(init[c]) * row_bytes;
+            cent[c * dim + d] = dtype == SVSB200_F32 ? reinterpret_cast<const float*>(x)[d]
+                                                     : __half2float(reinterpret_cast<const __half*>(x)[d]);
+        }
+    const bool ip_like = metric != SVSB200_L2;
+    if (ip_like) ivf_normalize(cent, C, dim);
+    OwnStream own;
+    CUDA_TRY(cudaStreamCreateWithFlags(&own.s, cudaStreamNonBlocking));
+    std::unique_ptr<svsb200_flat> cix;
+    if (int rc = ivf_centroid_index(cent.data(), C, dim, metric, device, &cix)) return rc;
+    Replica* crep = cix->ix->reps[0].get();
+    DeviceBuffer<char> d_train;
+    DeviceBuffer<uint32_t> d_assign, d_counts;
+    DeviceBuffer<float> d_cent;
+    CUDA_TRY(d_train.ensure(m * row_bytes));
+    CUDA_TRY(d_assign.ensure(std::max(m, n)));
+    CUDA_TRY(d_counts.ensure(C));
+    CUDA_TRY(d_cent.ensure(C * dim));
+    CUDA_TRY(cudaMemcpy(d_train.ptr, train.data(), m * row_bytes, cudaMemcpyHostToDevice));
+    std::vector<uint32_t> counts(C);
+    // 3. iterations
+    for (size_t it = 0; it < num_iterations; ++it) {
+        if (int rc = ivf_assign(cix.get(), d_train.ptr, dtype, m, row_bytes, minibatch_size, d_assign.ptr, own.s)) return rc;
+        CUDA_TRY(cudaMemcpyAsync(d_cent.ptr, cent.data(), C * dim * 4, cudaMemcpyHostToDevice, own.s));
+        const unsigned warps = 8;
+        const LaunchConfig cfg{int((C + warps - 1) / warps), int(warps), 0, own.s};
+        CUDA_TRY(dispatch(IvfRows{}, dtype, [&](auto row) {
+            return launch_kernel(ivf_kmeans_update_kernel<decltype(row)::value>, cfg, size_t(cfg.grid), false,
+                                 static_cast<const char*>(d_train.ptr), uint32_t(row_bytes), uint32_t(m), uint32_t(dim),
+                                 static_cast<const uint32_t*>(d_assign.ptr), uint32_t(C), d_cent.ptr, d_counts.ptr);
+        }));
+        CUDA_TRY(cudaMemcpyAsync(cent.data(), d_cent.ptr, C * dim * 4, cudaMemcpyDeviceToHost, own.s));
+        CUDA_TRY(cudaMemcpyAsync(counts.data(), d_counts.ptr, C * 4, cudaMemcpyDeviceToHost, own.s));
+        CUDA_TRY(cudaStreamSynchronize(own.s));
+        ivf_split(cent, counts, dim, m, s);
+        if (ip_like) ivf_normalize(cent, C, dim);
+        // the centroid index takes the new rows; its GEMM operands are rebuilt by the next search
+        CUDA_TRY(cudaMemcpy2D(crep->d_vectors.ptr, cix->ix->row_stride, cent.data(), dim * 4, dim * 4, C, cudaMemcpyHostToDevice));
+        flat_slots_reset(crep);
+    }
+    // 4. final assignment of every row
+    DeviceBuffer<char> d_rows;
+    CUDA_TRY(d_rows.ensure(n * row_bytes));
+    CUDA_TRY(cudaMemcpy(d_rows.ptr, vectors, n * row_bytes, cudaMemcpyHostToDevice));
+    if (int rc = ivf_assign(cix.get(), d_rows.ptr, dtype, n, row_bytes, minibatch_size, d_assign.ptr, own.s)) return rc;
+    CUDA_TRY(cudaMemcpy(out_assignments, d_assign.ptr, n * 4, cudaMemcpyDeviceToHost));
+    std::copy(cent.begin(), cent.end(), out_centroids);
+    return 0;
+}
+
+int svsb200_ivf_create(const void* vectors, int dtype, size_t n, size_t dim, int metric, const float* centroids,
+                       size_t num_centroids, const uint32_t* assignments, int device, svsb200_ivf** out) {
+    const char* who = "svsb200_ivf_create";
+    if (!out) return fail("svsb200_ivf_create: out is NULL");
+    *out = nullptr;
+    if (int rc = ivf_check_rows(who, vectors, dtype, n, dim, metric)) return rc;
+    const size_t C = num_centroids;
+    if (!centroids) return fail("svsb200_ivf_create: NULL centroids");
+    if (C == 0 || C >= (size_t(1) << 31)) return fail("svsb200_ivf_create: num_centroids must be in [1, 2^31)");
+    if (assignments)
+        for (size_t i = 0; i < n; ++i)
+            if (assignments[i] >= C) return fail("svsb200_ivf_create: assignment " + std::to_string(i) + " is not a cluster");
+    cudaDeviceProp prop;
+    if (int rc = check_device(who, device, &prop)) return rc;
+    CUDA_TRY(cudaSetDevice(device));
+    auto iv = std::make_unique<svsb200_ivf>();
+    iv->n = n;
+    iv->C = C;
+    iv->centroids.assign(centroids, centroids + C * dim);
+    if (int rc = ivf_centroid_index(centroids, C, dim, metric, device, &iv->cent)) return rc;
+    const size_t row_bytes = dim * esize(dtype);
+    std::vector<uint32_t> assign(n);
+    if (assignments) {
+        std::copy(assignments, assignments + n, assign.begin());
+    } else {
+        OwnStream own;
+        CUDA_TRY(cudaStreamCreateWithFlags(&own.s, cudaStreamNonBlocking));
+        DeviceBuffer<char> d_rows;
+        DeviceBuffer<uint32_t> d_assign;
+        CUDA_TRY(d_rows.ensure(n * row_bytes));
+        CUDA_TRY(d_assign.ensure(n));
+        CUDA_TRY(cudaMemcpy(d_rows.ptr, vectors, n * row_bytes, cudaMemcpyHostToDevice));
+        if (int rc = ivf_assign(iv->cent.get(), d_rows.ptr, dtype, n, row_bytes, 65536, d_assign.ptr, own.s)) return rc;
+        CUDA_TRY(cudaMemcpy(assign.data(), d_assign.ptr, n * 4, cudaMemcpyDeviceToHost));
+    }
+    // cluster-major layout: clusters in order, each from a 32-row boundary, its rows in ascending id
+    iv->sizes.assign(C, 0);
+    for (uint32_t a : assign) ++iv->sizes[a];
+    std::vector<uint32_t> start(C), fill(C);
+    size_t stored = 0;
+    for (size_t c = 0; c < C; ++c) {
+        start[c] = uint32_t(stored);
+        fill[c] = uint32_t(stored);
+        stored += round_up(iv->sizes[c], 32);
+    }
+    if (stored >= (size_t(1) << 32)) return fail("svsb200_ivf_create: too many rows");
+    auto ix = std::make_unique<svsb200_index>();
+    ix->dtype = dtype;
+    ix->metric = metric;
+    ix->storage = SVSB200_PLAIN;
+    ix->n = std::max<size_t>(stored, 1);
+    ix->dim = dim;
+    ix->row_stride = data_row_stride(SVSB200_PLAIN, dtype, dim);
+    ix->gstride = 32;
+    std::vector<uint32_t> row_ids(ix->n, 0xFFFFFFFFu);
+    std::vector<char> rows(ix->n * size_t(ix->row_stride), 0);
+    const char* src = static_cast<const char*>(vectors);
+    for (size_t i = 0; i < n; ++i) {
+        const uint32_t r = fill[assign[i]]++;
+        row_ids[r] = uint32_t(i);
+        std::copy(src + i * row_bytes, src + (i + 1) * row_bytes, rows.data() + size_t(r) * ix->row_stride);
+    }
+    ix->reps.push_back(std::make_unique<Replica>());
+    Replica* rep = ix->reps.back().get();
+    rep->device = device;
+    rep->sm_count = prop.multiProcessorCount;
+    CUDA_TRY(rep->d_vectors.ensure(rows.size()));
+    CUDA_TRY(cudaMemcpy(rep->d_vectors.ptr, rows.data(), rows.size(), cudaMemcpyHostToDevice));
+    CUDA_TRY(iv->d_row_ids.ensure(row_ids.size()));
+    CUDA_TRY(cudaMemcpy(iv->d_row_ids.ptr, row_ids.data(), row_ids.size() * 4, cudaMemcpyHostToDevice));
+    CUDA_TRY(iv->d_start.ensure(C));
+    CUDA_TRY(cudaMemcpy(iv->d_start.ptr, start.data(), C * 4, cudaMemcpyHostToDevice));
+    CUDA_TRY(iv->d_count.ensure(C));
+    CUDA_TRY(cudaMemcpy(iv->d_count.ptr, iv->sizes.data(), C * 4, cudaMemcpyHostToDevice));
+    ix->device_bytes = rows.size() + row_ids.size() * 4 + C * 8 + iv->cent->ix->device_bytes;
+    iv->ix = std::move(ix);
+    *out = iv.release();
+    return 0;
+}
+
+int svsb200_ivf_destroy(svsb200_ivf* index) {
+    delete index;
+    return 0;
+}
+
+size_t svsb200_ivf_size(const svsb200_ivf* index) { return index ? index->n : 0; }
+size_t svsb200_ivf_dimensions(const svsb200_ivf* index) { return index ? index->ix->dim : 0; }
+size_t svsb200_ivf_num_clusters(const svsb200_ivf* index) { return index ? index->C : 0; }
+size_t svsb200_ivf_device_bytes(const svsb200_ivf* index) { return index ? index->ix->device_bytes : 0; }
+
+int svsb200_ivf_cluster_sizes(const svsb200_ivf* index, uint32_t* out) {
+    if (!index || !out) return fail("svsb200_ivf_cluster_sizes: NULL argument");
+    std::copy(index->sizes.begin(), index->sizes.end(), out);
+    return 0;
+}
+
+int svsb200_ivf_centroids(const svsb200_ivf* index, float* out) {
+    if (!index || !out) return fail("svsb200_ivf_centroids: NULL argument");
+    std::copy(index->centroids.begin(), index->centroids.end(), out);
+    return 0;
+}
+
+int svsb200_ivf_search_device(svsb200_ivf* index, const void* d_queries, int qdtype, size_t nq, size_t k, size_t n_probes,
+                              uint64_t* d_out_ids, float* d_out_dists, void* stream_) {
+    if (int rc = ivf_check_search("svsb200_ivf_search_device", index, qdtype, k, n_probes)) return rc;
+    if (nq == 0) return 0;
+    if (!d_queries || !d_out_ids || !d_out_dists) return fail("svsb200_ivf_search_device: NULL buffer");
+    Replica* rep = index->ix->reps[0].get();
+    CUDA_TRY(cudaSetDevice(rep->device));
+    std::string err;
+    Scratch* sc = scratch_for_stream(rep, static_cast<cudaStream_t>(stream_), &err);
+    if (!sc) return fail(err);
+    return ivf_search_on_device(index, sc, d_queries, qdtype, nq, k, n_probes, d_out_ids, d_out_dists);
+}
+
+int svsb200_ivf_search(svsb200_ivf* index, const void* queries, int qdtype, size_t nq, size_t k, size_t n_probes,
+                       uint64_t* out_ids, float* out_dists) {
+    if (int rc = ivf_check_search("svsb200_ivf_search", index, qdtype, k, n_probes)) return rc;
+    if (nq == 0) return 0;
+    if (!queries || !out_ids || !out_dists) return fail("svsb200_ivf_search: NULL buffer");
+    Replica* rep = index->ix->reps[0].get();
+    CUDA_TRY(cudaSetDevice(rep->device));
+    std::string err;
+    Scratch* sc = acquire(rep, &err);
+    if (!sc) return fail(err);
+    const int rc = [&]() -> int {
+        const size_t qbytes = nq * index->ix->dim * esize(qdtype);
+        CUDA_TRY(sc->q_raw.ensure(qbytes));
+        CUDA_TRY(sc->ids.ensure(nq * k * 8));
+        CUDA_TRY(sc->dists.ensure(nq * k));
+        CUDA_TRY(cudaMemcpyAsync(sc->q_raw.ptr, queries, qbytes, cudaMemcpyHostToDevice, sc->stream));
+        if (int rc = ivf_search_on_device(index, sc, sc->q_raw.ptr, qdtype, nq, k, n_probes,
+                                          reinterpret_cast<uint64_t*>(sc->ids.ptr), sc->dists.ptr))
+            return rc;
+        CUDA_TRY(cudaMemcpyAsync(out_ids, sc->ids.ptr, nq * k * 8, cudaMemcpyDeviceToHost, sc->stream));
+        CUDA_TRY(cudaMemcpyAsync(out_dists, sc->dists.ptr, nq * k * 4, cudaMemcpyDeviceToHost, sc->stream));
+        CUDA_TRY(cudaStreamSynchronize(sc->stream));
+        return 0;
+    }();
+    release(rep, sc);
+    return rc;
+}
+
+}  // extern "C"

@@ -1,0 +1,335 @@
+// ivf_kernel.cuh -- kernels of the IVF index (ivf.cu): the cluster-major leaf scan and the k-means update.
+//
+// Replaces, for float32 / float16 rows (file:line under the reference's include/svs):
+//   index/ivf/index.h  IVFIndex::search's leaf scan (one thread per query walks each probed cluster)
+//   index/ivf/common.h:446-490 centroid_adjustment (the k-means update)
+//
+// ivf_scan_kernel: one work item is (cluster, chunk of up to Q queries probing it).  Persistent CTAs pull work items
+// from a counter; a CTA streams the cluster's rows through a two-slot shared-memory ring (cp.async, 16 bytes per
+// copy), so a probed cluster's rows leave HBM once per query chunk instead of once per query.  Each warp scores its
+// queries against every staged tile with the search path's own distance code (float_rows in its shared-memory form,
+// finish_distance), bit for bit, and keeps one sorted top-k list per (query, probe) in shared memory.  A cluster's rows
+// are stored in ascending original id, and a new row goes after an equal old key, so every list is ordered by
+// (distance, original id): the TotalOrder of the merge that follows (merge_topk_kernel).
+#pragma once
+
+#include "search_kernel.cuh"
+
+namespace svsb200 {
+
+constexpr int IVF_WARPS = 8;              // warps per CTA of the scan
+constexpr uint32_t IVF_TILE_ROWS = 32;    // rows per ring slot (fewer for very wide rows: ivf.cu)
+constexpr uint32_t IVF_QMAX = 64;         // queries per work item
+
+struct IvfScanParams {
+    SearchParams p;                 // dim, row_stride, qf / qaux / qstride, greater (the distance code's fields)
+    const char* rows;               // cluster-major rows, each cluster starting on a 32-row boundary
+    const uint32_t* row_ids;        // original id of every stored row
+    const uint32_t* cl_start;       // [C] first stored row of each cluster
+    const uint32_t* cl_count;       // [C] rows of each cluster
+    const uint32_t* list_off;       // [C+1] per-cluster query lists: entries list_off[c] .. list_off[c+1]
+    const uint32_t* list;           // entry = query * P + probe, ascending within a list
+    const uint32_t* item_off;       // [C+1] work items of each cluster (ceil(list length / Q)); item_off[C] = total
+    uint32_t C, P, nq, k, Q, tile_rows;
+    uint64_t* out_ids;              // [P][nq][k] per (probe, query) lists, original ids
+    float* out_dists;
+    unsigned int* work_counter;
+};
+
+// Shared memory of one CTA: the ring, then per query slot {query, keys, ids}, then per warp {candidate keys, positions}.
+__host__ __device__ inline size_t ivf_slot_bytes(uint32_t qstride, uint32_t k) {
+    return size_t(qstride) * 4 + (size_t(k) * 8 + 15) / 16 * 16;
+}
+__host__ __device__ inline size_t ivf_smem_bytes(uint32_t row_stride, uint32_t tile_rows, uint32_t qstride, uint32_t k,
+                                                 uint32_t Q) {
+    return 2 * size_t(tile_rows) * row_stride + size_t(Q) * ivf_slot_bytes(qstride, k) + size_t(IVF_WARPS) * 32 * 8;
+}
+
+// Merges the `count` scored rows of a tile (keys in ckey[0..count), ids ids[0..count), ascending) into the sorted list
+// (bkey, bid) of `size` <= k entries: the result of inserting them one by one, each after the equal keys already there,
+// truncated at k.  Warp-collective.
+__device__ __forceinline__ void ivf_merge(float* bkey, uint32_t* bid, uint32_t& size, uint32_t k, const float* ckey,
+                                          const uint32_t* ids, uint32_t count, uint32_t* spos, int lane) {
+    constexpr unsigned FULL = 0xFFFFFFFFu;
+    const bool valid = uint32_t(lane) < count;
+    const float d = valid ? ckey[lane] : 0.0f;
+    const bool surv = valid && (size < k || d < bkey[size - 1]);
+    const unsigned m = __ballot_sync(FULL, surv);
+    if (!m) return;
+    uint32_t ipos = 0;   // entries with a key <= d: upper bound
+    if (surv) {
+        uint32_t lo = 0, hi = size;
+        while (lo < hi) {
+            const uint32_t mid = (lo + hi) >> 1;
+            if (d < bkey[mid]) hi = mid; else lo = mid + 1;
+        }
+        ipos = lo;
+    }
+    uint32_t rank = 0;   // survivors before this one: smaller keys, or equal keys on lower lanes
+    for (int s = 0; s < 32; ++s) {
+        const float ds = __shfl_sync(FULL, d, s);
+        if (surv && ((m >> s) & 1u)) rank += (ds < d) || (!(d < ds) && s < lane);
+    }
+    const uint32_t S = __popc(m);
+    if (surv) spos[__popc(m & ((1u << lane) - 1u))] = ipos;
+    const uint32_t minpos = __reduce_min_sync(FULL, surv ? ipos : 0xFFFFFFFFu);
+    const uint32_t id = valid ? ids[lane] : 0u;
+    __syncwarp();
+    if (minpos < size) {   // old entries move up by the number of survivors inserted at or before them, top first
+        for (int ch = int((size - 1) >> 5); ch >= int(minpos >> 5); --ch) {
+            const uint32_t j = uint32_t(ch) * 32 + lane;
+            const bool have = j < size;
+            const float kk = have ? bkey[j] : 0.0f;
+            const uint32_t ii = have ? bid[j] : 0u;
+            uint32_t shift = 0;
+            for (uint32_t s = 0; s < S; ++s) shift += spos[s] <= j;
+            __syncwarp();
+            if (have && j + shift < k) {
+                bkey[j + shift] = kk;
+                bid[j + shift] = ii;
+            }
+            __syncwarp();
+        }
+    }
+    const uint32_t fp = ipos + rank;
+    if (surv && fp < k) {
+        bkey[fp] = d;
+        bid[fp] = id;
+    }
+    size = min(size + S, k);
+    __syncwarp();
+}
+
+template <int ROWT, int OP, int DS, int NR>
+__global__ void __launch_bounds__(IVF_WARPS * 32, 2) ivf_scan_kernel(const __grid_constant__ IvfScanParams ip) {
+    constexpr int G = 16 / Row<ROWT>::LPT;   // threads per row
+    constexpr int GROUPS = 32 / G;            // rows per warp and pass
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    const SearchParams& p = ip.p;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int g = lane / G, t = lane % G;
+    const uint32_t tile_bytes = ip.tile_rows * p.row_stride;
+    unsigned char* ring = smem_raw;
+    unsigned char* slots = smem_raw + 2 * size_t(tile_bytes);
+    const size_t slot_bytes = ivf_slot_bytes(p.qstride, ip.k);
+    float* ckey = reinterpret_cast<float*>(slots + size_t(ip.Q) * slot_bytes) + warp * 64;
+    uint32_t* spos = reinterpret_cast<uint32_t*>(ckey + 32);
+    const float ksign = p.greater ? -1.0f : 1.0f;
+    __shared__ uint32_t s_item;
+    __shared__ uint32_t s_size[IVF_QMAX];   // list length of every slot
+    const uint32_t total = ip.item_off[ip.C];
+
+    for (;;) {
+        if (threadIdx.x == 0) s_item = atomicAdd(ip.work_counter, 1u);
+        __syncthreads();
+        const uint32_t item = s_item;
+        __syncthreads();
+        if (item >= total) break;
+        // the cluster of this item: last c with item_off[c] <= item
+        uint32_t lo = 0, hi = ip.C;
+        while (hi - lo > 1) {
+            const uint32_t mid = (lo + hi) >> 1;
+            if (ip.item_off[mid] <= item) lo = mid; else hi = mid;
+        }
+        const uint32_t c = lo;
+        const uint32_t first = ip.list_off[c] + (item - ip.item_off[c]) * ip.Q;
+        const uint32_t nslots = min(ip.Q, ip.list_off[c + 1] - first);
+        const uint32_t count = ip.cl_count[c];
+        const char* crows = ip.rows + size_t(ip.cl_start[c]) * p.row_stride;
+        const uint32_t* cids = ip.row_ids + ip.cl_start[c];
+        const uint32_t ntiles = (count + ip.tile_rows - 1) / ip.tile_rows;
+        auto stage = [&](uint32_t tile) {   // whole tile, padding rows included (the cluster's storage is 32-row aligned)
+            const char* src = crows + size_t(tile) * tile_bytes;
+            unsigned char* dst = ring + (tile & 1u) * tile_bytes;
+            for (uint32_t o = threadIdx.x * 16; o < tile_bytes; o += IVF_WARPS * 32 * 16) cp_async16(dst + o, src + o);
+            cp_async_commit();
+        };
+        if (ntiles) stage(0);
+        // the slots' queries (prepared as for the scan) and empty lists
+        for (uint32_t s = 0; s < nslots; ++s) {
+            const uint32_t q = ip.list[first + s] / ip.P;
+            float* q_s = reinterpret_cast<float*>(slots + s * slot_bytes);
+            for (uint32_t i = threadIdx.x; i < p.qstride; i += IVF_WARPS * 32) q_s[i] = p.qf[size_t(q) * p.qstride + i];
+        }
+        if (threadIdx.x < IVF_QMAX) s_size[threadIdx.x] = 0;
+        __syncthreads();
+        for (uint32_t tile = 0; tile < ntiles; ++tile) {
+            if (tile + 1 < ntiles) {
+                stage(tile + 1);
+                asm volatile("cp.async.wait_group 1;" ::: "memory");
+            } else {
+                cp_async_wait_all();
+            }
+            __syncthreads();
+            const char* trow = reinterpret_cast<const char*>(ring + (tile & 1u) * tile_bytes);
+            const uint32_t rows = min(ip.tile_rows, count - tile * ip.tile_rows);
+#pragma unroll 1
+            for (uint32_t i = 0; i < IVF_QMAX / IVF_WARPS; ++i) {
+                const uint32_t s = warp + IVF_WARPS * i;
+                if (s >= nslots) break;
+                const float* q_s = reinterpret_cast<const float*>(slots + s * slot_bytes);
+                float* bkey = const_cast<float*>(q_s) + p.qstride;
+                uint32_t* bid = reinterpret_cast<uint32_t*>(bkey + ip.k);
+                const uint32_t q = ip.list[first + s] / ip.P;
+                const float aux0 = p.qaux[2 * size_t(q)];
+                for (uint32_t base = 0; base < rows; base += NR * GROUPS) {
+                    const char* rowp[NR];
+                    uint32_t idx[NR];
+#pragma unroll
+                    for (int r = 0; r < NR; ++r) {
+                        idx[r] = base + r * GROUPS + g;
+                        rowp[r] = idx[r] < rows ? trow + size_t(idx[r]) * p.row_stride : nullptr;
+                    }
+                    float sum[NR], nrm[NR];
+                    float_rows<ROWT, OP, DS, NR, false, true>(p, q_s, rowp, t, sum, nrm);
+#pragma unroll
+                    for (int r = 0; r < NR; ++r) {
+                        const float d = finish_distance<OP>(p, sum[r], nrm[r], 0, 0, aux0, 0.0f);
+                        if (t == 0 && rowp[r]) ckey[idx[r]] = __fmul_rn(d, ksign);
+                    }
+                }
+                __syncwarp();
+                uint32_t size = s_size[s];
+                ivf_merge(bkey, bid, size, ip.k, ckey, cids + tile * ip.tile_rows, rows, spos, lane);
+                if (lane == 0) s_size[s] = size;
+            }
+            __syncthreads();   // (the slot is staged again two tiles on)
+        }
+        // the lists out, padded with all-ones ids and the worst distance
+#pragma unroll 1
+        for (uint32_t i = 0; i < IVF_QMAX / IVF_WARPS; ++i) {
+            const uint32_t s = warp + IVF_WARPS * i;
+            if (s >= nslots) break;
+            const float* bkey = reinterpret_cast<const float*>(slots + s * slot_bytes) + p.qstride;
+            const uint32_t* bid = reinterpret_cast<const uint32_t*>(bkey + ip.k);
+            const uint32_t e = ip.list[first + s], q = e / ip.P, probe = e - q * ip.P;
+            const size_t o = (size_t(probe) * ip.nq + q) * ip.k;
+            for (uint32_t j = lane; j < ip.k; j += 32) {
+                const bool v = j < s_size[s];
+                ip.out_ids[o + j] = v ? uint64_t(bid[j]) : ~uint64_t(0);
+                ip.out_dists[o + j] = v ? __fmul_rn(bkey[j], ksign) : (p.greater ? -INFINITY : INFINITY);
+            }
+        }
+        __syncthreads();   // (the slots and s_size are refilled by the next item)
+    }
+}
+
+// ---- inversion of the probes: per-cluster lists of (query, probe), ascending ----
+// counts[c] += 1 for every probe of c.
+__global__ void ivf_count_kernel(const uint64_t* __restrict__ probes, size_t total, uint32_t* __restrict__ counts) {
+    const size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (i < total) atomicAdd(counts + probes[i], 1u);
+}
+// One CTA: list_off = exclusive scan of counts, item_off = exclusive scan of ceil(counts / Q); cursor = list_off.
+__global__ void ivf_scan_offsets_kernel(const uint32_t* __restrict__ counts, uint32_t C, uint32_t Q, uint32_t* __restrict__ list_off,
+                                        uint32_t* __restrict__ item_off, uint32_t* __restrict__ cursor) {
+    __shared__ uint32_t part_l[1024], part_i[1024];
+    const uint32_t per = (C + blockDim.x - 1) / blockDim.x, lo = min(C, threadIdx.x * per), hi = min(C, lo + per);
+    uint32_t sl = 0, si = 0;
+    for (uint32_t c = lo; c < hi; ++c) {
+        sl += counts[c];
+        si += (counts[c] + Q - 1) / Q;
+    }
+    part_l[threadIdx.x] = sl;
+    part_i[threadIdx.x] = si;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        uint32_t al = 0, ai = 0;
+        for (uint32_t i = 0; i < blockDim.x; ++i) {
+            const uint32_t vl = part_l[i], vi = part_i[i];
+            part_l[i] = al;
+            part_i[i] = ai;
+            al += vl;
+            ai += vi;
+        }
+        list_off[C] = al;
+        item_off[C] = ai;
+    }
+    __syncthreads();
+    sl = part_l[threadIdx.x];
+    si = part_i[threadIdx.x];
+    for (uint32_t c = lo; c < hi; ++c) {
+        list_off[c] = sl;
+        cursor[c] = sl;
+        item_off[c] = si;
+        sl += counts[c];
+        si += (counts[c] + Q - 1) / Q;
+    }
+}
+// Every (query, probe) into its cluster's list (in arbitrary order; ivf_sort_lists_kernel orders them).
+__global__ void ivf_fill_kernel(const uint64_t* __restrict__ probes, size_t total, uint32_t* __restrict__ cursor,
+                                uint32_t* __restrict__ list) {
+    const size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (i < total) list[atomicAdd(cursor + probes[i], 1u)] = uint32_t(i);   // i = query * P + probe
+}
+// One CTA per cluster: bitonic sort of its list in shared memory (lists hold distinct entries, so the order is unique).
+__global__ void ivf_sort_lists_kernel(const uint32_t* __restrict__ list_off, uint32_t* __restrict__ list) {
+    extern __shared__ uint32_t buf[];
+    const uint32_t lo = list_off[blockIdx.x], len = list_off[blockIdx.x + 1] - lo;
+    if (len < 2) return;
+    uint32_t n2 = 1;
+    while (n2 < len) n2 <<= 1;
+    for (uint32_t i = threadIdx.x; i < n2; i += blockDim.x) buf[i] = i < len ? list[lo + i] : 0xFFFFFFFFu;
+    __syncthreads();
+    for (uint32_t size = 2; size <= n2; size <<= 1) {
+        for (uint32_t stride = size >> 1; stride; stride >>= 1) {
+            for (uint32_t i = threadIdx.x; i < n2; i += blockDim.x) {
+                const uint32_t j = i ^ stride;
+                if (j > i) {
+                    const bool up = (i & size) == 0;
+                    const uint32_t a = buf[i], b = buf[j];
+                    if ((a > b) == up) {
+                        buf[i] = b;
+                        buf[j] = a;
+                    }
+                }
+            }
+            __syncthreads();
+        }
+    }
+    for (uint32_t i = threadIdx.x; i < len; i += blockDim.x) list[lo + i] = buf[i];
+}
+
+// ---- k-means ----
+// The update of centroid_adjustment (common.h:446-490): one warp per centroid, lanes over the dimensions.  The members
+// are the training rows assigned to it, summed in float32 in ascending row order onto the old centroid; a centroid
+// with members becomes that sum times float(1.0 / (count + 1)) (the old centroid counts as one point); counts[c] is the
+// number of members.
+template <int ROWT>
+__global__ void ivf_kmeans_update_kernel(const char* __restrict__ train, uint32_t row_bytes, uint32_t ntrain, uint32_t dim,
+                                         const uint32_t* __restrict__ assign, uint32_t C, float* __restrict__ cent,
+                                         uint32_t* __restrict__ counts) {
+    const uint32_t c = blockIdx.x * (blockDim.x / 32) + threadIdx.x / 32;
+    const int lane = threadIdx.x & 31;
+    if (c >= C) return;
+    float* row = cent + size_t(c) * dim;
+    uint32_t cnt = 0;
+    for (uint32_t i0 = 0; i0 < ntrain; i0 += 32) {
+        const uint32_t i = i0 + lane;
+        unsigned m = __ballot_sync(0xFFFFFFFFu, i < ntrain && assign[i] == c);
+        cnt += __popc(m);
+        while (m) {
+            const uint32_t r = i0 + __ffs(m) - 1;
+            m &= m - 1;
+            const char* x = train + size_t(r) * row_bytes;
+            for (uint32_t d = lane; d < dim; d += 32) {
+                const float v = ROWT == SVSB200_F32 ? reinterpret_cast<const float*>(x)[d]
+                                                    : __half2float(reinterpret_cast<const __half*>(x)[d]);
+                row[d] = __fadd_rn(row[d], v);
+            }
+        }
+    }
+    if (cnt) {
+        const float inv = __double2float_rn(__ddiv_rn(1.0, double(cnt) + 1.0));
+        for (uint32_t d = lane; d < dim; d += 32) row[d] = __fmul_rn(row[d], inv);
+    }
+    if (lane == 0) counts[c] = cnt;
+}
+
+// probes / assignments: 64-bit search ids -> 32-bit cluster numbers
+__global__ void ivf_narrow_ids_kernel(const uint64_t* __restrict__ in, size_t count, uint32_t* __restrict__ out) {
+    const size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (i < count) out[i] = uint32_t(in[i]);
+}
+
+}  // namespace svsb200

@@ -37,6 +37,7 @@ template <> struct Row<SVSB200_F32> {
     __device__ static __forceinline__ raw_t load(const char* p) {
         return __ldg(reinterpret_cast<const float4*>(p));
     }
+    __device__ static __forceinline__ raw_t lds(const char* p) { return *reinterpret_cast<const float4*>(p); }
     __device__ static __forceinline__ void cvt(const raw_t& r, float (&y)[4]) {
         y[0] = r.x; y[1] = r.y; y[2] = r.z; y[3] = r.w;
     }
@@ -47,6 +48,7 @@ template <> struct Row<SVSB200_F16> {
     __device__ static __forceinline__ raw_t load(const char* p) {
         return __ldg(reinterpret_cast<const uint4*>(p));
     }
+    __device__ static __forceinline__ raw_t lds(const char* p) { return *reinterpret_cast<const uint4*>(p); }
     __device__ static __forceinline__ void cvt(const raw_t& r, float (&y)[8]) {
         // __half2float is exact and honours subnormals, like vcvtph2ps (simd_utils.h:270).
         const uint32_t w[4] = {r.x, r.y, r.z, r.w};
@@ -157,8 +159,9 @@ template <int LPT> __device__ __forceinline__ float reduce_lanes(float (&s)[LPT]
 //   rowp[r]   this thread group's row base pointers (nullptr = inactive slot)
 //   t         thread index inside the group
 // Returns the *raw* reduced sums (op, norm) -- identical in every thread of the group.
+// SMEM = true: the rows are staged in shared memory (the IVF scan, ivf_kernel.cuh); float32 / float16 rows only.
 // ---------------------------------------------------------------------------------------
-template <int ROWT, int OP, int DS, int NROWS, bool DENSE = false>
+template <int ROWT, int OP, int DS, int NROWS, bool DENSE = false, bool SMEM = false>
 __device__ __forceinline__ void float_rows(
     const SearchParams& p, const float* __restrict__ q_s, const char* const (&rowp)[NROWS], int t,
     float (&sum)[NROWS], float (&nrm)[NROWS]) {
@@ -213,7 +216,10 @@ __device__ __forceinline__ void float_rows(
         for (int r = 0; r < NROWS; ++r)
 #pragma unroll
             for (int k = 0; k < 4; ++k)
-                if (DENSE || rowp[r]) raw[r][k] = R::load(rowp[r] + size_t(base + 16 * k + thread_elem) * R::ESIZE);
+                if (DENSE || rowp[r]) {
+                    const char* a = rowp[r] + size_t(base + 16 * k + thread_elem) * R::ESIZE;
+                    if constexpr (SMEM) raw[r][k] = R::lds(a); else raw[r][k] = R::load(a);
+                }
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
             float x[LPT];
@@ -254,8 +260,10 @@ __device__ __forceinline__ void float_rows(
         for (int r = 0; r < NROWS; ++r)
 #pragma unroll
             for (int k = 0; k < 4; ++k)
-                if ((DENSE || rowp[r]) && base + 16 * k + thread_elem < D)
-                    raw[r][k] = R::load(rowp[r] + size_t(base + 16 * k + thread_elem) * R::ESIZE);
+                if ((DENSE || rowp[r]) && base + 16 * k + thread_elem < D) {
+                    const char* a = rowp[r] + size_t(base + 16 * k + thread_elem) * R::ESIZE;
+                    if constexpr (SMEM) raw[r][k] = R::lds(a); else raw[r][k] = R::load(a);
+                }
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
             const int e0 = base + 16 * k + thread_elem;

@@ -1,0 +1,168 @@
+"""IVF index on the GPU, mirroring the reference's ``svs.IVF`` and ``svs.Clustering`` (bindings/python/src/ivf.cpp):
+
+    clustering = Clustering.build(IVFBuildParameters(num_centroids=1024), data, DistanceType.L2)
+    index = IVF.assemble_from_clustering(clustering, data, DistanceType.L2)
+    index.search_parameters = IVFSearchParameters(n_probes=16)
+    I, D = index.search(queries, 10)                   # numpy (nq, k) uint64 / float32
+
+Backed by ``svsb200_ivf_*`` of ``libsvsb200.so``.  The k-means is the reference's flat k-means made deterministic (an own
+documented random sequence, float32 sums in row order), so ``is_hierarchical`` defaults to False here and True is
+refused.  A search returns the exact top k over the probed clusters, bit for bit the distances of the exact scan.
+"""
+from __future__ import annotations
+
+import ctypes as C
+from dataclasses import dataclass
+
+import numpy as np
+
+from . import _lib
+from .vamana import _DTYPE_CODE, DistanceType
+
+
+@dataclass
+class IVFBuildParameters:
+    """``svs.IVFBuildParameters`` (index/ivf/common.h:70-118); ``is_hierarchical`` defaults to False (see module)."""
+    num_centroids: int = 1000
+    minibatch_size: int = 10_000
+    num_iterations: int = 10
+    is_hierarchical: bool = False
+    training_fraction: float = 0.1
+    hierarchical_level1_clusters: int = 0
+    seed: int = 0xC0FFEE
+
+
+@dataclass
+class IVFSearchParameters:
+    """``svs.IVFSearchParameters``: clusters probed per query, and ``k_reorder`` (>= 1), which cannot change the top k
+    of uncompressed rows (the reference only widens its leaf buffer to k_reorder * k and returns the first k)."""
+    n_probes: int = 1
+    k_reorder: float = 1.0
+
+
+def _rows(data) -> np.ndarray:
+    data = data.load() if hasattr(data, "load") else data
+    data = np.ascontiguousarray(data)
+    if data.ndim != 2:
+        raise ValueError("data must be a 2-D array")
+    if data.dtype not in _DTYPE_CODE:
+        raise TypeError(f"unsupported data type {data.dtype}")
+    return data
+
+
+class Clustering:
+    """``svs.Clustering``: centroids float32 [C, dim] and one cluster per data row (uint32 [n])."""
+
+    def __init__(self, centroids, assignments=None):
+        self.centroids = np.ascontiguousarray(centroids, dtype=np.float32)
+        if self.centroids.ndim != 2:
+            raise ValueError("centroids must be [C, dim]")
+        self.assignments = None if assignments is None else np.ascontiguousarray(assignments, dtype=np.uint32)
+
+    @property
+    def num_clusters(self) -> int:
+        return self.centroids.shape[0]
+
+    @staticmethod
+    def build(build_parameters: IVFBuildParameters, data, distance: DistanceType = DistanceType.L2,
+              device: int = 0) -> "Clustering":
+        """``svs.Clustering.build``: the flat k-means on the GPU (``svsb200_ivf_cluster``)."""
+        x = _rows(data)
+        bp = build_parameters
+        n, dim = x.shape
+        centroids = np.empty((int(bp.num_centroids), dim), dtype=np.float32)
+        assignments = np.empty(n, dtype=np.uint32)
+        _lib.check(_lib.lib().svsb200_ivf_cluster(
+            x.ctypes.data, _DTYPE_CODE[x.dtype], n, dim, int(DistanceType(distance)), int(bp.num_centroids),
+            int(bp.minibatch_size), int(bp.num_iterations), int(bool(bp.is_hierarchical)), float(bp.training_fraction),
+            int(bp.seed), int(device), centroids.ctypes.data, assignments.ctypes.data))
+        return Clustering(centroids, assignments)
+
+
+class IVF:
+    """``svs.IVF`` on one CUDA device."""
+
+    def __init__(self, handle, lib, distance: DistanceType):
+        self._h, self._lib, self._distance = handle, lib, distance
+        self.search_parameters = IVFSearchParameters()
+
+    @staticmethod
+    def assemble_from_clustering(clustering: Clustering, data, distance: DistanceType = DistanceType.L2,
+                                 device: int = 0) -> "IVF":
+        """``svs.IVF.assemble_from_clustering``: the rows grouped as the clustering says (a clustering without
+        assignments puts every row in its nearest cluster)."""
+        x = _rows(data)
+        cent = clustering.centroids
+        if cent.shape[1] != x.shape[1]:
+            raise ValueError(f"centroids have {cent.shape[1]} dimensions, data {x.shape[1]}")
+        a = clustering.assignments
+        if a is not None and a.shape != (x.shape[0],):
+            raise ValueError("the clustering has one assignment per data row")
+        lib = _lib.lib()
+        handle = C.c_void_p()
+        _lib.check(lib.svsb200_ivf_create(x.ctypes.data, _DTYPE_CODE[x.dtype], x.shape[0], x.shape[1],
+                                          int(DistanceType(distance)), cent.ctypes.data, cent.shape[0],
+                                          None if a is None else a.ctypes.data, int(device), C.byref(handle)))
+        return IVF(handle, lib, DistanceType(distance))
+
+    def __del__(self):
+        h = getattr(self, "_h", None)
+        if h:
+            self._lib.svsb200_ivf_destroy(h)
+            self._h = None
+
+    @property
+    def size(self) -> int:
+        return self._lib.svsb200_ivf_size(self._h)
+
+    @property
+    def dimensions(self) -> int:
+        return self._lib.svsb200_ivf_dimensions(self._h)
+
+    @property
+    def num_clusters(self) -> int:
+        return self._lib.svsb200_ivf_num_clusters(self._h)
+
+    @property
+    def device_bytes(self) -> int:
+        return self._lib.svsb200_ivf_device_bytes(self._h)
+
+    @property
+    def cluster_sizes(self) -> np.ndarray:
+        out = np.empty(self.num_clusters, dtype=np.uint32)
+        _lib.check(self._lib.svsb200_ivf_cluster_sizes(self._h, out.ctypes.data))
+        return out
+
+    @property
+    def centroids(self) -> np.ndarray:
+        out = np.empty((self.num_clusters, self.dimensions), dtype=np.float32)
+        _lib.check(self._lib.svsb200_ivf_centroids(self._h, out.ctypes.data))
+        return out
+
+    def _n_probes(self) -> int:
+        sp = self.search_parameters
+        if not sp.k_reorder >= 1.0:
+            raise ValueError(f"k_reorder must be at least 1, got {sp.k_reorder}")
+        return int(sp.n_probes)
+
+    def search(self, queries: np.ndarray, n_neighbors: int):
+        """``svs.IVF.search(queries, n_neighbors)`` -> (ids uint64 [nq,k], distances float32 [nq,k])."""
+        n_probes = self._n_probes()
+        q = np.ascontiguousarray(queries)
+        if q.ndim != 2 or q.shape[1] != self.dimensions:
+            raise ValueError(f"queries must be [nq, {self.dimensions}]")
+        if q.dtype not in _DTYPE_CODE:
+            raise TypeError(f"unsupported query type {q.dtype}")
+        nq, k = q.shape[0], int(n_neighbors)
+        ids = np.empty((nq, k), dtype=np.uint64)
+        dists = np.empty((nq, k), dtype=np.float32)
+        _lib.check(self._lib.svsb200_ivf_search(self._h, q.ctypes.data, _DTYPE_CODE[q.dtype], nq, k, n_probes,
+                                                ids.ctypes.data, dists.ctypes.data))
+        return ids, dists
+
+    def search_device(self, d_queries: int, qdtype: np.dtype, nq: int, n_neighbors: int, d_ids: int, d_dists: int,
+                      stream: int = 0) -> None:
+        """Device-buffer form (raw pointers, e.g. ``tensor.data_ptr()``; ids uint64), enqueued on ``stream``."""
+        n_probes = self._n_probes()
+        _lib.check(self._lib.svsb200_ivf_search_device(self._h, d_queries, _DTYPE_CODE[np.dtype(qdtype)], nq,
+                                                       int(n_neighbors), n_probes, d_ids, d_dists, stream or None))
