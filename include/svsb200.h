@@ -508,6 +508,68 @@ int svsb200_ivf_search_device(svsb200_ivf* index, const void* d_queries, int qdt
 int svsb200_ivf_search(svsb200_ivf* index, const void* queries, int qdtype, size_t nq, size_t k, size_t n_probes,
                        uint64_t* out_ids, float* out_dists);
 
+/* Dynamic IVF index.  Replaces: DynamicIVFIndex (include/svs/index/ivf/dynamic_ivf.h) with svs::DynamicIVF: the IVF
+ * index over a mutable set of float32 / float16 rows on one device, L2 / MIP / cosine, addressed by external ids.  A
+ * distinct handle type.  Every slot (internal id) is Valid or Empty; a delete empties it at once and leaves a tombstone
+ * in its cluster, which no search returns.  The centroids never move after assembly: an added row joins its nearest
+ * centroid, ranked as a probe ranks centroids (the flat search at k = 1, ties to the lower centroid).  External id
+ * 2^64 - 1 is reserved (it marks padding).  Searches may run concurrently with each other; a mutation (add, delete,
+ * compact) first waits for every search of the index enqueued so far, including the work that
+ * svsb200_dynamic_ivf_search_device leaves queued on the caller's stream, so it may follow such a call without a
+ * synchronisation; a search enqueued while a mutation runs is the caller's error. */
+typedef struct svsb200_dynamic_ivf svsb200_dynamic_ivf;
+
+/* assemble_from_clustering: n x dim rows (HOST) with one distinct external id each, grouped by `assignments` (uint32
+ * [n], each < C; NULL: every row goes to its nearest centroid) around C float32 centroids [C][dim].  Row i takes slot
+ * i.  n = 0 makes an empty index to be filled by svsb200_dynamic_ivf_add. */
+int svsb200_dynamic_ivf_create(const void* vectors, int dtype, size_t n, size_t dim, int metric, const float* centroids,
+                               size_t num_centroids, const uint32_t* assignments, const uint64_t* external_ids, int device,
+                               svsb200_dynamic_ivf** out);
+/* Frees the handle and its device memory (NULL is ignored). */
+int svsb200_dynamic_ivf_destroy(svsb200_dynamic_ivf* index);
+/* Valid rows, slots (Valid or Empty), dimensions, clusters, and the device memory held (rows pool with its dead
+ * regions until a compaction, entries, statuses, external ids, centroids); 0 for NULL. */
+size_t svsb200_dynamic_ivf_size(const svsb200_dynamic_ivf* index);
+size_t svsb200_dynamic_ivf_num_slots(const svsb200_dynamic_ivf* index);
+size_t svsb200_dynamic_ivf_dimensions(const svsb200_dynamic_ivf* index);
+size_t svsb200_dynamic_ivf_num_clusters(const svsb200_dynamic_ivf* index);
+size_t svsb200_dynamic_ivf_device_bytes(const svsb200_dynamic_ivf* index);
+/* Valid rows per cluster (uint32 [C]) and the centroids (float32 [C][dim]), HOST buffers. */
+int svsb200_dynamic_ivf_cluster_sizes(const svsb200_dynamic_ivf* index, uint32_t* out);
+int svsb200_dynamic_ivf_centroids(const svsb200_dynamic_ivf* index, float* out);
+/* add_points (dynamic_ivf.h:474-527): `count` rows of the index's dtype (dense, HOST) with one new external id each.
+ * Without reuse_empty every row takes a new slot past the end; with it, Empty slots are taken in ascending order from
+ * slot 0 first.  Each row is appended to its nearest centroid's cluster, in input order.  Everything (dtype, repeated,
+ * present or reserved ids, 2^31-1 slots) is checked before anything changes.  `slots_out` (optional, `count` entries)
+ * receives the slots used. */
+int svsb200_dynamic_ivf_add(svsb200_dynamic_ivf* index, const void* vectors, int dtype, size_t count, const uint64_t* ids,
+                            int reuse_empty, uint64_t* slots_out);
+/* delete_entries (dynamic_ivf.h:547-636): the slots become Empty and their stored rows tombstones.  Fails without
+ * changing anything unless every id is present and listed once. */
+int svsb200_dynamic_ivf_delete(svsb200_dynamic_ivf* index, const uint64_t* ids, size_t count);
+/* compact (dynamic_ivf.h:932-961): the Valid slots are renumbered 0 .. size-1 in slot order, the tombstones dropped;
+ * every cluster keeps the order of its rows and is laid out tightly again.  consolidate is a no-op and has no function
+ * here. */
+int svsb200_dynamic_ivf_compact(svsb200_dynamic_ivf* index);
+/* The external ids of the Valid slots, in slot order (*count: room on entry, out_ids may be NULL; ids on return), and
+ * has_id. */
+int svsb200_dynamic_ivf_ids(const svsb200_dynamic_ivf* index, uint64_t* out_ids, size_t* count);
+int svsb200_dynamic_ivf_has_id(const svsb200_dynamic_ivf* index, uint64_t id, int* out);
+/* The slot state for inspection, per slot: status uint8 (0 Empty, 1 Valid), external id uint64 (2^64 - 1 when Empty)
+ * and cluster uint32 (2^32 - 1 when Empty); slots = svsb200_dynamic_ivf_num_slots.  Any output may be NULL. */
+int svsb200_dynamic_ivf_export(const svsb200_dynamic_ivf* index, uint8_t* status_out, uint64_t* ext_ids_out,
+                               uint32_t* cluster_out);
+/* search: the exact top k (1 <= k <= 1024) over the Valid rows of the n_probes (1 <= n_probes <= min(C, 1024)) probed
+ * clusters, as EXTERNAL ids: the scan's bit-exact distances, ordered by distance, then slot, padded with all-ones ids
+ * and +-inf distances.  With n_probes = C the result is the exact scan over the Valid rows in slot order, its ids mapped
+ * through the slots.  Queries float32 / float16 in DEVICE buffers, enqueued on `stream` apart from the synchronisations
+ * of the centroid search. */
+int svsb200_dynamic_ivf_search_device(svsb200_dynamic_ivf* index, const void* d_queries, int qdtype, size_t nq, size_t k,
+                                      size_t n_probes, uint64_t* d_out_ids, float* d_out_dists, void* stream);
+/* The same with HOST buffers (blocking). */
+int svsb200_dynamic_ivf_search(svsb200_dynamic_ivf* index, const void* queries, int qdtype, size_t nq, size_t k,
+                               size_t n_probes, uint64_t* out_ids, float* out_dists);
+
 #ifdef __cplusplus
 }
 #endif

@@ -9,8 +9,10 @@ from .vamana import (DataType, DistanceType, DynamicVamana, GraphLoader, SearchB
 from .flat import Flat
 from .dynamic_flat import DynamicFlat
 from .ivf import IVF, Clustering, IVFBuildParameters, IVFSearchParameters
+from .dynamic_ivf import DynamicIVF
 from ._lib import Svsb200Error
 
 __all__ = ["DataType", "DistanceType", "GraphLoader", "SearchBufferConfig", "Vamana", "VamanaSearchParameters",
            "VectorDataLoader", "Svsb200Error", "lvq8_compress", "ShardedVamana", "VamanaBuildParameters", "build_graph",
-           "DynamicVamana", "Flat", "DynamicFlat", "IVF", "Clustering", "IVFBuildParameters", "IVFSearchParameters"]
+           "DynamicVamana", "Flat", "DynamicFlat", "IVF", "Clustering", "IVFBuildParameters", "IVFSearchParameters",
+           "DynamicIVF"]

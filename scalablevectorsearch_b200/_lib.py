@@ -36,6 +36,12 @@ SYMBOLS = [
     "svsb200_ivf_random", "svsb200_ivf_cluster", "svsb200_ivf_create", "svsb200_ivf_destroy", "svsb200_ivf_size",
     "svsb200_ivf_dimensions", "svsb200_ivf_num_clusters", "svsb200_ivf_device_bytes", "svsb200_ivf_cluster_sizes",
     "svsb200_ivf_centroids", "svsb200_ivf_search", "svsb200_ivf_search_device",
+    "svsb200_dynamic_ivf_create", "svsb200_dynamic_ivf_destroy", "svsb200_dynamic_ivf_size",
+    "svsb200_dynamic_ivf_num_slots", "svsb200_dynamic_ivf_dimensions", "svsb200_dynamic_ivf_num_clusters",
+    "svsb200_dynamic_ivf_device_bytes", "svsb200_dynamic_ivf_cluster_sizes", "svsb200_dynamic_ivf_centroids",
+    "svsb200_dynamic_ivf_add", "svsb200_dynamic_ivf_delete", "svsb200_dynamic_ivf_compact", "svsb200_dynamic_ivf_ids",
+    "svsb200_dynamic_ivf_has_id", "svsb200_dynamic_ivf_export", "svsb200_dynamic_ivf_search",
+    "svsb200_dynamic_ivf_search_device",
 ]
 
 _lib = None
@@ -139,6 +145,21 @@ def lib() -> C.CDLL:
     l.svsb200_ivf_centroids.argtypes = [vp, vp]
     l.svsb200_ivf_search.argtypes = [vp, vp, i32, sz, sz, sz, vp, vp]
     l.svsb200_ivf_search_device.argtypes = [vp, vp, i32, sz, sz, sz, vp, vp, vp]
+    l.svsb200_dynamic_ivf_create.argtypes = [vp, i32, sz, sz, i32, vp, sz, vp, vp, i32, C.POINTER(vp)]
+    l.svsb200_dynamic_ivf_destroy.argtypes = [vp]
+    for name in ("size", "num_slots", "dimensions", "num_clusters", "device_bytes"):
+        fn = getattr(l, f"svsb200_dynamic_ivf_{name}")
+        fn.restype, fn.argtypes = sz, [vp]
+    l.svsb200_dynamic_ivf_cluster_sizes.argtypes = [vp, vp]
+    l.svsb200_dynamic_ivf_centroids.argtypes = [vp, vp]
+    l.svsb200_dynamic_ivf_add.argtypes = [vp, vp, i32, sz, vp, i32, vp]
+    l.svsb200_dynamic_ivf_delete.argtypes = [vp, vp, sz]
+    l.svsb200_dynamic_ivf_compact.argtypes = [vp]
+    l.svsb200_dynamic_ivf_ids.argtypes = [vp, vp, C.POINTER(sz)]
+    l.svsb200_dynamic_ivf_has_id.argtypes = [vp, C.c_uint64, C.POINTER(i32)]
+    l.svsb200_dynamic_ivf_export.argtypes = [vp, vp, vp, vp]
+    l.svsb200_dynamic_ivf_search.argtypes = [vp, vp, i32, sz, sz, sz, vp, vp]
+    l.svsb200_dynamic_ivf_search_device.argtypes = [vp, vp, i32, sz, sz, sz, vp, vp, vp]
     _lib = l
     return l
 

@@ -22,6 +22,15 @@
 // probes n_probes clusters (the build's default search parameters, overridden per call).  A non-null IDFilter, save /
 // load, LeanVec and the other storage kinds are NOT_IMPLEMENTED; is_hierarchical must be false (the GPU k-means is
 // flat), and unspecified build parameters take the Python IVFBuildParameters' defaults.
+//
+// And `svs::runtime::v0::DynamicIVFIndex` (bindings/cpp/include/svs/runtime/dynamic_ivf_index.h) on the dynamic IVF
+// index (svsb200_dynamic_ivf_*) for FP32 and FP16 storage, with the behaviour of the reference's DynamicIVFIndexImpl
+// (bindings/cpp/src/dynamic_ivf_index_impl.h): `build` with rows clusters them as IVFIndex::build does and assembles
+// the index; without rows there is no index until the first `add`, which clusters its own rows; before that, `search`
+// is NOT_INITIALIZED (labels -1, distances +inf), `remove` / `remove_selected` / `consolidate` / `compact` are
+// NOT_INITIALIZED and `has_id` is false.  k = 0 is INVALID_ARGUMENT; a non-null IDFilter, save / load and LeanVec are
+// NOT_IMPLEMENTED.
+#include "svs/runtime/dynamic_ivf_index.h"
 #include "svs/runtime/flat_index.h"
 #include "svs/runtime/ivf_index.h"
 #include "svs/runtime/vamana_index.h"
@@ -532,6 +541,220 @@ Status IVFIndexLeanVec::build(IVFIndex** index, size_t, MetricType, StorageKind,
 Status IVFIndexLeanVec::build(IVFIndex** index, size_t, MetricType, StorageKind, size_t, const float*,
                               const LeanVecTrainingData*, const IVFIndex::BuildParams&, const IVFIndex::SearchParams&, size_t,
                               size_t) noexcept {
+    if (index) *index = nullptr;
+    return Status(ErrorCode::NOT_IMPLEMENTED, "LeanVec storage is not available on the GPU");
+}
+
+// ---- DynamicIVFIndex ----
+namespace {
+
+// Clusters n rows (svsb200_ivf_cluster, unspecified parameters taking the Python defaults) and assembles a dynamic
+// index over them with the given labels.
+Status cluster_and_assemble(size_t dim, MetricType metric, StorageKind kind, const IVFIndex::BuildParams& params, size_t n,
+                            const float* data, const size_t* labels, svsb200_dynamic_ivf** out) {
+    const size_t C = is_specified(params.num_centroids) ? params.num_centroids : 1000;
+    const size_t minibatch = is_specified(params.minibatch_size) ? params.minibatch_size : 10000;
+    const size_t iters = is_specified(params.num_iterations) ? params.num_iterations : 10;
+    const int hier = params.is_hierarchical.is_enabled() ? 1 : 0;
+    const float frac = is_specified(params.training_fraction) ? params.training_fraction : 0.1f;
+    const size_t seed = is_specified(params.seed) ? params.seed : 0xC0FFEE;
+    const int m = metric == MetricType::L2 ? SVSB200_L2 : SVSB200_IP;
+    const void* rows = data;
+    int dtype = SVSB200_F32;
+    std::vector<uint16_t> half;
+    if (kind == StorageKind::FP16) {
+        half.resize(n * dim);
+        for (size_t i = 0; i < n * dim; ++i) half[i] = to_half(data[i]);
+        rows = half.data();
+        dtype = SVSB200_F16;
+    }
+    std::vector<float> centroids(C * dim);
+    std::vector<uint32_t> assignments(n);
+    if (svsb200_ivf_cluster(rows, dtype, n, dim, m, C, minibatch, iters, hier, frac, seed, 0, centroids.data(),
+                            assignments.data()))
+        return gpu_error();
+    static_assert(sizeof(size_t) == 8, "labels are 64-bit");
+    if (svsb200_dynamic_ivf_create(rows, dtype, n, dim, m, centroids.data(), C, assignments.data(),
+                                   reinterpret_cast<const uint64_t*>(labels), 0, out))
+        return gpu_error();
+    return Status_Ok;
+}
+
+Status not_initialized() { return Status(ErrorCode::NOT_INITIALIZED, "Index not initialized"); }
+
+class GpuDynamicIVFIndex final : public DynamicIVFIndex {
+  public:
+    GpuDynamicIVFIndex(size_t dim, MetricType metric, StorageKind kind, const BuildParams& bp, const SearchParams& sp,
+                       size_t threads, size_t intra)
+        : dim_(dim), metric_(metric), kind_(kind), bp_(bp), sp_(sp), threads_(threads), intra_(intra) {}
+    ~GpuDynamicIVFIndex() override {
+        if (index_) svsb200_dynamic_ivf_destroy(index_);
+    }
+    Status init(size_t n, const float* data, const size_t* labels) noexcept {
+        try {
+            return cluster_and_assemble(dim_, metric_, kind_, bp_, n, data, labels, &index_);
+        } catch (...) {
+            return Status(ErrorCode::RUNTIME_ERROR, "out of memory");
+        }
+    }
+
+    Status add(size_t n, const size_t* labels, const float* x, bool reuse_empty) noexcept override {
+        if (n == 0) return Status_Ok;
+        if (!labels || !x) return Status(ErrorCode::INVALID_ARGUMENT, "null input");
+        if (!index_) return init(n, x, labels);   // the first add clusters its own rows (init_impl)
+        try {
+            const void* rows = x;
+            int dtype = SVSB200_F32;
+            std::vector<uint16_t> half;
+            if (kind_ == StorageKind::FP16) {
+                half.resize(n * dim_);
+                for (size_t i = 0; i < n * dim_; ++i) half[i] = to_half(x[i]);
+                rows = half.data();
+                dtype = SVSB200_F16;
+            }
+            if (svsb200_dynamic_ivf_add(index_, rows, dtype, n, reinterpret_cast<const uint64_t*>(labels), reuse_empty ? 1 : 0,
+                                        nullptr))
+                return gpu_error();
+            return Status_Ok;
+        } catch (...) {
+            return Status(ErrorCode::RUNTIME_ERROR, "out of memory");
+        }
+    }
+    Status remove(size_t n, const size_t* labels) noexcept override {
+        if (!index_) return not_initialized();
+        if (svsb200_dynamic_ivf_delete(index_, reinterpret_cast<const uint64_t*>(labels), n)) return gpu_error();
+        return Status_Ok;
+    }
+    Status remove_selected(size_t* num_removed, const IDFilter& selector) noexcept override {
+        if (!index_) return not_initialized();
+        try {
+            size_t count = svsb200_dynamic_ivf_size(index_);
+            std::vector<uint64_t> ids(count), gone;
+            if (svsb200_dynamic_ivf_ids(index_, ids.data(), &count)) return gpu_error();
+            for (size_t i = 0; i < count; ++i)
+                if (selector(size_t(ids[i]))) gone.push_back(ids[i]);
+            if (svsb200_dynamic_ivf_delete(index_, gone.data(), gone.size())) return gpu_error();
+            if (num_removed) *num_removed = gone.size();
+            return Status_Ok;
+        } catch (...) {
+            return Status(ErrorCode::RUNTIME_ERROR, "out of memory");
+        }
+    }
+    Status has_id(bool* exists, size_t id) const noexcept override {
+        if (!exists) return Status(ErrorCode::INVALID_ARGUMENT, "null output");
+        *exists = false;
+        if (!index_) return Status_Ok;
+        int out = 0;
+        if (svsb200_dynamic_ivf_has_id(index_, id, &out)) return gpu_error();
+        *exists = out != 0;
+        return Status_Ok;
+    }
+    Status consolidate() noexcept override { return index_ ? Status_Ok : not_initialized(); }
+    Status compact(size_t) noexcept override {
+        if (!index_) return not_initialized();
+        if (svsb200_dynamic_ivf_compact(index_)) return gpu_error();
+        return Status_Ok;
+    }
+    Status search(size_t n, const float* x, size_t k, float* distances, size_t* labels, const SearchParams* params,
+                  IDFilter* filter) const noexcept override {
+        if (!index_) {
+            for (size_t i = 0; i < n * k; ++i) {
+                labels[i] = size_t(-1);
+                distances[i] = INFINITY;
+            }
+            return not_initialized();
+        }
+        if (filter) return Status(ErrorCode::NOT_IMPLEMENTED, "filtered IVF search is not available on the GPU");
+        if (k == 0) return Status(ErrorCode::INVALID_ARGUMENT, "k must be greater than 0");
+        if (n == 0) return Status_Ok;
+        size_t n_probes = is_specified(sp_.n_probes) ? sp_.n_probes : 1;
+        float k_reorder = is_specified(sp_.k_reorder) ? sp_.k_reorder : 1.0f;
+        if (params && is_specified(params->n_probes)) n_probes = params->n_probes;
+        if (params && is_specified(params->k_reorder)) k_reorder = params->k_reorder;
+        if (!(k_reorder >= 1.0f)) return Status(ErrorCode::INVALID_ARGUMENT, "k_reorder must be at least 1");
+        if (svsb200_dynamic_ivf_search(index_, x, SVSB200_F32, n, k, n_probes, reinterpret_cast<uint64_t*>(labels),
+                                       distances))
+            return gpu_error();
+        return Status_Ok;
+    }
+    Status save(std::ostream&) const noexcept override {
+        return Status(ErrorCode::NOT_IMPLEMENTED, "save stays on the reference's CPU index");
+    }
+    Status set_num_threads(size_t n) noexcept override {
+        threads_ = n;
+        return Status_Ok;
+    }
+    Status get_num_threads(size_t* n) const noexcept override {
+        if (n) *n = threads_;
+        return Status_Ok;
+    }
+    Status set_intra_query_threads(size_t n) noexcept override {
+        intra_ = n;
+        return Status_Ok;
+    }
+    Status get_intra_query_threads(size_t* n) const noexcept override {
+        if (n) *n = intra_;
+        return Status_Ok;
+    }
+
+  private:
+    svsb200_dynamic_ivf* index_ = nullptr;
+    size_t dim_;
+    MetricType metric_;
+    StorageKind kind_;
+    BuildParams bp_;
+    SearchParams sp_;
+    size_t threads_, intra_;
+};
+
+}  // namespace
+
+Status DynamicIVFIndex::check_storage_kind(StorageKind kind) noexcept {
+    return kind == StorageKind::FP32 || kind == StorageKind::FP16
+               ? Status_Ok
+               : Status(ErrorCode::NOT_IMPLEMENTED, "DynamicIVFIndex on the GPU supports FP32 and FP16 storage only");
+}
+
+Status DynamicIVFIndex::build(DynamicIVFIndex** index, size_t dim, MetricType metric, StorageKind storage_kind, size_t n,
+                              const float* data, const size_t* labels, const IVFIndex::BuildParams& params,
+                              const IVFIndex::SearchParams& default_search_params, size_t num_threads,
+                              size_t intra_query_threads) noexcept {
+    if (!index) return Status(ErrorCode::INVALID_ARGUMENT, "null output");
+    *index = nullptr;
+    if (Status st = check_storage_kind(storage_kind); !st.ok()) return st;
+    if (dim == 0) return Status(ErrorCode::INVALID_ARGUMENT, "dim must be positive");
+    auto* h = new (std::nothrow)
+        GpuDynamicIVFIndex(dim, metric, storage_kind, params, default_search_params, num_threads, intra_query_threads);
+    if (!h) return Status(ErrorCode::RUNTIME_ERROR, "out of memory");
+    if (n > 0 && data && labels) {   // (no rows: the first add initialises the index)
+        if (Status st = h->init(n, data, labels); !st.ok()) {
+            delete h;
+            return st;
+        }
+    }
+    *index = h;
+    return Status_Ok;
+}
+
+Status DynamicIVFIndex::destroy(DynamicIVFIndex* index) noexcept {
+    delete index;
+    return Status_Ok;
+}
+
+Status DynamicIVFIndex::load(DynamicIVFIndex** index, std::istream&, MetricType, StorageKind, size_t, size_t) noexcept {
+    if (index) *index = nullptr;
+    return Status(ErrorCode::NOT_IMPLEMENTED, "load stays on the reference's CPU library");
+}
+
+Status DynamicIVFIndexLeanVec::build(DynamicIVFIndex** index, size_t, MetricType, StorageKind, size_t, const float*,
+                                     const size_t*, size_t, const IVFIndex::BuildParams&, const IVFIndex::SearchParams&,
+                                     size_t, size_t) noexcept {
+    if (index) *index = nullptr;
+    return Status(ErrorCode::NOT_IMPLEMENTED, "LeanVec storage is not available on the GPU");
+}
+Status DynamicIVFIndexLeanVec::build(DynamicIVFIndex** index, size_t, MetricType, StorageKind, size_t, const float*,
+                                     const size_t*, const LeanVecTrainingData*, const IVFIndex::BuildParams&,
+                                     const IVFIndex::SearchParams&, size_t, size_t) noexcept {
     if (index) *index = nullptr;
     return Status(ErrorCode::NOT_IMPLEMENTED, "LeanVec storage is not available on the GPU");
 }

@@ -46,8 +46,8 @@ static cudaError_t move_rows(const void* src, const uint32_t* src_idx, void* dst
     return cudaGetLastError();
 }
 
-static cudaError_t mark_slots(const uint32_t* d_slots, const uint64_t* d_ids, size_t count, uint8_t value, Replica* rep,
-                              cudaStream_t stream) {
+cudaError_t mark_slots(const uint32_t* d_slots, const uint64_t* d_ids, size_t count, uint8_t value, Replica* rep,
+                       cudaStream_t stream) {
     if (count == 0) return cudaSuccess;
     mark_slots_kernel<<<unsigned((count + 255) / 256), 256, 0, stream>>>(d_slots, d_ids, uint32_t(count), value,
                                                                           rep->d_status.ptr, rep->d_ext_ids.ptr);
@@ -58,27 +58,6 @@ static cudaError_t mark_slots(const uint32_t* d_slots, const uint64_t* d_ids, si
 // Bytes of device memory the rows, statuses and external ids of `slots` slots hold (the GEMM's tiles not counted).
 static size_t slot_bytes(const svsb200_index* ix, size_t slots) {
     return slots * (size_t(ix->row_stride) + 1 + sizeof(uint64_t));
-}
-
-// Runs a mutation `body(rep, stream)` on a scratch stream of the index's device, once every search of the index
-// enqueued so far has finished: svsb200_dynamic_flat_search_device returns with work still queued on the caller's
-// stream (the fallback scan and the mapping to external ids, which reads the slots' external ids), and the mutation
-// rewrites statuses, external ids and tiles.  Every flat search records its scratch's ev_done at its end (flat.cu).
-template <typename F> static int on_stream(svsb200_index* ix, F body) {
-    Replica* rep = ix->reps[0].get();
-    CUDA_TRY(cudaSetDevice(rep->device));
-    std::vector<cudaEvent_t> searches;
-    {
-        std::lock_guard<std::mutex> lock(rep->mu);
-        for (const auto& sc : rep->all) searches.push_back(sc->ev_done);
-    }
-    for (cudaEvent_t ev : searches) CUDA_TRY(cudaEventSynchronize(ev));   // (never recorded: returns at once)
-    std::string err;
-    Scratch* sc = acquire(rep, &err);
-    if (!sc) return fail(err);
-    const int rc = body(rep, sc->stream);
-    release(rep, sc);
-    return rc;
 }
 
 static svsb200_index* index_of(svsb200_dynamic_flat* h) { return h ? h->ix.get() : nullptr; }
@@ -182,7 +161,7 @@ int svsb200_dynamic_flat_add(svsb200_dynamic_flat* index, const void* vectors, i
     const size_t old_n = ix->n, new_n = old_n + (count - slots.size());
     if (new_n >= (size_t(1) << 31)) return fail("svsb200_dynamic_flat_add: more than 2^31-1 slots");
     for (size_t s = old_n; s < new_n; ++s) slots.push_back(uint32_t(s));
-    int rc = on_stream(ix, [&](Replica* rep, cudaStream_t stream) -> int {
+    int rc = after_searches(ix,[&](Replica* rep, cudaStream_t stream) -> int {
         // geometric growth: many small calls do not copy the index each time
         const size_t cap = rep->d_status.count;
         if (new_n > cap) {
@@ -252,7 +231,7 @@ int svsb200_dynamic_flat_delete(svsb200_dynamic_flat* index, const uint64_t* ids
         slots.push_back(it->second);
     }
     if (count == 0) return 0;
-    int rc = on_stream(ix, [&](Replica* rep, cudaStream_t stream) -> int {
+    int rc = after_searches(ix,[&](Replica* rep, cudaStream_t stream) -> int {
         Replica::SlotStaging& st = rep->staging;
         CUDA_TRY(st.slots.ensure(count));
         CUDA_TRY(cudaMemcpyAsync(st.slots.ptr, slots.data(), count * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
@@ -290,7 +269,7 @@ int svsb200_dynamic_flat_compact(svsb200_dynamic_flat* index) {
     const size_t m = new_to_old.size(), cap = std::max<size_t>(m, 1);
     std::vector<uint64_t> ext(m);
     for (size_t i = 0; i < m; ++i) ext[i] = ix->ext_ids[new_to_old[i]];
-    int rc = on_stream(ix, [&](Replica* rep, cudaStream_t stream) -> int {
+    int rc = after_searches(ix,[&](Replica* rep, cudaStream_t stream) -> int {
         DeviceBuffer<uint32_t> d_n2o;
         DeviceBuffer<unsigned char> vectors;
         DeviceBuffer<uint8_t> status;

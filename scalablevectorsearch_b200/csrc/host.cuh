@@ -337,6 +337,31 @@ int row_degrees(const GraphBuild& b);
 // Slots -> external ids in place, `count` ids (padding ids stay all-ones; search.cu), enqueued on `stream`.
 cudaError_t slots_to_external(uint64_t* d_ids, size_t count, const uint64_t* d_ext_ids, cudaStream_t stream);
 
+// ---- mutations of the dynamic flat and dynamic IVF indexes (dynamic_flat.cu, dynamic_ivf.cu) ----
+// rep->d_status[d_slots[i]] = value and, with d_ids, rep->d_ext_ids[d_slots[i]] = d_ids[i], enqueued on `stream`.
+cudaError_t mark_slots(const uint32_t* d_slots, const uint64_t* d_ids, size_t count, uint8_t value, Replica* rep,
+                       cudaStream_t stream);
+// Runs a mutation `body(rep, stream)` on a scratch stream of the index's device, once every search of the index
+// enqueued so far has finished: a device-buffer search returns with work still queued on the caller's stream (the
+// mapping to external ids reads the slots' external ids, the scan reads the rows), and the mutation rewrites them.
+// Every search of a dynamic flat or dynamic IVF index records its scratch's ev_done at its end (flat.cu, ivf.cu).
+template <typename F> int after_searches(svsb200_index* ix, F body) {
+    Replica* rep = ix->reps[0].get();
+    CUDA_TRY(cudaSetDevice(rep->device));
+    std::vector<cudaEvent_t> searches;
+    {
+        std::lock_guard<std::mutex> lock(rep->mu);
+        for (const auto& sc : rep->all) searches.push_back(sc->ev_done);
+    }
+    for (cudaEvent_t ev : searches) CUDA_TRY(cudaEventSynchronize(ev));   // (never recorded: returns at once)
+    std::string err;
+    Scratch* sc = acquire(rep, &err);
+    if (!sc) return fail(err);
+    const int rc = body(rep, sc->stream);
+    release(rep, sc);
+    return rc;
+}
+
 // ---- flat search (flat.cu), shared by the Flat handle and the dynamic flat index ----
 // The two search bodies: `who` names the entry point in errors, `max_kc` is the deepest candidate list allowed.  The
 // device form is enqueued on the caller's stream, the host form blocks.

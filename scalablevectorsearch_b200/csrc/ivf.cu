@@ -10,7 +10,7 @@
 //      every (query, probe) as [P][nq][k];
 //   5. merge_topk_kernel (search.cu) merges the P lists of a query with TotalOrder into [nq][k].
 // The per-(query, probe) lists are kept under IVF_LIST_BUDGET bytes by cutting the batch into query chunks.
-#include "host.cuh"
+#include "ivf.cuh"
 #include "ivf_kernel.cuh"
 
 #include <algorithm>
@@ -84,26 +84,15 @@ static void ivf_split(std::vector<float>& cent, std::vector<uint32_t>& counts, s
     }
 }
 
-// An own stream for the blocking entry points, destroyed on scope exit.
-struct OwnStream {
-    cudaStream_t s = nullptr;
-    ~OwnStream() {
-        if (s) cudaStreamDestroy(s);
-    }
-};
-
-// The centroids as a graph-free flat index (float32 rows), so that probing and assignment are one flat search.
-static int ivf_centroid_index(const float* centroids, size_t C, size_t dim, int metric, int device,
-                              std::unique_ptr<svsb200_flat>* out) {
+int ivf_centroid_index(const float* centroids, size_t C, size_t dim, int metric, int device, std::unique_ptr<svsb200_flat>* out) {
     svsb200_flat* f = nullptr;
     if (int rc = svsb200_flat_index_create(centroids, SVSB200_F32, C, dim, 0, metric, device, &f)) return rc;
     out->reset(f);
     return 0;
 }
 
-// Nearest centroid of `count` dense rows (device, row_bytes apart) in batches of `batch`, written to d_assign (uint32).
-static int ivf_assign(svsb200_flat* cent, const char* d_rows, int dtype, size_t count, size_t row_bytes, size_t batch,
-                      uint32_t* d_assign, cudaStream_t stream) {
+int ivf_assign(svsb200_flat* cent, const char* d_rows, int dtype, size_t count, size_t row_bytes, size_t batch,
+               uint32_t* d_assign, cudaStream_t stream) {
     DeviceBuffer<uint64_t> ids;
     DeviceBuffer<float> dists;
     const size_t b = std::min(batch, count);
@@ -122,40 +111,15 @@ static int ivf_assign(svsb200_flat* cent, const char* d_rows, int dtype, size_t 
     return 0;
 }
 
-struct IvfScratch {
-    DeviceBuffer<uint64_t> probe_ids, list_ids;
-    DeviceBuffer<float> probe_dists, list_dists;
-    DeviceBuffer<uint32_t> counts, list_off, item_off, cursor, list;
-};
-
-}  // namespace svsb200
-
-using namespace svsb200;
-
-struct svsb200_ivf {
-    std::unique_ptr<svsb200_index> ix;      // the cluster-major rows (each cluster from a 32-row boundary, zero padding)
-    std::unique_ptr<svsb200_flat> cent;     // the centroids
-    size_t n = 0, C = 0;
-    std::vector<uint32_t> sizes;
-    std::vector<float> centroids;
-    DeviceBuffer<uint32_t> d_row_ids, d_start, d_count;
-    std::mutex mu;
-    std::map<Scratch*, std::unique_ptr<IvfScratch>> scratch;   // per search scratch of ix's replica
-    ~svsb200_ivf() {
-        if (ix) cudaSetDevice(ix->reps[0]->device);
-    }
-};
-
-namespace svsb200 {
-
-template <int ROWT> static cudaError_t launch_ivf_scan(int op, const IvfScanParams& ip, const LaunchConfig& cfg) {
+template <int ROWT, bool DYN> static cudaError_t launch_ivf_scan(int op, const IvfScanParams& ip, const LaunchConfig& cfg) {
     return dispatch(IvfOps{}, op, [&](auto o) {
         constexpr int OP = decltype(o)::value;
-        // rows per group and pass: two where they fit the register bound without spilling, one for float16 rows and
-        // cosine (as for the masked scan)
-        constexpr int NR = ROWT == SVSB200_F16 || OP == OP_COSF ? 1 : 2;
         return with_shape<OP, true>(ip.p.dim, false, [&](auto ds, auto) {
-            return launch_kernel(ivf_scan_kernel<ROWT, OP, decltype(ds)::value, NR>, cfg, size_t(1) << 20, true, ip);
+            constexpr int DS = decltype(ds)::value;
+            // rows per group and pass: two where they fit the register bound without spilling, one for float16 rows
+            // and cosine (as for the masked scan) and for the dynamic form's generic dimension
+            constexpr int NR = ROWT == SVSB200_F16 || OP == OP_COSF || (DYN && DS == 0) ? 1 : 2;
+            return launch_kernel(ivf_scan_kernel<ROWT, OP, DS, NR, DYN>, cfg, size_t(1) << 20, true, ip);
         });
     });
 }
@@ -165,9 +129,8 @@ static size_t ivf_chunk(size_t P, size_t k) {
     return std::max<size_t>(1, std::min(IVF_MAX_CHUNK, IVF_LIST_BUDGET / (P * k * 12)));
 }
 
-// The search body on device buffers, enqueued on sc->stream (the centroid search synchronises it).
-static int ivf_search_on_device(svsb200_ivf* iv, Scratch* sc, const void* d_queries, int qdtype, size_t nq, size_t k,
-                                size_t P, uint64_t* d_out_ids, float* d_out_dists) {
+int ivf_search_on_device(svsb200_ivf* iv, Scratch* sc, const void* d_queries, int qdtype, size_t nq, size_t k, size_t P,
+                         uint64_t* d_out_ids, float* d_out_dists, const uint64_t* d_ext_ids) {
     svsb200_index* ix = iv->ix.get();
     Replica* rep = ix->reps[0].get();
     cudaStream_t stream = sc->stream;
@@ -254,16 +217,48 @@ static int ivf_search_on_device(svsb200_ivf* iv, Scratch* sc, const void* d_quer
         CUDA_TRY(cudaMemsetAsync(sc->d_counter.ptr, 0, sizeof(unsigned int), stream));
         const LaunchConfig cfg{-rep->sm_count, IVF_WARPS, ivf_smem_bytes(ix->row_stride, tile_rows, qstride, uint32_t(k), uint32_t(Q)),
                                stream};
-        CUDA_TRY(dispatch(IvfRows{}, ix->dtype, [&](auto row) { return launch_ivf_scan<decltype(row)::value>(op, ip, cfg); }));
+        CUDA_TRY(dispatch(IvfRows{}, ix->dtype, [&](auto row) {
+            return d_ext_ids ? launch_ivf_scan<decltype(row)::value, true>(op, ip, cfg)
+                             : launch_ivf_scan<decltype(row)::value, false>(op, ip, cfg);
+        }));
         // 5. merge
         if (int rc = svsb200_merge_topk_device(is->list_ids.ptr, is->list_dists.ptr, P, nqc, k, ix->metric, d_out_ids + q0 * k,
                                                d_out_dists + q0 * k, rep->device, stream))
             return rc;
     }
+    if (d_ext_ids) {   // slots -> external ids; a mutation of the dynamic index waits for ev_done (dynamic_ivf.cu)
+        CUDA_TRY(slots_to_external(d_out_ids, nq * k, d_ext_ids, stream));
+        CUDA_TRY(cudaEventRecord(sc->ev_done, stream));
+    }
     return 0;
 }
 
-static int ivf_check_search(const char* who, const svsb200_ivf* iv, int qdtype, size_t k, size_t n_probes) {
+int ivf_search_host(svsb200_ivf* iv, const void* queries, int qdtype, size_t nq, size_t k, size_t P, uint64_t* out_ids,
+                    float* out_dists, const uint64_t* d_ext_ids) {
+    Replica* rep = iv->ix->reps[0].get();
+    CUDA_TRY(cudaSetDevice(rep->device));
+    std::string err;
+    Scratch* sc = acquire(rep, &err);
+    if (!sc) return fail(err);
+    const int rc = [&]() -> int {
+        const size_t qbytes = nq * iv->ix->dim * esize(qdtype);
+        CUDA_TRY(sc->q_raw.ensure(qbytes));
+        CUDA_TRY(sc->ids.ensure(nq * k * 8));
+        CUDA_TRY(sc->dists.ensure(nq * k));
+        CUDA_TRY(cudaMemcpyAsync(sc->q_raw.ptr, queries, qbytes, cudaMemcpyHostToDevice, sc->stream));
+        if (int rc = ivf_search_on_device(iv, sc, sc->q_raw.ptr, qdtype, nq, k, P, reinterpret_cast<uint64_t*>(sc->ids.ptr),
+                                          sc->dists.ptr, d_ext_ids))
+            return rc;
+        CUDA_TRY(cudaMemcpyAsync(out_ids, sc->ids.ptr, nq * k * 8, cudaMemcpyDeviceToHost, sc->stream));
+        CUDA_TRY(cudaMemcpyAsync(out_dists, sc->dists.ptr, nq * k * 4, cudaMemcpyDeviceToHost, sc->stream));
+        CUDA_TRY(cudaStreamSynchronize(sc->stream));
+        return 0;
+    }();
+    release(rep, sc);
+    return rc;
+}
+
+int ivf_check_search(const char* who, const svsb200_ivf* iv, int qdtype, size_t k, size_t n_probes) {
     const std::string w(who);
     if (!iv) return fail(w + ": NULL index");
     if (k == 0 || k > 1024) return fail(w + ": k must be in [1, 1024]");
@@ -286,6 +281,8 @@ static int ivf_check_rows(const char* who, const void* vectors, int dtype, size_
 }
 
 }  // namespace svsb200
+
+using namespace svsb200;
 
 extern "C" {
 
@@ -492,7 +489,7 @@ int svsb200_ivf_search_device(svsb200_ivf* index, const void* d_queries, int qdt
     std::string err;
     Scratch* sc = scratch_for_stream(rep, static_cast<cudaStream_t>(stream_), &err);
     if (!sc) return fail(err);
-    return ivf_search_on_device(index, sc, d_queries, qdtype, nq, k, n_probes, d_out_ids, d_out_dists);
+    return ivf_search_on_device(index, sc, d_queries, qdtype, nq, k, n_probes, d_out_ids, d_out_dists, nullptr);
 }
 
 int svsb200_ivf_search(svsb200_ivf* index, const void* queries, int qdtype, size_t nq, size_t k, size_t n_probes,
@@ -500,27 +497,7 @@ int svsb200_ivf_search(svsb200_ivf* index, const void* queries, int qdtype, size
     if (int rc = ivf_check_search("svsb200_ivf_search", index, qdtype, k, n_probes)) return rc;
     if (nq == 0) return 0;
     if (!queries || !out_ids || !out_dists) return fail("svsb200_ivf_search: NULL buffer");
-    Replica* rep = index->ix->reps[0].get();
-    CUDA_TRY(cudaSetDevice(rep->device));
-    std::string err;
-    Scratch* sc = acquire(rep, &err);
-    if (!sc) return fail(err);
-    const int rc = [&]() -> int {
-        const size_t qbytes = nq * index->ix->dim * esize(qdtype);
-        CUDA_TRY(sc->q_raw.ensure(qbytes));
-        CUDA_TRY(sc->ids.ensure(nq * k * 8));
-        CUDA_TRY(sc->dists.ensure(nq * k));
-        CUDA_TRY(cudaMemcpyAsync(sc->q_raw.ptr, queries, qbytes, cudaMemcpyHostToDevice, sc->stream));
-        if (int rc = ivf_search_on_device(index, sc, sc->q_raw.ptr, qdtype, nq, k, n_probes,
-                                          reinterpret_cast<uint64_t*>(sc->ids.ptr), sc->dists.ptr))
-            return rc;
-        CUDA_TRY(cudaMemcpyAsync(out_ids, sc->ids.ptr, nq * k * 8, cudaMemcpyDeviceToHost, sc->stream));
-        CUDA_TRY(cudaMemcpyAsync(out_dists, sc->dists.ptr, nq * k * 4, cudaMemcpyDeviceToHost, sc->stream));
-        CUDA_TRY(cudaStreamSynchronize(sc->stream));
-        return 0;
-    }();
-    release(rep, sc);
-    return rc;
+    return ivf_search_host(index, queries, qdtype, nq, k, n_probes, out_ids, out_dists, nullptr);
 }
 
 }  // extern "C"

@@ -48,9 +48,66 @@ __host__ __device__ inline size_t ivf_smem_bytes(uint32_t row_stride, uint32_t t
 // Merges the `count` scored rows of a tile (keys in ckey[0..count), ids ids[0..count), ascending) into the sorted list
 // (bkey, bid) of `size` <= k entries: the result of inserting them one by one, each after the equal keys already there,
 // truncated at k.  Warp-collective.
+// DYN (the dynamic IVF index, dynamic_ivf.cu): the ids are slots in no particular order, all-ones marking a tombstone,
+// which is not a candidate; the list is ordered by (key, slot), so both the upper bound and the rank among the tile's
+// survivors compare (key, id) lexicographically.
+template <bool DYN = false>
 __device__ __forceinline__ void ivf_merge(float* bkey, uint32_t* bid, uint32_t& size, uint32_t k, const float* ckey,
                                           const uint32_t* ids, uint32_t count, uint32_t* spos, int lane) {
     constexpr unsigned FULL = 0xFFFFFFFFu;
+    if constexpr (DYN) {
+        const uint32_t id = uint32_t(lane) < count ? ids[lane] : 0xFFFFFFFFu;
+        const bool valid = id != 0xFFFFFFFFu;
+        const float d = valid ? ckey[lane] : 0.0f;
+        // (d, id) before (e, j): distinct ids, so no pair is equal
+        auto before = [](float d, uint32_t id, float e, uint32_t j) { return d < e || (!(e < d) && id < j); };
+        const bool surv = valid && (size < k || before(d, id, bkey[size - 1], bid[size - 1]));
+        const unsigned m = __ballot_sync(FULL, surv);
+        if (!m) return;
+        uint32_t ipos = 0;   // entries before (d, id): upper bound
+        if (surv) {
+            uint32_t lo = 0, hi = size;
+            while (lo < hi) {
+                const uint32_t mid = (lo + hi) >> 1;
+                if (before(d, id, bkey[mid], bid[mid])) hi = mid; else lo = mid + 1;
+            }
+            ipos = lo;
+        }
+        uint32_t rank = 0;   // survivors before this one
+        for (int s = 0; s < 32; ++s) {
+            const float ds = __shfl_sync(FULL, d, s);
+            const uint32_t is = __shfl_sync(FULL, id, s);
+            if (surv && ((m >> s) & 1u)) rank += before(ds, is, d, id);
+        }
+        const uint32_t S = __popc(m);
+        if (surv) spos[__popc(m & ((1u << lane) - 1u))] = ipos;
+        const uint32_t minpos = __reduce_min_sync(FULL, surv ? ipos : 0xFFFFFFFFu);
+        __syncwarp();
+        if (minpos < size) {   // (as below)
+            for (int ch = int((size - 1) >> 5); ch >= int(minpos >> 5); --ch) {
+                const uint32_t j = uint32_t(ch) * 32 + lane;
+                const bool have = j < size;
+                const float kk = have ? bkey[j] : 0.0f;
+                const uint32_t ii = have ? bid[j] : 0u;
+                uint32_t shift = 0;
+                for (uint32_t s = 0; s < S; ++s) shift += spos[s] <= j;
+                __syncwarp();
+                if (have && j + shift < k) {
+                    bkey[j + shift] = kk;
+                    bid[j + shift] = ii;
+                }
+                __syncwarp();
+            }
+        }
+        const uint32_t fp = ipos + rank;
+        if (surv && fp < k) {
+            bkey[fp] = d;
+            bid[fp] = id;
+        }
+        size = min(size + S, k);
+        __syncwarp();
+        return;
+    }
     const bool valid = uint32_t(lane) < count;
     const float d = valid ? ckey[lane] : 0.0f;
     const bool surv = valid && (size < k || d < bkey[size - 1]);
@@ -100,7 +157,8 @@ __device__ __forceinline__ void ivf_merge(float* bkey, uint32_t* bid, uint32_t& 
     __syncwarp();
 }
 
-template <int ROWT, int OP, int DS, int NR>
+// DYN: the dynamic IVF index (ivf_merge<true>): row_ids holds slots, all-ones for a tombstone; lists by (distance, slot).
+template <int ROWT, int OP, int DS, int NR, bool DYN = false>
 __global__ void __launch_bounds__(IVF_WARPS * 32, 2) ivf_scan_kernel(const __grid_constant__ IvfScanParams ip) {
     constexpr int G = 16 / Row<ROWT>::LPT;   // threads per row
     constexpr int GROUPS = 32 / G;            // rows per warp and pass
@@ -190,7 +248,7 @@ __global__ void __launch_bounds__(IVF_WARPS * 32, 2) ivf_scan_kernel(const __gri
                 }
                 __syncwarp();
                 uint32_t size = s_size[s];
-                ivf_merge(bkey, bid, size, ip.k, ckey, cids + tile * ip.tile_rows, rows, spos, lane);
+                ivf_merge<DYN>(bkey, bid, size, ip.k, ckey, cids + tile * ip.tile_rows, rows, spos, lane);
                 if (lane == 0) s_size[s] = size;
             }
             __syncthreads();   // (the slot is staged again two tiles on)

@@ -1,0 +1,192 @@
+"""Dynamic IVF index on the GPU, mirroring the reference's ``svs.DynamicIVF`` (bindings/python/src/dynamic_ivf.cpp,
+include/svs/index/ivf/dynamic_ivf.h):
+
+    clustering = Clustering.build(IVFBuildParameters(num_centroids=1024), data, DistanceType.L2)
+    index = DynamicIVF.assemble_from_clustering(clustering, data, ids, DistanceType.L2)
+    slots = index.add(points, new_ids)                 # appended to their nearest clusters
+    index.delete(old_ids)                              # tombstones at once
+    index.search_parameters = IVFSearchParameters(n_probes=16)
+    I, D = index.search(queries, 10)                   # external ids (uint64), float32 distances
+
+Backed by ``svsb200_dynamic_ivf_*`` of ``libsvsb200.so``: the IVF index's exact cluster-probed search over the Valid rows,
+ties by slot.  The centroids never move after assembly.  Mutations must not run concurrently with searches of the same
+index.
+"""
+from __future__ import annotations
+
+import ctypes as C
+
+import numpy as np
+
+from . import _lib
+from .ivf import Clustering, IVFSearchParameters
+from .vamana import _DTYPE_CODE, DistanceType
+
+
+class DynamicIVF:
+    """``svs.DynamicIVF`` on one CUDA device: float32 / float16 rows, L2 / MIP / cosine."""
+
+    @classmethod
+    def assemble_from_clustering(cls, clustering: Clustering, data, ids, distance: DistanceType = DistanceType.L2,
+                                 num_threads: int = 1, intra_query_threads: int = 1, device: int = 0) -> "DynamicIVF":
+        """``svs.DynamicIVF.assemble_from_clustering``: one external id per row of ``data``, the rows grouped as the
+        clustering says (a clustering without assignments puts every row in its nearest cluster).  An empty ``data``
+        ([0, dim]) makes an empty index to be filled with :meth:`add`.  The thread counts are kept for interface
+        parity only."""
+        x = data.load() if hasattr(data, "load") else data
+        x = np.ascontiguousarray(x)
+        if x.ndim != 2:
+            raise ValueError("data must be a 2-D array")
+        if x.dtype not in _DTYPE_CODE:
+            raise TypeError(f"unsupported data type {x.dtype}")
+        ids = np.ascontiguousarray(np.atleast_1d(ids), dtype=np.uint64)
+        if ids.shape != (x.shape[0],):
+            raise ValueError("Expected IDs to be the same length as the number of rows in points!")
+        cent = clustering.centroids
+        if cent.shape[1] != x.shape[1]:
+            raise ValueError(f"centroids have {cent.shape[1]} dimensions, data {x.shape[1]}")
+        a = clustering.assignments
+        if a is not None and a.shape != (x.shape[0],):
+            raise ValueError("the clustering has one assignment per data row")
+        self = cls.__new__(cls)
+        self._lib = _lib.lib()
+        self._distance = DistanceType(distance)
+        self._dtype = x.dtype
+        self.num_threads, self.intra_query_threads = int(num_threads), int(intra_query_threads)
+        self.search_parameters = IVFSearchParameters()
+        handle = C.c_void_p()
+        _lib.check(self._lib.svsb200_dynamic_ivf_create(
+            x.ctypes.data, _DTYPE_CODE[x.dtype], x.shape[0], x.shape[1], int(self._distance), cent.ctypes.data,
+            cent.shape[0], None if a is None else a.ctypes.data, ids.ctypes.data, int(device), C.byref(handle)))
+        self._h = handle
+        return self
+
+    def __del__(self):
+        h = getattr(self, "_h", None)
+        if h:
+            self._lib.svsb200_dynamic_ivf_destroy(h)
+            self._h = None
+
+    @property
+    def size(self) -> int:
+        """Valid rows."""
+        return self._lib.svsb200_dynamic_ivf_size(self._h)
+
+    @property
+    def num_slots(self) -> int:
+        """Slots, Valid or Empty."""
+        return self._lib.svsb200_dynamic_ivf_num_slots(self._h)
+
+    @property
+    def dimensions(self) -> int:
+        return self._lib.svsb200_dynamic_ivf_dimensions(self._h)
+
+    @property
+    def num_clusters(self) -> int:
+        return self._lib.svsb200_dynamic_ivf_num_clusters(self._h)
+
+    @property
+    def device_bytes(self) -> int:
+        """Device memory held, the regions that clusters left when they grew included until :meth:`compact`."""
+        return self._lib.svsb200_dynamic_ivf_device_bytes(self._h)
+
+    @property
+    def cluster_sizes(self) -> np.ndarray:
+        """Valid rows per cluster."""
+        out = np.empty(self.num_clusters, dtype=np.uint32)
+        _lib.check(self._lib.svsb200_dynamic_ivf_cluster_sizes(self._h, out.ctypes.data))
+        return out
+
+    @property
+    def centroids(self) -> np.ndarray:
+        out = np.empty((self.num_clusters, self.dimensions), dtype=np.float32)
+        _lib.check(self._lib.svsb200_dynamic_ivf_centroids(self._h, out.ctypes.data))
+        return out
+
+    def add(self, points, ids, reuse_empty: bool = False) -> np.ndarray:
+        """``add_points``: rows with new external ids, each appended to its nearest centroid's cluster.  Without
+        ``reuse_empty`` every row takes a new slot at the end; with it, Empty slots from slot 0 come first.  Rows of the
+        index's dtype; float32 rows given to a float16 index are rounded to nearest even.  Fails without changing
+        anything on a repeated, present or reserved id.  Returns the slots used."""
+        pts = np.ascontiguousarray(points)
+        if pts.dtype == np.float32 and self._dtype == np.float16:
+            pts = pts.astype(np.float16)
+        ids = np.ascontiguousarray(np.atleast_1d(ids), dtype=np.uint64)
+        if pts.ndim != 2 or pts.shape[1] != self.dimensions:
+            raise ValueError(f"points must be [count, {self.dimensions}]")
+        if pts.shape[0] != len(ids):
+            raise ValueError(f"Number of points ({pts.shape[0]}) not equal to the number of external ids ({len(ids)})!")
+        if pts.dtype not in _DTYPE_CODE:
+            raise TypeError(f"unsupported data type {pts.dtype}")
+        slots = np.empty(len(ids), dtype=np.uint64)
+        _lib.check(self._lib.svsb200_dynamic_ivf_add(self._h, pts.ctypes.data, _DTYPE_CODE[pts.dtype], len(ids),
+                                                      ids.ctypes.data, int(bool(reuse_empty)), slots.ctypes.data))
+        return slots
+
+    def delete(self, ids) -> int:
+        """``delete``: the slots become Empty at once.  Fails without changing anything unless every id is present,
+        once.  Returns the number of deleted entries."""
+        ids = np.ascontiguousarray(np.atleast_1d(ids), dtype=np.uint64)
+        _lib.check(self._lib.svsb200_dynamic_ivf_delete(self._h, ids.ctypes.data, len(ids)))
+        return len(ids)
+
+    def consolidate(self) -> None:
+        """No-op, as in the reference: deletion is direct."""
+
+    def compact(self, batchsize: int = 1_000_000) -> None:
+        """``compact``: the Valid slots are renumbered in order and the clusters laid out without tombstones.
+        ``batchsize`` only tunes the reference's copy and is ignored."""
+        _lib.check(self._lib.svsb200_dynamic_ivf_compact(self._h))
+
+    def has_id(self, id: int) -> bool:
+        out = C.c_int()
+        _lib.check(self._lib.svsb200_dynamic_ivf_has_id(self._h, int(id), C.byref(out)))
+        return bool(out.value)
+
+    def all_ids(self) -> np.ndarray:
+        """External ids of every Valid slot, in slot order."""
+        n = C.c_size_t(self.size)
+        out = np.empty(n.value, dtype=np.uint64)
+        _lib.check(self._lib.svsb200_dynamic_ivf_ids(self._h, out.ctypes.data, C.byref(n)))
+        return out[: n.value]
+
+    def export(self):
+        """Per slot: (status uint8 (0 Empty, 1 Valid), external id (2^64 - 1 where Empty), cluster uint32 (2^32 - 1
+        where Empty))."""
+        n = self.num_slots
+        status = np.empty(n, dtype=np.uint8)
+        ids = np.empty(n, dtype=np.uint64)
+        cluster = np.empty(n, dtype=np.uint32)
+        _lib.check(self._lib.svsb200_dynamic_ivf_export(self._h, status.ctypes.data, ids.ctypes.data, cluster.ctypes.data))
+        return status, ids, cluster
+
+    def _n_probes(self) -> int:
+        sp = self.search_parameters
+        if not sp.k_reorder >= 1.0:
+            raise ValueError(f"k_reorder must be at least 1, got {sp.k_reorder}")
+        return int(sp.n_probes)
+
+    def search(self, queries: np.ndarray, n_neighbors: int):
+        """``svs.DynamicIVF.search(queries, n_neighbors)`` -> (external ids uint64 [nq,k], distances float32 [nq,k]):
+        the exact top k over the Valid rows of the probed clusters, ties by slot; short rows padded with 2^64 - 1 and
+        +-inf."""
+        n_probes = self._n_probes()
+        q = np.ascontiguousarray(queries)
+        if q.ndim != 2 or q.shape[1] != self.dimensions:
+            raise ValueError(f"queries must be [nq, {self.dimensions}]")
+        if q.dtype not in _DTYPE_CODE:
+            raise TypeError(f"unsupported query type {q.dtype}")
+        nq, k = q.shape[0], int(n_neighbors)
+        ids = np.empty((nq, k), dtype=np.uint64)
+        dists = np.empty((nq, k), dtype=np.float32)
+        _lib.check(self._lib.svsb200_dynamic_ivf_search(self._h, q.ctypes.data, _DTYPE_CODE[q.dtype], nq, k, n_probes,
+                                                        ids.ctypes.data, dists.ctypes.data))
+        return ids, dists
+
+    def search_device(self, d_queries: int, qdtype: np.dtype, nq: int, n_neighbors: int, d_ids: int, d_dists: int,
+                      stream: int = 0) -> None:
+        """Device-buffer form (raw pointers, e.g. ``tensor.data_ptr()``; ids uint64), enqueued on ``stream``."""
+        n_probes = self._n_probes()
+        _lib.check(self._lib.svsb200_dynamic_ivf_search_device(self._h, d_queries, _DTYPE_CODE[np.dtype(qdtype)], nq,
+                                                               int(n_neighbors), n_probes, d_ids, d_dists,
+                                                               stream or None))
