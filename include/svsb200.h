@@ -461,7 +461,8 @@ int svsb200_dynamic_flat_search(svsb200_dynamic_flat* index, const void* queries
  * rounding is the BLAS's) and returns the exact top k (1 <= k <= 1024) over the union of the probed clusters' rows:
  * the search path's bit-exact distances, ordered by distance, then original row id, padded with all-ones ids and
  * +-inf distances when the probed clusters hold fewer than k rows.  With n_probes = C the result equals
- * svsb200_exhaustive_device over the same rows bit for bit.  Integer, SQ and LVQ rows are refused. */
+ * svsb200_exhaustive_device over the same rows bit for bit.  Integer and LVQ rows are refused; SQ codes are assembled by
+ * svsb200_ivf_create_sq. */
 typedef struct svsb200_ivf svsb200_ivf;
 
 /* The random sequence of svsb200_ivf_cluster: the first `count` outputs of splitmix64 seeded with `seed` (state +=
@@ -490,6 +491,25 @@ int svsb200_ivf_cluster(const void* vectors, int dtype, size_t n, size_t dim, in
  * every row goes to its exact nearest centroid, computed on the device) around C float32 centroids [C][dim]. */
 int svsb200_ivf_create(const void* vectors, int dtype, size_t n, size_t dim, int metric, const float* centroids,
                        size_t num_centroids, const uint32_t* assignments, int device, svsb200_ivf** out);
+/* Scalar quantisation, SQDataset<int8_t / uint8_t>::compress (quantization/scalar/scalar.h:447-469), on the device:
+ * n x dim float32 rows (HOST) become codes (int8 / uint8, `code_type`, HOST, n x dim) with one global scale and bias:
+ * scale = (max - min) / (MAX - MIN), bias = min - MIN * scale (each operation rounded on its own), code =
+ * clamp(roundf((x - bias) / scale), MIN, MAX), [MIN, MAX] = [-128, 127] or [0, 255].  Data holding a NaN or an infinity,
+ * and constant data (max == min), are refused: the reference's result is undefined there. */
+int svsb200_sq_compress(const float* data, size_t n, size_t dim, int code_type, int device, void* out_codes, float* out_scale,
+                        float* out_bias);
+/* assemble_from_clustering over SQ codes (IVFIndex with StorageKind::SQI8 and its uint8 twin): n x dim int8 / uint8
+ * codes (HOST) with the `scale` (finite, positive) and `bias` (finite) they were compressed with, C float32 centroids,
+ * and REQUIRED assignments (uint32 [n], each < C): without float rows nothing can be ranked against the centroids.
+ * The handle is an ordinary svsb200_ivf.  The probe is unchanged (float32 / float16 queries against the float32
+ * centroids); the result is the exact top k over the probed clusters with the SQ search path's bit-exact distances
+ * (EuclideanCompressed, InnerProductCompressed, CosineSimilarityCompressed), ordered by (distance, id).  With
+ * n_probes = C it equals svsb200_exhaustive_device on an SQ svsb200_index over the same codes.  L2 runs on the integer
+ * tensor cores (int32 sums, which wrap past dim * 255^2 >= 2^31 exactly as the search path's do); MIP and cosine run
+ * the float trees. */
+int svsb200_ivf_create_sq(const void* codes, int code_type, size_t n, size_t dim, int metric, float scale, float bias,
+                          const float* centroids, size_t num_centroids, const uint32_t* assignments, int device,
+                          svsb200_ivf** out);
 /* Frees the handle and its device memory (NULL is ignored). */
 int svsb200_ivf_destroy(svsb200_ivf* index);
 /* Rows, dimensions, clusters, device memory held (rows, ids, centroids); 0 for NULL. */

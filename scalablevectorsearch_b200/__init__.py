@@ -8,11 +8,11 @@ from .vamana import (DataType, DistanceType, DynamicVamana, GraphLoader, SearchB
                      VamanaBuildParameters, VamanaSearchParameters, VectorDataLoader, build_graph, lvq8_compress)
 from .flat import Flat
 from .dynamic_flat import DynamicFlat
-from .ivf import IVF, Clustering, IVFBuildParameters, IVFSearchParameters
+from .ivf import IVF, Clustering, IVFBuildParameters, IVFSearchParameters, sq_compress
 from .dynamic_ivf import DynamicIVF
 from ._lib import Svsb200Error
 
 __all__ = ["DataType", "DistanceType", "GraphLoader", "SearchBufferConfig", "Vamana", "VamanaSearchParameters",
            "VectorDataLoader", "Svsb200Error", "lvq8_compress", "ShardedVamana", "VamanaBuildParameters", "build_graph",
            "DynamicVamana", "Flat", "DynamicFlat", "IVF", "Clustering", "IVFBuildParameters", "IVFSearchParameters",
-           "DynamicIVF"]
+           "DynamicIVF", "sq_compress"]

@@ -35,7 +35,8 @@ SYMBOLS = [
     "svsb200_dynamic_flat_search_device",
     "svsb200_ivf_random", "svsb200_ivf_cluster", "svsb200_ivf_create", "svsb200_ivf_destroy", "svsb200_ivf_size",
     "svsb200_ivf_dimensions", "svsb200_ivf_num_clusters", "svsb200_ivf_device_bytes", "svsb200_ivf_cluster_sizes",
-    "svsb200_ivf_centroids", "svsb200_ivf_search", "svsb200_ivf_search_device",
+    "svsb200_ivf_centroids", "svsb200_ivf_search", "svsb200_ivf_search_device", "svsb200_sq_compress",
+    "svsb200_ivf_create_sq",
     "svsb200_dynamic_ivf_create", "svsb200_dynamic_ivf_destroy", "svsb200_dynamic_ivf_size",
     "svsb200_dynamic_ivf_num_slots", "svsb200_dynamic_ivf_dimensions", "svsb200_dynamic_ivf_num_clusters",
     "svsb200_dynamic_ivf_device_bytes", "svsb200_dynamic_ivf_cluster_sizes", "svsb200_dynamic_ivf_centroids",
@@ -137,6 +138,8 @@ def lib() -> C.CDLL:
     l.svsb200_ivf_random.argtypes = [C.c_uint64, sz, vp]
     l.svsb200_ivf_cluster.argtypes = [vp, i32, sz, sz, i32, sz, sz, sz, i32, C.c_float, C.c_uint64, i32, vp, vp]
     l.svsb200_ivf_create.argtypes = [vp, i32, sz, sz, i32, vp, sz, vp, i32, C.POINTER(vp)]
+    l.svsb200_ivf_create_sq.argtypes = [vp, i32, sz, sz, i32, C.c_float, C.c_float, vp, sz, vp, i32, C.POINTER(vp)]
+    l.svsb200_sq_compress.argtypes = [vp, sz, sz, i32, i32, vp, vp, vp]
     l.svsb200_ivf_destroy.argtypes = [vp]
     for name in ("size", "dimensions", "num_clusters", "device_bytes"):
         fn = getattr(l, f"svsb200_ivf_{name}")

@@ -124,6 +124,8 @@ constexpr size_t kSmemOptInMax = 227 * 1024;   // dynamic shared memory a block 
 //   consolidate pool, dynamic search (MUT)        DynamicRows L2F IPF COSF   -                 -
 //   flat rescore                                  DataRows    L2F IPF        L2F IPF L2I IPI   -
 //   IVF leaf scan (ivf_kernel.cuh)                IvfRows     L2F IPF COSF   -                 -
+//   IVF leaf scan over SQ codes                   IvfSqRows   -              IPF COSF (+ the
+//                                                                            tensor-core L2 leaf)
 // int8 / uint8 rows take float and integer queries in a search; the builder's datum is its own query.
 template <int... V> struct IntList {};
 template <int ROWT> constexpr bool kIntRow = ROWT == SVSB200_I8 || ROWT == SVSB200_U8;
@@ -141,6 +143,8 @@ template <int ROWT> using BuildOps = std::conditional_t<kIntRow<ROWT>, IntOps, F
 using DynamicOps = FloatOps;
 using IvfRows = IntList<SVSB200_F32, SVSB200_F16>;
 using IvfOps = FloatOps;
+using IvfSqRows = IntList<SVSB200_I8, SVSB200_U8>;
+using IvfSqOps = IntList<OP_IPF, OP_COSF>;
 template <int ROWT>
 using RescoreOps = std::conditional_t<kIntRow<ROWT>, IntList<OP_L2F, OP_IPF, OP_L2I, OP_IPI>, IntList<OP_L2F, OP_IPF>>;
 

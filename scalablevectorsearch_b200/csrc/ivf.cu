@@ -15,6 +15,7 @@
 
 #include <algorithm>
 #include <cmath>
+#include <cstring>
 #include <map>
 #include <numeric>
 #include <vector>
@@ -111,14 +112,15 @@ int ivf_assign(svsb200_flat* cent, const char* d_rows, int dtype, size_t count, 
     return 0;
 }
 
-template <int ROWT, bool DYN> static cudaError_t launch_ivf_scan(int op, const IvfScanParams& ip, const LaunchConfig& cfg) {
-    return dispatch(IvfOps{}, op, [&](auto o) {
+template <int ROWT, bool DYN, typename Ops = IvfOps>
+static cudaError_t launch_ivf_scan(int op, const IvfScanParams& ip, const LaunchConfig& cfg) {
+    return dispatch(Ops{}, op, [&](auto o) {
         constexpr int OP = decltype(o)::value;
         return with_shape<OP, true>(ip.p.dim, false, [&](auto ds, auto) {
             constexpr int DS = decltype(ds)::value;
-            // rows per group and pass: two where they fit the register bound without spilling, one for float16 rows
-            // and cosine (as for the masked scan) and for the dynamic form's generic dimension
-            constexpr int NR = ROWT == SVSB200_F16 || OP == OP_COSF || (DYN && DS == 0) ? 1 : 2;
+            // rows per group and pass: two where they fit the register bound without spilling, one for float16 rows,
+            // SQ codes and cosine (as for the masked scan) and for the dynamic form's generic dimension
+            constexpr int NR = ROWT == SVSB200_F16 || kIntRow<ROWT> || OP == OP_COSF || (DYN && DS == 0) ? 1 : 2;
             return launch_kernel(ivf_scan_kernel<ROWT, OP, DS, NR, DYN>, cfg, size_t(1) << 20, true, ip);
         });
     });
@@ -142,15 +144,24 @@ int ivf_search_on_device(svsb200_ivf* iv, Scratch* sc, const void* d_queries, in
         is = slot.get();
     }
     const uint32_t C = uint32_t(iv->C), dim = uint32_t(ix->dim), qstride = query_stride(dim);
+    // SQ rows: MIP and cosine run ivf_scan_kernel on the decompressed float tree, L2 the tensor-core leaf
+    const bool sq = ix->storage == SVSB200_SQ;
+    const bool sq_l2 = sq && ix->metric == SVSB200_L2;
+    if (sq && d_ext_ids) return fail("svsb200_ivf_search: SQ rows in a dynamic IVF index are not supported");
     // ring tiles: 32 rows, fewer for rows so wide that two tiles would pass 96 KB
     uint32_t tile_rows = IVF_TILE_ROWS;
     while (tile_rows > 1 && 2 * size_t(tile_rows) * ix->row_stride > (size_t(96) << 10)) tile_rows >>= 1;
+    auto smem = [&](size_t q) {
+        return sq_l2 ? ivf_sq_l2_smem_bytes(ix->row_stride, tile_rows, dim, uint32_t(k), uint32_t(q))
+                     : ivf_smem_bytes(ix->row_stride, tile_rows, qstride, uint32_t(k), uint32_t(q));
+    };
     // queries per work item: two CTAs per SM where they fit, else one
-    const size_t fixed = ivf_smem_bytes(ix->row_stride, tile_rows, qstride, uint32_t(k), 0);
-    const size_t slot = ivf_slot_bytes(qstride, uint32_t(k));
+    const size_t fixed = smem(0);
+    const size_t slot = smem(1) - fixed;
     const size_t limit = kSmemOptInMax - 1024;   // (the kernel's static shared memory)
-    size_t Q = fixed < limit / 2 ? std::min<size_t>(IVF_QMAX, (limit / 2 - fixed) / slot) : 0;
-    if (Q == 0 && fixed < limit) Q = std::min<size_t>(IVF_QMAX, (limit - fixed) / slot);
+    auto fit = [&](size_t room) { return fixed < room ? std::min<size_t>(IVF_QMAX, (room - fixed) / slot) : 0; };
+    size_t Q = fit(limit / 2);
+    if (Q == 0) Q = fit(limit);
     if (Q == 0) return fail("svsb200_ivf_search: k and the row size need more shared memory than a CTA has");
     const size_t chunk = ivf_chunk(P, k);
     const size_t qrow = size_t(dim) * esize(qdtype);
@@ -164,7 +175,8 @@ int ivf_search_on_device(svsb200_ivf* iv, Scratch* sc, const void* d_queries, in
     CUDA_TRY(is->item_off.ensure(C + 1));
     CUDA_TRY(is->cursor.ensure(C));
     CUDA_TRY(is->list.ensure(cmax * P));
-    int op = ix->metric == SVSB200_L2 ? OP_L2F : ix->metric == SVSB200_IP ? OP_IPF : OP_COSF;
+    const int op = sq_l2 ? OP_L2I : ix->metric == SVSB200_L2 ? OP_L2F : ix->metric == SVSB200_IP ? OP_IPF : OP_COSF;
+    const int prep = !sq ? PREP_FLOAT : sq_l2 ? PREP_SQ_L2 : ix->metric == SVSB200_IP ? PREP_SQ_IP : PREP_SQ_COS;
     for (size_t q0 = 0; q0 < nq; q0 += chunk) {
         const size_t nqc = std::min(chunk, nq - q0);
         const char* qp = static_cast<const char*>(d_queries) + q0 * qrow;
@@ -173,7 +185,7 @@ int ivf_search_on_device(svsb200_ivf* iv, Scratch* sc, const void* d_queries, in
                                         is->probe_ids.ptr, is->probe_dists.ptr, stream, nullptr, flat_max_kc_deep()))
             return rc;
         // 2. the scan's query operands
-        if (int rc = prepare_queries(ix, rep, sc, qp, qdtype, nqc, PREP_FLOAT, stream)) return rc;
+        if (int rc = prepare_queries(ix, rep, sc, qp, qdtype, nqc, prep, stream)) return rc;
         // 3. inversion
         const size_t total = nqc * P;
         const unsigned tb = unsigned((total + 255) / 256);
@@ -192,8 +204,12 @@ int ivf_search_on_device(svsb200_ivf* iv, Scratch* sc, const void* d_queries, in
         ip.p.dim = dim;
         ip.p.row_stride = ix->row_stride;
         ip.p.greater = ix->metric != SVSB200_L2;
-        ip.p.scale = 1.0f;
+        ip.p.sq = sq;
+        ip.p.scale = sq ? ix->scale : 1.0f;
+        ip.p.bias = ix->bias;
+        ip.p.scale_sq = ix->scale * ix->scale;   // EuclideanCompressed ctor (scalar.h:68-72)
         ip.p.qf = sc->q_f32.ptr;
+        ip.p.qcodes = sc->q_codes.ptr;
         ip.p.qaux = sc->q_aux.ptr;
         ip.p.qstride = qstride;
         ip.p.nq = uint32_t(nqc);
@@ -215,12 +231,21 @@ int ivf_search_on_device(svsb200_ivf* iv, Scratch* sc, const void* d_queries, in
         ip.out_dists = is->list_dists.ptr;
         ip.work_counter = sc->d_counter.ptr;
         CUDA_TRY(cudaMemsetAsync(sc->d_counter.ptr, 0, sizeof(unsigned int), stream));
-        const LaunchConfig cfg{-rep->sm_count, IVF_WARPS, ivf_smem_bytes(ix->row_stride, tile_rows, qstride, uint32_t(k), uint32_t(Q)),
-                               stream};
-        CUDA_TRY(dispatch(IvfRows{}, ix->dtype, [&](auto row) {
-            return d_ext_ids ? launch_ivf_scan<decltype(row)::value, true>(op, ip, cfg)
-                             : launch_ivf_scan<decltype(row)::value, false>(op, ip, cfg);
-        }));
+        const LaunchConfig cfg{-rep->sm_count, IVF_WARPS, smem(Q), stream};
+        if (sq_l2) {   // (the dynamic IVF index holds float rows only: SQ rows never take the DYN form)
+            CUDA_TRY(dispatch(IvfSqRows{}, ix->dtype, [&](auto row) {
+                return launch_kernel(ivf_scan_sq_l2_kernel<decltype(row)::value, false>, cfg, size_t(1) << 20, true, ip);
+            }));
+        } else if (sq) {
+            CUDA_TRY(dispatch(IvfSqRows{}, ix->dtype, [&](auto row) {
+                return launch_ivf_scan<decltype(row)::value, false, IvfSqOps>(op, ip, cfg);
+            }));
+        } else {
+            CUDA_TRY(dispatch(IvfRows{}, ix->dtype, [&](auto row) {
+                return d_ext_ids ? launch_ivf_scan<decltype(row)::value, true>(op, ip, cfg)
+                                 : launch_ivf_scan<decltype(row)::value, false>(op, ip, cfg);
+            }));
+        }
         // 5. merge
         if (int rc = svsb200_merge_topk_device(is->list_ids.ptr, is->list_dists.ptr, P, nqc, k, ix->metric, d_out_ids + q0 * k,
                                                d_out_dists + q0 * k, rep->device, stream))
@@ -269,16 +294,108 @@ int ivf_check_search(const char* who, const svsb200_ivf* iv, int qdtype, size_t 
     return 0;
 }
 
-static int ivf_check_rows(const char* who, const void* vectors, int dtype, size_t n, size_t dim, int metric) {
+static int ivf_check_rows(const char* who, const void* vectors, int dtype, size_t n, size_t dim, int metric, bool sq = false) {
     const std::string w(who);
     if (!vectors) return fail(w + ": NULL input");
-    if (dtype != SVSB200_F32 && dtype != SVSB200_F16)
+    if (sq) {
+        if (dtype != SVSB200_I8 && dtype != SVSB200_U8) return fail(w + ": SQ codes must be int8 or uint8");
+    } else if (dtype != SVSB200_F32 && dtype != SVSB200_F16) {
         return fail(w + ": rows must be float32 or float16 (integer, SQ and LVQ rows are not supported)");
+    }
     if (metric < SVSB200_L2 || metric > SVSB200_COSINE) return fail(w + ": bad metric");
     if (n == 0 || dim == 0) return fail(w + ": empty dataset");
     if (n >= (size_t(1) << 31)) return fail(w + ": more than 2^31-1 vectors");
     return 0;
 }
+
+static int sq_check_params(const char* who, float scale, float bias) {
+    if (!(scale > 0.0f) || !std::isfinite(scale) || !std::isfinite(bias))
+        return fail(std::string(who) + ": the SQ scale must be finite and positive and the bias finite");
+    return 0;
+}
+
+// IVFIndex::assemble_from_clustering over checked rows (SQ codes when `storage` is SVSB200_SQ): the cluster-major layout,
+// each cluster from a 32-row boundary, its rows in ascending id, zero padding.
+static int ivf_assemble(const char* who, const void* vectors, int dtype, int storage, float scale, float bias, size_t n,
+                        size_t dim, int metric, const float* centroids, size_t num_centroids, const uint32_t* assignments,
+                        int device, svsb200_ivf** out) {
+    const std::string w(who);
+    const size_t C = num_centroids;
+    if (!centroids) return fail(w + ": NULL centroids");
+    if (C == 0 || C >= (size_t(1) << 31)) return fail(w + ": num_centroids must be in [1, 2^31)");
+    if (assignments)
+        for (size_t i = 0; i < n; ++i)
+            if (assignments[i] >= C) return fail(w + ": assignment " + std::to_string(i) + " is not a cluster");
+    cudaDeviceProp prop;
+    if (int rc = check_device(who, device, &prop)) return rc;
+    CUDA_TRY(cudaSetDevice(device));
+    auto iv = std::make_unique<svsb200_ivf>();
+    iv->n = n;
+    iv->C = C;
+    iv->centroids.assign(centroids, centroids + C * dim);
+    if (int rc = ivf_centroid_index(centroids, C, dim, metric, device, &iv->cent)) return rc;
+    const size_t row_bytes = dim * esize(dtype);
+    std::vector<uint32_t> assign(n);
+    if (assignments) {
+        std::copy(assignments, assignments + n, assign.begin());
+    } else {
+        OwnStream own;
+        CUDA_TRY(cudaStreamCreateWithFlags(&own.s, cudaStreamNonBlocking));
+        DeviceBuffer<char> d_rows;
+        DeviceBuffer<uint32_t> d_assign;
+        CUDA_TRY(d_rows.ensure(n * row_bytes));
+        CUDA_TRY(d_assign.ensure(n));
+        CUDA_TRY(cudaMemcpy(d_rows.ptr, vectors, n * row_bytes, cudaMemcpyHostToDevice));
+        if (int rc = ivf_assign(iv->cent.get(), d_rows.ptr, dtype, n, row_bytes, 65536, d_assign.ptr, own.s)) return rc;
+        CUDA_TRY(cudaMemcpy(assign.data(), d_assign.ptr, n * 4, cudaMemcpyDeviceToHost));
+    }
+    // cluster-major layout: clusters in order, each from a 32-row boundary, its rows in ascending id
+    iv->sizes.assign(C, 0);
+    for (uint32_t a : assign) ++iv->sizes[a];
+    std::vector<uint32_t> start(C), fill(C);
+    size_t stored = 0;
+    for (size_t c = 0; c < C; ++c) {
+        start[c] = uint32_t(stored);
+        fill[c] = uint32_t(stored);
+        stored += round_up(iv->sizes[c], 32);
+    }
+    if (stored >= (size_t(1) << 32)) return fail(w + ": too many rows");
+    auto ix = std::make_unique<svsb200_index>();
+    ix->dtype = dtype;
+    ix->metric = metric;
+    ix->storage = storage;
+    ix->scale = scale;
+    ix->bias = bias;
+    ix->n = std::max<size_t>(stored, 1);
+    ix->dim = dim;
+    ix->row_stride = data_row_stride(storage, dtype, dim);
+    ix->gstride = 32;
+    std::vector<uint32_t> row_ids(ix->n, 0xFFFFFFFFu);
+    std::vector<char> rows(ix->n * size_t(ix->row_stride), 0);
+    const char* src = static_cast<const char*>(vectors);
+    for (size_t i = 0; i < n; ++i) {
+        const uint32_t r = fill[assign[i]]++;
+        row_ids[r] = uint32_t(i);
+        std::copy(src + i * row_bytes, src + (i + 1) * row_bytes, rows.data() + size_t(r) * ix->row_stride);
+    }
+    ix->reps.push_back(std::make_unique<Replica>());
+    Replica* rep = ix->reps.back().get();
+    rep->device = device;
+    rep->sm_count = prop.multiProcessorCount;
+    CUDA_TRY(rep->d_vectors.ensure(rows.size()));
+    CUDA_TRY(cudaMemcpy(rep->d_vectors.ptr, rows.data(), rows.size(), cudaMemcpyHostToDevice));
+    CUDA_TRY(iv->d_row_ids.ensure(row_ids.size()));
+    CUDA_TRY(cudaMemcpy(iv->d_row_ids.ptr, row_ids.data(), row_ids.size() * 4, cudaMemcpyHostToDevice));
+    CUDA_TRY(iv->d_start.ensure(C));
+    CUDA_TRY(cudaMemcpy(iv->d_start.ptr, start.data(), C * 4, cudaMemcpyHostToDevice));
+    CUDA_TRY(iv->d_count.ensure(C));
+    CUDA_TRY(cudaMemcpy(iv->d_count.ptr, iv->sizes.data(), C * 4, cudaMemcpyHostToDevice));
+    ix->device_bytes = rows.size() + row_ids.size() * 4 + C * 8 + iv->cent->ix->device_bytes;
+    iv->ix = std::move(ix);
+    *out = iv.release();
+    return 0;
+}
+
 
 }  // namespace svsb200
 
@@ -383,77 +500,92 @@ int svsb200_ivf_create(const void* vectors, int dtype, size_t n, size_t dim, int
     if (!out) return fail("svsb200_ivf_create: out is NULL");
     *out = nullptr;
     if (int rc = ivf_check_rows(who, vectors, dtype, n, dim, metric)) return rc;
-    const size_t C = num_centroids;
-    if (!centroids) return fail("svsb200_ivf_create: NULL centroids");
-    if (C == 0 || C >= (size_t(1) << 31)) return fail("svsb200_ivf_create: num_centroids must be in [1, 2^31)");
-    if (assignments)
-        for (size_t i = 0; i < n; ++i)
-            if (assignments[i] >= C) return fail("svsb200_ivf_create: assignment " + std::to_string(i) + " is not a cluster");
+    return ivf_assemble(who, vectors, dtype, SVSB200_PLAIN, 0.0f, 0.0f, n, dim, metric, centroids, num_centroids, assignments,
+                        device, out);
+}
+
+int svsb200_ivf_create_sq(const void* codes, int code_type, size_t n, size_t dim, int metric, float scale, float bias,
+                          const float* centroids, size_t num_centroids, const uint32_t* assignments, int device,
+                          svsb200_ivf** out) {
+    const char* who = "svsb200_ivf_create_sq";
+    if (!out) return fail("svsb200_ivf_create_sq: out is NULL");
+    *out = nullptr;
+    if (int rc = ivf_check_rows(who, codes, code_type, n, dim, metric, true)) return rc;
+    if (int rc = sq_check_params(who, scale, bias)) return rc;
+    if (!assignments) return fail("svsb200_ivf_create_sq: SQ rows need assignments (there is no float row to rank)");
+    return ivf_assemble(who, codes, code_type, SVSB200_SQ, scale, bias, n, dim, metric, centroids, num_centroids, assignments,
+                        device, out);
+}
+
+int svsb200_sq_compress(const float* data, size_t n, size_t dim, int code_type, int device, void* out_codes, float* out_scale,
+                        float* out_bias) {
+    const char* who = "svsb200_sq_compress";
+    if (!data || !out_codes || !out_scale || !out_bias) return fail("svsb200_sq_compress: NULL argument");
+    if (code_type != SVSB200_I8 && code_type != SVSB200_U8) return fail("svsb200_sq_compress: codes must be int8 or uint8");
+    const size_t count = n * dim;
+    if (count == 0) return fail("svsb200_sq_compress: empty dataset");
     cudaDeviceProp prop;
     if (int rc = check_device(who, device, &prop)) return rc;
     CUDA_TRY(cudaSetDevice(device));
-    auto iv = std::make_unique<svsb200_ivf>();
-    iv->n = n;
-    iv->C = C;
-    iv->centroids.assign(centroids, centroids + C * dim);
-    if (int rc = ivf_centroid_index(centroids, C, dim, metric, device, &iv->cent)) return rc;
-    const size_t row_bytes = dim * esize(dtype);
-    std::vector<uint32_t> assign(n);
-    if (assignments) {
-        std::copy(assignments, assignments + n, assign.begin());
-    } else {
-        OwnStream own;
-        CUDA_TRY(cudaStreamCreateWithFlags(&own.s, cudaStreamNonBlocking));
-        DeviceBuffer<char> d_rows;
-        DeviceBuffer<uint32_t> d_assign;
-        CUDA_TRY(d_rows.ensure(n * row_bytes));
-        CUDA_TRY(d_assign.ensure(n));
-        CUDA_TRY(cudaMemcpy(d_rows.ptr, vectors, n * row_bytes, cudaMemcpyHostToDevice));
-        if (int rc = ivf_assign(iv->cent.get(), d_rows.ptr, dtype, n, row_bytes, 65536, d_assign.ptr, own.s)) return rc;
-        CUDA_TRY(cudaMemcpy(assign.data(), d_assign.ptr, n * 4, cudaMemcpyDeviceToHost));
+    OwnStream own;
+    CUDA_TRY(cudaStreamCreateWithFlags(&own.s, cudaStreamNonBlocking));
+    // the values pass through the device in pieces of at most 2^26, twice: min and max, then the codes
+    const size_t piece = std::min(count, size_t(1) << 26);
+    DeviceBuffer<float> d_x;
+    DeviceBuffer<uint8_t> d_codes;
+    DeviceBuffer<uint32_t> d_red;
+    DeviceBuffer<unsigned long long> d_zero;
+    CUDA_TRY(d_x.ensure(piece));
+    CUDA_TRY(d_codes.ensure(piece));
+    CUDA_TRY(d_red.ensure(3));
+    CUDA_TRY(d_zero.ensure(1));
+    const uint32_t init[3] = {0xFFFFFFFFu, 0u, 0u};
+    CUDA_TRY(cudaMemcpyAsync(d_red.ptr, init, sizeof(init), cudaMemcpyHostToDevice, own.s));
+    CUDA_TRY(cudaMemsetAsync(d_zero.ptr, 0xFF, sizeof(unsigned long long), own.s));
+    const unsigned grid = unsigned(std::min<size_t>((piece + 255) / 256, size_t(prop.multiProcessorCount) * 8));
+    for (size_t lo = 0; lo < count; lo += piece) {
+        const size_t m = std::min(piece, count - lo);
+        CUDA_TRY(cudaMemcpyAsync(d_x.ptr, data + lo, m * 4, cudaMemcpyHostToDevice, own.s));
+        sq_minmax_kernel<<<grid, 256, 0, own.s>>>(d_x.ptr, m, lo, d_red.ptr, d_zero.ptr);
+        count_launch();
+        CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(cudaStreamSynchronize(own.s));   // (d_x is reused)
     }
-    // cluster-major layout: clusters in order, each from a 32-row boundary, its rows in ascending id
-    iv->sizes.assign(C, 0);
-    for (uint32_t a : assign) ++iv->sizes[a];
-    std::vector<uint32_t> start(C), fill(C);
-    size_t stored = 0;
-    for (size_t c = 0; c < C; ++c) {
-        start[c] = uint32_t(stored);
-        fill[c] = uint32_t(stored);
-        stored += round_up(iv->sizes[c], 32);
+    uint32_t red[3];
+    unsigned long long first_zero = 0;
+    CUDA_TRY(cudaMemcpy(red, d_red.ptr, sizeof(red), cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(&first_zero, d_zero.ptr, sizeof(first_zero), cudaMemcpyDeviceToHost));
+    if (red[2]) return fail("svsb200_sq_compress: the data hold a NaN or an infinity");
+    auto from_key = [](uint32_t k) {
+        const uint32_t u = (k & 0x80000000u) ? (k & 0x7FFFFFFFu) : ~k;
+        float f;
+        std::memcpy(&f, &u, 4);
+        return f;
+    };
+    float mn = from_key(red[0]);
+    const float mx = from_key(red[1]);
+    if (mn == 0.0f) mn = data[first_zero];   // the sign of the first zero, as the reference's sequential min keeps it
+    if (!(mx > mn)) return fail("svsb200_sq_compress: constant data (max == min) have no SQ scale");
+    // scale = (max - min) / (MAX - MIN), bias = min - MIN * scale: every operation rounded on its own, no contraction
+    const float MIN = code_type == SVSB200_I8 ? -128.0f : 0.0f, MAX = code_type == SVSB200_I8 ? 127.0f : 255.0f;
+    volatile float range = mx - mn;
+    const float scale = range / (MAX - MIN);
+    volatile float t = MIN * scale;
+    const float bias = mn - t;
+    for (size_t lo = 0; lo < count; lo += piece) {
+        const size_t m = std::min(piece, count - lo);
+        CUDA_TRY(cudaMemcpyAsync(d_x.ptr, data + lo, m * 4, cudaMemcpyHostToDevice, own.s));
+        if (code_type == SVSB200_I8)
+            sq_encode_kernel<SVSB200_I8><<<grid, 256, 0, own.s>>>(d_x.ptr, m, scale, bias, d_codes.ptr);
+        else
+            sq_encode_kernel<SVSB200_U8><<<grid, 256, 0, own.s>>>(d_x.ptr, m, scale, bias, d_codes.ptr);
+        count_launch();
+        CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(cudaMemcpyAsync(static_cast<uint8_t*>(out_codes) + lo, d_codes.ptr, m, cudaMemcpyDeviceToHost, own.s));
+        CUDA_TRY(cudaStreamSynchronize(own.s));   // (d_x and d_codes are reused)
     }
-    if (stored >= (size_t(1) << 32)) return fail("svsb200_ivf_create: too many rows");
-    auto ix = std::make_unique<svsb200_index>();
-    ix->dtype = dtype;
-    ix->metric = metric;
-    ix->storage = SVSB200_PLAIN;
-    ix->n = std::max<size_t>(stored, 1);
-    ix->dim = dim;
-    ix->row_stride = data_row_stride(SVSB200_PLAIN, dtype, dim);
-    ix->gstride = 32;
-    std::vector<uint32_t> row_ids(ix->n, 0xFFFFFFFFu);
-    std::vector<char> rows(ix->n * size_t(ix->row_stride), 0);
-    const char* src = static_cast<const char*>(vectors);
-    for (size_t i = 0; i < n; ++i) {
-        const uint32_t r = fill[assign[i]]++;
-        row_ids[r] = uint32_t(i);
-        std::copy(src + i * row_bytes, src + (i + 1) * row_bytes, rows.data() + size_t(r) * ix->row_stride);
-    }
-    ix->reps.push_back(std::make_unique<Replica>());
-    Replica* rep = ix->reps.back().get();
-    rep->device = device;
-    rep->sm_count = prop.multiProcessorCount;
-    CUDA_TRY(rep->d_vectors.ensure(rows.size()));
-    CUDA_TRY(cudaMemcpy(rep->d_vectors.ptr, rows.data(), rows.size(), cudaMemcpyHostToDevice));
-    CUDA_TRY(iv->d_row_ids.ensure(row_ids.size()));
-    CUDA_TRY(cudaMemcpy(iv->d_row_ids.ptr, row_ids.data(), row_ids.size() * 4, cudaMemcpyHostToDevice));
-    CUDA_TRY(iv->d_start.ensure(C));
-    CUDA_TRY(cudaMemcpy(iv->d_start.ptr, start.data(), C * 4, cudaMemcpyHostToDevice));
-    CUDA_TRY(iv->d_count.ensure(C));
-    CUDA_TRY(cudaMemcpy(iv->d_count.ptr, iv->sizes.data(), C * 4, cudaMemcpyHostToDevice));
-    ix->device_bytes = rows.size() + row_ids.size() * 4 + C * 8 + iv->cent->ix->device_bytes;
-    iv->ix = std::move(ix);
-    *out = iv.release();
+    *out_scale = scale;
+    *out_bias = bias;
     return 0;
 }
 

@@ -272,6 +272,230 @@ __global__ void __launch_bounds__(IVF_WARPS * 32, 2) ivf_scan_kernel(const __gri
     }
 }
 
+// ---- SQ rows under L2: the leaf on the integer tensor cores ----
+// EuclideanCompressed (quantization/scalar/scalar.h:58-105) is scale^2 * float(sum (qc - x)^2) with an exact integer
+// sum, so qq + xx - 2 <qc, x> from int8 / uint8 MMAs gives the same bits in any order.  The arithmetic is int32 and
+// wraps as the search path's dp4a sums do, so even past the reference's own bound (dim * 255^2 < 2^31) the keys equal
+// finish_distance<OP_L2I>'s.
+// Shared memory of one CTA: the ring; per query slot {query codes zero-padded to kpad = dim rounded up to 32 bytes, keys,
+// ids}; per warp {candidate keys, positions}; per query slot the 32 dot products of a tile; the 32 rows' xx.
+__host__ __device__ inline size_t ivf_sq_slot_bytes(uint32_t dim, uint32_t k) {
+    return size_t((dim + 31) & ~31u) + (size_t(k) * 8 + 15) / 16 * 16;
+}
+__host__ __device__ inline size_t ivf_sq_l2_smem_bytes(uint32_t row_stride, uint32_t tile_rows, uint32_t dim, uint32_t k,
+                                                       uint32_t Q) {
+    return 2 * size_t(tile_rows) * row_stride + size_t(Q) * (ivf_sq_slot_bytes(dim, k) + 32 * 4) + size_t(IVF_WARPS) * 32 * 8 +
+           32 * 4;
+}
+
+template <int ROWT>
+__device__ __forceinline__ void mma_m16n8k32_int(int (&c)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
+    if constexpr (ROWT == SVSB200_I8) {
+        asm volatile("mma.sync.aligned.m16n8k32.row.col.s32.s8.s8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                     : "+r"(c[0]), "+r"(c[1]), "+r"(c[2]), "+r"(c[3])
+                     : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
+    } else {
+        asm volatile("mma.sync.aligned.m16n8k32.row.col.s32.u8.u8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                     : "+r"(c[0]), "+r"(c[1]), "+r"(c[2]), "+r"(c[3])
+                     : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
+    }
+}
+
+// Work items, ring, lists and output are ivf_scan_kernel's.  Per staged tile: the slots' query codes (the A operand,
+// zero-padded to a multiple of 32 bytes) times the tile's codes (the B operand) on mma.m16n8k32, warp w taking the
+// queries 16 (w / 2) .. + 16 and the rows 16 (w % 2) .. + 16; warp 0 also sums each row's xx with dp4a.  Code bytes
+// past a row's stride, rows past the tile and queries past the work item's slots count as zero, so Q and the tile
+// need not fill whole MMA blocks.  Then every slot's 32 keys go through ivf_merge<DYN>.
+template <int ROWT, bool DYN>
+__global__ void __launch_bounds__(IVF_WARPS * 32, 2) ivf_scan_sq_l2_kernel(const __grid_constant__ IvfScanParams ip) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    const SearchParams& p = ip.p;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int grp = lane >> 2, tig = lane & 3;
+    const uint32_t tile_bytes = ip.tile_rows * p.row_stride;
+    const uint32_t kpad = (p.dim + 31) & ~31u;
+    unsigned char* ring = smem_raw;
+    unsigned char* slots = smem_raw + 2 * size_t(tile_bytes);
+    const size_t slot_bytes = ivf_sq_slot_bytes(p.dim, ip.k);
+    float* ckey = reinterpret_cast<float*>(slots + size_t(ip.Q) * slot_bytes) + warp * 64;
+    uint32_t* spos = reinterpret_cast<uint32_t*>(ckey + 32);
+    int* dots = reinterpret_cast<int*>(slots + size_t(ip.Q) * slot_bytes + size_t(IVF_WARPS) * 32 * 8);   // [Q][32]
+    int* xxs = dots + size_t(ip.Q) * 32;                                                                  // [32]
+    __shared__ uint32_t s_item;
+    __shared__ uint32_t s_size[IVF_QMAX];
+    const uint32_t total = ip.item_off[ip.C];
+
+    for (;;) {
+        if (threadIdx.x == 0) s_item = atomicAdd(ip.work_counter, 1u);
+        __syncthreads();
+        const uint32_t item = s_item;
+        __syncthreads();
+        if (item >= total) break;
+        uint32_t lo = 0, hi = ip.C;
+        while (hi - lo > 1) {
+            const uint32_t mid = (lo + hi) >> 1;
+            if (ip.item_off[mid] <= item) lo = mid; else hi = mid;
+        }
+        const uint32_t c = lo;
+        const uint32_t first = ip.list_off[c] + (item - ip.item_off[c]) * ip.Q;
+        const uint32_t nslots = min(ip.Q, ip.list_off[c + 1] - first);
+        const uint32_t count = ip.cl_count[c];
+        const char* crows = ip.rows + size_t(ip.cl_start[c]) * p.row_stride;
+        const uint32_t* cids = ip.row_ids + ip.cl_start[c];
+        const uint32_t ntiles = (count + ip.tile_rows - 1) / ip.tile_rows;
+        auto stage = [&](uint32_t tile) {
+            const char* src = crows + size_t(tile) * tile_bytes;
+            unsigned char* dst = ring + (tile & 1u) * tile_bytes;
+            for (uint32_t o = threadIdx.x * 16; o < tile_bytes; o += IVF_WARPS * 32 * 16) cp_async16(dst + o, src + o);
+            cp_async_commit();
+        };
+        if (ntiles) stage(0);
+        // the slots' query codes (prepared as for the SQ search: PREP_SQ_L2), zero past qstride up to kpad
+        for (uint32_t s = 0; s < nslots; ++s) {
+            uint32_t* q_s = reinterpret_cast<uint32_t*>(slots + s * slot_bytes);
+            const uint32_t* src = reinterpret_cast<const uint32_t*>(p.qcodes + size_t(ip.list[first + s] / ip.P) * p.qstride);
+            for (uint32_t i = threadIdx.x; i < kpad / 4; i += IVF_WARPS * 32) q_s[i] = 4 * i < p.qstride ? src[i] : 0u;
+        }
+        if (threadIdx.x < IVF_QMAX) s_size[threadIdx.x] = 0;
+        __syncthreads();
+        for (uint32_t tile = 0; tile < ntiles; ++tile) {
+            if (tile + 1 < ntiles) {
+                stage(tile + 1);
+                asm volatile("cp.async.wait_group 1;" ::: "memory");
+            } else {
+                cp_async_wait_all();
+            }
+            __syncthreads();
+            const unsigned char* trow = ring + (tile & 1u) * tile_bytes;
+            const uint32_t rows = min(ip.tile_rows, count - tile * ip.tile_rows);
+            // dot products: A block m = warp / 2, row blocks n0 = 16 (warp % 2) and n0 + 8
+            const uint32_t m0 = uint32_t(warp >> 1) * 16, r0 = uint32_t(warp & 1) * 16;
+            if (m0 < nslots && r0 < rows) {
+                int acc[2][4] = {};
+                const unsigned char* qa = slots + size_t(m0 + grp) * slot_bytes;
+                const unsigned char* qb = qa + 8 * slot_bytes;
+                const bool qlive0 = m0 + grp < nslots, qlive1 = m0 + grp + 8 < nslots;   // (slots past Q do not exist)
+                const bool live0 = r0 + grp < rows, live1 = r0 + 8 + grp < rows;
+                const unsigned char* b0row = trow + size_t(r0 + grp) * p.row_stride;
+                const unsigned char* b1row = b0row + 8 * size_t(p.row_stride);
+#pragma unroll 1
+                for (uint32_t k0 = 0; k0 < kpad; k0 += 32) {
+                    const uint32_t o0 = k0 + 4 * tig, o1 = o0 + 16;
+                    const uint32_t a[4] = {qlive0 ? *reinterpret_cast<const uint32_t*>(qa + o0) : 0u,
+                                           qlive1 ? *reinterpret_cast<const uint32_t*>(qb + o0) : 0u,
+                                           qlive0 ? *reinterpret_cast<const uint32_t*>(qa + o1) : 0u,
+                                           qlive1 ? *reinterpret_cast<const uint32_t*>(qb + o1) : 0u};
+                    const uint32_t b0[2] = {live0 && o0 < p.row_stride ? *reinterpret_cast<const uint32_t*>(b0row + o0) : 0u,
+                                            live0 && o1 < p.row_stride ? *reinterpret_cast<const uint32_t*>(b0row + o1) : 0u};
+                    const uint32_t b1[2] = {live1 && o0 < p.row_stride ? *reinterpret_cast<const uint32_t*>(b1row + o0) : 0u,
+                                            live1 && o1 < p.row_stride ? *reinterpret_cast<const uint32_t*>(b1row + o1) : 0u};
+                    mma_m16n8k32_int<ROWT>(acc[0], a, b0);
+                    mma_m16n8k32_int<ROWT>(acc[1], a, b1);
+                }
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const uint32_t col = r0 + 8 * h + 2 * tig;
+                    if (qlive0) {
+                        dots[(m0 + grp) * 32 + col] = acc[h][0];
+                        dots[(m0 + grp) * 32 + col + 1] = acc[h][1];
+                    }
+                    if (qlive1) {
+                        dots[(m0 + grp + 8) * 32 + col] = acc[h][2];
+                        dots[(m0 + grp + 8) * 32 + col + 1] = acc[h][3];
+                    }
+                }
+            }
+            if (warp == 0) {   // xx of every row of the tile
+                int xx = 0;
+                if (uint32_t(lane) < rows) {
+                    const uint32_t* w = reinterpret_cast<const uint32_t*>(trow + size_t(lane) * p.row_stride);
+                    for (uint32_t i = 0; i < p.row_stride / 4; ++i) {
+                        if constexpr (ROWT == SVSB200_I8) xx = __dp4a(int(w[i]), int(w[i]), xx);
+                        else xx = int(__dp4a(w[i], w[i], unsigned(xx)));
+                    }
+                }
+                xxs[lane] = xx;
+            }
+            __syncthreads();
+#pragma unroll 1
+            for (uint32_t i = 0; i < IVF_QMAX / IVF_WARPS; ++i) {
+                const uint32_t s = warp + IVF_WARPS * i;
+                if (s >= nslots) break;
+                float* bkey = reinterpret_cast<float*>(slots + s * slot_bytes + kpad);
+                uint32_t* bid = reinterpret_cast<uint32_t*>(bkey + ip.k);
+                const uint32_t q = ip.list[first + s] / ip.P;
+                const uint32_t qq = __float_as_uint(p.qaux[2 * size_t(q) + 1]);   // int32 bits of sum qc^2
+                if (uint32_t(lane) < rows) {
+                    const uint32_t l2 = qq + uint32_t(xxs[lane]) - 2u * uint32_t(dots[s * 32 + lane]);
+                    ckey[lane] = __fmul_rn(p.scale_sq, float(int(l2)));
+                }
+                __syncwarp();
+                uint32_t size = s_size[s];
+                ivf_merge<DYN>(bkey, bid, size, ip.k, ckey, cids + tile * ip.tile_rows, rows, spos, lane);
+                if (lane == 0) s_size[s] = size;
+            }
+            __syncthreads();
+        }
+#pragma unroll 1
+        for (uint32_t i = 0; i < IVF_QMAX / IVF_WARPS; ++i) {
+            const uint32_t s = warp + IVF_WARPS * i;
+            if (s >= nslots) break;
+            const float* bkey = reinterpret_cast<const float*>(slots + s * slot_bytes + kpad);
+            const uint32_t* bid = reinterpret_cast<const uint32_t*>(bkey + ip.k);
+            const uint32_t e = ip.list[first + s], q = e / ip.P, probe = e - q * ip.P;
+            const size_t o = (size_t(probe) * ip.nq + q) * ip.k;
+            for (uint32_t j = lane; j < ip.k; j += 32) {
+                const bool v = j < s_size[s];
+                ip.out_ids[o + j] = v ? uint64_t(bid[j]) : ~uint64_t(0);
+                ip.out_dists[o + j] = v ? bkey[j] : INFINITY;
+            }
+        }
+        __syncthreads();
+    }
+}
+
+// ---- SQ compression (SQDataset::compress, quantization/scalar/scalar.h:447-469) ----
+// out[0] = min and out[1] = max as order-preserving keys (atomicMin / atomicMax), out[2] = non-zero when a value is not
+// finite, out[3] = the first index holding a zero (the reference's sequential min keeps the sign of the first zero).
+__device__ __forceinline__ uint32_t sq_order_key(float v) {
+    const uint32_t u = __float_as_uint(__fadd_rn(v, 0.0f));   // -0 -> +0: both zeros are one key
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__global__ void sq_minmax_kernel(const float* __restrict__ x, size_t count, uint64_t base, uint32_t* __restrict__ out,
+                                 unsigned long long* __restrict__ first_zero) {
+    uint32_t mn = 0xFFFFFFFFu, mx = 0u, bad = 0u;
+    unsigned long long fz = ~0ull;
+    for (size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x; i < count; i += size_t(gridDim.x) * blockDim.x) {
+        const float v = x[i];
+        if (!isfinite(v)) bad = 1u;
+        const uint32_t key = sq_order_key(v);
+        mn = min(mn, key);
+        mx = max(mx, key);
+        if (v == 0.0f && fz == ~0ull) fz = base + i;
+    }
+    for (int o = 16; o; o >>= 1) {
+        mn = min(mn, __shfl_xor_sync(0xFFFFFFFFu, mn, o));
+        mx = max(mx, __shfl_xor_sync(0xFFFFFFFFu, mx, o));
+        bad |= __shfl_xor_sync(0xFFFFFFFFu, bad, o);
+        fz = min(fz, __shfl_xor_sync(0xFFFFFFFFu, fz, o));
+    }
+    if ((threadIdx.x & 31) == 0) {
+        atomicMin(out, mn);
+        atomicMax(out + 1, mx);
+        if (bad) atomicOr(out + 2, 1u);
+        if (fz != ~0ull) atomicMin(first_zero, fz);
+    }
+}
+// detail::compress (scalar.h:38-42): clamp(round((x - bias) / scale), MIN, MAX), halves away from zero.
+template <int CODE>
+__global__ void sq_encode_kernel(const float* __restrict__ x, size_t count, float scale, float bias, uint8_t* __restrict__ out) {
+    constexpr float lo = CODE == SVSB200_I8 ? -128.f : 0.f, hi = CODE == SVSB200_I8 ? 127.f : 255.f;
+    for (size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x; i < count; i += size_t(gridDim.x) * blockDim.x) {
+        const float r = fminf(fmaxf(roundf(__fdiv_rn(__fsub_rn(x[i], bias), scale)), lo), hi);
+        out[i] = CODE == SVSB200_I8 ? uint8_t(int8_t(int(r))) : uint8_t(int(r));
+    }
+}
+
 // ---- inversion of the probes: per-cluster lists of (query, probe), ascending ----
 // counts[c] += 1 for every probe of c.
 __global__ void ivf_count_kernel(const uint64_t* __restrict__ probes, size_t total, uint32_t* __restrict__ counts) {

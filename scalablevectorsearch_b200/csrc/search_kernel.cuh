@@ -66,6 +66,7 @@ template <> struct Row<SVSB200_I8> {
     __device__ static __forceinline__ raw_t load(const char* p) {
         return __ldg(reinterpret_cast<const uint2*>(p));
     }
+    __device__ static __forceinline__ raw_t lds(const char* p) { return *reinterpret_cast<const uint2*>(p); }
     __device__ static __forceinline__ void cvt(const raw_t& r, float (&y)[8]) {
         const uint32_t w[2] = {r.x, r.y};
 #pragma unroll
@@ -80,6 +81,7 @@ template <> struct Row<SVSB200_U8> {
     __device__ static __forceinline__ raw_t load(const char* p) {
         return __ldg(reinterpret_cast<const uint2*>(p));
     }
+    __device__ static __forceinline__ raw_t lds(const char* p) { return *reinterpret_cast<const uint2*>(p); }
     __device__ static __forceinline__ void cvt(const raw_t& r, float (&y)[8]) {
         const uint32_t w[2] = {r.x, r.y};
 #pragma unroll
@@ -159,7 +161,8 @@ template <int LPT> __device__ __forceinline__ float reduce_lanes(float (&s)[LPT]
 //   rowp[r]   this thread group's row base pointers (nullptr = inactive slot)
 //   t         thread index inside the group
 // Returns the *raw* reduced sums (op, norm) -- identical in every thread of the group.
-// SMEM = true: the rows are staged in shared memory (the IVF scan, ivf_kernel.cuh); float32 / float16 rows only.
+// SMEM = true: the rows are staged in shared memory (the IVF scan, ivf_kernel.cuh); float32 / float16 rows and, for the
+// SQ index's MIP and cosine, int8 / uint8 codes.
 // ---------------------------------------------------------------------------------------
 template <int ROWT, int OP, int DS, int NROWS, bool DENSE = false, bool SMEM = false>
 __device__ __forceinline__ void float_rows(

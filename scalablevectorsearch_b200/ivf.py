@@ -5,6 +5,11 @@
     index.search_parameters = IVFSearchParameters(n_probes=16)
     I, D = index.search(queries, 10)                   # numpy (nq, k) uint64 / float32
 
+Scalar-quantised rows (the reference's ``StorageKind::SQI8`` and its uint8 twin) take four times less device memory:
+
+    codes, scale, bias = sq_compress(data)             # int8 codes, one global scale and bias
+    index = IVF.assemble_from_clustering(clustering, codes, DistanceType.L2, sq=(scale, bias))
+
 Backed by ``svsb200_ivf_*`` of ``libsvsb200.so``.  The k-means is the reference's flat k-means made deterministic (an own
 documented random sequence, float32 sums in row order), so ``is_hierarchical`` defaults to False here and True is
 refused.  A search returns the exact top k over the probed clusters, bit for bit the distances of the exact scan.
@@ -50,6 +55,36 @@ def _rows(data) -> np.ndarray:
     return data
 
 
+def sq_compress(data, dtype=np.int8, device: int = 0):
+    """``SQDataset<int8_t / uint8_t>::compress`` on the GPU (``svsb200_sq_compress``): float32 rows [n, dim] ->
+    (codes [n, dim] of ``dtype``, scale, bias).  NaN, infinite and constant data are refused."""
+    x = np.ascontiguousarray(data.load() if hasattr(data, "load") else data)
+    if x.ndim != 2:
+        raise ValueError("data must be a 2-D array")
+    if x.dtype != np.float32:
+        raise TypeError(f"sq_compress takes float32 rows, got {x.dtype}")
+    dtype = np.dtype(dtype)
+    if dtype not in (np.dtype(np.int8), np.dtype(np.uint8)):
+        raise TypeError(f"SQ codes are int8 or uint8, got {dtype}")
+    codes = np.empty(x.shape, dtype=dtype)
+    scale, bias = C.c_float(), C.c_float()
+    _lib.check(_lib.lib().svsb200_sq_compress(x.ctypes.data, x.shape[0], x.shape[1], _DTYPE_CODE[dtype], int(device),
+                                              codes.ctypes.data, C.byref(scale), C.byref(bias)))
+    return codes, float(np.float32(scale.value)), float(np.float32(bias.value))
+
+
+def _sq_codes(data, sq) -> np.ndarray:
+    """The codes of an SQ ``assemble_from_clustering``: int8 / uint8 rows."""
+    x = np.ascontiguousarray(data.load() if hasattr(data, "load") else data)
+    if x.ndim != 2:
+        raise ValueError("data must be a 2-D array")
+    if x.dtype not in (np.dtype(np.int8), np.dtype(np.uint8)):
+        raise TypeError(f"with sq=(scale, bias) the data are int8 or uint8 codes, got {x.dtype}")
+    if len(sq) != 2:
+        raise ValueError("sq must be (scale, bias)")
+    return x
+
+
 class Clustering:
     """``svs.Clustering``: centroids float32 [C, dim] and one cluster per data row (uint32 [n])."""
 
@@ -88,10 +123,11 @@ class IVF:
 
     @staticmethod
     def assemble_from_clustering(clustering: Clustering, data, distance: DistanceType = DistanceType.L2,
-                                 device: int = 0) -> "IVF":
+                                 device: int = 0, sq: tuple | None = None) -> "IVF":
         """``svs.IVF.assemble_from_clustering``: the rows grouped as the clustering says (a clustering without
-        assignments puts every row in its nearest cluster)."""
-        x = _rows(data)
+        assignments puts every row in its nearest cluster).  ``sq=(scale, bias)`` marks ``data`` as int8 / uint8 SQ
+        codes (see :func:`sq_compress`); the clustering must then carry assignments."""
+        x = _rows(data) if sq is None else _sq_codes(data, sq)
         cent = clustering.centroids
         if cent.shape[1] != x.shape[1]:
             raise ValueError(f"centroids have {cent.shape[1]} dimensions, data {x.shape[1]}")
@@ -100,6 +136,12 @@ class IVF:
             raise ValueError("the clustering has one assignment per data row")
         lib = _lib.lib()
         handle = C.c_void_p()
+        if sq is not None:
+            _lib.check(lib.svsb200_ivf_create_sq(x.ctypes.data, _DTYPE_CODE[x.dtype], x.shape[0], x.shape[1],
+                                                 int(DistanceType(distance)), float(sq[0]), float(sq[1]), cent.ctypes.data,
+                                                 cent.shape[0], None if a is None else a.ctypes.data, int(device),
+                                                 C.byref(handle)))
+            return IVF(handle, lib, DistanceType(distance))
         _lib.check(lib.svsb200_ivf_create(x.ctypes.data, _DTYPE_CODE[x.dtype], x.shape[0], x.shape[1],
                                           int(DistanceType(distance)), cent.ctypes.data, cent.shape[0],
                                           None if a is None else a.ctypes.data, int(device), C.byref(handle)))
