@@ -529,14 +529,14 @@ int svsb200_ivf_search(svsb200_ivf* index, const void* queries, int qdtype, size
                        uint64_t* out_ids, float* out_dists);
 
 /* Dynamic IVF index.  Replaces: DynamicIVFIndex (include/svs/index/ivf/dynamic_ivf.h) with svs::DynamicIVF: the IVF
- * index over a mutable set of float32 / float16 rows on one device, L2 / MIP / cosine, addressed by external ids.  A
- * distinct handle type.  Every slot (internal id) is Valid or Empty; a delete empties it at once and leaves a tombstone
- * in its cluster, which no search returns.  The centroids never move after assembly: an added row joins its nearest
- * centroid, ranked as a probe ranks centroids (the flat search at k = 1, ties to the lower centroid).  External id
- * 2^64 - 1 is reserved (it marks padding).  Searches may run concurrently with each other; a mutation (add, delete,
- * compact) first waits for every search of the index enqueued so far, including the work that
- * svsb200_dynamic_ivf_search_device leaves queued on the caller's stream, so it may follow such a call without a
- * synchronisation; a search enqueued while a mutation runs is the caller's error. */
+ * index over a mutable set of float32 / float16 rows (or SQ codes, svsb200_dynamic_ivf_create_sq) on one device, L2 /
+ * MIP / cosine, addressed by external ids.  A distinct handle type.  Every slot (internal id) is Valid or Empty; a
+ * delete empties it at once and leaves a tombstone in its cluster, which no search returns.  The centroids never move
+ * after assembly: an added row joins its nearest centroid, ranked as a probe ranks centroids (the flat search at k = 1,
+ * ties to the lower centroid).  External id 2^64 - 1 is reserved (it marks padding).  Searches may run concurrently
+ * with each other; a mutation (add, delete, compact) first waits for every search of the index enqueued so far,
+ * including the work that svsb200_dynamic_ivf_search_device leaves queued on the caller's stream, so it may follow such
+ * a call without a synchronisation; a search enqueued while a mutation runs is the caller's error. */
 typedef struct svsb200_dynamic_ivf svsb200_dynamic_ivf;
 
 /* assemble_from_clustering: n x dim rows (HOST) with one distinct external id each, grouped by `assignments` (uint32
@@ -545,6 +545,21 @@ typedef struct svsb200_dynamic_ivf svsb200_dynamic_ivf;
 int svsb200_dynamic_ivf_create(const void* vectors, int dtype, size_t n, size_t dim, int metric, const float* centroids,
                                size_t num_centroids, const uint32_t* assignments, const uint64_t* external_ids, int device,
                                svsb200_dynamic_ivf** out);
+/* assemble_from_clustering over SQ codes (DynamicIVFIndex with StorageKind::SQI8 and its uint8 twin): n x dim int8 /
+ * uint8 codes (HOST) with the `scale` (finite, positive) and `bias` (finite) they were compressed with, C float32
+ * centroids, one distinct external id per row, and assignments (uint32 [n], each < C), REQUIRED when n > 0: without
+ * float rows nothing can be ranked against the centroids.  Row i takes slot i.  n = 0 makes an empty SQ index whose
+ * scale and bias are fixed from the start.  Slots, mutations and refusals are the float index's, except that
+ * svsb200_dynamic_ivf_add takes float32 rows only (float16 and integer rows, and rows holding a NaN or an infinity, are
+ * refused before anything changes): each joins its nearest centroid, ranked from its float32 values as in a float
+ * index, and is encoded with the index's scale and bias as SQDataset::set_datum does (quantization/scalar/scalar.h:
+ * 417-429): clamp(roundf((x - bias) / scale), MIN, MAX), each operation rounded on its own, so that values outside
+ * the compressed range clamp.  A search returns the exact top k over the Valid rows of the probed clusters with the SQ
+ * search path's bit-exact distances (as svsb200_ivf_create_sq), ordered by (distance, slot); with n_probes = C it
+ * equals svsb200_exhaustive_device on an SQ svsb200_index over the Valid slots' codes in slot order. */
+int svsb200_dynamic_ivf_create_sq(const void* codes, int code_type, size_t n, size_t dim, int metric, float scale, float bias,
+                                  const float* centroids, size_t num_centroids, const uint32_t* assignments,
+                                  const uint64_t* external_ids, int device, svsb200_dynamic_ivf** out);
 /* Frees the handle and its device memory (NULL is ignored). */
 int svsb200_dynamic_ivf_destroy(svsb200_dynamic_ivf* index);
 /* Valid rows, slots (Valid or Empty), dimensions, clusters, and the device memory held (rows pool with its dead
@@ -557,7 +572,8 @@ size_t svsb200_dynamic_ivf_device_bytes(const svsb200_dynamic_ivf* index);
 /* Valid rows per cluster (uint32 [C]) and the centroids (float32 [C][dim]), HOST buffers. */
 int svsb200_dynamic_ivf_cluster_sizes(const svsb200_dynamic_ivf* index, uint32_t* out);
 int svsb200_dynamic_ivf_centroids(const svsb200_dynamic_ivf* index, float* out);
-/* add_points (dynamic_ivf.h:474-527): `count` rows of the index's dtype (dense, HOST) with one new external id each.
+/* add_points (dynamic_ivf.h:474-527): `count` rows of the index's dtype (float32 for an SQ index; dense, HOST) with one
+ * new external id each.
  * Without reuse_empty every row takes a new slot past the end; with it, Empty slots are taken in ascending order from
  * slot 0 first.  Each row is appended to its nearest centroid's cluster, in input order.  Everything (dtype, repeated,
  * present or reserved ids, 2^31-1 slots) is checked before anything changes.  `slots_out` (optional, `count` entries)

@@ -42,7 +42,7 @@ SYMBOLS = [
     "svsb200_dynamic_ivf_device_bytes", "svsb200_dynamic_ivf_cluster_sizes", "svsb200_dynamic_ivf_centroids",
     "svsb200_dynamic_ivf_add", "svsb200_dynamic_ivf_delete", "svsb200_dynamic_ivf_compact", "svsb200_dynamic_ivf_ids",
     "svsb200_dynamic_ivf_has_id", "svsb200_dynamic_ivf_export", "svsb200_dynamic_ivf_search",
-    "svsb200_dynamic_ivf_search_device",
+    "svsb200_dynamic_ivf_search_device", "svsb200_dynamic_ivf_create_sq",
 ]
 
 _lib = None
@@ -149,6 +149,8 @@ def lib() -> C.CDLL:
     l.svsb200_ivf_search.argtypes = [vp, vp, i32, sz, sz, sz, vp, vp]
     l.svsb200_ivf_search_device.argtypes = [vp, vp, i32, sz, sz, sz, vp, vp, vp]
     l.svsb200_dynamic_ivf_create.argtypes = [vp, i32, sz, sz, i32, vp, sz, vp, vp, i32, C.POINTER(vp)]
+    l.svsb200_dynamic_ivf_create_sq.argtypes = [vp, i32, sz, sz, i32, C.c_float, C.c_float, vp, sz, vp, vp, i32,
+                                                C.POINTER(vp)]
     l.svsb200_dynamic_ivf_destroy.argtypes = [vp]
     for name in ("size", "num_slots", "dimensions", "num_clusters", "device_bytes"):
         fn = getattr(l, f"svsb200_dynamic_ivf_{name}")

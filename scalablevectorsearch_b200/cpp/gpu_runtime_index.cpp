@@ -18,15 +18,20 @@
 // INVALID_ARGUMENT.  Divergence: k > 1024 is INVALID_ARGUMENT (the GPU search returns at most 1024 neighbours).
 //
 // And `svs::runtime::v0::IVFIndex` (bindings/cpp/include/svs/runtime/ivf_index.h) on the IVF index of libsvsb200
-// (svsb200_ivf_*) for FP32 and FP16 storage: `build` clusters (svsb200_ivf_cluster) and assembles the index, `search`
-// probes n_probes clusters (the build's default search parameters, overridden per call).  A non-null IDFilter, save /
-// load, LeanVec and the other storage kinds are NOT_IMPLEMENTED; is_hierarchical must be false (the GPU k-means is
-// flat), and unspecified build parameters take the Python IVFBuildParameters' defaults.
+// (svsb200_ivf_*) for FP32, FP16 and SQI8 storage: `build` clusters (svsb200_ivf_cluster) and assembles the index,
+// `search` probes n_probes clusters (the build's default search parameters, overridden per call).  SQI8 follows the
+// reference's init_impl: the float32 rows are clustered, then compressed to int8 (svsb200_sq_compress), then assembled
+// with the clustering's assignments (svsb200_ivf_create_sq); data that cannot be compressed (constant, or holding a
+// NaN or an infinity) is a RUNTIME_ERROR.  A non-null IDFilter, save / load, LeanVec and the other storage kinds are
+// NOT_IMPLEMENTED; is_hierarchical must be false (the GPU k-means is flat), and unspecified build parameters take the
+// Python IVFBuildParameters' defaults.
 //
 // And `svs::runtime::v0::DynamicIVFIndex` (bindings/cpp/include/svs/runtime/dynamic_ivf_index.h) on the dynamic IVF
-// index (svsb200_dynamic_ivf_*) for FP32 and FP16 storage, with the behaviour of the reference's DynamicIVFIndexImpl
-// (bindings/cpp/src/dynamic_ivf_index_impl.h): `build` with rows clusters them as IVFIndex::build does and assembles
-// the index; without rows there is no index until the first `add`, which clusters its own rows; before that, `search`
+// index (svsb200_dynamic_ivf_*) for FP32, FP16 and SQI8 storage, with the behaviour of the reference's
+// DynamicIVFIndexImpl (bindings/cpp/src/dynamic_ivf_index_impl.h): `build` with rows clusters (and for SQI8
+// compresses) them as IVFIndex::build does and assembles the index; without rows there is no index until the first
+// `add`, which clusters its own rows (and fixes the SQ scale and bias from them); a later SQI8 `add` passes its float32
+// rows through, to be encoded with that scale and bias; before initialisation, `search`
 // is NOT_INITIALIZED (labels -1, distances +inf), `remove` / `remove_selected` / `consolidate` / `compact` are
 // NOT_INITIALIZED and `has_id` is false.  k = 0 is INVALID_ARGUMENT; a non-null IDFilter, save / load and LeanVec are
 // NOT_IMPLEMENTED.
@@ -471,9 +476,9 @@ uint16_t to_half(float f) {
 }  // namespace
 
 Status IVFIndex::check_storage_kind(StorageKind kind) noexcept {
-    return kind == StorageKind::FP32 || kind == StorageKind::FP16
+    return kind == StorageKind::FP32 || kind == StorageKind::FP16 || kind == StorageKind::SQI8
                ? Status_Ok
-               : Status(ErrorCode::NOT_IMPLEMENTED, "IVFIndex on the GPU supports FP32 and FP16 storage only");
+               : Status(ErrorCode::NOT_IMPLEMENTED, "IVFIndex on the GPU supports FP32, FP16 and SQI8 storage only");
 }
 
 Status IVFIndex::build(IVFIndex** index, size_t dim, MetricType metric, StorageKind storage_kind, size_t n, const float* data,
@@ -506,7 +511,16 @@ Status IVFIndex::build(IVFIndex** index, size_t dim, MetricType metric, StorageK
                                 assignments.data()))
             return gpu_error();
         svsb200_ivf* h = nullptr;
-        if (svsb200_ivf_create(rows, dtype, n, dim, m, centroids.data(), C, assignments.data(), 0, &h)) return gpu_error();
+        if (storage_kind == StorageKind::SQI8) {   // compressed after clustering, as the reference's init_impl does
+            std::vector<int8_t> codes(n * dim);
+            float scale = 0.0f, bias = 0.0f;
+            if (svsb200_sq_compress(data, n, dim, SVSB200_I8, 0, codes.data(), &scale, &bias) ||
+                svsb200_ivf_create_sq(codes.data(), SVSB200_I8, n, dim, m, scale, bias, centroids.data(), C,
+                                      assignments.data(), 0, &h))
+                return gpu_error();
+        } else if (svsb200_ivf_create(rows, dtype, n, dim, m, centroids.data(), C, assignments.data(), 0, &h)) {
+            return gpu_error();
+        }
         *index = new (std::nothrow) GpuIVFIndex(h, default_search_params, num_threads, intra_query_threads);
         if (!*index) {
             svsb200_ivf_destroy(h);
@@ -574,8 +588,17 @@ Status cluster_and_assemble(size_t dim, MetricType metric, StorageKind kind, con
                             assignments.data()))
         return gpu_error();
     static_assert(sizeof(size_t) == 8, "labels are 64-bit");
-    if (svsb200_dynamic_ivf_create(rows, dtype, n, dim, m, centroids.data(), C, assignments.data(),
-                                   reinterpret_cast<const uint64_t*>(labels), 0, out))
+    const uint64_t* ids = reinterpret_cast<const uint64_t*>(labels);
+    if (kind == StorageKind::SQI8) {   // compressed after clustering (dynamic_ivf_index_impl.h:391-425)
+        std::vector<int8_t> codes(n * dim);
+        float scale = 0.0f, bias = 0.0f;
+        if (svsb200_sq_compress(data, n, dim, SVSB200_I8, 0, codes.data(), &scale, &bias) ||
+            svsb200_dynamic_ivf_create_sq(codes.data(), SVSB200_I8, n, dim, m, scale, bias, centroids.data(), C,
+                                          assignments.data(), ids, 0, out))
+            return gpu_error();
+        return Status_Ok;
+    }
+    if (svsb200_dynamic_ivf_create(rows, dtype, n, dim, m, centroids.data(), C, assignments.data(), ids, 0, out))
         return gpu_error();
     return Status_Ok;
 }
@@ -710,9 +733,9 @@ class GpuDynamicIVFIndex final : public DynamicIVFIndex {
 }  // namespace
 
 Status DynamicIVFIndex::check_storage_kind(StorageKind kind) noexcept {
-    return kind == StorageKind::FP32 || kind == StorageKind::FP16
+    return kind == StorageKind::FP32 || kind == StorageKind::FP16 || kind == StorageKind::SQI8
                ? Status_Ok
-               : Status(ErrorCode::NOT_IMPLEMENTED, "DynamicIVFIndex on the GPU supports FP32 and FP16 storage only");
+               : Status(ErrorCode::NOT_IMPLEMENTED, "DynamicIVFIndex on the GPU supports FP32, FP16 and SQI8 storage only");
 }
 
 Status DynamicIVFIndex::build(DynamicIVFIndex** index, size_t dim, MetricType metric, StorageKind storage_kind, size_t n,

@@ -12,9 +12,14 @@
 //
 // Searches are the IVF index's (ivf.cu) with the scan's DYN form: tombstones are not candidates, and the lists are
 // ordered by (distance, slot) before the slots become external ids.
+//
+// SQ storage (svsb200_dynamic_ivf_create_sq): the pool holds int8 / uint8 codes under one scale and bias fixed at
+// assembly.  An add takes float32 rows, ranks them against the centroids as a float index does, and encodes them on the
+// device (sq_encode) before they are placed; delete and compact move codes as they move float rows.
 #include "ivf.cuh"
 
 #include <algorithm>
+#include <cmath>
 #include <unordered_set>
 
 struct svsb200_dynamic_ivf {
@@ -24,7 +29,7 @@ struct svsb200_dynamic_ivf {
     std::vector<uint32_t> slot_cluster, slot_index;  // per slot: where its entry is (all-ones for an Empty slot)
     size_t pool_used = 0;                   // pool rows handed out to cluster regions
     // staging of a mutation, kept between calls
-    svsb200::DeviceBuffer<unsigned char> dense, rows;
+    svsb200::DeviceBuffer<unsigned char> dense, rows, codes;   // (codes: an SQ index's added rows, encoded)
     svsb200::DeviceBuffer<uint32_t> assign, src_pos, dst_pos, vals;
     svsb200::DeviceBuffer<uint64_t> ids;
 };
@@ -131,27 +136,23 @@ static svsb200_ivf* ivf_of(svsb200_dynamic_ivf* h) { return h ? &h->iv : nullptr
 
 using namespace svsb200;
 
-extern "C" {
-
-int svsb200_dynamic_ivf_create(const void* vectors, int dtype, size_t n, size_t dim, int metric, const float* centroids,
-                               size_t num_centroids, const uint32_t* assignments, const uint64_t* external_ids, int device,
-                               svsb200_dynamic_ivf** out) {
-    const char* who = "svsb200_dynamic_ivf_create";
-    if (!out) return fail("svsb200_dynamic_ivf_create: NULL output");
-    *out = nullptr;
-    if (n && (!vectors || !external_ids)) return fail("svsb200_dynamic_ivf_create: NULL input");
-    if (dtype != SVSB200_F32 && dtype != SVSB200_F16)
-        return fail("svsb200_dynamic_ivf_create: rows must be float32 or float16 (integer, SQ and LVQ rows are not supported)");
-    if (metric < SVSB200_L2 || metric > SVSB200_COSINE) return fail("svsb200_dynamic_ivf_create: bad metric");
-    if (dim == 0) return fail("svsb200_dynamic_ivf_create: dim must be positive");
-    if (n >= (size_t(1) << 31)) return fail("svsb200_dynamic_ivf_create: more than 2^31-1 slots");
+// assemble_from_clustering over checked rows (SQ codes when `storage` is SVSB200_SQ): the static layout, clusters in
+// order, each from a 32-row boundary, its rows in ascending slot.
+static int dynamic_ivf_assemble(const char* who, const void* vectors, int dtype, int storage, float scale, float bias,
+                                size_t n, size_t dim, int metric, const float* centroids, size_t num_centroids,
+                                const uint32_t* assignments, const uint64_t* external_ids, int device,
+                                svsb200_dynamic_ivf** out) {
+    const std::string w(who);
+    if (metric < SVSB200_L2 || metric > SVSB200_COSINE) return fail(w + ": bad metric");
+    if (dim == 0) return fail(w + ": dim must be positive");
+    if (n >= (size_t(1) << 31)) return fail(w + ": more than 2^31-1 slots");
     const size_t C = num_centroids;
-    if (!centroids) return fail("svsb200_dynamic_ivf_create: NULL centroids");
-    if (C == 0 || C >= (size_t(1) << 31)) return fail("svsb200_dynamic_ivf_create: num_centroids must be in [1, 2^31)");
+    if (!centroids) return fail(w + ": NULL centroids");
+    if (C == 0 || C >= (size_t(1) << 31)) return fail(w + ": num_centroids must be in [1, 2^31)");
     if (assignments)
         for (size_t i = 0; i < n; ++i)
             if (assignments[i] >= C)
-                return fail("svsb200_dynamic_ivf_create: assignment " + std::to_string(i) + " is not a cluster");
+                return fail(w + ": assignment " + std::to_string(i) + " is not a cluster");
     if (int rc = check_ids_new(who, nullptr, external_ids, n)) return rc;
     cudaDeviceProp prop;
     if (int rc = check_device(who, device, &prop)) return rc;
@@ -165,9 +166,11 @@ int svsb200_dynamic_ivf_create(const void* vectors, int dtype, size_t n, size_t 
     svsb200_index* ix = iv.ix.get();
     ix->dtype = dtype;
     ix->metric = metric;
-    ix->storage = SVSB200_PLAIN;
+    ix->storage = storage;
+    ix->scale = scale;
+    ix->bias = bias;
     ix->dim = dim;
-    ix->row_stride = data_row_stride(SVSB200_PLAIN, dtype, dim);
+    ix->row_stride = data_row_stride(storage, dtype, dim);
     ix->gstride = 32;
     ix->status.assign(n, SLOT_VALID);
     ix->ext_ids.assign(external_ids, external_ids + n);
@@ -202,7 +205,7 @@ int svsb200_dynamic_ivf_create(const void* vectors, int dtype, size_t n, size_t 
         h->cap[c] = uint32_t(round_up(h->count[c], 32));
         used += h->cap[c];
     }
-    if (used >= (size_t(1) << 32)) return fail("svsb200_dynamic_ivf_create: too many rows");
+    if (used >= (size_t(1) << 32)) return fail(w + ": too many rows");
     h->live = h->count;
     h->pool_used = used;
     const size_t pool = std::max(used, IVF_MIN_POOL);
@@ -242,6 +245,36 @@ int svsb200_dynamic_ivf_create(const void* vectors, int dtype, size_t n, size_t 
     return 0;
 }
 
+extern "C" {
+
+int svsb200_dynamic_ivf_create(const void* vectors, int dtype, size_t n, size_t dim, int metric, const float* centroids,
+                               size_t num_centroids, const uint32_t* assignments, const uint64_t* external_ids, int device,
+                               svsb200_dynamic_ivf** out) {
+    if (!out) return fail("svsb200_dynamic_ivf_create: NULL output");
+    *out = nullptr;
+    if (n && (!vectors || !external_ids)) return fail("svsb200_dynamic_ivf_create: NULL input");
+    if (dtype != SVSB200_F32 && dtype != SVSB200_F16)
+        return fail("svsb200_dynamic_ivf_create: rows must be float32 or float16 (integer, SQ and LVQ rows are not supported)");
+    return dynamic_ivf_assemble("svsb200_dynamic_ivf_create", vectors, dtype, SVSB200_PLAIN, 0.0f, 0.0f, n, dim, metric,
+                                centroids, num_centroids, assignments, external_ids, device, out);
+}
+
+int svsb200_dynamic_ivf_create_sq(const void* codes, int code_type, size_t n, size_t dim, int metric, float scale, float bias,
+                                  const float* centroids, size_t num_centroids, const uint32_t* assignments,
+                                  const uint64_t* external_ids, int device, svsb200_dynamic_ivf** out) {
+    const char* who = "svsb200_dynamic_ivf_create_sq";
+    if (!out) return fail("svsb200_dynamic_ivf_create_sq: NULL output");
+    *out = nullptr;
+    if (n && (!codes || !external_ids)) return fail("svsb200_dynamic_ivf_create_sq: NULL input");
+    if (code_type != SVSB200_I8 && code_type != SVSB200_U8)
+        return fail("svsb200_dynamic_ivf_create_sq: SQ codes must be int8 or uint8");
+    if (int rc = sq_check_params(who, scale, bias)) return rc;
+    if (n && !assignments)
+        return fail("svsb200_dynamic_ivf_create_sq: SQ rows need assignments (there is no float row to rank)");
+    return dynamic_ivf_assemble(who, codes, code_type, SVSB200_SQ, scale, bias, n, dim, metric, centroids, num_centroids,
+                                assignments, external_ids, device, out);
+}
+
 int svsb200_dynamic_ivf_destroy(svsb200_dynamic_ivf* index) {
     if (index) cudaSetDevice(index->iv.ix->reps[0]->device);
     delete index;
@@ -274,7 +307,16 @@ int svsb200_dynamic_ivf_add(svsb200_dynamic_ivf* index, const void* vectors, int
     if (!vectors || !ids) return fail("svsb200_dynamic_ivf_add: NULL argument");
     svsb200_dynamic_ivf* h = index;
     svsb200_index* ix = h->iv.ix.get();
-    if (dtype != ix->dtype) return fail("svsb200_dynamic_ivf_add: the points' dtype differs from the index's");
+    // an SQ index takes float32 rows and encodes them with its fixed scale and bias (SQDataset::set_datum)
+    const bool sq = ix->storage == SVSB200_SQ;
+    if (sq) {
+        if (dtype != SVSB200_F32) return fail("svsb200_dynamic_ivf_add: an SQ index takes float32 points");
+        const float* x = static_cast<const float*>(vectors);
+        for (size_t i = 0; i < count * ix->dim; ++i)
+            if (!std::isfinite(x[i])) return fail("svsb200_dynamic_ivf_add: the points hold a NaN or an infinity");
+    } else if (dtype != ix->dtype) {
+        return fail("svsb200_dynamic_ivf_add: the points' dtype differs from the index's");
+    }
     if (int rc = check_ids_new(who, ix, ids, count)) return rc;
     // slots (add_points, dynamic_ivf.h:474-527): Empty ones from slot 0 with reuse_empty, then appended
     std::vector<uint32_t> slots;
@@ -285,7 +327,7 @@ int svsb200_dynamic_ivf_add(svsb200_dynamic_ivf* index, const void* vectors, int
     const size_t old_n = ix->status.size(), new_n = old_n + (count - slots.size());
     if (new_n >= (size_t(1) << 31)) return fail("svsb200_dynamic_ivf_add: more than 2^31-1 slots");
     for (size_t s = old_n; s < new_n; ++s) slots.push_back(uint32_t(s));
-    const size_t C = h->iv.C, stride = ix->row_stride, row_bytes = ix->dim * esize(dtype);
+    const size_t C = h->iv.C, stride = ix->row_stride, in_bytes = ix->dim * esize(dtype), row_bytes = ix->dim * esize(ix->dtype);
     // the new layout, made inside the mutation and taken over once every device step has succeeded
     std::vector<uint32_t> assign(count), index_in(count), start = h->start, cnt = h->count, cap = h->cap;
     std::vector<uint32_t> reloc_src, reloc_dst, reloc_val;
@@ -295,10 +337,10 @@ int svsb200_dynamic_ivf_add(svsb200_dynamic_ivf* index, const void* vectors, int
         // regions the old starts do not reach, until the new starts and counts are uploaded.
         if (int rc2 = reserve_slots(rep, old_n, new_n, stream)) return rc2;
         // 1. the nearest centroid of every row, as a probe ranks them
-        CUDA_TRY(h->dense.ensure(count * row_bytes));
+        CUDA_TRY(h->dense.ensure(count * in_bytes));
         CUDA_TRY(h->assign.ensure(count));
-        CUDA_TRY(cudaMemcpyAsync(h->dense.ptr, vectors, count * row_bytes, cudaMemcpyHostToDevice, stream));
-        if (int rc2 = ivf_assign(h->iv.cent.get(), reinterpret_cast<const char*>(h->dense.ptr), dtype, count, row_bytes,
+        CUDA_TRY(cudaMemcpyAsync(h->dense.ptr, vectors, count * in_bytes, cudaMemcpyHostToDevice, stream));
+        if (int rc2 = ivf_assign(h->iv.cent.get(), reinterpret_cast<const char*>(h->dense.ptr), dtype, count, in_bytes,
                                  65536, h->assign.ptr, stream))
             return rc2;
         CUDA_TRY(cudaMemcpy(assign.data(), h->assign.ptr, count * 4, cudaMemcpyDeviceToHost));
@@ -327,13 +369,23 @@ int svsb200_dynamic_ivf_add(svsb200_dynamic_ivf* index, const void* vectors, int
                            h->iv.d_row_ids.ptr, reloc_src.size(), uint32_t(stride), stream));
             CUDA_TRY(cudaStreamSynchronize(stream));   // (before the staging buffers are refilled)
         }
-        // 4. the rows and their slots into place
+        // 4. the rows (SQ: their codes) and their slots into place
         const void* src = h->dense.ptr;
+        const void* from = vectors;   // the dense rows as stored, `row_bytes` apart
+        cudaMemcpyKind kind = cudaMemcpyHostToDevice;
+        if (sq) {
+            const size_t values = count * ix->dim;
+            const unsigned grid = unsigned(std::min<size_t>((values + 255) / 256, size_t(rep->sm_count) * 8));
+            CUDA_TRY(h->codes.ensure(values));
+            CUDA_TRY(sq_encode(reinterpret_cast<const float*>(h->dense.ptr), values, ix->dtype, ix->scale, ix->bias,
+                               h->codes.ptr, grid, stream));
+            src = from = h->codes.ptr;
+            kind = cudaMemcpyDeviceToDevice;
+        }
         if (row_bytes != stride) {   // (the row padding stays zero)
             CUDA_TRY(h->rows.ensure(count * stride));
             CUDA_TRY(cudaMemsetAsync(h->rows.ptr, 0, count * stride, stream));
-            CUDA_TRY(cudaMemcpy2DAsync(h->rows.ptr, stride, vectors, row_bytes, row_bytes, count, cudaMemcpyHostToDevice,
-                                       stream));
+            CUDA_TRY(cudaMemcpy2DAsync(h->rows.ptr, stride, from, row_bytes, row_bytes, count, kind, stream));
             src = h->rows.ptr;
         }
         std::vector<uint32_t> dst(count);

@@ -147,7 +147,6 @@ int ivf_search_on_device(svsb200_ivf* iv, Scratch* sc, const void* d_queries, in
     // SQ rows: MIP and cosine run ivf_scan_kernel on the decompressed float tree, L2 the tensor-core leaf
     const bool sq = ix->storage == SVSB200_SQ;
     const bool sq_l2 = sq && ix->metric == SVSB200_L2;
-    if (sq && d_ext_ids) return fail("svsb200_ivf_search: SQ rows in a dynamic IVF index are not supported");
     // ring tiles: 32 rows, fewer for rows so wide that two tiles would pass 96 KB
     uint32_t tile_rows = IVF_TILE_ROWS;
     while (tile_rows > 1 && 2 * size_t(tile_rows) * ix->row_stride > (size_t(96) << 10)) tile_rows >>= 1;
@@ -232,13 +231,16 @@ int ivf_search_on_device(svsb200_ivf* iv, Scratch* sc, const void* d_queries, in
         ip.work_counter = sc->d_counter.ptr;
         CUDA_TRY(cudaMemsetAsync(sc->d_counter.ptr, 0, sizeof(unsigned int), stream));
         const LaunchConfig cfg{-rep->sm_count, IVF_WARPS, smem(Q), stream};
-        if (sq_l2) {   // (the dynamic IVF index holds float rows only: SQ rows never take the DYN form)
+        if (sq_l2) {
             CUDA_TRY(dispatch(IvfSqRows{}, ix->dtype, [&](auto row) {
-                return launch_kernel(ivf_scan_sq_l2_kernel<decltype(row)::value, false>, cfg, size_t(1) << 20, true, ip);
+                constexpr int R = decltype(row)::value;
+                return d_ext_ids ? launch_kernel(ivf_scan_sq_l2_kernel<R, true>, cfg, size_t(1) << 20, true, ip)
+                                 : launch_kernel(ivf_scan_sq_l2_kernel<R, false>, cfg, size_t(1) << 20, true, ip);
             }));
         } else if (sq) {
             CUDA_TRY(dispatch(IvfSqRows{}, ix->dtype, [&](auto row) {
-                return launch_ivf_scan<decltype(row)::value, false, IvfSqOps>(op, ip, cfg);
+                return d_ext_ids ? launch_ivf_scan<decltype(row)::value, true, IvfSqOps>(op, ip, cfg)
+                                 : launch_ivf_scan<decltype(row)::value, false, IvfSqOps>(op, ip, cfg);
             }));
         } else {
             CUDA_TRY(dispatch(IvfRows{}, ix->dtype, [&](auto row) {
@@ -308,10 +310,14 @@ static int ivf_check_rows(const char* who, const void* vectors, int dtype, size_
     return 0;
 }
 
-static int sq_check_params(const char* who, float scale, float bias) {
-    if (!(scale > 0.0f) || !std::isfinite(scale) || !std::isfinite(bias))
-        return fail(std::string(who) + ": the SQ scale must be finite and positive and the bias finite");
-    return 0;
+cudaError_t sq_encode(const float* d_x, size_t count, int code_type, float scale, float bias, uint8_t* d_codes, unsigned grid,
+                      cudaStream_t stream) {
+    if (code_type == SVSB200_I8)
+        sq_encode_kernel<SVSB200_I8><<<grid, 256, 0, stream>>>(d_x, count, scale, bias, d_codes);
+    else
+        sq_encode_kernel<SVSB200_U8><<<grid, 256, 0, stream>>>(d_x, count, scale, bias, d_codes);
+    count_launch();
+    return cudaGetLastError();
 }
 
 // IVFIndex::assemble_from_clustering over checked rows (SQ codes when `storage` is SVSB200_SQ): the cluster-major layout,
@@ -575,12 +581,7 @@ int svsb200_sq_compress(const float* data, size_t n, size_t dim, int code_type, 
     for (size_t lo = 0; lo < count; lo += piece) {
         const size_t m = std::min(piece, count - lo);
         CUDA_TRY(cudaMemcpyAsync(d_x.ptr, data + lo, m * 4, cudaMemcpyHostToDevice, own.s));
-        if (code_type == SVSB200_I8)
-            sq_encode_kernel<SVSB200_I8><<<grid, 256, 0, own.s>>>(d_x.ptr, m, scale, bias, d_codes.ptr);
-        else
-            sq_encode_kernel<SVSB200_U8><<<grid, 256, 0, own.s>>>(d_x.ptr, m, scale, bias, d_codes.ptr);
-        count_launch();
-        CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(sq_encode(d_x.ptr, m, code_type, scale, bias, d_codes.ptr, grid, own.s));
         CUDA_TRY(cudaMemcpyAsync(static_cast<uint8_t*>(out_codes) + lo, d_codes.ptr, m, cudaMemcpyDeviceToHost, own.s));
         CUDA_TRY(cudaStreamSynchronize(own.s));   // (d_x and d_codes are reused)
     }

@@ -3,6 +3,8 @@
 
 #include "host.cuh"
 
+#include <cmath>
+
 namespace svsb200 {
 
 // An own stream for the blocking entry points, destroyed on scope exit.
@@ -52,5 +54,16 @@ int ivf_search_on_device(svsb200_ivf* iv, Scratch* sc, const void* d_queries, in
 // The blocking form over HOST buffers.
 int ivf_search_host(svsb200_ivf* iv, const void* queries, int qdtype, size_t nq, size_t k, size_t P, uint64_t* out_ids,
                     float* out_dists, const uint64_t* d_ext_ids);
+
+// An SQ index's scale and bias: the scale finite and positive, the bias finite.
+inline int sq_check_params(const char* who, float scale, float bias) {
+    if (!(scale > 0.0f) || !std::isfinite(scale) || !std::isfinite(bias))
+        return fail(std::string(who) + ": the SQ scale must be finite and positive and the bias finite");
+    return 0;
+}
+// `count` float32 values (DEVICE) -> int8 / uint8 codes (`code_type`, DEVICE) with a fixed scale and bias, as
+// SQDataset::set_datum encodes (detail::compress); enqueued on `stream` over `grid` blocks.
+cudaError_t sq_encode(const float* d_x, size_t count, int code_type, float scale, float bias, uint8_t* d_codes, unsigned grid,
+                      cudaStream_t stream);
 
 }  // namespace svsb200

@@ -8,6 +8,13 @@ include/svs/index/ivf/dynamic_ivf.h):
     index.search_parameters = IVFSearchParameters(n_probes=16)
     I, D = index.search(queries, 10)                   # external ids (uint64), float32 distances
 
+Scalar-quantised rows (the reference's ``StorageKind::SQI8`` and its uint8 twin) take four times less device memory.
+The index keeps the scale and bias it was assembled with; later adds take float32 rows and encode them with those:
+
+    codes, scale, bias = sq_compress(data)             # int8 codes, one global scale and bias
+    index = DynamicIVF.assemble_from_clustering(clustering, codes, ids, DistanceType.L2, sq=(scale, bias))
+    index.add(points, new_ids)                         # float32 rows, encoded on the device (values past the range clamp)
+
 Backed by ``svsb200_dynamic_ivf_*`` of ``libsvsb200.so``: the IVF index's exact cluster-probed search over the Valid rows,
 ties by slot.  The centroids never move after assembly.  Mutations must not run concurrently with searches of the same
 index.
@@ -19,26 +26,31 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from .ivf import Clustering, IVFSearchParameters
+from .ivf import Clustering, IVFSearchParameters, _sq_codes
 from .vamana import _DTYPE_CODE, DistanceType
 
 
 class DynamicIVF:
-    """``svs.DynamicIVF`` on one CUDA device: float32 / float16 rows, L2 / MIP / cosine."""
+    """``svs.DynamicIVF`` on one CUDA device: float32 / float16 rows or int8 / uint8 SQ codes, L2 / MIP / cosine."""
 
     @classmethod
     def assemble_from_clustering(cls, clustering: Clustering, data, ids, distance: DistanceType = DistanceType.L2,
-                                 num_threads: int = 1, intra_query_threads: int = 1, device: int = 0) -> "DynamicIVF":
+                                 num_threads: int = 1, intra_query_threads: int = 1, device: int = 0,
+                                 sq: tuple | None = None) -> "DynamicIVF":
         """``svs.DynamicIVF.assemble_from_clustering``: one external id per row of ``data``, the rows grouped as the
         clustering says (a clustering without assignments puts every row in its nearest cluster).  An empty ``data``
-        ([0, dim]) makes an empty index to be filled with :meth:`add`.  The thread counts are kept for interface
-        parity only."""
-        x = data.load() if hasattr(data, "load") else data
-        x = np.ascontiguousarray(x)
-        if x.ndim != 2:
-            raise ValueError("data must be a 2-D array")
-        if x.dtype not in _DTYPE_CODE:
-            raise TypeError(f"unsupported data type {x.dtype}")
+        ([0, dim]) makes an empty index to be filled with :meth:`add`.  ``sq=(scale, bias)`` marks ``data`` as int8 /
+        uint8 SQ codes (see :func:`sq_compress`); the clustering must then carry assignments unless ``data`` is empty.
+        The thread counts are kept for interface parity only."""
+        if sq is None:
+            x = data.load() if hasattr(data, "load") else data
+            x = np.ascontiguousarray(x)
+            if x.ndim != 2:
+                raise ValueError("data must be a 2-D array")
+            if x.dtype not in _DTYPE_CODE:
+                raise TypeError(f"unsupported data type {x.dtype}")
+        else:
+            x = _sq_codes(data, sq)
         ids = np.ascontiguousarray(np.atleast_1d(ids), dtype=np.uint64)
         if ids.shape != (x.shape[0],):
             raise ValueError("Expected IDs to be the same length as the number of rows in points!")
@@ -55,9 +67,15 @@ class DynamicIVF:
         self.num_threads, self.intra_query_threads = int(num_threads), int(intra_query_threads)
         self.search_parameters = IVFSearchParameters()
         handle = C.c_void_p()
-        _lib.check(self._lib.svsb200_dynamic_ivf_create(
-            x.ctypes.data, _DTYPE_CODE[x.dtype], x.shape[0], x.shape[1], int(self._distance), cent.ctypes.data,
-            cent.shape[0], None if a is None else a.ctypes.data, ids.ctypes.data, int(device), C.byref(handle)))
+        a_ptr = None if a is None else a.ctypes.data
+        if sq is not None:
+            _lib.check(self._lib.svsb200_dynamic_ivf_create_sq(
+                x.ctypes.data, _DTYPE_CODE[x.dtype], x.shape[0], x.shape[1], int(self._distance), float(sq[0]),
+                float(sq[1]), cent.ctypes.data, cent.shape[0], a_ptr, ids.ctypes.data, int(device), C.byref(handle)))
+        else:
+            _lib.check(self._lib.svsb200_dynamic_ivf_create(
+                x.ctypes.data, _DTYPE_CODE[x.dtype], x.shape[0], x.shape[1], int(self._distance), cent.ctypes.data,
+                cent.shape[0], a_ptr, ids.ctypes.data, int(device), C.byref(handle)))
         self._h = handle
         return self
 
@@ -106,8 +124,9 @@ class DynamicIVF:
     def add(self, points, ids, reuse_empty: bool = False) -> np.ndarray:
         """``add_points``: rows with new external ids, each appended to its nearest centroid's cluster.  Without
         ``reuse_empty`` every row takes a new slot at the end; with it, Empty slots from slot 0 come first.  Rows of the
-        index's dtype; float32 rows given to a float16 index are rounded to nearest even.  Fails without changing
-        anything on a repeated, present or reserved id.  Returns the slots used."""
+        index's dtype; float32 rows given to a float16 index are rounded to nearest even.  An SQ index takes float32
+        rows (finite) and encodes them with its scale and bias.  Fails without changing anything on a repeated, present
+        or reserved id.  Returns the slots used."""
         pts = np.ascontiguousarray(points)
         if pts.dtype == np.float32 and self._dtype == np.float16:
             pts = pts.astype(np.float16)
