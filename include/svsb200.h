@@ -185,9 +185,16 @@ int svsb200_get_option(svsb200_index* index, const char* name, long* value);
  * Here the membership test runs on the device: the caller hands the filter over as a bitmap of n bits
  * (bit i = id i may be returned), every query searches with a result list that grows (x4) until k members were
  * found or the search is exhausted, and the first k members in result order are returned -- distances are the graph
- * search's.  Short rows are padded with id = all-ones, distance = +inf (the reference's `Unspecify`).
- *   svsb200_range_search returns, per query, the results closer than `radius` (further than, for MIP):
- *   counts[nq] and two malloc'ed arrays holding the concatenated ids / distances (release with svsb200_free). */
+ * search's.  Short rows are padded with id = all-ones, distance = +inf for every metric (the reference's
+ * `Unspecify`; the plain search pads MIP / cosine rows with -inf instead).
+ *   The whole batch shares one list length: it starts at max(k, window), is at most n, and stops growing at 16384 or
+ *   once no query is short of k members with its search not exhausted; every query's row is taken from the last list.
+ *   svsb200_range_search returns, per query, the results closer than `radius` (further than, for MIP / cosine; the
+ *   comparison is strict, so a NaN radius returns nothing): counts[nq] and two malloc'ed arrays holding the
+ *   concatenated ids / distances (release with svsb200_free).  Its list starts at max(window, 16) and grows the same
+ *   way while some query's whole list is inside the radius.
+ *   On a shard (svsb200_set_id_offset) the bitmap is over the shard's own rows, bit i = row i, and both calls return
+ *   ids with the offset added, as the plain search does. */
 int svsb200_search_filtered(
     svsb200_index* index, const void* queries, int qdtype, size_t nq, size_t k, size_t window,
     const uint32_t* id_bitmap, uint64_t* out_ids, float* out_dists, uint32_t* out_found);

@@ -196,10 +196,12 @@ __global__ void merge_topk_kernel(const uint64_t* __restrict__ ids, const float*
 }
 
 // Filtered search (bindings/cpp/src/vamana_index_impl.h:139-218): out of a query's `kk` search results (sorted), keep
-// the first k whose id is a member of the filter bitmap; `found[q]` = how many there were.
+// the first k whose id is a member of the filter bitmap; `found[q]` = how many there were.  The bitmap is over the
+// index's own rows: on a shard the listed ids carry `id_offset`, which is taken off for the membership test only.
 __global__ void filter_topk_kernel(const uint64_t* __restrict__ ids, const float* __restrict__ dists, uint32_t nq, uint32_t kk,
-                                   uint32_t k, const uint32_t* __restrict__ bitmap, uint64_t* __restrict__ out_ids,
-                                   float* __restrict__ out_dists, uint32_t* __restrict__ found, uint32_t* __restrict__ unfinished) {
+                                   uint32_t k, const uint32_t* __restrict__ bitmap, uint64_t id_offset,
+                                   uint64_t* __restrict__ out_ids, float* __restrict__ out_dists, uint32_t* __restrict__ found,
+                                   uint32_t* __restrict__ unfinished) {
     const uint32_t q = blockIdx.x * (blockDim.x / 32) + threadIdx.x / 32;
     const uint32_t lane = threadIdx.x & 31;
     if (q >= nq) return;
@@ -209,7 +211,8 @@ __global__ void filter_topk_kernel(const uint64_t* __restrict__ ids, const float
         const uint32_t j = j0 + lane;
         const uint64_t id = j < kk ? ids[size_t(q) * kk + j] : ~uint64_t(0);
         const bool valid = id != ~uint64_t(0);
-        const bool pass = valid && ((bitmap[id >> 5] >> (id & 31)) & 1u);
+        const uint64_t row = id - id_offset;
+        const bool pass = valid && ((bitmap[row >> 5] >> (row & 31)) & 1u);
         const unsigned m = __ballot_sync(0xFFFFFFFFu, pass);
         const uint32_t o = cnt + __popc(m & ((1u << lane) - 1u));
         if (pass && o < k) {
@@ -679,7 +682,7 @@ static int search_filtered(svsb200_index* ix, Replica* rep, Scratch* sc, const v
     int rc = grow_until_done(ix, rep, sc, qdtype, nq, window, &kk, d_found.ptr + nq, [&](size_t len) {
         filter_topk_kernel<<<unsigned((nq + 3) / 4), 128, 0, sc->stream>>>(
             reinterpret_cast<const uint64_t*>(sc->ids.ptr), sc->dists.ptr, uint32_t(nq), uint32_t(len), uint32_t(k),
-            d_bitmap.ptr, d_oi.ptr, d_od.ptr, d_found.ptr, d_found.ptr + nq);
+            d_bitmap.ptr, ix->id_offset, d_oi.ptr, d_od.ptr, d_found.ptr, d_found.ptr + nq);
     });
     sc->dyn_slot_ids = false;
     if (rc) return rc;

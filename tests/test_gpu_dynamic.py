@@ -131,44 +131,6 @@ def test_deleted_ids_never_returned_and_bookkeeping(dataset):
         index.flat_search(dataset.queries[:2], 10)
 
 
-def test_filtered_search_returns_valid_members_as_external_ids(dataset):
-    from scalablevectorsearch_b200 import SearchBufferConfig
-    rng = np.random.default_rng(5)
-    index, data, ext, valid = make_index(dataset, "l2", np.float32, 0.2, rng, delete_entry=True)
-    n, q, k, w = len(ext), dataset.queries[:64], 10, 40
-    index.search_window_size = w
-    # every slot allowed: Deleted ones are cleared from the set, so this is the plain search on a list of max(k, w)
-    ids, dists, found = index.search_filtered(q, k, np.ones(n, dtype=bool))
-    index.search_parameters.buffer_config = SearchBufferConfig(w, w)
-    want_ids, want_dists = index.search(q, w)
-    assert (found == k).all()
-    assert np.array_equal(ids, want_ids[:, :k]) and np.array_equal(bits(dists), bits(want_dists[:, :k]))
-    # half of the slots allowed: only allowed, valid members come back, in search order
-    allowed = rng.random(n) < 0.5
-    ids, dists, found = index.search_filtered(q, k, allowed)
-    members = set(ext[allowed & valid].tolist())
-    for row, d, f in zip(ids, dists, found):
-        assert all(int(i) in members for i in row[:f]) and (row[f:] == np.uint64(2**64 - 1)).all()
-        assert (np.diff(d[:f]) >= 0).all()
-    assert found.mean() > k - 1
-
-
-def test_range_search_returns_only_valid_external_ids(dataset):
-    rng = np.random.default_rng(6)
-    index, data, ext, valid = make_index(dataset, "l2", np.float32, 0.3, rng)
-    index.search_window_size = 30
-    q = dataset.queries[:32]
-    _, d10 = index.search(q, 10)
-    radius = float(np.median(d10[:, 9]))
-    live = set(ext[valid].tolist())
-    res = index.range_search(q, radius)
-    assert sum(len(ids) for ids, _ in res) > 0
-    for (ids, d), ref_d in zip(res, d10):
-        assert all(int(i) in live for i in ids)
-        assert (d < radius).all() and (np.diff(d) >= 0).all()
-        assert len(ids) >= int((ref_d < radius).sum())
-
-
 def test_cancellation_is_polled_during_a_dynamic_search(dataset):
     rng = np.random.default_rng(8)
     index, data, ext, valid = make_index(dataset, "l2", np.float32, 0.5, rng)

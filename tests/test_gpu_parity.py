@@ -478,42 +478,6 @@ def test_sharded_index_in_one_process_matches_reference_per_shard_plus_merge(dat
     assert np.array_equal(ids.astype(np.int64), want_i) and np.array_equal(bits(dists), bits(want_d))
 
 
-def test_filtered_and_range_search(dataset, oracle):
-    """The runtime ABI's filtered / range searches (vamana_index.h:75-92) with the filter evaluated on the device:
-    checked against the oracle's plain search results post-processed on the host (members in result order; results
-    inside the radius)."""
-    from scalablevectorsearch_b200 import SearchBufferConfig
-    index = make_index(dataset.data, dataset.graph, dataset.entry_point, "l2")
-    index.search_parameters.buffer_config = SearchBufferConfig(64)
-    want = oracle.index(dataset.data, dataset.graph, dataset.entry_point, "l2")
-    q = dataset.queries[:100]
-    rng = np.random.default_rng(0)
-    allowed = rng.random(dataset.data.shape[0]) < 0.3
-    ids, dists, found = index.search_filtered(q, 10, allowed)
-    assert np.all(found == 10)
-    assert np.all(allowed[ids.astype(np.int64)])
-    assert np.all(np.diff(dists, axis=1) >= 0)
-    # the first 10 members of the oracle's result list of the same length (64 first; the whole batch is re-run with a
-    # 256-entry list when any query found fewer than 10 members in it)
-    w64 = want.search(q, 64, 64, 64)
-    w256 = want.search(q, 256, 256, 256)
-    grown = any(int(allowed[w64[0][i].astype(np.int64)].sum()) < 10 for i in range(len(q)))
-    wi, wd = w256 if grown else w64
-    for i in range(len(q)):
-        keep = [j for j in range(wi.shape[1]) if allowed[int(wi[i, j])]][:10]
-        assert np.array_equal(ids[i], wi[i, keep]) and np.array_equal(bits(dists[i]), bits(wd[i, keep])), i
-    wi, wd = w256
-    # nothing allowed -> empty rows, padded
-    ids0, d0, f0 = index.search_filtered(q[:5], 3, np.zeros(dataset.data.shape[0], dtype=bool))
-    assert np.all(f0 == 0) and np.all(ids0 == np.uint64(0xFFFFFFFFFFFFFFFF)) and np.all(np.isposinf(d0))
-    # range search: everything closer than the 20th-nearest distance of query 0
-    radius = float(wd[0, 20])
-    res = index.range_search(q[:8], radius)
-    for i, (ri, rd) in enumerate(res):
-        assert np.all(rd < radius) and np.all(np.diff(rd) >= 0)
-        assert len(ri) >= int(np.sum(wd[i, :50] < radius)) - 1
-
-
 def test_runtime_abi_demo_program(tmp_path):
     """A C++ program written against the reference's runtime header only (svs::runtime::v0::VamanaIndex: build / add /
     search / IDFilter / range_search / get_distance), linked with libsvsb200_runtime.so instead of libsvs_runtime."""
