@@ -534,6 +534,28 @@ int svsb200_ivf_search_device(svsb200_ivf* index, const void* d_queries, int qdt
 /* The same with HOST buffers (blocking). */
 int svsb200_ivf_search(svsb200_ivf* index, const void* queries, int qdtype, size_t nq, size_t k, size_t n_probes,
                        uint64_t* out_ids, float* out_dists);
+/* Filtered search (svs::runtime::v0::IVFIndex::search with an IDFilter): the plain search restricted to the ALLOWED rows,
+ * with the probe count growing per query until k allowed rows are in reach.
+ *   Bitmap: bit i (word i / 32, bit i % 32) set = original id i may be returned; (n + 31) / 32 words.  NULL is refused.
+ *   Growth: the probe order is the plain search's (the flat search over the centroids, ties to the lower centroid).
+ *   P_0 = n_probes, P_{j+1} = min(4 P_j, P_max), P_max = min(C, 1024).  Query q uses the first P_j whose nearest P_j
+ *   clusters hold at least k allowed rows, or P_max when none does.  The choice is per query: a query's row does not
+ *   depend on the other queries of the batch.
+ *   Result: the exact top k over the allowed rows of the query's probed clusters, with the scan's bit-exact distances,
+ *   ordered by distance, then original id.  Short rows are padded with all-ones ids and +inf distances for EVERY metric
+ *   (as svsb200_search_filtered; the plain search pads MIP / cosine with -inf).
+ *   Per-query outputs, uint32 [nq] each, each may be NULL: out_probes the P used, out_allowed the allowed rows in those
+ *   clusters, out_rows all rows in those clusters; min(k, out_allowed) entries of the row are not padding.
+ *   Limits and refusals are the plain search's (1 <= k <= 1024, 1 <= n_probes <= P_max, float32 / float16 queries,
+ *   every row type and storage kind). */
+int svsb200_ivf_search_filtered(svsb200_ivf* index, const void* queries, int qdtype, size_t nq, size_t k, size_t n_probes,
+                                const uint32_t* id_bitmap, uint64_t* out_ids, float* out_dists, uint32_t* out_probes,
+                                uint32_t* out_allowed, uint32_t* out_rows);
+/* The same with the queries, bitmap and every output in DEVICE memory, enqueued on `stream` apart from the
+ * synchronisations of the centroid searches and of each growth decision (which reads the allowed counts back). */
+int svsb200_ivf_search_filtered_device(svsb200_ivf* index, const void* d_queries, int qdtype, size_t nq, size_t k,
+                                       size_t n_probes, const uint32_t* d_id_bitmap, uint64_t* d_out_ids, float* d_out_dists,
+                                       uint32_t* d_out_probes, uint32_t* d_out_allowed, uint32_t* d_out_rows, void* stream);
 
 /* Dynamic IVF index.  Replaces: DynamicIVFIndex (include/svs/index/ivf/dynamic_ivf.h) with svs::DynamicIVF: the IVF
  * index over a mutable set of float32 / float16 rows (or SQ codes, svsb200_dynamic_ivf_create_sq) on one device, L2 /
@@ -612,6 +634,17 @@ int svsb200_dynamic_ivf_search_device(svsb200_dynamic_ivf* index, const void* d_
 /* The same with HOST buffers (blocking). */
 int svsb200_dynamic_ivf_search(svsb200_dynamic_ivf* index, const void* queries, int qdtype, size_t nq, size_t k,
                                size_t n_probes, uint64_t* out_ids, float* out_dists);
+/* Filtered search: svsb200_ivf_search_filtered over the Valid rows, with the bitmap over SLOTS ((num_slots + 31) / 32
+ * words, bit s = slot s may be returned; the bits of Empty slots are ignored), as svsb200_search_filtered does for the
+ * dynamic Vamana index.  Results are ordered by distance, then slot, and returned as EXTERNAL ids; out_rows counts the
+ * Valid rows of the probed clusters.  Like every search, a mutation waits for it, the device form included. */
+int svsb200_dynamic_ivf_search_filtered(svsb200_dynamic_ivf* index, const void* queries, int qdtype, size_t nq, size_t k,
+                                        size_t n_probes, const uint32_t* slot_bitmap, uint64_t* out_ids, float* out_dists,
+                                        uint32_t* out_probes, uint32_t* out_allowed, uint32_t* out_rows);
+int svsb200_dynamic_ivf_search_filtered_device(svsb200_dynamic_ivf* index, const void* d_queries, int qdtype, size_t nq,
+                                               size_t k, size_t n_probes, const uint32_t* d_slot_bitmap, uint64_t* d_out_ids,
+                                               float* d_out_dists, uint32_t* d_out_probes, uint32_t* d_out_allowed,
+                                               uint32_t* d_out_rows, void* stream);
 
 #ifdef __cplusplus
 }

@@ -36,13 +36,14 @@ SYMBOLS = [
     "svsb200_ivf_random", "svsb200_ivf_cluster", "svsb200_ivf_create", "svsb200_ivf_destroy", "svsb200_ivf_size",
     "svsb200_ivf_dimensions", "svsb200_ivf_num_clusters", "svsb200_ivf_device_bytes", "svsb200_ivf_cluster_sizes",
     "svsb200_ivf_centroids", "svsb200_ivf_search", "svsb200_ivf_search_device", "svsb200_sq_compress",
-    "svsb200_ivf_create_sq",
+    "svsb200_ivf_create_sq", "svsb200_ivf_search_filtered", "svsb200_ivf_search_filtered_device",
     "svsb200_dynamic_ivf_create", "svsb200_dynamic_ivf_destroy", "svsb200_dynamic_ivf_size",
     "svsb200_dynamic_ivf_num_slots", "svsb200_dynamic_ivf_dimensions", "svsb200_dynamic_ivf_num_clusters",
     "svsb200_dynamic_ivf_device_bytes", "svsb200_dynamic_ivf_cluster_sizes", "svsb200_dynamic_ivf_centroids",
     "svsb200_dynamic_ivf_add", "svsb200_dynamic_ivf_delete", "svsb200_dynamic_ivf_compact", "svsb200_dynamic_ivf_ids",
     "svsb200_dynamic_ivf_has_id", "svsb200_dynamic_ivf_export", "svsb200_dynamic_ivf_search",
-    "svsb200_dynamic_ivf_search_device", "svsb200_dynamic_ivf_create_sq",
+    "svsb200_dynamic_ivf_search_device", "svsb200_dynamic_ivf_create_sq", "svsb200_dynamic_ivf_search_filtered",
+    "svsb200_dynamic_ivf_search_filtered_device",
 ]
 
 _lib = None
@@ -148,6 +149,8 @@ def lib() -> C.CDLL:
     l.svsb200_ivf_centroids.argtypes = [vp, vp]
     l.svsb200_ivf_search.argtypes = [vp, vp, i32, sz, sz, sz, vp, vp]
     l.svsb200_ivf_search_device.argtypes = [vp, vp, i32, sz, sz, sz, vp, vp, vp]
+    l.svsb200_ivf_search_filtered.argtypes = [vp, vp, i32, sz, sz, sz, vp, vp, vp, vp, vp, vp]
+    l.svsb200_ivf_search_filtered_device.argtypes = [vp, vp, i32, sz, sz, sz, vp, vp, vp, vp, vp, vp, vp]
     l.svsb200_dynamic_ivf_create.argtypes = [vp, i32, sz, sz, i32, vp, sz, vp, vp, i32, C.POINTER(vp)]
     l.svsb200_dynamic_ivf_create_sq.argtypes = [vp, i32, sz, sz, i32, C.c_float, C.c_float, vp, sz, vp, vp, i32,
                                                 C.POINTER(vp)]
@@ -165,6 +168,8 @@ def lib() -> C.CDLL:
     l.svsb200_dynamic_ivf_export.argtypes = [vp, vp, vp, vp]
     l.svsb200_dynamic_ivf_search.argtypes = [vp, vp, i32, sz, sz, sz, vp, vp]
     l.svsb200_dynamic_ivf_search_device.argtypes = [vp, vp, i32, sz, sz, sz, vp, vp, vp]
+    l.svsb200_dynamic_ivf_search_filtered.argtypes = [vp, vp, i32, sz, sz, sz, vp, vp, vp, vp, vp, vp]
+    l.svsb200_dynamic_ivf_search_filtered_device.argtypes = [vp, vp, i32, sz, sz, sz, vp, vp, vp, vp, vp, vp, vp]
     _lib = l
     return l
 

@@ -22,9 +22,11 @@
 // `search` probes n_probes clusters (the build's default search parameters, overridden per call).  SQI8 follows the
 // reference's init_impl: the float32 rows are clustered, then compressed to int8 (svsb200_sq_compress), then assembled
 // with the clustering's assignments (svsb200_ivf_create_sq); data that cannot be compressed (constant, or holding a
-// NaN or an infinity) is a RUNTIME_ERROR.  A non-null IDFilter, save / load, LeanVec and the other storage kinds are
-// NOT_IMPLEMENTED; is_hierarchical must be false (the GPU k-means is flat), and unspecified build parameters take the
-// Python IVFBuildParameters' defaults.
+// NaN or an infinity) is a RUNTIME_ERROR.  save / load, LeanVec and the other storage kinds are NOT_IMPLEMENTED;
+// is_hierarchical must be false (the GPU k-means is flat), and unspecified build parameters take the Python
+// IVFBuildParameters' defaults.  A non-null IDFilter becomes a bitmap over the ids (is_member(i) for every id) for
+// svsb200_ivf_search_filtered, whose probe count grows per query until k allowed rows are in reach; filter_stop and
+// filter_estimate_batch are honoured as described at filtered_search below.
 //
 // And `svs::runtime::v0::DynamicIVFIndex` (bindings/cpp/include/svs/runtime/dynamic_ivf_index.h) on the dynamic IVF
 // index (svsb200_dynamic_ivf_*) for FP32, FP16 and SQI8 storage, with the behaviour of the reference's
@@ -33,8 +35,9 @@
 // `add`, which clusters its own rows (and fixes the SQ scale and bias from them); a later SQI8 `add` passes its float32
 // rows through, to be encoded with that scale and bias; before initialisation, `search`
 // is NOT_INITIALIZED (labels -1, distances +inf), `remove` / `remove_selected` / `consolidate` / `compact` are
-// NOT_INITIALIZED and `has_id` is false.  k = 0 is INVALID_ARGUMENT; a non-null IDFilter, save / load and LeanVec are
-// NOT_IMPLEMENTED.
+// NOT_INITIALIZED and `has_id` is false.  k = 0 is INVALID_ARGUMENT; save / load and LeanVec are NOT_IMPLEMENTED.  A
+// non-null IDFilter becomes a bitmap over the slots (is_member(external id) for every Valid slot) for
+// svsb200_dynamic_ivf_search_filtered, with IVFIndex's filter_stop and filter_estimate_batch.
 #include "svs/runtime/dynamic_ivf_index.h"
 #include "svs/runtime/flat_index.h"
 #include "svs/runtime/ivf_index.h"
@@ -46,6 +49,7 @@
 #include <cstring>
 #include <memory>
 #include <new>
+#include <random>
 #include <vector>
 
 namespace svs {
@@ -408,6 +412,64 @@ Status FlatIndex::map_to_memory(FlatIndex** index, void*, size_t, MetricType, si
 // ---- IVFIndex ----
 namespace {
 
+// Filtered IVF search.  As the reference's IVF runtime classes do (ivf_index_impl.h, dynamic_ivf_index_impl.h), two
+// search parameters let a caller give up on a filter that lets too little through, so that it can fall back to an
+// exact search: filter_stop (unspecified: 0, never give up) and filter_estimate_batch (unspecified: true).
+//   * Estimate: with filter_estimate_batch, max(200, int(1 / filter_stop)) ids (at most the index's size) are drawn
+//     uniformly from [0, size) with std::mt19937(42), at most four times as many draws, skipping ids the index does not
+//     hold (dynamic index); when none of them or a fraction below filter_stop passes the filter, every row is padded.
+//   * Per query: a query whose probed clusters hold allowed / rows < filter_stop (no allowed row included) gets a padded
+//     row.  The reference divides by the candidates its iterator has yielded so far instead: a documented divergence.
+// Padded rows are labels SIZE_MAX, distances +inf, and the status stays OK.
+struct FilterStop {
+    float stop = 0.0f;
+    bool estimate = true;
+};
+
+FilterStop filter_stop_of(const IVFIndex::SearchParams& sp, const IVFIndex::SearchParams* params) {
+    FilterStop fs;
+    if (is_specified(sp.filter_stop)) fs.stop = sp.filter_stop;
+    if (is_specified(sp.filter_estimate_batch)) fs.estimate = sp.filter_estimate_batch.is_enabled();
+    if (params && is_specified(params->filter_stop)) fs.stop = params->filter_stop;
+    if (params && is_specified(params->filter_estimate_batch)) fs.estimate = params->filter_estimate_batch.is_enabled();
+    return fs;
+}
+
+// The estimate: true when the sampled ids say give up.  `held(id)` skips ids the index does not hold.
+template <typename Held> bool sample_says_stop(const IDFilter& filter, size_t size, float stop, Held held) {
+    if (!(stop > 0.0f) || size == 0) return false;
+    const size_t want = std::min(std::max<size_t>(200, size_t(1.0f / stop)), size);
+    std::mt19937 rng(42);
+    std::uniform_int_distribution<size_t> draw(0, size - 1);
+    size_t checked = 0, hits = 0;
+    for (size_t tries = 0; checked < want && tries < 4 * want; ++tries) {
+        const size_t id = draw(rng);
+        if (!held(id)) continue;
+        ++checked;
+        if (filter.is_member(id)) ++hits;
+    }
+    return checked > 0 && (hits == 0 || float(hits) / float(checked) < stop);
+}
+
+void pad_rows(size_t from, size_t to, size_t k, float* distances, size_t* labels) {
+    for (size_t i = from * k; i < to * k; ++i) {
+        labels[i] = SIZE_MAX;
+        distances[i] = INFINITY;
+    }
+}
+
+// Runs `search(probes, allowed, rows)` (a filtered search writing labels and distances) and pads the rows of the
+// queries below filter_stop.
+template <typename Search>
+Status filtered_search(size_t n, size_t k, float* distances, size_t* labels, float stop, Search search) {
+    std::vector<uint32_t> probes(n), allowed(n), rows(n);
+    if (search(probes.data(), allowed.data(), rows.data())) return gpu_error();
+    if (stop > 0.0f)
+        for (size_t q = 0; q < n; ++q)
+            if (allowed[q] == 0 || float(allowed[q]) / float(rows[q]) < stop) pad_rows(q, q + 1, k, distances, labels);
+    return Status_Ok;
+}
+
 class GpuIVFIndex final : public IVFIndex {
   public:
     GpuIVFIndex(svsb200_ivf* index, const SearchParams& sp, size_t threads, size_t intra)
@@ -416,7 +478,6 @@ class GpuIVFIndex final : public IVFIndex {
 
     Status search(size_t n, const float* x, size_t k, float* distances, size_t* labels, const SearchParams* params,
                   IDFilter* filter) const noexcept override {
-        if (filter) return Status(ErrorCode::NOT_IMPLEMENTED, "filtered IVF search is not available on the GPU");
         if (k == 0) return Status(ErrorCode::INVALID_ARGUMENT, "k must be greater than 0");
         if (n == 0) return Status_Ok;
         size_t n_probes = is_specified(sp_.n_probes) ? sp_.n_probes : 1;
@@ -425,6 +486,25 @@ class GpuIVFIndex final : public IVFIndex {
         if (params && is_specified(params->k_reorder)) k_reorder = params->k_reorder;
         if (!(k_reorder >= 1.0f)) return Status(ErrorCode::INVALID_ARGUMENT, "k_reorder must be at least 1");
         static_assert(sizeof(size_t) == 8, "labels are 64-bit");
+        if (filter) {
+            const FilterStop fs = filter_stop_of(sp_, params);
+            const size_t size = svsb200_ivf_size(index_);
+            if (fs.estimate && sample_says_stop(*filter, size, fs.stop, [](size_t) { return true; })) {
+                pad_rows(0, n, k, distances, labels);
+                return Status_Ok;
+            }
+            try {
+                std::vector<uint32_t> bitmap((size + 31) / 32, 0u);   // bit i: id i
+                for (size_t i = 0; i < size; ++i)
+                    if (filter->is_member(i)) bitmap[i >> 5] |= 1u << (i & 31);
+                return filtered_search(n, k, distances, labels, fs.stop, [&](uint32_t* p, uint32_t* a, uint32_t* r) {
+                    return svsb200_ivf_search_filtered(index_, x, SVSB200_F32, n, k, n_probes, bitmap.data(),
+                                                       reinterpret_cast<uint64_t*>(labels), distances, p, a, r);
+                });
+            } catch (...) {
+                return Status(ErrorCode::RUNTIME_ERROR, "out of memory");
+            }
+        }
         if (svsb200_ivf_search(index_, x, SVSB200_F32, n, k, n_probes, reinterpret_cast<uint64_t*>(labels), distances))
             return gpu_error();
         return Status_Ok;
@@ -687,7 +767,6 @@ class GpuDynamicIVFIndex final : public DynamicIVFIndex {
             }
             return not_initialized();
         }
-        if (filter) return Status(ErrorCode::NOT_IMPLEMENTED, "filtered IVF search is not available on the GPU");
         if (k == 0) return Status(ErrorCode::INVALID_ARGUMENT, "k must be greater than 0");
         if (n == 0) return Status_Ok;
         size_t n_probes = is_specified(sp_.n_probes) ? sp_.n_probes : 1;
@@ -695,6 +774,32 @@ class GpuDynamicIVFIndex final : public DynamicIVFIndex {
         if (params && is_specified(params->n_probes)) n_probes = params->n_probes;
         if (params && is_specified(params->k_reorder)) k_reorder = params->k_reorder;
         if (!(k_reorder >= 1.0f)) return Status(ErrorCode::INVALID_ARGUMENT, "k_reorder must be at least 1");
+        if (filter) {
+            const FilterStop fs = filter_stop_of(sp_, params);
+            auto held = [this](size_t id) {
+                int out = 0;
+                return svsb200_dynamic_ivf_has_id(index_, id, &out) == 0 && out != 0;
+            };
+            if (fs.estimate && sample_says_stop(*filter, svsb200_dynamic_ivf_size(index_), fs.stop, held)) {
+                pad_rows(0, n, k, distances, labels);
+                return Status_Ok;
+            }
+            try {
+                const size_t slots = svsb200_dynamic_ivf_num_slots(index_);
+                std::vector<uint8_t> status(slots);
+                std::vector<uint64_t> ext(slots);
+                if (svsb200_dynamic_ivf_export(index_, status.data(), ext.data(), nullptr)) return gpu_error();
+                std::vector<uint32_t> bitmap((slots + 31) / 32, 0u);   // bit s: slot s
+                for (size_t s = 0; s < slots; ++s)
+                    if (status[s] && filter->is_member(size_t(ext[s]))) bitmap[s >> 5] |= 1u << (s & 31);
+                return filtered_search(n, k, distances, labels, fs.stop, [&](uint32_t* p, uint32_t* a, uint32_t* r) {
+                    return svsb200_dynamic_ivf_search_filtered(index_, x, SVSB200_F32, n, k, n_probes, bitmap.data(),
+                                                               reinterpret_cast<uint64_t*>(labels), distances, p, a, r);
+                });
+            } catch (...) {
+                return Status(ErrorCode::RUNTIME_ERROR, "out of memory");
+            }
+        }
         if (svsb200_dynamic_ivf_search(index_, x, SVSB200_F32, n, k, n_probes, reinterpret_cast<uint64_t*>(labels),
                                        distances))
             return gpu_error();

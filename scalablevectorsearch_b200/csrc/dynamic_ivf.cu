@@ -601,4 +601,34 @@ int svsb200_dynamic_ivf_search(svsb200_dynamic_ivf* index, const void* queries, 
                            index->iv.ix->reps[0]->d_ext_ids.ptr);
 }
 
+int svsb200_dynamic_ivf_search_filtered_device(svsb200_dynamic_ivf* index, const void* d_queries, int qdtype, size_t nq,
+                                               size_t k, size_t n_probes, const uint32_t* d_slot_bitmap, uint64_t* d_out_ids,
+                                               float* d_out_dists, uint32_t* d_out_probes, uint32_t* d_out_allowed,
+                                               uint32_t* d_out_rows, void* stream_) {
+    const char* who = "svsb200_dynamic_ivf_search_filtered_device";
+    if (int rc = ivf_check_search(who, ivf_of(index), qdtype, k, n_probes)) return rc;
+    if (!d_slot_bitmap) return fail("svsb200_dynamic_ivf_search_filtered_device: NULL bitmap");
+    if (nq == 0) return 0;
+    if (!d_queries || !d_out_ids || !d_out_dists) return fail("svsb200_dynamic_ivf_search_filtered_device: NULL buffer");
+    Replica* rep = index->iv.ix->reps[0].get();
+    CUDA_TRY(cudaSetDevice(rep->device));
+    std::string err;
+    Scratch* sc = scratch_for_stream(rep, static_cast<cudaStream_t>(stream_), &err);
+    if (!sc) return fail(err);
+    return ivf_search_filtered_on_device(&index->iv, sc, d_queries, qdtype, nq, k, n_probes, d_slot_bitmap, d_out_ids,
+                                         d_out_dists, d_out_probes, d_out_allowed, d_out_rows, rep->d_ext_ids.ptr);
+}
+
+int svsb200_dynamic_ivf_search_filtered(svsb200_dynamic_ivf* index, const void* queries, int qdtype, size_t nq, size_t k,
+                                        size_t n_probes, const uint32_t* slot_bitmap, uint64_t* out_ids, float* out_dists,
+                                        uint32_t* out_probes, uint32_t* out_allowed, uint32_t* out_rows) {
+    if (int rc = ivf_check_search("svsb200_dynamic_ivf_search_filtered", ivf_of(index), qdtype, k, n_probes)) return rc;
+    if (!slot_bitmap) return fail("svsb200_dynamic_ivf_search_filtered: NULL bitmap");
+    if (nq == 0) return 0;
+    if (!queries || !out_ids || !out_dists) return fail("svsb200_dynamic_ivf_search_filtered: NULL buffer");
+    return ivf_search_filtered_host(&index->iv, queries, qdtype, nq, k, n_probes, slot_bitmap,
+                                    (index->iv.ix->status.size() + 31) / 32, out_ids, out_dists, out_probes, out_allowed,
+                                    out_rows, index->iv.ix->reps[0]->d_ext_ids.ptr);
+}
+
 }  // extern "C"

@@ -131,18 +131,19 @@ static size_t ivf_chunk(size_t P, size_t k) {
     return std::max<size_t>(1, std::min(IVF_MAX_CHUNK, IVF_LIST_BUDGET / (P * k * 12)));
 }
 
+static IvfScratch* ivf_scratch(svsb200_ivf* iv, Scratch* sc) {
+    std::lock_guard<std::mutex> lock(iv->mu);
+    auto& slot = iv->scratch[sc];
+    if (!slot) slot = std::make_unique<IvfScratch>();
+    return slot.get();
+}
+
 int ivf_search_on_device(svsb200_ivf* iv, Scratch* sc, const void* d_queries, int qdtype, size_t nq, size_t k, size_t P,
-                         uint64_t* d_out_ids, float* d_out_dists, const uint64_t* d_ext_ids) {
+                         uint64_t* d_out_ids, float* d_out_dists, const uint64_t* d_ext_ids, const uint32_t* d_masked_ids) {
     svsb200_index* ix = iv->ix.get();
     Replica* rep = ix->reps[0].get();
     cudaStream_t stream = sc->stream;
-    IvfScratch* is = nullptr;
-    {
-        std::lock_guard<std::mutex> lock(iv->mu);
-        auto& slot = iv->scratch[sc];
-        if (!slot) slot = std::make_unique<IvfScratch>();
-        is = slot.get();
-    }
+    IvfScratch* is = ivf_scratch(iv, sc);
     const uint32_t C = uint32_t(iv->C), dim = uint32_t(ix->dim), qstride = query_stride(dim);
     // SQ rows: MIP and cosine run ivf_scan_kernel on the decompressed float tree, L2 the tensor-core leaf
     const bool sq = ix->storage == SVSB200_SQ;
@@ -176,6 +177,7 @@ int ivf_search_on_device(svsb200_ivf* iv, Scratch* sc, const void* d_queries, in
     CUDA_TRY(is->list.ensure(cmax * P));
     const int op = sq_l2 ? OP_L2I : ix->metric == SVSB200_L2 ? OP_L2F : ix->metric == SVSB200_IP ? OP_IPF : OP_COSF;
     const int prep = !sq ? PREP_FLOAT : sq_l2 ? PREP_SQ_L2 : ix->metric == SVSB200_IP ? PREP_SQ_IP : PREP_SQ_COS;
+    const bool dyn = d_ext_ids || d_masked_ids;   // the scan's DYN form: all-ones ids are not candidates
     for (size_t q0 = 0; q0 < nq; q0 += chunk) {
         const size_t nqc = std::min(chunk, nq - q0);
         const char* qp = static_cast<const char*>(d_queries) + q0 * qrow;
@@ -214,7 +216,7 @@ int ivf_search_on_device(svsb200_ivf* iv, Scratch* sc, const void* d_queries, in
         ip.p.nq = uint32_t(nqc);
         ip.p.k = uint32_t(k);
         ip.rows = reinterpret_cast<const char*>(rep->d_vectors.ptr);
-        ip.row_ids = iv->d_row_ids.ptr;
+        ip.row_ids = d_masked_ids ? d_masked_ids : iv->d_row_ids.ptr;
         ip.cl_start = iv->d_start.ptr;
         ip.cl_count = iv->d_count.ptr;
         ip.list_off = is->list_off.ptr;
@@ -234,17 +236,17 @@ int ivf_search_on_device(svsb200_ivf* iv, Scratch* sc, const void* d_queries, in
         if (sq_l2) {
             CUDA_TRY(dispatch(IvfSqRows{}, ix->dtype, [&](auto row) {
                 constexpr int R = decltype(row)::value;
-                return d_ext_ids ? launch_kernel(ivf_scan_sq_l2_kernel<R, true>, cfg, size_t(1) << 20, true, ip)
+                return dyn ? launch_kernel(ivf_scan_sq_l2_kernel<R, true>, cfg, size_t(1) << 20, true, ip)
                                  : launch_kernel(ivf_scan_sq_l2_kernel<R, false>, cfg, size_t(1) << 20, true, ip);
             }));
         } else if (sq) {
             CUDA_TRY(dispatch(IvfSqRows{}, ix->dtype, [&](auto row) {
-                return d_ext_ids ? launch_ivf_scan<decltype(row)::value, true, IvfSqOps>(op, ip, cfg)
+                return dyn ? launch_ivf_scan<decltype(row)::value, true, IvfSqOps>(op, ip, cfg)
                                  : launch_ivf_scan<decltype(row)::value, false, IvfSqOps>(op, ip, cfg);
             }));
         } else {
             CUDA_TRY(dispatch(IvfRows{}, ix->dtype, [&](auto row) {
-                return d_ext_ids ? launch_ivf_scan<decltype(row)::value, true>(op, ip, cfg)
+                return dyn ? launch_ivf_scan<decltype(row)::value, true>(op, ip, cfg)
                                  : launch_ivf_scan<decltype(row)::value, false>(op, ip, cfg);
             }));
         }
@@ -278,6 +280,143 @@ int ivf_search_host(svsb200_ivf* iv, const void* queries, int qdtype, size_t nq,
             return rc;
         CUDA_TRY(cudaMemcpyAsync(out_ids, sc->ids.ptr, nq * k * 8, cudaMemcpyDeviceToHost, sc->stream));
         CUDA_TRY(cudaMemcpyAsync(out_dists, sc->dists.ptr, nq * k * 4, cudaMemcpyDeviceToHost, sc->stream));
+        CUDA_TRY(cudaStreamSynchronize(sc->stream));
+        return 0;
+    }();
+    release(rep, sc);
+    return rc;
+}
+
+// Filtered search, per call:
+//   1. ivf_filter_mask_kernel: the row ids with every disallowed row all-ones, and per cluster the allowed and Valid rows;
+//   2. growth: the probe at P, ivf_filter_count_kernel sums the counts over each query's P clusters; the queries short of
+//      k allowed rows go on to min(4 P, P_max), and only they are probed again;
+//   3. the queries grouped by their final P: the plain body over the masked ids (the scan's DYN form, which skips
+//      all-ones ids and orders by (distance, id)) on the gathered queries, its rows scattered back with +inf padding.
+int ivf_search_filtered_on_device(svsb200_ivf* iv, Scratch* sc, const void* d_queries, int qdtype, size_t nq, size_t k,
+                                  size_t n_probes, const uint32_t* d_bitmap, uint64_t* d_out_ids, float* d_out_dists,
+                                  uint32_t* d_probes, uint32_t* d_allowed, uint32_t* d_rows, const uint64_t* d_ext_ids) {
+    const char* who = "svsb200_ivf_search_filtered";
+    svsb200_index* ix = iv->ix.get();
+    cudaStream_t stream = sc->stream;
+    IvfScratch* is = ivf_scratch(iv, sc);
+    const uint32_t C = uint32_t(iv->C);
+    const size_t p_max = std::min<size_t>(C, 1024);
+    const size_t qrow = ix->dim * esize(qdtype);
+    const auto* queries = static_cast<const unsigned char*>(d_queries);
+    // 1. the masked ids
+    CUDA_TRY(is->masked.ensure(iv->d_row_ids.count));
+    CUDA_TRY(is->cl_allowed.ensure(C));
+    CUDA_TRY(is->cl_rows.ensure(C));
+    ivf_filter_mask_kernel<<<C, 256, 0, stream>>>(iv->d_row_ids.ptr, iv->d_start.ptr, iv->d_count.ptr, d_bitmap,
+                                                  is->masked.ptr, is->cl_allowed.ptr, is->cl_rows.ptr);
+    count_launch();
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(is->q_probes.ensure(nq));
+    CUDA_TRY(is->q_allowed.ensure(nq));
+    CUDA_TRY(is->q_rows.ensure(nq));
+    CUDA_TRY(is->qidx.ensure(nq));
+    // `count` queries at positions idx into is->gq (the batch itself when they are all of it, in order)
+    auto gather = [&](const std::vector<uint32_t>& idx) -> const unsigned char* {
+        if (idx.size() == nq) return queries;
+        if (is->gq.ensure(idx.size() * qrow) != cudaSuccess) return nullptr;
+        const size_t bytes = idx.size() * qrow;
+        ivf_gather_rows_kernel<<<unsigned(std::min<size_t>((bytes + 255) / 256, 4096)), 256, 0, stream>>>(
+            queries, is->qidx.ptr, idx.size(), qrow, is->gq.ptr);
+        count_launch();
+        return cudaGetLastError() == cudaSuccess ? is->gq.ptr : nullptr;
+    };
+    // 2. growth
+    std::vector<uint32_t> active(nq), allowed(nq);
+    std::iota(active.begin(), active.end(), 0u);
+    std::map<size_t, std::vector<uint32_t>> groups;   // final P -> its queries, ascending
+    for (size_t P = n_probes;; P = std::min(4 * P, p_max)) {
+        const size_t na = active.size();
+        CUDA_TRY(cudaMemcpyAsync(is->qidx.ptr, active.data(), na * 4, cudaMemcpyHostToDevice, stream));
+        const unsigned char* qp = gather(active);
+        if (!qp) return fail(std::string(who) + ": gathering the queries failed");
+        const size_t pc = std::max<size_t>(1, std::min(na, IVF_LIST_BUDGET / (P * 12)));
+        CUDA_TRY(is->f_probe_ids.ensure(pc * P));
+        CUDA_TRY(is->f_probe_dists.ensure(pc * P));
+        for (size_t a0 = 0; a0 < na; a0 += pc) {
+            const size_t m = std::min(pc, na - a0);
+            if (int rc = flat_search_device("svsb200_ivf_search_filtered: probe", iv->cent->ix.get(), qp + a0 * qrow, qdtype,
+                                            m, P, is->f_probe_ids.ptr, is->f_probe_dists.ptr, stream, nullptr,
+                                            flat_max_kc_deep()))
+                return rc;
+            ivf_filter_count_kernel<<<unsigned((m + 7) / 8), 256, 0, stream>>>(
+                is->f_probe_ids.ptr, uint32_t(m), uint32_t(P), is->qidx.ptr + a0, is->cl_allowed.ptr, is->cl_rows.ptr,
+                is->q_probes.ptr, is->q_allowed.ptr, is->q_rows.ptr);
+            count_launch();
+            CUDA_TRY(cudaGetLastError());
+        }
+        if (P == p_max) {
+            groups[P] = std::move(active);
+            break;
+        }
+        CUDA_TRY(cudaMemcpyAsync(allowed.data(), is->q_allowed.ptr, nq * 4, cudaMemcpyDeviceToHost, stream));
+        CUDA_TRY(cudaStreamSynchronize(stream));
+        std::vector<uint32_t> short_of_k;
+        for (uint32_t q : active) (allowed[q] >= k ? groups[P] : short_of_k).push_back(q);
+        if (short_of_k.empty()) break;
+        active = std::move(short_of_k);
+    }
+    // 3. the scan per group
+    for (auto& [P, idx] : groups) {
+        const size_t ng = idx.size();
+        CUDA_TRY(cudaMemcpyAsync(is->qidx.ptr, idx.data(), ng * 4, cudaMemcpyHostToDevice, stream));
+        const unsigned char* qp = gather(idx);
+        if (!qp) return fail(std::string(who) + ": gathering the queries failed");
+        const bool whole = ng == nq;   // the batch in order: the body writes the outputs, padded +inf in place
+        if (!whole) {
+            CUDA_TRY(is->g_ids.ensure(ng * k));
+            CUDA_TRY(is->g_dists.ensure(ng * k));
+        }
+        uint64_t* gi = whole ? d_out_ids : is->g_ids.ptr;
+        float* gd = whole ? d_out_dists : is->g_dists.ptr;
+        if (int rc = ivf_search_on_device(iv, sc, qp, qdtype, ng, k, P, gi, gd, nullptr, is->masked.ptr)) return rc;
+        ivf_filter_scatter_kernel<<<unsigned((ng * k + 255) / 256), 256, 0, stream>>>(
+            gi, gd, whole ? nullptr : is->qidx.ptr, ng, uint32_t(k), d_out_ids, d_out_dists);
+        count_launch();
+        CUDA_TRY(cudaGetLastError());
+    }
+    if (d_probes) CUDA_TRY(cudaMemcpyAsync(d_probes, is->q_probes.ptr, nq * 4, cudaMemcpyDeviceToDevice, stream));
+    if (d_allowed) CUDA_TRY(cudaMemcpyAsync(d_allowed, is->q_allowed.ptr, nq * 4, cudaMemcpyDeviceToDevice, stream));
+    if (d_rows) CUDA_TRY(cudaMemcpyAsync(d_rows, is->q_rows.ptr, nq * 4, cudaMemcpyDeviceToDevice, stream));
+    if (d_ext_ids) {   // slots -> external ids; a mutation of the dynamic index waits for ev_done (dynamic_ivf.cu)
+        CUDA_TRY(slots_to_external(d_out_ids, nq * k, d_ext_ids, stream));
+        CUDA_TRY(cudaEventRecord(sc->ev_done, stream));
+    }
+    return 0;
+}
+
+int ivf_search_filtered_host(svsb200_ivf* iv, const void* queries, int qdtype, size_t nq, size_t k, size_t n_probes,
+                             const uint32_t* bitmap, size_t bitmap_words, uint64_t* out_ids, float* out_dists,
+                             uint32_t* out_probes, uint32_t* out_allowed, uint32_t* out_rows, const uint64_t* d_ext_ids) {
+    Replica* rep = iv->ix->reps[0].get();
+    CUDA_TRY(cudaSetDevice(rep->device));
+    std::string err;
+    Scratch* sc = acquire(rep, &err);
+    if (!sc) return fail(err);
+    const int rc = [&]() -> int {
+        const size_t qbytes = nq * iv->ix->dim * esize(qdtype);
+        IvfScratch* is = ivf_scratch(iv, sc);
+        CUDA_TRY(sc->q_raw.ensure(qbytes));
+        CUDA_TRY(sc->ids.ensure(nq * k * 8));
+        CUDA_TRY(sc->dists.ensure(nq * k));
+        CUDA_TRY(is->bitmap.ensure(std::max<size_t>(bitmap_words, 1)));
+        CUDA_TRY(cudaMemcpyAsync(sc->q_raw.ptr, queries, qbytes, cudaMemcpyHostToDevice, sc->stream));
+        if (bitmap_words)
+            CUDA_TRY(cudaMemcpyAsync(is->bitmap.ptr, bitmap, bitmap_words * 4, cudaMemcpyHostToDevice, sc->stream));
+        if (int rc = ivf_search_filtered_on_device(iv, sc, sc->q_raw.ptr, qdtype, nq, k, n_probes, is->bitmap.ptr,
+                                                   reinterpret_cast<uint64_t*>(sc->ids.ptr), sc->dists.ptr, nullptr, nullptr,
+                                                   nullptr, d_ext_ids))
+            return rc;
+        CUDA_TRY(cudaMemcpyAsync(out_ids, sc->ids.ptr, nq * k * 8, cudaMemcpyDeviceToHost, sc->stream));
+        CUDA_TRY(cudaMemcpyAsync(out_dists, sc->dists.ptr, nq * k * 4, cudaMemcpyDeviceToHost, sc->stream));
+        if (out_probes) CUDA_TRY(cudaMemcpyAsync(out_probes, is->q_probes.ptr, nq * 4, cudaMemcpyDeviceToHost, sc->stream));
+        if (out_allowed) CUDA_TRY(cudaMemcpyAsync(out_allowed, is->q_allowed.ptr, nq * 4, cudaMemcpyDeviceToHost, sc->stream));
+        if (out_rows) CUDA_TRY(cudaMemcpyAsync(out_rows, is->q_rows.ptr, nq * 4, cudaMemcpyDeviceToHost, sc->stream));
         CUDA_TRY(cudaStreamSynchronize(sc->stream));
         return 0;
     }();
@@ -631,6 +770,34 @@ int svsb200_ivf_search(svsb200_ivf* index, const void* queries, int qdtype, size
     if (nq == 0) return 0;
     if (!queries || !out_ids || !out_dists) return fail("svsb200_ivf_search: NULL buffer");
     return ivf_search_host(index, queries, qdtype, nq, k, n_probes, out_ids, out_dists, nullptr);
+}
+
+int svsb200_ivf_search_filtered_device(svsb200_ivf* index, const void* d_queries, int qdtype, size_t nq, size_t k,
+                                       size_t n_probes, const uint32_t* d_id_bitmap, uint64_t* d_out_ids, float* d_out_dists,
+                                       uint32_t* d_out_probes, uint32_t* d_out_allowed, uint32_t* d_out_rows, void* stream_) {
+    const char* who = "svsb200_ivf_search_filtered_device";
+    if (int rc = ivf_check_search(who, index, qdtype, k, n_probes)) return rc;
+    if (!d_id_bitmap) return fail("svsb200_ivf_search_filtered_device: NULL bitmap");
+    if (nq == 0) return 0;
+    if (!d_queries || !d_out_ids || !d_out_dists) return fail("svsb200_ivf_search_filtered_device: NULL buffer");
+    Replica* rep = index->ix->reps[0].get();
+    CUDA_TRY(cudaSetDevice(rep->device));
+    std::string err;
+    Scratch* sc = scratch_for_stream(rep, static_cast<cudaStream_t>(stream_), &err);
+    if (!sc) return fail(err);
+    return ivf_search_filtered_on_device(index, sc, d_queries, qdtype, nq, k, n_probes, d_id_bitmap, d_out_ids, d_out_dists,
+                                         d_out_probes, d_out_allowed, d_out_rows, nullptr);
+}
+
+int svsb200_ivf_search_filtered(svsb200_ivf* index, const void* queries, int qdtype, size_t nq, size_t k, size_t n_probes,
+                                const uint32_t* id_bitmap, uint64_t* out_ids, float* out_dists, uint32_t* out_probes,
+                                uint32_t* out_allowed, uint32_t* out_rows) {
+    if (int rc = ivf_check_search("svsb200_ivf_search_filtered", index, qdtype, k, n_probes)) return rc;
+    if (!id_bitmap) return fail("svsb200_ivf_search_filtered: NULL bitmap");
+    if (nq == 0) return 0;
+    if (!queries || !out_ids || !out_dists) return fail("svsb200_ivf_search_filtered: NULL buffer");
+    return ivf_search_filtered_host(index, queries, qdtype, nq, k, n_probes, id_bitmap, (index->n + 31) / 32, out_ids,
+                                    out_dists, out_probes, out_allowed, out_rows, nullptr);
 }
 
 }  // extern "C"

@@ -608,6 +608,76 @@ __global__ void ivf_kmeans_update_kernel(const char* __restrict__ train, uint32_
     if (lane == 0) counts[c] = cnt;
 }
 
+// ---- filtered search (ivf.cu, ivf_search_filtered_on_device) ----
+// One CTA per cluster: masked[r] = row_ids[r] where that id's bit of `bitmap` is set, all-ones otherwise (a tombstone or
+// padding entry already is), for the cluster's stored rows [cl_start, cl_start + cl_count); cl_allowed[c] counts the
+// entries kept, cl_rows[c] the entries that are not all-ones.  The ids index the bitmap: original ids of the static
+// index, slots of the dynamic one.
+__global__ void ivf_filter_mask_kernel(const uint32_t* __restrict__ row_ids, const uint32_t* __restrict__ cl_start,
+                                       const uint32_t* __restrict__ cl_count, const uint32_t* __restrict__ bitmap,
+                                       uint32_t* __restrict__ masked, uint32_t* __restrict__ cl_allowed,
+                                       uint32_t* __restrict__ cl_rows) {
+    const uint32_t c = blockIdx.x, start = cl_start[c], count = cl_count[c];
+    uint32_t allowed = 0, rows = 0;
+    for (uint32_t base = 0; base < count; base += blockDim.x) {   // (uniform trip count: __syncthreads_count inside)
+        const uint32_t i = base + threadIdx.x;
+        const uint32_t id = i < count ? row_ids[start + i] : 0xFFFFFFFFu;
+        const bool valid = id != 0xFFFFFFFFu;
+        const bool keep = valid && ((bitmap[id >> 5] >> (id & 31u)) & 1u);
+        if (i < count) masked[start + i] = keep ? id : 0xFFFFFFFFu;
+        allowed += __syncthreads_count(keep);
+        rows += __syncthreads_count(valid);
+    }
+    if (threadIdx.x == 0) {
+        cl_allowed[c] = allowed;
+        cl_rows[c] = rows;
+    }
+}
+// One warp per query of a probe round: the allowed and Valid rows of its first P probes (probes [nq][P]) summed and
+// written, with P, to query qidx[i] (qidx NULL: i) of the per-query outputs.
+__global__ void ivf_filter_count_kernel(const uint64_t* __restrict__ probes, uint32_t nq, uint32_t P,
+                                        const uint32_t* __restrict__ qidx, const uint32_t* __restrict__ cl_allowed,
+                                        const uint32_t* __restrict__ cl_rows, uint32_t* __restrict__ q_probes,
+                                        uint32_t* __restrict__ q_allowed, uint32_t* __restrict__ q_rows) {
+    const uint32_t i = blockIdx.x * (blockDim.x / 32) + threadIdx.x / 32;
+    const int lane = threadIdx.x & 31;
+    if (i >= nq) return;
+    uint32_t a = 0, r = 0;
+    for (uint32_t j = lane; j < P; j += 32) {
+        const uint64_t c = probes[size_t(i) * P + j];
+        a += cl_allowed[c];
+        r += cl_rows[c];
+    }
+    a = __reduce_add_sync(0xFFFFFFFFu, a);
+    r = __reduce_add_sync(0xFFFFFFFFu, r);
+    if (lane == 0) {
+        const uint32_t q = qidx ? qidx[i] : i;
+        q_probes[q] = P;
+        q_allowed[q] = a;
+        q_rows[q] = r;
+    }
+}
+// dst row i <- src row idx[i], rows of `row_bytes` bytes.
+__global__ void ivf_gather_rows_kernel(const unsigned char* __restrict__ src, const uint32_t* __restrict__ idx, size_t count,
+                                       size_t row_bytes, unsigned char* __restrict__ dst) {
+    for (size_t e = size_t(blockIdx.x) * blockDim.x + threadIdx.x; e < count * row_bytes; e += size_t(gridDim.x) * blockDim.x) {
+        const size_t i = e / row_bytes;
+        dst[e] = src[size_t(idx[i]) * row_bytes + (e - i * row_bytes)];
+    }
+}
+// Result row i of a query group -> row idx[i] of the batch's result (idx NULL: i), `k` entries a row; a padding entry
+// (all-ones id) gets distance +inf, whatever the metric.
+// (In place when idx is NULL: each entry is read and written by one thread.)
+__global__ void ivf_filter_scatter_kernel(const uint64_t* ids, const float* dists, const uint32_t* __restrict__ idx,
+                                          size_t count, uint32_t k, uint64_t* out_ids, float* out_dists) {
+    const size_t e = size_t(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (e >= count * k) return;
+    const size_t i = e / k, o = (idx ? size_t(idx[i]) : i) * k + (e - i * k);
+    const uint64_t id = ids[e];
+    out_ids[o] = id;
+    out_dists[o] = id == ~uint64_t(0) ? INFINITY : dists[e];
+}
+
 // probes / assignments: 64-bit search ids -> 32-bit cluster numbers
 __global__ void ivf_narrow_ids_kernel(const uint64_t* __restrict__ in, size_t count, uint32_t* __restrict__ out) {
     const size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x;

@@ -26,7 +26,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from .ivf import Clustering, IVFSearchParameters, _sq_codes
+from .ivf import Clustering, IVFSearchParameters, _bitmap, _search_filtered, _sq_codes
 from .vamana import _DTYPE_CODE, DistanceType
 
 
@@ -209,3 +209,18 @@ class DynamicIVF:
         _lib.check(self._lib.svsb200_dynamic_ivf_search_device(self._h, d_queries, _DTYPE_CODE[np.dtype(qdtype)], nq,
                                                                int(n_neighbors), n_probes, d_ids, d_dists,
                                                                stream or None))
+
+    def search_filtered(self, queries: np.ndarray, n_neighbors: int, allowed: np.ndarray, with_counts: bool = False):
+        """:meth:`IVF.search_filtered` over the Valid rows: ``allowed`` is a boolean mask over the SLOTS
+        (``num_slots`` entries, in the order of :meth:`export`); Empty slots are never returned.  Returns external ids,
+        distances and the number found per query; ``with_counts`` adds (probes used, allowed rows, Valid rows)."""
+        return _search_filtered(self._lib.svsb200_dynamic_ivf_search_filtered, self._h, self.dimensions, queries,
+                                n_neighbors, self._n_probes(), _bitmap(allowed, self.num_slots), with_counts)
+
+    def search_filtered_device(self, d_queries: int, qdtype: np.dtype, nq: int, n_neighbors: int, d_bitmap: int,
+                               d_ids: int, d_dists: int, d_probes: int = 0, d_allowed: int = 0, d_rows: int = 0,
+                               stream: int = 0) -> None:
+        """Device-buffer form of :meth:`search_filtered` (bitmap over slots, (num_slots + 31) / 32 words)."""
+        _lib.check(self._lib.svsb200_dynamic_ivf_search_filtered_device(
+            self._h, d_queries, _DTYPE_CODE[np.dtype(qdtype)], nq, int(n_neighbors), self._n_probes(), d_bitmap, d_ids,
+            d_dists, d_probes or None, d_allowed or None, d_rows or None, stream or None))

@@ -73,6 +73,34 @@ def sq_compress(data, dtype=np.int8, device: int = 0):
     return codes, float(np.float32(scale.value)), float(np.float32(bias.value))
 
 
+def _bitmap(allowed, n: int) -> np.ndarray:
+    """A boolean mask of n entries -> the uint32 bitmap of the filtered searches ((n + 31) / 32 words)."""
+    mask = np.ascontiguousarray(allowed, dtype=bool)
+    if mask.shape != (n,):
+        raise ValueError(f"allowed must hold {n} booleans")
+    b = np.packbits(mask, bitorder="little")
+    return np.concatenate([b, np.zeros((-len(b)) % 4, dtype=np.uint8)]).view(np.uint32)
+
+
+def _search_filtered(fn, h, dims: int, queries, n_neighbors: int, n_probes: int, bitmap: np.ndarray, with_counts: bool):
+    """The host form of both indexes' filtered searches."""
+    q = np.ascontiguousarray(queries)
+    if q.ndim != 2 or q.shape[1] != dims:
+        raise ValueError(f"queries must be [nq, {dims}]")
+    if q.dtype not in _DTYPE_CODE:
+        raise TypeError(f"unsupported query type {q.dtype}")
+    nq, k = q.shape[0], int(n_neighbors)
+    ids = np.empty((nq, k), dtype=np.uint64)
+    dists = np.empty((nq, k), dtype=np.float32)
+    probes, allowed, rows = (np.empty(nq, dtype=np.uint32) for _ in range(3))
+    _lib.check(fn(h, q.ctypes.data, _DTYPE_CODE[q.dtype], nq, k, n_probes, bitmap.ctypes.data, ids.ctypes.data,
+                  dists.ctypes.data, probes.ctypes.data, allowed.ctypes.data, rows.ctypes.data))
+    found = np.minimum(allowed, np.uint32(k))
+    if with_counts:
+        return ids, dists, found, (probes, allowed, rows)
+    return ids, dists, found
+
+
 def _sq_codes(data, sq) -> np.ndarray:
     """The codes of an SQ ``assemble_from_clustering``: int8 / uint8 rows."""
     x = np.ascontiguousarray(data.load() if hasattr(data, "load") else data)
@@ -208,3 +236,22 @@ class IVF:
         n_probes = self._n_probes()
         _lib.check(self._lib.svsb200_ivf_search_device(self._h, d_queries, _DTYPE_CODE[np.dtype(qdtype)], nq,
                                                        int(n_neighbors), n_probes, d_ids, d_dists, stream or None))
+
+    def search_filtered(self, queries: np.ndarray, n_neighbors: int, allowed: np.ndarray, with_counts: bool = False):
+        """``svs::runtime::IVFIndex::search(..., IDFilter*)``: ``allowed`` is a boolean mask over the ids.  Each query
+        probes ``search_parameters.n_probes`` clusters, four times more while they hold fewer than k allowed rows (at
+        most min(C, 1024)), and gets the exact top k over the allowed rows of those clusters.  Returns (ids uint64,
+        distances, found per query); short rows are padded with all-ones / +inf for every metric.  ``with_counts``
+        adds (probes used, allowed rows, rows) of the probed clusters per query."""
+        return _search_filtered(self._lib.svsb200_ivf_search_filtered, self._h, self.dimensions, queries, n_neighbors,
+                                self._n_probes(), _bitmap(allowed, self.size), with_counts)
+
+    def search_filtered_device(self, d_queries: int, qdtype: np.dtype, nq: int, n_neighbors: int, d_bitmap: int,
+                               d_ids: int, d_dists: int, d_probes: int = 0, d_allowed: int = 0, d_rows: int = 0,
+                               stream: int = 0) -> None:
+        """Device-buffer form of :meth:`search_filtered`: the uint32 bitmap ((size + 31) / 32 words, bit i = id i) and
+        the outputs are raw device pointers (the per-query uint32 outputs may be 0), enqueued on ``stream`` apart from
+        the probes and the growth decisions."""
+        _lib.check(self._lib.svsb200_ivf_search_filtered_device(
+            self._h, d_queries, _DTYPE_CODE[np.dtype(qdtype)], nq, int(n_neighbors), self._n_probes(), d_bitmap, d_ids,
+            d_dists, d_probes or None, d_allowed or None, d_rows or None, stream or None))
