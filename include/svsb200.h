@@ -335,6 +335,30 @@ int svsb200_flat_index_search_device(svsb200_flat* index, const void* d_queries,
 int svsb200_flat_index_search(svsb200_flat* index, const void* queries, int qdtype, size_t nq, size_t k, uint64_t* out_ids,
                               float* out_dists);
 
+/* Filtered exact search: FlatIndex::search with a predicate over the data index (index/flat/flat.h:421-465).
+ * `id_bitmap` ((n + 31) / 32 words; NULL is refused): bit i % 32 of word i / 32 set means row i may be returned; bits
+ * past n are ignored.  Each query gets the exact top k (1 <= k <= 1024) over the A allowed rows: the scan's bit-exact
+ * distances, ordered by (distance, id), min(k, A) real entries, the rest padded with all-ones ids and +inf for EVERY
+ * metric.  The result equals svsb200_flat_index_search over a Flat built from the allowed rows in ascending id order,
+ * its ids mapped back, bit for bit (only the padding's distance differs: +inf).  Query and row types, metrics and
+ * limits are svsb200_flat_index_search's.  `out_allowed` (optional) receives A.
+ * Routes (svsb200_flat_filter_plan): the dense route runs svsb200_flat_index_search's routing with the disallowed
+ * rows masked (the GEMM never offers them to a list, the scans skip them); the sparse route gathers the allowed rows
+ * and runs the exact scan over them alone.  All per-call state lives in the caller stream's scratch, so searches of
+ * one index with different bitmaps may run concurrently on different streams.  `fallback_queries` (optional) receives
+ * how many queries ran on a scan.  The device form (queries, bitmap and outputs in device memory) is enqueued on
+ * `stream` apart from one synchronisation for A and, on the dense route, the fallback count's. */
+int svsb200_flat_index_search_filtered_device(svsb200_flat* index, const void* d_queries, int qdtype, size_t nq, size_t k,
+                                              const uint32_t* d_id_bitmap, uint64_t* d_out_ids, float* d_out_dists,
+                                              void* stream, size_t* out_allowed, uint32_t* fallback_queries);
+/* The same with HOST buffers (blocking). */
+int svsb200_flat_index_search_filtered(svsb200_flat* index, const void* queries, int qdtype, size_t nq, size_t k,
+                                       const uint32_t* id_bitmap, uint64_t* out_ids, float* out_dists, size_t* out_allowed);
+/* The route of a filtered flat search with `allowed` of `n` rows allowed (host arithmetic only): SPARSE when
+ * allowed * 64 <= n (so always when allowed = 0), DENSE otherwise.  Fails for allowed > n. */
+enum { SVSB200_FLAT_ROUTE_DENSE = 0, SVSB200_FLAT_ROUTE_SPARSE = 1 };
+int svsb200_flat_filter_plan(size_t n, size_t allowed, int* route);
+
 /* Dynamic index.  Replaces: MutableVamanaIndex(graph, data, entry_point, distance, external_ids, threadpool)
  * (include/svs/index/vamana/dynamic_index.h:178-202) for float32 / float16 plain storage on one device, adjacency rows
  * of at most 128 neighbours, L2 / MIP / cosine.  Arguments as svsb200_index_create (dense rows), plus one distinct
@@ -460,6 +484,19 @@ int svsb200_dynamic_flat_search_device(svsb200_dynamic_flat* index, const void* 
 /* The same with HOST buffers (blocking). */
 int svsb200_dynamic_flat_search(svsb200_dynamic_flat* index, const void* queries, int qdtype, size_t nq, size_t k,
                                 uint64_t* out_ids, float* out_dists);
+/* search with a predicate over the data index (dynamic_flat.h:513-573, 653-661): svsb200_flat_index_search_filtered's
+ * contract with the bitmap over SLOTS ((num_slots + 31) / 32 words; Empty slots' bits are ignored), EXTERNAL ids and
+ * ties by slot.  The result equals svsb200_flat_index_search over the rows of the slots that are both Valid and
+ * allowed, in slot order, its ids mapped to the external ids.  `out_allowed` receives the number of such slots.  As
+ * every search here, the device form records the scratch's event, so a mutation waits for it. */
+int svsb200_dynamic_flat_search_filtered_device(svsb200_dynamic_flat* index, const void* d_queries, int qdtype, size_t nq,
+                                                size_t k, const uint32_t* d_slot_bitmap, uint64_t* d_out_ids,
+                                                float* d_out_dists, void* stream, size_t* out_allowed,
+                                                uint32_t* fallback_queries);
+/* The same with HOST buffers (blocking). */
+int svsb200_dynamic_flat_search_filtered(svsb200_dynamic_flat* index, const void* queries, int qdtype, size_t nq, size_t k,
+                                         const uint32_t* slot_bitmap, uint64_t* out_ids, float* out_dists,
+                                         size_t* out_allowed);
 
 /* IVF index.  Replaces: IVFIndex (include/svs/index/ivf/index.h) with svs::IVF and svs::Clustering
  * (index/ivf/kmeans.h, common.h): float32 / float16 rows on one device, L2 / MIP / cosine, grouped into C clusters

@@ -33,6 +33,8 @@ SYMBOLS = [
     "svsb200_dynamic_flat_add", "svsb200_dynamic_flat_delete", "svsb200_dynamic_flat_compact", "svsb200_dynamic_flat_ids",
     "svsb200_dynamic_flat_has_id", "svsb200_dynamic_flat_export", "svsb200_dynamic_flat_search",
     "svsb200_dynamic_flat_search_device",
+    "svsb200_flat_index_search_filtered", "svsb200_flat_index_search_filtered_device", "svsb200_flat_filter_plan",
+    "svsb200_dynamic_flat_search_filtered", "svsb200_dynamic_flat_search_filtered_device",
     "svsb200_ivf_random", "svsb200_ivf_cluster", "svsb200_ivf_create", "svsb200_ivf_destroy", "svsb200_ivf_size",
     "svsb200_ivf_dimensions", "svsb200_ivf_num_clusters", "svsb200_ivf_device_bytes", "svsb200_ivf_cluster_sizes",
     "svsb200_ivf_centroids", "svsb200_ivf_search", "svsb200_ivf_search_device", "svsb200_sq_compress",
@@ -78,6 +80,10 @@ def lib() -> C.CDLL:
         fn.restype, fn.argtypes = sz, [vp]
     l.svsb200_flat_index_search.argtypes = [vp, vp, i32, sz, sz, vp, vp]
     l.svsb200_flat_index_search_device.argtypes = [vp, vp, i32, sz, sz, vp, vp, vp, C.POINTER(u32)]
+    l.svsb200_flat_index_search_filtered.argtypes = [vp, vp, i32, sz, sz, vp, vp, vp, C.POINTER(sz)]
+    l.svsb200_flat_index_search_filtered_device.argtypes = [vp, vp, i32, sz, sz, vp, vp, vp, vp, C.POINTER(sz),
+                                                            C.POINTER(u32)]
+    l.svsb200_flat_filter_plan.argtypes = [sz, sz, C.POINTER(i32)]
     l.svsb200_index_create.argtypes = [vp, i32, sz, sz, sz, vp, sz, u32, i32, i32, vp, i32, C.POINTER(vp)]
     l.svsb200_index_destroy.argtypes = [vp]
     for name in ("size", "dimensions", "max_degree", "device_bytes"):
@@ -136,6 +142,9 @@ def lib() -> C.CDLL:
     l.svsb200_dynamic_flat_export.argtypes = [vp, vp, vp]
     l.svsb200_dynamic_flat_search.argtypes = [vp, vp, i32, sz, sz, vp, vp]
     l.svsb200_dynamic_flat_search_device.argtypes = [vp, vp, i32, sz, sz, vp, vp, vp, C.POINTER(u32)]
+    l.svsb200_dynamic_flat_search_filtered.argtypes = [vp, vp, i32, sz, sz, vp, vp, vp, C.POINTER(sz)]
+    l.svsb200_dynamic_flat_search_filtered_device.argtypes = [vp, vp, i32, sz, sz, vp, vp, vp, vp, C.POINTER(sz),
+                                                              C.POINTER(u32)]
     l.svsb200_ivf_random.argtypes = [C.c_uint64, sz, vp]
     l.svsb200_ivf_cluster.argtypes = [vp, i32, sz, sz, i32, sz, sz, sz, i32, C.c_float, C.c_uint64, i32, vp, vp]
     l.svsb200_ivf_create.argtypes = [vp, i32, sz, sz, i32, vp, sz, vp, i32, C.POINTER(vp)]
@@ -177,3 +186,37 @@ def lib() -> C.CDLL:
 def check(rc: int) -> None:
     if rc != 0:
         raise Svsb200Error(lib().svsb200_last_error().decode(errors="replace"))
+
+
+def _bitmap(allowed, n: int):
+    """A boolean mask of n entries -> the uint32 bitmap of the filtered searches ((n + 31) / 32 words)."""
+    import numpy as np
+
+    mask = np.ascontiguousarray(allowed, dtype=bool)
+    if mask.shape != (n,):
+        raise ValueError(f"allowed must hold {n} booleans")
+    b = np.packbits(mask, bitorder="little")
+    return np.concatenate([b, np.zeros((-len(b)) % 4, dtype=np.uint8)]).view(np.uint32)
+
+
+def _flat_search_filtered(fn, h, dims: int, queries, n_neighbors: int, bitmap, with_counts: bool):
+    """The host form of the Flat and DynamicFlat filtered searches: (ids, dists, found[, allowed rows])."""
+    import numpy as np
+
+    from .vamana import _DTYPE_CODE
+
+    q = np.ascontiguousarray(queries)
+    if q.ndim != 2 or q.shape[1] != dims:
+        raise ValueError(f"queries must be [nq, {dims}]")
+    if q.dtype not in _DTYPE_CODE:
+        raise TypeError(f"unsupported query type {q.dtype}")
+    nq, k = q.shape[0], int(n_neighbors)
+    ids = np.empty((nq, k), dtype=np.uint64)
+    dists = np.empty((nq, k), dtype=np.float32)
+    allowed = C.c_size_t()
+    check(fn(h, q.ctypes.data, _DTYPE_CODE[q.dtype], nq, k, bitmap.ctypes.data, ids.ctypes.data, dists.ctypes.data,
+             C.byref(allowed)))
+    found = np.full(nq, min(k, allowed.value), dtype=np.uint32)
+    if with_counts:
+        return ids, dists, found, int(allowed.value)
+    return ids, dists, found

@@ -343,4 +343,19 @@ int svsb200_dynamic_flat_search(svsb200_dynamic_flat* index, const void* queries
                             flat_max_kc_deep());
 }
 
+int svsb200_dynamic_flat_search_filtered_device(svsb200_dynamic_flat* index, const void* d_queries, int qdtype, size_t nq,
+                                                size_t k, const uint32_t* d_slot_bitmap, uint64_t* d_out_ids,
+                                                float* d_out_dists, void* stream, size_t* out_allowed,
+                                                uint32_t* fallback_queries) {
+    return flat_search_filtered_device("svsb200_dynamic_flat_search_filtered_device", index_of(index), d_queries, qdtype, nq,
+                                       k, d_slot_bitmap, d_out_ids, d_out_dists, stream, out_allowed, fallback_queries);
+}
+
+int svsb200_dynamic_flat_search_filtered(svsb200_dynamic_flat* index, const void* queries, int qdtype, size_t nq, size_t k,
+                                         const uint32_t* slot_bitmap, uint64_t* out_ids, float* out_dists,
+                                         size_t* out_allowed) {
+    return flat_search_filtered_host("svsb200_dynamic_flat_search_filtered", index_of(index), queries, qdtype, nq, k,
+                                     slot_bitmap, out_ids, out_dists, out_allowed);
+}
+
 }  // extern "C"

@@ -64,6 +64,12 @@
 //       one with K = T.K has an id above T.id > id_k.  (At |v| = 2^24 the bound fails: 2^24 + 1 rounds to 2^24.)
 // Below 2^24 (b) always holds, so no query falls back.  The GEMM key is also checked against the rescored distance,
 // F(K) == the exact distance for every candidate: a wrong integer GEMM shows as a fallback, not a wrong answer.
+//
+// Filtered search (DESIGN.md §9d): the GEMM reads a per-call copy of the bias in which every disallowed column has the
+// empty bias, so such a column is never offered to a list (fp16: its key is +inf or NaN; integer kinds: the MASKED
+// epilogue gives it the empty key).  The certificate keeps its form and needs no new proof: every allowed row that is
+// not a candidate still has an approximate key >= T, and the excluded rows are now a subset of those it already
+// covered.  Xmax stays the index's (or the Valid slots'): sound, if looser than the allowed rows' maximum.
 #include "host.cuh"
 #include "search_kernel.cuh"
 
@@ -305,7 +311,10 @@ template <int KIND> __device__ __forceinline__ bool flat_beats(flat_key_t<KIND> 
 
 // (The shape is named through the type alias `Shape` only: a kernel-local constant would make the compiler order the
 // main loop's stage counters differently and change the FLAT_KC instantiations' code.)
-template <int KIND, uint32_t KC>
+// MASKED (integer kinds, the filtered search): a column whose bias is the empty bias INT32_MAX gets the empty key
+// whatever its blob holds.  The wrapping key bias - 2 s of such a column over a non-zero blob looks like an ordinary key
+// (and would send the query to the scan through the rescoring's mismatch check); no real |x|^2 reaches INT32_MAX.
+template <int KIND, uint32_t KC, bool MASKED = false>
 __global__ void __launch_bounds__(FLAT_THREADS, 1) flat_gemm_topk_kernel(const __grid_constant__ FlatParams fp) {
     using acc_t = std::conditional_t<KIND == FLAT_F16, float, int>;
     using Shape = FlatShape<KC>;
@@ -469,6 +478,8 @@ __global__ void __launch_bounds__(FLAT_THREADS, 1) flat_gemm_topk_kernel(const _
                 const uint32_t b = v & 1u ? b2.y : b2.x;
                 if constexpr (KIND == FLAT_F16) key[v] = fmaf(fp.key_scale, d[4 * c + v], __uint_as_float(b));
                 else key[v] = (b + uint32_t(int(fp.key_scale)) * uint32_t(d[4 * c + v])) ^ 0x80000000u;
+                if constexpr (MASKED && KIND != FLAT_F16)
+                    if (b == 0x7FFFFFFFu) key[v] = 0xFFFFFFFFu;
             }
             const bool any = flat_beats<KIND>(min(key[0], key[1]), thr[0][h]) || flat_beats<KIND>(min(key[2], key[3]), thr[1][h]);
             if (!__any_sync(0xFFFFFFFFu, any)) continue;
@@ -805,6 +816,76 @@ __global__ void flat_masked_xmax_kernel(const float* __restrict__ norms, const u
     if ((threadIdx.x & 31) == 0 && m) atomicMax(xmax_bits, m);
 }
 
+// ---- filtered search: the per-call mask (all of it in the scratch) ---------------------------------------------------
+// Row i is allowed iff bit i % 32 of bitmap word i / 32 is set, i < n and (a dynamic flat index) its slot is Valid:
+// status[i] = Valid / Empty, and the allowed rows again as bitmap words (zero past n).  One warp per word.
+__global__ void flat_filter_rows_kernel(const uint32_t* __restrict__ bitmap, const uint8_t* __restrict__ slot_status,
+                                        uint32_t n, uint8_t* __restrict__ status, uint32_t* __restrict__ words) {
+    const uint32_t w = blockIdx.x * (blockDim.x / 32) + threadIdx.x / 32, lane = threadIdx.x & 31;
+    if (w >= (n + 31) / 32) return;
+    const uint32_t i = 32 * w + lane;
+    const bool ok = i < n && ((__ldg(bitmap + w) >> lane) & 1u) && (!slot_status || slot_status[i] == SLOT_VALID);
+    const uint32_t m = __ballot_sync(0xFFFFFFFFu, ok);
+    if (i < n) status[i] = ok ? SLOT_VALID : SLOT_EMPTY;
+    if (lane == 0) words[w] = m;
+}
+
+// The set bits of `words` as ascending row ids: ids[0 .. *count).  One block; each thread takes a run of words.
+__global__ void __launch_bounds__(1024) flat_compact_kernel(const uint32_t* __restrict__ words, uint32_t nwords,
+                                                            uint32_t* __restrict__ ids, uint32_t* __restrict__ count) {
+    __shared__ uint32_t warp_total[32];
+    const uint32_t per = (nwords + blockDim.x - 1) / blockDim.x;
+    const uint32_t w0 = min(nwords, threadIdx.x * per), w1 = min(nwords, w0 + per);
+    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    uint32_t c = 0;
+    for (uint32_t w = w0; w < w1; ++w) c += __popc(words[w]);
+    uint32_t x = c;   // inclusive prefix over the warp, then over the warps
+    for (uint32_t o = 1; o < 32; o <<= 1) {
+        const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, x, o);
+        if (lane >= o) x += y;
+    }
+    if (lane == 31) warp_total[warp] = x;
+    __syncthreads();
+    if (warp == 0) {
+        uint32_t t = lane < blockDim.x / 32 ? warp_total[lane] : 0u;
+        for (uint32_t o = 1; o < 32; o <<= 1) {
+            const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, t, o);
+            if (lane >= o) t += y;
+        }
+        warp_total[lane] = t;
+    }
+    __syncthreads();
+    uint32_t o = x - c + (warp ? warp_total[warp - 1] : 0u);
+    for (uint32_t w = w0; w < w1; ++w)
+        for (uint32_t b = words[w]; b; b &= b - 1) ids[o++] = 32 * w + uint32_t(__ffs(int(b)) - 1);
+    if (threadIdx.x == blockDim.x - 1) *count = o;
+}
+
+// The GEMM's bias for this call: row i keeps bias[i] when it is allowed, every other column gets the empty bias.
+__global__ void flat_mask_bias_kernel(const uint32_t* __restrict__ bias, const uint32_t* __restrict__ words, uint32_t n,
+                                      uint32_t rows, uint32_t empty_bias, uint32_t* __restrict__ out) {
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < rows; i += gridDim.x * blockDim.x)
+        out[i] = i < n && ((words[i >> 5] >> (i & 31)) & 1u) ? bias[i] : empty_bias;
+}
+
+// Ids of a search over the gathered allowed rows -> row ids (`rows`, the compacted ids) -> external ids (`ext_ids`,
+// a dynamic flat index).  Padding ids stay all-ones.
+__global__ void flat_unmap_ids_kernel(uint64_t* __restrict__ ids, size_t count, const uint32_t* __restrict__ rows,
+                                      const uint64_t* __restrict__ ext_ids) {
+    for (size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x; i < count; i += size_t(gridDim.x) * blockDim.x) {
+        const uint64_t id = ids[i];
+        if (id == ~uint64_t(0)) continue;
+        const uint32_t r = rows[id];
+        ids[i] = ext_ids ? ext_ids[r] : r;
+    }
+}
+
+// The filtered searches pad with +inf for every metric (the scan pads inner product with -inf).
+__global__ void flat_pad_inf_kernel(const uint64_t* __restrict__ ids, float* __restrict__ dists, size_t count) {
+    for (size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x; i < count; i += size_t(gridDim.x) * blockDim.x)
+        if (ids[i] == ~uint64_t(0)) dists[i] = INFINITY;
+}
+
 // ---- launchers ------------------------------------------------------------------------------------------------------
 // Rows -> the operand blobs of `kind`: flat_tile_kernel (fp16) or flat_tile8_kernel (8-bit, which has no norms).
 // `bias` (float, or int32 for 8-bit blobs), `norms` and `max_norm_bits` may be NULL.
@@ -863,7 +944,7 @@ static void flat_plan(uint32_t mtiles, uint32_t ntiles, uint32_t sm_count, uint3
 
 static cudaError_t flat_gemm_topk(int kind, int kc, const void* a_tiles, const void* b_tiles, const void* b_bias, uint32_t KB, uint32_t ntiles,
                                   uint32_t mtiles, uint32_t ctas, uint32_t share, uint32_t nlists, float key_scale, float* cand_key,
-                                  uint32_t* cand_id, uint32_t* progress, cudaStream_t stream) {
+                                  uint32_t* cand_id, uint32_t* progress, cudaStream_t stream, bool masked = false) {
     FlatParams fp{};
     fp.a_tiles = static_cast<const __half*>(a_tiles);
     fp.b_tiles = static_cast<const __half*>(b_tiles);
@@ -886,7 +967,11 @@ static cudaError_t flat_gemm_topk(int kind, int kc, const void* a_tiles, const v
         constexpr int KC = decltype(c)::value;
         const LaunchConfig cfg{int(ctas), int(FLAT_THREADS / 32), FlatShape<KC>::SMEM, stream};
         return dispatch(IntList<FLAT_F16, FLAT_S8, FLAT_U8>{}, kind, [&](auto k) {
-            return launch_kernel(flat_gemm_topk_kernel<decltype(k)::value, uint32_t(KC)>, cfg, ctas, true, fp);
+            constexpr int KIND = decltype(k)::value;
+            // (fp16 keys need no mask: fmaf(scale, s, +inf) is +inf or NaN, which no list is offered)
+            if constexpr (KIND != FLAT_F16)
+                if (masked) return launch_kernel(flat_gemm_topk_kernel<KIND, uint32_t(KC), true>, cfg, ctas, true, fp);
+            return launch_kernel(flat_gemm_topk_kernel<KIND, uint32_t(KC)>, cfg, ctas, true, fp);
         });
     });
 }
@@ -1007,9 +1092,12 @@ static int ensure_slots_xmax(svsb200_index* ix, Replica* rep, cudaStream_t strea
 // for one synchronisation (the count of queries that need the exact-scan fallback).  `max_kc` is the deepest list the
 // caller allows: k + 8 <= FLAT_KC runs the FLAT_KC lists, k + 8 <= FLAT_KC_DEEP (Flat handles only) the deep ones.
 // Ids are row numbers (dynamic flat index: slots; flat_on_device maps them to external ids).
+// Filtered (flat_filtered_on_device): `row_bits` / `row_status` mark the allowed rows (a dynamic index's: allowed and
+// Valid) as a bitmap and as status bytes, both in the scratch.  The GEMM reads a scratch copy of the bias whose other
+// columns are empty, so they are never offered to a list; the scans skip them through the status bytes.
 static int flat_rows_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, const void* d_queries, int qdtype, size_t nq,
                                size_t k, uint64_t* d_out_ids, float* d_out_dists, uint32_t* fallback_queries,
-                               uint32_t max_kc) {
+                               uint32_t max_kc, const uint32_t* row_bits = nullptr, const uint8_t* row_status = nullptr) {
     if (fallback_queries) *fallback_queries = 0;
     if (nq == 0) return 0;
     cudaStream_t stream = sc->stream;
@@ -1026,7 +1114,8 @@ static int flat_rows_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, con
                           flat_rescore_smem<OP_L2F>(query_stride(ix->dim)) <= kSmemOptInMax;
     if (!int_gemm && !f16_gemm) {   // shapes outside the GEMM paths: the exact scan
         if (fallback_queries) *fallback_queries = uint32_t(nq);
-        return search_on_device(ix, rep, sc, d_queries, qdtype, nq, k, k, k, d_out_ids, 8, d_out_dists, stream, true);
+        return search_on_device(ix, rep, sc, d_queries, qdtype, nq, k, k, k, d_out_ids, 8, d_out_dists, stream, true,
+                                row_status);
     }
     const uint32_t n = uint32_t(ix->n), dim = uint32_t(ix->dim);
     const int kind = !int_gemm ? FLAT_F16 : ix->dtype == SVSB200_I8 ? FLAT_S8 : FLAT_U8;
@@ -1037,6 +1126,16 @@ static int flat_rows_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, con
     if (ix->slot_mask && kind == FLAT_F16)
         if (int rc = ensure_slots_xmax(ix, rep, stream)) return rc;
     const Replica::FlatBase& base = kind == FLAT_F16 ? rep->flat_f16 : rep->flat_int;
+    const void* bias = base.bias.ptr;
+    if (row_bits) {
+        CUDA_TRY(sc->flt_bias.ensure(size_t(ntiles) * FLAT_BN));
+        const unsigned grid = unsigned(std::min<size_t>((size_t(ntiles) * FLAT_BN + 255) / 256, size_t(rep->sm_count) * 8));
+        flat_mask_bias_kernel<<<grid, 256, 0, stream>>>(reinterpret_cast<const uint32_t*>(base.bias.ptr), row_bits, n,
+                                                         ntiles * FLAT_BN, flat_empty_bias(kind), sc->flt_bias.ptr);
+        count_launch();
+        CUDA_TRY(cudaGetLastError());
+        bias = sc->flt_bias.ptr;
+    }
     // one CTA per SM over equal runs of output tiles; `nsplit` = candidate lists per query (flat_plan)
     uint32_t flat_ctas = 1, flat_share = 1, nsplit = 2;
     flat_plan(mtiles, ntiles, uint32_t(rep->sm_count), kc, &flat_ctas, &flat_share, &nsplit);
@@ -1051,8 +1150,9 @@ static int flat_rows_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, con
     // (query norms: the fp16 path's error bound only)
     CUDA_TRY(flat_tile_rows(kind, qdtype, d_queries, uint32_t(qrow), uint32_t(nq), dim, 128, 0, sc->flat_a.ptr, nullptr,
                             kind == FLAT_F16 ? sc->flat_qnorm.ptr : nullptr, nullptr, stream));
-    CUDA_TRY(flat_gemm_topk(kind, kc, sc->flat_a.ptr, base.tiles.ptr, base.bias.ptr, KB, ntiles, mtiles, flat_ctas, flat_share, nsplit,
-                            l2 ? -2.0f : -1.0f, sc->flat_ckey.ptr, sc->flat_cid.ptr, sc->flat_progress.ptr, stream));
+    CUDA_TRY(flat_gemm_topk(kind, kc, sc->flat_a.ptr, base.tiles.ptr, bias, KB, ntiles, mtiles, flat_ctas, flat_share, nsplit,
+                            l2 ? -2.0f : -1.0f, sc->flat_ckey.ptr, sc->flat_cid.ptr, sc->flat_progress.ptr, stream,
+                            row_bits != nullptr));
     // exact re-scoring with the search path's distance code: prepared queries as for a search
     if (int rc = prepare_queries(ix, rep, sc, d_queries, qdtype, nq, int_gemm ? PREP_INT : PREP_FLOAT, stream)) return rc;
     SearchParams p{};
@@ -1083,7 +1183,8 @@ static int flat_rows_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, con
         CUDA_TRY(sc->flat_i2.ensure(size_t(nunv) * k));
         CUDA_TRY(sc->flat_d2.ensure(size_t(nunv) * k));
         CUDA_TRY(flat_move_rows(d_queries, sc->flat_q2.ptr, sc->flat_unv.ptr + 1, sc->flat_unv.ptr, nunv, uint32_t(qrow), 0, stream));
-        int rc = search_on_device(ix, rep, sc, sc->flat_q2.ptr, qdtype, nunv, k, k, k, sc->flat_i2.ptr, 8, sc->flat_d2.ptr, stream, true);
+        int rc = search_on_device(ix, rep, sc, sc->flat_q2.ptr, qdtype, nunv, k, k, k, sc->flat_i2.ptr, 8, sc->flat_d2.ptr, stream, true,
+                                  row_status);
         if (rc) return rc;
         CUDA_TRY(flat_move_rows(sc->flat_i2.ptr, d_out_ids, sc->flat_unv.ptr + 1, sc->flat_unv.ptr, nunv, uint32_t(k * 8), 1, stream));
         CUDA_TRY(flat_move_rows(sc->flat_d2.ptr, d_out_dists, sc->flat_unv.ptr + 1, sc->flat_unv.ptr, nunv, uint32_t(k * 4), 1, stream));
@@ -1100,6 +1201,82 @@ static int flat_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, const vo
         CUDA_TRY(slots_to_external(d_out_ids, nq * k, rep->d_ext_ids.ptr, sc->stream));
         CUDA_TRY(cudaEventRecord(sc->ev_done, sc->stream));   // (a mutation waits for it: dynamic_flat.cu, on_stream)
     }
+    return 0;
+}
+
+// ---- filtered search (include/svsb200.h, svsb200_flat_index_search_filtered) ----
+// Route of a filtered search with `allowed` of `n` rows allowed (svsb200_flat_filter_plan): at most n / FLAT_SPARSE_DIV
+// allowed rows are gathered and scanned alone (the sparse route), more run the index's own routing with the disallowed
+// rows masked out (the dense route).  DESIGN.md §9d has the measurement behind the divisor.
+constexpr size_t FLAT_SPARSE_DIV = 64;
+static int flat_filter_route(size_t n, size_t allowed) {
+    return allowed * FLAT_SPARSE_DIV <= n ? SVSB200_FLAT_ROUTE_SPARSE : SVSB200_FLAT_ROUTE_DENSE;
+}
+
+// The filtered search on device buffers, enqueued on sc->stream apart from one synchronisation for the count of allowed
+// rows (and the dense route's own).  Ids are external ids for a dynamic flat index.
+static int flat_filtered_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, const void* d_queries, int qdtype, size_t nq,
+                                   size_t k, const uint32_t* d_bitmap, uint64_t* d_out_ids, float* d_out_dists,
+                                   size_t* out_allowed, uint32_t* fallback_queries) {
+    if (fallback_queries) *fallback_queries = 0;
+    cudaStream_t stream = sc->stream;
+    const uint32_t n = uint32_t(ix->n), words = (n + 31) / 32;
+    CUDA_TRY(sc->flt_status.ensure(std::max<size_t>(n, 1)));
+    CUDA_TRY(sc->flt_bits.ensure(std::max<size_t>(words, 1)));
+    CUDA_TRY(sc->flt_ids.ensure(size_t(n) + 1));   // [count][ids]
+    if (words) {
+        flat_filter_rows_kernel<<<(words + 7) / 8, 256, 0, stream>>>(d_bitmap, ix->slot_mask ? rep->d_status.ptr : nullptr, n,
+                                                                   sc->flt_status.ptr, sc->flt_bits.ptr);
+        count_launch();
+    }
+    flat_compact_kernel<<<1, 1024, 0, stream>>>(sc->flt_bits.ptr, words, sc->flt_ids.ptr + 1, sc->flt_ids.ptr);
+    count_launch();
+    CUDA_TRY(cudaGetLastError());
+    uint32_t allowed = 0;
+    CUDA_TRY(cudaMemcpyAsync(&allowed, sc->flt_ids.ptr, 4, cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaStreamSynchronize(stream));
+    if (out_allowed) *out_allowed = allowed;
+    if (nq == 0) return 0;
+    const uint32_t max_kc = FLAT_KC_DEEP;   // (the Flat handle's and the dynamic flat index's deepest lists)
+    const uint64_t* ext_ids = ix->slot_mask ? rep->d_ext_ids.ptr : nullptr;
+    const unsigned grid = unsigned(std::min<size_t>((nq * k + 255) / 256, size_t(rep->sm_count) * 8));
+    if (allowed == 0) {
+        CUDA_TRY(cudaMemsetAsync(d_out_ids, 0xFF, nq * k * 8, stream));
+    } else if (flat_filter_route(n, allowed) == SVSB200_FLAT_ROUTE_SPARSE) {
+        // the allowed rows, gathered in ascending order, and the exact scan over them alone (ties by position == by
+        // row); the scratch lends them to a transient index on the same device for the call
+        const uint32_t* rows = sc->flt_ids.ptr + 1;
+        CUDA_TRY(sc->flt_rows.ensure(size_t(allowed) * ix->row_stride));
+        CUDA_TRY(flat_move_rows(rep->d_vectors.ptr, sc->flt_rows.ptr, rows, sc->flt_ids.ptr, allowed, ix->row_stride, 0, stream));
+        svsb200_index sub;
+        sub.dtype = ix->dtype;
+        sub.metric = ix->metric;
+        sub.storage = ix->storage;
+        sub.n = allowed;
+        sub.dim = ix->dim;
+        sub.row_stride = ix->row_stride;
+        sub.gstride = 32;
+        Replica subrep;
+        subrep.device = rep->device;
+        subrep.sm_count = rep->sm_count;
+        subrep.d_vectors = std::move(sc->flt_rows);
+        const int rc = search_on_device(&sub, &subrep, sc, d_queries, qdtype, nq, k, k, k, d_out_ids, 8, d_out_dists, stream,
+                                        true);
+        sc->flt_rows = std::move(subrep.d_vectors);
+        if (rc) return rc;
+        if (fallback_queries) *fallback_queries = uint32_t(nq);
+        flat_unmap_ids_kernel<<<grid, 256, 0, stream>>>(d_out_ids, nq * k, rows, ext_ids);
+        count_launch();
+    } else {
+        if (int rc = flat_rows_on_device(ix, rep, sc, d_queries, qdtype, nq, k, d_out_ids, d_out_dists, fallback_queries, max_kc,
+                                         sc->flt_bits.ptr, sc->flt_status.ptr))
+            return rc;
+        if (ext_ids) CUDA_TRY(slots_to_external(d_out_ids, nq * k, ext_ids, stream));
+    }
+    flat_pad_inf_kernel<<<grid, 256, 0, stream>>>(d_out_ids, d_out_dists, nq * k);
+    count_launch();
+    CUDA_TRY(cudaGetLastError());
+    if (ix->slot_mask) CUDA_TRY(cudaEventRecord(sc->ev_done, stream));   // (a mutation waits for it)
     return 0;
 }
 
@@ -1238,7 +1415,91 @@ int svsb200::flat_search_host(const char* who, svsb200_index* ix, const void* qu
     return rc;
 }
 
+// The checks of both filtered forms: the arguments, and the query types the unfiltered search takes (an empty mask
+// would otherwise let any query type through).
+static int flat_filtered_check(const std::string& w, svsb200_index* ix, const void* bitmap, int qdtype, size_t k) {
+    if (!ix) return fail(w + ": NULL index");
+    if (!bitmap) return fail(w + ": NULL bitmap");
+    if (k == 0 || k > 1024) return fail(w + ": k must be in [1, 1024]");
+    if (qdtype < SVSB200_F32 || qdtype > SVSB200_U8) return fail("bad query dtype");
+    if (ix->dynamic) return fail(w + ": flat search is not available on a dynamic index");
+    const bool int_rows = ix->dtype == SVSB200_I8 || ix->dtype == SVSB200_U8;
+    if ((qdtype == SVSB200_I8 || qdtype == SVSB200_U8) && qdtype != ix->dtype)
+        return fail(w + ": int8/uint8 queries need rows of the same type");
+    if (qdtype == SVSB200_F16 && int_rows) return fail(w + ": float16 queries need float32/float16 rows");
+    return 0;
+}
+
+int svsb200::flat_search_filtered_device(const char* who, svsb200_index* ix, const void* d_queries, int qdtype, size_t nq,
+                                         size_t k, const uint32_t* d_bitmap, uint64_t* d_out_ids, float* d_out_dists,
+                                         void* stream_, size_t* out_allowed, uint32_t* fallback_queries) {
+    const std::string w(who);
+    if (int rc = flat_filtered_check(w, ix, d_bitmap, qdtype, k)) return rc;
+    if (nq && (!d_queries || !d_out_ids || !d_out_dists)) return fail(w + ": NULL buffer");
+    if (ix->reps.size() != 1) return fail(w + ": the index must live on exactly one device");
+    Replica* rep = ix->reps[0].get();
+    CUDA_TRY(cudaSetDevice(rep->device));
+    std::string err;
+    Scratch* sc = scratch_for_stream(rep, static_cast<cudaStream_t>(stream_), &err);
+    if (!sc) return fail(err);
+    return flat_filtered_on_device(ix, rep, sc, d_queries, qdtype, nq, k, d_bitmap, d_out_ids, d_out_dists, out_allowed,
+                                   fallback_queries);
+}
+
+int svsb200::flat_search_filtered_host(const char* who, svsb200_index* ix, const void* queries, int qdtype, size_t nq, size_t k,
+                                       const uint32_t* bitmap, uint64_t* out_ids, float* out_dists, size_t* out_allowed) {
+    const std::string w(who);
+    if (int rc = flat_filtered_check(w, ix, bitmap, qdtype, k)) return rc;
+    if (nq && (!queries || !out_ids || !out_dists)) return fail(w + ": NULL buffer");
+    Replica* rep = ix->reps[0].get();
+    CUDA_TRY(cudaSetDevice(rep->device));
+    std::string err;
+    Scratch* sc = acquire(rep, &err);
+    if (!sc) return fail(err);
+    const int rc = [&]() -> int {
+        const size_t qbytes = nq * ix->dim * esize(qdtype), words = (ix->n + 31) / 32;
+        CUDA_TRY(sc->q_raw.ensure(std::max<size_t>(qbytes, 1)));
+        CUDA_TRY(sc->ids.ensure(std::max<size_t>(nq * k * 8, 1)));
+        CUDA_TRY(sc->dists.ensure(std::max<size_t>(nq * k, 1)));
+        CUDA_TRY(sc->flt_in.ensure(std::max<size_t>(words, 1)));
+        CUDA_TRY(cudaMemcpyAsync(sc->flt_in.ptr, bitmap, words * 4, cudaMemcpyHostToDevice, sc->stream));
+        if (qbytes) CUDA_TRY(cudaMemcpyAsync(sc->q_raw.ptr, queries, qbytes, cudaMemcpyHostToDevice, sc->stream));
+        if (int rc = flat_filtered_on_device(ix, rep, sc, sc->q_raw.ptr, qdtype, nq, k, sc->flt_in.ptr,
+                                             reinterpret_cast<uint64_t*>(sc->ids.ptr), sc->dists.ptr, out_allowed, nullptr))
+            return rc;
+        if (nq) {
+            CUDA_TRY(cudaMemcpyAsync(out_ids, sc->ids.ptr, nq * k * 8, cudaMemcpyDeviceToHost, sc->stream));
+            CUDA_TRY(cudaMemcpyAsync(out_dists, sc->dists.ptr, nq * k * 4, cudaMemcpyDeviceToHost, sc->stream));
+        }
+        CUDA_TRY(cudaStreamSynchronize(sc->stream));
+        return 0;
+    }();
+    release(rep, sc);
+    return rc;
+}
+
 extern "C" {
+
+int svsb200_flat_filter_plan(size_t n, size_t allowed, int* route) {
+    if (!route) return fail("svsb200_flat_filter_plan: NULL output");
+    if (allowed > n) return fail("svsb200_flat_filter_plan: more allowed rows than rows");
+    *route = flat_filter_route(n, allowed);
+    return 0;
+}
+
+int svsb200_flat_index_search_filtered_device(svsb200_flat* index, const void* d_queries, int qdtype, size_t nq, size_t k,
+                                              const uint32_t* d_id_bitmap, uint64_t* d_out_ids, float* d_out_dists,
+                                              void* stream, size_t* out_allowed, uint32_t* fallback_queries) {
+    return flat_search_filtered_device("svsb200_flat_index_search_filtered_device", index ? index->ix.get() : nullptr,
+                                       d_queries, qdtype, nq, k, d_id_bitmap, d_out_ids, d_out_dists, stream, out_allowed,
+                                       fallback_queries);
+}
+
+int svsb200_flat_index_search_filtered(svsb200_flat* index, const void* queries, int qdtype, size_t nq, size_t k,
+                                       const uint32_t* id_bitmap, uint64_t* out_ids, float* out_dists, size_t* out_allowed) {
+    return flat_search_filtered_host("svsb200_flat_index_search_filtered", index ? index->ix.get() : nullptr, queries, qdtype,
+                                     nq, k, id_bitmap, out_ids, out_dists, out_allowed);
+}
 
 // How svsb200_flat_search* splits a problem (include/svsb200.h): host arithmetic only, so that the work split -- which the
 // kernel recomputes from the same inline functions -- can be checked without a device (tests/test_flat_plan.py).

@@ -127,7 +127,11 @@ struct Scratch {
     DeviceBuffer<uint32_t> flat_cid, flat_unv;         // candidates, unverified list (+ its counter in slot 0)
     DeviceBuffer<uint32_t> flat_progress;              // per CTA of the flat GEMM: tiles started (keeps row groups in step)
     DeviceBuffer<uint64_t> flat_i2;
-    DeviceBuffer<uint32_t> dyn_ovf, dyn_qlist;         // dynamic search: overflowed queries, the list being re-run
+    // filtered flat search, per call: the caller's bitmap (host form), each row's status (Valid = allowed), the allowed
+    // rows as a bitmap, their ids compacted (count first), the bias with every other column empty, the gathered rows
+    DeviceBuffer<uint32_t> flt_in, flt_bits, flt_ids, flt_bias;
+    DeviceBuffer<unsigned char> flt_status, flt_rows;
+    DeviceBuffer<uint32_t> dyn_ovf, dyn_qlist;        // dynamic search: overflowed queries, the list being re-run
     bool dyn_slot_ids = false;                         // dynamic search: write slots, not external ids (filtered / range)
     int (*cancel_fn)(void*) = nullptr;                 // the caller's cancellation predicate while a search runs
     void* cancel_arg = nullptr;
@@ -302,10 +306,11 @@ int prepare_queries(const svsb200_index* ix, const Replica* rep, Scratch* sc, co
                     int mode, cudaStream_t stream);
 
 // Shared body of every graph-search entry point: everything on one device, enqueued on `stream`.  `exhaustive`
-// scans every base row instead of walking the graph.
+// scans every base row instead of walking the graph; with `row_status` (one byte per row, the filtered flat search's)
+// it scans only the rows whose byte is SLOT_VALID, which replaces a dynamic flat index's own slot status.
 int search_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, const void* d_queries, int qdtype, size_t nq, size_t k,
                      size_t window, size_t capacity, void* d_out_ids, int id_bytes, float* d_out_dists, cudaStream_t stream,
-                     bool exhaustive = false);
+                     bool exhaustive = false, const uint8_t* row_status = nullptr);
 
 // ---- graph construction (build.cu), shared by svsb200_build_vamana and the dynamic index ----
 // A float32 / float16 / int8 / uint8 graph (the dynamic index: float32 / float16) on the current device: n rows
@@ -369,6 +374,13 @@ int flat_search_device(const char* who, svsb200_index* ix, const void* d_queries
                        uint64_t* d_out_ids, float* d_out_dists, void* stream, uint32_t* fallback_queries, uint32_t max_kc);
 int flat_search_host(const char* who, svsb200_index* ix, const void* queries, int qdtype, size_t nq, size_t k,
                      uint64_t* out_ids, float* out_dists, uint32_t max_kc);
+// The filtered flat search (svsb200_flat_index_search_filtered): `bitmap` over the rows (a dynamic flat index: over
+// the slots, Empty slots' bits ignored), in device memory for the device form and in host memory for the host form.
+int flat_search_filtered_device(const char* who, svsb200_index* ix, const void* d_queries, int qdtype, size_t nq, size_t k,
+                                const uint32_t* d_bitmap, uint64_t* d_out_ids, float* d_out_dists, void* stream,
+                                size_t* out_allowed, uint32_t* fallback_queries);
+int flat_search_filtered_host(const char* who, svsb200_index* ix, const void* queries, int qdtype, size_t nq, size_t k,
+                              const uint32_t* bitmap, uint64_t* out_ids, float* out_dists, size_t* out_allowed);
 // Deepest list of the Flat handles' searches (k <= 121 on the GEMM).
 uint32_t flat_max_kc_deep();
 // Incremental upkeep of a dynamic flat index's GEMM operands, for every operand kind already built (nothing before the

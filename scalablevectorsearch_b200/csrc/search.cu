@@ -506,7 +506,7 @@ static int search_dynamic(svsb200_index* ix, Replica* rep, Scratch* sc, SearchPa
 
 int search_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, const void* d_queries, int qdtype, size_t nq, size_t k,
                      size_t window, size_t capacity, void* d_out_ids, int id_bytes, float* d_out_dists, cudaStream_t stream,
-                     bool exhaustive) {
+                     bool exhaustive, const uint8_t* row_status) {
     if (id_bytes != 4 && id_bytes != 8) return fail("id_bytes must be 4 or 8");
     if (qdtype < SVSB200_F32 || qdtype > SVSB200_U8) return fail("bad query dtype");
     if (ix->dynamic && id_bytes != 8) return fail("a dynamic index returns 64-bit external ids: id_bytes must be 8");
@@ -534,6 +534,7 @@ int search_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, const void* d
 
     SearchParams p = search_params(ix, rep, sc, nq, k, window, capacity, d_out_ids, id_bytes, d_out_dists, exhaustive);
     if (exhaustive && ix->slot_mask) p.status = rep->d_status.ptr;   // dynamic flat index: the Valid slots only
+    if (exhaustive && row_status) p.status = row_status;             // filtered flat search: the allowed rows only
     LaunchConfig cfg{};
     bool use_fast = false;
     if (int rc = choose_launch(ix, rep, &p, exhaustive, stream, &cfg, &use_fast)) return rc;

@@ -160,3 +160,21 @@ class DynamicFlat:
                                                                 int(n_neighbors), d_ids, d_dists, stream or None,
                                                                 C.byref(fb)))
         return int(fb.value)
+
+    def search_filtered(self, queries: np.ndarray, n_neighbors: int, allowed: np.ndarray, with_counts: bool = False):
+        """``search`` with a predicate over the data index (dynamic_flat.h:513-573): ``allowed`` is a boolean mask over
+        the slots, in :meth:`export` order; Empty slots' entries are ignored.  Returns (external ids, distances, found
+        per query = min(k, allowed Valid slots)); ties by slot, short rows padded with 2^64 - 1 / +inf for every
+        metric.  ``with_counts`` adds the number of allowed Valid slots."""
+        return _lib._flat_search_filtered(self._lib.svsb200_dynamic_flat_search_filtered, self._h, self.dimensions,
+                                          queries, n_neighbors, _lib._bitmap(allowed, self.num_slots), with_counts)
+
+    def search_filtered_device(self, d_queries: int, qdtype: np.dtype, nq: int, n_neighbors: int, d_bitmap: int,
+                               d_ids: int, d_dists: int, stream: int = 0) -> int:
+        """Device-buffer form of :meth:`search_filtered` (raw pointers; the uint32 bitmap has (num_slots + 31) / 32
+        words, bit i = slot i); returns how many queries ran on a scan.  A mutation may follow it at once."""
+        fb = C.c_uint32()
+        _lib.check(self._lib.svsb200_dynamic_flat_search_filtered_device(
+            self._h, d_queries, _DTYPE_CODE[np.dtype(qdtype)], nq, int(n_neighbors), d_bitmap, d_ids, d_dists,
+            stream or None, None, C.byref(fb)))
+        return int(fb.value)

@@ -26,7 +26,8 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from .ivf import Clustering, IVFSearchParameters, _bitmap, _search_filtered, _sq_codes
+from ._lib import _bitmap
+from .ivf import Clustering, IVFSearchParameters, _search_filtered, _sq_codes
 from .vamana import _DTYPE_CODE, DistanceType
 
 

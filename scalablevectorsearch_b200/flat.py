@@ -86,3 +86,29 @@ class Flat:
                                                               int(n_neighbors), d_ids, d_dists, stream or None,
                                                               C.byref(fb)))
         return int(fb.value)
+
+    def search_filtered(self, queries: np.ndarray, n_neighbors: int, allowed: np.ndarray, with_counts: bool = False):
+        """``FlatIndex::search`` with a predicate (flat.h:421-465): ``allowed`` is a boolean mask over the ids.  Returns
+        (ids uint64 [nq,k], distances float32 [nq,k], found per query = min(k, allowed rows)): the exact top k over the
+        allowed rows, equal to :meth:`search` on a Flat of those rows with its ids mapped back; short rows are padded
+        with 2^64 - 1 / +inf for every metric.  ``with_counts`` adds the number of allowed rows."""
+        return _lib._flat_search_filtered(self._lib.svsb200_flat_index_search_filtered, self._h, self.dimensions,
+                                          queries, n_neighbors, _lib._bitmap(allowed, self.size), with_counts)
+
+    def search_filtered_device(self, d_queries: int, qdtype: np.dtype, nq: int, n_neighbors: int, d_bitmap: int,
+                               d_ids: int, d_dists: int, stream: int = 0) -> int:
+        """Device-buffer form of :meth:`search_filtered` (raw pointers; the uint32 bitmap has (size + 31) / 32 words,
+        bit i = id i); returns how many queries ran on a scan."""
+        fb = C.c_uint32()
+        _lib.check(self._lib.svsb200_flat_index_search_filtered_device(
+            self._h, d_queries, _DTYPE_CODE[np.dtype(qdtype)], nq, int(n_neighbors), d_bitmap, d_ids, d_dists,
+            stream or None, None, C.byref(fb)))
+        return int(fb.value)
+
+
+def filter_route(n: int, allowed: int) -> str:
+    """The route a filtered flat search takes with ``allowed`` of ``n`` rows allowed: "sparse" (the allowed rows are
+    gathered and scanned alone) or "dense" (the index's own routing with the other rows masked)."""
+    route = C.c_int()
+    _lib.check(_lib.lib().svsb200_flat_filter_plan(int(n), int(allowed), C.byref(route)))
+    return "sparse" if route.value == 1 else "dense"

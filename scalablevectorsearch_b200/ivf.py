@@ -22,6 +22,7 @@ from dataclasses import dataclass
 import numpy as np
 
 from . import _lib
+from ._lib import _bitmap
 from .vamana import _DTYPE_CODE, DistanceType
 
 
@@ -71,15 +72,6 @@ def sq_compress(data, dtype=np.int8, device: int = 0):
     _lib.check(_lib.lib().svsb200_sq_compress(x.ctypes.data, x.shape[0], x.shape[1], _DTYPE_CODE[dtype], int(device),
                                               codes.ctypes.data, C.byref(scale), C.byref(bias)))
     return codes, float(np.float32(scale.value)), float(np.float32(bias.value))
-
-
-def _bitmap(allowed, n: int) -> np.ndarray:
-    """A boolean mask of n entries -> the uint32 bitmap of the filtered searches ((n + 31) / 32 words)."""
-    mask = np.ascontiguousarray(allowed, dtype=bool)
-    if mask.shape != (n,):
-        raise ValueError(f"allowed must hold {n} booleans")
-    b = np.packbits(mask, bitorder="little")
-    return np.concatenate([b, np.zeros((-len(b)) % 4, dtype=np.uint8)]).view(np.uint32)
 
 
 def _search_filtered(fn, h, dims: int, queries, n_neighbors: int, n_probes: int, bitmap: np.ndarray, with_counts: bool):
