@@ -8,6 +8,8 @@ from __future__ import annotations
 import ctypes as C
 import os
 
+import numpy as np
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 # SVSB200_LIB lets experiments point at an alternative build; the default is the in-tree library.
 LIB_PATH = os.environ.get("SVSB200_LIB") or os.path.join(_HERE, "libsvsb200.so")
@@ -49,6 +51,8 @@ SYMBOLS = [
 ]
 
 _lib = None
+#: the C ABI's element-type codes (SVSB200_F32 .. SVSB200_U8)
+_DTYPE_CODE = {np.dtype(np.float32): 0, np.dtype(np.float16): 1, np.dtype(np.int8): 2, np.dtype(np.uint8): 3}
 #: the cancellation predicate of svsb200_search_cancellable: int (*)(void*)
 CANCEL_FN = C.CFUNCTYPE(C.c_int, C.c_void_p)
 
@@ -190,8 +194,6 @@ def check(rc: int) -> None:
 
 def _bitmap(allowed, n: int):
     """A boolean mask of n entries -> the uint32 bitmap of the filtered searches ((n + 31) / 32 words)."""
-    import numpy as np
-
     mask = np.ascontiguousarray(allowed, dtype=bool)
     if mask.shape != (n,):
         raise ValueError(f"allowed must hold {n} booleans")
@@ -199,12 +201,52 @@ def _bitmap(allowed, n: int):
     return np.concatenate([b, np.zeros((-len(b)) % 4, dtype=np.uint8)]).view(np.uint32)
 
 
+class _Slots:
+    """``has_id``, ``all_ids``, ``delete`` and the argument checks of ``add``, shared by the dynamic indexes over their
+    C functions ``{_ABI}_has_id``, ``_ids``, ``_delete`` and ``_add``."""
+
+    _ABI = ""
+
+    def _fn(self, name: str):
+        return getattr(self._lib, f"{self._ABI}_{name}")
+
+    def has_id(self, id: int) -> bool:
+        out = C.c_int()
+        check(self._fn("has_id")(self._h, int(id), C.byref(out)))
+        return bool(out.value)
+
+    def all_ids(self):
+        """External ids of every Valid slot, in slot order."""
+        n = C.c_size_t(self.size)
+        out = np.empty(n.value, dtype=np.uint64)
+        check(self._fn("ids")(self._h, out.ctypes.data, C.byref(n)))
+        return out[: n.value]
+
+    def delete(self, ids) -> int:
+        """Deletes the entries of these external ids (what becomes of their slots: the class's docstring).  Fails
+        without changing anything unless every id is present, once.  Returns the number of deleted entries."""
+        ids = np.ascontiguousarray(np.atleast_1d(ids), dtype=np.uint64)
+        check(self._fn("delete")(self._h, ids.ctypes.data, len(ids)))
+        return len(ids)
+
+    def _add(self, points, ids, reuse_empty: bool):
+        """The body of ``add``: rows [count, dimensions] with one new external id each; returns the slots used."""
+        pts = np.ascontiguousarray(points)
+        ids = np.ascontiguousarray(np.atleast_1d(ids), dtype=np.uint64)
+        if pts.ndim != 2 or pts.shape[1] != self.dimensions:
+            raise ValueError(f"points must be [count, {self.dimensions}]")
+        if pts.shape[0] != len(ids):
+            raise ValueError(f"Number of points ({pts.shape[0]}) not equal to the number of external ids ({len(ids)})!")
+        if pts.dtype not in _DTYPE_CODE:
+            raise TypeError(f"unsupported data type {pts.dtype}")
+        slots = np.empty(len(ids), dtype=np.uint64)
+        check(self._fn("add")(self._h, pts.ctypes.data, _DTYPE_CODE[pts.dtype], len(ids), ids.ctypes.data,
+                              int(bool(reuse_empty)), slots.ctypes.data))
+        return slots
+
+
 def _flat_search_filtered(fn, h, dims: int, queries, n_neighbors: int, bitmap, with_counts: bool):
     """The host form of the Flat and DynamicFlat filtered searches: (ids, dists, found[, allowed rows])."""
-    import numpy as np
-
-    from .vamana import _DTYPE_CODE
-
     q = np.ascontiguousarray(queries)
     if q.ndim != 2 or q.shape[1] != dims:
         raise ValueError(f"queries must be [nq, {dims}]")

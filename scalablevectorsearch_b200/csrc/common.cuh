@@ -11,6 +11,7 @@
 #include <type_traits>
 
 #include "../../include/svsb200.h"
+#include "slots.h"   // SlotStatus
 
 namespace svsb200 {
 
@@ -85,8 +86,6 @@ struct SearchParams {
     const uint32_t* qlist;       // optional: run only these queries (a re-run of overflowed ones)
 };
 
-// SlotMetadata of the reference's MutableVamanaIndex (index/vamana/dynamic_index.h:60-79).
-enum SlotStatus : uint8_t { SLOT_EMPTY = 0, SLOT_VALID = 1, SLOT_DELETED = 2 };
 constexpr uint32_t kInvalidBit = 0x40000000u;   // MUT kernels: PredicatedSearchNeighbor::valid() == false, packed into the id
 
 struct LaunchConfig {

@@ -1,23 +1,17 @@
 // dynamic.cu -- the dynamic (mutable) Vamana index of the C ABI: MutableVamanaIndex
 // (index/vamana/dynamic_index.h) built or assembled from a graph, data and external ids, with insertion, soft
 // deletion, consolidation and compaction.  Every slot has a status (Valid / Deleted / Empty) and an external id in
-// HBM; the external -> slot translator (core/translation.h) lives on the host.  Searches go through svsb200_search*
-// and run the lean kernel's MutableBuffer form (search_fast.cuh, MUT = true); insertion runs the graph builder over
-// the new slots (build.cu), consolidation its prune kernel over pools selected by consolidate_pool_kernel.
+// HBM; the external -> slot translator (core/translation.h) lives on the host, and the slot rules are slots.h's.
+// Searches go through svsb200_search* and run the lean kernel's MutableBuffer form (search_fast.cuh, MUT = true);
+// insertion runs the graph builder over the new slots (build.cu), consolidation its prune kernel over pools selected by
+// consolidate_pool_kernel.
 #include "build_kernels.cuh"
 #include "host.cuh"
 
 #include <algorithm>
 #include <cmath>
-#include <unordered_set>
 
 namespace svsb200 {
-
-// status[slots[i]] = value
-__global__ void set_status_kernel(const uint32_t* __restrict__ slots, uint32_t count, uint8_t value, uint8_t* __restrict__ status) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < count) status[slots[i]] = value;
-}
 
 static int check_dynamic(const svsb200_index* ix, const char* who) {
     if (!ix) return fail(std::string(who) + ": NULL index");
@@ -36,15 +30,6 @@ __global__ void place_rows_kernel(const uint4* __restrict__ src, const uint32_t*
     const size_t s = slots[i], words = row_stride / 16;
     for (size_t j = lane; j < words; j += 32) vectors[s * words + j] = src[i * words + j];
     for (uint32_t j = lane; j < gstride; j += 32) graph[s * gstride + j] = kNoNeighbor;
-}
-
-// status[slots[i]] = Valid, ext_ids[slots[i]] = ids[i]
-__global__ void mark_added_kernel(const uint32_t* __restrict__ slots, const uint64_t* __restrict__ ids, uint32_t count,
-                                  uint8_t* __restrict__ status, uint64_t* __restrict__ ext_ids) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= count) return;
-    status[slots[i]] = SLOT_VALID;
-    ext_ids[slots[i]] = ids[i];
 }
 
 __global__ void deleted_to_empty_kernel(uint8_t* __restrict__ status, uint32_t n) {
@@ -136,18 +121,6 @@ static GraphBuild graph_build(const svsb200_index* ix, Replica* rep, uint32_t* d
     return b;
 }
 
-// Runs `body(stream)` on a scratch stream of the index's device.
-template <typename F> static int on_stream(svsb200_index* ix, F body) {
-    Replica* rep = ix->reps[0].get();
-    CUDA_TRY(cudaSetDevice(rep->device));
-    std::string err;
-    Scratch* sc = acquire(rep, &err);
-    if (!sc) return fail(err);
-    const int rc = body(rep, sc->stream);
-    release(rep, sc);
-    return rc;
-}
-
 }  // namespace svsb200
 
 using namespace svsb200;
@@ -157,6 +130,7 @@ extern "C" {
 int svsb200_dynamic_create(const void* vectors, int dtype, size_t n, size_t dim, const uint32_t* graph_rows,
                            size_t graph_row_len, uint32_t entry_point, int metric, const uint64_t* external_ids, int device,
                            svsb200_index** out) {
+    const char* who = "svsb200_dynamic_create";
     if (!out) return fail("svsb200_dynamic_create: NULL output");
     *out = nullptr;
     if (n && !external_ids) return fail("svsb200_dynamic_create: NULL external ids");
@@ -164,32 +138,20 @@ int svsb200_dynamic_create(const void* vectors, int dtype, size_t n, size_t dim,
     if (graph_row_len < 2 || graph_row_len - 1 > 32u * kFastMaxGW)
         return fail("svsb200_dynamic_create: graph_max_degree must be in [1, 128]");
     if (n >= (size_t(1) << 30)) return fail("svsb200_dynamic_create: at most 2^30 - 1 slots");
-    // IDTranslator::insert (core/translation.h:105-127)
-    std::unordered_map<uint64_t, uint32_t> translator;
-    translator.reserve(n);
-    for (size_t i = 0; i < n; ++i)
-        if (external_ids[i] == ~uint64_t(0))   // (marks the padding of short result rows)
-            return fail("svsb200_dynamic_create: external id 2^64 - 1 is reserved");
-        else if (!translator.emplace(external_ids[i], uint32_t(i)).second)
-            return fail("svsb200_dynamic_create: External IDs contain repeat elements!");
+    SlotTable slots;
+    if (int rc = slots.assign(who, external_ids, n)) return rc;
     svsb200_index* ix = nullptr;
     if (int rc = svsb200_index_create(vectors, dtype, n, dim, 0, graph_rows, graph_row_len, entry_point, metric, SVSB200_PLAIN,
                                       nullptr, device, &ix))
         return rc;
     std::unique_ptr<svsb200_index, int (*)(svsb200_index*)> owner(ix, svsb200_index_destroy);
-    ix->status.assign(n, SLOT_VALID);
-    ix->ext_ids.assign(external_ids, external_ids + n);
-    ix->translator = std::move(translator);
+    ix->slots = std::move(slots);
     Replica* rep = ix->reps[0].get();
     CUDA_TRY(cudaSetDevice(rep->device));
-    CUDA_TRY(rep->d_status.ensure(std::max<size_t>(n, 1)));
-    CUDA_TRY(rep->d_ext_ids.ensure(std::max<size_t>(n, 1)));
-    CUDA_TRY(cudaMemcpy(rep->d_status.ptr, ix->status.data(), n, cudaMemcpyHostToDevice));
-    CUDA_TRY(cudaMemcpy(rep->d_ext_ids.ptr, ix->ext_ids.data(), n * sizeof(uint64_t), cudaMemcpyHostToDevice));
+    if (int rc = upload_slots(rep, ix->slots)) return rc;
     ix->device_bytes += n * (1 + sizeof(uint64_t));
     ix->dynamic = true;
-    ix->first_empty = n;
-    if (int rc = resolve_mutation_parameters("svsb200_dynamic_create", metric, ix->max_degree, &ix->dyn_alpha, &ix->dyn_window,
+    if (int rc = resolve_mutation_parameters(who, metric, ix->max_degree, &ix->dyn_alpha, &ix->dyn_window,
                                              &ix->dyn_max_candidates, &ix->dyn_prune_to))
         return rc;
     *out = owner.release();
@@ -199,64 +161,32 @@ int svsb200_dynamic_create(const void* vectors, int dtype, size_t n, size_t dim,
 int svsb200_dynamic_delete(svsb200_index* ix, const uint64_t* ids, size_t count) {
     if (int rc = check_dynamic(ix, "svsb200_dynamic_delete")) return rc;
     if (count && !ids) return fail("svsb200_dynamic_delete: NULL ids");
-    // translator_.check_external_exist (core/translation.h:395-407): nothing changes unless every id is present
     std::vector<uint32_t> slots;
-    slots.reserve(count);
-    std::unordered_set<uint64_t> seen;
-    for (size_t i = 0; i < count; ++i) {
-        auto it = ix->translator.find(ids[i]);
-        if (it == ix->translator.end() || !seen.insert(ids[i]).second)
-            return fail("svsb200_dynamic_delete: External ID " + std::to_string(ids[i]) + " does not exist!");
-        slots.push_back(it->second);
-    }
+    if (int rc = ix->slots.find("svsb200_dynamic_delete", ids, count, &slots)) return rc;
     if (count == 0) return 0;
-    Replica* rep = ix->reps[0].get();
-    CUDA_TRY(cudaSetDevice(rep->device));
-    std::string err;
-    Scratch* sc = acquire(rep, &err);
-    if (!sc) return fail(err);
-    // (mutations must not run concurrently with searches of the same index; once this stream is drained the new status
-    // is visible to every later search of it, whatever its stream)
-    auto run = [&]() -> int {
-        DeviceBuffer<uint32_t> d_slots;
-        CUDA_TRY(d_slots.ensure(count));
-        CUDA_TRY(cudaMemcpyAsync(d_slots.ptr, slots.data(), count * sizeof(uint32_t), cudaMemcpyHostToDevice, sc->stream));
-        set_status_kernel<<<unsigned((count + 255) / 256), 256, 0, sc->stream>>>(d_slots.ptr, uint32_t(count), SLOT_DELETED,
-                                                                                  rep->d_status.ptr);
-        count_launch();
-        CUDA_TRY(cudaGetLastError());
-        CUDA_TRY(cudaStreamSynchronize(sc->stream));
+    // (once this stream is drained the new status is visible to every later search of the index, whatever its stream)
+    int rc = after_searches(ix, [&](Replica* rep, cudaStream_t stream) -> int {
+        Replica::SlotStaging& st = rep->staging;
+        CUDA_TRY(st.slots.ensure(count));
+        CUDA_TRY(cudaMemcpyAsync(st.slots.ptr, slots.data(), count * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
+        CUDA_TRY(mark_slots(st.slots.ptr, nullptr, count, SLOT_DELETED, rep, stream));
+        CUDA_TRY(cudaStreamSynchronize(stream));
         return 0;
-    };
-    const int rc = run();
-    release(rep, sc);
+    });
     if (rc) return rc;
     // delete_entry + translator_.delete_external (dynamic_index.h:773-788)
-    for (size_t i = 0; i < count; ++i) {
-        ix->status[slots[i]] = SLOT_DELETED;
-        ix->translator.erase(ids[i]);
-    }
+    ix->slots.commit_delete(slots, ids, SLOT_DELETED);
     return 0;
 }
 
 int svsb200_dynamic_ids(const svsb200_index* ix, uint64_t* out_ids, size_t* count) {
     if (int rc = check_dynamic(ix, "svsb200_dynamic_ids")) return rc;
-    if (!count) return fail("svsb200_dynamic_ids: NULL count");
-    if (out_ids) {
-        if (*count < ix->translator.size()) return fail("svsb200_dynamic_ids: output too small");
-        size_t o = 0;
-        for (size_t s = 0; s < ix->status.size(); ++s)   // slot order
-            if (ix->status[s] == SLOT_VALID) out_ids[o++] = ix->ext_ids[s];
-    }
-    *count = ix->translator.size();
-    return 0;
+    return ix->slots.ids("svsb200_dynamic_ids", out_ids, count);
 }
 
 int svsb200_dynamic_has_id(const svsb200_index* ix, uint64_t id, int* out) {
     if (int rc = check_dynamic(ix, "svsb200_dynamic_has_id")) return rc;
-    if (!out) return fail("svsb200_dynamic_has_id: NULL output");
-    *out = ix->translator.count(id) ? 1 : 0;
-    return 0;
+    return ix->slots.has_id("svsb200_dynamic_has_id", id, out);
 }
 
 int svsb200_dynamic_export(const svsb200_index* ix, uint32_t* graph_rows_out, uint8_t* status_out, uint64_t* ext_ids_out,
@@ -278,8 +208,7 @@ int svsb200_dynamic_export(const svsb200_index* ix, uint32_t* graph_rows_out, ui
             for (size_t j = 0; j < R; ++j) o[1 + j] = j < d ? in[j] : 0u;
         }
     }
-    if (status_out) std::copy(ix->status.begin(), ix->status.end(), status_out);
-    if (ext_ids_out) std::copy(ix->ext_ids.begin(), ix->ext_ids.end(), ext_ids_out);
+    ix->slots.export_to(status_out, ext_ids_out);
     if (entry_point_out) *entry_point_out = ix->entry_point;
     return 0;
 }
@@ -314,61 +243,43 @@ int svsb200_dynamic_add(svsb200_index* ix, const void* vectors, int dtype, size_
     if (count == 0) return 0;
     if (!vectors || !ids) return fail("svsb200_dynamic_add: NULL argument");
     if (dtype != ix->dtype) return fail("svsb200_dynamic_add: the points' dtype differs from the index's");
-    // translator_.insert (core/translation.h:105-127), checked before anything changes
-    {
-        std::unordered_set<uint64_t> seen;
-        seen.reserve(count);
-        for (size_t i = 0; i < count; ++i) {
-            if (ids[i] == ~uint64_t(0)) return fail("svsb200_dynamic_add: external id 2^64 - 1 is reserved");
-            if (!seen.insert(ids[i]).second) return fail("svsb200_dynamic_add: External IDs contain repeat elements!");
-            if (ix->translator.count(ids[i]))
-                return fail("svsb200_dynamic_add: External ID " + std::to_string(ids[i]) + " already exists!");
-        }
-    }
+    if (int rc = ix->slots.check_new(who, ids, count)) return rc;
     // slots (add_points, dynamic_index.h:670-706): Empty ones from first_empty_ (from 0 with reuse_empty), then appended
     std::vector<uint32_t> slots;
-    slots.reserve(count);
-    for (size_t s = reuse_empty ? 0 : ix->first_empty; s < ix->status.size() && slots.size() < count; ++s)
-        if (ix->status[s] == SLOT_EMPTY) slots.push_back(uint32_t(s));
-    const size_t old_n = ix->n, new_n = old_n + (count - slots.size());
+    const size_t old_n = ix->n, new_n = ix->slots.choose(count, reuse_empty ? 0 : ix->slots.first_empty, &slots);
     if (new_n >= (size_t(1) << 30)) return fail("svsb200_dynamic_add: at most 2^30 - 1 slots");
-    for (size_t s = old_n; s < new_n; ++s) slots.push_back(uint32_t(s));
     {
         GraphBuild b;
         b = graph_build(ix, ix->reps[0].get(), nullptr, nullptr);
         b.n = new_n;
         if (int rc = check_construct(who, b)) return rc;
     }
-    int rc = on_stream(ix, [&](Replica* rep, cudaStream_t stream) -> int {
-        // geometric growth: many small calls do not copy the index each time
-        const size_t cap = rep->d_status.count;
-        if (new_n > cap) {
-            const size_t want = std::max(new_n, 2 * cap);
+    int rc = after_searches(ix, [&](Replica* rep, cudaStream_t stream) -> int {
+        if (const size_t cap = slot_capacity(rep, new_n)) {   // (these first: d_status's size is the capacity)
             CUDA_TRY(cudaStreamSynchronize(stream));
-            CUDA_TRY(grow(rep->d_vectors, old_n * ix->row_stride, want * ix->row_stride));
-            CUDA_TRY(grow(rep->d_graph, old_n * ix->gstride, want * ix->gstride));
-            CUDA_TRY(grow(rep->d_ref_degree, old_n, want));
-            CUDA_TRY(grow(rep->d_status, old_n, want));
-            CUDA_TRY(grow(rep->d_ext_ids, old_n, want));
-            ix->device_bytes = dynamic_bytes(ix, want);
+            CUDA_TRY(grow(rep->d_vectors, old_n * ix->row_stride, cap * ix->row_stride));
+            CUDA_TRY(grow(rep->d_graph, old_n * ix->gstride, cap * ix->gstride));
+            CUDA_TRY(grow(rep->d_ref_degree, old_n, cap));
+            if (int rc2 = grow_slots(rep, old_n, cap, stream)) return rc2;
+            ix->device_bytes = dynamic_bytes(ix, cap);
         }
+        // (the mirror grows before the graph is built: a failed construct_graph leaves edges to the new slots)
         ix->n = new_n;
-        ix->status.resize(new_n, SLOT_EMPTY);
-        ix->ext_ids.resize(new_n, 0);
-        DeviceBuffer<unsigned char> d_src;
-        DeviceBuffer<uint32_t> d_slots, d_deg;
-        DeviceBuffer<uint64_t> d_ids;
-        CUDA_TRY(d_src.ensure(count * ix->row_stride));
-        CUDA_TRY(d_slots.ensure(count));
-        CUDA_TRY(d_ids.ensure(count));
+        ix->slots.status.resize(new_n, SLOT_EMPTY);
+        ix->slots.ext_ids.resize(new_n, 0);
+        Replica::SlotStaging& st = rep->staging;
+        DeviceBuffer<uint32_t> d_deg;
+        CUDA_TRY(st.rows.ensure(count * ix->row_stride));
+        CUDA_TRY(st.slots.ensure(count));
+        CUDA_TRY(st.ids.ensure(count));
         CUDA_TRY(d_deg.ensure(new_n));
-        CUDA_TRY(cudaMemsetAsync(d_src.ptr, 0, count * ix->row_stride, stream));
+        CUDA_TRY(cudaMemsetAsync(st.rows.ptr, 0, count * ix->row_stride, stream));
         const size_t row_bytes = ix->dim * esize(ix->dtype);
-        CUDA_TRY(cudaMemcpy2DAsync(d_src.ptr, ix->row_stride, vectors, row_bytes, row_bytes, count, cudaMemcpyHostToDevice, stream));
-        CUDA_TRY(cudaMemcpyAsync(d_slots.ptr, slots.data(), count * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
-        CUDA_TRY(cudaMemcpyAsync(d_ids.ptr, ids, count * sizeof(uint64_t), cudaMemcpyHostToDevice, stream));
+        CUDA_TRY(cudaMemcpy2DAsync(st.rows.ptr, ix->row_stride, vectors, row_bytes, row_bytes, count, cudaMemcpyHostToDevice, stream));
+        CUDA_TRY(cudaMemcpyAsync(st.slots.ptr, slots.data(), count * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
+        CUDA_TRY(cudaMemcpyAsync(st.ids.ptr, ids, count * sizeof(uint64_t), cudaMemcpyHostToDevice, stream));
         place_rows_kernel<<<unsigned((count + 7) / 8), 256, 0, stream>>>(
-            reinterpret_cast<const uint4*>(d_src.ptr), d_slots.ptr, uint32_t(count), ix->row_stride,
+            reinterpret_cast<const uint4*>(st.rows.ptr), st.slots.ptr, uint32_t(count), ix->row_stride,
             reinterpret_cast<uint4*>(rep->d_vectors.ptr), rep->d_graph.ptr, ix->gstride);
         count_launch();
         CUDA_TRY(cudaGetLastError());
@@ -376,24 +287,16 @@ int svsb200_dynamic_add(svsb200_index* ix, const void* vectors, int dtype, size_
         if (int rc2 = row_degrees(b)) return rc2;
         // builder.construct(alpha_, entry_point(), slots) (dynamic_index.h:719-739): its greedy search ignores the slot
         // status, so Deleted slots are walked and may become neighbours of the new points, as in the reference
-        if (int rc2 = construct_graph(who, b, ix->dyn_alpha, ix->entry_point, d_slots.ptr, count)) return rc2;
+        if (int rc2 = construct_graph(who, b, ix->dyn_alpha, ix->entry_point, st.slots.ptr, count)) return rc2;
         ref_degree_kernel<<<unsigned((new_n + 255) / 256), 256, 0, stream>>>(d_deg.ptr, uint32_t(new_n), rep->d_ref_degree.ptr);
         count_launch();
-        mark_added_kernel<<<unsigned((count + 255) / 256), 256, 0, stream>>>(d_slots.ptr, d_ids.ptr, uint32_t(count),
-                                                                            rep->d_status.ptr, rep->d_ext_ids.ptr);
-        count_launch();
         CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(mark_slots(st.slots.ptr, st.ids.ptr, count, SLOT_VALID, rep, stream));
         CUDA_TRY(cudaStreamSynchronize(stream));
         return 0;
     });
     if (rc) return rc;
-    for (size_t i = 0; i < count; ++i) {
-        ix->status[slots[i]] = SLOT_VALID;
-        ix->ext_ids[slots[i]] = ids[i];
-        ix->translator.emplace(ids[i], slots[i]);
-        if (slots_out) slots_out[i] = slots[i];
-    }
-    ix->first_empty = std::max<size_t>(ix->first_empty, size_t(slots.back()) + 1);
+    ix->slots.commit_add(slots, ids, slots_out);
     return 0;
 }
 
@@ -401,12 +304,12 @@ int svsb200_dynamic_consolidate(svsb200_index* ix) {
     const char* who = "svsb200_dynamic_consolidate";
     if (int rc = check_dynamic(ix, who)) return rc;
     const size_t n = ix->n, R = ix->max_degree;
-    const size_t valid = ix->translator.size();
-    const bool replace_entry = ix->status[ix->entry_point] == SLOT_DELETED;
+    const size_t valid = ix->slots.size();
+    const bool replace_entry = ix->slots.status[ix->entry_point] == SLOT_DELETED;
     // (the reference would silently pick slot 0)
     if (replace_entry && valid == 0) return fail("svsb200_dynamic_consolidate: no Valid slot left for the entry point");
     uint32_t entry_point = ix->entry_point;
-    int rc = on_stream(ix, [&](Replica* rep, cudaStream_t stream) -> int {
+    int rc = after_searches(ix, [&](Replica* rep, cudaStream_t stream) -> int {
         DeviceBuffer<uint32_t> d_deg, d_nodes, d_count;
         CUDA_TRY(d_deg.ensure(n));
         CUDA_TRY(d_nodes.ensure(n));
@@ -495,7 +398,7 @@ int svsb200_dynamic_consolidate(svsb200_index* ix) {
     });
     if (rc) return rc;
     ix->entry_point = entry_point;
-    for (auto& st : ix->status)
+    for (auto& st : ix->slots.status)
         if (st == SLOT_DELETED) st = SLOT_EMPTY;
     return 0;
 }
@@ -504,23 +407,18 @@ int svsb200_dynamic_compact(svsb200_index* ix) {
     const char* who = "svsb200_dynamic_compact";
     if (int rc = check_dynamic(ix, who)) return rc;
     // (the reference throws from robin_map::at after it has already moved the data)
-    if (std::find(ix->status.begin(), ix->status.end(), uint8_t(SLOT_DELETED)) != ix->status.end())
+    if (std::find(ix->slots.status.begin(), ix->slots.status.end(), uint8_t(SLOT_DELETED)) != ix->slots.status.end())
         return fail("svsb200_dynamic_compact: the index holds Deleted slots; consolidate first");
     // nonmissing_indices (dynamic_index.h:800-809): the Valid slots, ascending
     const size_t n = ix->n;
-    std::vector<uint32_t> new_to_old, old_to_new(n, kNoNeighbor);
-    new_to_old.reserve(ix->translator.size());
-    for (size_t s = 0; s < n; ++s)
-        if (ix->status[s] == SLOT_VALID) {
-            old_to_new[s] = uint32_t(new_to_old.size());
-            new_to_old.push_back(uint32_t(s));
-        }
+    std::vector<uint64_t> ext;
+    const std::vector<uint32_t> new_to_old = ix->slots.valid_slots(&ext);
+    std::vector<uint32_t> old_to_new(n, kNoNeighbor);
+    for (size_t i = 0; i < new_to_old.size(); ++i) old_to_new[new_to_old[i]] = uint32_t(i);
     const size_t m = new_to_old.size();
     if (m == 0 || old_to_new[ix->entry_point] == kNoNeighbor)
         return fail("svsb200_dynamic_compact: the entry point is not Valid; consolidate first");
-    std::vector<uint64_t> ext(m);
-    for (size_t i = 0; i < m; ++i) ext[i] = ix->ext_ids[new_to_old[i]];
-    int rc = on_stream(ix, [&](Replica* rep, cudaStream_t stream) -> int {
+    int rc = after_searches(ix, [&](Replica* rep, cudaStream_t stream) -> int {
         DeviceBuffer<uint32_t> d_n2o, d_o2n, graph;
         DeviceBuffer<unsigned char> vectors;
         DeviceBuffer<uint16_t> refdeg;
@@ -531,12 +429,9 @@ int svsb200_dynamic_compact(svsb200_index* ix) {
         CUDA_TRY(vectors.ensure(m * ix->row_stride));
         CUDA_TRY(graph.ensure(m * ix->gstride));
         CUDA_TRY(refdeg.ensure(m));
-        CUDA_TRY(status.ensure(m));
-        CUDA_TRY(ext_ids.ensure(m));
         CUDA_TRY(cudaMemcpyAsync(d_n2o.ptr, new_to_old.data(), m * 4, cudaMemcpyHostToDevice, stream));
         CUDA_TRY(cudaMemcpyAsync(d_o2n.ptr, old_to_new.data(), n * 4, cudaMemcpyHostToDevice, stream));
-        CUDA_TRY(cudaMemcpyAsync(ext_ids.ptr, ext.data(), m * 8, cudaMemcpyHostToDevice, stream));
-        CUDA_TRY(cudaMemsetAsync(status.ptr, SLOT_VALID, m, stream));
+        if (int rc2 = compacted_slots(ext, m, &status, &ext_ids, stream)) return rc2;
         compact_kernel<<<unsigned((m + 7) / 8), 256, 0, stream>>>(
             d_n2o.ptr, d_o2n.ptr, uint32_t(m), ix->row_stride, ix->gstride, reinterpret_cast<const uint4*>(rep->d_vectors.ptr),
             rep->d_graph.ptr, rep->d_ref_degree.ptr, reinterpret_cast<uint4*>(vectors.ptr), graph.ptr, refdeg.ptr);
@@ -553,11 +448,8 @@ int svsb200_dynamic_compact(svsb200_index* ix) {
     if (rc) return rc;
     ix->n = m;
     ix->device_bytes = dynamic_bytes(ix, m);
-    ix->status.assign(m, SLOT_VALID);
-    ix->ext_ids = std::move(ext);
-    for (size_t i = 0; i < m; ++i) ix->translator[ix->ext_ids[i]] = uint32_t(i);
+    ix->slots.commit_compact(std::move(ext));
     ix->entry_point = old_to_new[ix->entry_point];
-    ix->first_empty = m;
     return 0;
 }
 

@@ -7,8 +7,8 @@
 // included) and the rest of the region is zero rows with all-ones entries, as the ring of ivf_scan_kernel needs.  An
 // add that overflows a cluster moves the cluster to the pool's tail with a doubled capacity; the pool itself grows by
 // doubling; compaction lays every cluster out tightly again.  Slots, their statuses, external ids and the external ->
-// slot translator are kept as the dynamic flat index keeps them (dynamic_flat.cu); the host also keeps the pool's
-// entries and every Valid slot's (cluster, index in the cluster).
+// slot translator follow slots.h's rules, as the dynamic flat index's do; the host also keeps the pool's entries and
+// every Valid slot's (cluster, index in the cluster).
 //
 // Searches are the IVF index's (ivf.cu) with the scan's DYN form: tombstones are not candidates, and the lists are
 // ordered by (distance, slot) before the slots become external ids.
@@ -20,7 +20,6 @@
 
 #include <algorithm>
 #include <cmath>
-#include <unordered_set>
 
 struct svsb200_dynamic_ivf {
     svsb200_ivf iv;                         // the rows pool, its entries, the clusters and the centroids
@@ -30,40 +29,13 @@ struct svsb200_dynamic_ivf {
     size_t pool_used = 0;                   // pool rows handed out to cluster regions
     // staging of a mutation, kept between calls
     svsb200::DeviceBuffer<unsigned char> dense, rows, codes;   // (codes: an SQ index's added rows, encoded)
-    svsb200::DeviceBuffer<uint32_t> assign, src_pos, dst_pos, vals;
-    svsb200::DeviceBuffer<uint64_t> ids;
+    svsb200::DeviceBuffer<uint32_t> assign, src_pos, dst_pos;   // (the entries' values go in Replica::staging.slots)
 };
 
 namespace svsb200 {
 
 constexpr uint32_t IVF_NONE = 0xFFFFFFFFu;
 constexpr size_t IVF_MIN_POOL = 32;   // rows: an index without rows still has one ring tile of pool
-
-// Row dst_pos[i] of `dst` <- row src_pos[i] of `src` (src_pos NULL: i; src NULL: no row moves), and entry dst_pos[i]
-// <- vals[i] (vals NULL: all-ones); rows of `words` 16-byte words, one warp per row.
-__global__ void ivf_place_kernel(const uint4* src, const uint32_t* __restrict__ src_pos, uint4* dst,
-                                 const uint32_t* __restrict__ dst_pos, const uint32_t* __restrict__ vals,
-                                 uint32_t* __restrict__ entries, uint32_t count, uint32_t words) {
-    const uint32_t i = blockIdx.x * (blockDim.x / 32) + threadIdx.x / 32;
-    const uint32_t lane = threadIdx.x & 31;
-    if (i >= count) return;
-    const size_t d = dst_pos[i];
-    if (src) {
-        const size_t s = src_pos ? src_pos[i] : i;
-        for (uint32_t j = lane; j < words; j += 32) dst[d * words + j] = src[s * words + j];
-    }
-    if (lane == 0) entries[d] = vals ? vals[i] : IVF_NONE;
-}
-
-static cudaError_t place(const void* src, const uint32_t* src_pos, void* dst, const uint32_t* dst_pos, const uint32_t* vals,
-                         uint32_t* entries, size_t count, uint32_t row_stride, cudaStream_t stream) {
-    if (count == 0) return cudaSuccess;
-    ivf_place_kernel<<<unsigned((count + 7) / 8), 256, 0, stream>>>(static_cast<const uint4*>(src), src_pos,
-                                                                     static_cast<uint4*>(dst), dst_pos, vals, entries,
-                                                                     uint32_t(count), row_stride / 16);
-    count_launch();
-    return cudaGetLastError();
-}
 
 template <typename T> static cudaError_t upload(DeviceBuffer<T>& buf, const std::vector<T>& v, cudaStream_t stream) {
     cudaError_t e = buf.ensure(std::max<size_t>(v.size(), 1));
@@ -105,31 +77,6 @@ static int reserve_pool(svsb200_dynamic_ivf* h, Replica* rep, size_t used, cudaS
     return 0;
 }
 
-// Room for `slots` slots in the device statuses and external ids, growing geometrically; new slots are Empty.
-static int reserve_slots(Replica* rep, size_t used, size_t slots, cudaStream_t stream) {
-    const size_t have = rep->d_status.count;
-    if (slots <= have) return 0;
-    const size_t want = std::max(slots, 2 * have);
-    CUDA_TRY(cudaStreamSynchronize(stream));
-    CUDA_TRY(grow(rep->d_status, used, want));
-    CUDA_TRY(grow(rep->d_ext_ids, used, want));
-    CUDA_TRY(cudaMemsetAsync(rep->d_status.ptr + used, SLOT_EMPTY, want - used, stream));
-    return 0;
-}
-
-static int check_ids_new(const char* who, const svsb200_index* ix, const uint64_t* ids, size_t count) {
-    const std::string w(who);
-    std::unordered_set<uint64_t> seen;
-    seen.reserve(count);
-    for (size_t i = 0; i < count; ++i) {
-        if (ids[i] == ~uint64_t(0)) return fail(w + ": external id 2^64 - 1 is reserved");
-        if (!seen.insert(ids[i]).second) return fail(w + ": External IDs contain repeat elements!");
-        if (ix && ix->translator.count(ids[i]))
-            return fail(w + ": External ID " + std::to_string(ids[i]) + " already exists!");
-    }
-    return 0;
-}
-
 static svsb200_ivf* ivf_of(svsb200_dynamic_ivf* h) { return h ? &h->iv : nullptr; }
 
 }  // namespace svsb200
@@ -153,7 +100,8 @@ static int dynamic_ivf_assemble(const char* who, const void* vectors, int dtype,
         for (size_t i = 0; i < n; ++i)
             if (assignments[i] >= C)
                 return fail(w + ": assignment " + std::to_string(i) + " is not a cluster");
-    if (int rc = check_ids_new(who, nullptr, external_ids, n)) return rc;
+    SlotTable slot_table;
+    if (int rc = slot_table.assign(who, external_ids, n)) return rc;
     cudaDeviceProp prop;
     if (int rc = check_device(who, device, &prop)) return rc;
     CUDA_TRY(cudaSetDevice(device));
@@ -172,9 +120,7 @@ static int dynamic_ivf_assemble(const char* who, const void* vectors, int dtype,
     ix->dim = dim;
     ix->row_stride = data_row_stride(storage, dtype, dim);
     ix->gstride = 32;
-    ix->status.assign(n, SLOT_VALID);
-    ix->ext_ids.assign(external_ids, external_ids + n);
-    for (size_t i = 0; i < n; ++i) ix->translator.emplace(external_ids[i], uint32_t(i));
+    ix->slots = std::move(slot_table);
     ix->reps.push_back(std::make_unique<Replica>());
     Replica* rep = ix->reps.back().get();
     rep->device = device;
@@ -232,14 +178,7 @@ static int dynamic_ivf_assemble(const char* who, const void* vectors, int dtype,
     CUDA_TRY(cudaMemcpy(iv.d_start.ptr, h->start.data(), C * 4, cudaMemcpyHostToDevice));
     CUDA_TRY(iv.d_count.ensure(C));
     CUDA_TRY(cudaMemcpy(iv.d_count.ptr, h->count.data(), C * 4, cudaMemcpyHostToDevice));
-    const size_t slots = std::max<size_t>(n, 1);
-    CUDA_TRY(rep->d_status.ensure(slots));
-    CUDA_TRY(rep->d_ext_ids.ensure(slots));
-    CUDA_TRY(cudaMemset(rep->d_status.ptr, SLOT_EMPTY, slots));
-    if (n) {
-        CUDA_TRY(cudaMemcpy(rep->d_status.ptr, ix->status.data(), n, cudaMemcpyHostToDevice));
-        CUDA_TRY(cudaMemcpy(rep->d_ext_ids.ptr, external_ids, n * 8, cudaMemcpyHostToDevice));
-    }
+    if (int rc = upload_slots(rep, ix->slots)) return rc;
     update_device_bytes(h.get());
     *out = h.release();
     return 0;
@@ -281,8 +220,8 @@ int svsb200_dynamic_ivf_destroy(svsb200_dynamic_ivf* index) {
     return 0;
 }
 
-size_t svsb200_dynamic_ivf_size(const svsb200_dynamic_ivf* index) { return index ? index->iv.ix->translator.size() : 0; }
-size_t svsb200_dynamic_ivf_num_slots(const svsb200_dynamic_ivf* index) { return index ? index->iv.ix->status.size() : 0; }
+size_t svsb200_dynamic_ivf_size(const svsb200_dynamic_ivf* index) { return index ? index->iv.ix->slots.size() : 0; }
+size_t svsb200_dynamic_ivf_num_slots(const svsb200_dynamic_ivf* index) { return index ? index->iv.ix->slots.num_slots() : 0; }
 size_t svsb200_dynamic_ivf_dimensions(const svsb200_dynamic_ivf* index) { return index ? index->iv.ix->dim : 0; }
 size_t svsb200_dynamic_ivf_num_clusters(const svsb200_dynamic_ivf* index) { return index ? index->iv.C : 0; }
 size_t svsb200_dynamic_ivf_device_bytes(const svsb200_dynamic_ivf* index) { return index ? index->iv.ix->device_bytes : 0; }
@@ -317,16 +256,12 @@ int svsb200_dynamic_ivf_add(svsb200_dynamic_ivf* index, const void* vectors, int
     } else if (dtype != ix->dtype) {
         return fail("svsb200_dynamic_ivf_add: the points' dtype differs from the index's");
     }
-    if (int rc = check_ids_new(who, ix, ids, count)) return rc;
+    if (int rc = ix->slots.check_new(who, ids, count)) return rc;
     // slots (add_points, dynamic_ivf.h:474-527): Empty ones from slot 0 with reuse_empty, then appended
     std::vector<uint32_t> slots;
-    slots.reserve(count);
-    if (reuse_empty)
-        for (size_t s = 0; s < ix->status.size() && slots.size() < count; ++s)
-            if (ix->status[s] == SLOT_EMPTY) slots.push_back(uint32_t(s));
-    const size_t old_n = ix->status.size(), new_n = old_n + (count - slots.size());
+    const size_t old_n = ix->slots.num_slots();
+    const size_t new_n = ix->slots.choose(count, reuse_empty ? 0 : old_n, &slots);
     if (new_n >= (size_t(1) << 31)) return fail("svsb200_dynamic_ivf_add: more than 2^31-1 slots");
-    for (size_t s = old_n; s < new_n; ++s) slots.push_back(uint32_t(s));
     const size_t C = h->iv.C, stride = ix->row_stride, in_bytes = ix->dim * esize(dtype), row_bytes = ix->dim * esize(ix->dtype);
     // the new layout, made inside the mutation and taken over once every device step has succeeded
     std::vector<uint32_t> assign(count), index_in(count), start = h->start, cnt = h->count, cap = h->cap;
@@ -335,7 +270,8 @@ int svsb200_dynamic_ivf_add(svsb200_dynamic_ivf* index, const void* vectors, int
     int rc = after_searches(ix, [&](Replica* rep, cudaStream_t stream) -> int {
         // Nothing a search reads changes before the last step: the new entries lie past the clusters' old counts or in
         // regions the old starts do not reach, until the new starts and counts are uploaded.
-        if (int rc2 = reserve_slots(rep, old_n, new_n, stream)) return rc2;
+        if (const size_t cap = slot_capacity(rep, new_n))
+            if (int rc2 = grow_slots(rep, old_n, cap, stream)) return rc2;
         // 1. the nearest centroid of every row, as a probe ranks them
         CUDA_TRY(h->dense.ensure(count * in_bytes));
         CUDA_TRY(h->assign.ensure(count));
@@ -361,12 +297,13 @@ int svsb200_dynamic_ivf_add(svsb200_dynamic_ivf* index, const void* vectors, int
         }
         if (used >= (size_t(1) << 32)) return fail("svsb200_dynamic_ivf_add: the rows pool would pass 2^32 rows");
         if (int rc2 = reserve_pool(h, rep, used, stream)) return rc2;
+        Replica::SlotStaging& st = rep->staging;
         if (!reloc_src.empty()) {
             CUDA_TRY(upload(h->src_pos, reloc_src, stream));
             CUDA_TRY(upload(h->dst_pos, reloc_dst, stream));
-            CUDA_TRY(upload(h->vals, reloc_val, stream));
-            CUDA_TRY(place(rep->d_vectors.ptr, h->src_pos.ptr, rep->d_vectors.ptr, h->dst_pos.ptr, h->vals.ptr,
-                           h->iv.d_row_ids.ptr, reloc_src.size(), uint32_t(stride), stream));
+            CUDA_TRY(upload(st.slots, reloc_val, stream));
+            CUDA_TRY(move_rows(rep->d_vectors.ptr, h->src_pos.ptr, rep->d_vectors.ptr, h->dst_pos.ptr, st.slots.ptr,
+                               h->iv.d_row_ids.ptr, reloc_src.size(), uint32_t(stride), stream));
             CUDA_TRY(cudaStreamSynchronize(stream));   // (before the staging buffers are refilled)
         }
         // 4. the rows (SQ: their codes) and their slots into place
@@ -391,13 +328,13 @@ int svsb200_dynamic_ivf_add(svsb200_dynamic_ivf* index, const void* vectors, int
         std::vector<uint32_t> dst(count);
         for (size_t i = 0; i < count; ++i) dst[i] = start[assign[i]] + index_in[i];
         CUDA_TRY(upload(h->dst_pos, dst, stream));
-        CUDA_TRY(upload(h->vals, slots, stream));
-        CUDA_TRY(place(src, nullptr, rep->d_vectors.ptr, h->dst_pos.ptr, h->vals.ptr, h->iv.d_row_ids.ptr, count,
-                       uint32_t(stride), stream));
+        CUDA_TRY(upload(st.slots, slots, stream));
+        CUDA_TRY(move_rows(src, nullptr, rep->d_vectors.ptr, h->dst_pos.ptr, st.slots.ptr, h->iv.d_row_ids.ptr, count,
+                           uint32_t(stride), stream));
         // 5. the slots become Valid, then the clusters' new layout takes effect
-        CUDA_TRY(h->ids.ensure(count));
-        CUDA_TRY(cudaMemcpyAsync(h->ids.ptr, ids, count * 8, cudaMemcpyHostToDevice, stream));
-        CUDA_TRY(mark_slots(h->vals.ptr, h->ids.ptr, count, SLOT_VALID, rep, stream));
+        CUDA_TRY(st.ids.ensure(count));
+        CUDA_TRY(cudaMemcpyAsync(st.ids.ptr, ids, count * 8, cudaMemcpyHostToDevice, stream));
+        CUDA_TRY(mark_slots(st.slots.ptr, st.ids.ptr, count, SLOT_VALID, rep, stream));
         CUDA_TRY(cudaMemcpyAsync(h->iv.d_start.ptr, start.data(), C * 4, cudaMemcpyHostToDevice, stream));
         CUDA_TRY(cudaMemcpyAsync(h->iv.d_count.ptr, cnt.data(), C * 4, cudaMemcpyHostToDevice, stream));
         CUDA_TRY(cudaStreamSynchronize(stream));
@@ -410,8 +347,6 @@ int svsb200_dynamic_ivf_add(svsb200_dynamic_ivf* index, const void* vectors, int
     h->count = std::move(cnt);
     h->cap = std::move(cap);
     h->pool_used = used;
-    ix->status.resize(new_n, SLOT_EMPTY);
-    ix->ext_ids.resize(new_n, ~uint64_t(0));
     h->slot_cluster.resize(new_n, IVF_NONE);
     h->slot_index.resize(new_n, IVF_NONE);
     for (size_t i = 0; i < count; ++i) {
@@ -420,11 +355,8 @@ int svsb200_dynamic_ivf_add(svsb200_dynamic_ivf* index, const void* vectors, int
         h->slot_cluster[s] = c;
         h->slot_index[s] = index_in[i];
         ++h->live[c];
-        ix->status[s] = SLOT_VALID;
-        ix->ext_ids[s] = ids[i];
-        ix->translator.emplace(ids[i], s);
-        if (slots_out) slots_out[i] = s;
     }
+    ix->slots.commit_add(slots, ids, slots_out);
     update_device_bytes(h);
     return 0;
 }
@@ -436,25 +368,17 @@ int svsb200_dynamic_ivf_delete(svsb200_dynamic_ivf* index, const uint64_t* ids, 
     svsb200_index* ix = h->iv.ix.get();
     // nothing changes unless every id is present, once (dynamic_ivf.h:547-636)
     std::vector<uint32_t> slots, pos;
-    slots.reserve(count);
-    pos.reserve(count);
-    std::unordered_set<uint64_t> seen;
-    seen.reserve(count);
-    for (size_t i = 0; i < count; ++i) {
-        auto it = ix->translator.find(ids[i]);
-        if (it == ix->translator.end() || !seen.insert(ids[i]).second)
-            return fail("svsb200_dynamic_ivf_delete: External ID " + std::to_string(ids[i]) + " does not exist!");
-        slots.push_back(it->second);
-        pos.push_back(h->start[h->slot_cluster[it->second]] + h->slot_index[it->second]);
-    }
+    if (int rc = ix->slots.find("svsb200_dynamic_ivf_delete", ids, count, &slots)) return rc;
     if (count == 0) return 0;
+    pos.reserve(count);
+    for (uint32_t s : slots) pos.push_back(h->start[h->slot_cluster[s]] + h->slot_index[s]);
     int rc = after_searches(ix, [&](Replica* rep, cudaStream_t stream) -> int {
         // the entries become tombstones, then the slots Empty
         CUDA_TRY(upload(h->dst_pos, pos, stream));
-        CUDA_TRY(upload(h->vals, slots, stream));
-        CUDA_TRY(place(nullptr, nullptr, nullptr, h->dst_pos.ptr, nullptr, h->iv.d_row_ids.ptr, count, uint32_t(ix->row_stride),
-                       stream));
-        CUDA_TRY(mark_slots(h->vals.ptr, nullptr, count, SLOT_EMPTY, rep, stream));
+        CUDA_TRY(upload(rep->staging.slots, slots, stream));
+        CUDA_TRY(move_rows(nullptr, nullptr, nullptr, h->dst_pos.ptr, nullptr, h->iv.d_row_ids.ptr, count,
+                           uint32_t(ix->row_stride), stream));
+        CUDA_TRY(mark_slots(rep->staging.slots.ptr, nullptr, count, SLOT_EMPTY, rep, stream));
         CUDA_TRY(cudaStreamSynchronize(stream));
         return 0;
     });
@@ -465,10 +389,8 @@ int svsb200_dynamic_ivf_delete(svsb200_dynamic_ivf* index, const uint64_t* ids, 
         --h->live[h->slot_cluster[s]];
         h->slot_cluster[s] = IVF_NONE;
         h->slot_index[s] = IVF_NONE;
-        ix->status[s] = SLOT_EMPTY;
-        ix->ext_ids[s] = ~uint64_t(0);
-        ix->translator.erase(ids[i]);
     }
+    ix->slots.commit_delete(slots, ids, SLOT_EMPTY);
     return 0;
 }
 
@@ -476,18 +398,14 @@ int svsb200_dynamic_ivf_compact(svsb200_dynamic_ivf* index) {
     if (!index) return fail("svsb200_dynamic_ivf_compact: NULL index");
     svsb200_dynamic_ivf* h = index;
     svsb200_index* ix = h->iv.ix.get();
-    const size_t C = h->iv.C, n = ix->status.size(), stride = ix->row_stride;
+    const size_t C = h->iv.C, stride = ix->row_stride;
     // compact (dynamic_ivf.h:932-961): the Valid slots renumbered 0 .. m-1 in slot order; every cluster keeps the
     // stored order of its live entries, laid out tightly from a 32-row boundary
-    std::vector<uint32_t> renum(n, IVF_NONE);
     std::vector<uint64_t> ext;
-    ext.reserve(ix->translator.size());
-    for (size_t s = 0; s < n; ++s)
-        if (ix->status[s] == SLOT_VALID) {
-            renum[s] = uint32_t(ext.size());
-            ext.push_back(ix->ext_ids[s]);
-        }
-    const size_t m = ext.size();
+    const std::vector<uint32_t> new_to_old = ix->slots.valid_slots(&ext);
+    const size_t m = new_to_old.size();
+    std::vector<uint32_t> renum(ix->slots.num_slots(), IVF_NONE);
+    for (size_t i = 0; i < m; ++i) renum[new_to_old[i]] = uint32_t(i);
     std::vector<uint32_t> start(C), cap(C), src, dst, val, slot_cluster(m), slot_index(m);
     size_t used = 0;
     for (size_t c = 0; c < C; ++c) {
@@ -512,16 +430,12 @@ int svsb200_dynamic_ivf_compact(svsb200_dynamic_ivf* index) {
         DeviceBuffer<uint8_t> status;
         DeviceBuffer<uint64_t> ext_ids;
         if (int rc2 = new_pool(vectors, entries, pool, uint32_t(stride), stream)) return rc2;
-        CUDA_TRY(status.ensure(slots));
-        CUDA_TRY(ext_ids.ensure(slots));
-        CUDA_TRY(cudaMemsetAsync(status.ptr, SLOT_EMPTY, slots, stream));
-        CUDA_TRY(cudaMemsetAsync(status.ptr, SLOT_VALID, m, stream));
-        if (m) CUDA_TRY(cudaMemcpyAsync(ext_ids.ptr, ext.data(), m * 8, cudaMemcpyHostToDevice, stream));
+        if (int rc2 = compacted_slots(ext, slots, &status, &ext_ids, stream)) return rc2;
         CUDA_TRY(upload(h->src_pos, src, stream));
         CUDA_TRY(upload(h->dst_pos, dst, stream));
-        CUDA_TRY(upload(h->vals, val, stream));
-        CUDA_TRY(place(rep->d_vectors.ptr, h->src_pos.ptr, vectors.ptr, h->dst_pos.ptr, h->vals.ptr, entries.ptr, m,
-                       uint32_t(stride), stream));
+        CUDA_TRY(upload(rep->staging.slots, val, stream));
+        CUDA_TRY(move_rows(rep->d_vectors.ptr, h->src_pos.ptr, vectors.ptr, h->dst_pos.ptr, rep->staging.slots.ptr,
+                           entries.ptr, m, uint32_t(stride), stream));
         CUDA_TRY(cudaMemcpyAsync(h->iv.d_start.ptr, start.data(), C * 4, cudaMemcpyHostToDevice, stream));
         CUDA_TRY(cudaMemcpyAsync(h->iv.d_count.ptr, h->live.data(), C * 4, cudaMemcpyHostToDevice, stream));
         CUDA_TRY(cudaStreamSynchronize(stream));
@@ -540,40 +454,25 @@ int svsb200_dynamic_ivf_compact(svsb200_dynamic_ivf* index) {
     h->pool_used = used;
     h->slot_cluster = std::move(slot_cluster);
     h->slot_index = std::move(slot_index);
-    ix->status.assign(m, SLOT_VALID);
-    ix->ext_ids = std::move(ext);
-    for (size_t i = 0; i < m; ++i) ix->translator[ix->ext_ids[i]] = uint32_t(i);
+    ix->slots.commit_compact(std::move(ext));
     update_device_bytes(h);
     return 0;
 }
 
 int svsb200_dynamic_ivf_ids(const svsb200_dynamic_ivf* index, uint64_t* out_ids, size_t* count) {
     if (!index) return fail("svsb200_dynamic_ivf_ids: NULL index");
-    if (!count) return fail("svsb200_dynamic_ivf_ids: NULL count");
-    const svsb200_index* ix = index->iv.ix.get();
-    if (out_ids) {
-        if (*count < ix->translator.size()) return fail("svsb200_dynamic_ivf_ids: output too small");
-        size_t o = 0;
-        for (size_t s = 0; s < ix->status.size(); ++s)   // slot order
-            if (ix->status[s] == SLOT_VALID) out_ids[o++] = ix->ext_ids[s];
-    }
-    *count = ix->translator.size();
-    return 0;
+    return index->iv.ix->slots.ids("svsb200_dynamic_ivf_ids", out_ids, count);
 }
 
 int svsb200_dynamic_ivf_has_id(const svsb200_dynamic_ivf* index, uint64_t id, int* out) {
     if (!index) return fail("svsb200_dynamic_ivf_has_id: NULL index");
-    if (!out) return fail("svsb200_dynamic_ivf_has_id: NULL output");
-    *out = index->iv.ix->translator.count(id) ? 1 : 0;
-    return 0;
+    return index->iv.ix->slots.has_id("svsb200_dynamic_ivf_has_id", id, out);
 }
 
 int svsb200_dynamic_ivf_export(const svsb200_dynamic_ivf* index, uint8_t* status_out, uint64_t* ext_ids_out,
                                uint32_t* cluster_out) {
     if (!index) return fail("svsb200_dynamic_ivf_export: NULL index");
-    const svsb200_index* ix = index->iv.ix.get();
-    if (status_out) std::copy(ix->status.begin(), ix->status.end(), status_out);
-    if (ext_ids_out) std::copy(ix->ext_ids.begin(), ix->ext_ids.end(), ext_ids_out);
+    index->iv.ix->slots.export_to(status_out, ext_ids_out);
     if (cluster_out) std::copy(index->slot_cluster.begin(), index->slot_cluster.end(), cluster_out);
     return 0;
 }
@@ -627,7 +526,7 @@ int svsb200_dynamic_ivf_search_filtered(svsb200_dynamic_ivf* index, const void* 
     if (nq == 0) return 0;
     if (!queries || !out_ids || !out_dists) return fail("svsb200_dynamic_ivf_search_filtered: NULL buffer");
     return ivf_search_filtered_host(&index->iv, queries, qdtype, nq, k, n_probes, slot_bitmap,
-                                    (index->iv.ix->status.size() + 31) / 32, out_ids, out_dists, out_probes, out_allowed,
+                                    (index->iv.ix->slots.num_slots() + 31) / 32, out_ids, out_dists, out_probes, out_allowed,
                                     out_rows, index->iv.ix->reps[0]->d_ext_ids.ptr);
 }
 

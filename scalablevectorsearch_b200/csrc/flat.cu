@@ -1061,7 +1061,7 @@ static int ensure_flat_base(svsb200_index* ix, Replica* rep, int kind, cudaStrea
     if (ix->slot_mask) {   // slots that are not Valid become padding rows
         std::vector<uint32_t> empty;
         for (uint32_t s = 0; s < n; ++s)
-            if (ix->status[s] != SLOT_VALID) empty.push_back(s);
+            if (ix->slots.status[s] != SLOT_VALID) empty.push_back(s);
         DeviceBuffer<uint32_t> d_empty;
         CUDA_TRY(d_empty.ensure(std::max<size_t>(empty.size(), 1)));
         CUDA_TRY(cudaMemcpyAsync(d_empty.ptr, empty.data(), empty.size() * 4, cudaMemcpyHostToDevice, stream));
@@ -1199,7 +1199,7 @@ static int flat_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, const vo
         return rc;
     if (ix->slot_mask) {
         CUDA_TRY(slots_to_external(d_out_ids, nq * k, rep->d_ext_ids.ptr, sc->stream));
-        CUDA_TRY(cudaEventRecord(sc->ev_done, sc->stream));   // (a mutation waits for it: dynamic_flat.cu, on_stream)
+        CUDA_TRY(cudaEventRecord(sc->ev_done, sc->stream));   // (a mutation waits for it: after_searches)
     }
     return 0;
 }

@@ -25,7 +25,6 @@
 
 namespace svsb200 {
 
-int fail(const std::string& msg);   // records the calling thread's svsb200_last_error(); returns 1
 #define CUDA_TRY(expr)                                                                         \
     do {                                                                                       \
         cudaError_t err__ = (expr);                                                            \
@@ -175,7 +174,7 @@ struct Replica {
     FlatBase flat_f16;                       // fp16 tiles
     DeviceBuffer<unsigned int> flat_xmax;    // ... and the largest norm of their rows
     bool flat_xmax_stale = false;            // dynamic flat index: the Valid slots changed since flat_xmax was taken
-    // dynamic flat index: staging of a mutation (the added rows, their slots and ids, and the rows tiled 8 to a tile),
+    // dynamic indexes: staging of a mutation (the added rows, their slots and ids, and the rows tiled 8 to a tile),
     // kept between calls so that an add or delete allocates -- and synchronises the device -- only when it outgrows them
     struct SlotStaging {
         DeviceBuffer<unsigned char> rows, tiles;
@@ -264,16 +263,13 @@ struct svsb200_index {
     std::mutex mu;
     svsb200::Scratch* last = nullptr; // scratch of the most recent search: counters, kernel time, kernel kind
     // dynamic index (svsb200_dynamic_*, MutableVamanaIndex): slot status and external ids live on the device
-    // (Replica::d_status / d_ext_ids) and are mirrored here with the external -> slot translator.
+    // (Replica::d_status / d_ext_ids) and are mirrored here with the external -> slot translator (slots.h).
     bool dynamic = false;
-    std::vector<uint8_t> status;
-    std::vector<uint64_t> ext_ids;
-    std::unordered_map<uint64_t, uint32_t> translator;
+    svsb200::SlotTable slots;         // also the dynamic flat and dynamic IVF indexes'
     long dyn_slack = -1;              // option "dynamic_slack"
     std::atomic<long> dyn_reruns{0};  // queries re-run with a larger buffer so far
-    size_t first_empty = 0;           // first_empty_: where add_points looks for Empty slots unless told to reuse
-    // dynamic flat index (svsb200_dynamic_flat_*, DynamicFlatIndex): the same slot fields, statuses Valid / Empty only,
-    // and every flat search skips the slots that are not Valid and returns external ids.  `dynamic` stays false.
+    // dynamic flat index (svsb200_dynamic_flat_*, DynamicFlatIndex): the same slots, statuses Valid / Empty only, and
+    // every flat search skips the slots that are not Valid and returns external ids.  `dynamic` stays false.
     bool slot_mask = false;
     // mutation parameters (alpha_, construction_window_size_, max_candidates_, prune_to_)
     float dyn_alpha = 0.f;
@@ -342,14 +338,36 @@ int row_degrees(const GraphBuild& b);
 // Slots -> external ids in place, `count` ids (padding ids stay all-ones; search.cu), enqueued on `stream`.
 cudaError_t slots_to_external(uint64_t* d_ids, size_t count, const uint64_t* d_ext_ids, cudaStream_t stream);
 
-// ---- mutations of the dynamic flat and dynamic IVF indexes (dynamic_flat.cu, dynamic_ivf.cu) ----
+// ---- mutations of the dynamic Vamana, dynamic flat and dynamic IVF indexes (dynamic.cu, dynamic_flat.cu,
+// dynamic_ivf.cu): the device side of their slots (slots.cu; the host side is slots.h) ----
+// rep->d_status / d_ext_ids hold the slots of `t`, with room for at least one slot (synchronous).
+int upload_slots(Replica* rep, const SlotTable& t);
+// The slot capacity an add to `slots` slots needs: 0 when rep->d_status already has room, else a geometric step (many
+// small adds do not copy the per-slot arrays each time).
+inline size_t slot_capacity(const Replica* rep, size_t slots) {
+    const size_t have = rep->d_status.count;
+    return slots <= have ? 0 : std::max(slots, 2 * have);
+}
+// rep->d_ext_ids, then rep->d_status, grown to `cap` slots, the first `used` kept; the new statuses are Empty.
+// d_status's size is the capacity every later add checks, so an index grows its own per-slot arrays (rows, adjacency)
+// to `cap` before calling this: a failed allocation then leaves the capacity as it was and the next add retries.
+int grow_slots(Replica* rep, size_t used, size_t cap, cudaStream_t stream);
+// The statuses and external ids after compaction: `ext.size()` Valid slots with external ids `ext`, Empty ones up to
+// `cap`, in new buffers (the caller moves them into rep once the stream is drained), enqueued on `stream`.
+int compacted_slots(const std::vector<uint64_t>& ext, size_t cap, DeviceBuffer<uint8_t>* status,
+                    DeviceBuffer<uint64_t>* ext_ids, cudaStream_t stream);
 // rep->d_status[d_slots[i]] = value and, with d_ids, rep->d_ext_ids[d_slots[i]] = d_ids[i], enqueued on `stream`.
 cudaError_t mark_slots(const uint32_t* d_slots, const uint64_t* d_ids, size_t count, uint8_t value, Replica* rep,
                        cudaStream_t stream);
+// Row dst_pos[i] of `dst` <- row src_pos[i] of `src` (an index array NULL: i; src NULL: no row moves), rows of
+// row_stride bytes (a multiple of 16); with `entries`, entry dst_pos[i] <- vals[i] (vals NULL: all-ones).  Enqueued on
+// `stream`.
+cudaError_t move_rows(const void* src, const uint32_t* src_pos, void* dst, const uint32_t* dst_pos, const uint32_t* vals,
+                      uint32_t* entries, size_t count, uint32_t row_stride, cudaStream_t stream);
 // Runs a mutation `body(rep, stream)` on a scratch stream of the index's device, once every search of the index
 // enqueued so far has finished: a device-buffer search returns with work still queued on the caller's stream (the
 // mapping to external ids reads the slots' external ids, the scan reads the rows), and the mutation rewrites them.
-// Every search of a dynamic flat or dynamic IVF index records its scratch's ev_done at its end (flat.cu, ivf.cu).
+// Every search of a dynamic index records its scratch's ev_done at its end (search.cu, flat.cu, ivf.cu).
 template <typename F> int after_searches(svsb200_index* ix, F body) {
     Replica* rep = ix->reps[0].get();
     CUDA_TRY(cudaSetDevice(rep->device));

@@ -19,8 +19,11 @@ from . import _lib
 from .vamana import _DTYPE_CODE, DistanceType
 
 
-class DynamicFlat:
-    """``svs.DynamicFlat`` on one CUDA device: float32 / float16 / int8 / uint8 rows, L2 / MIP / cosine."""
+class DynamicFlat(_lib._Slots):
+    """``svs.DynamicFlat`` on one CUDA device: float32 / float16 / int8 / uint8 rows, L2 / MIP / cosine.  A delete
+    (``delete_entries``, dynamic_flat.h:292-307) empties the slots at once."""
+
+    _ABI = "svsb200_dynamic_flat"
 
     @classmethod
     def build(cls, data, ids, distance_type: DistanceType = DistanceType.L2, num_threads: int = 1,
@@ -88,25 +91,7 @@ class DynamicFlat:
         """``add_points`` (dynamic_flat.h:214-276): rows of the index's dtype with new external ids.  Empty slots are
         used first (from slot 0 with ``reuse_empty``, else from the first slot past the last add), then the index
         grows.  Fails without changing anything on a repeated, present or reserved id.  Returns the slots used."""
-        pts = np.ascontiguousarray(points)
-        ids = np.ascontiguousarray(np.atleast_1d(ids), dtype=np.uint64)
-        if pts.ndim != 2 or pts.shape[1] != self.dimensions:
-            raise ValueError(f"points must be [count, {self.dimensions}]")
-        if pts.shape[0] != len(ids):
-            raise ValueError(f"Number of points ({pts.shape[0]}) not equal to the number of external ids ({len(ids)})!")
-        if pts.dtype not in _DTYPE_CODE:
-            raise TypeError(f"unsupported data type {pts.dtype}")
-        slots = np.empty(len(ids), dtype=np.uint64)
-        _lib.check(self._lib.svsb200_dynamic_flat_add(self._h, pts.ctypes.data, _DTYPE_CODE[pts.dtype], len(ids),
-                                                       ids.ctypes.data, int(bool(reuse_empty)), slots.ctypes.data))
-        return slots
-
-    def delete(self, ids) -> int:
-        """``delete_entries`` (dynamic_flat.h:292-307): the slots become Empty at once.  Fails without changing
-        anything unless every id is present, once.  Returns the number of deleted entries."""
-        ids = np.ascontiguousarray(np.atleast_1d(ids), dtype=np.uint64)
-        _lib.check(self._lib.svsb200_dynamic_flat_delete(self._h, ids.ctypes.data, len(ids)))
-        return len(ids)
+        return self._add(points, ids, reuse_empty)
 
     def consolidate(self) -> None:
         """No-op, as in the reference: deletion is direct."""
@@ -115,18 +100,6 @@ class DynamicFlat:
         """``compact`` (dynamic_flat.h:335-367): the Valid slots move, in order, to the front.  ``batchsize`` only
         tunes the reference's copy and is ignored."""
         _lib.check(self._lib.svsb200_dynamic_flat_compact(self._h))
-
-    def has_id(self, id: int) -> bool:
-        out = C.c_int()
-        _lib.check(self._lib.svsb200_dynamic_flat_has_id(self._h, int(id), C.byref(out)))
-        return bool(out.value)
-
-    def all_ids(self) -> np.ndarray:
-        """External ids of every Valid slot, in slot order."""
-        n = C.c_size_t(self.size)
-        out = np.empty(n.value, dtype=np.uint64)
-        _lib.check(self._lib.svsb200_dynamic_flat_ids(self._h, out.ctypes.data, C.byref(n)))
-        return out[: n.value]
 
     def export(self):
         """(status uint8 (0 Empty, 1 Valid), external ids (2^64 - 1 where Empty)) over every slot."""

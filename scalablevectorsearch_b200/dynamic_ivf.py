@@ -31,8 +31,11 @@ from .ivf import Clustering, IVFSearchParameters, _search_filtered, _sq_codes
 from .vamana import _DTYPE_CODE, DistanceType
 
 
-class DynamicIVF:
-    """``svs.DynamicIVF`` on one CUDA device: float32 / float16 rows or int8 / uint8 SQ codes, L2 / MIP / cosine."""
+class DynamicIVF(_lib._Slots):
+    """``svs.DynamicIVF`` on one CUDA device: float32 / float16 rows or int8 / uint8 SQ codes, L2 / MIP / cosine.  A
+    delete empties the slots at once and leaves tombstones in their clusters."""
+
+    _ABI = "svsb200_dynamic_ivf"
 
     @classmethod
     def assemble_from_clustering(cls, clustering: Clustering, data, ids, distance: DistanceType = DistanceType.L2,
@@ -131,24 +134,7 @@ class DynamicIVF:
         pts = np.ascontiguousarray(points)
         if pts.dtype == np.float32 and self._dtype == np.float16:
             pts = pts.astype(np.float16)
-        ids = np.ascontiguousarray(np.atleast_1d(ids), dtype=np.uint64)
-        if pts.ndim != 2 or pts.shape[1] != self.dimensions:
-            raise ValueError(f"points must be [count, {self.dimensions}]")
-        if pts.shape[0] != len(ids):
-            raise ValueError(f"Number of points ({pts.shape[0]}) not equal to the number of external ids ({len(ids)})!")
-        if pts.dtype not in _DTYPE_CODE:
-            raise TypeError(f"unsupported data type {pts.dtype}")
-        slots = np.empty(len(ids), dtype=np.uint64)
-        _lib.check(self._lib.svsb200_dynamic_ivf_add(self._h, pts.ctypes.data, _DTYPE_CODE[pts.dtype], len(ids),
-                                                      ids.ctypes.data, int(bool(reuse_empty)), slots.ctypes.data))
-        return slots
-
-    def delete(self, ids) -> int:
-        """``delete``: the slots become Empty at once.  Fails without changing anything unless every id is present,
-        once.  Returns the number of deleted entries."""
-        ids = np.ascontiguousarray(np.atleast_1d(ids), dtype=np.uint64)
-        _lib.check(self._lib.svsb200_dynamic_ivf_delete(self._h, ids.ctypes.data, len(ids)))
-        return len(ids)
+        return self._add(pts, ids, reuse_empty)
 
     def consolidate(self) -> None:
         """No-op, as in the reference: deletion is direct."""
@@ -157,18 +143,6 @@ class DynamicIVF:
         """``compact``: the Valid slots are renumbered in order and the clusters laid out without tombstones.
         ``batchsize`` only tunes the reference's copy and is ignored."""
         _lib.check(self._lib.svsb200_dynamic_ivf_compact(self._h))
-
-    def has_id(self, id: int) -> bool:
-        out = C.c_int()
-        _lib.check(self._lib.svsb200_dynamic_ivf_has_id(self._h, int(id), C.byref(out)))
-        return bool(out.value)
-
-    def all_ids(self) -> np.ndarray:
-        """External ids of every Valid slot, in slot order."""
-        n = C.c_size_t(self.size)
-        out = np.empty(n.value, dtype=np.uint64)
-        _lib.check(self._lib.svsb200_dynamic_ivf_ids(self._h, out.ctypes.data, C.byref(n)))
-        return out[: n.value]
 
     def export(self):
         """Per slot: (status uint8 (0 Empty, 1 Valid), external id (2^64 - 1 where Empty), cluster uint32 (2^32 - 1

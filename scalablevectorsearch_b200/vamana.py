@@ -22,6 +22,7 @@ from dataclasses import dataclass, field
 import numpy as np
 
 from . import _lib, io
+from ._lib import _DTYPE_CODE
 
 
 class DistanceType(enum.IntEnum):
@@ -39,7 +40,6 @@ class DataType(enum.Enum):
     uint8 = np.dtype(np.uint8)
 
 
-_DTYPE_CODE = {np.dtype(np.float32): 0, np.dtype(np.float16): 1, np.dtype(np.int8): 2, np.dtype(np.uint8): 3}
 _STORAGE_PLAIN, _STORAGE_SQ, _STORAGE_LVQ8 = 0, 1, 2
 
 
@@ -487,13 +487,16 @@ class ShardedVamana:
         return ids, dists
 
 
-class DynamicVamana(Vamana):
+class DynamicVamana(_lib._Slots, Vamana):
     """GPU-backed dynamic Vamana index: the reference's ``svs.DynamicVamana`` / ``MutableVamanaIndex``
     (bindings/python/src/dynamic_vamana.cpp, include/svs/index/vamana/dynamic_index.h) built on the GPU or assembled
     from a graph, its data and one external id per row, with ``add``, soft ``delete``, ``consolidate`` and
     ``compact``.  Searches return external ids and never return a deleted one, while the walk still goes through
     deleted rows, exactly as ``MutableVamanaIndex::search`` does.  Mutations must not run concurrently with searches
-    of the same index.  float32 / float16 data, one device."""
+    of the same index.  float32 / float16 data, one device.  A delete (``delete_entries``, dynamic_index.h:773-788)
+    is soft: the slots are Deleted, and keep their rows and external ids until :meth:`consolidate`."""
+
+    _ABI = "svsb200_dynamic"
 
     @classmethod
     def build(cls, parameters: VamanaBuildParameters, data: np.ndarray, ids=None, distance: "DistanceType" = None,
@@ -568,41 +571,11 @@ class DynamicVamana(Vamana):
         """Rows held on the device, deleted ones included."""
         return self._lib.svsb200_index_size(self._h)
 
-    def all_ids(self) -> np.ndarray:
-        """External ids of every valid entry (``all_ids``), in slot order."""
-        n = C.c_size_t(self.size)
-        out = np.empty(n.value, dtype=np.uint64)
-        _lib.check(self._lib.svsb200_dynamic_ids(self._h, out.ctypes.data, C.byref(n)))
-        return out[: n.value]
-
-    def has_id(self, id: int) -> bool:
-        out = C.c_int()
-        _lib.check(self._lib.svsb200_dynamic_has_id(self._h, int(id), C.byref(out)))
-        return bool(out.value)
-
-    def delete(self, ids) -> int:
-        """Soft deletion (``delete_entries``, dynamic_index.h:773-788): fails without changing anything unless every
-        id is present.  Returns the number of deleted entries."""
-        ids = np.ascontiguousarray(np.atleast_1d(ids), dtype=np.uint64)
-        _lib.check(self._lib.svsb200_dynamic_delete(self._h, ids.ctypes.data, len(ids)))
-        return len(ids)
-
     def add(self, points: np.ndarray, ids, reuse_empty: bool = False) -> np.ndarray:
         """``add_points`` (dynamic_index.h:657-749): insert rows of the index's dtype with new external ids.  Empty
         slots are used first (from the start with ``reuse_empty``), then the index grows.  Fails without changing
         anything on a repeated, present or reserved id.  Returns the slots used."""
-        pts = np.ascontiguousarray(points)
-        ids = np.ascontiguousarray(np.atleast_1d(ids), dtype=np.uint64)
-        if pts.ndim != 2 or pts.shape[1] != self.dimensions:
-            raise ValueError(f"points must be [count, {self.dimensions}]")
-        if pts.shape[0] != len(ids):
-            raise ValueError(f"Number of points ({pts.shape[0]}) not equal to the number of external ids ({len(ids)})!")
-        if pts.dtype not in _DTYPE_CODE:
-            raise TypeError(f"unsupported data type {pts.dtype}")
-        slots = np.empty(len(ids), dtype=np.uint64)
-        _lib.check(self._lib.svsb200_dynamic_add(self._h, pts.ctypes.data, _DTYPE_CODE[pts.dtype], len(ids), ids.ctypes.data,
-                                                 int(bool(reuse_empty)), slots.ctypes.data))
-        return slots
+        return self._add(points, ids, reuse_empty)
 
     def consolidate(self):
         """``consolidate`` (dynamic_index.h:976-1013): unlink the deleted entries from the graph; their slots become
