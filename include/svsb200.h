@@ -257,6 +257,23 @@ int svsb200_build_vamana(
     float alpha, size_t graph_max_degree, size_t window_size, size_t max_candidate_pool_size,
     size_t prune_to, int device, uint32_t* graph_rows_out, uint32_t* entry_point_out);
 
+/* GPU graph construction over scalar-quantised codes.  Replaces: auto_build over SQDataset<int8_t / uint8_t>
+ * (the reference's VamanaBuildAdaptor for SQ data, extensions/vamana/scalar.h:47-95).  Every datum is its own query
+ * through DecompressionAdaptor (quantization/scalar/scalar.h:547-600): its codes are decompressed to fp32 as
+ * scale * c + bias and prepared as the SQ search prepares an fp32 query, so the build's distances are the SQ
+ * search's: L2 compresses the decompressed row again (the round trip may move codes) and scales the integer L2 of the
+ * two code rows by scale^2; MIP is scale * <v, c> + bias * sum(v); cosine decompresses both sides.  The entry point is
+ * the medoid of the codes as integers (find_medioid over get_datum).  The result is searched with
+ * svsb200_index_create(..., SVSB200_SQ, {scale, bias}).
+ *   codes       n x dim int8 / uint8 codes (`code_type` SVSB200_I8 / SVSB200_U8), dense, HOST (svsb200_sq_compress
+ *               writes them);
+ *   scale, bias the SQ parameters: the scale finite and positive, the bias finite;
+ * everything else, the output layout, the defaults, the refusals and the parity bar are svsb200_build_vamana's. */
+int svsb200_build_vamana_sq(
+    const void* codes, int code_type, size_t n, size_t dim, int metric, float scale, float bias,
+    float alpha, size_t graph_max_degree, size_t window_size, size_t max_candidate_pool_size,
+    size_t prune_to, int device, uint32_t* graph_rows_out, uint32_t* entry_point_out);
+
 /* How svsb200_flat_search* will split a problem of `nq` queries over `n` base vectors on a device with `sm_count`
  * SMs (introspection, host arithmetic only; nothing in the reference corresponds): `ctas` thread blocks are
  * launched; the 128-query tiles are taken `share` at a time and the (row group, 256-row base tile) pairs form one

@@ -23,7 +23,7 @@ SYMBOLS = [
     "svsb200_get_counters", "svsb200_get_fetched", "svsb200_last_kernel_ms", "svsb200_launch_count", "svsb200_set_option", "svsb200_get_option",
     "svsb200_merge_topk_device", "svsb200_exhaustive_device", "svsb200_lvq8_row_stride", "svsb200_lvq8_compress",
     "svsb200_index_create_multi", "svsb200_index_num_devices", "svsb200_search_cancellable", "svsb200_set_id_offset",
-    "svsb200_search_sharded", "svsb200_build_vamana", "svsb200_flat_search_device", "svsb200_flat_search", "svsb200_index_assemble", "svsb200_toml_get", "svsb200_search_filtered", "svsb200_range_search", "svsb200_free", "svsb200_set_entry_points",
+    "svsb200_search_sharded", "svsb200_build_vamana", "svsb200_build_vamana_sq", "svsb200_flat_search_device", "svsb200_flat_search", "svsb200_index_assemble", "svsb200_toml_get", "svsb200_search_filtered", "svsb200_range_search", "svsb200_free", "svsb200_set_entry_points",
     "svsb200_flat_plan", "svsb200_flat_plan_k",
     "svsb200_flat_index_create", "svsb200_flat_index_destroy", "svsb200_flat_index_size", "svsb200_flat_index_dimensions",
     "svsb200_flat_index_device_bytes", "svsb200_flat_index_search", "svsb200_flat_index_search_device",
@@ -122,6 +122,8 @@ def lib() -> C.CDLL:
     l.svsb200_free.restype = None
     l.svsb200_set_entry_points.argtypes = [vp, vp, sz]
     l.svsb200_build_vamana.argtypes = [vp, i32, sz, sz, sz, i32, C.c_float, sz, sz, sz, sz, i32, vp, C.POINTER(u32)]
+    l.svsb200_build_vamana_sq.argtypes = [vp, i32, sz, sz, i32, C.c_float, C.c_float, C.c_float, sz, sz, sz, sz, i32, vp,
+                                          C.POINTER(u32)]
     l.svsb200_dynamic_create.argtypes = [vp, i32, sz, sz, vp, sz, u32, i32, vp, i32, C.POINTER(vp)]
     l.svsb200_dynamic_delete.argtypes = [vp, vp, sz]
     l.svsb200_dynamic_ids.argtypes = [vp, vp, C.POINTER(sz)]

@@ -1,9 +1,13 @@
 // gpu_runtime_index.cpp -- the FAISS-facing runtime ABI of the reference (SURVEY.md §8 f4), backed by libsvsb200.
 //
 // Implements `svs::runtime::v0::VamanaIndex` (bindings/cpp/include/svs/runtime/vamana_index.h:61-143) for the
-// uncompressed storage kinds (FP32, FP16) on the GPU: `build` + `add` construct the graph with svsb200_build_vamana,
-// `search` is the batched GPU search (optionally through an IDFilter evaluated on the device as a bitmap),
-// `range_search` grows the result lists until they leave the radius.  It stands where the reference's
+// uncompressed storage kinds (FP32, FP16) and SQI8 on the GPU: `build` + `add` construct the graph with
+// svsb200_build_vamana, `search` is the batched GPU search (optionally through an IDFilter evaluated on the device as a
+// bitmap), `range_search` grows the result lists until they leave the radius.  SQI8 follows the reference's
+// VamanaIndexImpl (vamana_index_impl.h:413-450): the first `add` compresses its float32 rows to int8 codes with one
+// global scale and bias (svsb200_sq_compress; constant rows, or rows holding a NaN or an infinity, are a RUNTIME_ERROR)
+// and builds the graph over the codes (svsb200_build_vamana_sq); the searches run the SQ search, `reconstruct_at`
+// decompresses (scale * c + bias, the reference's DecompressionAccessor) and the host keeps the codes only.  It stands where the reference's
 // libsvs_runtime implementation sits (bindings/cpp/src/vamana_index.cpp, vamana_index_impl.h:60-330): a program
 // written against the runtime header links this object instead and runs on the H100.
 //
@@ -86,12 +90,31 @@ class GpuVamanaIndex final : public VamanaIndex {
         if (index_) return Status(ErrorCode::INVALID_ARGUMENT, "Vamana index does not support adding points after initialization");
         if (n == 0 || !x) return Status(ErrorCode::INVALID_ARGUMENT, "no data");
         try {
-            data_.assign(x, x + n * dim_);
             const int metric = metric_ == MetricType::L2 ? SVSB200_L2 : SVSB200_IP;
             const size_t R = is_specified(bp_.graph_max_degree) ? bp_.graph_max_degree : 32;
             const size_t window = is_specified(bp_.construction_window_size) ? bp_.construction_window_size : 200;
+            const float alpha = is_specified(bp_.alpha) ? bp_.alpha : 0.f;
+            const size_t pool = is_specified(bp_.max_candidate_pool_size) ? bp_.max_candidate_pool_size : 0;
+            const size_t prune_to = is_specified(bp_.prune_to) ? bp_.prune_to : 0;
             std::vector<uint32_t> graph(n * (R + 1));
             uint32_t ep = 0;
+            if (kind_ == StorageKind::SQI8) {   // int8 codes with one global scale and bias (vamana_index_impl.h:413-450)
+                std::vector<int8_t> codes(n * dim_);
+                float sq[2] = {0.f, 0.f};
+                if (svsb200_sq_compress(x, n, dim_, SVSB200_I8, 0, codes.data(), &sq[0], &sq[1]) ||
+                    svsb200_build_vamana_sq(codes.data(), SVSB200_I8, n, dim_, metric, sq[0], sq[1], alpha, R, window, pool,
+                                            prune_to, 0, graph.data(), &ep) ||
+                    svsb200_index_create(codes.data(), SVSB200_I8, n, dim_, 0, graph.data(), R + 1, ep, metric, SVSB200_SQ,
+                                         sq, 0, &index_))
+                    return gpu_error();
+                codes_ = std::move(codes);
+                scale_ = sq[0];
+                bias_ = sq[1];
+                n_ = n;
+                graph_bytes_ = graph.size() * 4;
+                return Status_Ok;
+            }
+            data_.assign(x, x + n * dim_);
             const void* rows = data_.data();
             int dtype = SVSB200_F32;
             if (kind_ == StorageKind::FP16) {   // stored as float16, like the reference's FP16 storage kind
@@ -100,9 +123,7 @@ class GpuVamanaIndex final : public VamanaIndex {
                 rows = half_.data();
                 dtype = SVSB200_F16;
             }
-            if (svsb200_build_vamana(rows, dtype, n, dim_, 0, metric, is_specified(bp_.alpha) ? bp_.alpha : 0.f, R, window,
-                                     is_specified(bp_.max_candidate_pool_size) ? bp_.max_candidate_pool_size : 0,
-                                     is_specified(bp_.prune_to) ? bp_.prune_to : 0, 0, graph.data(), &ep))
+            if (svsb200_build_vamana(rows, dtype, n, dim_, 0, metric, alpha, R, window, pool, prune_to, 0, graph.data(), &ep))
                 return gpu_error();
             if (svsb200_index_create(rows, dtype, n, dim_, 0, graph.data(), R + 1, ep, metric, SVSB200_PLAIN, nullptr, 0, &index_))
                 return gpu_error();
@@ -119,6 +140,7 @@ class GpuVamanaIndex final : public VamanaIndex {
         index_ = nullptr;
         data_.clear();
         half_.clear();
+        codes_.clear();
         n_ = 0;
         return Status_Ok;
     }
@@ -192,7 +214,9 @@ class GpuVamanaIndex final : public VamanaIndex {
         uint32_t found = 0;
         if (svsb200_search_filtered(index_, query, SVSB200_F32, 1, 1, n_ < 4096 ? n_ : 4096, bitmap.data(), &label, distance, &found))
             return gpu_error();
-        if (!found) {   // not reached by the graph walk: plain arithmetic on the host copy
+        if (!found && kind_ == StorageKind::SQI8) {   // not reached by the graph walk: the query-side compressed distance
+            *distance = sq_distance(query, &codes_[id * dim_]);
+        } else if (!found) {   // not reached by the graph walk: plain arithmetic on the host copy
             float acc = 0.f;
             for (size_t i = 0; i < dim_; ++i) {
                 const float v = kind_ == StorageKind::FP16 ? from_half(half_[id * dim_ + i]) : data_[id * dim_ + i];
@@ -207,7 +231,9 @@ class GpuVamanaIndex final : public VamanaIndex {
         for (size_t i = 0; i < n; ++i) {
             if (ids[i] >= n_) return Status(ErrorCode::INVALID_ARGUMENT, "id out of range");
             for (size_t d = 0; d < dim_; ++d)
-                output[i * dim_ + d] = kind_ == StorageKind::FP16 ? from_half(half_[ids[i] * dim_ + d]) : data_[ids[i] * dim_ + d];
+                output[i * dim_ + d] = kind_ == StorageKind::SQI8   ? decompress(codes_[ids[i] * dim_ + d])
+                                       : kind_ == StorageKind::FP16 ? from_half(half_[ids[i] * dim_ + d])
+                                                                    : data_[ids[i] * dim_ + d];
         }
         return Status_Ok;
     }
@@ -225,6 +251,32 @@ class GpuVamanaIndex final : public VamanaIndex {
     }
 
   private:
+    // DecompressionAccessor (quantization/scalar/scalar.h:606-620): scale * c + bias, two roundings
+    float decompress(int8_t c) const {
+        const float scaled = scale_ * float(c);
+        return scaled + bias_;
+    }
+    // The SQ search's distance of a float32 query to one row of codes (EuclideanCompressed / InnerProductCompressed,
+    // quantization/scalar/scalar.h:58-153): L2 compresses the query and scales the integer L2 by scale^2; MIP is
+    // scale * <q, c> + bias * sum(q).  The sums run in order (the device's MIP tree may round differently).
+    float sq_distance(const float* q, const int8_t* c) const {
+        if (metric_ == MetricType::L2) {
+            int64_t l2 = 0;
+            for (size_t i = 0; i < dim_; ++i) {
+                float r = std::round((q[i] - bias_) / scale_);   // detail::compress
+                r = r < -128.f ? -128.f : r > 127.f ? 127.f : r;
+                const int64_t diff = int64_t(r) - int64_t(c[i]);
+                l2 += diff * diff;
+            }
+            return (scale_ * scale_) * float(int32_t(l2));
+        }
+        float ip = 0.f, sum = 0.f;
+        for (size_t i = 0; i < dim_; ++i) {
+            ip += q[i] * float(c[i]);
+            sum += q[i];
+        }
+        return scale_ * ip + bias_ * sum;
+    }
     void window_of(const SearchParams* params, size_t k, size_t& window, size_t& capacity) const {
         window = is_specified(sp_.search_window_size) ? sp_.search_window_size : 10;
         capacity = is_specified(sp_.search_buffer_capacity) ? sp_.search_buffer_capacity : 0;
@@ -285,15 +337,17 @@ class GpuVamanaIndex final : public VamanaIndex {
     SearchParams sp_;
     std::vector<float> data_;
     std::vector<uint16_t> half_;
+    std::vector<int8_t> codes_;   // SQI8: the codes, scale_ and bias_
+    float scale_ = 1.f, bias_ = 0.f;
     svsb200_index* index_ = nullptr;
 };
 
 }  // namespace
 
 Status VamanaIndex::check_storage_kind(StorageKind kind) noexcept {
-    return kind == StorageKind::FP32 || kind == StorageKind::FP16
+    return kind == StorageKind::FP32 || kind == StorageKind::FP16 || kind == StorageKind::SQI8
                ? Status_Ok
-               : Status(ErrorCode::NOT_IMPLEMENTED, "the GPU runtime holds FP32 / FP16 storage (compressed kinds: reference CPU library)");
+               : Status(ErrorCode::NOT_IMPLEMENTED, "the GPU runtime holds FP32 / FP16 / SQI8 storage (LVQ and LeanVec: reference CPU library)");
 }
 
 Status VamanaIndex::build(VamanaIndex** index, size_t dim, MetricType metric, StorageKind storage_kind, const BuildParams& params,

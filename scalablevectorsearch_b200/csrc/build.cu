@@ -1,9 +1,11 @@
 // build.cu -- host side of the GPU Vamana graph builder (SURVEY.md §8 f1) + its small helper kernels.
 // Replaces index::vamana::auto_build / VamanaBuilder::construct (index/vamana/index.h:404-440,968-994,
 // vamana_build.h:221-310) for float32 / float16 / int8 / uint8 data with L2, inner-product or cosine distance.  Integer
-// rows are built with exact int x int distances, float rows with the fp32 expression tree of the search.
+// rows are built with exact int x int distances, float rows with the fp32 expression tree of the search, SQ codes with
+// the SQ search's distances from each decompressed datum (svsb200_build_vamana_sq).
 #include "build_kernels.cuh"
 #include "host.cuh"
+#include "ivf.cuh"   // sq_check_params
 
 #include <type_traits>
 #include <vector>
@@ -249,7 +251,10 @@ static int build_search_config(const char* who, const GraphBuild& b, SearchParam
     p->row_stride = b.row_stride;
     p->gstride = b.gstride;
     p->greater = b.metric != SVSB200_L2;
-    p->scale = 1.f;
+    p->sq = b.sq;
+    p->scale = b.sq ? b.scale : 1.f;
+    p->bias = b.bias;
+    p->scale_sq = b.scale * b.scale;   // EuclideanCompressed ctor (scalar.h:68-72)
     p->qcodes = nullptr;
     p->qstride = query_stride(b.dim);
     p->k = 0;
@@ -310,7 +315,12 @@ int construct_graph(const char* who, const GraphBuild& b, float reverse_alpha, u
     CUDA_TRY(cudaMemsetAsync(d_counts.ptr + 2, 0, 4, stream));
     CUDA_TRY(d_hist.ensure(batchsize * size_t(p.hist_cap)));
     CUDA_TRY(d_hist_count.ensure(batchsize));
-    const bool ints = int_dtype(dtype);
+    // integer rows: int x int distances throughout, as the reference's default build adaptor uses the datum itself as
+    // the query (extensions.h:114-282); SQ codes: the SQ search's operators over the decompressed datum
+    const int op = b.sq ? (b.metric == SVSB200_L2 ? OP_L2I : b.metric == SVSB200_IP ? OP_IPF : OP_COSF)
+                 : int_dtype(dtype) ? (b.metric == SVSB200_L2 ? OP_L2I : b.metric == SVSB200_IP ? OP_IPI : OP_COSI)
+                                    : (b.metric == SVSB200_L2 ? OP_L2F : b.metric == SVSB200_IP ? OP_IPF : OP_COSF);
+    const bool ints = op >= OP_L2I;
     if (ints) CUDA_TRY(d_qcodes.ensure(batchsize * size_t(qstride)));
     else CUDA_TRY(d_qf.ensure(batchsize * size_t(qstride)));
     CUDA_TRY(d_qaux.ensure(batchsize * 2));
@@ -323,10 +333,6 @@ int construct_graph(const char* who, const GraphBuild& b, float reverse_alpha, u
     p.work_counter = d_work.ptr;
     p.hist = d_hist.ptr;
     p.hist_count = d_hist_count.ptr;
-    // integer rows: int x int distances throughout, as the reference's default build adaptor uses the datum itself as
-    // the query (extensions.h:114-282)
-    const int op = ints ? (b.metric == SVSB200_L2 ? OP_L2I : b.metric == SVSB200_IP ? OP_IPI : OP_COSI)
-                        : (b.metric == SVSB200_L2 ? OP_L2F : b.metric == SVSB200_IP ? OP_IPF : OP_COSF);
 
     BuildParams bp{};
     bp.hist = d_hist.ptr;
@@ -348,24 +354,38 @@ int construct_graph(const char* who, const GraphBuild& b, float reverse_alpha, u
     bp.slots = d_slots;
     const int prune_grid = b.sm_count * 16;
     const char* vectors = static_cast<const char*>(b.vectors);
+    auto prune = [&](int grid) {
+        if (b.sq) return dispatch(BuildSqRows{}, dtype, [&](auto t) { return launch_build_prune_sq<decltype(t)::value>(op, p, bp, grid, stream); });
+        return dispatch(DataRows{}, dtype, [&](auto t) { return launch_build_prune_op<decltype(t)::value>(op, p, bp, grid, stream); });
+    };
 
     for (size_t bi = 0; bi < num_batches; ++bi) {
         const size_t start = std::min(count, batchsize * bi), stop = std::min(count, batchsize * (bi + 1));
         if (stop == start) continue;
         const uint32_t B = uint32_t(stop - start);
         // 1. generate_neighbors: search ...
-        CUDA_TRY(dispatch(DataRows{}, dtype, [&](auto t) {
-            constexpr int T = decltype(t)::value;
-            if constexpr (T == SVSB200_I8 || T == SVSB200_U8)
-                batch_codes_kernel<T><<<(B + 7) / 8, 256, 0, stream>>>(vectors, row_stride, uint32_t(b.dim), qstride, uint32_t(start), B, d_slots, d_qcodes.ptr, d_qaux.ptr);
-            else
-                batch_queries_kernel<T><<<(B + 7) / 8, 256, 0, stream>>>(vectors, row_stride, uint32_t(b.dim), qstride, uint32_t(start), B, d_slots, d_qf.ptr, d_qaux.ptr);
-            return cudaSuccess;
-        }));
-        count_launch();
+        if (b.sq) {
+            CUDA_TRY(dispatch(BuildSqRows{}, dtype, [&](auto t) {
+                return launch_build_batch_sq<decltype(t)::value>(op, p, uint32_t(start), B, d_slots, d_qf.ptr, d_qcodes.ptr,
+                                                                 d_qaux.ptr, stream);
+            }));
+        } else {
+            CUDA_TRY(dispatch(DataRows{}, dtype, [&](auto t) {
+                constexpr int T = decltype(t)::value;
+                if constexpr (T == SVSB200_I8 || T == SVSB200_U8)
+                    batch_codes_kernel<T><<<(B + 7) / 8, 256, 0, stream>>>(vectors, row_stride, uint32_t(b.dim), qstride, uint32_t(start), B, d_slots, d_qcodes.ptr, d_qaux.ptr);
+                else
+                    batch_queries_kernel<T><<<(B + 7) / 8, 256, 0, stream>>>(vectors, row_stride, uint32_t(b.dim), qstride, uint32_t(start), B, d_slots, d_qf.ptr, d_qaux.ptr);
+                return cudaSuccess;
+            }));
+            count_launch();
+        }
         CUDA_TRY(cudaMemsetAsync(d_work.ptr, 0, 4, stream));
         p.nq = B;
-        CUDA_TRY(dispatch(DataRows{}, dtype, [&](auto t) { return launch_build_search<decltype(t)::value>(op, p, cfg); }));
+        // SQ L2: the integer builder's OP_L2I search, which reads SearchParams::sq
+        CUDA_TRY(b.sq && op != OP_L2I
+                     ? dispatch(BuildSqRows{}, dtype, [&](auto t) { return launch_build_search_sq<decltype(t)::value>(op, p, cfg); })
+                     : dispatch(DataRows{}, dtype, [&](auto t) { return launch_build_search<decltype(t)::value>(op, p, cfg); }));
         // ... pool + prune (always with the configured alpha, vamana_build.h:268-272)
         CUDA_TRY(cudaMemsetAsync(d_work.ptr, 0, 4, stream));
         bp.reverse = PRUNE_FORWARD;
@@ -373,9 +393,7 @@ int construct_graph(const char* who, const GraphBuild& b, float reverse_alpha, u
         bp.count = B;
         bp.limit = R;
         bp.alpha = b.alpha;
-        CUDA_TRY(dispatch(DataRows{}, dtype, [&](auto t) {
-            return launch_build_prune_op<decltype(t)::value>(op, p, bp, std::min<int>(prune_grid, int(B)), stream);
-        }));
+        CUDA_TRY(prune(std::min<int>(prune_grid, int(B))));
         // 2. add_reverse_edges
         CUDA_TRY(cudaMemsetAsync(d_counts.ptr, 0, 8, stream));
         reverse_insert_kernel<<<unsigned((size_t(B) * R + 255) / 256), 256, 0, stream>>>(
@@ -386,9 +404,7 @@ int construct_graph(const char* who, const GraphBuild& b, float reverse_alpha, u
         bp.reverse = PRUNE_REVERSE;
         bp.limit = uint32_t(b.prune_to);
         bp.alpha = reverse_alpha;
-        CUDA_TRY(dispatch(DataRows{}, dtype, [&](auto t) {
-            return launch_build_prune_op<decltype(t)::value>(op, p, bp, prune_grid, stream);
-        }));
+        CUDA_TRY(prune(prune_grid));
         reset_heads_kernel<<<unsigned((pair_cap + 255) / 256), 256, 0, stream>>>(d_touched.ptr, d_counts.ptr + 1, d_head.ptr);
         count_launch();
         CUDA_TRY(cudaGetLastError());
@@ -406,26 +422,28 @@ int construct_graph(const char* who, const GraphBuild& b, float reverse_alpha, u
 
 using namespace svsb200;
 
-extern "C" int svsb200_build_vamana(const void* vectors, int dtype, size_t n, size_t dim, size_t row_stride_bytes, int metric,
-                                    float alpha, size_t graph_max_degree, size_t window_size,
-                                    size_t max_candidate_pool_size, size_t prune_to, int device, uint32_t* graph_rows_out,
-                                    uint32_t* entry_point_out) {
-    const char* who = "svsb200_build_vamana";
-    if (!vectors || !graph_rows_out || !entry_point_out) return fail("svsb200_build_vamana: NULL argument");
-    if (dtype < SVSB200_F32 || dtype > SVSB200_U8) return fail("svsb200_build_vamana: bad dtype");
-    if (metric < SVSB200_L2 || metric > SVSB200_COSINE) return fail("svsb200_build_vamana: bad metric");
-    if (n < 2 || dim == 0 || n >= (size_t(1) << 31)) return fail("svsb200_build_vamana: bad shape");
-    if (graph_max_degree == 0 || graph_max_degree > 32u * kFastMaxGW) return fail("svsb200_build_vamana: graph_max_degree must be in [1, 128]");
-    if (window_size == 0) return fail("svsb200_build_vamana: window_size must be positive");
+// The static build of both entry points; `sq` marks int8 / uint8 rows as SQ codes of `scale` and `bias`.  Errors read
+// "<who>: ...".
+static int build_static(const char* who, const void* vectors, int dtype, size_t n, size_t dim, size_t row_stride_bytes,
+                        int metric, bool sq, float scale, float bias, float alpha, size_t graph_max_degree,
+                        size_t window_size, size_t max_candidate_pool_size, size_t prune_to, int device,
+                        uint32_t* graph_rows_out, uint32_t* entry_point_out) {
+    const std::string w = who;
+    if (!vectors || !graph_rows_out || !entry_point_out) return fail(w + ": NULL argument");
+    if (dtype < SVSB200_F32 || dtype > SVSB200_U8) return fail(w + ": bad dtype");
+    if (metric < SVSB200_L2 || metric > SVSB200_COSINE) return fail(w + ": bad metric");
+    if (n < 2 || dim == 0 || n >= (size_t(1) << 31)) return fail(w + ": bad shape");
+    if (graph_max_degree == 0 || graph_max_degree > 32u * kFastMaxGW) return fail(w + ": graph_max_degree must be in [1, 128]");
+    if (window_size == 0) return fail(w + ": window_size must be positive");
     // verify_and_set_default_index_parameters (index/vamana/index.h:1079-1110)
     // The candidate pool holds kPoolMax entries: the default is clamped to it, a larger value refused.
     if (max_candidate_pool_size == 0) max_candidate_pool_size = std::min<size_t>(3 * window_size, kPoolMax);
     if (max_candidate_pool_size > kPoolMax)
-        return fail("svsb200_build_vamana: max_candidate_pool_size above 512, the GPU builder's candidate pool");
+        return fail(w + ": max_candidate_pool_size above 512, the GPU builder's candidate pool");
     if (prune_to == 0) prune_to = graph_max_degree >= 16 ? graph_max_degree - 4 : graph_max_degree;
-    if (prune_to > graph_max_degree) return fail("svsb200_build_vamana: prune_to must be <= graph_max_degree");
+    if (prune_to > graph_max_degree) return fail(w + ": prune_to must be <= graph_max_degree");
     if (alpha == 0.f) alpha = metric == SVSB200_L2 ? 1.2f : 0.95f;
-    if (metric == SVSB200_L2 ? alpha < 1.0f : alpha > 1.0f) return fail("svsb200_build_vamana: alpha on the wrong side of 1 for this metric");
+    if (metric == SVSB200_L2 ? alpha < 1.0f : alpha > 1.0f) return fail(w + ": alpha on the wrong side of 1 for this metric");
     const uint32_t R = uint32_t(graph_max_degree);
     cudaDeviceProp prop;
     if (int rc = check_device(who, device, &prop)) return rc;
@@ -445,6 +463,9 @@ extern "C" int svsb200_build_vamana(const void* vectors, int dtype, size_t n, si
     b.max_candidates = max_candidate_pool_size;
     b.prune_to = prune_to;
     b.alpha = alpha;
+    b.sq = sq;
+    b.scale = scale;
+    b.bias = bias;
     b.sm_count = prop.multiProcessorCount;
     if (int rc = check_construct(who, b)) return rc;
 
@@ -483,4 +504,24 @@ extern "C" int svsb200_build_vamana(const void* vectors, int dtype, size_t n, si
     CUDA_TRY(cudaStreamSynchronize(stream));
     *entry_point_out = entry_point;
     return 0;
+}
+
+extern "C" int svsb200_build_vamana(const void* vectors, int dtype, size_t n, size_t dim, size_t row_stride_bytes, int metric,
+                                    float alpha, size_t graph_max_degree, size_t window_size,
+                                    size_t max_candidate_pool_size, size_t prune_to, int device, uint32_t* graph_rows_out,
+                                    uint32_t* entry_point_out) {
+    return build_static("svsb200_build_vamana", vectors, dtype, n, dim, row_stride_bytes, metric, false, 1.f, 0.f, alpha,
+                        graph_max_degree, window_size, max_candidate_pool_size, prune_to, device, graph_rows_out,
+                        entry_point_out);
+}
+
+extern "C" int svsb200_build_vamana_sq(const void* codes, int code_type, size_t n, size_t dim, int metric, float scale,
+                                       float bias, float alpha, size_t graph_max_degree, size_t window_size,
+                                       size_t max_candidate_pool_size, size_t prune_to, int device, uint32_t* graph_rows_out,
+                                       uint32_t* entry_point_out) {
+    const char* who = "svsb200_build_vamana_sq";
+    if (code_type != SVSB200_I8 && code_type != SVSB200_U8) return fail("svsb200_build_vamana_sq: codes must be int8 or uint8");
+    if (int rc = sq_check_params(who, scale, bias)) return rc;
+    return build_static(who, codes, code_type, n, dim, 0, metric, true, scale, bias, alpha, graph_max_degree, window_size,
+                        max_candidate_pool_size, prune_to, device, graph_rows_out, entry_point_out);
 }

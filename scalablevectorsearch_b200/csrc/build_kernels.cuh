@@ -23,12 +23,16 @@
 // (tests/integration/vamana/index_build.cpp:96,139).
 // Distances inside the builder use the search path's bit-exact code (eval_pass), keys = sign * distance: the float tree
 // for float32 / float16 rows, the exact integer ops (OP_*I) for int8 / uint8 rows, whose datum is its own query.
+// SQ rows (int8 / uint8 codes with one global scale and bias, SQ = true) follow the reference's VamanaBuildAdaptor for
+// SQ data (extensions/vamana/scalar.h:47-86): the datum is decompressed and prepared as the SQ search prepares an fp32
+// query (stage_sq_datum), then measured with the SQ search's operators (OP_L2I scaled by scale^2, OP_IPF, OP_COSF).
 //
 // The dynamic index reuses these kernels: add_points runs `construct` over a list of slots (BuildParams::slots),
 // and consolidate (consolidate.h) selects each node's candidate pool with `consolidate_pool_kernel` and prunes it
 // with `build_prune_kernel` in mode CONSOLIDATE.
 #pragma once
 
+#include "query_prep.cuh"
 #include "search_fast.cuh"
 
 #include <cfloat>
@@ -118,14 +122,56 @@ __device__ __forceinline__ float codes_norm(const char* row, uint32_t dim, int x
     return __fsqrt_rn(acc);
 }
 
+// An SQ datum as its own query: DecompressionAdaptor::fix_argument (quantization/scalar/scalar.h:583-589) decompresses
+// the codes to fp32 and hands them to the compressed distance's fix_argument, which is what prepare_queries_kernel
+// does for an fp32 query of the SQ search (query_prep.cuh).  OP_L2I (EuclideanCompressed): the fp32 row compressed
+// again -- the round trip need not return the datum's codes -- to qstride bytes at `dst`, `aux1` = the int32 bits of
+// their sum x*x.  OP_IPF / OP_COSF: the fp32 row, zero-padded to qstride floats at `dst`; returns the MIP offset or the
+// cosine norm.  One warp; `dst` in shared or global memory.
+template <int ROWT, int OP>
+__device__ __forceinline__ float stage_sq_datum(const SearchParams& p, const char* row, void* dst, int lane, float& aux1) {
+    auto code = [&](uint32_t i) { return ROWT == SVSB200_I8 ? int(int8_t(row[i])) : int(uint8_t(row[i])); };
+    if constexpr (OP == OP_L2I) {
+        uint8_t* c = static_cast<uint8_t*>(dst);
+        int xx = 0;
+        for (uint32_t i = lane; i < p.qstride; i += 32) {
+            uint8_t cv = 0;
+            if (i < p.dim) {
+                cv = sq_compress_code(sq_decompress(code(i), p.scale, p.bias), ROWT, p.scale, p.bias);
+                const int v = ROWT == SVSB200_I8 ? int(int8_t(cv)) : int(cv);
+                xx += v * v;
+            }
+            c[i] = cv;
+        }
+        for (int o = 16; o; o >>= 1) xx += __shfl_xor_sync(0xFFFFFFFFu, xx, o);
+        aux1 = __int_as_float(xx);
+        __syncwarp();
+        return 0.f;
+    } else {
+        static_assert(OP == OP_IPF || OP == OP_COSF, "SQ builds measure with OP_L2I, OP_IPF or OP_COSF");
+        float* f = static_cast<float*>(dst);
+        for (uint32_t i = lane; i < p.qstride; i += 32) f[i] = i < p.dim ? sq_decompress(code(i), p.scale, p.bias) : 0.f;
+        __syncwarp();
+        float aux0 = 0.f;
+        if (lane == 0) {
+            if constexpr (OP == OP_IPF) aux0 = sq_ip_offset(f, p.dim, p.bias);
+            else aux0 = sequential_norm(p.dim, [&](uint32_t i) { return __fmul_rn(f[i], f[i]); });
+        }
+        return __shfl_sync(0xFFFFFFFFu, aux0, 0);
+    }
+}
+
 // Row `id` of the dataset as the operand the distance code expects in q_s (what prepare_queries_kernel does for a
 // query): for the float ops the exact fp32 conversion, zero padding; for the integer ops the raw codes (stage_codes),
-// with `aux1` = the int32 bits of sum x*x that OP_L2I needs.
-// Returns the row's Euclidean norm (the `a_norm` of CosineSimilarity::fix_argument, cosine.h:117-119).
-template <int ROWT, int OP>
+// with `aux1` = the int32 bits of sum x*x that OP_L2I needs; for SQ rows stage_sq_datum.
+// Returns the row's Euclidean norm (the `a_norm` of CosineSimilarity::fix_argument, cosine.h:117-119), or for SQ rows
+// stage_sq_datum's value.
+template <int ROWT, int OP, bool SQ = false>
 __device__ __forceinline__ float stage_row(const SearchParams& p, uint32_t id, float* q_s, int lane, float& aux1) {
     const char* row = reinterpret_cast<const char*>(p.vectors) + size_t(id) * p.row_stride;
-    if constexpr (OP >= OP_L2I) {
+    if constexpr (SQ) {
+        return stage_sq_datum<ROWT, OP>(p, row, q_s, lane, aux1);
+    } else if constexpr (OP >= OP_L2I) {
         const int xx = stage_codes<ROWT>(row, p.dim, p.qstride, reinterpret_cast<uint32_t*>(q_s), lane);
         aux1 = __int_as_float(xx);
         return codes_norm<ROWT>(row, p.dim, xx, lane);
@@ -205,8 +251,8 @@ __device__ __forceinline__ uint32_t merge_into_pool(float* ckey, uint32_t* cid, 
     return out;
 }
 
-template <int ROWT, int OP, int DS, int KS>
-__global__ void __launch_bounds__(32, 16) build_prune_kernel(const __grid_constant__ SearchParams p,
+template <int ROWT, int OP, int DS, int KS, bool SQ = false>
+__global__ void __launch_bounds__(32, SQ ? kSqBuildMinBlocks : 16) build_prune_kernel(const __grid_constant__ SearchParams p,
                                                             const __grid_constant__ BuildParams bp) {
     constexpr int G = OP >= OP_L2I ? 4 : KS * 16 / Row<ROWT>::LPT;   // threads per row, as in eval_pass
     constexpr int GROUPS = 32 / G;
@@ -243,7 +289,7 @@ __global__ void __launch_bounds__(32, 16) build_prune_kernel(const __grid_consta
         float qaux1 = 0.f;    // OP_L2I: int32 bits of sum x*x of the vector currently staged as the query
         if (bp.reverse == PRUNE_CONSOLIDATE) {
             // the whole pool, keys included, as consolidate_pool_kernel selected it
-            qnorm = stage_row<ROWT, OP>(p, node, q_s, lane, qaux1);
+            qnorm = stage_row<ROWT, OP, SQ>(p, node, q_s, lane, qaux1);
             P = min(bp.hist_count[w], min(bp.hist_cap, kPoolMax));
             for (uint32_t i = lane; i < P; i += 32) {
                 const uint2 e = bp.hist[size_t(w) * bp.hist_cap + i];
@@ -314,7 +360,7 @@ __global__ void __launch_bounds__(32, 16) build_prune_kernel(const __grid_consta
                 }
             }
         } else {
-            qnorm = stage_row<ROWT, OP>(p, node, q_s, lane, qaux1);
+            qnorm = stage_row<ROWT, OP, SQ>(p, node, q_s, lane, qaux1);
             // overflow edges of this round (vamana_build.h:528-531): one per node of the round that links here, so
             // they are distinct and none is the node itself
             uint32_t nover = 0;
@@ -428,7 +474,7 @@ __global__ void __launch_bounds__(32, 16) build_prune_kernel(const __grid_consta
                     res[nres] = cid[j];
                 }
                 ++nres;
-                qnorm = stage_row<ROWT, OP>(p, cid[j], q_s, lane, qaux1);
+                qnorm = stage_row<ROWT, OP, SQ>(p, cid[j], q_s, lane, qaux1);
                 __syncwarp();
                 // the later entries still available at this level, compacted
                 uint32_t L = 0;
@@ -588,6 +634,52 @@ cudaError_t launch_build_prune_op(int op, const SearchParams& p, const BuildPara
         });
     });
 }
+// SQ rows: batch rows [first, first+count) (or slots[first + q]) prepared as their own queries (stage_sq_datum) into
+// qcodes (OP_L2I) or qf, and qaux = {aux0, aux1}.  One warp per row.
+template <int ROWT, int OP>
+__global__ void batch_sq_kernel(const __grid_constant__ SearchParams p, uint32_t first, uint32_t count,
+                                const uint32_t* __restrict__ slots, float* __restrict__ qf, uint8_t* __restrict__ qcodes,
+                                float* __restrict__ qaux) {
+    const uint32_t q = blockIdx.x * (blockDim.x / 32) + threadIdx.x / 32;
+    const int lane = threadIdx.x & 31;
+    if (q >= count) return;
+    const char* row = reinterpret_cast<const char*>(p.vectors) + size_t(slots ? slots[first + q] : first + q) * p.row_stride;
+    void* dst = OP == OP_L2I ? static_cast<void*>(qcodes + size_t(q) * p.qstride) : static_cast<void*>(qf + size_t(q) * p.qstride);
+    float aux1 = 0.f;
+    const float aux0 = stage_sq_datum<ROWT, OP>(p, row, dst, lane, aux1);
+    if (lane == 0) {
+        qaux[2 * size_t(q)] = aux0;
+        qaux[2 * size_t(q) + 1] = aux1;
+    }
+}
+
+// The SQ builder's launchers (BuildSqOps), instantiated once per code type in build_sq_<type>.cu.  The lean search's
+// OP_L2I form reads SearchParams::sq at run time, so the integer builder's launch_build_search serves SQ L2; this one
+// takes OP_IPF and OP_COSF.
+template <int ROWT> cudaError_t launch_build_search_sq(int op, const SearchParams& p, const LaunchConfig& cfg) {
+    return dispatch(IntList<OP_IPF, OP_COSF>{}, op, [&](auto o) { return launch_fast<ROWT, decltype(o)::value, true, false>(p, cfg); });
+}
+template <int ROWT>
+cudaError_t launch_build_prune_sq(int op, const SearchParams& p, const BuildParams& bp, int grid, cudaStream_t stream) {
+    const LaunchConfig cfg{grid, 1, build_smem_bytes(p.qstride), stream};
+    return dispatch(BuildSqOps{}, op, [&](auto o) {
+        constexpr int OP = decltype(o)::value;
+        return with_shape<OP, false>(p.dim, true, [&](auto ds, auto ks) {
+            return launch_kernel(build_prune_kernel<ROWT, OP, decltype(ds)::value, decltype(ks)::value, true>, cfg, grid,
+                                 true, p, bp);
+        });
+    });
+}
+template <int ROWT>
+cudaError_t launch_build_batch_sq(int op, const SearchParams& p, uint32_t first, uint32_t count, const uint32_t* slots,
+                                  float* qf, uint8_t* qcodes, float* qaux, cudaStream_t stream) {
+    const LaunchConfig cfg{int((count + 7) / 8), 8, 0, stream};
+    return dispatch(BuildSqOps{}, op, [&](auto o) {
+        return launch_kernel(batch_sq_kernel<ROWT, decltype(o)::value>, cfg, size_t(cfg.grid), false, p, first, count,
+                             slots, qf, qcodes, qaux);
+    });
+}
+
 template <int ROWT>
 cudaError_t launch_consolidate_pool_op(int op, const SearchParams& p, const BuildParams& bp, int grid, cudaStream_t stream) {
     const LaunchConfig cfg{grid, 1, size_t(p.qstride) * 4, stream};
@@ -608,6 +700,14 @@ extern template cudaError_t launch_build_prune_op<SVSB200_F32>(int, const Search
 extern template cudaError_t launch_build_prune_op<SVSB200_F16>(int, const SearchParams&, const BuildParams&, int, cudaStream_t);
 extern template cudaError_t launch_build_prune_op<SVSB200_I8>(int, const SearchParams&, const BuildParams&, int, cudaStream_t);
 extern template cudaError_t launch_build_prune_op<SVSB200_U8>(int, const SearchParams&, const BuildParams&, int, cudaStream_t);
+extern template cudaError_t launch_build_search_sq<SVSB200_I8>(int, const SearchParams&, const LaunchConfig&);
+extern template cudaError_t launch_build_search_sq<SVSB200_U8>(int, const SearchParams&, const LaunchConfig&);
+extern template cudaError_t launch_build_prune_sq<SVSB200_I8>(int, const SearchParams&, const BuildParams&, int, cudaStream_t);
+extern template cudaError_t launch_build_prune_sq<SVSB200_U8>(int, const SearchParams&, const BuildParams&, int, cudaStream_t);
+extern template cudaError_t launch_build_batch_sq<SVSB200_I8>(int, const SearchParams&, uint32_t, uint32_t, const uint32_t*,
+                                                             float*, uint8_t*, float*, cudaStream_t);
+extern template cudaError_t launch_build_batch_sq<SVSB200_U8>(int, const SearchParams&, uint32_t, uint32_t, const uint32_t*,
+                                                             float*, uint8_t*, float*, cudaStream_t);
 extern template cudaError_t launch_consolidate_pool_op<SVSB200_F32>(int, const SearchParams&, const BuildParams&, int, cudaStream_t);
 extern template cudaError_t launch_consolidate_pool_op<SVSB200_F16>(int, const SearchParams&, const BuildParams&, int, cudaStream_t);
 

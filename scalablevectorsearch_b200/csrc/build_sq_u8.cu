@@ -1,0 +1,11 @@
+// build_sq_u8.cu -- graph-builder kernel instantiations for SQ uint8 codes: the SQ search's operators (BuildSqOps).
+#include "build_kernels.cuh"
+
+namespace svsb200 {
+
+template cudaError_t launch_build_search_sq<SVSB200_U8>(int, const SearchParams&, const LaunchConfig&);
+template cudaError_t launch_build_prune_sq<SVSB200_U8>(int, const SearchParams&, const BuildParams&, int, cudaStream_t);
+template cudaError_t launch_build_batch_sq<SVSB200_U8>(int, const SearchParams&, uint32_t, uint32_t, const uint32_t*, float*,
+                                                        uint8_t*, float*, cudaStream_t);
+
+}  // namespace svsb200

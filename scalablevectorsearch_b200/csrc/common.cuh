@@ -120,12 +120,14 @@ constexpr size_t kSmemOptInMax = 227 * 1024;   // dynamic shared memory a block 
 //   family                                        rows      F32, F16       I8, U8            LVQ8
 //   generic search, exhaustive scan, lean search  SearchRows  L2F IPF COSF   all six           L2F IPF
 //   builder search (HIST), builder prune          DataRows    L2F IPF COSF   L2I IPI COSI      -
+//   the same over SQ codes (build_sq_<type>.cu)   BuildSqRows -              L2I IPF COSF      -
 //   consolidate pool, dynamic search (MUT)        DynamicRows L2F IPF COSF   -                 -
 //   flat rescore                                  DataRows    L2F IPF        L2F IPF L2I IPI   -
 //   IVF leaf scan (ivf_kernel.cuh)                IvfRows     L2F IPF COSF   -                 -
 //   IVF leaf scan over SQ codes                   IvfSqRows   -              IPF COSF (+ the
 //                                                                            tensor-core L2 leaf)
-// int8 / uint8 rows take float and integer queries in a search; the builder's datum is its own query.
+// int8 / uint8 rows take float and integer queries in a search; the builder's datum is its own query.  Over SQ codes
+// the builder's datum is decompressed and prepared as the SQ search's fp32 query, so it takes the SQ search's operators.
 template <int... V> struct IntList {};
 template <int ROWT> constexpr bool kIntRow = ROWT == SVSB200_I8 || ROWT == SVSB200_U8;
 using FloatOps = IntList<OP_L2F, OP_IPF, OP_COSF>;
@@ -139,6 +141,8 @@ using SearchOps = std::conditional_t<ROWT == ROW_LVQ8, IntList<OP_L2F, OP_IPF>,
                                      std::conditional_t<kIntRow<ROWT>, IntList<OP_L2F, OP_IPF, OP_COSF, OP_L2I, OP_IPI, OP_COSI>,
                                                         FloatOps>>;
 template <int ROWT> using BuildOps = std::conditional_t<kIntRow<ROWT>, IntOps, FloatOps>;
+using BuildSqRows = IntList<SVSB200_I8, SVSB200_U8>;
+using BuildSqOps = IntList<OP_L2I, OP_IPF, OP_COSF>;
 using DynamicOps = FloatOps;
 using IvfRows = IntList<SVSB200_F32, SVSB200_F16>;
 using IvfOps = FloatOps;

@@ -321,6 +321,8 @@ struct GraphBuild {
     uint32_t* deg = nullptr;
     size_t window = 0, max_candidates = 0, prune_to = 0;
     float alpha = 1.f;                // forward pruning
+    bool sq = false;                  // int8 / uint8 rows are SQ codes of `scale` and `bias` (svsb200_build_vamana_sq)
+    float scale = 1.f, bias = 0.f;
     int sm_count = 0;
     cudaStream_t stream = nullptr;
 };

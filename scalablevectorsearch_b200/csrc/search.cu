@@ -2,6 +2,7 @@
 // kernel choice and launch, the blocking / enqueue-only / cancellable / sharded / filtered / range / exhaustive entry
 // points, result gather, and the counters and kernel time of the last search.
 #include "host.cuh"
+#include "query_prep.cuh"
 
 #include <algorithm>
 #include <chrono>
@@ -58,11 +59,7 @@ __global__ void prepare_queries_kernel(const void* __restrict__ queries, uint32_
             } else if (mode == PREP_INT) {
                 if constexpr (QT == SVSB200_I8 || QT == SVSB200_U8) cv = static_cast<const uint8_t*>(src)[i];
             } else if (mode == PREP_SQ_L2) {
-                // detail::compress (scalar.h:38-42)
-                const float lo = code_type == SVSB200_I8 ? -128.f : 0.f, hi = code_type == SVSB200_I8 ? 127.f : 255.f;
-                float r = roundf(__fdiv_rn(__fsub_rn(q_scalar<QT>(src, i), bias), scale));
-                r = fminf(fmaxf(r, lo), hi);
-                cv = code_type == SVSB200_I8 ? uint8_t(int8_t(int(r))) : uint8_t(int(r));
+                cv = sq_compress_code(q_scalar<QT>(src, i), code_type, scale, bias);
             } else {
                 fv = q_scalar<QT>(src, i);
             }
@@ -85,35 +82,21 @@ __global__ void prepare_queries_kernel(const void* __restrict__ queries, uint32_
     }
     const bool need_norm = (metric == SVSB200_COSINE) && (mode == PREP_FLOAT || mode == PREP_INT || mode == PREP_SQ_COS);
     if (need_norm) {
-        // distance::norm (distance_core.h:45-66): sequential fp32 `accum += v * v`, sqrt.
-        float acc = 0.f;
-        for (uint32_t i = 0; i < dim; ++i) {
-            float sq;
+        aux0 = sequential_norm(dim, [&](uint32_t i) {
             if constexpr (QT == SVSB200_I8 || QT == SVSB200_U8) {
                 int v = QT == SVSB200_I8 ? int(static_cast<const int8_t*>(src)[i]) : int(static_cast<const uint8_t*>(src)[i]);
-                sq = float(v * v);
+                return float(v * v);
             } else {
                 float v = q_scalar<QT>(src, i);
-                sq = __fmul_rn(v, v);
+                return __fmul_rn(v, v);
             }
-            acc = __fadd_rn(acc, sq);
-        }
-        aux0 = __fsqrt_rn(acc);
+        });
     } else if (mode == PREP_LVQ_IP) {
         float acc = 0.f;
         for (uint32_t i = 0; i < dim; ++i) acc = __fmaf_rn(f[i], mean[i], acc);
         aux0 = acc;
     } else if (mode == PREP_SQ_IP) {
-        // std::reduce over the fp32 query (libstdc++: four at a time, then the tail).
-        float acc = 0.f;
-        uint32_t i = 0;
-        for (; i + 4 <= dim; i += 4) {
-            float v1 = __fadd_rn(f[i], f[i + 1]);
-            float v2 = __fadd_rn(f[i + 2], f[i + 3]);
-            acc = __fadd_rn(acc, __fadd_rn(v1, v2));
-        }
-        for (; i < dim; ++i) acc = __fadd_rn(acc, f[i]);
-        aux0 = __fmul_rn(bias, acc);
+        aux0 = sq_ip_offset(f, dim, bias);
     }
     qaux[2 * size_t(q)] = aux0;
     qaux[2 * size_t(q) + 1] = aux1;

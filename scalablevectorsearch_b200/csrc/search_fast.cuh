@@ -30,11 +30,14 @@ namespace svsb200 {
 // Resident CTAs (= warps = queries) per SM the compiler must allow for: 16 (128 registers).  On sm_90 the
 // 80-register budget of 24 CTAs spills in most instantiations (ptxas -v, csrc/*.ptxas.log), and on the C2 workload
 // (H100 SXM, 400 W) 24 CTAs ran at 2.9 M QPS against 4.3 M with 16.
-template <int ROWT, int OP, int DS, int KS> constexpr int fast_min_blocks() {
+// The graph builder's kernels over SQ codes with a float operator (MIP, cosine) decompress every element of a row on
+// the fly; at 128 registers they spill, so they are compiled for 8 CTAs per SM (up to 255 registers, no spills; ptxas -v).
+constexpr int kSqBuildMinBlocks = 8;
+template <int ROWT, int OP, int DS, int KS, bool HIST = false> constexpr int fast_min_blocks() {
 #ifdef SVSB200_FAST_MIN_BLOCKS
     return SVSB200_FAST_MIN_BLOCKS;
 #else
-    return 16;
+    return HIST && kIntRow<ROWT> && OP < OP_L2I ? kSqBuildMinBlocks : 16;
 #endif
 }
 
@@ -63,7 +66,7 @@ static __device__ unsigned long long g_phase_clocks[8];   // (one copy per trans
 // entries, and a query whose cut point would lie beyond them stops, lists itself in `ovf` and is re-run by the host
 // with more room.  The copy-out is cleanup() + the first k valid entries, as external ids.
 template <int ROWT, int OP, int DS, int KS, bool HIST = false, bool MUT = false>
-__global__ void __launch_bounds__(32, fast_min_blocks<ROWT, OP, DS, KS>()) vamana_search_fast_kernel(const __grid_constant__ SearchParams p) {
+__global__ void __launch_bounds__(32, fast_min_blocks<ROWT, OP, DS, KS, HIST>()) vamana_search_fast_kernel(const __grid_constant__ SearchParams p) {
     constexpr int NROWS = 2;
     constexpr bool kInt = (OP >= OP_L2I);
     constexpr int G = kInt ? 4 : KS * 16 / Row<ROWT>::LPT;   // threads per row

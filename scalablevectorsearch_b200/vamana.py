@@ -144,24 +144,33 @@ class VamanaBuildParameters:
     use_full_search_history: bool = True
 
 
-def build_graph(data: np.ndarray, distance: "DistanceType", parameters: VamanaBuildParameters, device: int = 0):
+def build_graph(data: np.ndarray, distance: "DistanceType", parameters: VamanaBuildParameters, device: int = 0,
+                sq: tuple | None = None):
     """Vamana graph construction on the GPU (``svsb200_build_vamana``; stands where ``svs.Vamana.build`` /
     ``index::vamana::auto_build`` runs the reference's CPU builder).  Returns ``(graph uint32[n][R+1] in the
     reference's degree-first layout, entry_point)``.  int8 / uint8 rows are built with exact integer distances, as the
-    reference builds ``SimpleData<int8_t / uint8_t>``."""
+    reference builds ``SimpleData<int8_t / uint8_t>``.  ``sq=(scale, bias)`` marks ``data`` as scalar-quantised
+    int8 / uint8 codes (from :func:`scalablevectorsearch_b200.ivf.sq_compress`), built as the reference builds
+    ``SQDataset`` (``svsb200_build_vamana_sq``)."""
     data = np.ascontiguousarray(data)
     if data.dtype not in _DTYPE_CODE or data.ndim != 2:
         raise TypeError("build_graph takes a 2-D float32 / float16 / int8 / uint8 array")
+    if sq is not None and data.dtype not in (np.int8, np.uint8):
+        raise TypeError("SQ codes are int8 or uint8")
     if not parameters.use_full_search_history:
         raise ValueError("the GPU builder always keeps the full search history (the reference's default)")
     lib = _lib.lib()
     n, R = data.shape[0], int(parameters.graph_max_degree)
     graph = np.empty((n, R + 1), dtype=np.uint32)
     ep = C.c_uint32()
-    _lib.check(lib.svsb200_build_vamana(
-        data.ctypes.data, _DTYPE_CODE[data.dtype], n, data.shape[1], 0, int(distance), float(parameters.alpha), R,
-        int(parameters.window_size), int(parameters.max_candidate_pool_size), int(parameters.prune_to), int(device),
-        graph.ctypes.data, C.byref(ep)))
+    tail = (float(parameters.alpha), R, int(parameters.window_size), int(parameters.max_candidate_pool_size),
+            int(parameters.prune_to), int(device), graph.ctypes.data, C.byref(ep))
+    if sq is None:
+        _lib.check(lib.svsb200_build_vamana(data.ctypes.data, _DTYPE_CODE[data.dtype], n, data.shape[1], 0, int(distance),
+                                            *tail))
+    else:
+        _lib.check(lib.svsb200_build_vamana_sq(data.ctypes.data, _DTYPE_CODE[data.dtype], n, data.shape[1], int(distance),
+                                               float(sq[0]), float(sq[1]), *tail))
     return graph, int(ep.value)
 
 
@@ -170,13 +179,14 @@ class Vamana:
 
     @classmethod
     def build(cls, parameters: VamanaBuildParameters, data: np.ndarray, distance: "DistanceType" = None, device=0,
-              num_threads: int = 1) -> "Vamana":
+              num_threads: int = 1, sq: tuple | None = None) -> "Vamana":
         """``svs.Vamana.build(parameters, data_loader, distance_type, num_threads)``
-        (bindings/python/src/vamana.cpp:171-240): graph construction and the resulting index, all on the GPU."""
+        (bindings/python/src/vamana.cpp:171-240): graph construction and the resulting index, all on the GPU.
+        ``sq=(scale, bias)`` as in :meth:`from_arrays`: ``data`` are SQ codes, and the result is an SQ index."""
         distance = DistanceType.L2 if distance is None else distance
         dev0 = device[0] if isinstance(device, (list, tuple)) else device
-        graph, ep = build_graph(data, distance, parameters, dev0)
-        self = cls.from_arrays(data, graph, ep, distance, device=device, num_threads=num_threads)
+        graph, ep = build_graph(data, distance, parameters, dev0, sq=sq)
+        self = cls.from_arrays(data, graph, ep, distance, device=device, sq=sq, num_threads=num_threads)
         self.build_parameters = parameters
         return self
 
