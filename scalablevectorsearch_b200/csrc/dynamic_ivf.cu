@@ -483,12 +483,10 @@ int svsb200_dynamic_ivf_search_device(svsb200_dynamic_ivf* index, const void* d_
     if (nq == 0) return 0;
     if (!d_queries || !d_out_ids || !d_out_dists) return fail("svsb200_dynamic_ivf_search_device: NULL buffer");
     Replica* rep = index->iv.ix->reps[0].get();
-    CUDA_TRY(cudaSetDevice(rep->device));
-    std::string err;
-    Scratch* sc = scratch_for_stream(rep, static_cast<cudaStream_t>(stream_), &err);
-    if (!sc) return fail(err);
-    return ivf_search_on_device(&index->iv, sc, d_queries, qdtype, nq, k, n_probes, d_out_ids, d_out_dists,
-                                rep->d_ext_ids.ptr);
+    return run_on_stream(rep, stream_, [&](Scratch* sc) {
+        return ivf_search_on_device(&index->iv, sc, d_queries, qdtype, nq, k, n_probes, d_out_ids, d_out_dists,
+                                    rep->d_ext_ids.ptr);
+    });
 }
 
 int svsb200_dynamic_ivf_search(svsb200_dynamic_ivf* index, const void* queries, int qdtype, size_t nq, size_t k,
@@ -496,8 +494,12 @@ int svsb200_dynamic_ivf_search(svsb200_dynamic_ivf* index, const void* queries, 
     if (int rc = ivf_check_search("svsb200_dynamic_ivf_search", ivf_of(index), qdtype, k, n_probes)) return rc;
     if (nq == 0) return 0;
     if (!queries || !out_ids || !out_dists) return fail("svsb200_dynamic_ivf_search: NULL buffer");
-    return ivf_search_host(&index->iv, queries, qdtype, nq, k, n_probes, out_ids, out_dists,
-                           index->iv.ix->reps[0]->d_ext_ids.ptr);
+    Replica* rep = index->iv.ix->reps[0].get();
+    return run_host_search(rep, {queries, nullptr, out_ids, out_dists}, nq * index->iv.ix->dim * esize(qdtype), 0, nq, k,
+                           [&](Scratch* sc, const StagedBuffers& d) {
+                               return ivf_search_on_device(&index->iv, sc, d.queries, qdtype, nq, k, n_probes, d.ids, d.dists,
+                                                           rep->d_ext_ids.ptr);
+                           });
 }
 
 int svsb200_dynamic_ivf_search_filtered_device(svsb200_dynamic_ivf* index, const void* d_queries, int qdtype, size_t nq,
@@ -510,12 +512,10 @@ int svsb200_dynamic_ivf_search_filtered_device(svsb200_dynamic_ivf* index, const
     if (nq == 0) return 0;
     if (!d_queries || !d_out_ids || !d_out_dists) return fail("svsb200_dynamic_ivf_search_filtered_device: NULL buffer");
     Replica* rep = index->iv.ix->reps[0].get();
-    CUDA_TRY(cudaSetDevice(rep->device));
-    std::string err;
-    Scratch* sc = scratch_for_stream(rep, static_cast<cudaStream_t>(stream_), &err);
-    if (!sc) return fail(err);
-    return ivf_search_filtered_on_device(&index->iv, sc, d_queries, qdtype, nq, k, n_probes, d_slot_bitmap, d_out_ids,
-                                         d_out_dists, d_out_probes, d_out_allowed, d_out_rows, rep->d_ext_ids.ptr);
+    return run_on_stream(rep, stream_, [&](Scratch* sc) {
+        return ivf_search_filtered_on_device(&index->iv, sc, d_queries, qdtype, nq, k, n_probes, d_slot_bitmap, d_out_ids,
+                                             d_out_dists, d_out_probes, d_out_allowed, d_out_rows, rep->d_ext_ids.ptr);
+    });
 }
 
 int svsb200_dynamic_ivf_search_filtered(svsb200_dynamic_ivf* index, const void* queries, int qdtype, size_t nq, size_t k,
@@ -525,9 +525,14 @@ int svsb200_dynamic_ivf_search_filtered(svsb200_dynamic_ivf* index, const void* 
     if (!slot_bitmap) return fail("svsb200_dynamic_ivf_search_filtered: NULL bitmap");
     if (nq == 0) return 0;
     if (!queries || !out_ids || !out_dists) return fail("svsb200_dynamic_ivf_search_filtered: NULL buffer");
-    return ivf_search_filtered_host(&index->iv, queries, qdtype, nq, k, n_probes, slot_bitmap,
-                                    (index->iv.ix->slots.num_slots() + 31) / 32, out_ids, out_dists, out_probes, out_allowed,
-                                    out_rows, index->iv.ix->reps[0]->d_ext_ids.ptr);
+    Replica* rep = index->iv.ix->reps[0].get();
+    return run_host_search(rep, {queries, slot_bitmap, out_ids, out_dists, {out_probes, out_allowed, out_rows}},
+                           nq * index->iv.ix->dim * esize(qdtype), (index->iv.ix->slots.num_slots() + 31) / 32, nq, k,
+                           [&](Scratch* sc, const StagedBuffers& d) {
+                               return ivf_search_filtered_on_device(&index->iv, sc, d.queries, qdtype, nq, k, n_probes, d.bitmap,
+                                                                    d.ids, d.dists, d.per_query[0], d.per_query[1],
+                                                                    d.per_query[2], rep->d_ext_ids.ptr);
+                           });
 }
 
 }  // extern "C"

@@ -1197,10 +1197,7 @@ static int flat_on_device(svsb200_index* ix, Replica* rep, Scratch* sc, const vo
                           uint64_t* d_out_ids, float* d_out_dists, uint32_t* fallback_queries, uint32_t max_kc) {
     if (int rc = flat_rows_on_device(ix, rep, sc, d_queries, qdtype, nq, k, d_out_ids, d_out_dists, fallback_queries, max_kc))
         return rc;
-    if (ix->slot_mask) {
-        CUDA_TRY(slots_to_external(d_out_ids, nq * k, rep->d_ext_ids.ptr, sc->stream));
-        CUDA_TRY(cudaEventRecord(sc->ev_done, sc->stream));   // (a mutation waits for it: after_searches)
-    }
+    if (ix->slot_mask) CUDA_TRY(slots_to_external(d_out_ids, nq * k, rep->d_ext_ids.ptr, sc->stream));
     return 0;
 }
 
@@ -1276,7 +1273,6 @@ static int flat_filtered_on_device(svsb200_index* ix, Replica* rep, Scratch* sc,
     flat_pad_inf_kernel<<<grid, 256, 0, stream>>>(d_out_ids, d_out_dists, nq * k);
     count_launch();
     CUDA_TRY(cudaGetLastError());
-    if (ix->slot_mask) CUDA_TRY(cudaEventRecord(sc->ev_done, stream));   // (a mutation waits for it)
     return 0;
 }
 
@@ -1375,11 +1371,9 @@ int svsb200::flat_search_device(const char* who, svsb200_index* ix, const void* 
     if (ix->reps.size() != 1) return fail(w + ": the index must live on exactly one device");
     if (ix->dynamic) return fail(w + ": flat search is not available on a dynamic index");
     Replica* rep = ix->reps[0].get();
-    CUDA_TRY(cudaSetDevice(rep->device));
-    std::string err;
-    Scratch* sc = scratch_for_stream(rep, static_cast<cudaStream_t>(stream_), &err);
-    if (!sc) return fail(err);
-    return flat_on_device(ix, rep, sc, d_queries, qdtype, nq, k, d_out_ids, d_out_dists, fallback_queries, max_kc);
+    return run_on_stream(rep, stream_, [&](Scratch* sc) {
+        return flat_on_device(ix, rep, sc, d_queries, qdtype, nq, k, d_out_ids, d_out_dists, fallback_queries, max_kc);
+    });
 }
 
 // Blocking form on host buffers, on a scratch set of the pool (the first replica's).
@@ -1393,26 +1387,10 @@ int svsb200::flat_search_host(const char* who, svsb200_index* ix, const void* qu
     if (qdtype < SVSB200_F32 || qdtype > SVSB200_U8) return fail("bad query dtype");
     if (ix->dynamic) return fail(w + ": flat search is not available on a dynamic index");
     Replica* rep = ix->reps[0].get();
-    CUDA_TRY(cudaSetDevice(rep->device));
-    std::string err;
-    Scratch* sc = acquire(rep, &err);
-    if (!sc) return fail(err);
-    const int rc = [&]() -> int {
-        const size_t qbytes = nq * ix->dim * esize(qdtype);
-        CUDA_TRY(sc->q_raw.ensure(qbytes));
-        CUDA_TRY(sc->ids.ensure(nq * k * 8));
-        CUDA_TRY(sc->dists.ensure(nq * k));
-        CUDA_TRY(cudaMemcpyAsync(sc->q_raw.ptr, queries, qbytes, cudaMemcpyHostToDevice, sc->stream));
-        if (int rc = flat_on_device(ix, rep, sc, sc->q_raw.ptr, qdtype, nq, k, reinterpret_cast<uint64_t*>(sc->ids.ptr),
-                                    sc->dists.ptr, nullptr, max_kc))
-            return rc;
-        CUDA_TRY(cudaMemcpyAsync(out_ids, sc->ids.ptr, nq * k * 8, cudaMemcpyDeviceToHost, sc->stream));
-        CUDA_TRY(cudaMemcpyAsync(out_dists, sc->dists.ptr, nq * k * 4, cudaMemcpyDeviceToHost, sc->stream));
-        CUDA_TRY(cudaStreamSynchronize(sc->stream));
-        return 0;
-    }();
-    release(rep, sc);
-    return rc;
+    return run_host_search(rep, {queries, nullptr, out_ids, out_dists}, nq * ix->dim * esize(qdtype), 0, nq, k,
+                           [&](Scratch* sc, const StagedBuffers& d) {
+                               return flat_on_device(ix, rep, sc, d.queries, qdtype, nq, k, d.ids, d.dists, nullptr, max_kc);
+                           });
 }
 
 // The checks of both filtered forms: the arguments, and the query types the unfiltered search takes (an empty mask
@@ -1438,12 +1416,10 @@ int svsb200::flat_search_filtered_device(const char* who, svsb200_index* ix, con
     if (nq && (!d_queries || !d_out_ids || !d_out_dists)) return fail(w + ": NULL buffer");
     if (ix->reps.size() != 1) return fail(w + ": the index must live on exactly one device");
     Replica* rep = ix->reps[0].get();
-    CUDA_TRY(cudaSetDevice(rep->device));
-    std::string err;
-    Scratch* sc = scratch_for_stream(rep, static_cast<cudaStream_t>(stream_), &err);
-    if (!sc) return fail(err);
-    return flat_filtered_on_device(ix, rep, sc, d_queries, qdtype, nq, k, d_bitmap, d_out_ids, d_out_dists, out_allowed,
-                                   fallback_queries);
+    return run_on_stream(rep, stream_, [&](Scratch* sc) {
+        return flat_filtered_on_device(ix, rep, sc, d_queries, qdtype, nq, k, d_bitmap, d_out_ids, d_out_dists, out_allowed,
+                                       fallback_queries);
+    });
 }
 
 int svsb200::flat_search_filtered_host(const char* who, svsb200_index* ix, const void* queries, int qdtype, size_t nq, size_t k,
@@ -1452,30 +1428,11 @@ int svsb200::flat_search_filtered_host(const char* who, svsb200_index* ix, const
     if (int rc = flat_filtered_check(w, ix, bitmap, qdtype, k)) return rc;
     if (nq && (!queries || !out_ids || !out_dists)) return fail(w + ": NULL buffer");
     Replica* rep = ix->reps[0].get();
-    CUDA_TRY(cudaSetDevice(rep->device));
-    std::string err;
-    Scratch* sc = acquire(rep, &err);
-    if (!sc) return fail(err);
-    const int rc = [&]() -> int {
-        const size_t qbytes = nq * ix->dim * esize(qdtype), words = (ix->n + 31) / 32;
-        CUDA_TRY(sc->q_raw.ensure(std::max<size_t>(qbytes, 1)));
-        CUDA_TRY(sc->ids.ensure(std::max<size_t>(nq * k * 8, 1)));
-        CUDA_TRY(sc->dists.ensure(std::max<size_t>(nq * k, 1)));
-        CUDA_TRY(sc->flt_in.ensure(std::max<size_t>(words, 1)));
-        CUDA_TRY(cudaMemcpyAsync(sc->flt_in.ptr, bitmap, words * 4, cudaMemcpyHostToDevice, sc->stream));
-        if (qbytes) CUDA_TRY(cudaMemcpyAsync(sc->q_raw.ptr, queries, qbytes, cudaMemcpyHostToDevice, sc->stream));
-        if (int rc = flat_filtered_on_device(ix, rep, sc, sc->q_raw.ptr, qdtype, nq, k, sc->flt_in.ptr,
-                                             reinterpret_cast<uint64_t*>(sc->ids.ptr), sc->dists.ptr, out_allowed, nullptr))
-            return rc;
-        if (nq) {
-            CUDA_TRY(cudaMemcpyAsync(out_ids, sc->ids.ptr, nq * k * 8, cudaMemcpyDeviceToHost, sc->stream));
-            CUDA_TRY(cudaMemcpyAsync(out_dists, sc->dists.ptr, nq * k * 4, cudaMemcpyDeviceToHost, sc->stream));
-        }
-        CUDA_TRY(cudaStreamSynchronize(sc->stream));
-        return 0;
-    }();
-    release(rep, sc);
-    return rc;
+    return run_host_search(rep, {queries, bitmap, out_ids, out_dists}, nq * ix->dim * esize(qdtype), (ix->n + 31) / 32, nq, k,
+                           [&](Scratch* sc, const StagedBuffers& d) {
+                               return flat_filtered_on_device(ix, rep, sc, d.queries, qdtype, nq, k, d.bitmap, d.ids, d.dists,
+                                                              out_allowed, nullptr);
+                           });
 }
 
 extern "C" {

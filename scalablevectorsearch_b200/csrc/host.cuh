@@ -126,10 +126,17 @@ struct Scratch {
     DeviceBuffer<uint32_t> flat_cid, flat_unv;         // candidates, unverified list (+ its counter in slot 0)
     DeviceBuffer<uint32_t> flat_progress;              // per CTA of the flat GEMM: tiles started (keeps row groups in step)
     DeviceBuffer<uint64_t> flat_i2;
-    // filtered flat search, per call: the caller's bitmap (host form), each row's status (Valid = allowed), the allowed
-    // rows as a bitmap, their ids compacted (count first), the bias with every other column empty, the gathered rows
-    DeviceBuffer<uint32_t> flt_in, flt_bits, flt_ids, flt_bias;
+    // filtered flat search, per call: each row's status (Valid = allowed), the allowed rows as a bitmap, their ids
+    // compacted (count first), the bias with every other column empty, the gathered rows
+    DeviceBuffer<uint32_t> flt_bits, flt_ids, flt_bias;
     DeviceBuffer<unsigned char> flt_status, flt_rows;
+    DeviceBuffer<uint32_t> grow_unfinished;            // filtered and range search: queries whose lists must grow
+    DeviceBuffer<uint32_t> range_counts;               // range search: results per query
+    // host-buffer searches (run_host_search; the queries go in q_raw): the caller's bitmap and the outputs on their way
+    // back.  No search body works in these, so a body's own use of the scratch never overwrites them.
+    DeviceBuffer<uint32_t> stage_bitmap, stage_per_query;
+    DeviceBuffer<uint64_t> stage_ids;
+    DeviceBuffer<float> stage_dists;
     DeviceBuffer<uint32_t> dyn_ovf, dyn_qlist;        // dynamic search: overflowed queries, the list being re-run
     bool dyn_slot_ids = false;                         // dynamic search: write slots, not external ids (filtered / range)
     int (*cancel_fn)(void*) = nullptr;                 // the caller's cancellation predicate while a search runs
@@ -218,28 +225,137 @@ inline Scratch* new_scratch(Replica* rep, cudaStream_t caller_stream, std::strin
     return raw;
 }
 
-// Blocking API: any idle scratch of the replica (a new one if all are busy -- one per concurrent caller).
-inline Scratch* acquire(Replica* rep, std::string* err) {
-    std::lock_guard<std::mutex> lock(rep->mu);
-    if (!rep->idle.empty()) {
-        Scratch* sc = rep->idle.back();
-        rep->idle.pop_back();
+// The rows of an index that keeps a slot table on its replica (the dynamic Vamana, dynamic flat and dynamic IVF
+// indexes) are slots, which a mutation rewrites (after_searches).
+inline bool rows_are_slots(const Replica* rep) { return rep->d_ext_ids.ptr != nullptr; }
+
+// One call's hold on a scratch of a replica.  Checkout selects the replica's device first.
+class ScratchLease {
+  public:
+    ScratchLease() = default;
+    ScratchLease(const ScratchLease&) = delete;
+    ScratchLease& operator=(const ScratchLease&) = delete;
+    ScratchLease(ScratchLease&& o) noexcept : rep_(o.rep_), sc_(o.sc_), pooled_(o.pooled_) { o.sc_ = nullptr; }
+    ~ScratchLease() {
+        if (sc_ && pooled_) release(rep_, sc_);
+    }
+    // Blocking API: any idle scratch of the replica (a new one if all are busy -- one per concurrent caller), back in
+    // the idle list when the lease ends.
+    int checkout(Replica* rep) { return take(rep, true, nullptr); }
+    // Enqueue-only API: the scratch bound to the caller's stream (NULL: one the replica keeps for that purpose).  Work
+    // on one stream is ordered, so the scratch stays bound to it and the lease gives nothing back.
+    int checkout(Replica* rep, void* stream) { return take(rep, false, static_cast<cudaStream_t>(stream)); }
+    Scratch* get() const { return sc_; }
+    Scratch* operator->() const { return sc_; }
+    // Runs the search `body(scratch)`.  On an index whose rows are slots it then records the scratch's ev_done on its
+    // stream, behind the body's last device write: after_searches waits for that event before a mutation rewrites the
+    // rows or their external ids, so every search kind is covered without its body knowing.
+    template <typename F> int run(F body) {
+        Scratch* sc = sc_;
+        if (int rc = body(sc)) return rc;
+        if (rows_are_slots(rep_)) CUDA_TRY(cudaEventRecord(sc->ev_done, sc->stream));
+        return 0;
+    }
+
+  private:
+    int take(Replica* rep, bool pooled, cudaStream_t stream) {
+        CUDA_TRY(cudaSetDevice(rep->device));
+        std::string err;
+        Scratch* sc = pooled ? acquire(rep, &err) : scratch_for_stream(rep, stream, &err);
+        if (!sc) return fail(err);
+        rep_ = rep;
+        sc_ = sc;
+        pooled_ = pooled;
+        return 0;
+    }
+    static Scratch* acquire(Replica* rep, std::string* err) {
+        std::lock_guard<std::mutex> lock(rep->mu);
+        if (!rep->idle.empty()) {
+            Scratch* sc = rep->idle.back();
+            rep->idle.pop_back();
+            return sc;
+        }
+        return new_scratch(rep, nullptr, err);
+    }
+    static void release(Replica* rep, Scratch* sc) {
+        std::lock_guard<std::mutex> lock(rep->mu);
+        rep->idle.push_back(sc);
+    }
+    static Scratch* scratch_for_stream(Replica* rep, cudaStream_t stream, std::string* err) {
+        std::lock_guard<std::mutex> lock(rep->mu);
+        auto it = rep->by_stream.find(stream);
+        if (it != rep->by_stream.end()) return it->second;
+        Scratch* sc = new_scratch(rep, stream, err);
+        if (sc) rep->by_stream[stream] = sc;
         return sc;
     }
-    return new_scratch(rep, nullptr, err);
+    Replica* rep_ = nullptr;
+    Scratch* sc_ = nullptr;
+    bool pooled_ = false;
+};
+
+// The device form of a search: `body(scratch)` on the scratch bound to the caller's stream, enqueued there.
+template <typename F> int run_on_stream(Replica* rep, void* stream, F body) {
+    ScratchLease lease;
+    if (int rc = lease.checkout(rep, stream)) return rc;
+    return lease.run(body);
 }
-inline void release(Replica* rep, Scratch* sc) {
-    std::lock_guard<std::mutex> lock(rep->mu);
-    rep->idle.push_back(sc);
-}
-// Enqueue-only API: the scratch bound to the caller's stream (work on one stream is ordered, so it is reusable).
-inline Scratch* scratch_for_stream(Replica* rep, cudaStream_t stream, std::string* err) {
-    std::lock_guard<std::mutex> lock(rep->mu);
-    auto it = rep->by_stream.find(stream);
-    if (it != rep->by_stream.end()) return it->second;
-    Scratch* sc = new_scratch(rep, stream, err);
-    if (sc) rep->by_stream[stream] = sc;
-    return sc;
+
+// The buffers of a blocking search over host memory (run_host_search): the queries, the bitmap (NULL: none), k ids and
+// distances per query (k = 0: none) and up to three per-query arrays of uint32 (NULL: not wanted).
+struct HostBuffers {
+    const void* queries = nullptr;
+    const uint32_t* bitmap = nullptr;
+    uint64_t* ids = nullptr;
+    float* dists = nullptr;
+    uint32_t* per_query[3] = {};
+};
+// ... and the same buffers in device memory, as run_host_search hands them to its body: the queries and the bitmap are
+// copies the body may rewrite; a per-query array is NULL where the caller wants none.
+struct StagedBuffers {
+    const void* queries = nullptr;
+    uint32_t* bitmap = nullptr;
+    uint64_t* ids = nullptr;
+    float* dists = nullptr;
+    uint32_t* per_query[3] = {};
+};
+
+// The blocking form of a search over host buffers, on a scratch of the replica's pool: `query_bytes` of queries and
+// `bitmap_words` of bitmap are copied in, `body(scratch, staged)` runs, the nq * k results and the per-query arrays are
+// copied out, and the stream is synchronised.  Copies of zero bytes are skipped.
+template <typename F>
+int run_host_search(Replica* rep, const HostBuffers& host, size_t query_bytes, size_t bitmap_words, size_t nq, size_t k,
+                    F body) {
+    ScratchLease lease;
+    if (int rc = lease.checkout(rep)) return rc;
+    Scratch* sc = lease.get();
+    const cudaStream_t s = sc->stream;
+    const size_t results = nq * k;
+    CUDA_TRY(sc->q_raw.ensure(std::max<size_t>(query_bytes, 1)));
+    CUDA_TRY(sc->stage_ids.ensure(std::max<size_t>(results, 1)));
+    CUDA_TRY(sc->stage_dists.ensure(std::max<size_t>(results, 1)));
+    StagedBuffers dev{sc->q_raw.ptr, nullptr, sc->stage_ids.ptr, sc->stage_dists.ptr};
+    if (query_bytes) CUDA_TRY(cudaMemcpyAsync(sc->q_raw.ptr, host.queries, query_bytes, cudaMemcpyHostToDevice, s));
+    if (host.bitmap) {
+        CUDA_TRY(sc->stage_bitmap.ensure(std::max<size_t>(bitmap_words, 1)));
+        if (bitmap_words) CUDA_TRY(cudaMemcpyAsync(sc->stage_bitmap.ptr, host.bitmap, bitmap_words * 4, cudaMemcpyHostToDevice, s));
+        dev.bitmap = sc->stage_bitmap.ptr;
+    }
+    for (int i = 0; i < 3; ++i) {
+        if (!host.per_query[i]) continue;
+        CUDA_TRY(sc->stage_per_query.ensure(3 * nq));
+        dev.per_query[i] = sc->stage_per_query.ptr + i * nq;
+    }
+    if (int rc = lease.run([&](Scratch* scratch) { return body(scratch, dev); })) return rc;
+    if (results) {
+        CUDA_TRY(cudaMemcpyAsync(host.ids, dev.ids, results * 8, cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(cudaMemcpyAsync(host.dists, dev.dists, results * 4, cudaMemcpyDeviceToHost, s));
+    }
+    for (int i = 0; i < 3; ++i)
+        if (host.per_query[i] && nq)
+            CUDA_TRY(cudaMemcpyAsync(host.per_query[i], dev.per_query[i], nq * 4, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    return 0;
 }
 
 }  // namespace svsb200
@@ -369,7 +485,10 @@ cudaError_t move_rows(const void* src, const uint32_t* src_pos, void* dst, const
 // Runs a mutation `body(rep, stream)` on a scratch stream of the index's device, once every search of the index
 // enqueued so far has finished: a device-buffer search returns with work still queued on the caller's stream (the
 // mapping to external ids reads the slots' external ids, the scan reads the rows), and the mutation rewrites them.
-// Every search of a dynamic index records its scratch's ev_done at its end (search.cu, flat.cu, ivf.cu).
+// Every search of an index whose rows are slots runs through ScratchLease::run, which records its scratch's ev_done
+// at its end -- except svsb200_search_cancellable on a dynamic Vamana index, which holds its leases itself: that search
+// records ev_done behind each launch and waits for it (search_dynamic), and its kernel writes the external ids, so
+// nothing of the index is read once it returns.
 template <typename F> int after_searches(svsb200_index* ix, F body) {
     Replica* rep = ix->reps[0].get();
     CUDA_TRY(cudaSetDevice(rep->device));
@@ -379,26 +498,24 @@ template <typename F> int after_searches(svsb200_index* ix, F body) {
         for (const auto& sc : rep->all) searches.push_back(sc->ev_done);
     }
     for (cudaEvent_t ev : searches) CUDA_TRY(cudaEventSynchronize(ev));   // (never recorded: returns at once)
-    std::string err;
-    Scratch* sc = acquire(rep, &err);
-    if (!sc) return fail(err);
-    const int rc = body(rep, sc->stream);
-    release(rep, sc);
-    return rc;
+    ScratchLease lease;
+    if (int rc = lease.checkout(rep)) return rc;
+    return body(rep, lease->stream);
 }
 
 // ---- flat search (flat.cu), shared by the Flat handle and the dynamic flat index ----
-// The two search bodies: `who` names the entry point in errors, `max_kc` is the deepest candidate list allowed.  The
-// device form is enqueued on the caller's stream, the host form blocks.
+// The device forms, enqueued on the caller's stream: `who` names the entry point in errors, `max_kc` is the deepest
+// candidate list allowed.
 int flat_search_device(const char* who, svsb200_index* ix, const void* d_queries, int qdtype, size_t nq, size_t k,
                        uint64_t* d_out_ids, float* d_out_dists, void* stream, uint32_t* fallback_queries, uint32_t max_kc);
-int flat_search_host(const char* who, svsb200_index* ix, const void* queries, int qdtype, size_t nq, size_t k,
-                     uint64_t* out_ids, float* out_dists, uint32_t max_kc);
 // The filtered flat search (svsb200_flat_index_search_filtered): `bitmap` over the rows (a dynamic flat index: over
-// the slots, Empty slots' bits ignored), in device memory for the device form and in host memory for the host form.
+// the slots, Empty slots' bits ignored).
 int flat_search_filtered_device(const char* who, svsb200_index* ix, const void* d_queries, int qdtype, size_t nq, size_t k,
                                 const uint32_t* d_bitmap, uint64_t* d_out_ids, float* d_out_dists, void* stream,
                                 size_t* out_allowed, uint32_t* fallback_queries);
+// The blocking forms over host buffers: the same bodies on a scratch of the pool (run_host_search).
+int flat_search_host(const char* who, svsb200_index* ix, const void* queries, int qdtype, size_t nq, size_t k,
+                     uint64_t* out_ids, float* out_dists, uint32_t max_kc);
 int flat_search_filtered_host(const char* who, svsb200_index* ix, const void* queries, int qdtype, size_t nq, size_t k,
                               const uint32_t* bitmap, uint64_t* out_ids, float* out_dists, size_t* out_allowed);
 // Deepest list of the Flat handles' searches (k <= 121 on the GEMM).

@@ -255,36 +255,8 @@ int ivf_search_on_device(svsb200_ivf* iv, Scratch* sc, const void* d_queries, in
                                                d_out_dists + q0 * k, rep->device, stream))
             return rc;
     }
-    if (d_ext_ids) {   // slots -> external ids; a mutation of the dynamic index waits for ev_done (dynamic_ivf.cu)
-        CUDA_TRY(slots_to_external(d_out_ids, nq * k, d_ext_ids, stream));
-        CUDA_TRY(cudaEventRecord(sc->ev_done, stream));
-    }
+    if (d_ext_ids) CUDA_TRY(slots_to_external(d_out_ids, nq * k, d_ext_ids, stream));   // slots -> external ids
     return 0;
-}
-
-int ivf_search_host(svsb200_ivf* iv, const void* queries, int qdtype, size_t nq, size_t k, size_t P, uint64_t* out_ids,
-                    float* out_dists, const uint64_t* d_ext_ids) {
-    Replica* rep = iv->ix->reps[0].get();
-    CUDA_TRY(cudaSetDevice(rep->device));
-    std::string err;
-    Scratch* sc = acquire(rep, &err);
-    if (!sc) return fail(err);
-    const int rc = [&]() -> int {
-        const size_t qbytes = nq * iv->ix->dim * esize(qdtype);
-        CUDA_TRY(sc->q_raw.ensure(qbytes));
-        CUDA_TRY(sc->ids.ensure(nq * k * 8));
-        CUDA_TRY(sc->dists.ensure(nq * k));
-        CUDA_TRY(cudaMemcpyAsync(sc->q_raw.ptr, queries, qbytes, cudaMemcpyHostToDevice, sc->stream));
-        if (int rc = ivf_search_on_device(iv, sc, sc->q_raw.ptr, qdtype, nq, k, P, reinterpret_cast<uint64_t*>(sc->ids.ptr),
-                                          sc->dists.ptr, d_ext_ids))
-            return rc;
-        CUDA_TRY(cudaMemcpyAsync(out_ids, sc->ids.ptr, nq * k * 8, cudaMemcpyDeviceToHost, sc->stream));
-        CUDA_TRY(cudaMemcpyAsync(out_dists, sc->dists.ptr, nq * k * 4, cudaMemcpyDeviceToHost, sc->stream));
-        CUDA_TRY(cudaStreamSynchronize(sc->stream));
-        return 0;
-    }();
-    release(rep, sc);
-    return rc;
 }
 
 // Filtered search, per call:
@@ -383,45 +355,8 @@ int ivf_search_filtered_on_device(svsb200_ivf* iv, Scratch* sc, const void* d_qu
     if (d_probes) CUDA_TRY(cudaMemcpyAsync(d_probes, is->q_probes.ptr, nq * 4, cudaMemcpyDeviceToDevice, stream));
     if (d_allowed) CUDA_TRY(cudaMemcpyAsync(d_allowed, is->q_allowed.ptr, nq * 4, cudaMemcpyDeviceToDevice, stream));
     if (d_rows) CUDA_TRY(cudaMemcpyAsync(d_rows, is->q_rows.ptr, nq * 4, cudaMemcpyDeviceToDevice, stream));
-    if (d_ext_ids) {   // slots -> external ids; a mutation of the dynamic index waits for ev_done (dynamic_ivf.cu)
-        CUDA_TRY(slots_to_external(d_out_ids, nq * k, d_ext_ids, stream));
-        CUDA_TRY(cudaEventRecord(sc->ev_done, stream));
-    }
+    if (d_ext_ids) CUDA_TRY(slots_to_external(d_out_ids, nq * k, d_ext_ids, stream));   // slots -> external ids
     return 0;
-}
-
-int ivf_search_filtered_host(svsb200_ivf* iv, const void* queries, int qdtype, size_t nq, size_t k, size_t n_probes,
-                             const uint32_t* bitmap, size_t bitmap_words, uint64_t* out_ids, float* out_dists,
-                             uint32_t* out_probes, uint32_t* out_allowed, uint32_t* out_rows, const uint64_t* d_ext_ids) {
-    Replica* rep = iv->ix->reps[0].get();
-    CUDA_TRY(cudaSetDevice(rep->device));
-    std::string err;
-    Scratch* sc = acquire(rep, &err);
-    if (!sc) return fail(err);
-    const int rc = [&]() -> int {
-        const size_t qbytes = nq * iv->ix->dim * esize(qdtype);
-        IvfScratch* is = ivf_scratch(iv, sc);
-        CUDA_TRY(sc->q_raw.ensure(qbytes));
-        CUDA_TRY(sc->ids.ensure(nq * k * 8));
-        CUDA_TRY(sc->dists.ensure(nq * k));
-        CUDA_TRY(is->bitmap.ensure(std::max<size_t>(bitmap_words, 1)));
-        CUDA_TRY(cudaMemcpyAsync(sc->q_raw.ptr, queries, qbytes, cudaMemcpyHostToDevice, sc->stream));
-        if (bitmap_words)
-            CUDA_TRY(cudaMemcpyAsync(is->bitmap.ptr, bitmap, bitmap_words * 4, cudaMemcpyHostToDevice, sc->stream));
-        if (int rc = ivf_search_filtered_on_device(iv, sc, sc->q_raw.ptr, qdtype, nq, k, n_probes, is->bitmap.ptr,
-                                                   reinterpret_cast<uint64_t*>(sc->ids.ptr), sc->dists.ptr, nullptr, nullptr,
-                                                   nullptr, d_ext_ids))
-            return rc;
-        CUDA_TRY(cudaMemcpyAsync(out_ids, sc->ids.ptr, nq * k * 8, cudaMemcpyDeviceToHost, sc->stream));
-        CUDA_TRY(cudaMemcpyAsync(out_dists, sc->dists.ptr, nq * k * 4, cudaMemcpyDeviceToHost, sc->stream));
-        if (out_probes) CUDA_TRY(cudaMemcpyAsync(out_probes, is->q_probes.ptr, nq * 4, cudaMemcpyDeviceToHost, sc->stream));
-        if (out_allowed) CUDA_TRY(cudaMemcpyAsync(out_allowed, is->q_allowed.ptr, nq * 4, cudaMemcpyDeviceToHost, sc->stream));
-        if (out_rows) CUDA_TRY(cudaMemcpyAsync(out_rows, is->q_rows.ptr, nq * 4, cudaMemcpyDeviceToHost, sc->stream));
-        CUDA_TRY(cudaStreamSynchronize(sc->stream));
-        return 0;
-    }();
-    release(rep, sc);
-    return rc;
 }
 
 int ivf_check_search(const char* who, const svsb200_ivf* iv, int qdtype, size_t k, size_t n_probes) {
@@ -756,12 +691,9 @@ int svsb200_ivf_search_device(svsb200_ivf* index, const void* d_queries, int qdt
     if (int rc = ivf_check_search("svsb200_ivf_search_device", index, qdtype, k, n_probes)) return rc;
     if (nq == 0) return 0;
     if (!d_queries || !d_out_ids || !d_out_dists) return fail("svsb200_ivf_search_device: NULL buffer");
-    Replica* rep = index->ix->reps[0].get();
-    CUDA_TRY(cudaSetDevice(rep->device));
-    std::string err;
-    Scratch* sc = scratch_for_stream(rep, static_cast<cudaStream_t>(stream_), &err);
-    if (!sc) return fail(err);
-    return ivf_search_on_device(index, sc, d_queries, qdtype, nq, k, n_probes, d_out_ids, d_out_dists, nullptr);
+    return run_on_stream(index->ix->reps[0].get(), stream_, [&](Scratch* sc) {
+        return ivf_search_on_device(index, sc, d_queries, qdtype, nq, k, n_probes, d_out_ids, d_out_dists, nullptr);
+    });
 }
 
 int svsb200_ivf_search(svsb200_ivf* index, const void* queries, int qdtype, size_t nq, size_t k, size_t n_probes,
@@ -769,7 +701,10 @@ int svsb200_ivf_search(svsb200_ivf* index, const void* queries, int qdtype, size
     if (int rc = ivf_check_search("svsb200_ivf_search", index, qdtype, k, n_probes)) return rc;
     if (nq == 0) return 0;
     if (!queries || !out_ids || !out_dists) return fail("svsb200_ivf_search: NULL buffer");
-    return ivf_search_host(index, queries, qdtype, nq, k, n_probes, out_ids, out_dists, nullptr);
+    return run_host_search(index->ix->reps[0].get(), {queries, nullptr, out_ids, out_dists}, nq * index->ix->dim * esize(qdtype),
+                           0, nq, k, [&](Scratch* sc, const StagedBuffers& d) {
+                               return ivf_search_on_device(index, sc, d.queries, qdtype, nq, k, n_probes, d.ids, d.dists, nullptr);
+                           });
 }
 
 int svsb200_ivf_search_filtered_device(svsb200_ivf* index, const void* d_queries, int qdtype, size_t nq, size_t k,
@@ -780,13 +715,10 @@ int svsb200_ivf_search_filtered_device(svsb200_ivf* index, const void* d_queries
     if (!d_id_bitmap) return fail("svsb200_ivf_search_filtered_device: NULL bitmap");
     if (nq == 0) return 0;
     if (!d_queries || !d_out_ids || !d_out_dists) return fail("svsb200_ivf_search_filtered_device: NULL buffer");
-    Replica* rep = index->ix->reps[0].get();
-    CUDA_TRY(cudaSetDevice(rep->device));
-    std::string err;
-    Scratch* sc = scratch_for_stream(rep, static_cast<cudaStream_t>(stream_), &err);
-    if (!sc) return fail(err);
-    return ivf_search_filtered_on_device(index, sc, d_queries, qdtype, nq, k, n_probes, d_id_bitmap, d_out_ids, d_out_dists,
-                                         d_out_probes, d_out_allowed, d_out_rows, nullptr);
+    return run_on_stream(index->ix->reps[0].get(), stream_, [&](Scratch* sc) {
+        return ivf_search_filtered_on_device(index, sc, d_queries, qdtype, nq, k, n_probes, d_id_bitmap, d_out_ids, d_out_dists,
+                                             d_out_probes, d_out_allowed, d_out_rows, nullptr);
+    });
 }
 
 int svsb200_ivf_search_filtered(svsb200_ivf* index, const void* queries, int qdtype, size_t nq, size_t k, size_t n_probes,
@@ -796,8 +728,13 @@ int svsb200_ivf_search_filtered(svsb200_ivf* index, const void* queries, int qdt
     if (!id_bitmap) return fail("svsb200_ivf_search_filtered: NULL bitmap");
     if (nq == 0) return 0;
     if (!queries || !out_ids || !out_dists) return fail("svsb200_ivf_search_filtered: NULL buffer");
-    return ivf_search_filtered_host(index, queries, qdtype, nq, k, n_probes, id_bitmap, (index->n + 31) / 32, out_ids,
-                                    out_dists, out_probes, out_allowed, out_rows, nullptr);
+    return run_host_search(index->ix->reps[0].get(), {queries, id_bitmap, out_ids, out_dists, {out_probes, out_allowed, out_rows}},
+                           nq * index->ix->dim * esize(qdtype), (index->n + 31) / 32, nq, k,
+                           [&](Scratch* sc, const StagedBuffers& d) {
+                               return ivf_search_filtered_on_device(index, sc, d.queries, qdtype, nq, k, n_probes, d.bitmap, d.ids,
+                                                                    d.dists, d.per_query[0], d.per_query[1], d.per_query[2],
+                                                                    nullptr);
+                           });
 }
 
 }  // extern "C"

@@ -21,7 +21,7 @@ struct IvfScratch {
     DeviceBuffer<uint32_t> counts, list_off, item_off, cursor, list;
     // filtered search: the masked row ids, per-cluster counts, per-query P / allowed / Valid rows, a query group's
     // positions in the batch, its queries and its results, and the probes of a growth round
-    DeviceBuffer<uint32_t> masked, cl_allowed, cl_rows, q_probes, q_allowed, q_rows, qidx, bitmap;
+    DeviceBuffer<uint32_t> masked, cl_allowed, cl_rows, q_probes, q_allowed, q_rows, qidx;
     DeviceBuffer<unsigned char> gq;
     DeviceBuffer<uint64_t> g_ids, f_probe_ids;
     DeviceBuffer<float> g_dists, f_probe_dists;
@@ -59,19 +59,12 @@ int ivf_check_search(const char* who, const svsb200_ivf* iv, int qdtype, size_t 
 int ivf_search_on_device(svsb200_ivf* iv, Scratch* sc, const void* d_queries, int qdtype, size_t nq, size_t k, size_t P,
                          uint64_t* d_out_ids, float* d_out_dists, const uint64_t* d_ext_ids,
                          const uint32_t* d_masked_ids = nullptr);
-// The blocking form over HOST buffers.
-int ivf_search_host(svsb200_ivf* iv, const void* queries, int qdtype, size_t nq, size_t k, size_t P, uint64_t* out_ids,
-                    float* out_dists, const uint64_t* d_ext_ids);
 // The filtered search (include/svsb200.h, svsb200_ivf_search_filtered) on device buffers: `d_bitmap` over the row ids
 // (original ids, or slots of the dynamic index, whose results are mapped to d_ext_ids); per-query outputs may be NULL.
 // Enqueued on sc->stream apart from the probes and the growth decisions, which synchronise it.
 int ivf_search_filtered_on_device(svsb200_ivf* iv, Scratch* sc, const void* d_queries, int qdtype, size_t nq, size_t k,
                                   size_t n_probes, const uint32_t* d_bitmap, uint64_t* d_out_ids, float* d_out_dists,
                                   uint32_t* d_probes, uint32_t* d_allowed, uint32_t* d_rows, const uint64_t* d_ext_ids);
-// The blocking form over HOST buffers; the bitmap has `bitmap_words` words.
-int ivf_search_filtered_host(svsb200_ivf* iv, const void* queries, int qdtype, size_t nq, size_t k, size_t n_probes,
-                             const uint32_t* bitmap, size_t bitmap_words, uint64_t* out_ids, float* out_dists,
-                             uint32_t* out_probes, uint32_t* out_allowed, uint32_t* out_rows, const uint64_t* d_ext_ids);
 
 // An SQ index's scale and bias: the scale finite and positive, the bias finite.
 inline int sq_check_params(const char* who, float scale, float bias) {

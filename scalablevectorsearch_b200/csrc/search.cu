@@ -610,24 +610,25 @@ static int wait_all(const std::vector<Scratch*>& scs) {
     return 0;
 }
 
-// Filtered and range search: runs the batch (already in sc->q_raw) with result lists of `kk` entries per query
-// (window = capacity = max(window, kk)) into the scratch's own id / distance blocks, and lets `check(kk)` launch the
-// kernel that counts in *d_unfinished the queries that need a longer list.  Lists grow (x4) until no query is
-// unfinished, a list holds the whole index or 16384 entries, like the reference's batch iterator asks for further
+// Filtered and range search: runs the batch `d_queries` with result lists of `kk` entries per query
+// (window = capacity = max(window, kk)) into the scratch's own id / distance blocks, and lets `check(kk, d_unfinished)`
+// launch the kernel that counts in *d_unfinished the queries that need a longer list.  Lists grow (x4) until no query
+// is unfinished, a list holds the whole index or 16384 entries, like the reference's batch iterator asks for further
 // batches (vamana_index_impl.h:183-205).  Returns the final list length in *kk.
 template <typename Check>
-static int grow_until_done(svsb200_index* ix, Replica* rep, Scratch* sc, int qdtype, size_t nq, size_t window, size_t* kk,
-                           uint32_t* d_unfinished, Check check) {
+static int grow_until_done(svsb200_index* ix, Replica* rep, Scratch* sc, const void* d_queries, int qdtype, size_t nq,
+                           size_t window, size_t* kk, Check check) {
+    CUDA_TRY(sc->grow_unfinished.ensure(1));
+    uint32_t* d_unfinished = sc->grow_unfinished.ptr;
     for (;;) {
         *kk = std::min(*kk, ix->n);
         CUDA_TRY(sc->ids.ensure(nq * *kk * 8));
         CUDA_TRY(sc->dists.ensure(nq * *kk));
         const size_t w = std::max(window, *kk);
-        if (int rc = search_on_device(ix, rep, sc, sc->q_raw.ptr, qdtype, nq, *kk, w, w, sc->ids.ptr, 8, sc->dists.ptr,
-                                      sc->stream))
+        if (int rc = search_on_device(ix, rep, sc, d_queries, qdtype, nq, *kk, w, w, sc->ids.ptr, 8, sc->dists.ptr, sc->stream))
             return rc;
         CUDA_TRY(cudaMemsetAsync(d_unfinished, 0, 4, sc->stream));
-        check(*kk);
+        check(*kk, d_unfinished);
         count_launch();
         CUDA_TRY(cudaGetLastError());
         uint32_t unfinished = 0;
@@ -638,74 +639,49 @@ static int grow_until_done(svsb200_index* ix, Replica* rep, Scratch* sc, int qdt
     }
 }
 
-// Filtered search body, on a scratch set checked out by the caller.
-static int search_filtered(svsb200_index* ix, Replica* rep, Scratch* sc, const void* queries, int qdtype, size_t nq, size_t k,
-                           size_t window, const uint32_t* id_bitmap, uint64_t* out_ids, float* out_dists, uint32_t* out_found) {
+// Filtered search body on device buffers: `d_bitmap` (rewritten on a dynamic index), the k results per query and the
+// number found per query, enqueued on sc->stream apart from the growth decisions, which synchronise it.
+static int search_filtered(svsb200_index* ix, Replica* rep, Scratch* sc, const void* d_queries, int qdtype, size_t nq, size_t k,
+                           size_t window, uint32_t* d_bitmap, uint64_t* d_oi, float* d_od, uint32_t* d_found) {
     const size_t words = (ix->n + 31) / 32;
-    const size_t qbytes = nq * ix->dim * esize(qdtype);
-    DeviceBuffer<uint32_t> d_bitmap, d_found;
-    DeviceBuffer<uint64_t> d_oi;
-    DeviceBuffer<float> d_od;
-    CUDA_TRY(d_bitmap.ensure(words));
-    CUDA_TRY(d_found.ensure(nq + 1));
-    CUDA_TRY(d_oi.ensure(nq * k));
-    CUDA_TRY(d_od.ensure(nq * k));
-    CUDA_TRY(sc->q_raw.ensure(qbytes));
-    CUDA_TRY(cudaMemcpyAsync(d_bitmap.ptr, id_bitmap, words * 4, cudaMemcpyHostToDevice, sc->stream));
-    CUDA_TRY(cudaMemcpyAsync(sc->q_raw.ptr, queries, qbytes, cudaMemcpyHostToDevice, sc->stream));
-    CUDA_TRY(cudaMemsetAsync(d_oi.ptr, 0xFF, nq * k * 8, sc->stream));
+    CUDA_TRY(cudaMemsetAsync(d_oi, 0xFF, nq * k * 8, sc->stream));
     if (ix->dynamic) {
         // the bitmap is over slots: only Valid slots may be returned; the search lists slots, translated at the end
-        keep_valid_kernel<<<unsigned((words + 255) / 256), 256, 0, sc->stream>>>(d_bitmap.ptr, rep->d_status.ptr, ix->n);
+        keep_valid_kernel<<<unsigned((words + 255) / 256), 256, 0, sc->stream>>>(d_bitmap, rep->d_status.ptr, ix->n);
         count_launch();
         CUDA_TRY(cudaGetLastError());
         sc->dyn_slot_ids = true;
     }
     // lists grow until every query has k members or its search is exhausted
     size_t kk = std::max(k, window);
-    int rc = grow_until_done(ix, rep, sc, qdtype, nq, window, &kk, d_found.ptr + nq, [&](size_t len) {
+    int rc = grow_until_done(ix, rep, sc, d_queries, qdtype, nq, window, &kk, [&](size_t len, uint32_t* d_unfinished) {
         filter_topk_kernel<<<unsigned((nq + 3) / 4), 128, 0, sc->stream>>>(
             reinterpret_cast<const uint64_t*>(sc->ids.ptr), sc->dists.ptr, uint32_t(nq), uint32_t(len), uint32_t(k),
-            d_bitmap.ptr, ix->id_offset, d_oi.ptr, d_od.ptr, d_found.ptr, d_found.ptr + nq);
+            d_bitmap, ix->id_offset, d_oi, d_od, d_found, d_unfinished);
     });
     sc->dyn_slot_ids = false;
     if (rc) return rc;
     if (ix->dynamic) {
-        slots_to_external_kernel<<<unsigned((nq * k + 255) / 256), 256, 0, sc->stream>>>(d_oi.ptr, nq * k, rep->d_ext_ids.ptr);
+        slots_to_external_kernel<<<unsigned((nq * k + 255) / 256), 256, 0, sc->stream>>>(d_oi, nq * k, rep->d_ext_ids.ptr);
         count_launch();
         CUDA_TRY(cudaGetLastError());
-    }
-    std::vector<uint32_t> found(nq);
-    CUDA_TRY(cudaMemcpyAsync(found.data(), d_found.ptr, nq * 4, cudaMemcpyDeviceToHost, sc->stream));
-    CUDA_TRY(cudaMemcpyAsync(out_ids, d_oi.ptr, nq * k * 8, cudaMemcpyDeviceToHost, sc->stream));
-    CUDA_TRY(cudaMemcpyAsync(out_dists, d_od.ptr, nq * k * 4, cudaMemcpyDeviceToHost, sc->stream));
-    CUDA_TRY(cudaStreamSynchronize(sc->stream));
-    for (size_t q = 0; q < nq; ++q) {   // pad like the reference: unspecified id (all-ones), +inf distance
-        for (size_t j = found[q]; j < k; ++j) {
-            out_ids[q * k + j] = ~uint64_t(0);
-            out_dists[q * k + j] = INFINITY;
-        }
-        if (out_found) out_found[q] = found[q];
     }
     return 0;
 }
 
-// Range search body, on a scratch set checked out by the caller.
-static int range_search(svsb200_index* ix, Replica* rep, Scratch* sc, const void* queries, int qdtype, size_t nq, float radius,
-                        size_t window, uint32_t* out_counts, uint64_t** out_ids, float** out_dists) {
-    const size_t qbytes = nq * ix->dim * esize(qdtype);
-    DeviceBuffer<uint32_t> d_counts;
-    CUDA_TRY(d_counts.ensure(nq + 1));
-    CUDA_TRY(sc->q_raw.ensure(qbytes));
-    CUDA_TRY(cudaMemcpyAsync(sc->q_raw.ptr, queries, qbytes, cudaMemcpyHostToDevice, sc->stream));
+// Range search body, on the batch `d_queries` in the scratch checked out by the caller; blocks.
+static int range_search(svsb200_index* ix, Replica* rep, Scratch* sc, const void* d_queries, int qdtype, size_t nq,
+                        float radius, size_t window, uint32_t* out_counts, uint64_t** out_ids, float** out_dists) {
+    CUDA_TRY(sc->range_counts.ensure(nq));
+    uint32_t* d_counts = sc->range_counts.ptr;
     size_t kk = std::max<size_t>(window, 16);
-    int rc = grow_until_done(ix, rep, sc, qdtype, nq, window, &kk, d_counts.ptr + nq, [&](size_t len) {
+    int rc = grow_until_done(ix, rep, sc, d_queries, qdtype, nq, window, &kk, [&](size_t len, uint32_t* d_unfinished) {
         range_count_kernel<<<unsigned((nq + 127) / 128), 128, 0, sc->stream>>>(
             sc->dists.ptr, reinterpret_cast<const uint64_t*>(sc->ids.ptr), uint32_t(nq), uint32_t(len), radius,
-            ix->metric != SVSB200_L2, d_counts.ptr, d_counts.ptr + nq);
+            ix->metric != SVSB200_L2, d_counts, d_unfinished);
     });
     if (rc) return rc;   // (on a dynamic index the list holds no Deleted slot and its ids are already external)
-    CUDA_TRY(cudaMemcpyAsync(out_counts, d_counts.ptr, nq * 4, cudaMemcpyDeviceToHost, sc->stream));
+    CUDA_TRY(cudaMemcpyAsync(out_counts, d_counts, nq * 4, cudaMemcpyDeviceToHost, sc->stream));
     std::vector<uint64_t> ids(nq * kk);
     std::vector<float> dd(nq * kk);
     CUDA_TRY(cudaMemcpyAsync(ids.data(), sc->ids.ptr, nq * kk * 8, cudaMemcpyDeviceToHost, sc->stream));
@@ -818,13 +794,10 @@ int svsb200_search_device(svsb200_index* ix, const void* d_queries, int qdtype, 
     if (nq && (!d_queries || !d_out_ids || !d_out_dists)) return fail("svsb200_search_device: NULL buffer");
     if (ix->reps.size() != 1) return fail("svsb200_search_device: the index must live on exactly one device");
     Replica* rep = ix->reps[0].get();
-    CUDA_TRY(cudaSetDevice(rep->device));
-    std::string err;
-    // NULL = the stream of a scratch this index keeps for that purpose (ordered against itself)
-    Scratch* sc = scratch_for_stream(rep, static_cast<cudaStream_t>(stream_), &err);
-    if (!sc) return fail(err);
-    return search_on_device(ix, rep, sc, d_queries, qdtype, nq, k, window, capacity, d_out_ids, id_bytes, d_out_dists,
-                            sc->stream);
+    return run_on_stream(rep, stream_, [&](Scratch* sc) {
+        return search_on_device(ix, rep, sc, d_queries, qdtype, nq, k, window, capacity, d_out_ids, id_bytes, d_out_dists,
+                                sc->stream);
+    });
 }
 
 int svsb200_search_cancellable(svsb200_index* ix, const void* queries, int qdtype, size_t nq, size_t k, size_t window,
@@ -840,9 +813,11 @@ int svsb200_search_cancellable(svsb200_index* ix, const void* queries, int qdtyp
     if (stream_ && R != 1) return fail("svsb200_search: a caller stream needs a single-device index");
     if (cancel && cancel(cancel_arg)) return 0;   // index.h:575 checks before any work
     const size_t qrow = ix->dim * esize(qdtype);
-    std::vector<Scratch*> used;
-    std::vector<Replica*> used_rep;
-    std::vector<size_t> used_lo, used_m;
+    struct Piece {
+        ScratchLease lease;
+        size_t lo, m;   // the piece's queries: [lo, lo + m)
+    };
+    std::vector<Piece> pieces;
     int rc = 0;
     // Every device's share is cut into C pieces, each on its own stream: the host-to-device copy of piece i+1 and the
     // device-to-host copy of piece i-1 run under the kernel of piece i (the kernels of consecutive pieces overlap
@@ -862,22 +837,12 @@ int svsb200_search_cancellable(svsb200_index* ix, const void* queries, int qdtyp
         balance(nq, R * C, part, &lo, &hi);
         if (hi == lo) continue;
         Replica* rep = ix->reps[r].get();
-        cudaError_t e = cudaSetDevice(rep->device);
-        if (e != cudaSuccess) {
-            rc = fail(std::string("cudaSetDevice: ") + cudaGetErrorString(e));
-            break;
-        }
-        std::string err;
-        Scratch* sc = stream_ ? scratch_for_stream(rep, static_cast<cudaStream_t>(stream_), &err) : acquire(rep, &err);
-        if (!sc) {
-            rc = fail(err);
-            break;
-        }
-        used.push_back(sc);
-        used_rep.push_back(stream_ ? nullptr : rep);
+        ScratchLease lease;
+        rc = stream_ ? lease.checkout(rep, stream_) : lease.checkout(rep);
+        if (rc) break;
+        Scratch* sc = lease.get();
         const size_t m = hi - lo;
-        used_lo.push_back(lo);
-        used_m.push_back(m);
+        pieces.push_back({std::move(lease), lo, m});
         sc->timed = false;
         sc->poll_cancel = cancel != nullptr;
         sc->cancel_fn = ix->dynamic ? cancel : nullptr;   // a dynamic search waits for its kernels itself
@@ -894,17 +859,20 @@ int svsb200_search_cancellable(svsb200_index* ix, const void* queries, int qdtyp
         rc = step();
     }
     std::string first_error = svsb200_last_error();
+    std::vector<Scratch*> used;
+    for (const Piece& piece : pieces) used.push_back(piece.lease.get());
     // the kernels of every replica are in flight: poll the predicate until they finish (a copy into pageable host
     // memory would block this thread, so the device-to-host copies are only enqueued afterwards)
     int rc_wait = wait_kernels(used, cancel, cancel_arg);
-    for (size_t i = 0; i < used.size() && rc == 0 && rc_wait == 0; ++i) {
+    for (size_t i = 0; i < pieces.size() && rc == 0 && rc_wait == 0; ++i) {
         Scratch* sc = used[i];
         if (!sc->timed) continue;
+        const Piece& piece = pieces[i];
         auto copy_out = [&]() -> int {
             CUDA_TRY(cudaSetDevice(sc->device));
-            CUDA_TRY(cudaMemcpyAsync(static_cast<char*>(out_ids) + used_lo[i] * k * size_t(id_bytes), sc->ids.ptr,
-                                     used_m[i] * k * size_t(id_bytes), cudaMemcpyDeviceToHost, sc->stream));
-            CUDA_TRY(cudaMemcpyAsync(out_dists + used_lo[i] * k, sc->dists.ptr, used_m[i] * k * sizeof(float),
+            CUDA_TRY(cudaMemcpyAsync(static_cast<char*>(out_ids) + piece.lo * k * size_t(id_bytes), sc->ids.ptr,
+                                     piece.m * k * size_t(id_bytes), cudaMemcpyDeviceToHost, sc->stream));
+            CUDA_TRY(cudaMemcpyAsync(out_dists + piece.lo * k, sc->dists.ptr, piece.m * k * sizeof(float),
                                      cudaMemcpyDeviceToHost, sc->stream));
             return 0;
         };
@@ -912,10 +880,9 @@ int svsb200_search_cancellable(svsb200_index* ix, const void* queries, int qdtyp
         if (rc) first_error = svsb200_last_error();
     }
     if (rc_wait == 0) rc_wait = wait_all(used);
-    for (size_t i = 0; i < used.size(); ++i) {
-        used[i]->poll_cancel = false;
-        used[i]->cancel_fn = nullptr;
-        if (used_rep[i]) release(used_rep[i], used[i]);
+    for (Scratch* sc : used) {   // (before the leases give the pooled scratch sets back)
+        sc->poll_cancel = false;
+        sc->cancel_fn = nullptr;
     }
     if (rc) return fail(first_error);
     return rc_wait;
@@ -935,13 +902,21 @@ int svsb200_search_filtered(svsb200_index* ix, const void* queries, int qdtype, 
     if (k == 0) return fail("k must be greater than 0");
     if (qdtype < SVSB200_F32 || qdtype > SVSB200_U8) return fail("bad query dtype");
     Replica* rep = ix->reps[0].get();
-    CUDA_TRY(cudaSetDevice(rep->device));
-    std::string err;
-    Scratch* sc = acquire(rep, &err);
-    if (!sc) return fail(err);
-    int rc = search_filtered(ix, rep, sc, queries, qdtype, nq, k, window, id_bitmap, out_ids, out_dists, out_found);
-    release(rep, sc);
-    return rc;
+    std::vector<uint32_t> found(nq);
+    if (int rc = run_host_search(rep, {queries, id_bitmap, out_ids, out_dists, {found.data()}}, nq * ix->dim * esize(qdtype),
+                                 (ix->n + 31) / 32, nq, k, [&](Scratch* sc, const StagedBuffers& d) {
+                                     return search_filtered(ix, rep, sc, d.queries, qdtype, nq, k, window, d.bitmap, d.ids,
+                                                            d.dists, d.per_query[0]);
+                                 }))
+        return rc;
+    for (size_t q = 0; q < nq; ++q) {   // pad like the reference: unspecified id (all-ones), +inf distance
+        for (size_t j = found[q]; j < k; ++j) {
+            out_ids[q * k + j] = ~uint64_t(0);
+            out_dists[q * k + j] = INFINITY;
+        }
+        if (out_found) out_found[q] = found[q];
+    }
+    return 0;
 }
 
 int svsb200_range_search(svsb200_index* ix, const void* queries, int qdtype, size_t nq, float radius, size_t window,
@@ -953,13 +928,9 @@ int svsb200_range_search(svsb200_index* ix, const void* queries, int qdtype, siz
     *out_ids = nullptr;
     *out_dists = nullptr;
     Replica* rep = ix->reps[0].get();
-    CUDA_TRY(cudaSetDevice(rep->device));
-    std::string err;
-    Scratch* sc = acquire(rep, &err);
-    if (!sc) return fail(err);
-    int rc = range_search(ix, rep, sc, queries, qdtype, nq, radius, window, out_counts, out_ids, out_dists);
-    release(rep, sc);
-    return rc;
+    return run_host_search(rep, {queries}, nq * ix->dim * esize(qdtype), 0, nq, 0, [&](Scratch* sc, const StagedBuffers& d) {
+        return range_search(ix, rep, sc, d.queries, qdtype, nq, radius, window, out_counts, out_ids, out_dists);
+    });
 }
 
 void svsb200_free(void* p) { free(p); }
@@ -977,25 +948,15 @@ int svsb200_search_sharded(svsb200_index* const* shards, size_t nshards, const v
         if (shards[s]->dim != shards[0]->dim || shards[s]->metric != shards[0]->metric)
             return fail("svsb200_search_sharded: shards disagree on dimension or metric");
     }
+    std::vector<ScratchLease> leases(nshards);
     std::vector<Scratch*> scs;
-    std::string err;
-    auto give_back = [&]() {
-        for (size_t s = 0; s < scs.size(); ++s) release(shards[s]->reps[0].get(), scs[s]);
-    };
     for (size_t s = 0; s < nshards; ++s) {
-        Replica* rep = shards[s]->reps[0].get();
-        cudaSetDevice(rep->device);
-        Scratch* sc = acquire(rep, &err);
-        if (!sc) {
-            give_back();
-            return fail(err);
-        }
-        scs.push_back(sc);
+        if (int rc = leases[s].checkout(shards[s]->reps[0].get())) return rc;
+        scs.push_back(leases[s].get());
     }
     int rc = search_sharded(shards, scs, queries, qdtype, nq, k, window, capacity, out_ids, out_dists);
     const std::string first_error = svsb200_last_error();
     int rc_wait = wait_all(scs);
-    give_back();
     if (rc) return fail(first_error);
     return rc_wait;
 }
@@ -1051,11 +1012,9 @@ int svsb200_exhaustive_device(svsb200_index* ix, const void* d_queries, int qdty
     if (k == 0 || k > 1024) return fail("svsb200_exhaustive_device: k must be in [1, 1024]");
     if (ix->reps.size() != 1) return fail("svsb200_exhaustive_device: the index must live on exactly one device");
     Replica* rep = ix->reps[0].get();
-    CUDA_TRY(cudaSetDevice(rep->device));
-    std::string err;
-    Scratch* sc = scratch_for_stream(rep, static_cast<cudaStream_t>(stream_), &err);
-    if (!sc) return fail(err);
-    return search_on_device(ix, rep, sc, d_queries, qdtype, nq, k, k, k, d_out_ids, 8, d_out_dists, sc->stream, true);
+    return run_on_stream(rep, stream_, [&](Scratch* sc) {
+        return search_on_device(ix, rep, sc, d_queries, qdtype, nq, k, k, k, d_out_ids, 8, d_out_dists, sc->stream, true);
+    });
 }
 
 }  // extern "C"
