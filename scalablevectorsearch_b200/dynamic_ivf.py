@@ -26,16 +26,23 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import _bitmap
-from .ivf import Clustering, IVFSearchParameters, _search_filtered, _sq_codes
-from .vamana import _DTYPE_CODE, DistanceType
+from ._lib import _DTYPE_CODE
+from .ivf import Clustering, IVFSearchParameters, _index_rows, _IVFSearch
+from .vamana import DistanceType
 
 
-class DynamicIVF(_lib._Slots):
+class DynamicIVF(_lib._Slots, _IVFSearch):
     """``svs.DynamicIVF`` on one CUDA device: float32 / float16 rows or int8 / uint8 SQ codes, L2 / MIP / cosine.  A
-    delete empties the slots at once and leaves tombstones in their clusters."""
+    delete empties the slots at once and leaves tombstones in their clusters.  ``size`` counts the Valid rows,
+    ``num_slots`` the slots, Valid or Empty, and ``device_bytes`` the device memory held, the regions that clusters left
+    when they grew included until :meth:`compact`.  A search returns external ids: the exact top k over the Valid rows
+    of the probed clusters, ties by slot; short rows are padded with 2^64 - 1 and +-inf.  The filtered search is
+    :meth:`IVF.search_filtered` over the Valid rows: ``allowed`` is a boolean mask over the SLOTS (``num_slots``
+    entries, in the order of :meth:`export`; the device form's bitmap has (num_slots + 31) / 32 words), Empty slots are
+    never returned, and ``with_counts`` adds (probes used, allowed rows, Valid rows)."""
 
-    _ABI = "svsb200_dynamic_ivf"
+    _ABI = _PREFIX = "svsb200_dynamic_ivf"
+    _MASK = "num_slots"
 
     @classmethod
     def assemble_from_clustering(cls, clustering: Clustering, data, ids, distance: DistanceType = DistanceType.L2,
@@ -46,15 +53,7 @@ class DynamicIVF(_lib._Slots):
         ([0, dim]) makes an empty index to be filled with :meth:`add`.  ``sq=(scale, bias)`` marks ``data`` as int8 /
         uint8 SQ codes (see :func:`sq_compress`); the clustering must then carry assignments unless ``data`` is empty.
         The thread counts are kept for interface parity only."""
-        if sq is None:
-            x = data.load() if hasattr(data, "load") else data
-            x = np.ascontiguousarray(x)
-            if x.ndim != 2:
-                raise ValueError("data must be a 2-D array")
-            if x.dtype not in _DTYPE_CODE:
-                raise TypeError(f"unsupported data type {x.dtype}")
-        else:
-            x = _sq_codes(data, sq)
+        x = _index_rows(data, sq)
         ids = np.ascontiguousarray(np.atleast_1d(ids), dtype=np.uint64)
         if ids.shape != (x.shape[0],):
             raise ValueError("Expected IDs to be the same length as the number of rows in points!")
@@ -83,47 +82,9 @@ class DynamicIVF(_lib._Slots):
         self._h = handle
         return self
 
-    def __del__(self):
-        h = getattr(self, "_h", None)
-        if h:
-            self._lib.svsb200_dynamic_ivf_destroy(h)
-            self._h = None
-
-    @property
-    def size(self) -> int:
-        """Valid rows."""
-        return self._lib.svsb200_dynamic_ivf_size(self._h)
-
     @property
     def num_slots(self) -> int:
-        """Slots, Valid or Empty."""
         return self._lib.svsb200_dynamic_ivf_num_slots(self._h)
-
-    @property
-    def dimensions(self) -> int:
-        return self._lib.svsb200_dynamic_ivf_dimensions(self._h)
-
-    @property
-    def num_clusters(self) -> int:
-        return self._lib.svsb200_dynamic_ivf_num_clusters(self._h)
-
-    @property
-    def device_bytes(self) -> int:
-        """Device memory held, the regions that clusters left when they grew included until :meth:`compact`."""
-        return self._lib.svsb200_dynamic_ivf_device_bytes(self._h)
-
-    @property
-    def cluster_sizes(self) -> np.ndarray:
-        """Valid rows per cluster."""
-        out = np.empty(self.num_clusters, dtype=np.uint32)
-        _lib.check(self._lib.svsb200_dynamic_ivf_cluster_sizes(self._h, out.ctypes.data))
-        return out
-
-    @property
-    def centroids(self) -> np.ndarray:
-        out = np.empty((self.num_clusters, self.dimensions), dtype=np.float32)
-        _lib.check(self._lib.svsb200_dynamic_ivf_centroids(self._h, out.ctypes.data))
-        return out
 
     def add(self, points, ids, reuse_empty: bool = False) -> np.ndarray:
         """``add_points``: rows with new external ids, each appended to its nearest centroid's cluster.  Without
@@ -153,49 +114,3 @@ class DynamicIVF(_lib._Slots):
         cluster = np.empty(n, dtype=np.uint32)
         _lib.check(self._lib.svsb200_dynamic_ivf_export(self._h, status.ctypes.data, ids.ctypes.data, cluster.ctypes.data))
         return status, ids, cluster
-
-    def _n_probes(self) -> int:
-        sp = self.search_parameters
-        if not sp.k_reorder >= 1.0:
-            raise ValueError(f"k_reorder must be at least 1, got {sp.k_reorder}")
-        return int(sp.n_probes)
-
-    def search(self, queries: np.ndarray, n_neighbors: int):
-        """``svs.DynamicIVF.search(queries, n_neighbors)`` -> (external ids uint64 [nq,k], distances float32 [nq,k]):
-        the exact top k over the Valid rows of the probed clusters, ties by slot; short rows padded with 2^64 - 1 and
-        +-inf."""
-        n_probes = self._n_probes()
-        q = np.ascontiguousarray(queries)
-        if q.ndim != 2 or q.shape[1] != self.dimensions:
-            raise ValueError(f"queries must be [nq, {self.dimensions}]")
-        if q.dtype not in _DTYPE_CODE:
-            raise TypeError(f"unsupported query type {q.dtype}")
-        nq, k = q.shape[0], int(n_neighbors)
-        ids = np.empty((nq, k), dtype=np.uint64)
-        dists = np.empty((nq, k), dtype=np.float32)
-        _lib.check(self._lib.svsb200_dynamic_ivf_search(self._h, q.ctypes.data, _DTYPE_CODE[q.dtype], nq, k, n_probes,
-                                                        ids.ctypes.data, dists.ctypes.data))
-        return ids, dists
-
-    def search_device(self, d_queries: int, qdtype: np.dtype, nq: int, n_neighbors: int, d_ids: int, d_dists: int,
-                      stream: int = 0) -> None:
-        """Device-buffer form (raw pointers, e.g. ``tensor.data_ptr()``; ids uint64), enqueued on ``stream``."""
-        n_probes = self._n_probes()
-        _lib.check(self._lib.svsb200_dynamic_ivf_search_device(self._h, d_queries, _DTYPE_CODE[np.dtype(qdtype)], nq,
-                                                               int(n_neighbors), n_probes, d_ids, d_dists,
-                                                               stream or None))
-
-    def search_filtered(self, queries: np.ndarray, n_neighbors: int, allowed: np.ndarray, with_counts: bool = False):
-        """:meth:`IVF.search_filtered` over the Valid rows: ``allowed`` is a boolean mask over the SLOTS
-        (``num_slots`` entries, in the order of :meth:`export`); Empty slots are never returned.  Returns external ids,
-        distances and the number found per query; ``with_counts`` adds (probes used, allowed rows, Valid rows)."""
-        return _search_filtered(self._lib.svsb200_dynamic_ivf_search_filtered, self._h, self.dimensions, queries,
-                                n_neighbors, self._n_probes(), _bitmap(allowed, self.num_slots), with_counts)
-
-    def search_filtered_device(self, d_queries: int, qdtype: np.dtype, nq: int, n_neighbors: int, d_bitmap: int,
-                               d_ids: int, d_dists: int, d_probes: int = 0, d_allowed: int = 0, d_rows: int = 0,
-                               stream: int = 0) -> None:
-        """Device-buffer form of :meth:`search_filtered` (bitmap over slots, (num_slots + 31) / 32 words)."""
-        _lib.check(self._lib.svsb200_dynamic_ivf_search_filtered_device(
-            self._h, d_queries, _DTYPE_CODE[np.dtype(qdtype)], nq, int(n_neighbors), self._n_probes(), d_bitmap, d_ids,
-            d_dists, d_probes or None, d_allowed or None, d_rows or None, stream or None))

@@ -22,8 +22,8 @@ from dataclasses import dataclass
 import numpy as np
 
 from . import _lib
-from ._lib import _bitmap
-from .vamana import _DTYPE_CODE, DistanceType
+from ._lib import _DTYPE_CODE
+from .vamana import DistanceType
 
 
 @dataclass
@@ -46,24 +46,10 @@ class IVFSearchParameters:
     k_reorder: float = 1.0
 
 
-def _rows(data) -> np.ndarray:
-    data = data.load() if hasattr(data, "load") else data
-    data = np.ascontiguousarray(data)
-    if data.ndim != 2:
-        raise ValueError("data must be a 2-D array")
-    if data.dtype not in _DTYPE_CODE:
-        raise TypeError(f"unsupported data type {data.dtype}")
-    return data
-
-
 def sq_compress(data, dtype=np.int8, device: int = 0):
     """``SQDataset<int8_t / uint8_t>::compress`` on the GPU (``svsb200_sq_compress``): float32 rows [n, dim] ->
     (codes [n, dim] of ``dtype``, scale, bias).  NaN, infinite and constant data are refused."""
-    x = np.ascontiguousarray(data.load() if hasattr(data, "load") else data)
-    if x.ndim != 2:
-        raise ValueError("data must be a 2-D array")
-    if x.dtype != np.float32:
-        raise TypeError(f"sq_compress takes float32 rows, got {x.dtype}")
+    x = _lib._rows(data, (np.float32,), dtype_error="sq_compress takes float32 rows, got {}")
     dtype = np.dtype(dtype)
     if dtype not in (np.dtype(np.int8), np.dtype(np.uint8)):
         raise TypeError(f"SQ codes are int8 or uint8, got {dtype}")
@@ -74,32 +60,12 @@ def sq_compress(data, dtype=np.int8, device: int = 0):
     return codes, float(np.float32(scale.value)), float(np.float32(bias.value))
 
 
-def _search_filtered(fn, h, dims: int, queries, n_neighbors: int, n_probes: int, bitmap: np.ndarray, with_counts: bool):
-    """The host form of both indexes' filtered searches."""
-    q = np.ascontiguousarray(queries)
-    if q.ndim != 2 or q.shape[1] != dims:
-        raise ValueError(f"queries must be [nq, {dims}]")
-    if q.dtype not in _DTYPE_CODE:
-        raise TypeError(f"unsupported query type {q.dtype}")
-    nq, k = q.shape[0], int(n_neighbors)
-    ids = np.empty((nq, k), dtype=np.uint64)
-    dists = np.empty((nq, k), dtype=np.float32)
-    probes, allowed, rows = (np.empty(nq, dtype=np.uint32) for _ in range(3))
-    _lib.check(fn(h, q.ctypes.data, _DTYPE_CODE[q.dtype], nq, k, n_probes, bitmap.ctypes.data, ids.ctypes.data,
-                  dists.ctypes.data, probes.ctypes.data, allowed.ctypes.data, rows.ctypes.data))
-    found = np.minimum(allowed, np.uint32(k))
-    if with_counts:
-        return ids, dists, found, (probes, allowed, rows)
-    return ids, dists, found
-
-
-def _sq_codes(data, sq) -> np.ndarray:
-    """The codes of an SQ ``assemble_from_clustering``: int8 / uint8 rows."""
-    x = np.ascontiguousarray(data.load() if hasattr(data, "load") else data)
-    if x.ndim != 2:
-        raise ValueError("data must be a 2-D array")
-    if x.dtype not in (np.dtype(np.int8), np.dtype(np.uint8)):
-        raise TypeError(f"with sq=(scale, bias) the data are int8 or uint8 codes, got {x.dtype}")
+def _index_rows(data, sq) -> np.ndarray:
+    """The rows of an ``assemble_from_clustering``: int8 / uint8 SQ codes with ``sq=(scale, bias)``."""
+    if sq is None:
+        return _lib._rows(data)
+    x = _lib._rows(data, (np.int8, np.uint8),
+                   dtype_error="with sq=(scale, bias) the data are int8 or uint8 codes, got {}")
     if len(sq) != 2:
         raise ValueError("sq must be (scale, bias)")
     return x
@@ -122,7 +88,7 @@ class Clustering:
     def build(build_parameters: IVFBuildParameters, data, distance: DistanceType = DistanceType.L2,
               device: int = 0) -> "Clustering":
         """``svs.Clustering.build``: the flat k-means on the GPU (``svsb200_ivf_cluster``)."""
-        x = _rows(data)
+        x = _lib._rows(data)
         bp = build_parameters
         n, dim = x.shape
         centroids = np.empty((int(bp.num_centroids), dim), dtype=np.float32)
@@ -134,8 +100,83 @@ class Clustering:
         return Clustering(centroids, assignments)
 
 
-class IVF:
-    """``svs.IVF`` on one CUDA device."""
+class _IVFSearch(_lib._Handle):
+    """The search forms, probes and cluster accessors of IVF and DynamicIVF over ``{_PREFIX}_*``.  The filter mask has
+    one entry per ``_MASK`` (``size`` or ``num_slots``), and the bitmap of the device form (_MASK + 31) / 32 uint32
+    words."""
+
+    _MASK = "size"
+
+    @property
+    def num_clusters(self) -> int:
+        return self._cfn("num_clusters")(self._h)
+
+    @property
+    def cluster_sizes(self) -> np.ndarray:
+        """Rows per cluster (Valid rows, in a DynamicIVF)."""
+        out = np.empty(self.num_clusters, dtype=np.uint32)
+        _lib.check(self._cfn("cluster_sizes")(self._h, out.ctypes.data))
+        return out
+
+    @property
+    def centroids(self) -> np.ndarray:
+        out = np.empty((self.num_clusters, self.dimensions), dtype=np.float32)
+        _lib.check(self._cfn("centroids")(self._h, out.ctypes.data))
+        return out
+
+    def _n_probes(self) -> int:
+        sp = self.search_parameters
+        if not sp.k_reorder >= 1.0:
+            raise ValueError(f"k_reorder must be at least 1, got {sp.k_reorder}")
+        return int(sp.n_probes)
+
+    def search(self, queries: np.ndarray, n_neighbors: int):
+        """``search(queries, n_neighbors)`` -> (ids uint64 [nq,k], distances float32 [nq,k]): the exact top k over the
+        probed clusters."""
+        n_probes = self._n_probes()
+        q = _lib._queries(queries, self.dimensions)
+        return _lib._search(self._cfn("search"), (self._h,), q, n_neighbors, (n_probes,))
+
+    def search_device(self, d_queries: int, qdtype: np.dtype, nq: int, n_neighbors: int, d_ids: int, d_dists: int,
+                      stream: int = 0) -> None:
+        """Device-buffer form (raw pointers, e.g. ``tensor.data_ptr()``; ids uint64), enqueued on ``stream``."""
+        n_probes = self._n_probes()
+        _lib.check(self._cfn("search_device")(self._h, d_queries, _DTYPE_CODE[np.dtype(qdtype)], nq, int(n_neighbors),
+                                              n_probes, d_ids, d_dists, stream or None))
+
+    def search_filtered(self, queries: np.ndarray, n_neighbors: int, allowed: np.ndarray, with_counts: bool = False):
+        """``svs::runtime::IVFIndex::search(..., IDFilter*)``: ``allowed`` is a boolean mask (see the class).  Each
+        query probes ``search_parameters.n_probes`` clusters, four times more while they hold fewer than k allowed rows
+        (at most min(C, 1024)), and gets the exact top k over the allowed rows of those clusters.  Returns (ids uint64,
+        distances, found per query); short rows are padded with all-ones / +inf for every metric.  ``with_counts``
+        adds (probes used, allowed rows, rows) of the probed clusters per query."""
+        dims, n_probes = self.dimensions, self._n_probes()
+        bitmap = _lib._bitmap(allowed, getattr(self, self._MASK))
+        q = _lib._queries(queries, dims)
+        counts = tuple(np.empty(q.shape[0], dtype=np.uint32) for _ in range(3))   # probes, allowed rows, rows
+        ids, dists = _lib._search(self._cfn("search_filtered"), (self._h,), q, n_neighbors,
+                                  (n_probes, bitmap.ctypes.data), tuple(c.ctypes.data for c in counts))
+        found = np.minimum(counts[1], np.uint32(int(n_neighbors)))
+        if with_counts:
+            return ids, dists, found, counts
+        return ids, dists, found
+
+    def search_filtered_device(self, d_queries: int, qdtype: np.dtype, nq: int, n_neighbors: int, d_bitmap: int,
+                               d_ids: int, d_dists: int, d_probes: int = 0, d_allowed: int = 0, d_rows: int = 0,
+                               stream: int = 0) -> None:
+        """Device-buffer form of :meth:`search_filtered`: the uint32 bitmap (see the class) and the outputs are raw
+        device pointers (the per-query uint32 outputs may be 0), enqueued on ``stream`` apart from the probes and the
+        growth decisions."""
+        _lib.check(self._cfn("search_filtered_device")(
+            self._h, d_queries, _DTYPE_CODE[np.dtype(qdtype)], nq, int(n_neighbors), self._n_probes(), d_bitmap, d_ids,
+            d_dists, d_probes or None, d_allowed or None, d_rows or None, stream or None))
+
+
+class IVF(_IVFSearch):
+    """``svs.IVF`` on one CUDA device.  The filter mask of the filtered searches is over the ids: ``size`` entries,
+    bit i of the device form's bitmap = id i."""
+
+    _PREFIX = "svsb200_ivf"
 
     def __init__(self, handle, lib, distance: DistanceType):
         self._h, self._lib, self._distance = handle, lib, distance
@@ -147,7 +188,7 @@ class IVF:
         """``svs.IVF.assemble_from_clustering``: the rows grouped as the clustering says (a clustering without
         assignments puts every row in its nearest cluster).  ``sq=(scale, bias)`` marks ``data`` as int8 / uint8 SQ
         codes (see :func:`sq_compress`); the clustering must then carry assignments."""
-        x = _rows(data) if sq is None else _sq_codes(data, sq)
+        x = _index_rows(data, sq)
         cent = clustering.centroids
         if cent.shape[1] != x.shape[1]:
             raise ValueError(f"centroids have {cent.shape[1]} dimensions, data {x.shape[1]}")
@@ -166,84 +207,3 @@ class IVF:
                                           int(DistanceType(distance)), cent.ctypes.data, cent.shape[0],
                                           None if a is None else a.ctypes.data, int(device), C.byref(handle)))
         return IVF(handle, lib, DistanceType(distance))
-
-    def __del__(self):
-        h = getattr(self, "_h", None)
-        if h:
-            self._lib.svsb200_ivf_destroy(h)
-            self._h = None
-
-    @property
-    def size(self) -> int:
-        return self._lib.svsb200_ivf_size(self._h)
-
-    @property
-    def dimensions(self) -> int:
-        return self._lib.svsb200_ivf_dimensions(self._h)
-
-    @property
-    def num_clusters(self) -> int:
-        return self._lib.svsb200_ivf_num_clusters(self._h)
-
-    @property
-    def device_bytes(self) -> int:
-        return self._lib.svsb200_ivf_device_bytes(self._h)
-
-    @property
-    def cluster_sizes(self) -> np.ndarray:
-        out = np.empty(self.num_clusters, dtype=np.uint32)
-        _lib.check(self._lib.svsb200_ivf_cluster_sizes(self._h, out.ctypes.data))
-        return out
-
-    @property
-    def centroids(self) -> np.ndarray:
-        out = np.empty((self.num_clusters, self.dimensions), dtype=np.float32)
-        _lib.check(self._lib.svsb200_ivf_centroids(self._h, out.ctypes.data))
-        return out
-
-    def _n_probes(self) -> int:
-        sp = self.search_parameters
-        if not sp.k_reorder >= 1.0:
-            raise ValueError(f"k_reorder must be at least 1, got {sp.k_reorder}")
-        return int(sp.n_probes)
-
-    def search(self, queries: np.ndarray, n_neighbors: int):
-        """``svs.IVF.search(queries, n_neighbors)`` -> (ids uint64 [nq,k], distances float32 [nq,k])."""
-        n_probes = self._n_probes()
-        q = np.ascontiguousarray(queries)
-        if q.ndim != 2 or q.shape[1] != self.dimensions:
-            raise ValueError(f"queries must be [nq, {self.dimensions}]")
-        if q.dtype not in _DTYPE_CODE:
-            raise TypeError(f"unsupported query type {q.dtype}")
-        nq, k = q.shape[0], int(n_neighbors)
-        ids = np.empty((nq, k), dtype=np.uint64)
-        dists = np.empty((nq, k), dtype=np.float32)
-        _lib.check(self._lib.svsb200_ivf_search(self._h, q.ctypes.data, _DTYPE_CODE[q.dtype], nq, k, n_probes,
-                                                ids.ctypes.data, dists.ctypes.data))
-        return ids, dists
-
-    def search_device(self, d_queries: int, qdtype: np.dtype, nq: int, n_neighbors: int, d_ids: int, d_dists: int,
-                      stream: int = 0) -> None:
-        """Device-buffer form (raw pointers, e.g. ``tensor.data_ptr()``; ids uint64), enqueued on ``stream``."""
-        n_probes = self._n_probes()
-        _lib.check(self._lib.svsb200_ivf_search_device(self._h, d_queries, _DTYPE_CODE[np.dtype(qdtype)], nq,
-                                                       int(n_neighbors), n_probes, d_ids, d_dists, stream or None))
-
-    def search_filtered(self, queries: np.ndarray, n_neighbors: int, allowed: np.ndarray, with_counts: bool = False):
-        """``svs::runtime::IVFIndex::search(..., IDFilter*)``: ``allowed`` is a boolean mask over the ids.  Each query
-        probes ``search_parameters.n_probes`` clusters, four times more while they hold fewer than k allowed rows (at
-        most min(C, 1024)), and gets the exact top k over the allowed rows of those clusters.  Returns (ids uint64,
-        distances, found per query); short rows are padded with all-ones / +inf for every metric.  ``with_counts``
-        adds (probes used, allowed rows, rows) of the probed clusters per query."""
-        return _search_filtered(self._lib.svsb200_ivf_search_filtered, self._h, self.dimensions, queries, n_neighbors,
-                                self._n_probes(), _bitmap(allowed, self.size), with_counts)
-
-    def search_filtered_device(self, d_queries: int, qdtype: np.dtype, nq: int, n_neighbors: int, d_bitmap: int,
-                               d_ids: int, d_dists: int, d_probes: int = 0, d_allowed: int = 0, d_rows: int = 0,
-                               stream: int = 0) -> None:
-        """Device-buffer form of :meth:`search_filtered`: the uint32 bitmap ((size + 31) / 32 words, bit i = id i) and
-        the outputs are raw device pointers (the per-query uint32 outputs may be 0), enqueued on ``stream`` apart from
-        the probes and the growth decisions."""
-        _lib.check(self._lib.svsb200_ivf_search_filtered_device(
-            self._h, d_queries, _DTYPE_CODE[np.dtype(qdtype)], nq, int(n_neighbors), self._n_probes(), d_bitmap, d_ids,
-            d_dists, d_probes or None, d_allowed or None, d_rows or None, stream or None))

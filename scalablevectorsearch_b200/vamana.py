@@ -152,9 +152,8 @@ def build_graph(data: np.ndarray, distance: "DistanceType", parameters: VamanaBu
     reference builds ``SimpleData<int8_t / uint8_t>``.  ``sq=(scale, bias)`` marks ``data`` as scalar-quantised
     int8 / uint8 codes (from :func:`scalablevectorsearch_b200.ivf.sq_compress`), built as the reference builds
     ``SQDataset`` (``svsb200_build_vamana_sq``)."""
-    data = np.ascontiguousarray(data)
-    if data.dtype not in _DTYPE_CODE or data.ndim != 2:
-        raise TypeError("build_graph takes a 2-D float32 / float16 / int8 / uint8 array")
+    data = _lib._rows(data, ndim_error=None,
+                      dtype_error="build_graph takes a 2-D float32 / float16 / int8 / uint8 array")
     if sq is not None and data.dtype not in (np.int8, np.uint8):
         raise TypeError("SQ codes are int8 or uint8")
     if not parameters.use_full_search_history:
@@ -174,8 +173,10 @@ def build_graph(data: np.ndarray, distance: "DistanceType", parameters: VamanaBu
     return graph, int(ep.value)
 
 
-class Vamana:
+class Vamana(_lib._Handle):
     """GPU-backed static Vamana index exposing the reference's search surface."""
+
+    _PREFIX = "svsb200_index"
 
     @classmethod
     def build(cls, parameters: VamanaBuildParameters, data: np.ndarray, distance: "DistanceType" = None, device=0,
@@ -235,12 +236,10 @@ class Vamana:
         return self
 
     def _init(self, data, graph, entry_point, distance, device, num_threads, sq=None, lvq8=None):
-        data = np.ascontiguousarray(data)
         graph = np.ascontiguousarray(graph, dtype=np.uint32)
-        if data.ndim != 2 or graph.ndim != 2:
+        if graph.ndim != 2:
             raise ValueError("data and graph must be 2-D")
-        if data.dtype not in _DTYPE_CODE:
-            raise TypeError(f"unsupported data type {data.dtype}")
+        data = _lib._rows(data, ndim_error="data and graph must be 2-D")
         if graph.shape[0] != data.shape[0]:
             raise ValueError("Wrong sizes!")  # index/vamana/index.h:417-419
         self._lib = _lib.lib()
@@ -267,33 +266,10 @@ class Vamana:
             C.cast(aux, C.c_void_p) if aux is not None else None, dev_arr, len(devices), C.byref(handle)))
         self._h = handle
 
-    def __del__(self):
-        h = getattr(self, "_h", None)
-        if h:
-            self._lib.svsb200_index_destroy(h)
-            self._h = None
-
     # ---- properties (bindings/python/include/svs/python/manager.h:85-110) -------------
-    @property
-    def size(self) -> int:
-        return self._lib.svsb200_index_size(self._h)
-
-    @property
-    def dimensions(self) -> int:
-        return self._lib.svsb200_index_dimensions(self._h)
-
     @property
     def graph_max_degree(self) -> int:
         return self._lib.svsb200_index_max_degree(self._h)
-
-    @property
-    def num_threads(self) -> int:
-        """Kept for interface parity: the reference's thread pool is replaced by the grid."""
-        return self._num_threads
-
-    @num_threads.setter
-    def num_threads(self, n: int):
-        self._num_threads = int(n)
 
     @property
     def search_parameters(self) -> VamanaSearchParameters:
@@ -311,10 +287,6 @@ class Vamana:
     def search_window_size(self, w: int):
         # orchestrators/vamana.h set_search_window_size: window == capacity
         self._params.buffer_config = SearchBufferConfig(int(w))
-
-    @property
-    def device_bytes(self) -> int:
-        return self._lib.svsb200_index_device_bytes(self._h)
 
     # ---- search ------------------------------------------------------------------------
     @property
@@ -338,8 +310,7 @@ class Vamana:
         if q.shape[1] != self.dimensions:
             raise ValueError(f"Query has dimension {q.shape[1]}, index has {self.dimensions}")
         nq, k = q.shape[0], int(n_neighbors)
-        ids = np.empty((nq, k), dtype=np.uint64)
-        dists = np.empty((nq, k), dtype=np.float32)
+        ids, dists = _lib._results(nq, k)
         cfg = self._params.buffer_config
         if cancel is None:
             _lib.check(self._lib.svsb200_search(
@@ -374,26 +345,21 @@ class Vamana:
         """``svs::runtime::VamanaIndex::search(..., IDFilter*)`` (bindings/cpp/include/svs/runtime/vamana_index.h:75-83):
         ``allowed`` is a boolean mask over the ids (the filter's ``is_member``), evaluated on the device.
         Returns (ids uint64, distances, found per query); short rows are padded with all-ones / +inf."""
-        q = np.ascontiguousarray(queries)
-        mask = np.ascontiguousarray(allowed, dtype=bool)
-        if mask.shape != (self._lib.svsb200_index_size(self._h),):
-            raise ValueError("allowed must hold one boolean per indexed vector")
-        bitmap = np.packbits(mask, bitorder="little")
-        bitmap = np.concatenate([bitmap, np.zeros((-len(bitmap)) % 4, dtype=np.uint8)]).view(np.uint32)
-        nq, k = q.shape[0], int(n_neighbors)
-        ids = np.empty((nq, k), dtype=np.uint64)
-        dists = np.empty((nq, k), dtype=np.float32)
-        found = np.empty(nq, dtype=np.uint32)
-        _lib.check(self._lib.svsb200_search_filtered(self._h, q.ctypes.data, _DTYPE_CODE[q.dtype], nq, k,
-                                                     self._params.buffer_config.search_window_size, bitmap.ctypes.data,
-                                                     ids.ctypes.data, dists.ctypes.data, found.ctypes.data))
+        bitmap = _lib._bitmap(allowed, self._lib.svsb200_index_size(self._h))   # rows held, deleted ones included
+        q = _lib._queries(queries, self.dimensions)
+        found = np.empty(q.shape[0], dtype=np.uint32)
+        ids, dists = _lib._search(self._lib.svsb200_search_filtered, (self._h,), q, n_neighbors,
+                                  (self._params.buffer_config.search_window_size, bitmap.ctypes.data),
+                                  (found.ctypes.data,))
         return ids, dists, found
 
     def range_search(self, queries: np.ndarray, radius: float):
         """``svs::runtime::VamanaIndex::range_search`` (vamana_index.h:85-92): per query, every graph-search result
         closer than ``radius`` (greater than, for MIP).  Returns a list of (ids, distances) pairs."""
-        q = np.ascontiguousarray(queries)
+        q = _lib._queries(queries, self.dimensions)
         nq = q.shape[0]
+        if nq == 0:
+            return []
         counts = np.empty(nq, dtype=np.uint32)
         pi, pd = C.c_void_p(), C.c_void_p()
         _lib.check(self._lib.svsb200_range_search(self._h, q.ctypes.data, _DTYPE_CODE[q.dtype], nq, float(radius),
@@ -411,15 +377,8 @@ class Vamana:
         """Exact top-k of every query over ALL base vectors -- what ``svs.Flat(...).search`` computes
         (index/flat/flat.h:421-465) -- on the tensor cores, with the graph search's bit-exact distances
         (``svsb200_flat_search``)."""
-        q = np.ascontiguousarray(queries)
-        if q.ndim != 2 or q.shape[1] != self.dimensions:
-            raise ValueError("queries must be [nq, dim]")
-        nq, k = q.shape[0], int(n_neighbors)
-        ids = np.empty((nq, k), dtype=np.uint64)
-        dists = np.empty((nq, k), dtype=np.float32)
-        _lib.check(self._lib.svsb200_flat_search(self._h, q.ctypes.data, _DTYPE_CODE[q.dtype], nq, k, ids.ctypes.data,
-                                                 dists.ctypes.data))
-        return ids, dists
+        q = _lib._queries(queries, self.dimensions, "dim")
+        return _lib._search(self._lib.svsb200_flat_search, (self._h,), q, n_neighbors)
 
     def flat_search_device(self, d_queries: int, qdtype: np.dtype, nq: int, n_neighbors: int, d_ids: int, d_dists: int,
                            stream: int = 0) -> int:
@@ -483,18 +442,11 @@ class ShardedVamana:
         return sum(sh.size for sh in self._shards)
 
     def search(self, queries: np.ndarray, n_neighbors: int):
-        q = np.ascontiguousarray(queries)
-        if q.ndim != 2 or q.shape[1] != self._shards[0].dimensions:
-            raise ValueError("queries must be [nq, dim]")
-        nq, k = q.shape[0], int(n_neighbors)
-        ids = np.empty((nq, k), dtype=np.uint64)
-        dists = np.empty((nq, k), dtype=np.float32)
+        q = _lib._queries(queries, self._shards[0].dimensions, "dim")
         cfg = self.search_parameters.buffer_config
         handles = (C.c_void_p * len(self._shards))(*[sh._h for sh in self._shards])
-        _lib.check(self._lib.svsb200_search_sharded(handles, len(self._shards), q.ctypes.data, _DTYPE_CODE[q.dtype], nq, k,
-                                                    cfg.search_window_size, cfg.search_buffer_capacity,
-                                                    ids.ctypes.data, dists.ctypes.data))
-        return ids, dists
+        return _lib._search(self._lib.svsb200_search_sharded, (handles, len(self._shards)), q, n_neighbors,
+                            (cfg.search_window_size, cfg.search_buffer_capacity))
 
 
 class DynamicVamana(_lib._Slots, Vamana):
@@ -515,9 +467,8 @@ class DynamicVamana(_lib._Slots, Vamana):
         external_ids, distance)``, dynamic_index.h:208-261): the GPU builder's graph, with ``parameters`` kept as the
         mutation parameters.  ``ids`` defaults to ``0 .. n-1``."""
         distance = DistanceType.L2 if distance is None else DistanceType(distance)
-        data = np.ascontiguousarray(data)
-        if data.ndim != 2 or data.dtype not in (np.float32, np.float16):
-            raise TypeError("DynamicVamana.build takes a 2-D float32 / float16 array")
+        data = _lib._rows(data, (np.float32, np.float16), ndim_error=None,
+                          dtype_error="DynamicVamana.build takes a 2-D float32 / float16 array")
         if not parameters.use_full_search_history:
             raise ValueError("the GPU builder always keeps the full search history (the reference's default)")
         n = data.shape[0]
@@ -544,12 +495,11 @@ class DynamicVamana(_lib._Slots, Vamana):
                     distance: DistanceType = DistanceType.L2, device: int = 0, num_threads: int = 1) -> "DynamicVamana":
         """``MutableVamanaIndex(graph, data, entry_point, distance, external_ids, threadpool)``
         (dynamic_index.h:178-202); ``ids`` defaults to ``0 .. n-1``."""
-        data = np.ascontiguousarray(data)
         graph = np.ascontiguousarray(graph, dtype=np.uint32)
-        if data.ndim != 2 or graph.ndim != 2:
+        if graph.ndim != 2:
             raise ValueError("data and graph must be 2-D")
-        if data.dtype not in (np.float32, np.float16):
-            raise TypeError("a dynamic index takes float32 / float16 data")
+        data = _lib._rows(data, (np.float32, np.float16), "data and graph must be 2-D",
+                          "a dynamic index takes float32 / float16 data")
         if graph.shape[0] != data.shape[0]:
             raise ValueError("Wrong sizes!")
         n = data.shape[0]

@@ -14,6 +14,27 @@ def header_symbols():
     return sorted(set(re.findall(r"\b(svsb200_[a-z0-9_]+)\s*\(", text)))
 
 
+def header_prototypes():
+    """{symbol: (return type, [parameter declarations])} of include/svsb200.h; ``(void)`` has no parameters."""
+    text = open(os.path.join(ROOT, "include", "svsb200.h")).read()
+    text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
+    protos = {}
+    for m in re.finditer(r"(\w+\**)\s*\**\s*\b(svsb200_[a-z0-9_]+)\s*\(", text):
+        params, depth, i = [""], 1, m.end()
+        while depth:   # split at the top-level commas: a parameter may be a function pointer
+            ch = text[i]
+            depth += {"(": 1, ")": -1}.get(ch, 0)
+            if ch == "," and depth == 1:
+                params.append("")
+            elif depth:
+                params[-1] += ch
+            i += 1
+        params = [" ".join(p.split()) for p in params]
+        ret = text[m.start():m.end()].split(m.group(2))[0].strip()
+        protos[m.group(2)] = (ret, [] if params == ["void"] else params)
+    return protos
+
+
 def test_header_declares_the_expected_surface():
     syms = header_symbols()
     for name in ("svsb200_index_create", "svsb200_search", "svsb200_search_device", "svsb200_merge_topk_device",
@@ -28,6 +49,23 @@ def test_library_exports_every_declared_symbol():
     assert not missing, f"libsvsb200.so lacks {missing}"
     assert sorted(_lib.SYMBOLS) == header_symbols(), "python binding list out of sync with the header"
     assert lib.svsb200_version() == 201
+
+
+def test_abi_table_matches_the_header_prototypes():
+    """Every entry of the binding's ABI table has one argtype per parameter of its prototype, a pointer type exactly
+    where the parameter is a pointer, and the prototype's return type (no library needed)."""
+    from scalablevectorsearch_b200 import _lib
+    returns = {"int": ctypes.c_int, "size_t": ctypes.c_size_t, "uint64_t": ctypes.c_uint64, "char*": ctypes.c_char_p,
+               "void": None}
+    protos = header_prototypes()
+    assert sorted(_lib.ABI) == sorted(protos)
+    for name, (restype, argtypes) in _lib.ABI.items():
+        ret, params = protos[name]
+        assert len(argtypes) == len(params), f"{name}: {len(argtypes)} argtypes for {len(params)} parameters"
+        assert restype is returns[ret], name
+        for i, (t, p) in enumerate(zip(argtypes, params)):
+            pointer = t in (ctypes.c_void_p, ctypes.c_char_p) or issubclass(t, (ctypes._Pointer, ctypes._CFuncPtr))
+            assert pointer == ("*" in p), f"{name} parameter {i} ({p}) is bound as {t.__name__}"
 
 
 def test_no_cpu_fallback_without_a_device():
