@@ -548,6 +548,30 @@ int svsb200_ivf_random(uint64_t seed, size_t count, uint64_t* out);
 int svsb200_ivf_cluster(const void* vectors, int dtype, size_t n, size_t dim, int metric, size_t num_centroids,
                         size_t minibatch_size, size_t num_iterations, int is_hierarchical, float training_fraction,
                         uint64_t seed, int device, float* out_centroids, uint32_t* out_assignments);
+/* hierarchical_kmeans_clustering (ivf/hierarchical_kmeans.h:68-358), the reference's default IVF clustering, over the
+ * rows svsb200_ivf_cluster takes (float32 / float16, L2 / MIP / cosine, the same checks), deterministic:
+ *   1. the m training rows of svsb200_ivf_cluster's step 1 (m from C, refused when m < C);
+ *   2. L1 = level1_clusters, or size_t(sqrt(double(C))) when it is 0; refused when L1 > C;
+ *   3. svsb200_ivf_cluster's steps 2-3 with L1 centroids on the sample (split draws take m as denominator);
+ *   4. every training row to its exact nearest level-1 centroid: t_g rows in group g;
+ *   5. c_g = size_t(double(t_g) / m * C) level-2 centroids per group, then until they sum to C: j = r % L1 for the next
+ *      draw r, c_j += 1 unless t_j = 0 or c_j = t_j (then the draw is discarded), so that c_g <= t_g always;
+ *   6. every row to its exact nearest level-1 centroid among the groups with c_g > 0 (ties to the lower index);
+ *   7. per group g with c_g > 0, all groups in lockstep: its training rows in ascending order; centroid j = its row
+ *      p[j], p the first c_g of a shuffle of [0, t_g); num_iterations rounds of step 3 among its own rows and centroids
+ *      (assignment to the nearest of its own centroids, the same update, splits with t_g as denominator, MIP / cosine
+ *      normalised); finally each row of group g goes to the nearest of g's final centroids.
+ * The random sequence is svsb200_ivf_random's: the main stream (seeded with `seed`) draws the sample shuffle, the
+ * level-1 shuffle, the level-1 splits, the draws of step 5, then one value per level-1 group in ascending order (groups
+ * with c_g = 0 included), which seeds that group's own stream for its shuffle and then its splits.  Distances are exact
+ * (the search path's), ties to the lower centroid.
+ * out_centroids: float32 [C][dim], group by group (group g's from cluster_start_g = sum of c_h over h < g);
+ * out_assignments: uint32 [n], cluster_start_g + the row's centroid within its group g (not necessarily the globally
+ * nearest centroid); out_level2_counts (optional, NULL allowed): uint32 [L1], c_g. */
+int svsb200_ivf_cluster_hierarchical(const void* vectors, int dtype, size_t n, size_t dim, int metric, size_t num_centroids,
+                                     size_t level1_clusters, size_t minibatch_size, size_t num_iterations,
+                                     float training_fraction, uint64_t seed, int device, float* out_centroids,
+                                     uint32_t* out_assignments, uint32_t* out_level2_counts);
 /* IVFIndex::assemble_from_clustering: n x dim rows (HOST) grouped by `assignments` (uint32 [n], each < C; NULL:
  * every row goes to its exact nearest centroid, computed on the device) around C float32 centroids [C][dim]. */
 int svsb200_ivf_create(const void* vectors, int dtype, size_t n, size_t dim, int metric, const float* centroids,

@@ -82,6 +82,7 @@ ABI = {
     "svsb200_dynamic_flat_search_filtered_device": (i32, [vp, vp, i32, sz, sz, vp, vp, vp, vp, P(sz), P(u32)]),
     "svsb200_ivf_random": (i32, [u64, sz, vp]),
     "svsb200_ivf_cluster": (i32, [vp, i32, sz, sz, i32, sz, sz, sz, i32, f32, u64, i32, vp, vp]),
+    "svsb200_ivf_cluster_hierarchical": (i32, [vp, i32, sz, sz, i32, sz, sz, sz, sz, f32, u64, i32, vp, vp, vp]),
     "svsb200_sq_compress": (i32, [vp, sz, sz, i32, i32, vp, vp, vp]),
     "svsb200_ivf_create": (i32, [vp, i32, sz, sz, i32, vp, sz, vp, i32, P(vp)]),
     "svsb200_ivf_create_sq": (i32, [vp, i32, sz, sz, i32, f32, f32, vp, sz, vp, i32, P(vp)]),

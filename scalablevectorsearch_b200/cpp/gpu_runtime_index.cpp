@@ -22,12 +22,13 @@
 // INVALID_ARGUMENT.  Divergence: k > 1024 is INVALID_ARGUMENT (the GPU search returns at most 1024 neighbours).
 //
 // And `svs::runtime::v0::IVFIndex` (bindings/cpp/include/svs/runtime/ivf_index.h) on the IVF index of libsvsb200
-// (svsb200_ivf_*) for FP32, FP16 and SQI8 storage: `build` clusters (svsb200_ivf_cluster) and assembles the index,
+// (svsb200_ivf_*) for FP32, FP16 and SQI8 storage: `build` clusters (svsb200_ivf_cluster, or
+// svsb200_ivf_cluster_hierarchical when is_hierarchical is enabled) and assembles the index,
 // `search` probes n_probes clusters (the build's default search parameters, overridden per call).  SQI8 follows the
 // reference's init_impl: the float32 rows are clustered, then compressed to int8 (svsb200_sq_compress), then assembled
 // with the clustering's assignments (svsb200_ivf_create_sq); data that cannot be compressed (constant, or holding a
 // NaN or an infinity) is a RUNTIME_ERROR.  save / load, LeanVec and the other storage kinds are NOT_IMPLEMENTED;
-// is_hierarchical must be false (the GPU k-means is flat), and unspecified build parameters take the Python
+// an unspecified is_hierarchical keeps the flat k-means, and the other unspecified build parameters take the Python
 // IVFBuildParameters' defaults.  A non-null IDFilter becomes a bitmap over the ids (is_member(i) for every id) for
 // svsb200_ivf_search_filtered, whose probe count grows per query until k allowed rows are in reach; filter_stop and
 // filter_estimate_batch are honoured as described at filtered_search below.
@@ -607,6 +608,23 @@ uint16_t to_half(float f) {
     return uint16_t(sign | h);
 }
 
+// Clusters n rows for IVFIndex / DynamicIVFIndex::build, unspecified parameters taking the Python defaults:
+// svsb200_ivf_cluster_hierarchical when is_hierarchical is enabled (level-1 groups: hierarchical_level1_clusters, the
+// square root of C when unspecified), else the flat svsb200_ivf_cluster.  Returns non-zero on a library error.
+int cluster_rows(const IVFIndex::BuildParams& params, const void* rows, int dtype, size_t n, size_t dim, int metric, size_t C,
+                 float* centroids, uint32_t* assignments) {
+    const size_t minibatch = is_specified(params.minibatch_size) ? params.minibatch_size : 10000;
+    const size_t iters = is_specified(params.num_iterations) ? params.num_iterations : 10;
+    const float frac = is_specified(params.training_fraction) ? params.training_fraction : 0.1f;
+    const size_t seed = is_specified(params.seed) ? params.seed : 0xC0FFEE;
+    if (params.is_hierarchical.is_enabled()) {
+        const size_t l1 = is_specified(params.hierarchical_level1_clusters) ? params.hierarchical_level1_clusters : 0;
+        return svsb200_ivf_cluster_hierarchical(rows, dtype, n, dim, metric, C, l1, minibatch, iters, frac, seed, 0, centroids,
+                                                assignments, nullptr);
+    }
+    return svsb200_ivf_cluster(rows, dtype, n, dim, metric, C, minibatch, iters, 0, frac, seed, 0, centroids, assignments);
+}
+
 }  // namespace
 
 Status IVFIndex::check_storage_kind(StorageKind kind) noexcept {
@@ -624,11 +642,6 @@ Status IVFIndex::build(IVFIndex** index, size_t dim, MetricType metric, StorageK
     if (dim == 0 || n == 0 || !data) return Status(ErrorCode::INVALID_ARGUMENT, "no data");
     try {
         const size_t C = is_specified(params.num_centroids) ? params.num_centroids : 1000;
-        const size_t minibatch = is_specified(params.minibatch_size) ? params.minibatch_size : 10000;
-        const size_t iters = is_specified(params.num_iterations) ? params.num_iterations : 10;
-        const int hier = params.is_hierarchical.is_enabled() ? 1 : 0;
-        const float frac = is_specified(params.training_fraction) ? params.training_fraction : 0.1f;
-        const size_t seed = is_specified(params.seed) ? params.seed : 0xC0FFEE;
         const int m = metric == MetricType::L2 ? SVSB200_L2 : SVSB200_IP;
         const void* rows = data;
         int dtype = SVSB200_F32;
@@ -641,9 +654,7 @@ Status IVFIndex::build(IVFIndex** index, size_t dim, MetricType metric, StorageK
         }
         std::vector<float> centroids(C * dim);
         std::vector<uint32_t> assignments(n);
-        if (svsb200_ivf_cluster(rows, dtype, n, dim, m, C, minibatch, iters, hier, frac, seed, 0, centroids.data(),
-                                assignments.data()))
-            return gpu_error();
+        if (cluster_rows(params, rows, dtype, n, dim, m, C, centroids.data(), assignments.data())) return gpu_error();
         svsb200_ivf* h = nullptr;
         if (storage_kind == StorageKind::SQI8) {   // compressed after clustering, as the reference's init_impl does
             std::vector<int8_t> codes(n * dim);
@@ -696,16 +707,10 @@ Status IVFIndexLeanVec::build(IVFIndex** index, size_t, MetricType, StorageKind,
 // ---- DynamicIVFIndex ----
 namespace {
 
-// Clusters n rows (svsb200_ivf_cluster, unspecified parameters taking the Python defaults) and assembles a dynamic
-// index over them with the given labels.
+// Clusters n rows (cluster_rows) and assembles a dynamic index over them with the given labels.
 Status cluster_and_assemble(size_t dim, MetricType metric, StorageKind kind, const IVFIndex::BuildParams& params, size_t n,
                             const float* data, const size_t* labels, svsb200_dynamic_ivf** out) {
     const size_t C = is_specified(params.num_centroids) ? params.num_centroids : 1000;
-    const size_t minibatch = is_specified(params.minibatch_size) ? params.minibatch_size : 10000;
-    const size_t iters = is_specified(params.num_iterations) ? params.num_iterations : 10;
-    const int hier = params.is_hierarchical.is_enabled() ? 1 : 0;
-    const float frac = is_specified(params.training_fraction) ? params.training_fraction : 0.1f;
-    const size_t seed = is_specified(params.seed) ? params.seed : 0xC0FFEE;
     const int m = metric == MetricType::L2 ? SVSB200_L2 : SVSB200_IP;
     const void* rows = data;
     int dtype = SVSB200_F32;
@@ -718,9 +723,7 @@ Status cluster_and_assemble(size_t dim, MetricType metric, StorageKind kind, con
     }
     std::vector<float> centroids(C * dim);
     std::vector<uint32_t> assignments(n);
-    if (svsb200_ivf_cluster(rows, dtype, n, dim, m, C, minibatch, iters, hier, frac, seed, 0, centroids.data(),
-                            assignments.data()))
-        return gpu_error();
+    if (cluster_rows(params, rows, dtype, n, dim, m, C, centroids.data(), assignments.data())) return gpu_error();
     static_assert(sizeof(size_t) == 8, "labels are 64-bit");
     const uint64_t* ids = reinterpret_cast<const uint64_t*>(labels);
     if (kind == StorageKind::SQI8) {   // compressed after clustering (dynamic_ivf_index_impl.h:391-425)

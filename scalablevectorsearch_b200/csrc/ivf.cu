@@ -1,5 +1,5 @@
-// ivf.cu -- the IVF index of the C ABI (include/svsb200.h, svsb200_ivf_*): k-means clustering, the cluster-major
-// layout and the search (DESIGN.md §15).
+// ivf.cu -- the IVF index of the C ABI (include/svsb200.h, svsb200_ivf_*): flat and hierarchical k-means clustering,
+// the cluster-major layout and the search (DESIGN.md §15).
 //
 // Search, per chunk of queries:
 //   1. probe: the flat search (flat.cu) over the centroids with k = n_probes -- exact distances of the search path,
@@ -12,6 +12,8 @@
 // The per-(query, probe) lists are kept under IVF_LIST_BUDGET bytes by cutting the batch into query chunks.
 #include "ivf.cuh"
 #include "ivf_kernel.cuh"
+
+#include <cub/device/device_radix_sort.cuh>
 
 #include <algorithm>
 #include <cmath>
@@ -45,9 +47,9 @@ static std::vector<uint32_t> ivf_shuffle_prefix(uint64_t& s, size_t n, size_t m)
 }
 
 // normalize_centroids (common.h:342-363): x * (1 / norm), the norm a sequential float32 sum of squares.
-static void ivf_normalize(std::vector<float>& cent, size_t C, size_t dim) {
+static void ivf_normalize(float* cent, size_t C, size_t dim) {
     for (size_t c = 0; c < C; ++c) {
-        float* x = cent.data() + c * dim;
+        float* x = cent + c * dim;
         float acc = 0.0f;
         for (size_t d = 0; d < dim; ++d) {
             const float sq = x[d] * x[d];
@@ -61,9 +63,8 @@ static void ivf_normalize(std::vector<float>& cent, size_t C, size_t dim) {
     }
 }
 
-// centroid_split (common.h:493-537) with the documented sequence.
-static void ivf_split(std::vector<float>& cent, std::vector<uint32_t>& counts, size_t dim, size_t m, uint64_t& s) {
-    const size_t C = counts.size();
+// centroid_split (common.h:493-537) with the documented sequence, over C centroids trained on m rows.
+static void ivf_split(float* cent, uint32_t* counts, size_t C, size_t dim, size_t m, uint64_t& s) {
     for (size_t i = 0; i < C; ++i) {
         if (counts[i] != 0) continue;
         size_t j = 0;
@@ -72,8 +73,8 @@ static void ivf_split(std::vector<float>& cent, std::vector<uint32_t>& counts, s
             const float p = float(counts[j]) / float(m);
             if (ivf_uniform(s) < p) break;
         }
-        float* ci = cent.data() + i * dim;
-        float* cj = cent.data() + j * dim;
+        float* ci = cent + i * dim;
+        float* cj = cent + j * dim;
         std::copy(cj, cj + dim, ci);
         for (size_t d = 0; d < dim; ++d) {
             const double up = 1.0 + IVF_EPSILON, down = 1.0 - IVF_EPSILON;
@@ -109,6 +110,162 @@ int ivf_assign(svsb200_flat* cent, const char* d_rows, int dtype, size_t count, 
         CUDA_TRY(cudaGetLastError());
     }
     CUDA_TRY(cudaStreamSynchronize(stream));   // (before ids and dists go)
+    return 0;
+}
+
+// The checks and the training-set size of both k-means (kmeans.h:54-66): m training rows, refused when m < C.
+static int ivf_training_size(const char* who, size_t n, size_t C, size_t minibatch_size, float training_fraction, size_t* m) {
+    const std::string w(who);
+    if (C == 0) return fail(w + ": num_centroids must be positive");
+    if (minibatch_size == 0) return fail(w + ": minibatch_size must be positive");
+    if (!(training_fraction >= 0.0f) || !std::isfinite(training_fraction))
+        return fail(w + ": training_fraction must be a finite non-negative number");
+    const size_t min_training = std::min(C * IVF_MIN_TRAINING_SAMPLE_MULTIPLIER, n);
+    *m = std::min(n, std::max(min_training, size_t(std::ceil(float(n) * training_fraction))));
+    if (*m < C)
+        return fail(w + ": insufficient data for clustering: " + std::to_string(*m) + " training rows, " + std::to_string(C) +
+                    " centroids required");
+    return 0;
+}
+
+// Step 1 of both k-means: the training sample, the first m of a shuffle of [0, n) in ascending order, gathered.
+static std::vector<char> ivf_training_rows(uint64_t& s, const void* vectors, size_t n, size_t m, size_t row_bytes) {
+    std::vector<uint32_t> sample = ivf_shuffle_prefix(s, n, m);
+    std::sort(sample.begin(), sample.end());
+    const char* src = static_cast<const char*>(vectors);
+    std::vector<char> train(m * row_bytes);
+    for (size_t i = 0; i < m; ++i)
+        std::copy(src + size_t(sample[i]) * row_bytes, src + size_t(sample[i] + 1) * row_bytes, train.data() + i * row_bytes);
+    return train;
+}
+
+// Row `i` of dense rows as float32.
+static void ivf_row_f32(const char* rows, int dtype, size_t row_bytes, size_t i, size_t dim, float* out) {
+    const char* x = rows + i * row_bytes;
+    for (size_t d = 0; d < dim; ++d)
+        out[d] = dtype == SVSB200_F32 ? reinterpret_cast<const float*>(x)[d] : __half2float(reinterpret_cast<const __half*>(x)[d]);
+}
+
+// Step 3 of the flat k-means: num_iterations rounds of assignment (the centroid index `cix`, which holds `cent`), update,
+// split and normalisation of the C centroids `cent` over the m training rows d_train; `cix` follows the centroids.
+// d_assign holds at least m entries.
+static int ivf_kmeans_iterate(svsb200_flat* cix, std::vector<float>& cent, size_t C, size_t dim, const char* d_train, int dtype,
+                              size_t m, size_t minibatch_size, size_t num_iterations, bool ip_like, uint64_t& s,
+                              uint32_t* d_assign, cudaStream_t stream) {
+    const size_t row_bytes = dim * esize(dtype);
+    Replica* crep = cix->ix->reps[0].get();
+    DeviceBuffer<uint32_t> d_counts;
+    DeviceBuffer<float> d_cent;
+    CUDA_TRY(d_counts.ensure(C));
+    CUDA_TRY(d_cent.ensure(C * dim));
+    std::vector<uint32_t> counts(C);
+    for (size_t it = 0; it < num_iterations; ++it) {
+        if (int rc = ivf_assign(cix, d_train, dtype, m, row_bytes, minibatch_size, d_assign, stream)) return rc;
+        CUDA_TRY(cudaMemcpyAsync(d_cent.ptr, cent.data(), C * dim * 4, cudaMemcpyHostToDevice, stream));
+        const unsigned warps = 8;
+        const LaunchConfig cfg{int((C + warps - 1) / warps), int(warps), 0, stream};
+        CUDA_TRY(dispatch(IvfRows{}, dtype, [&](auto row) {
+            return launch_kernel(ivf_kmeans_update_kernel<decltype(row)::value>, cfg, size_t(cfg.grid), false, d_train,
+                                 uint32_t(row_bytes), uint32_t(m), uint32_t(dim), static_cast<const uint32_t*>(d_assign),
+                                 uint32_t(C), d_cent.ptr, d_counts.ptr);
+        }));
+        CUDA_TRY(cudaMemcpyAsync(cent.data(), d_cent.ptr, C * dim * 4, cudaMemcpyDeviceToHost, stream));
+        CUDA_TRY(cudaMemcpyAsync(counts.data(), d_counts.ptr, C * 4, cudaMemcpyDeviceToHost, stream));
+        CUDA_TRY(cudaStreamSynchronize(stream));
+        ivf_split(cent.data(), counts.data(), C, dim, m, s);
+        if (ip_like) ivf_normalize(cent.data(), C, dim);
+        // the centroid index takes the new rows; its GEMM operands are rebuilt by the next search
+        CUDA_TRY(cudaMemcpy2D(crep->d_vectors.ptr, cix->ix->row_stride, cent.data(), dim * 4, dim * 4, C, cudaMemcpyHostToDevice));
+        flat_slots_reset(crep);
+    }
+    return 0;
+}
+
+// The group-major permutation of `count` rows by their group keys (each < ngroups): a stable radix sort of (key, row id),
+// so that the rows of a group stay in ascending id.  Synchronises `stream`.
+static int ivf_group_rows(const uint32_t* d_keys, size_t count, size_t ngroups, uint32_t* d_perm, cudaStream_t stream) {
+    DeviceBuffer<uint32_t> ids, keys;
+    DeviceBuffer<char> temp;
+    CUDA_TRY(ids.ensure(count));
+    CUDA_TRY(keys.ensure(count));
+    ivf_iota_kernel<<<unsigned((count + 255) / 256), 256, 0, stream>>>(ids.ptr, count);
+    count_launch();
+    CUDA_TRY(cudaGetLastError());
+    int end_bit = 1;
+    while (end_bit < 32 && (size_t(1) << end_bit) < ngroups) ++end_bit;
+    size_t bytes = 0;
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, bytes, d_keys, keys.ptr, ids.ptr, d_perm, int(count), 0, end_bit, stream));
+    CUDA_TRY(temp.ensure(std::max<size_t>(bytes, 1)));
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(temp.ptr, bytes, d_keys, keys.ptr, ids.ptr, d_perm, int(count), 0, end_bit, stream));
+    CUDA_TRY(cudaStreamSynchronize(stream));   // (before the buffers go)
+    return 0;
+}
+
+// A level-1 group as the grouped kernels see it: its positions in a group-major permutation and its centroids.
+struct IvfGroup {
+    size_t pos, rows, cent, cents;
+};
+
+// Nearest centroid of every position of the groups (each row among its own group's centroids d_cent [C][dim]),
+// ivf_group_assign_kernel over work items of at most `tile` positions, launched over `batch` positions at a time (which
+// changes no result).  out: global centroid per position, or per row id with by_row.  Synchronises `stream`.
+static int ivf_group_assign(const char* d_rows, int dtype, size_t dim, int metric, const uint32_t* d_perm,
+                            const std::vector<IvfGroup>& groups, size_t batch, const float* d_cent, uint32_t* d_out, bool by_row,
+                            cudaStream_t stream) {
+    const uint32_t qs = query_stride(dim);
+    uint32_t tile = 64;
+    while (tile > 1 && ivf_group_smem_bytes(qs, 2 * tile, 0) > (size_t(96) << 10)) tile >>= 1;
+    const size_t smem = ivf_group_smem_bytes(qs, tile, tile);
+    if (smem > kSmemOptInMax - 1024) return fail("svsb200_ivf_cluster_hierarchical: rows too wide for the grouped kernels");
+    size_t total = 0;
+    for (const IvfGroup& g : groups) total = std::max(total, g.pos + g.rows);
+    // the work items of every batch, in order, and where each batch's items start
+    std::vector<uint4> items;
+    std::vector<size_t> first;
+    for (size_t lo = 0; lo < total; lo += batch) {
+        const size_t hi = std::min(total, lo + batch);
+        first.push_back(items.size());
+        for (const IvfGroup& g : groups) {
+            if (g.cents == 0) continue;
+            const size_t a = std::max(lo, g.pos), b = std::min(hi, g.pos + g.rows);
+            for (size_t x = a; x < b; x += tile)
+                items.push_back(make_uint4(uint32_t(x), uint32_t(std::min(b, x + tile)), uint32_t(g.cent), uint32_t(g.cents)));
+        }
+    }
+    first.push_back(items.size());
+    if (items.empty()) return 0;
+    DeviceBuffer<uint4> d_items;
+    CUDA_TRY(d_items.ensure(items.size()));
+    CUDA_TRY(cudaMemcpyAsync(d_items.ptr, items.data(), items.size() * sizeof(uint4), cudaMemcpyHostToDevice, stream));
+    IvfGroupAssignParams gp{};
+    gp.p.dim = uint32_t(dim);
+    gp.p.qstride = qs;
+    gp.p.greater = metric != SVSB200_L2;
+    gp.rows = d_rows;
+    gp.row_bytes = uint32_t(dim * esize(dtype));
+    gp.perm = d_perm;
+    gp.cent = d_cent;
+    gp.tile = tile;
+    gp.chunk = tile;
+    gp.out = d_out;
+    gp.by_row = by_row;
+    const int op = metric == SVSB200_L2 ? OP_L2F : metric == SVSB200_IP ? OP_IPF : OP_COSF;
+    for (size_t b = 0; b + 1 < first.size(); ++b) {
+        const size_t count = first[b + 1] - first[b];
+        if (count == 0) continue;
+        gp.items = d_items.ptr + first[b];
+        const LaunchConfig cfg{int(count), IVF_WARPS, smem, stream};
+        CUDA_TRY(dispatch(IvfRows{}, dtype, [&](auto qt) {
+            return dispatch(IvfOps{}, op, [&](auto o) {
+                constexpr int OP = decltype(o)::value;
+                return with_shape<OP, true>(uint32_t(dim), false, [&](auto ds, auto) {
+                    return launch_kernel(ivf_group_assign_kernel<decltype(qt)::value, OP, decltype(ds)::value>, cfg, count,
+                                         true, gp);
+                });
+            });
+        }));
+    }
+    CUDA_TRY(cudaStreamSynchronize(stream));   // (before the items go)
     return 0;
 }
 
@@ -495,75 +652,37 @@ int svsb200_ivf_cluster(const void* vectors, int dtype, size_t n, size_t dim, in
     const char* who = "svsb200_ivf_cluster";
     if (int rc = ivf_check_rows(who, vectors, dtype, n, dim, metric)) return rc;
     if (is_hierarchical)
-        return fail("svsb200_ivf_cluster: is_hierarchical = true: hierarchical k-means is not supported (flat k-means only)");
+        return fail("svsb200_ivf_cluster: is_hierarchical = true: this entry point is the flat k-means; hierarchical k-means "
+                    "is svsb200_ivf_cluster_hierarchical");
     if (!out_centroids || !out_assignments) return fail("svsb200_ivf_cluster: NULL output");
     const size_t C = num_centroids;
-    if (C == 0) return fail("svsb200_ivf_cluster: num_centroids must be positive");
-    if (minibatch_size == 0) return fail("svsb200_ivf_cluster: minibatch_size must be positive");
-    if (!(training_fraction >= 0.0f) || !std::isfinite(training_fraction))
-        return fail("svsb200_ivf_cluster: training_fraction must be a finite non-negative number");
-    // kmeans.h:54-66
-    const size_t min_training = std::min(C * IVF_MIN_TRAINING_SAMPLE_MULTIPLIER, n);
-    const size_t m = std::min(n, std::max(min_training, size_t(std::ceil(float(n) * training_fraction))));
-    if (m < C)
-        return fail("svsb200_ivf_cluster: insufficient data for clustering: " + std::to_string(m) + " training rows, " +
-                    std::to_string(C) + " centroids required");
+    size_t m = 0;
+    if (int rc = ivf_training_size(who, n, C, minibatch_size, training_fraction, &m)) return rc;
     cudaDeviceProp prop;
     if (int rc = check_device(who, device, &prop)) return rc;
     CUDA_TRY(cudaSetDevice(device));
     const size_t row_bytes = dim * esize(dtype);
-    const char* src = static_cast<const char*>(vectors);
     // 1-2. training sample and initial centroids
     uint64_t s = seed;
-    std::vector<uint32_t> sample = ivf_shuffle_prefix(s, n, m);
-    std::sort(sample.begin(), sample.end());
+    const std::vector<char> train = ivf_training_rows(s, vectors, n, m, row_bytes);
     const std::vector<uint32_t> init = ivf_shuffle_prefix(s, m, C);
-    std::vector<char> train(m * row_bytes);
-    for (size_t i = 0; i < m; ++i) std::copy(src + size_t(sample[i]) * row_bytes, src + size_t(sample[i] + 1) * row_bytes,
-                                             train.data() + i * row_bytes);
     std::vector<float> cent(C * dim);
-    for (size_t c = 0; c < C; ++c)
-        for (size_t d = 0; d < dim; ++d) {
-            const char* x = train.data() + size_t(init[c]) * row_bytes;
-            cent[c * dim + d] = dtype == SVSB200_F32 ? reinterpret_cast<const float*>(x)[d]
-                                                     : __half2float(reinterpret_cast<const __half*>(x)[d]);
-        }
+    for (size_t c = 0; c < C; ++c) ivf_row_f32(train.data(), dtype, row_bytes, init[c], dim, cent.data() + c * dim);
     const bool ip_like = metric != SVSB200_L2;
-    if (ip_like) ivf_normalize(cent, C, dim);
+    if (ip_like) ivf_normalize(cent.data(), C, dim);
     OwnStream own;
     CUDA_TRY(cudaStreamCreateWithFlags(&own.s, cudaStreamNonBlocking));
     std::unique_ptr<svsb200_flat> cix;
     if (int rc = ivf_centroid_index(cent.data(), C, dim, metric, device, &cix)) return rc;
-    Replica* crep = cix->ix->reps[0].get();
     DeviceBuffer<char> d_train;
-    DeviceBuffer<uint32_t> d_assign, d_counts;
-    DeviceBuffer<float> d_cent;
+    DeviceBuffer<uint32_t> d_assign;
     CUDA_TRY(d_train.ensure(m * row_bytes));
     CUDA_TRY(d_assign.ensure(std::max(m, n)));
-    CUDA_TRY(d_counts.ensure(C));
-    CUDA_TRY(d_cent.ensure(C * dim));
     CUDA_TRY(cudaMemcpy(d_train.ptr, train.data(), m * row_bytes, cudaMemcpyHostToDevice));
-    std::vector<uint32_t> counts(C);
     // 3. iterations
-    for (size_t it = 0; it < num_iterations; ++it) {
-        if (int rc = ivf_assign(cix.get(), d_train.ptr, dtype, m, row_bytes, minibatch_size, d_assign.ptr, own.s)) return rc;
-        CUDA_TRY(cudaMemcpyAsync(d_cent.ptr, cent.data(), C * dim * 4, cudaMemcpyHostToDevice, own.s));
-        const unsigned warps = 8;
-        const LaunchConfig cfg{int((C + warps - 1) / warps), int(warps), 0, own.s};
-        CUDA_TRY(dispatch(IvfRows{}, dtype, [&](auto row) {
-            return launch_kernel(ivf_kmeans_update_kernel<decltype(row)::value>, cfg, size_t(cfg.grid), false,
-                                 static_cast<const char*>(d_train.ptr), uint32_t(row_bytes), uint32_t(m), uint32_t(dim),
-                                 static_cast<const uint32_t*>(d_assign.ptr), uint32_t(C), d_cent.ptr, d_counts.ptr);
-        }));
-        CUDA_TRY(cudaMemcpyAsync(cent.data(), d_cent.ptr, C * dim * 4, cudaMemcpyDeviceToHost, own.s));
-        CUDA_TRY(cudaMemcpyAsync(counts.data(), d_counts.ptr, C * 4, cudaMemcpyDeviceToHost, own.s));
-        CUDA_TRY(cudaStreamSynchronize(own.s));
-        ivf_split(cent, counts, dim, m, s);
-        if (ip_like) ivf_normalize(cent, C, dim);
-        // the centroid index takes the new rows; its GEMM operands are rebuilt by the next search
-        CUDA_TRY(cudaMemcpy2D(crep->d_vectors.ptr, cix->ix->row_stride, cent.data(), dim * 4, dim * 4, C, cudaMemcpyHostToDevice));
-        flat_slots_reset(crep);
-    }
+    if (int rc = ivf_kmeans_iterate(cix.get(), cent, C, dim, d_train.ptr, dtype, m, minibatch_size, num_iterations, ip_like, s,
+                                    d_assign.ptr, own.s))
+        return rc;
     // 4. final assignment of every row
     DeviceBuffer<char> d_rows;
     CUDA_TRY(d_rows.ensure(n * row_bytes));
@@ -571,6 +690,155 @@ int svsb200_ivf_cluster(const void* vectors, int dtype, size_t n, size_t dim, in
     if (int rc = ivf_assign(cix.get(), d_rows.ptr, dtype, n, row_bytes, minibatch_size, d_assign.ptr, own.s)) return rc;
     CUDA_TRY(cudaMemcpy(out_assignments, d_assign.ptr, n * 4, cudaMemcpyDeviceToHost));
     std::copy(cent.begin(), cent.end(), out_centroids);
+    return 0;
+}
+
+int svsb200_ivf_cluster_hierarchical(const void* vectors, int dtype, size_t n, size_t dim, int metric, size_t num_centroids,
+                                     size_t level1_clusters, size_t minibatch_size, size_t num_iterations,
+                                     float training_fraction, uint64_t seed, int device, float* out_centroids,
+                                     uint32_t* out_assignments, uint32_t* out_level2_counts) {
+    const char* who = "svsb200_ivf_cluster_hierarchical";
+    if (int rc = ivf_check_rows(who, vectors, dtype, n, dim, metric)) return rc;
+    if (!out_centroids || !out_assignments) return fail("svsb200_ivf_cluster_hierarchical: NULL output");
+    const size_t C = num_centroids;
+    size_t m = 0;
+    if (int rc = ivf_training_size(who, n, C, minibatch_size, training_fraction, &m)) return rc;
+    const size_t L1 = level1_clusters ? level1_clusters : size_t(std::sqrt(double(C)));
+    if (L1 > C)
+        return fail("svsb200_ivf_cluster_hierarchical: level1_clusters (" + std::to_string(L1) +
+                    ") must be at most num_centroids (" + std::to_string(C) + ")");
+    cudaDeviceProp prop;
+    if (int rc = check_device(who, device, &prop)) return rc;
+    CUDA_TRY(cudaSetDevice(device));
+    const size_t row_bytes = dim * esize(dtype);
+    const bool ip_like = metric != SVSB200_L2;
+    // 1. training sample
+    uint64_t s = seed;
+    const std::vector<char> train = ivf_training_rows(s, vectors, n, m, row_bytes);
+    // 2-3. level 1: the flat k-means with L1 centroids on the sample
+    const std::vector<uint32_t> init1 = ivf_shuffle_prefix(s, m, L1);
+    std::vector<float> cent1(L1 * dim);
+    for (size_t c = 0; c < L1; ++c) ivf_row_f32(train.data(), dtype, row_bytes, init1[c], dim, cent1.data() + c * dim);
+    if (ip_like) ivf_normalize(cent1.data(), L1, dim);
+    OwnStream own;
+    CUDA_TRY(cudaStreamCreateWithFlags(&own.s, cudaStreamNonBlocking));
+    std::unique_ptr<svsb200_flat> cix1;
+    if (int rc = ivf_centroid_index(cent1.data(), L1, dim, metric, device, &cix1)) return rc;
+    DeviceBuffer<char> d_train;
+    DeviceBuffer<uint32_t> d_tl1, d_tperm, d_tassign, d_counts;
+    CUDA_TRY(d_train.ensure(m * row_bytes));
+    CUDA_TRY(d_tl1.ensure(m));
+    CUDA_TRY(cudaMemcpy(d_train.ptr, train.data(), m * row_bytes, cudaMemcpyHostToDevice));
+    if (int rc = ivf_kmeans_iterate(cix1.get(), cent1, L1, dim, d_train.ptr, dtype, m, minibatch_size, num_iterations, ip_like, s,
+                                    d_tl1.ptr, own.s))
+        return rc;
+    // 4. the sample against the final level-1 centroids: t_g training rows per group
+    if (int rc = ivf_assign(cix1.get(), d_train.ptr, dtype, m, row_bytes, minibatch_size, d_tl1.ptr, own.s)) return rc;
+    std::vector<uint32_t> tl1(m);
+    CUDA_TRY(cudaMemcpy(tl1.data(), d_tl1.ptr, m * 4, cudaMemcpyDeviceToHost));
+    std::vector<size_t> t(L1, 0), c(L1), tstart(L1), cstart(L1);
+    for (uint32_t g : tl1) ++t[g];
+    // 5. level-2 centroids per group: the proportional floor, then remainder draws (a draw on a group without training
+    // rows, or with as many centroids as training rows, is discarded)
+    size_t total = 0;
+    for (size_t g = 0; g < L1; ++g) total += c[g] = size_t(double(t[g]) / double(m) * double(C));
+    while (total < C) {
+        const size_t j = ivf_next(s) % L1;
+        if (t[j] == 0 || c[j] == t[j]) continue;
+        ++c[j];
+        ++total;
+    }
+    std::vector<uint64_t> gs(L1);   // the groups' own streams
+    for (size_t g = 0; g < L1; ++g) gs[g] = ivf_next(s);
+    for (size_t g = 0, tp = 0, cp = 0; g < L1; tp += t[g], cp += c[g], ++g) {
+        tstart[g] = tp;
+        cstart[g] = cp;
+    }
+    // 7. level 2, every group in lockstep: the training rows group-major, each group's centroids from its own rows
+    CUDA_TRY(d_tperm.ensure(m));
+    if (int rc = ivf_group_rows(d_tl1.ptr, m, L1, d_tperm.ptr, own.s)) return rc;
+    std::vector<uint32_t> tperm(m);   // (the same permutation on the host, for the initial centroids)
+    {
+        std::vector<size_t> fill(tstart);
+        for (size_t i = 0; i < m; ++i) tperm[fill[tl1[i]]++] = uint32_t(i);
+    }
+    std::vector<float> cent(C * dim);
+    std::vector<IvfGroup> tgroups(L1);
+    std::vector<uint2> range(C);
+    for (size_t g = 0; g < L1; ++g) {
+        tgroups[g] = {tstart[g], t[g], cstart[g], c[g]};
+        if (c[g] == 0) continue;
+        const std::vector<uint32_t> init = ivf_shuffle_prefix(gs[g], t[g], c[g]);
+        for (size_t j = 0; j < c[g]; ++j) {
+            ivf_row_f32(train.data(), dtype, row_bytes, tperm[tstart[g] + init[j]], dim, cent.data() + (cstart[g] + j) * dim);
+            range[cstart[g] + j] = make_uint2(uint32_t(tstart[g]), uint32_t(tstart[g] + t[g]));
+        }
+    }
+    if (ip_like) ivf_normalize(cent.data(), C, dim);
+    DeviceBuffer<float> d_cent;
+    DeviceBuffer<uint2> d_range;
+    CUDA_TRY(d_cent.ensure(C * dim));
+    CUDA_TRY(d_range.ensure(C));
+    CUDA_TRY(d_tassign.ensure(m));
+    CUDA_TRY(d_counts.ensure(C));
+    CUDA_TRY(cudaMemcpy(d_range.ptr, range.data(), C * sizeof(uint2), cudaMemcpyHostToDevice));
+    std::vector<uint32_t> counts(C);
+    for (size_t it = 0; it < num_iterations; ++it) {
+        CUDA_TRY(cudaMemcpyAsync(d_cent.ptr, cent.data(), C * dim * 4, cudaMemcpyHostToDevice, own.s));
+        if (int rc = ivf_group_assign(d_train.ptr, dtype, dim, metric, d_tperm.ptr, tgroups, minibatch_size, d_cent.ptr,
+                                      d_tassign.ptr, false, own.s))
+            return rc;
+        const unsigned warps = 8;
+        const LaunchConfig cfg{int((C + warps - 1) / warps), int(warps), 0, own.s};
+        CUDA_TRY(dispatch(IvfRows{}, dtype, [&](auto row) {
+            return launch_kernel(ivf_kmeans_group_update_kernel<decltype(row)::value>, cfg, size_t(cfg.grid), false,
+                                 static_cast<const char*>(d_train.ptr), uint32_t(row_bytes),
+                                 static_cast<const uint32_t*>(d_tperm.ptr), static_cast<const uint2*>(d_range.ptr),
+                                 uint32_t(dim), static_cast<const uint32_t*>(d_tassign.ptr), uint32_t(C), d_cent.ptr,
+                                 d_counts.ptr);
+        }));
+        CUDA_TRY(cudaMemcpyAsync(cent.data(), d_cent.ptr, C * dim * 4, cudaMemcpyDeviceToHost, own.s));
+        CUDA_TRY(cudaMemcpyAsync(counts.data(), d_counts.ptr, C * 4, cudaMemcpyDeviceToHost, own.s));
+        CUDA_TRY(cudaStreamSynchronize(own.s));
+        for (size_t g = 0; g < L1; ++g)
+            if (c[g]) ivf_split(cent.data() + cstart[g] * dim, counts.data() + cstart[g], c[g], dim, t[g], gs[g]);
+        if (ip_like) ivf_normalize(cent.data(), C, dim);
+    }
+    // 6. every row to its nearest level-1 centroid among the groups with level-2 centroids
+    std::vector<uint32_t> pop;
+    for (size_t g = 0; g < L1; ++g)
+        if (c[g]) pop.push_back(uint32_t(g));
+    std::unique_ptr<svsb200_flat> cixp;
+    if (pop.size() < L1) {
+        std::vector<float> cp(pop.size() * dim);
+        for (size_t i = 0; i < pop.size(); ++i)
+            std::copy(cent1.begin() + pop[i] * dim, cent1.begin() + (pop[i] + 1) * dim, cp.begin() + i * dim);
+        if (int rc = ivf_centroid_index(cp.data(), pop.size(), dim, metric, device, &cixp)) return rc;
+    }
+    DeviceBuffer<char> d_rows;
+    DeviceBuffer<uint32_t> d_assign, d_perm;
+    CUDA_TRY(d_rows.ensure(n * row_bytes));
+    CUDA_TRY(d_assign.ensure(n));
+    CUDA_TRY(d_perm.ensure(n));
+    CUDA_TRY(cudaMemcpy(d_rows.ptr, vectors, n * row_bytes, cudaMemcpyHostToDevice));
+    if (int rc = ivf_assign(cixp ? cixp.get() : cix1.get(), d_rows.ptr, dtype, n, row_bytes, minibatch_size, d_assign.ptr, own.s))
+        return rc;
+    std::vector<uint32_t> al1(n);   // the index of the row's group in `pop`
+    CUDA_TRY(cudaMemcpy(al1.data(), d_assign.ptr, n * 4, cudaMemcpyDeviceToHost));
+    std::vector<size_t> a(pop.size(), 0);
+    for (uint32_t p : al1) ++a[p];
+    if (int rc = ivf_group_rows(d_assign.ptr, n, pop.size(), d_perm.ptr, own.s)) return rc;
+    std::vector<IvfGroup> agroups(pop.size());
+    for (size_t i = 0, ap = 0; i < pop.size(); ap += a[i], ++i) agroups[i] = {ap, a[i], cstart[pop[i]], c[pop[i]]};
+    // 7. every row to the nearest of its own group's level-2 centroids
+    CUDA_TRY(cudaMemcpy(d_cent.ptr, cent.data(), C * dim * 4, cudaMemcpyHostToDevice));
+    if (int rc = ivf_group_assign(d_rows.ptr, dtype, dim, metric, d_perm.ptr, agroups, minibatch_size, d_cent.ptr, d_assign.ptr,
+                                  true, own.s))
+        return rc;
+    CUDA_TRY(cudaMemcpy(out_assignments, d_assign.ptr, n * 4, cudaMemcpyDeviceToHost));
+    std::copy(cent.begin(), cent.end(), out_centroids);
+    if (out_level2_counts)
+        for (size_t g = 0; g < L1; ++g) out_level2_counts[g] = uint32_t(c[g]);
     return 0;
 }
 

@@ -1,4 +1,5 @@
-// ivf_kernel.cuh -- kernels of the IVF index (ivf.cu): the cluster-major leaf scan and the k-means update.
+// ivf_kernel.cuh -- kernels of the IVF index (ivf.cu): the cluster-major leaf scan, the k-means update and the grouped
+// assignment and update of the hierarchical k-means.
 //
 // Replaces, for float32 / float16 rows (file:line under the reference's include/svs):
 //   index/ivf/index.h  IVFIndex::search's leaf scan (one thread per query walks each probed cluster)
@@ -13,6 +14,7 @@
 // (distance, original id): the TotalOrder of the merge that follows (merge_topk_kernel).
 #pragma once
 
+#include "query_prep.cuh"
 #include "search_kernel.cuh"
 
 namespace svsb200 {
@@ -606,6 +608,174 @@ __global__ void ivf_kmeans_update_kernel(const char* __restrict__ train, uint32_
         for (uint32_t d = lane; d < dim; d += 32) row[d] = __fmul_rn(row[d], inv);
     }
     if (lane == 0) counts[c] = cnt;
+}
+
+// ---- hierarchical k-means: the level-2 problems of every level-1 group at once (ivf.cu, ivf_group_assign) ----
+// Rows are reached through a group-major permutation `perm` (ascending row id inside a group); a position is an index
+// into it.  One work item is a tile of at most `tile` positions of one group with that group's centroid range.
+struct IvfGroupAssignParams {
+    SearchParams p;           // dim, qstride, greater (the distance code's fields)
+    const char* rows;         // dense rows of the row type, row_bytes apart
+    uint32_t row_bytes;
+    const uint32_t* perm;     // position -> row id
+    const uint4* items;       // {first position, end position, first centroid, centroids}
+    const float* cent;        // [C][dim] dense float32 centroids
+    uint32_t tile, chunk;     // positions per item, centroids staged per round
+    uint32_t* out;            // global centroid of every position (by_row: of every row id)
+    int by_row;
+};
+
+// Shared memory of one CTA: the tile's prepared rows and the staged centroids (qstride floats each), then per row of the
+// tile the query's a_norm and its best (key, centroid).
+__host__ __device__ inline size_t ivf_group_smem_bytes(uint32_t qstride, uint32_t tile, uint32_t chunk) {
+    return (size_t(tile) + chunk) * qstride * 4 + size_t(tile) * 12;
+}
+
+// (key, centroid) a before b: NaN keys last, then key, then the lower centroid (the order of the model's lexsort).
+__device__ __forceinline__ bool ivf_nearer(float ka, uint32_t ia, float kb, uint32_t ib) {
+    const bool na = isnan(ka), nb = isnan(kb);
+    if (na != nb) return nb;
+    if (!na && (ka < kb || kb < ka)) return ka < kb;
+    return ia < ib;
+}
+
+// Nearest centroid of every position of an item among its group's centroids: each row of the tile is prepared in shared
+// memory as prepare_queries_kernel prepares a query (PREP_FLOAT), the group's centroids pass through shared memory
+// `chunk` at a time (each read once per tile), and a warp scores one row against the staged centroids with the scan's
+// distance code (float_rows over float32 rows in its shared-memory form, finish_distance) -- the bits of a search of the
+// row against the centroids.  Ties go to the lower centroid.
+template <int QT, int OP, int DS>
+__global__ void __launch_bounds__(IVF_WARPS * 32, 2) ivf_group_assign_kernel(const __grid_constant__ IvfGroupAssignParams gp) {
+    constexpr int NR = OP == OP_COSF || DS == 0 ? 1 : 2;   // (two centroids per pass spill at the generic dimension)
+    constexpr int G = 16 / Row<SVSB200_F32>::LPT;   // threads per centroid
+    constexpr int GROUPS = 32 / G;                  // centroids per warp and pass
+    constexpr unsigned FULL = 0xFFFFFFFFu;
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    const SearchParams& p = gp.p;
+    const uint32_t qs = p.qstride, dim = p.dim;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int g = lane / G, t = lane % G;
+    float* qv = reinterpret_cast<float*>(smem_raw);   // [tile][qs]
+    float* cv = qv + size_t(gp.tile) * qs;             // [chunk][qs]
+    float* aux = cv + size_t(gp.chunk) * qs;           // [tile]
+    float* bkey = aux + gp.tile;                       // [tile]
+    uint32_t* bidx = reinterpret_cast<uint32_t*>(bkey + gp.tile);
+    const float ksign = p.greater ? -1.0f : 1.0f;
+    const uint4 it = gp.items[blockIdx.x];
+    const uint32_t nrows = it.y - it.x;
+    for (uint32_t i = threadIdx.x; i < gp.tile * qs; i += IVF_WARPS * 32) {
+        const uint32_t r = i / qs, e = i - r * qs;
+        float v = 0.f;
+        if (r < nrows && e < dim) v = q_simd<QT>(gp.rows + size_t(gp.perm[it.x + r]) * gp.row_bytes, e);
+        qv[i] = v;
+    }
+    for (uint32_t i = threadIdx.x; i < gp.chunk * qs; i += IVF_WARPS * 32) cv[i] = 0.f;   // (the padding stays zero)
+    if (threadIdx.x < gp.tile) {
+        float a = 0.f;
+        if (OP == OP_COSF && threadIdx.x < nrows) {
+            const char* src = gp.rows + size_t(gp.perm[it.x + threadIdx.x]) * gp.row_bytes;
+            a = sequential_norm(dim, [&](uint32_t i) {
+                const float v = q_scalar<QT>(src, i);
+                return __fmul_rn(v, v);
+            });
+        }
+        aux[threadIdx.x] = a;
+        bkey[threadIdx.x] = __int_as_float(0x7FC00000);
+        bidx[threadIdx.x] = 0xFFFFFFFFu;
+    }
+    for (uint32_t c0 = 0; c0 < it.w; c0 += gp.chunk) {
+        const uint32_t cn = min(gp.chunk, it.w - c0);
+        __syncthreads();   // (the previous chunk is consumed; the first time: the preparation is done)
+        const float* src = gp.cent + size_t(it.z + c0) * dim;
+        for (uint32_t i = threadIdx.x; i < cn * dim; i += IVF_WARPS * 32) {
+            const uint32_t r = i / dim;
+            cv[r * qs + (i - r * dim)] = src[i];
+        }
+        __syncthreads();
+#pragma unroll 1
+        for (uint32_t r = warp; r < nrows; r += IVF_WARPS) {
+            const float* q_s = qv + size_t(r) * qs;
+            const float a = aux[r];
+            float best = __int_as_float(0x7FC00000);
+            uint32_t bi = 0xFFFFFFFFu;
+#pragma unroll 1
+            for (uint32_t base = 0; base < cn; base += NR * GROUPS) {
+                const char* rowp[NR];
+                uint32_t idx[NR];
+#pragma unroll
+                for (int k = 0; k < NR; ++k) {
+                    idx[k] = base + k * GROUPS + g;
+                    rowp[k] = idx[k] < cn ? reinterpret_cast<const char*>(cv + size_t(idx[k]) * qs) : nullptr;
+                }
+                float sum[NR], nrm[NR];
+                float_rows<SVSB200_F32, OP, DS, NR, false, true>(p, q_s, rowp, t, sum, nrm);
+#pragma unroll
+                for (int k = 0; k < NR; ++k) {
+                    const float key = __fmul_rn(finish_distance<OP>(p, sum[k], nrm[k], 0, 0, a, 0.0f), ksign);
+                    if (rowp[k] && ivf_nearer(key, c0 + idx[k], best, bi)) {
+                        best = key;
+                        bi = c0 + idx[k];
+                    }
+                }
+            }
+            for (int off = 16; off; off >>= 1) {
+                const float ok = __shfl_xor_sync(FULL, best, off);
+                const uint32_t oi = __shfl_xor_sync(FULL, bi, off);
+                if (ivf_nearer(ok, oi, best, bi)) {
+                    best = ok;
+                    bi = oi;
+                }
+            }
+            if (lane == 0 && ivf_nearer(best, bi, bkey[r], bidx[r])) {
+                bkey[r] = best;
+                bidx[r] = bi;
+            }
+        }
+    }
+    __syncthreads();
+    for (uint32_t r = threadIdx.x; r < nrows; r += IVF_WARPS * 32)
+        gp.out[gp.by_row ? gp.perm[it.x + r] : it.x + r] = it.z + bidx[r];
+}
+
+// ivf_kmeans_update_kernel's rule for the level-2 centroids: one warp per centroid c, whose members are the positions
+// of its group's range [range[c].x, range[c].y) assigned to it (assign is by position), summed in ascending position
+// (= ascending training row) order onto the old centroid.
+template <int ROWT>
+__global__ void ivf_kmeans_group_update_kernel(const char* __restrict__ train, uint32_t row_bytes, const uint32_t* __restrict__ perm,
+                                               const uint2* __restrict__ range, uint32_t dim, const uint32_t* __restrict__ assign,
+                                               uint32_t C, float* __restrict__ cent, uint32_t* __restrict__ counts) {
+    const uint32_t c = blockIdx.x * (blockDim.x / 32) + threadIdx.x / 32;
+    const int lane = threadIdx.x & 31;
+    if (c >= C) return;
+    float* row = cent + size_t(c) * dim;
+    const uint32_t lo = range[c].x, hi = range[c].y;
+    uint32_t cnt = 0;
+    for (uint32_t i0 = lo; i0 < hi; i0 += 32) {
+        const uint32_t i = i0 + lane;
+        unsigned m = __ballot_sync(0xFFFFFFFFu, i < hi && assign[i] == c);
+        cnt += __popc(m);
+        while (m) {
+            const uint32_t r = i0 + __ffs(m) - 1;
+            m &= m - 1;
+            const char* x = train + size_t(perm[r]) * row_bytes;
+            for (uint32_t d = lane; d < dim; d += 32) {
+                const float v = ROWT == SVSB200_F32 ? reinterpret_cast<const float*>(x)[d]
+                                                    : __half2float(reinterpret_cast<const __half*>(x)[d]);
+                row[d] = __fadd_rn(row[d], v);
+            }
+        }
+    }
+    if (cnt) {
+        const float inv = __double2float_rn(__ddiv_rn(1.0, double(cnt) + 1.0));
+        for (uint32_t d = lane; d < dim; d += 32) row[d] = __fmul_rn(row[d], inv);
+    }
+    if (lane == 0) counts[c] = cnt;
+}
+
+// out[i] = i: the row ids a stable sort by group permutes.
+__global__ void ivf_iota_kernel(uint32_t* __restrict__ out, size_t count) {
+    const size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (i < count) out[i] = uint32_t(i);
 }
 
 // ---- filtered search (ivf.cu, ivf_search_filtered_on_device) ----

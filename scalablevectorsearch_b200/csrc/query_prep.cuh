@@ -1,11 +1,31 @@
 // query_prep.cuh -- the element and per-query rules of query preparation (distance::maybe_fix_argument), shared by the
-// search's prepare_queries_kernel (search.cu) and the graph builder's preparation of an SQ datum as its own query
-// (build_kernels.cuh, stage_sq_datum).
+// search's prepare_queries_kernel (search.cu), the graph builder's preparation of an SQ datum as its own query
+// (build_kernels.cuh, stage_sq_datum) and the hierarchical k-means's rows prepared as queries (ivf_kernel.cuh,
+// ivf_group_assign_kernel).
 #pragma once
 
 #include "common.cuh"
 
 namespace svsb200 {
+
+// Float16 -> float the way non-SIMD reference code does it (lib/float16.h:45-52):
+// subnormals flush to signed zero.
+__device__ __forceinline__ float f16_scalar(uint16_t x) {
+    if ((x & 0x7C00u) == 0) return __uint_as_float(uint32_t(x & 0x8000u) << 16);
+    return __half2float(__ushort_as_half(x));
+}
+
+// Element i of a query as the SIMD kernels load it, and as the scalar code (norms, compression) reads it.
+template <int QT> __device__ __forceinline__ float q_simd(const void* q, uint32_t i) {
+    if constexpr (QT == SVSB200_F32) return static_cast<const float*>(q)[i];
+    if constexpr (QT == SVSB200_F16) return __half2float(__ushort_as_half(static_cast<const uint16_t*>(q)[i]));
+    if constexpr (QT == SVSB200_I8) return float(static_cast<const int8_t*>(q)[i]);
+    return float(static_cast<const uint8_t*>(q)[i]);
+}
+template <int QT> __device__ __forceinline__ float q_scalar(const void* q, uint32_t i) {
+    if constexpr (QT == SVSB200_F16) return f16_scalar(static_cast<const uint16_t*>(q)[i]);
+    return q_simd<QT>(q, i);
+}
 
 // detail::compress (quantization/scalar/scalar.h:38-42): clamp(round((x - bias) / scale)) as an int8 / uint8 code byte.
 __device__ __forceinline__ uint8_t sq_compress_code(float x, int code_type, float scale, float bias) {

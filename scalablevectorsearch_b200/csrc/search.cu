@@ -17,24 +17,6 @@ namespace svsb200 {
 // (concepts/distance.h:90-130), one warp per query.
 // ---------------------------------------------------------------------------------------
 
-// Float16 -> float the way non-SIMD reference code does it (lib/float16.h:45-52):
-// subnormals flush to signed zero.
-__device__ __forceinline__ float f16_scalar(uint16_t x) {
-    if ((x & 0x7C00u) == 0) return __uint_as_float(uint32_t(x & 0x8000u) << 16);
-    return __half2float(__ushort_as_half(x));
-}
-
-template <int QT> __device__ __forceinline__ float q_simd(const void* q, uint32_t i) {
-    if constexpr (QT == SVSB200_F32) return static_cast<const float*>(q)[i];
-    if constexpr (QT == SVSB200_F16) return __half2float(__ushort_as_half(static_cast<const uint16_t*>(q)[i]));
-    if constexpr (QT == SVSB200_I8) return float(static_cast<const int8_t*>(q)[i]);
-    return float(static_cast<const uint8_t*>(q)[i]);
-}
-template <int QT> __device__ __forceinline__ float q_scalar(const void* q, uint32_t i) {
-    if constexpr (QT == SVSB200_F16) return f16_scalar(static_cast<const uint16_t*>(q)[i]);
-    return q_simd<QT>(q, i);
-}
-
 template <int QT>
 __global__ void prepare_queries_kernel(const void* __restrict__ queries, uint32_t nq, uint32_t dim, uint32_t qstride,
                                        int mode, int metric, int code_type, float scale, float bias,

@@ -10,9 +10,14 @@ Scalar-quantised rows (the reference's ``StorageKind::SQI8`` and its uint8 twin)
     codes, scale, bias = sq_compress(data)             # int8 codes, one global scale and bias
     index = IVF.assemble_from_clustering(clustering, codes, DistanceType.L2, sq=(scale, bias))
 
-Backed by ``svsb200_ivf_*`` of ``libsvsb200.so``.  The k-means is the reference's flat k-means made deterministic (an own
-documented random sequence, float32 sums in row order), so ``is_hierarchical`` defaults to False here and True is
-refused.  A search returns the exact top k over the probed clusters, bit for bit the distances of the exact scan.
+The reference's default, hierarchical k-means, is a method of its own here (``is_hierarchical`` is not read by it):
+
+    clustering = Clustering.build_hierarchical(IVFBuildParameters(num_centroids=16384), data, DistanceType.L2)
+
+Backed by ``svsb200_ivf_*`` of ``libsvsb200.so``.  Both k-means are the reference's made deterministic (an own
+documented random sequence, float32 sums in row order).  ``Clustering.build`` is the flat k-means, so
+``is_hierarchical`` defaults to False here and True is refused by it.  A search returns the exact top k over the probed
+clusters, bit for bit the distances of the exact scan.
 """
 from __future__ import annotations
 
@@ -72,13 +77,15 @@ def _index_rows(data, sq) -> np.ndarray:
 
 
 class Clustering:
-    """``svs.Clustering``: centroids float32 [C, dim] and one cluster per data row (uint32 [n])."""
+    """``svs.Clustering``: centroids float32 [C, dim] and one cluster per data row (uint32 [n]); a hierarchical one also
+    the level-2 centroids of every level-1 group (uint32 [L1], ``level2_counts``, else None)."""
 
-    def __init__(self, centroids, assignments=None):
+    def __init__(self, centroids, assignments=None, level2_counts=None):
         self.centroids = np.ascontiguousarray(centroids, dtype=np.float32)
         if self.centroids.ndim != 2:
             raise ValueError("centroids must be [C, dim]")
         self.assignments = None if assignments is None else np.ascontiguousarray(assignments, dtype=np.uint32)
+        self.level2_counts = level2_counts
 
     @property
     def num_clusters(self) -> int:
@@ -98,6 +105,28 @@ class Clustering:
             int(bp.minibatch_size), int(bp.num_iterations), int(bool(bp.is_hierarchical)), float(bp.training_fraction),
             int(bp.seed), int(device), centroids.ctypes.data, assignments.ctypes.data))
         return Clustering(centroids, assignments)
+
+    @staticmethod
+    def build_hierarchical(build_parameters: IVFBuildParameters, data, distance: DistanceType = DistanceType.L2,
+                           device: int = 0) -> "Clustering":
+        """``hierarchical_kmeans_clustering`` on the GPU (``svsb200_ivf_cluster_hierarchical``): a flat k-means of
+        ``hierarchical_level1_clusters`` centroids (0: sqrt(num_centroids)), then a k-means inside every level-1 group
+        with centroids in proportion to its training rows, all groups trained together.  A row's cluster is the nearest
+        centroid of its own level-1 group.  ``is_hierarchical`` is not read.  The level-2 centroids per level-1 group
+        are kept as ``level2_counts``."""
+        x = _lib._rows(data)
+        bp = build_parameters
+        n, dim = x.shape
+        C = int(bp.num_centroids)
+        centroids = np.empty((C, dim), dtype=np.float32)
+        assignments = np.empty(n, dtype=np.uint32)
+        counts = np.zeros(int(bp.hierarchical_level1_clusters) or int(np.sqrt(float(C))), dtype=np.uint32)
+        _lib.check(_lib.lib().svsb200_ivf_cluster_hierarchical(
+            x.ctypes.data, _DTYPE_CODE[x.dtype], n, dim, int(DistanceType(distance)), C,
+            int(bp.hierarchical_level1_clusters), int(bp.minibatch_size), int(bp.num_iterations),
+            float(bp.training_fraction), int(bp.seed), int(device), centroids.ctypes.data, assignments.ctypes.data,
+            counts.ctypes.data))
+        return Clustering(centroids, assignments, level2_counts=counts)
 
 
 class _IVFSearch(_lib._Handle):
