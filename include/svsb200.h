@@ -230,7 +230,13 @@ int svsb200_merge_topk_device(
  *                 row stride = svsb200_lvq8_row_stride(dim) (a multiple of 32 bytes);
  *   compress    : encodes n float32 vectors against `mean[dim]` on the GPU into `out_rows`
  *                 (host buffers); pass the same `mean` as `aux` to svsb200_index_create with
- *                 storage = SVSB200_LVQ8, dtype = SVSB200_U8, row_stride_bytes = the stride. */
+ *                 storage = SVSB200_LVQ8, dtype = SVSB200_U8, row_stride_bytes = the stride.
+ *                 It fails, naming the first offending row and writing nothing, when a residual x_i - mean_i is
+ *                 not finite (a NaN or infinite input) or a row's delta or lower bound is not finite in float16
+ *                 (a residual range of 255 x 65520 or more, or a lower bound at or below -65520): such a row
+ *                 would decode to NaN or -inf.  A subnormal or zero float16 delta is finite and accepted; every
+ *                 element then still decodes within 0.5 delta16 + |lower - lower16| + 255 |delta - delta16| of
+ *                 its residual, plus fp32 rounding (DESIGN.md §12). */
 size_t svsb200_lvq8_row_stride(size_t dim);
 int svsb200_lvq8_compress(const float* data, size_t n, size_t dim, const float* mean, void* out_rows,
                           int device);

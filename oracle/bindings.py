@@ -219,15 +219,42 @@ class OracleLib(_Base):
     prefix = "oracle"
     path = os.path.join(HERE, "liboracle.so")
 
+    def sq_distance_rows(self, metric: str, query: np.ndarray, codes: np.ndarray, scale: float,
+                         bias: float) -> np.ndarray:
+        """:meth:`distance_rows` over SQ int8 / uint8 codes, as the SQ index search computes them."""
+        q, r = _c(query), _c(codes)
+        out = np.empty(r.shape[0], dtype=np.float32)
+        fn = self.lib.oracle_sq_distance_rows
+        fn.argtypes = [C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_size_t,
+                       C.c_size_t, C.c_void_p]
+        if fn(METRIC_CODES[metric], _code(q), _code(r), float(scale), float(bias), _ptr(q), _ptr(r),
+              C.c_size_t(r.shape[0]), C.c_size_t(r.shape[1]), _ptr(out)):
+            raise RuntimeError(self._err())
+        return out
+
     # ---- LVQ-8 (own specification; parity with Intel's closed LVQ is unpinned) ----
+    def lvq8_distance_rows(self, metric: str, query: np.ndarray, rows: np.ndarray, dim: int,
+                           mean: np.ndarray) -> np.ndarray:
+        """:meth:`distance_rows` over LVQ-8 rows (from :meth:`lvq8_compress`), as the LVQ-8 index search computes them."""
+        q, r, m = _c(query), _c(rows), _c(mean.astype(np.float32, copy=False))
+        out = np.empty(r.shape[0], dtype=np.float32)
+        fn = self.lib.oracle_lvq8_distance_rows
+        fn.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p]
+        if fn(METRIC_CODES[metric], _code(q), _ptr(q), _ptr(r), C.c_size_t(r.shape[0]), C.c_size_t(dim), _ptr(m),
+              _ptr(out)):
+            raise RuntimeError(self._err())
+        return out
+
     def lvq8_compress(self, data: np.ndarray, mean: np.ndarray) -> np.ndarray:
+        """Raises RuntimeError, naming the first offending row, where a residual or a float16 constant is not finite."""
         d, m = _c(data.astype(np.float32, copy=False)), _c(mean.astype(np.float32, copy=False))
         self.lib.oracle_lvq8_row_stride.restype = C.c_size_t
         self.lib.oracle_lvq8_row_stride.argtypes = [C.c_size_t]
         stride = self.lib.oracle_lvq8_row_stride(d.shape[1])
         rows = np.zeros((d.shape[0], stride), dtype=np.uint8)
         self.lib.oracle_lvq8_compress.argtypes = [C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p]
-        self.lib.oracle_lvq8_compress(_ptr(d), d.shape[0], d.shape[1], _ptr(m), _ptr(rows))
+        if self.lib.oracle_lvq8_compress(_ptr(d), d.shape[0], d.shape[1], _ptr(m), _ptr(rows)):
+            raise RuntimeError(self._err())
         return rows
 
     def lvq8_index(self, rows: np.ndarray, dim: int, mean: np.ndarray, graph: np.ndarray, entry_point: int,

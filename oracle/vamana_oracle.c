@@ -353,6 +353,34 @@ int oracle_distance_rows(int metric, int qtype, int dtype, const void* query, co
     return 0;
 }
 
+int oracle_sq_distance_rows(int metric, int qtype, int code_type, float scale, float bias, const void* query,
+                            const void* codes, size_t nrows, size_t dim, float* out) {
+    if (qtype != ORACLE_F32 && qtype != ORACLE_F16) FAIL("SQ: float32 / float16 queries only, got %d", qtype);
+    if (code_type != ORACLE_I8 && code_type != ORACLE_U8) FAIL("bad SQ code type %d", code_type);
+    FixedQuery f;
+    if (fixed_query_init(&f, metric, qtype, code_type, 1, dim, scale, bias)) FAIL("out of memory");
+    fix_argument(&f, query);
+    for (size_t i = 0; i < nrows; ++i) out[i] = compute_distance(&f, (const char*)codes + i * dim);
+    fixed_query_free(&f);
+    return 0;
+}
+
+int oracle_lvq8_distance_rows(int metric, int qtype, const void* query, const void* rows, size_t nrows, size_t dim,
+                              const float* mean, float* out) {
+    if (qtype != ORACLE_F32 && qtype != ORACLE_F16) FAIL("LVQ-8: float32 / float16 queries only, got %d", qtype);
+    if (metric == ORACLE_COS) FAIL("LVQ-8: cosine is not supported");
+    FixedQuery f;
+    if (fixed_query_init(&f, metric, qtype, ORACLE_U8, 0, dim, 0, 0)) FAIL("out of memory");
+    f.lvq = 1;
+    f.mean = mean;
+    f.lvq_const_offset = (dim + 3) / 4 * 4;
+    fix_argument(&f, query);
+    size_t stride = oracle_lvq8_row_stride(dim);
+    for (size_t i = 0; i < nrows; ++i) out[i] = compute_distance(&f, (const char*)rows + i * stride);
+    fixed_query_free(&f);
+    return 0;
+}
+
 /* ------------------------------------------------------------------------------------
  * SearchBuffer (index/vamana/search_buffer.h:104-497).
  * ---------------------------------------------------------------------------------- */
@@ -557,11 +585,27 @@ void* oracle_sq_index_create(int code_type, const float* data, size_t n, size_t 
  *   {delta, lower} stored as IEEE float16 (RNE); codes against the stored constants:
  *   c_i = clamp(rint((r_i - lower16) / delta16), 0, 255), 0 when delta16 == 0.
  *   Row = dim codes, padded to 4 bytes, then delta16, lower16; stride multiple of 32.
+ * A row with a residual that is not finite, or whose delta16 or lower16 is not finite (the range
+ * reaches 255 x 65520 or lower reaches -65520), is refused: it would decode to NaN or -inf.  A
+ * subnormal or zero delta16 is kept.  Nothing is written when a row is refused.
  * ---------------------------------------------------------------------------------- */
 size_t oracle_lvq8_row_stride(size_t dim) { return ((((dim + 3) / 4 * 4) + 4) + 31) / 32 * 32; }
 
 int oracle_lvq8_compress(const float* data, size_t n, size_t dim, const float* mean, void* out_rows) {
     size_t stride = oracle_lvq8_row_stride(dim), off = (dim + 3) / 4 * 4;
+    for (size_t r = 0; r < n; ++r) {
+        const float* x = data + r * dim;
+        float lo = INFINITY, hi = -INFINITY;
+        for (size_t i = 0; i < dim; ++i) {
+            float v = x[i] - mean[i];
+            if (!isfinite(v)) FAIL("LVQ-8: row %zu holds an element that is not finite after removing the mean", r);
+            lo = v < lo ? v : lo;
+            hi = v > hi ? v : hi;
+        }
+        _Float16 consts[2] = {(_Float16)((hi - lo) / 255.0f), (_Float16)lo};
+        if (!isfinite((float)consts[0]) || !isfinite((float)consts[1]))
+            FAIL("LVQ-8: row %zu has a delta or lower bound that float16 cannot hold", r);
+    }
     for (size_t r = 0; r < n; ++r) {
         const float* x = data + r * dim;
         uint8_t* out = (uint8_t*)out_rows + r * stride;

@@ -23,6 +23,13 @@ const char* oracle_last_error(void);
 /* distance::compute(f, query, row) for every row, after one maybe_fix_argument(query). */
 int oracle_distance_rows(int metric, int qtype, int dtype, const void* query, const void* rows,
                          size_t nrows, size_t dim, float* out);
+/* The same over compressed rows, through the code the SQ and LVQ-8 index searches use:
+ * SQ int8 / uint8 codes (dense, dim bytes each) with their scale and bias, and LVQ-8 rows
+ * (svsb200_lvq8_row_stride apart) with the dataset mean.  Queries are float32 or float16. */
+int oracle_sq_distance_rows(int metric, int qtype, int code_type, float scale, float bias, const void* query,
+                            const void* codes, size_t nrows, size_t dim, float* out);
+int oracle_lvq8_distance_rows(int metric, int qtype, const void* query, const void* rows, size_t nrows, size_t dim,
+                              const float* mean, float* out);
 
 /* graph_rows: uint32[n][max_degree+1], out-degree in element 0 (reference in-memory layout). */
 void* oracle_index_create(int dtype, const void* data, size_t n, size_t dim,
@@ -35,6 +42,7 @@ void* oracle_sq_index_create(int code_type, const float* data, size_t n, size_t 
                              void* codes_out);
 /* LVQ-8 (own specification; the reference's LVQ is closed source, parity unpinned). */
 size_t oracle_lvq8_row_stride(size_t dim);
+/* Fails, naming the first offending row, on a non-finite residual or float16 constant. */
 int oracle_lvq8_compress(const float* data, size_t n, size_t dim, const float* mean, void* out_rows);
 void* oracle_lvq8_index_create(const void* rows, size_t n, size_t dim, const float* mean,
                                const uint32_t* graph_rows, size_t max_degree, uint32_t entry_point, int metric);

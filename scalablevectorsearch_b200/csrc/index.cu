@@ -82,17 +82,21 @@ __global__ void repack_graph_kernel(const uint32_t* __restrict__ src, size_t row
 //   {delta, lower} are stored as float16 (round to nearest even) and the codes are computed against
 //   the *stored* constants:  c_i = clamp(rint((r_i - lower16) / delta16), 0, 255)   (0 when delta16 == 0)
 // so that decode y_i = fma(delta16, c_i, lower16) is the nearest representable grid point.
+// A row with a residual that is not finite, or whose delta16 or lower16 is not finite, would decode to NaN or -inf: its
+// index is recorded in *bad_row (atomicMin, so the host sees the first such row) and the host refuses the data.
 __global__ void lvq8_compress_kernel(const float* __restrict__ data, uint32_t n, uint32_t dim,
                                      const float* __restrict__ mean, uint8_t* __restrict__ rows, uint32_t stride,
-                                     uint32_t const_offset) {
+                                     uint32_t const_offset, uint32_t* __restrict__ bad_row) {
     const uint32_t row = blockIdx.x * (blockDim.x / 32) + threadIdx.x / 32;
     const int lane = threadIdx.x & 31;
     if (row >= n) return;
     const float* x = data + size_t(row) * dim;
     uint8_t* out = rows + size_t(row) * stride;
     float lo = INFINITY, hi = -INFINITY;
+    bool finite = true;
     for (uint32_t i = lane; i < dim; i += 32) {
         const float r = __fsub_rn(x[i], mean[i]);
+        finite &= isfinite(r);
         lo = fminf(lo, r);
         hi = fmaxf(hi, r);
     }
@@ -103,6 +107,10 @@ __global__ void lvq8_compress_kernel(const float* __restrict__ data, uint32_t n,
     const __half dh = __float2half_rn(__fdiv_rn(__fsub_rn(hi, lo), 255.0f));
     const __half lh = __float2half_rn(lo);
     const float d = __half2float(dh), l = __half2float(lh);
+    if (!__all_sync(0xFFFFFFFFu, finite) || !isfinite(d) || !isfinite(l)) {
+        if (lane == 0) atomicMin(bad_row, row);
+        return;
+    }
     for (uint32_t i = lane; i < stride; i += 32) {
         uint8_t c = 0;
         if (i < dim && d > 0.0f) {
@@ -646,17 +654,25 @@ int svsb200_lvq8_compress(const float* data, size_t n, size_t dim, const float* 
     const size_t stride = svsb200_lvq8_row_stride(dim);
     DeviceBuffer<float> d_data, d_mean;
     DeviceBuffer<uint8_t> d_rows;
+    DeviceBuffer<uint32_t> d_bad;
     CUDA_TRY(d_data.ensure(n * dim));
     CUDA_TRY(d_mean.ensure(dim));
     CUDA_TRY(d_rows.ensure(n * stride));
+    CUDA_TRY(d_bad.ensure(1));
     CUDA_TRY(cudaMemcpy(d_data.ptr, data, n * dim * sizeof(float), cudaMemcpyHostToDevice));
     CUDA_TRY(cudaMemcpy(d_mean.ptr, mean, dim * sizeof(float), cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemset(d_bad.ptr, 0xFF, sizeof(uint32_t)));
     const int warps = 8;
     lvq8_compress_kernel<<<unsigned((n + warps - 1) / warps), warps * 32>>>(d_data.ptr, uint32_t(n), uint32_t(dim), d_mean.ptr,
                                                                           d_rows.ptr, uint32_t(stride),
-                                                                          uint32_t(round_up(dim, 4)));
+                                                                          uint32_t(round_up(dim, 4)), d_bad.ptr);
     count_launch();
     CUDA_TRY(cudaGetLastError());
+    uint32_t bad = 0;
+    CUDA_TRY(cudaMemcpy(&bad, d_bad.ptr, sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    if (bad != 0xFFFFFFFFu)
+        return fail("svsb200_lvq8_compress: row " + std::to_string(bad) +
+                    " holds a value that is not finite, or a delta or lower bound that float16 cannot hold");
     CUDA_TRY(cudaMemcpy(out_rows, d_rows.ptr, n * stride, cudaMemcpyDeviceToHost));
     return 0;
 }

@@ -119,7 +119,8 @@ def _read_entry_point(config_path: str) -> int:
 def lvq8_compress(data: np.ndarray, mean: np.ndarray | None = None, device: int = 0):
     """LVQ-8 encode float32 vectors on the GPU (own specification, DESIGN.md §10; stands where the
     reference's closed ``LVQDataset<8>::compress(data, threadpool, padding)`` would).
-    Returns ``(rows uint8 [n, stride], mean float32 [dim])``."""
+    Returns ``(rows uint8 [n, stride], mean float32 [dim])``.  Raises :class:`Svsb200Error`, naming the first offending
+    row, when a value minus the mean is not finite or a row's delta or lower bound does not fit in float16."""
     data = np.ascontiguousarray(data, dtype=np.float32)
     if mean is None:
         mean = data.mean(axis=0, dtype=np.float64).astype(np.float32)

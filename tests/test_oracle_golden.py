@@ -124,3 +124,79 @@ def test_oracle_lvq8_codec_roundtrip(oracle):
     assert np.all(np.abs(dec - x) <= 0.5 * step + 1e-5)
     assert np.all(rows[5, :100] == 0) and float(delta[5, 0]) == 0.0
     assert np.all(rows[:, 104:] == 0)
+
+
+def _complete_graph(n):
+    graph = np.zeros((n, n), dtype=np.uint32)
+    graph[:, 0] = n - 1
+    for i in range(n):
+        graph[i, 1:] = [j for j in range(n) if j != i]
+    return graph
+
+
+def _assert_search_is_sorted_distances(index, q, d, metric, tag):
+    """window = capacity = n on a complete graph: the search returns every row, ordered by the comparator, with the
+    distances the search computes -- which must be `d`'s bits."""
+    n = len(d)
+    ids, dists = index.search(q[None, :], n, n, n)
+    ids, dists = ids[0].astype(np.int64), dists[0]
+    assert np.array_equal(np.sort(ids), np.arange(n)), tag
+    assert np.array_equal(bits(dists), bits(d[ids])), tag
+    want = np.sort(d) if metric == "l2" else -np.sort(-d)
+    assert np.array_equal(bits(dists), bits(want)), tag
+
+
+@pytest.mark.parametrize("metric", ["l2", "ip", "cosine"])
+@pytest.mark.parametrize("code", [np.int8, np.uint8])
+@pytest.mark.parametrize("dim", [3, 100])
+def test_oracle_sq_distance_rows_match_its_pinned_search(oracle, metric, code, dim):
+    """oracle_sq_distance_rows is the SQ search's distance: every distance the pinned SQ index search returns over a
+    complete graph."""
+    rng = np.random.default_rng(dim)
+    n = 60
+    x = (rng.standard_normal((n, dim)) * 2 + 0.3).astype(np.float32)
+    graph = _complete_graph(n)
+    index, codes, scale, bias = oracle.sq_index(x, graph, 0, metric, code)
+    for qt in (np.float32, np.float16):
+        for q in (rng.standard_normal((4, dim)) * 2 + 0.3).astype(qt):
+            d = oracle.sq_distance_rows(metric, q, codes, scale, bias)
+            _assert_search_is_sorted_distances(index, q, d, metric, f"sq {np.dtype(code).name} {metric} {np.dtype(qt).name}")
+
+
+@pytest.mark.parametrize("metric", ["l2", "ip"])
+@pytest.mark.parametrize("dim", [5, 96, 100])
+def test_oracle_lvq8_distance_rows_match_its_search(oracle, metric, dim):
+    """oracle_lvq8_distance_rows is the LVQ-8 search's distance, over a complete graph."""
+    rng = np.random.default_rng(dim + 1)
+    n = 60
+    x = (rng.standard_normal((n, dim)) * 0.5 + 1.0).astype(np.float32)
+    mean = x.mean(axis=0, dtype=np.float64).astype(np.float32)
+    rows = oracle.lvq8_compress(x, mean)
+    index = oracle.lvq8_index(rows, dim, mean, _complete_graph(n), 0, metric)
+    for qt in (np.float32, np.float16):
+        for q in (rng.standard_normal((4, dim)) + 1.0).astype(qt):
+            d = oracle.lvq8_distance_rows(metric, q, rows, dim, mean)
+            _assert_search_is_sorted_distances(index, q, d, metric, f"lvq8 {metric} {np.dtype(qt).name}")
+    with pytest.raises(RuntimeError):
+        oracle.lvq8_distance_rows("cosine", x[0], rows, dim, mean)
+
+
+def test_oracle_lvq8_refuses_what_float16_cannot_hold(oracle):
+    """A residual that is not finite, a delta of 65520 or more or a lower bound at or below -65520 would decode to NaN
+    or -inf: the encoder refuses the data, naming the first such row.  65504 - epsilon and subnormal deltas encode."""
+    mean = np.zeros(8, np.float32)
+    good = np.linspace(-1, 1, 32, dtype=np.float32).reshape(4, 8)
+    for tag, row in (("NaN", [np.nan] + [0.0] * 7), ("+inf", [np.inf] + [0.0] * 7), ("-inf", [0.0] * 7 + [-np.inf]),
+                     ("delta16 overflow", [0.0] * 7 + [255 * 65520.0]), ("lower16 overflow", [-65520.0] + [0.0] * 7)):
+        x = good.copy()
+        x[1] = row
+        x[3] = row
+        with pytest.raises(RuntimeError, match="row 1 "):
+            oracle.lvq8_compress(x, mean)
+    x = good.copy()
+    x[1] = [-65503.0] + [0.0] * 7
+    x[2] = [0.0] * 7 + [255 * 65504.0 * (1 - 2.0 ** -12)]
+    x[3] = np.linspace(0, 255 * 2.0 ** -20, 8, dtype=np.float32)    # delta16 in float16's subnormals
+    rows = oracle.lvq8_compress(x, mean)
+    consts = rows[:, 8:12].copy().view(np.float16).astype(np.float32)
+    assert np.all(np.isfinite(consts)) and consts[3, 0] == np.float32(2.0 ** -20)
