@@ -383,7 +383,8 @@ enum { SVSB200_FLAT_ROUTE_DENSE = 0, SVSB200_FLAT_ROUTE_SPARSE = 1 };
 int svsb200_flat_filter_plan(size_t n, size_t allowed, int* route);
 
 /* Dynamic index.  Replaces: MutableVamanaIndex(graph, data, entry_point, distance, external_ids, threadpool)
- * (include/svs/index/vamana/dynamic_index.h:178-202) for float32 / float16 plain storage on one device, adjacency rows
+ * (include/svs/index/vamana/dynamic_index.h:178-202) for float32 / float16 plain storage (SQ codes:
+ * svsb200_dynamic_create_sq) on one device, adjacency rows
  * of at most 128 neighbours, L2 / MIP / cosine.  Arguments as svsb200_index_create (dense rows), plus one distinct
  * external id per row; every slot starts Valid.  The result is an ordinary index handle:
  *   * svsb200_search / _cancellable / _device run MutableVamanaIndex::search (dynamic_index.h:482-571): the walk goes
@@ -450,6 +451,30 @@ int svsb200_dynamic_compact(svsb200_index* index);
 int svsb200_dynamic_build(const void* vectors, int dtype, size_t n, size_t dim, int metric, float alpha,
                           size_t graph_max_degree, size_t window_size, size_t max_candidates, size_t prune_to,
                           const uint64_t* external_ids, int device, svsb200_index** out);
+/* Dynamic index over scalar-quantised codes.  Replaces: MutableVamanaIndex over SQDataset<int8_t / uint8_t> (the
+ * runtime's DynamicVamanaIndex with StorageKind::SQI8 and its uint8 twin): n x dim int8 / uint8 codes (`code_type`,
+ * HOST, dense; svsb200_sq_compress writes them) with the `scale` (finite, positive) and `bias` (finite) they were
+ * compressed with, which stay fixed for the life of the index.  Arguments otherwise as svsb200_dynamic_create (one
+ * distinct external id per row, every slot Valid, n = 0 refused), and the result is an index handle with storage
+ * SVSB200_SQ on which every svsb200_dynamic_* call and search works as on a float index, with these differences:
+ *   * searches take float32 / float16 queries and measure with the SQ search's distances (svsb200_build_vamana_sq);
+ *   * svsb200_dynamic_add takes float32 rows only (float16 and integer rows, and rows holding a NaN or an infinity, are
+ *     refused before anything changes) and encodes them on the device as SQDataset::set_datum does (quantization/
+ *     scalar/scalar.h:417-429): clamp(roundf((x - bias) / scale), MIN, MAX), so values outside the compressed range
+ *     clamp; the codes are then linked in with the SQ builder's distances;
+ *   * svsb200_dynamic_consolidate measures candidates with the build adaptor's general distance over SQ data
+ *     (consolidate.h:241-244): the node decompressed and prepared as an SQ query, the SQ search's operators; a
+ *     Deleted entry point is replaced by the medoid of the Valid codes as integers;
+ *   * the rows take dim bytes of device memory (rounded up to 16) instead of 4 x dim or 2 x dim. */
+int svsb200_dynamic_create_sq(const void* codes, int code_type, size_t n, size_t dim, float scale, float bias,
+                              const uint32_t* graph_rows, size_t graph_row_len, uint32_t entry_point, int metric,
+                              const uint64_t* external_ids, int device, svsb200_index** out);
+/* MutableVamanaIndex(parameters, SQ data, external_ids, distance): svsb200_build_vamana_sq, then
+ * svsb200_dynamic_create_sq; the build parameters become the mutation parameters, as in svsb200_dynamic_build.  The
+ * code type, scale, bias and ids are checked before the build runs. */
+int svsb200_dynamic_build_sq(const void* codes, int code_type, size_t n, size_t dim, int metric, float scale, float bias,
+                             float alpha, size_t graph_max_degree, size_t window_size, size_t max_candidates,
+                             size_t prune_to, const uint64_t* external_ids, int device, svsb200_index** out);
 
 /* Dynamic flat index.  Replaces: DynamicFlatIndex (include/svs/index/flat/dynamic_flat.h:65) with svs::DynamicFlat
  * (orchestrators/dynamic_flat.h): an exact index over a mutable set of float32 / float16 / int8 / uint8 rows on one

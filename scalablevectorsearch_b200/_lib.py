@@ -53,6 +53,8 @@ ABI = {
     "svsb200_build_vamana_sq": (i32, [vp, i32, sz, sz, i32, f32, f32, f32, sz, sz, sz, sz, i32, vp, P(u32)]),
     "svsb200_dynamic_create": (i32, [vp, i32, sz, sz, vp, sz, u32, i32, vp, i32, P(vp)]),
     "svsb200_dynamic_build": (i32, [vp, i32, sz, sz, i32, f32, sz, sz, sz, sz, vp, i32, P(vp)]),
+    "svsb200_dynamic_create_sq": (i32, [vp, i32, sz, sz, f32, f32, vp, sz, u32, i32, vp, i32, P(vp)]),
+    "svsb200_dynamic_build_sq": (i32, [vp, i32, sz, sz, i32, f32, f32, f32, sz, sz, sz, sz, vp, i32, P(vp)]),
     "svsb200_dynamic_add": (i32, [vp, vp, i32, sz, vp, i32, vp]), "svsb200_dynamic_delete": (i32, [vp, vp, sz]),
     "svsb200_dynamic_ids": (i32, [vp, vp, P(sz)]), "svsb200_dynamic_has_id": (i32, [vp, u64, P(i32)]),
     "svsb200_dynamic_export": (i32, [vp, vp, vp, vp, P(u32)]),

@@ -538,11 +538,13 @@ __global__ void __launch_bounds__(32, SQ ? kSqBuildMinBlocks : 16) build_prune_k
 // repeats, then by TotalOrder (key, id) -- the reference sorts by distance alone, so its order among exactly equal
 // distances is unspecified -- and the best max_candidates go to hist[w] for build_prune_kernel (PRUNE_CONSOLIDATE).
 // The node itself stays in the pool when a deleted neighbour links back to it, as in the reference; the prune skips
-// it.  The kernel reads the node's own row and the rows of slots that are not Valid only.
-template <int ROWT, int OP, int DS, int KS>
-__global__ void __launch_bounds__(32, 16) consolidate_pool_kernel(const __grid_constant__ SearchParams p,
+// it.  The kernel reads the node's own row and the rows of slots that are not Valid only.  Over SQ codes (SQ = true) the
+// node is staged as the SQ build stages a datum (stage_sq_datum) and the candidates are measured with the SQ search's
+// operators: the general distance of the reference's build adaptor (consolidate.h:241-244).
+template <int ROWT, int OP, int DS, int KS, bool SQ = false>
+__global__ void __launch_bounds__(32, SQ && OP < OP_L2I ? kSqBuildMinBlocks : 16) consolidate_pool_kernel(const __grid_constant__ SearchParams p,
                                                                  const __grid_constant__ BuildParams bp) {
-    constexpr int G = KS * 16 / Row<ROWT>::LPT;
+    constexpr int G = OP >= OP_L2I ? 4 : KS * 16 / Row<ROWT>::LPT;   // threads per row, as in eval_pass
     constexpr int GROUPS = 32 / G;
     constexpr unsigned FULL = 0xFFFFFFFFu;
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -603,7 +605,7 @@ __global__ void __launch_bounds__(32, 16) consolidate_pool_kernel(const __grid_c
         __syncwarp();
         // ---- filter_candidates: distances from the node, TotalOrder ----
         float qaux1 = 0.f;
-        const float qnorm = stage_row<ROWT, OP>(p, node, q_s, lane, qaux1);
+        const float qnorm = stage_row<ROWT, OP, SQ>(p, node, q_s, lane, qaux1);
         __syncwarp();
         for (uint32_t base = 0; base < U; base += 2 * GROUPS)
             eval_pass<ROWT, OP, DS, 2, KS, true>(p, q_s, vectors, sid, skey, base, U, g, t, qnorm, qaux1, ksign);
@@ -618,7 +620,7 @@ __global__ void __launch_bounds__(32, 16) consolidate_pool_kernel(const __grid_c
 }
 
 // The builder's launchers, instantiated once per row type in build_<type>.cu.  Its lean search (HIST) and prune take
-// BuildOps; consolidation's candidate pools are for DynamicRows only.  The prune and the pool run on the caller's grid:
+// BuildOps; consolidation's candidate pools are for DynamicRows (and over SQ codes DynamicSqRows, build_sq_<type>.cu).  The prune and the pool run on the caller's grid:
 // `grid` warps, for the pool each with its own scratch slice (bp.scratch_len entries).
 template <int ROWT> cudaError_t launch_build_search(int op, const SearchParams& p, const LaunchConfig& cfg) {
     return dispatch(BuildOps<ROWT>{}, op, [&](auto o) { return launch_fast<ROWT, decltype(o)::value, true, false>(p, cfg); });
@@ -691,6 +693,17 @@ cudaError_t launch_consolidate_pool_op(int op, const SearchParams& p, const Buil
         });
     });
 }
+template <int ROWT>
+cudaError_t launch_consolidate_pool_sq(int op, const SearchParams& p, const BuildParams& bp, int grid, cudaStream_t stream) {
+    const LaunchConfig cfg{grid, 1, size_t(p.qstride) * 4, stream};
+    return dispatch(DynamicSqOps{}, op, [&](auto o) {
+        constexpr int OP = decltype(o)::value;
+        return with_shape<OP, false>(p.dim, true, [&](auto ds, auto ks) {
+            return launch_kernel(consolidate_pool_kernel<ROWT, OP, decltype(ds)::value, decltype(ks)::value, true>, cfg, grid,
+                                 false, p, bp);
+        });
+    });
+}
 
 extern template cudaError_t launch_build_search<SVSB200_F32>(int, const SearchParams&, const LaunchConfig&);
 extern template cudaError_t launch_build_search<SVSB200_F16>(int, const SearchParams&, const LaunchConfig&);
@@ -710,5 +723,7 @@ extern template cudaError_t launch_build_batch_sq<SVSB200_U8>(int, const SearchP
                                                              float*, uint8_t*, float*, cudaStream_t);
 extern template cudaError_t launch_consolidate_pool_op<SVSB200_F32>(int, const SearchParams&, const BuildParams&, int, cudaStream_t);
 extern template cudaError_t launch_consolidate_pool_op<SVSB200_F16>(int, const SearchParams&, const BuildParams&, int, cudaStream_t);
+extern template cudaError_t launch_consolidate_pool_sq<SVSB200_I8>(int, const SearchParams&, const BuildParams&, int, cudaStream_t);
+extern template cudaError_t launch_consolidate_pool_sq<SVSB200_U8>(int, const SearchParams&, const BuildParams&, int, cudaStream_t);
 
 }  // namespace svsb200

@@ -1,4 +1,5 @@
-// build_sq_u8.cu -- graph-builder kernel instantiations for SQ uint8 codes: the SQ search's operators (BuildSqOps).
+// build_sq_u8.cu -- graph-builder kernel instantiations for SQ uint8 codes: the SQ search's operators (BuildSqOps), and
+// consolidation's candidate pools of a dynamic index over such codes.
 #include "build_kernels.cuh"
 
 namespace svsb200 {
@@ -7,5 +8,6 @@ template cudaError_t launch_build_search_sq<SVSB200_U8>(int, const SearchParams&
 template cudaError_t launch_build_prune_sq<SVSB200_U8>(int, const SearchParams&, const BuildParams&, int, cudaStream_t);
 template cudaError_t launch_build_batch_sq<SVSB200_U8>(int, const SearchParams&, uint32_t, uint32_t, const uint32_t*, float*,
                                                         uint8_t*, float*, cudaStream_t);
+template cudaError_t launch_consolidate_pool_sq<SVSB200_U8>(int, const SearchParams&, const BuildParams&, int, cudaStream_t);
 
 }  // namespace svsb200

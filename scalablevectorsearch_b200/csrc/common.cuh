@@ -122,12 +122,14 @@ constexpr size_t kSmemOptInMax = 227 * 1024;   // dynamic shared memory a block 
 //   builder search (HIST), builder prune          DataRows    L2F IPF COSF   L2I IPI COSI      -
 //   the same over SQ codes (build_sq_<type>.cu)   BuildSqRows -              L2I IPF COSF      -
 //   consolidate pool, dynamic search (MUT)        DynamicRows L2F IPF COSF   -                 -
+//   the same over SQ codes (fast_dynamic_sq.cu)   DynamicSqRows -            L2I IPF COSF      -
 //   flat rescore                                  DataRows    L2F IPF        L2F IPF L2I IPI   -
 //   IVF leaf scan (ivf_kernel.cuh)                IvfRows     L2F IPF COSF   -                 -
 //   IVF leaf scan over SQ codes                   IvfSqRows   -              IPF COSF (+ the
 //                                                                            tensor-core L2 leaf)
 // int8 / uint8 rows take float and integer queries in a search; the builder's datum is its own query.  Over SQ codes
-// the builder's datum is decompressed and prepared as the SQ search's fp32 query, so it takes the SQ search's operators.
+// the builder's datum is decompressed and prepared as the SQ search's fp32 query, so it takes the SQ search's operators;
+// so does the dynamic index over SQ codes, in its search and in consolidation's candidate pools.
 template <int... V> struct IntList {};
 template <int ROWT> constexpr bool kIntRow = ROWT == SVSB200_I8 || ROWT == SVSB200_U8;
 using FloatOps = IntList<OP_L2F, OP_IPF, OP_COSF>;
@@ -144,6 +146,8 @@ template <int ROWT> using BuildOps = std::conditional_t<kIntRow<ROWT>, IntOps, F
 using BuildSqRows = IntList<SVSB200_I8, SVSB200_U8>;
 using BuildSqOps = IntList<OP_L2I, OP_IPF, OP_COSF>;
 using DynamicOps = FloatOps;
+using DynamicSqRows = IntList<SVSB200_I8, SVSB200_U8>;
+using DynamicSqOps = BuildSqOps;
 using IvfRows = IntList<SVSB200_F32, SVSB200_F16>;
 using IvfOps = FloatOps;
 using IvfSqRows = IntList<SVSB200_I8, SVSB200_U8>;
@@ -210,5 +214,7 @@ template <int ROWT> cudaError_t launch_search_exhaustive(int op, const SearchPar
 template <int ROWT> cudaError_t launch_search_fast(int op, const SearchParams& p, const LaunchConfig& cfg);
 // The lean kernel in its MutableBuffer mode (dynamic indexes, DynamicRows).
 template <int ROWT> cudaError_t launch_search_dynamic(int op, const SearchParams& p, const LaunchConfig& cfg);
+// The same over SQ codes (DynamicSqRows, DynamicSqOps).
+template <int ROWT> cudaError_t launch_search_dynamic_sq(int op, const SearchParams& p, const LaunchConfig& cfg);
 
 }  // namespace svsb200

@@ -5,8 +5,12 @@
 // Searches go through svsb200_search* and run the lean kernel's MutableBuffer form (search_fast.cuh, MUT = true);
 // insertion runs the graph builder over the new slots (build.cu), consolidation its prune kernel over pools selected by
 // consolidate_pool_kernel.
+// SQ storage (svsb200_dynamic_create_sq): the rows are int8 / uint8 codes under one scale and bias fixed at creation.
+// Searches, insertion and consolidation measure them with the SQ search's operators, as the SQ builder does (build.cu);
+// added float32 rows are encoded on the device (sq_encode) before they are placed; compact moves codes as it moves rows.
 #include "build_kernels.cuh"
 #include "host.cuh"
+#include "ivf.cuh"   // sq_check_params, sq_encode
 
 #include <algorithm>
 #include <cmath>
@@ -116,6 +120,9 @@ static GraphBuild graph_build(const svsb200_index* ix, Replica* rep, uint32_t* d
     b.max_candidates = ix->dyn_max_candidates;
     b.prune_to = ix->dyn_prune_to;
     b.alpha = ix->dyn_alpha;
+    b.sq = ix->storage == SVSB200_SQ;
+    b.scale = b.sq ? ix->scale : 1.f;
+    b.bias = b.sq ? ix->bias : 0.f;
     b.sm_count = rep->sm_count;
     b.stream = stream;
     return b;
@@ -125,24 +132,22 @@ static GraphBuild graph_build(const svsb200_index* ix, Replica* rep, uint32_t* d
 
 using namespace svsb200;
 
-extern "C" {
-
-int svsb200_dynamic_create(const void* vectors, int dtype, size_t n, size_t dim, const uint32_t* graph_rows,
-                           size_t graph_row_len, uint32_t entry_point, int metric, const uint64_t* external_ids, int device,
-                           svsb200_index** out) {
-    const char* who = "svsb200_dynamic_create";
-    if (!out) return fail("svsb200_dynamic_create: NULL output");
+// The body of svsb200_dynamic_create and svsb200_dynamic_create_sq, after their row checks: `storage` SVSB200_PLAIN, or
+// SVSB200_SQ with aux = {scale, bias}.  Errors read "<who>: ...".
+static int dynamic_create(const char* who, const void* vectors, int dtype, int storage, const float* aux, size_t n,
+                          size_t dim, const uint32_t* graph_rows, size_t graph_row_len, uint32_t entry_point, int metric,
+                          const uint64_t* external_ids, int device, svsb200_index** out) {
+    const std::string w(who);
+    if (!out) return fail(w + ": NULL output");
     *out = nullptr;
-    if (n && !external_ids) return fail("svsb200_dynamic_create: NULL external ids");
-    if (dtype != SVSB200_F32 && dtype != SVSB200_F16) return fail("svsb200_dynamic_create: float32 / float16 data only");
-    if (graph_row_len < 2 || graph_row_len - 1 > 32u * kFastMaxGW)
-        return fail("svsb200_dynamic_create: graph_max_degree must be in [1, 128]");
-    if (n >= (size_t(1) << 30)) return fail("svsb200_dynamic_create: at most 2^30 - 1 slots");
+    if (n && !external_ids) return fail(w + ": NULL external ids");
+    if (graph_row_len < 2 || graph_row_len - 1 > 32u * kFastMaxGW) return fail(w + ": graph_max_degree must be in [1, 128]");
+    if (n >= (size_t(1) << 30)) return fail(w + ": at most 2^30 - 1 slots");
     SlotTable slots;
     if (int rc = slots.assign(who, external_ids, n)) return rc;
     svsb200_index* ix = nullptr;
-    if (int rc = svsb200_index_create(vectors, dtype, n, dim, 0, graph_rows, graph_row_len, entry_point, metric, SVSB200_PLAIN,
-                                      nullptr, device, &ix))
+    if (int rc = svsb200_index_create(vectors, dtype, n, dim, 0, graph_rows, graph_row_len, entry_point, metric, storage, aux,
+                                      device, &ix))
         return rc;
     std::unique_ptr<svsb200_index, int (*)(svsb200_index*)> owner(ix, svsb200_index_destroy);
     ix->slots = std::move(slots);
@@ -156,6 +161,29 @@ int svsb200_dynamic_create(const void* vectors, int dtype, size_t n, size_t dim,
         return rc;
     *out = owner.release();
     return 0;
+}
+
+extern "C" {
+
+int svsb200_dynamic_create(const void* vectors, int dtype, size_t n, size_t dim, const uint32_t* graph_rows,
+                           size_t graph_row_len, uint32_t entry_point, int metric, const uint64_t* external_ids, int device,
+                           svsb200_index** out) {
+    if (out) *out = nullptr;
+    if (dtype != SVSB200_F32 && dtype != SVSB200_F16) return fail("svsb200_dynamic_create: float32 / float16 data only");
+    return dynamic_create("svsb200_dynamic_create", vectors, dtype, SVSB200_PLAIN, nullptr, n, dim, graph_rows, graph_row_len,
+                          entry_point, metric, external_ids, device, out);
+}
+
+int svsb200_dynamic_create_sq(const void* codes, int code_type, size_t n, size_t dim, float scale, float bias,
+                              const uint32_t* graph_rows, size_t graph_row_len, uint32_t entry_point, int metric,
+                              const uint64_t* external_ids, int device, svsb200_index** out) {
+    const char* who = "svsb200_dynamic_create_sq";
+    if (out) *out = nullptr;
+    if (code_type != SVSB200_I8 && code_type != SVSB200_U8) return fail("svsb200_dynamic_create_sq: codes must be int8 or uint8");
+    if (int rc = sq_check_params(who, scale, bias)) return rc;
+    const float aux[2] = {scale, bias};
+    return dynamic_create(who, codes, code_type, SVSB200_SQ, aux, n, dim, graph_rows, graph_row_len, entry_point, metric,
+                          external_ids, device, out);
 }
 
 int svsb200_dynamic_delete(svsb200_index* ix, const uint64_t* ids, size_t count) {
@@ -242,7 +270,16 @@ int svsb200_dynamic_add(svsb200_index* ix, const void* vectors, int dtype, size_
     if (int rc = check_dynamic(ix, who)) return rc;
     if (count == 0) return 0;
     if (!vectors || !ids) return fail("svsb200_dynamic_add: NULL argument");
-    if (dtype != ix->dtype) return fail("svsb200_dynamic_add: the points' dtype differs from the index's");
+    // an SQ index takes float32 rows and encodes them with its fixed scale and bias (SQDataset::set_datum)
+    const bool sq = ix->storage == SVSB200_SQ;
+    if (sq) {
+        if (dtype != SVSB200_F32) return fail("svsb200_dynamic_add: an SQ index takes float32 points");
+        const float* x = static_cast<const float*>(vectors);
+        for (size_t i = 0; i < count * ix->dim; ++i)
+            if (!std::isfinite(x[i])) return fail("svsb200_dynamic_add: the points hold a NaN or an infinity");
+    } else if (dtype != ix->dtype) {
+        return fail("svsb200_dynamic_add: the points' dtype differs from the index's");
+    }
     if (int rc = ix->slots.check_new(who, ids, count)) return rc;
     // slots (add_points, dynamic_index.h:670-706): Empty ones from first_empty_ (from 0 with reuse_empty), then appended
     std::vector<uint32_t> slots;
@@ -275,7 +312,21 @@ int svsb200_dynamic_add(svsb200_index* ix, const void* vectors, int dtype, size_
         CUDA_TRY(d_deg.ensure(new_n));
         CUDA_TRY(cudaMemsetAsync(st.rows.ptr, 0, count * ix->row_stride, stream));
         const size_t row_bytes = ix->dim * esize(ix->dtype);
-        CUDA_TRY(cudaMemcpy2DAsync(st.rows.ptr, ix->row_stride, vectors, row_bytes, row_bytes, count, cudaMemcpyHostToDevice, stream));
+        const void* from = vectors;   // the dense rows as stored, `row_bytes` apart
+        cudaMemcpyKind kind = cudaMemcpyHostToDevice;
+        DeviceBuffer<float> d_points;
+        DeviceBuffer<uint8_t> d_codes;
+        if (sq) {
+            const size_t values = count * ix->dim;
+            const unsigned grid = unsigned(std::min<size_t>((values + 255) / 256, size_t(rep->sm_count) * 8));
+            CUDA_TRY(d_points.ensure(values));
+            CUDA_TRY(d_codes.ensure(values));
+            CUDA_TRY(cudaMemcpyAsync(d_points.ptr, vectors, values * sizeof(float), cudaMemcpyHostToDevice, stream));
+            CUDA_TRY(sq_encode(d_points.ptr, values, ix->dtype, ix->scale, ix->bias, d_codes.ptr, grid, stream));
+            from = d_codes.ptr;
+            kind = cudaMemcpyDeviceToDevice;
+        }
+        CUDA_TRY(cudaMemcpy2DAsync(st.rows.ptr, ix->row_stride, from, row_bytes, row_bytes, count, kind, stream));
         CUDA_TRY(cudaMemcpyAsync(st.slots.ptr, slots.data(), count * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
         CUDA_TRY(cudaMemcpyAsync(st.ids.ptr, ids, count * sizeof(uint64_t), cudaMemcpyHostToDevice, stream));
         place_rows_kernel<<<unsigned((count + 7) / 8), 256, 0, stream>>>(
@@ -353,7 +404,10 @@ int svsb200_dynamic_consolidate(svsb200_index* ix) {
             p.row_stride = ix->row_stride;
             p.gstride = ix->gstride;
             p.greater = ix->metric != SVSB200_L2;
-            p.scale = 1.f;
+            p.sq = b.sq;
+            p.scale = b.scale;
+            p.bias = b.bias;
+            p.scale_sq = b.scale * b.scale;   // EuclideanCompressed ctor (scalar.h:68-72)
             p.qstride = query_stride(ix->dim);
             BuildParams bp{};
             bp.hist = d_hist.ptr;
@@ -372,20 +426,27 @@ int svsb200_dynamic_consolidate(svsb200_index* ix) {
             bp.scratch_ids = d_sid.ptr;
             bp.scratch_keys = d_skey.ptr;
             bp.scratch_len = scratch_len;
-            const int op = ix->metric == SVSB200_L2 ? OP_L2F : ix->metric == SVSB200_IP ? OP_IPF : OP_COSF;
+            // over SQ codes the build adaptor's general distance (consolidate.h:241-244): the SQ search's operators
+            const int op = ix->metric == SVSB200_L2 ? (b.sq ? OP_L2I : OP_L2F) : ix->metric == SVSB200_IP ? OP_IPF : OP_COSF;
             for (size_t start = 0; start < total; start += chunk) {
                 bp.nodes = d_nodes.ptr + start;
                 bp.count = uint32_t(std::min<size_t>(chunk, total - start));
                 CUDA_TRY(cudaMemsetAsync(d_work.ptr, 0, 4, stream));
-                CUDA_TRY(dispatch(DynamicRows{}, ix->dtype, [&](auto t) {
-                    return launch_consolidate_pool_op<decltype(t)::value>(op, p, bp, grid, stream);
-                }));
+                CUDA_TRY(b.sq ? dispatch(DynamicSqRows{}, ix->dtype, [&](auto t) {
+                                    return launch_consolidate_pool_sq<decltype(t)::value>(op, p, bp, grid, stream);
+                                })
+                              : dispatch(DynamicRows{}, ix->dtype, [&](auto t) {
+                                    return launch_consolidate_pool_op<decltype(t)::value>(op, p, bp, grid, stream);
+                                }));
                 CUDA_TRY(cudaMemsetAsync(d_work.ptr, 0, 4, stream));
                 bp.reverse = PRUNE_CONSOLIDATE;
                 const int prune_grid = int(std::min<size_t>(size_t(rep->sm_count) * 16, bp.count));
-                CUDA_TRY(dispatch(DynamicRows{}, ix->dtype, [&](auto t) {
-                    return launch_build_prune_op<decltype(t)::value>(op, p, bp, prune_grid, stream);
-                }));
+                CUDA_TRY(b.sq ? dispatch(DynamicSqRows{}, ix->dtype, [&](auto t) {
+                                    return launch_build_prune_sq<decltype(t)::value>(op, p, bp, prune_grid, stream);
+                                })
+                              : dispatch(DynamicRows{}, ix->dtype, [&](auto t) {
+                                    return launch_build_prune_op<decltype(t)::value>(op, p, bp, prune_grid, stream);
+                                }));
             }
             ref_degree_kernel<<<unsigned((n + 255) / 256), 256, 0, stream>>>(d_deg.ptr, uint32_t(n), rep->d_ref_degree.ptr);
             count_launch();
@@ -453,27 +514,40 @@ int svsb200_dynamic_compact(svsb200_index* ix) {
     return 0;
 }
 
-int svsb200_dynamic_build(const void* vectors, int dtype, size_t n, size_t dim, int metric, float alpha,
-                          size_t graph_max_degree, size_t window_size, size_t max_candidates, size_t prune_to,
-                          const uint64_t* external_ids, int device, svsb200_index** out) {
-    const char* who = "svsb200_dynamic_build";
-    if (!out) return fail("svsb200_dynamic_build: NULL output");
+}  // extern "C"
+
+// The body of svsb200_dynamic_build and svsb200_dynamic_build_sq, after their row checks: `sq` marks int8 / uint8 rows
+// as SQ codes of `scale` and `bias`.  Errors read "<who>: ...".
+static int dynamic_build(const char* who, const void* vectors, int dtype, bool sq, float scale, float bias, size_t n,
+                         size_t dim, int metric, float alpha, size_t graph_max_degree, size_t window_size,
+                         size_t max_candidates, size_t prune_to, const uint64_t* external_ids, int device,
+                         svsb200_index** out) {
+    const std::string w(who);
+    if (!out) return fail(w + ": NULL output");
     *out = nullptr;
-    if (dtype != SVSB200_F32 && dtype != SVSB200_F16) return fail("svsb200_dynamic_build: float32 / float16 data only");
-    if (metric < SVSB200_L2 || metric > SVSB200_COSINE) return fail("svsb200_dynamic_build: bad metric");
-    if (graph_max_degree == 0 || graph_max_degree > 32u * kFastMaxGW)
-        return fail("svsb200_dynamic_build: graph_max_degree must be in [1, 128]");
-    if (window_size == 0) return fail("svsb200_dynamic_build: window_size must be positive");
+    if (metric < SVSB200_L2 || metric > SVSB200_COSINE) return fail(w + ": bad metric");
+    if (graph_max_degree == 0 || graph_max_degree > 32u * kFastMaxGW) return fail(w + ": graph_max_degree must be in [1, 128]");
+    if (window_size == 0) return fail(w + ": window_size must be positive");
     if (int rc = resolve_mutation_parameters(who, metric, graph_max_degree, &alpha, &window_size, &max_candidates, &prune_to))
         return rc;
+    // the ids are checked as the create step checks them, before the build runs
+    const char* create = sq ? "svsb200_dynamic_create_sq" : "svsb200_dynamic_create";
+    if (n && !external_ids) return fail(std::string(create) + ": NULL external ids");
+    {
+        SlotTable probe;
+        if (int rc = probe.assign(create, external_ids, n)) return rc;
+    }
     std::vector<uint32_t> graph(n * (graph_max_degree + 1));
     uint32_t entry_point = 0;
-    if (int rc = svsb200_build_vamana(vectors, dtype, n, dim, 0, metric, alpha, graph_max_degree, window_size, max_candidates,
-                                      prune_to, device, graph.data(), &entry_point))
+    if (int rc = sq ? svsb200_build_vamana_sq(vectors, dtype, n, dim, metric, scale, bias, alpha, graph_max_degree, window_size,
+                                              max_candidates, prune_to, device, graph.data(), &entry_point)
+                    : svsb200_build_vamana(vectors, dtype, n, dim, 0, metric, alpha, graph_max_degree, window_size,
+                                           max_candidates, prune_to, device, graph.data(), &entry_point))
         return rc;
     svsb200_index* ix = nullptr;
-    if (int rc = svsb200_dynamic_create(vectors, dtype, n, dim, graph.data(), graph_max_degree + 1, entry_point, metric,
-                                        external_ids, device, &ix))
+    const float aux[2] = {scale, bias};
+    if (int rc = dynamic_create(create, vectors, dtype, sq ? SVSB200_SQ : SVSB200_PLAIN, sq ? aux : nullptr, n, dim, graph.data(),
+                                graph_max_degree + 1, entry_point, metric, external_ids, device, &ix))
         return rc;
     ix->dyn_alpha = alpha;
     ix->dyn_window = window_size;
@@ -481,6 +555,28 @@ int svsb200_dynamic_build(const void* vectors, int dtype, size_t n, size_t dim, 
     ix->dyn_prune_to = prune_to;
     *out = ix;
     return 0;
+}
+
+extern "C" {
+
+int svsb200_dynamic_build(const void* vectors, int dtype, size_t n, size_t dim, int metric, float alpha,
+                          size_t graph_max_degree, size_t window_size, size_t max_candidates, size_t prune_to,
+                          const uint64_t* external_ids, int device, svsb200_index** out) {
+    if (out) *out = nullptr;
+    if (dtype != SVSB200_F32 && dtype != SVSB200_F16) return fail("svsb200_dynamic_build: float32 / float16 data only");
+    return dynamic_build("svsb200_dynamic_build", vectors, dtype, false, 1.f, 0.f, n, dim, metric, alpha, graph_max_degree,
+                         window_size, max_candidates, prune_to, external_ids, device, out);
+}
+
+int svsb200_dynamic_build_sq(const void* codes, int code_type, size_t n, size_t dim, int metric, float scale, float bias,
+                             float alpha, size_t graph_max_degree, size_t window_size, size_t max_candidates,
+                             size_t prune_to, const uint64_t* external_ids, int device, svsb200_index** out) {
+    const char* who = "svsb200_dynamic_build_sq";
+    if (out) *out = nullptr;
+    if (code_type != SVSB200_I8 && code_type != SVSB200_U8) return fail("svsb200_dynamic_build_sq: codes must be int8 or uint8");
+    if (int rc = sq_check_params(who, scale, bias)) return rc;
+    return dynamic_build(who, codes, code_type, true, scale, bias, n, dim, metric, alpha, graph_max_degree, window_size,
+                         max_candidates, prune_to, external_ids, device, out);
 }
 
 }  // extern "C"

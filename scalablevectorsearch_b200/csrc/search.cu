@@ -417,9 +417,12 @@ static int wait_dynamic(Scratch* sc, cudaEvent_t ev, bool* cancelled) {
 static int search_dynamic(svsb200_index* ix, Replica* rep, Scratch* sc, SearchParams p, LaunchConfig cfg, int op, bool use_fast,
                           cudaStream_t stream) {
     const int rowt = ix->dtype;
-    if (ix->storage != SVSB200_PLAIN || (rowt != SVSB200_F32 && rowt != SVSB200_F16))
-        return fail("dynamic index: float32 / float16 plain storage only");
-    if (!use_fast || op > OP_COSF)
+    const bool sq = ix->storage == SVSB200_SQ;
+    if (sq ? rowt != SVSB200_I8 && rowt != SVSB200_U8
+           : ix->storage != SVSB200_PLAIN || (rowt != SVSB200_F32 && rowt != SVSB200_F16))
+        return fail("dynamic index: float32 / float16 plain storage or int8 / uint8 SQ codes only");
+    // (over SQ codes, L2 runs the integer operator on the compressed query: choose_op's OP_L2I)
+    if (!use_fast || (sq ? op != OP_L2I && op != OP_IPF && op != OP_COSF : op > OP_COSF))
         return fail("dynamic index: the search needs the lean kernel (visited filter on, generic_kernel off, float queries)");
     const size_t fixed = fast_smem_bytes(p.qstride, 0, p.deg_pad, p.filter_slots * 2u);
     const size_t max_cap = std::min<size_t>((kSmemOptInMax - fixed) / 8 / 32 * 32, size_t(1) << 24);
@@ -442,7 +445,8 @@ static int search_dynamic(svsb200_index* ix, Replica* rep, Scratch* sc, SearchPa
         cfg.smem_bytes = fast_smem_bytes(p.qstride, p.cap_pad, p.deg_pad, p.filter_slots * 2u);
         CUDA_TRY(cudaMemsetAsync(sc->d_counter.ptr, 0, sizeof(unsigned int), stream));
         CUDA_TRY(cudaMemsetAsync(p.ovf, 0, sizeof(uint32_t), stream));
-        CUDA_TRY(dispatch(DynamicRows{}, rowt, [&](auto t) { return launch_search_dynamic<decltype(t)::value>(op, p, cfg); }));
+        CUDA_TRY(sq ? dispatch(DynamicSqRows{}, rowt, [&](auto t) { return launch_search_dynamic_sq<decltype(t)::value>(op, p, cfg); })
+                    : dispatch(DynamicRows{}, rowt, [&](auto t) { return launch_search_dynamic<decltype(t)::value>(op, p, cfg); }));
         CUDA_TRY(cudaEventRecord(sc->ev_done, stream));
         bool cancelled = false;
         if (int rc = wait_dynamic(sc, sc->ev_done, &cancelled)) return rc;

@@ -32,12 +32,13 @@ namespace svsb200 {
 // (H100 SXM, 400 W) 24 CTAs ran at 2.9 M QPS against 4.3 M with 16.
 // The graph builder's kernels over SQ codes with a float operator (MIP, cosine) decompress every element of a row on
 // the fly; at 128 registers they spill, so they are compiled for 8 CTAs per SM (up to 255 registers, no spills; ptxas -v).
+// So is the MutableBuffer search of a dynamic index over SQ codes with those operators (DESIGN.md §14).
 constexpr int kSqBuildMinBlocks = 8;
-template <int ROWT, int OP, int DS, int KS, bool HIST = false> constexpr int fast_min_blocks() {
+template <int ROWT, int OP, int DS, int KS, bool HIST = false, bool MUT = false> constexpr int fast_min_blocks() {
 #ifdef SVSB200_FAST_MIN_BLOCKS
     return SVSB200_FAST_MIN_BLOCKS;
 #else
-    return HIST && kIntRow<ROWT> && OP < OP_L2I ? kSqBuildMinBlocks : 16;
+    return (HIST || MUT) && kIntRow<ROWT> && OP < OP_L2I ? kSqBuildMinBlocks : 16;
 #endif
 }
 
@@ -66,7 +67,7 @@ static __device__ unsigned long long g_phase_clocks[8];   // (one copy per trans
 // entries, and a query whose cut point would lie beyond them stops, lists itself in `ovf` and is re-run by the host
 // with more room.  The copy-out is cleanup() + the first k valid entries, as external ids.
 template <int ROWT, int OP, int DS, int KS, bool HIST = false, bool MUT = false>
-__global__ void __launch_bounds__(32, fast_min_blocks<ROWT, OP, DS, KS, HIST>()) vamana_search_fast_kernel(const __grid_constant__ SearchParams p) {
+__global__ void __launch_bounds__(32, fast_min_blocks<ROWT, OP, DS, KS, HIST, MUT>()) vamana_search_fast_kernel(const __grid_constant__ SearchParams p) {
     constexpr int NROWS = 2;
     constexpr bool kInt = (OP >= OP_L2I);
     constexpr int G = kInt ? 4 : KS * 16 / Row<ROWT>::LPT;   // threads per row
@@ -496,6 +497,11 @@ template <int ROWT> cudaError_t launch_search_fast(int op, const SearchParams& p
 template <int ROWT> cudaError_t launch_search_dynamic(int op, const SearchParams& p, const LaunchConfig& cfg) {
     return dispatch(DynamicOps{}, op, [&](auto o) { return launch_fast<ROWT, decltype(o)::value, false, true>(p, cfg); });
 }
+// Over SQ codes: OP_L2I reads SearchParams::sq at run time, OP_IPF / OP_COSF decompress the codes (as the static SQ
+// search does through launch_search_fast).
+template <int ROWT> cudaError_t launch_search_dynamic_sq(int op, const SearchParams& p, const LaunchConfig& cfg) {
+    return dispatch(DynamicSqOps{}, op, [&](auto o) { return launch_fast<ROWT, decltype(o)::value, false, true>(p, cfg); });
+}
 
 extern template cudaError_t launch_search_fast<SVSB200_F32>(int, const SearchParams&, const LaunchConfig&);
 extern template cudaError_t launch_search_fast<SVSB200_F16>(int, const SearchParams&, const LaunchConfig&);
@@ -504,5 +510,7 @@ extern template cudaError_t launch_search_fast<SVSB200_U8>(int, const SearchPara
 extern template cudaError_t launch_search_fast<ROW_LVQ8>(int, const SearchParams&, const LaunchConfig&);
 extern template cudaError_t launch_search_dynamic<SVSB200_F32>(int, const SearchParams&, const LaunchConfig&);
 extern template cudaError_t launch_search_dynamic<SVSB200_F16>(int, const SearchParams&, const LaunchConfig&);
+extern template cudaError_t launch_search_dynamic_sq<SVSB200_I8>(int, const SearchParams&, const LaunchConfig&);
+extern template cudaError_t launch_search_dynamic_sq<SVSB200_U8>(int, const SearchParams&, const LaunchConfig&);
 
 }  // namespace svsb200

@@ -456,20 +456,27 @@ class DynamicVamana(_lib._Slots, Vamana):
     from a graph, its data and one external id per row, with ``add``, soft ``delete``, ``consolidate`` and
     ``compact``.  Searches return external ids and never return a deleted one, while the walk still goes through
     deleted rows, exactly as ``MutableVamanaIndex::search`` does.  Mutations must not run concurrently with searches
-    of the same index.  float32 / float16 data, one device.  A delete (``delete_entries``, dynamic_index.h:773-788)
-    is soft: the slots are Deleted, and keep their rows and external ids until :meth:`consolidate`."""
+    of the same index.  float32 / float16 data, or scalar-quantised int8 / uint8 codes (``sq=(scale, bias)``: the
+    reference's ``MutableVamanaIndex`` over ``SQDataset``), one device.  A delete (``delete_entries``,
+    dynamic_index.h:773-788) is soft: the slots are Deleted, and keep their rows and external ids until
+    :meth:`consolidate`."""
 
     _ABI = "svsb200_dynamic"
 
     @classmethod
     def build(cls, parameters: VamanaBuildParameters, data: np.ndarray, ids=None, distance: "DistanceType" = None,
-              device: int = 0, num_threads: int = 1) -> "DynamicVamana":
+              device: int = 0, num_threads: int = 1, sq: tuple | None = None) -> "DynamicVamana":
         """``svs.DynamicVamana.build(parameters, data, ids, distance)`` (``MutableVamanaIndex(parameters, data,
         external_ids, distance)``, dynamic_index.h:208-261): the GPU builder's graph, with ``parameters`` kept as the
-        mutation parameters.  ``ids`` defaults to ``0 .. n-1``."""
+        mutation parameters.  ``ids`` defaults to ``0 .. n-1``.  ``sq=(scale, bias)`` marks ``data`` as SQ codes (as
+        in :meth:`from_arrays`), built as :meth:`Vamana.build` builds them."""
         distance = DistanceType.L2 if distance is None else DistanceType(distance)
-        data = _lib._rows(data, (np.float32, np.float16), ndim_error=None,
-                          dtype_error="DynamicVamana.build takes a 2-D float32 / float16 array")
+        if sq is not None:
+            data = _lib._rows(data, (np.int8, np.uint8), ndim_error=None,
+                              dtype_error="SQ codes are a 2-D int8 / uint8 array")
+        else:
+            data = _lib._rows(data, (np.float32, np.float16), ndim_error=None,
+                              dtype_error="DynamicVamana.build takes a 2-D float32 / float16 array")
         if not parameters.use_full_search_history:
             raise ValueError("the GPU builder always keeps the full search history (the reference's default)")
         n = data.shape[0]
@@ -483,24 +490,35 @@ class DynamicVamana(_lib._Slots, Vamana):
         self._params = VamanaSearchParameters()
         self._num_threads = int(num_threads)
         handle = C.c_void_p()
-        _lib.check(self._lib.svsb200_dynamic_build(
-            data.ctypes.data, _DTYPE_CODE[data.dtype], n, data.shape[1], int(distance), float(parameters.alpha),
-            int(parameters.graph_max_degree), int(parameters.window_size), int(parameters.max_candidate_pool_size),
-            int(parameters.prune_to), ids.ctypes.data, int(device), C.byref(handle)))
+        tail = (float(parameters.alpha), int(parameters.graph_max_degree), int(parameters.window_size),
+                int(parameters.max_candidate_pool_size), int(parameters.prune_to), ids.ctypes.data, int(device),
+                C.byref(handle))
+        if sq is None:
+            _lib.check(self._lib.svsb200_dynamic_build(data.ctypes.data, _DTYPE_CODE[data.dtype], n, data.shape[1],
+                                                       int(distance), *tail))
+        else:
+            _lib.check(self._lib.svsb200_dynamic_build_sq(data.ctypes.data, _DTYPE_CODE[data.dtype], n, data.shape[1],
+                                                          int(distance), float(sq[0]), float(sq[1]), *tail))
         self._h = handle
         self.build_parameters = parameters
         return self
 
     @classmethod
     def from_arrays(cls, data: np.ndarray, graph: np.ndarray, entry_point: int, ids=None,
-                    distance: DistanceType = DistanceType.L2, device: int = 0, num_threads: int = 1) -> "DynamicVamana":
+                    distance: DistanceType = DistanceType.L2, device: int = 0, num_threads: int = 1,
+                    sq: tuple | None = None) -> "DynamicVamana":
         """``MutableVamanaIndex(graph, data, entry_point, distance, external_ids, threadpool)``
-        (dynamic_index.h:178-202); ``ids`` defaults to ``0 .. n-1``."""
+        (dynamic_index.h:178-202); ``ids`` defaults to ``0 .. n-1``.  ``sq=(scale, bias)`` marks ``data`` as
+        scalar-quantised int8 / uint8 codes (from :func:`scalablevectorsearch_b200.ivf.sq_compress`): the scale and
+        bias stay fixed, and :meth:`add` then takes float32 rows, encoded with them as ``SQDataset::set_datum`` does."""
         graph = np.ascontiguousarray(graph, dtype=np.uint32)
         if graph.ndim != 2:
             raise ValueError("data and graph must be 2-D")
-        data = _lib._rows(data, (np.float32, np.float16), "data and graph must be 2-D",
-                          "a dynamic index takes float32 / float16 data")
+        if sq is not None:
+            data = _lib._rows(data, (np.int8, np.uint8), "data and graph must be 2-D", "SQ codes are int8 or uint8")
+        else:
+            data = _lib._rows(data, (np.float32, np.float16), "data and graph must be 2-D",
+                              "a dynamic index takes float32 / float16 data")
         if graph.shape[0] != data.shape[0]:
             raise ValueError("Wrong sizes!")
         n = data.shape[0]
@@ -514,9 +532,13 @@ class DynamicVamana(_lib._Slots, Vamana):
         self._params = VamanaSearchParameters()
         self._num_threads = int(num_threads)
         handle = C.c_void_p()
-        _lib.check(self._lib.svsb200_dynamic_create(
-            data.ctypes.data, _DTYPE_CODE[data.dtype], n, data.shape[1], graph.ctypes.data, graph.shape[1],
-            int(entry_point), int(self._distance), ids.ctypes.data, int(device), C.byref(handle)))
+        tail = (graph.ctypes.data, graph.shape[1], int(entry_point), int(self._distance), ids.ctypes.data, int(device),
+                C.byref(handle))
+        if sq is None:
+            _lib.check(self._lib.svsb200_dynamic_create(data.ctypes.data, _DTYPE_CODE[data.dtype], n, data.shape[1], *tail))
+        else:
+            _lib.check(self._lib.svsb200_dynamic_create_sq(data.ctypes.data, _DTYPE_CODE[data.dtype], n, data.shape[1],
+                                                           float(sq[0]), float(sq[1]), *tail))
         self._h = handle
         return self
 
@@ -533,9 +555,10 @@ class DynamicVamana(_lib._Slots, Vamana):
         return self._lib.svsb200_index_size(self._h)
 
     def add(self, points: np.ndarray, ids, reuse_empty: bool = False) -> np.ndarray:
-        """``add_points`` (dynamic_index.h:657-749): insert rows of the index's dtype with new external ids.  Empty
-        slots are used first (from the start with ``reuse_empty``), then the index grows.  Fails without changing
-        anything on a repeated, present or reserved id.  Returns the slots used."""
+        """``add_points`` (dynamic_index.h:657-749): insert rows of the index's dtype (float32 rows into an SQ index,
+        encoded with its scale and bias; a NaN or an infinity is refused) with new external ids.  Empty slots are used
+        first (from the start with ``reuse_empty``), then the index grows.  Fails without changing anything on a
+        repeated, present or reserved id.  Returns the slots used."""
         return self._add(points, ids, reuse_empty)
 
     def consolidate(self):
