@@ -666,6 +666,28 @@ int svsb200_ivf_search_filtered_device(svsb200_ivf* index, const void* d_queries
                                        size_t n_probes, const uint32_t* d_id_bitmap, uint64_t* d_out_ids, float* d_out_dists,
                                        uint32_t* d_out_probes, uint32_t* d_out_allowed, uint32_t* d_out_rows, void* stream);
 
+/* The shape svsb200_ivf_search* and svsb200_dynamic_ivf_search* run (introspection, host arithmetic only, like
+ * svsb200_flat_plan; the search calls this same arithmetic) for an index of `dim`-element rows of `dtype`: float32 /
+ * float16 with `storage` SVSB200_PLAIN, or int8 / uint8 codes with SVSB200_SQ; `dynamic` nonzero for the dynamic index
+ * and the filtered searches (the leaf's DYN form).
+ *   tile_rows:        rows per shared-memory ring slot: 32, halved while two slots would pass 96 KB;
+ *   queries_per_item: Q, the queries a work item scores together (at most 64);
+ *   ctas_per_sm:      2 where Q >= 1 fits half of the 227 KB - 1 KB a CTA may use, else 1;
+ *   query_chunk:      queries per pass, min(nq, max(1, min(8192, 256 MiB / (12 n_probes k))));
+ *   leaf:             0 = the float-tree scan (float rows; SQ MIP / cosine), 1 = the SQ L2 tensor-core scan;
+ *   static_dim:       96 or 128 where the float tree runs at that static dimension, else 0 (and 0 for leaf 1);
+ *   rows_per_pass:    rows per group and pass of the float tree (1 or 2; 0 for leaf 1);
+ *   smem_bytes:       dynamic shared memory of one CTA.
+ * Fails, with the search's own message, where no Q >= 1 fits one CTA per SM. */
+int svsb200_ivf_plan(size_t dim, int dtype, int storage, int metric, size_t k, size_t n_probes, size_t nq, int dynamic,
+                     uint32_t* tile_rows, uint32_t* queries_per_item, uint32_t* ctas_per_sm, uint32_t* query_chunk,
+                     uint32_t* leaf, uint32_t* static_dim, uint32_t* rows_per_pass, uint64_t* smem_bytes);
+/* The grouped assignment of svsb200_ivf_cluster_hierarchical for `dim`-element rows (host arithmetic only): `tile`
+ * rows per work item (64, halved while two tiles of prepared rows would pass 96 KB), the group's centroids staged
+ * `chunk` at a time, `smem_bytes` of dynamic shared memory per CTA.  Fails, with the clustering's own message, where
+ * that passes 227 KB - 1 KB. */
+int svsb200_ivf_group_plan(size_t dim, uint32_t* tile, uint32_t* chunk, uint64_t* smem_bytes);
+
 /* Dynamic IVF index.  Replaces: DynamicIVFIndex (include/svs/index/ivf/dynamic_ivf.h) with svs::DynamicIVF: the IVF
  * index over a mutable set of float32 / float16 rows (or SQ codes, svsb200_dynamic_ivf_create_sq) on one device, L2 /
  * MIP / cosine, addressed by external ids.  A distinct handle type.  Every slot (internal id) is Valid or Empty; a

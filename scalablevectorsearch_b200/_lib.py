@@ -95,6 +95,8 @@ ABI = {
     "svsb200_ivf_search_device": (i32, [vp, vp, i32, sz, sz, sz, vp, vp, vp]),
     "svsb200_ivf_search_filtered": (i32, [vp, vp, i32, sz, sz, sz, vp, vp, vp, vp, vp, vp]),
     "svsb200_ivf_search_filtered_device": (i32, [vp, vp, i32, sz, sz, sz, vp, vp, vp, vp, vp, vp, vp]),
+    "svsb200_ivf_plan": (i32, [sz, i32, i32, i32, sz, sz, sz, i32] + [P(u32)] * 7 + [P(u64)]),
+    "svsb200_ivf_group_plan": (i32, [sz, P(u32), P(u32), P(u64)]),
     "svsb200_dynamic_ivf_create": (i32, [vp, i32, sz, sz, i32, vp, sz, vp, vp, i32, P(vp)]),
     "svsb200_dynamic_ivf_create_sq": (i32, [vp, i32, sz, sz, i32, f32, f32, vp, sz, vp, vp, i32, P(vp)]),
     "svsb200_dynamic_ivf_destroy": _H, "svsb200_dynamic_ivf_size": _GET, "svsb200_dynamic_ivf_num_slots": _GET,

@@ -206,6 +206,21 @@ struct IvfGroup {
     size_t pos, rows, cent, cents;
 };
 
+// The shape of ivf_group_assign_kernel for `dim`-element rows (svsb200_ivf_group_plan): `tile` positions per work item,
+// 64 halved while two tiles of prepared rows would pass 96 KB, the centroids staged `tile` at a time.
+struct IvfGroupPlan {
+    uint32_t tile, chunk;
+    size_t smem;
+};
+static int ivf_group_plan(size_t dim, IvfGroupPlan* plan) {
+    const uint32_t qs = query_stride(dim);
+    uint32_t tile = 64;
+    while (tile > 1 && ivf_group_smem_bytes(qs, 2 * tile, 0) > (size_t(96) << 10)) tile >>= 1;
+    *plan = {tile, tile, ivf_group_smem_bytes(qs, tile, tile)};
+    if (plan->smem > kSmemOptInMax - 1024) return fail("svsb200_ivf_cluster_hierarchical: rows too wide for the grouped kernels");
+    return 0;
+}
+
 // Nearest centroid of every position of the groups (each row among its own group's centroids d_cent [C][dim]),
 // ivf_group_assign_kernel over work items of at most `tile` positions, launched over `batch` positions at a time (which
 // changes no result).  out: global centroid per position, or per row id with by_row.  Synchronises `stream`.
@@ -213,10 +228,10 @@ static int ivf_group_assign(const char* d_rows, int dtype, size_t dim, int metri
                             const std::vector<IvfGroup>& groups, size_t batch, const float* d_cent, uint32_t* d_out, bool by_row,
                             cudaStream_t stream) {
     const uint32_t qs = query_stride(dim);
-    uint32_t tile = 64;
-    while (tile > 1 && ivf_group_smem_bytes(qs, 2 * tile, 0) > (size_t(96) << 10)) tile >>= 1;
-    const size_t smem = ivf_group_smem_bytes(qs, tile, tile);
-    if (smem > kSmemOptInMax - 1024) return fail("svsb200_ivf_cluster_hierarchical: rows too wide for the grouped kernels");
+    IvfGroupPlan plan;
+    if (int rc = ivf_group_plan(dim, &plan)) return rc;
+    const uint32_t tile = plan.tile;
+    const size_t smem = plan.smem;
     size_t total = 0;
     for (const IvfGroup& g : groups) total = std::max(total, g.pos + g.rows);
     // the work items of every batch, in order, and where each batch's items start
@@ -246,7 +261,7 @@ static int ivf_group_assign(const char* d_rows, int dtype, size_t dim, int metri
     gp.perm = d_perm;
     gp.cent = d_cent;
     gp.tile = tile;
-    gp.chunk = tile;
+    gp.chunk = plan.chunk;
     gp.out = d_out;
     gp.by_row = by_row;
     const int op = metric == SVSB200_L2 ? OP_L2F : metric == SVSB200_IP ? OP_IPF : OP_COSF;
@@ -269,15 +284,19 @@ static int ivf_group_assign(const char* d_rows, int dtype, size_t dim, int metri
     return 0;
 }
 
+// Rows per group and pass of ivf_scan_kernel: two where they fit the register bound without spilling, one for float16
+// rows, SQ codes and cosine (as for the masked scan) and for the dynamic form's generic dimension.
+constexpr int ivf_scan_rows_per_pass(int rowt, int op, int ds, bool dyn) {
+    return rowt == SVSB200_F16 || rowt == SVSB200_I8 || rowt == SVSB200_U8 || op == OP_COSF || (dyn && ds == 0) ? 1 : 2;
+}
+
 template <int ROWT, bool DYN, typename Ops = IvfOps>
 static cudaError_t launch_ivf_scan(int op, const IvfScanParams& ip, const LaunchConfig& cfg) {
     return dispatch(Ops{}, op, [&](auto o) {
         constexpr int OP = decltype(o)::value;
         return with_shape<OP, true>(ip.p.dim, false, [&](auto ds, auto) {
             constexpr int DS = decltype(ds)::value;
-            // rows per group and pass: two where they fit the register bound without spilling, one for float16 rows,
-            // SQ codes and cosine (as for the masked scan) and for the dynamic form's generic dimension
-            constexpr int NR = ROWT == SVSB200_F16 || kIntRow<ROWT> || OP == OP_COSF || (DYN && DS == 0) ? 1 : 2;
+            constexpr int NR = ivf_scan_rows_per_pass(ROWT, OP, DS, DYN);
             return launch_kernel(ivf_scan_kernel<ROWT, OP, DS, NR, DYN>, cfg, size_t(1) << 20, true, ip);
         });
     });
@@ -286,6 +305,47 @@ static cudaError_t launch_ivf_scan(int op, const IvfScanParams& ip, const Launch
 // Queries per chunk: the per-(query, probe) lists under IVF_LIST_BUDGET.
 static size_t ivf_chunk(size_t P, size_t k) {
     return std::max<size_t>(1, std::min(IVF_MAX_CHUNK, IVF_LIST_BUDGET / (P * k * 12)));
+}
+
+// The shape of one search (svsb200_ivf_plan): the ring tile, Q and the CTAs per SM it implies, the query chunk, the
+// leaf kernel and, for the float tree, its static dimension and rows per pass.
+struct IvfPlan {
+    uint32_t tile_rows, Q, ctas, leaf, ds, nr;
+    size_t chunk, smem;
+};
+static int ivf_plan(size_t dim, int dtype, int storage, int metric, size_t k, size_t P, bool dyn, IvfPlan* plan) {
+    const uint32_t row_stride = data_row_stride(storage, dtype, dim), qstride = query_stride(dim);
+    // SQ rows: MIP and cosine run ivf_scan_kernel on the decompressed float tree, L2 the tensor-core leaf
+    const bool sq_l2 = storage == SVSB200_SQ && metric == SVSB200_L2;
+    // ring tiles: 32 rows, fewer for rows so wide that two tiles would pass 96 KB
+    uint32_t tile_rows = IVF_TILE_ROWS;
+    while (tile_rows > 1 && 2 * size_t(tile_rows) * row_stride > (size_t(96) << 10)) tile_rows >>= 1;
+    auto smem = [&](size_t q) {
+        return sq_l2 ? ivf_sq_l2_smem_bytes(row_stride, tile_rows, uint32_t(dim), uint32_t(k), uint32_t(q))
+                     : ivf_smem_bytes(row_stride, tile_rows, qstride, uint32_t(k), uint32_t(q));
+    };
+    // queries per work item: two CTAs per SM where they fit, else one
+    const size_t fixed = smem(0);
+    const size_t slot = smem(1) - fixed;
+    const size_t limit = kSmemOptInMax - 1024;   // (the kernel's static shared memory)
+    auto fit = [&](size_t room) { return fixed < room ? std::min<size_t>(IVF_QMAX, (room - fixed) / slot) : 0; };
+    size_t Q = fit(limit / 2);
+    const uint32_t ctas = Q ? 2 : 1;
+    if (Q == 0) Q = fit(limit);
+    if (Q == 0) return fail("svsb200_ivf_search: k and the row size need more shared memory than a CTA has");
+    *plan = {tile_rows, uint32_t(Q), ctas, sq_l2 ? 1u : 0u, 0, 0, ivf_chunk(P, k), smem(Q)};
+    if (sq_l2) return 0;
+    const int op = metric == SVSB200_L2 ? OP_L2F : metric == SVSB200_IP ? OP_IPF : OP_COSF;
+    CUDA_TRY(dispatch(IvfOps{}, op, [&](auto o) {
+        constexpr int OP = decltype(o)::value;
+        return with_shape<OP, true>(uint32_t(dim), false, [&](auto ds, auto) {
+            constexpr int DS = decltype(ds)::value;
+            plan->ds = DS;
+            plan->nr = ivf_scan_rows_per_pass(dtype, OP, DS, dyn);
+            return cudaSuccess;
+        });
+    }));
+    return 0;
 }
 
 static IvfScratch* ivf_scratch(svsb200_ivf* iv, Scratch* sc) {
@@ -302,25 +362,13 @@ int ivf_search_on_device(svsb200_ivf* iv, Scratch* sc, const void* d_queries, in
     cudaStream_t stream = sc->stream;
     IvfScratch* is = ivf_scratch(iv, sc);
     const uint32_t C = uint32_t(iv->C), dim = uint32_t(ix->dim), qstride = query_stride(dim);
-    // SQ rows: MIP and cosine run ivf_scan_kernel on the decompressed float tree, L2 the tensor-core leaf
     const bool sq = ix->storage == SVSB200_SQ;
     const bool sq_l2 = sq && ix->metric == SVSB200_L2;
-    // ring tiles: 32 rows, fewer for rows so wide that two tiles would pass 96 KB
-    uint32_t tile_rows = IVF_TILE_ROWS;
-    while (tile_rows > 1 && 2 * size_t(tile_rows) * ix->row_stride > (size_t(96) << 10)) tile_rows >>= 1;
-    auto smem = [&](size_t q) {
-        return sq_l2 ? ivf_sq_l2_smem_bytes(ix->row_stride, tile_rows, dim, uint32_t(k), uint32_t(q))
-                     : ivf_smem_bytes(ix->row_stride, tile_rows, qstride, uint32_t(k), uint32_t(q));
-    };
-    // queries per work item: two CTAs per SM where they fit, else one
-    const size_t fixed = smem(0);
-    const size_t slot = smem(1) - fixed;
-    const size_t limit = kSmemOptInMax - 1024;   // (the kernel's static shared memory)
-    auto fit = [&](size_t room) { return fixed < room ? std::min<size_t>(IVF_QMAX, (room - fixed) / slot) : 0; };
-    size_t Q = fit(limit / 2);
-    if (Q == 0) Q = fit(limit);
-    if (Q == 0) return fail("svsb200_ivf_search: k and the row size need more shared memory than a CTA has");
-    const size_t chunk = ivf_chunk(P, k);
+    const bool dyn = d_ext_ids || d_masked_ids;   // the scan's DYN form: all-ones ids are not candidates
+    IvfPlan plan;
+    if (int rc = ivf_plan(dim, ix->dtype, ix->storage, ix->metric, k, P, dyn, &plan)) return rc;
+    const uint32_t tile_rows = plan.tile_rows;
+    const size_t Q = plan.Q, chunk = plan.chunk;
     const size_t qrow = size_t(dim) * esize(qdtype);
     const size_t cmax = std::min(chunk, nq);
     CUDA_TRY(is->probe_ids.ensure(cmax * P));
@@ -334,7 +382,6 @@ int ivf_search_on_device(svsb200_ivf* iv, Scratch* sc, const void* d_queries, in
     CUDA_TRY(is->list.ensure(cmax * P));
     const int op = sq_l2 ? OP_L2I : ix->metric == SVSB200_L2 ? OP_L2F : ix->metric == SVSB200_IP ? OP_IPF : OP_COSF;
     const int prep = !sq ? PREP_FLOAT : sq_l2 ? PREP_SQ_L2 : ix->metric == SVSB200_IP ? PREP_SQ_IP : PREP_SQ_COS;
-    const bool dyn = d_ext_ids || d_masked_ids;   // the scan's DYN form: all-ones ids are not candidates
     for (size_t q0 = 0; q0 < nq; q0 += chunk) {
         const size_t nqc = std::min(chunk, nq - q0);
         const char* qp = static_cast<const char*>(d_queries) + q0 * qrow;
@@ -389,7 +436,7 @@ int ivf_search_on_device(svsb200_ivf* iv, Scratch* sc, const void* d_queries, in
         ip.out_dists = is->list_dists.ptr;
         ip.work_counter = sc->d_counter.ptr;
         CUDA_TRY(cudaMemsetAsync(sc->d_counter.ptr, 0, sizeof(unsigned int), stream));
-        const LaunchConfig cfg{-rep->sm_count, IVF_WARPS, smem(Q), stream};
+        const LaunchConfig cfg{-rep->sm_count, IVF_WARPS, plan.smem, stream};
         if (sq_l2) {
             CUDA_TRY(dispatch(IvfSqRows{}, ix->dtype, [&](auto row) {
                 constexpr int R = decltype(row)::value;
@@ -643,6 +690,47 @@ extern "C" {
 int svsb200_ivf_random(uint64_t seed, size_t count, uint64_t* out) {
     if (count && !out) return fail("svsb200_ivf_random: NULL output");
     for (size_t i = 0; i < count; ++i) out[i] = ivf_next(seed);
+    return 0;
+}
+
+// Host arithmetic only: the plan ivf_search_on_device runs, so that every shape can be checked without a device
+// (tests/test_ivf_plan.py).
+int svsb200_ivf_plan(size_t dim, int dtype, int storage, int metric, size_t k, size_t n_probes, size_t nq, int dynamic,
+                     uint32_t* tile_rows, uint32_t* queries_per_item, uint32_t* ctas_per_sm, uint32_t* query_chunk,
+                     uint32_t* leaf, uint32_t* static_dim, uint32_t* rows_per_pass, uint64_t* smem_bytes) {
+    const std::string w = "svsb200_ivf_plan";
+    if (!tile_rows || !queries_per_item || !ctas_per_sm || !query_chunk || !leaf || !static_dim || !rows_per_pass ||
+        !smem_bytes)
+        return fail(w + ": NULL output");
+    const bool plain = storage == SVSB200_PLAIN && (dtype == SVSB200_F32 || dtype == SVSB200_F16);
+    const bool sq = storage == SVSB200_SQ && (dtype == SVSB200_I8 || dtype == SVSB200_U8);
+    if (!plain && !sq) return fail(w + ": rows are float32 / float16 (plain) or int8 / uint8 (SQ)");
+    if (metric < SVSB200_L2 || metric > SVSB200_COSINE) return fail(w + ": bad metric");
+    if (dim == 0 || dim > (size_t(1) << 24)) return fail(w + ": dim must be in [1, 2^24]");
+    if (k == 0 || k > 1024) return fail(w + ": k must be in [1, 1024]");
+    if (n_probes == 0 || n_probes > 1024) return fail(w + ": n_probes must be in [1, 1024]");
+    if (nq == 0) return fail(w + ": nq must be positive");
+    IvfPlan plan;
+    if (int rc = ivf_plan(dim, dtype, storage, metric, k, n_probes, dynamic != 0, &plan)) return rc;
+    *tile_rows = plan.tile_rows;
+    *queries_per_item = plan.Q;
+    *ctas_per_sm = plan.ctas;
+    *query_chunk = uint32_t(std::min(plan.chunk, nq));
+    *leaf = plan.leaf;
+    *static_dim = plan.ds;
+    *rows_per_pass = plan.nr;
+    *smem_bytes = plan.smem;
+    return 0;
+}
+
+int svsb200_ivf_group_plan(size_t dim, uint32_t* tile, uint32_t* chunk, uint64_t* smem_bytes) {
+    if (!tile || !chunk || !smem_bytes) return fail("svsb200_ivf_group_plan: NULL output");
+    if (dim == 0 || dim > (size_t(1) << 24)) return fail("svsb200_ivf_group_plan: dim must be in [1, 2^24]");
+    IvfGroupPlan plan;
+    if (int rc = ivf_group_plan(dim, &plan)) return rc;
+    *tile = plan.tile;
+    *chunk = plan.chunk;
+    *smem_bytes = plan.smem;
     return 0;
 }
 

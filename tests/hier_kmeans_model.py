@@ -21,6 +21,7 @@ class Result:
     level1: np.ndarray          # [n]: every row's level-1 group
     seeds: list                 # the groups' stream seeds
     discarded: int              # remainder draws discarded by the allocation guard
+    level1_centroids: np.ndarray = None   # float32 [L1][dim]: the final level-1 centroids
 
 
 def level1_clusters(num_centroids: int, level1: int) -> int:
@@ -110,4 +111,4 @@ def hierarchical_kmeans(oracle, data: np.ndarray, metric: int, num_centroids: in
         rows = np.flatnonzero(level1_of == g)
         if rows.size:
             assign[rows] = start[g] + M.nearest(oracle, metric, data[rows], cent[start[g]:start[g + 1]], 1)[:, 0]
-    return Result(cent, assign, np.array(c, dtype=np.uint32), t, tl1, level1_of, seeds, discarded)
+    return Result(cent, assign, np.array(c, dtype=np.uint32), t, tl1, level1_of, seeds, discarded, cent1)

@@ -38,7 +38,7 @@ def header_prototypes():
 def test_header_declares_the_expected_surface():
     syms = header_symbols()
     for name in ("svsb200_index_create", "svsb200_search", "svsb200_search_device", "svsb200_merge_topk_device",
-                 "svsb200_get_counters", "svsb200_last_error"):
+                 "svsb200_get_counters", "svsb200_last_error", "svsb200_ivf_plan", "svsb200_ivf_group_plan"):
         assert name in syms
 
 

@@ -14,12 +14,13 @@
 import numpy as np
 import pytest
 
+import float64_layer as F64
 from conftest import bits, knn_graph
 
 pytestmark = pytest.mark.gpu
 
 METRICS = {"l2": 0, "ip": 1, "cosine": 2}
-U = 2.0 ** -24
+U = F64.U
 ALL_ONES = np.uint64(0xFFFFFFFFFFFFFFFF)
 WINDOWS = ((8, 8, 8), (33, 97, 20), (130, 300, 50))   # (window, capacity, k)
 
@@ -151,59 +152,28 @@ class Kind:
             y = (d16[:, None] * r[:, :self.dim] + l16[:, None]).astype(np.float32).astype(np.float64)
             return q, y
         if self.sq is not None:
-            scale, bias = self.sq
             # cosine decompresses scale * c + bias in fp32, one rounding per operation (scalar.h:44-46)
-            y = (scale * self.rows[ids].astype(np.float32) + bias).astype(np.float64)
-            return q, y
+            return q, F64.sq_decode(self.rows[ids], *self.sq)
         return q, self.rows[ids].astype(np.float64)
 
     def check_float64(self, metric, i, ids, d32, tag):
-        """|d32 - d64| <= (dim + 8) 2^-24 sum|terms| * 1.01 for every returned (id, distance); SQ L2 is exact."""
+        """Every returned (id, distance) within the float64 layer's bound (tests/float64_layer.py); SQ L2 is exact."""
         keep = ids != ALL_ONES
         ids, d32 = ids[keep].astype(np.int64), d32[keep].astype(np.float64)
         if len(ids) == 0:
             return
-        gamma = (self.dim + 8) * U * 1.01
         if self.sq is not None and metric == "l2":
-            scale, bias = self.sq
-            lo, hi = (-128, 127) if self.rows.dtype == np.int8 else (0, 255)
-            v = self.q[i].astype(np.float32)
-            t = ((v - bias) / scale).astype(np.float64)                    # fp32 subtract and divide, as compress does
-            qc = np.clip(np.sign(t) * np.floor(np.abs(t) + 0.5), lo, hi)   # roundf: half away from zero
-            l2 = ((self.rows[ids].astype(np.int64) - qc.astype(np.int64)) ** 2).sum(1)
-            want = np.float32(scale * scale) * l2.astype(np.float32)
+            want = F64.sq_l2_exact(self.q[i], self.rows[ids], *self.sq)
             assert np.array_equal(bits(d32.astype(np.float32)), bits(want)), f"{tag}: SQ L2 is not scale^2 * int L2"
             return
         if self.sq is not None and metric == "ip":
-            scale, bias = (float(s) for s in self.sq)
-            q, c = self.q[i].astype(np.float64), self.rows[ids].astype(np.float64)
-            d64 = (q * (scale * c + bias)).sum(1)
-            terms = (np.abs(q) * (np.abs(scale * c) + abs(bias))).sum(1)
-            err = np.abs(d32 - d64)
-            assert np.all(err <= gamma * terms), f"{tag}: SQ MIP off float64 by {np.max(err / np.maximum(terms, 1e-300))}"
-            return
-        q, y = self._operands(i, ids)
-        if self.lvq is not None and metric == "l2":
-            q = (self.q[i].astype(np.float32) - self.mean).astype(np.float64)   # fl32(q - mean), once per query
-        if metric == "l2":
-            t = (q[None, :] - y) ** 2
-            d64, terms = t.sum(1), t.sum(1)
-            bound = gamma * terms
-        elif metric == "ip":
-            t = q[None, :] * y
-            d64, terms = t.sum(1), np.abs(t).sum(1)
-            if self.lvq is not None:
-                m = q * self.mean.astype(np.float64)
-                d64, terms = d64 + m.sum(), terms + np.abs(m).sum()
-            bound = gamma * terms
+            d64, bound = F64.sq_ip(self.q[i], self.rows[ids], *self.sq)
         else:
-            t = q[None, :] * y
-            norms = np.sqrt((y * y).sum(1)) * np.sqrt((q * q).sum())
-            d64 = t.sum(1) / norms
-            bound = gamma * (np.abs(t).sum(1) / norms + 2 * np.abs(d64))
-        err = np.abs(d32 - d64)
-        bad = ~(err <= bound)
-        assert not np.any(bad), f"{tag}: off float64 by {err[bad][:4]} > {bound[bad][:4]}"
+            q, y = self._operands(i, ids)
+            if self.lvq is not None and metric == "l2":
+                q = (self.q[i].astype(np.float32) - self.mean).astype(np.float64)   # fl32(q - mean), once per query
+            d64, bound = F64.float_tree(metric, q, y, self.mean if self.lvq is not None else None)
+        F64.assert_within(d32, d64, bound, tag)
 
 
 def expected_topk(kind, oracle, metric, k):
