@@ -318,6 +318,22 @@ int svsb200_exhaustive_device(
     svsb200_index* index, const void* d_queries, int qdtype, size_t nq, size_t k,
     uint64_t* d_out_ids, float* d_out_dists, void* stream);
 
+/* Stored rows of a graph index.  Replaces: VamanaIndex::get_distance / MutableVamanaIndex::get_distance and
+ * reconstruct_at (index/vamana/index.h:915-933, dynamic_index.h:1152-1190, 1306-1322).  An id is what the handle's
+ * searches return: on a dynamic index the external id of a Valid slot (a Deleted or absent id is refused), otherwise a
+ * row id plus any svsb200_set_id_offset.  Every id is checked before any device work; a refused call names the first
+ * offending id and writes nothing.  All buffers are dense HOST memory; count = 0 succeeds and does nothing.  Plain and
+ * SQ rows (LVQ-8 is refused); a replicated index reads its first replica.  Blocking.
+ *   svsb200_index_distances: out[i] = the distance the index's search computes between query i (queries[count][dim]
+ *     of `qdtype`, any type svsb200_search takes on this handle) and the row named ids[i], bit for bit: the same query
+ *     preparation and the same expression tree, one warp per pair.
+ *   svsb200_index_reconstruct: out[count][dim] float32: plain rows widened (float16 as the reference's Float16
+ *     converts: subnormals become signed zero), SQ codes decompressed as scale * c + bias with two roundings
+ *     (DecompressionAccessor, quantization/scalar/scalar.h:606-620). */
+int svsb200_index_distances(svsb200_index* index, const void* queries, int qdtype, size_t count, const uint64_t* ids,
+                            float* out);
+int svsb200_index_reconstruct(svsb200_index* index, const uint64_t* ids, size_t count, float* out);
+
 /* The svsb200_flat_search* split for a given k (host arithmetic only, like svsb200_flat_plan): for k <= 25 exactly what
  * svsb200_flat_plan returns, with `list_entries` = 33; for 26 <= k <= 121 and nq > 256 the deep lists of a flat index
  * (svsb200_flat_index_search*): `list_entries` = 129, one list per query and piece, lists_per_query x 129 <= 1024.

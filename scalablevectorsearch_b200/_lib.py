@@ -40,6 +40,7 @@ ABI = {
     "svsb200_search_filtered": (i32, [vp, vp, i32, sz, sz, sz, vp, vp, vp, vp]),
     "svsb200_range_search": (i32, [vp, vp, i32, sz, f32, sz, vp, P(vp), P(vp)]), "svsb200_free": (None, [vp]),
     "svsb200_exhaustive_device": (i32, [vp, vp, i32, sz, sz, vp, vp, vp]),
+    "svsb200_index_distances": (i32, [vp, vp, i32, sz, vp, vp]), "svsb200_index_reconstruct": (i32, [vp, vp, sz, vp]),
     "svsb200_flat_search": (i32, [vp, vp, i32, sz, sz, vp, vp]),
     "svsb200_flat_search_device": (i32, [vp, vp, i32, sz, sz, vp, vp, vp, P(u32)]),
     "svsb200_merge_topk_device": (i32, [vp, vp, sz, sz, sz, i32, vp, vp, i32, vp]),

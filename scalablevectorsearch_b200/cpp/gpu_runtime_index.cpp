@@ -43,7 +43,16 @@
 // NOT_INITIALIZED and `has_id` is false.  k = 0 is INVALID_ARGUMENT; save / load and LeanVec are NOT_IMPLEMENTED.  A
 // non-null IDFilter becomes a bitmap over the slots (is_member(external id) for every Valid slot) for
 // svsb200_dynamic_ivf_search_filtered, with IVFIndex's filter_stop and filter_estimate_batch.
+//
+// And `svs::runtime::v0::DynamicVamanaIndex` (bindings/cpp/include/svs/runtime/dynamic_vamana_index.h) on the dynamic
+// Vamana index (svsb200_dynamic_*) for FP32, FP16 and SQI8 storage, with the behaviour of the reference's
+// DynamicVamanaIndexImpl (bindings/cpp/src/dynamic_vamana_index_impl.h): the first `add` builds the index, `remove`
+// consolidates and compacts once the soft deletions exceed half of the ids left, and `get_distance` / `reconstruct_at`
+// read the rows on the device (svsb200_index_distances / _reconstruct), so no host copy is kept.  The GPU storage is not
+// blocked: `blocksize_bytes` reports the block size the parameters ask for.  use_full_search_history = false is ignored
+// (the GPU builder always keeps the full history).  save / load and LeanVec are NOT_IMPLEMENTED.
 #include "svs/runtime/dynamic_ivf_index.h"
+#include "svs/runtime/dynamic_vamana_index.h"
 #include "svs/runtime/flat_index.h"
 #include "svs/runtime/ivf_index.h"
 #include "svs/runtime/vamana_index.h"
@@ -79,6 +88,61 @@ IVFIndex::~IVFIndex() = default;
 namespace {
 
 Status gpu_error() { return Status(ErrorCode::RUNTIME_ERROR, svsb200_last_error()); }
+
+// The search window and buffer capacity of a Vamana search: the index's default search parameters (window 10 when
+// unspecified), overridden by the call's, the window at least k and the capacity at least the window.
+void window_of(const VamanaIndex::SearchParams& defaults, const VamanaIndex::SearchParams* params, size_t k, size_t& window,
+               size_t& capacity) {
+    window = is_specified(defaults.search_window_size) ? defaults.search_window_size : 10;
+    capacity = is_specified(defaults.search_buffer_capacity) ? defaults.search_buffer_capacity : 0;
+    if (params) {
+        set_if_specified(window, params->search_window_size);
+        set_if_specified(capacity, params->search_buffer_capacity);
+    }
+    window = window < k ? k : window;
+    capacity = capacity < window ? window : capacity;
+}
+
+// float -> IEEE binary16, round to nearest even (FP16 storage)
+uint16_t to_half(float f) {
+    uint32_t x;
+    std::memcpy(&x, &f, 4);
+    const uint32_t sign = (x >> 16) & 0x8000u, ax = x & 0x7FFFFFFFu;
+    if (ax >= 0x7F800000u) return uint16_t(sign | 0x7C00u | (ax > 0x7F800000u ? 0x200u : 0u));
+    if (ax >= 0x477FF000u) return uint16_t(sign | 0x7C00u);   // rounds to >= 65520: inf
+    if (ax < 0x38800000u) {                                    // below 2^-14: subnormal half
+        const float v = std::fabs(f) * 16777216.0f;            // exact scaling by 2^24
+        return uint16_t(sign | uint32_t(std::nearbyint(v)));
+    }
+    const uint32_t mant = ax & 0x7FFFFFu, exp = (ax >> 23) - 112;
+    uint32_t h = (exp << 10) | (mant >> 13);
+    const uint32_t rest = mant & 0x1FFFu;
+    if (rest > 0x1000u || (rest == 0x1000u && (h & 1u))) ++h;
+    return uint16_t(sign | h);
+}
+
+// IEEE binary16 -> float, exact (subnormals included)
+float from_half(uint16_t h) {
+    const uint32_t sign = uint32_t(h & 0x8000u) << 16, e = (h >> 10) & 0x1F, m = h & 0x3FFu;
+    uint32_t x;
+    if (e == 0) {
+        if (m == 0) x = sign;
+        else {
+            int s = 0;
+            uint32_t mm = m;
+            while (!(mm & 0x400u)) {
+                mm <<= 1;
+                ++s;
+            }
+            x = sign | ((127 - 15 - s + 1) << 23) | ((mm & 0x3FFu) << 13);
+        }
+    } else if (e == 31) x = sign | 0x7F800000u | (m << 13);
+    else x = sign | ((e - 15 + 127) << 23) | (m << 13);
+    float f;
+    std::memcpy(&f, &x, 4);
+    return f;
+}
+
 
 class GpuVamanaIndex final : public VamanaIndex {
   public:
@@ -152,7 +216,7 @@ class GpuVamanaIndex final : public VamanaIndex {
         if (n == 0) return Status_Ok;
         if (k == 0) return Status(ErrorCode::INVALID_ARGUMENT, "k must be greater than 0");
         size_t window = 0, capacity = 0;
-        window_of(params, k, window, capacity);
+        window_of(sp_, params, k, window, capacity);
         static_assert(sizeof(size_t) == 8, "labels are 64-bit");
         if (!filter) {
             if (svsb200_search(index_, x, SVSB200_F32, n, k, window, capacity, 0, labels, 8, distances, nullptr)) return gpu_error();
@@ -176,7 +240,7 @@ class GpuVamanaIndex final : public VamanaIndex {
         if (!index_) return Status(ErrorCode::NOT_INITIALIZED, "Index not initialized");
         if (n == 0) return Status_Ok;
         size_t window = 0, capacity = 0;
-        window_of(params, 10, window, capacity);
+        window_of(sp_, params, 10, window, capacity);
         try {
             std::vector<uint32_t> counts(n);
             uint64_t* ids = nullptr;
@@ -278,59 +342,6 @@ class GpuVamanaIndex final : public VamanaIndex {
         }
         return scale_ * ip + bias_ * sum;
     }
-    void window_of(const SearchParams* params, size_t k, size_t& window, size_t& capacity) const {
-        window = is_specified(sp_.search_window_size) ? sp_.search_window_size : 10;
-        capacity = is_specified(sp_.search_buffer_capacity) ? sp_.search_buffer_capacity : 0;
-        if (params) {
-            set_if_specified(window, params->search_window_size);
-            set_if_specified(capacity, params->search_buffer_capacity);
-        }
-        window = window < k ? k : window;
-        capacity = capacity < window ? window : capacity;
-    }
-    static uint16_t to_half(float f) {   // round to nearest even, like lib/float16.h:54-79 (F16C)
-        uint32_t x;
-        std::memcpy(&x, &f, 4);
-        const uint32_t sign = (x >> 16) & 0x8000u;
-        int32_t e = int32_t((x >> 23) & 0xFF) - 127 + 15;
-        uint32_t m = x & 0x7FFFFFu;
-        if (((x >> 23) & 0xFF) == 0xFF) return uint16_t(sign | 0x7C00u | (m ? 0x200u : 0));
-        if (e >= 31) return uint16_t(sign | 0x7C00u);
-        if (e <= 0) {
-            if (e < -10) return uint16_t(sign);
-            m |= 0x800000u;
-            const uint32_t shift = uint32_t(14 - e);
-            uint32_t h = m >> shift;
-            const uint32_t rem = m & ((1u << shift) - 1), half = 1u << (shift - 1);
-            if (rem > half || (rem == half && (h & 1))) ++h;
-            return uint16_t(sign | h);
-        }
-        uint32_t h = (uint32_t(e) << 10) | (m >> 13);
-        const uint32_t rem = m & 0x1FFFu;
-        if (rem > 0x1000u || (rem == 0x1000u && (h & 1))) ++h;
-        return uint16_t(sign | h);
-    }
-    static float from_half(uint16_t h) {
-        const uint32_t sign = uint32_t(h & 0x8000u) << 16, e = (h >> 10) & 0x1F, m = h & 0x3FFu;
-        uint32_t x;
-        if (e == 0) {
-            if (m == 0) x = sign;
-            else {
-                int s = 0;
-                uint32_t mm = m;
-                while (!(mm & 0x400u)) {
-                    mm <<= 1;
-                    ++s;
-                }
-                x = sign | ((127 - 15 - s + 1) << 23) | ((mm & 0x3FFu) << 13);
-            }
-        } else if (e == 31) x = sign | 0x7F800000u | (m << 13);
-        else x = sign | ((e - 15 + 127) << 23) | (m << 13);
-        float f;
-        std::memcpy(&f, &x, 4);
-        return f;
-    }
-
     size_t dim_, n_ = 0, graph_bytes_ = 0;
     MetricType metric_;
     StorageKind kind_;
@@ -481,7 +492,7 @@ struct FilterStop {
     bool estimate = true;
 };
 
-FilterStop filter_stop_of(const IVFIndex::SearchParams& sp, const IVFIndex::SearchParams* params) {
+template <typename SearchParams> FilterStop filter_stop_of(const SearchParams& sp, const SearchParams* params) {
     FilterStop fs;
     if (is_specified(sp.filter_stop)) fs.stop = sp.filter_stop;
     if (is_specified(sp.filter_estimate_batch)) fs.estimate = sp.filter_estimate_batch.is_enabled();
@@ -589,24 +600,6 @@ class GpuIVFIndex final : public IVFIndex {
     SearchParams sp_;
     size_t threads_, intra_;
 };
-
-// float -> IEEE binary16, round to nearest even (FP16 storage)
-uint16_t to_half(float f) {
-    uint32_t x;
-    std::memcpy(&x, &f, 4);
-    const uint32_t sign = (x >> 16) & 0x8000u, ax = x & 0x7FFFFFFFu;
-    if (ax >= 0x7F800000u) return uint16_t(sign | 0x7C00u | (ax > 0x7F800000u ? 0x200u : 0u));
-    if (ax >= 0x477FF000u) return uint16_t(sign | 0x7C00u);   // rounds to >= 65520: inf
-    if (ax < 0x38800000u) {                                    // below 2^-14: subnormal half
-        const float v = std::fabs(f) * 16777216.0f;            // exact scaling by 2^24
-        return uint16_t(sign | uint32_t(std::nearbyint(v)));
-    }
-    const uint32_t mant = ax & 0x7FFFFFu, exp = (ax >> 23) - 112;
-    uint32_t h = (exp << 10) | (mant >> 13);
-    const uint32_t rest = mant & 0x1FFFu;
-    if (rest > 0x1000u || (rest == 0x1000u && (h & 1u))) ++h;
-    return uint16_t(sign | h);
-}
 
 // Clusters n rows for IVFIndex / DynamicIVFIndex::build, unspecified parameters taking the Python defaults:
 // svsb200_ivf_cluster_hierarchical when is_hierarchical is enabled (level-1 groups: hierarchical_level1_clusters, the
@@ -940,6 +933,334 @@ Status DynamicIVFIndexLeanVec::build(DynamicIVFIndex** index, size_t, MetricType
 Status DynamicIVFIndexLeanVec::build(DynamicIVFIndex** index, size_t, MetricType, StorageKind, size_t, const float*,
                                      const size_t*, const LeanVecTrainingData*, const IVFIndex::BuildParams&,
                                      const IVFIndex::SearchParams&, size_t, size_t) noexcept {
+    if (index) *index = nullptr;
+    return Status(ErrorCode::NOT_IMPLEMENTED, "LeanVec storage is not available on the GPU");
+}
+
+// ---- DynamicVamanaIndex ----
+namespace {
+
+// The graph builder's parameters of a runtime BuildParams, unspecified ones as GpuVamanaIndex::add maps them: degree 32,
+// window 200, and 0 (the library's default) for alpha, the candidate pool and prune_to.
+struct GraphParams {
+    size_t R, window, pool, prune_to;
+    float alpha;
+};
+GraphParams graph_params(const VamanaIndex::BuildParams& bp) {
+    return {is_specified(bp.graph_max_degree) ? bp.graph_max_degree : 32,
+            is_specified(bp.construction_window_size) ? bp.construction_window_size : 200,
+            is_specified(bp.max_candidate_pool_size) ? bp.max_candidate_pool_size : 0,
+            is_specified(bp.prune_to) ? bp.prune_to : 0, is_specified(bp.alpha) ? bp.alpha : 0.f};
+}
+
+class GpuDynamicVamanaIndex final : public DynamicVamanaIndex {
+  public:
+    GpuDynamicVamanaIndex(size_t dim, MetricType metric, StorageKind kind, const BuildParams& bp, const SearchParams& sp,
+                          const DynamicIndexParams& dp)
+        : dim_(dim), metric_(metric), kind_(kind), bp_(bp), sp_(sp), dp_(dp) {}
+    ~GpuDynamicVamanaIndex() override { svsb200_index_destroy(index_); }
+
+    using DynamicVamanaIndex::add;   // (add(n, x) without labels: NOT_IMPLEMENTED, as the header defines it)
+
+    // DynamicVamanaIndexImpl::add (dynamic_vamana_index_impl.h:95-102): the first add builds the index over its rows,
+    // later ones are add_points with reuse_empty = false
+    Status add(size_t n, const size_t* labels, const float* x) noexcept override {
+        if (n == 0) return Status_Ok;
+        if (!labels || !x) return Status(ErrorCode::INVALID_ARGUMENT, "null input");
+        static_assert(sizeof(size_t) == 8, "labels are 64-bit");
+        const uint64_t* ids = reinterpret_cast<const uint64_t*>(labels);
+        try {
+            if (!index_) return init(n, ids, x);
+            const void* rows = x;
+            int dtype = SVSB200_F32;   // (an SQI8 index encodes float32 rows with its fixed scale and bias)
+            std::vector<uint16_t> half;
+            if (kind_ == StorageKind::FP16) {
+                half.resize(n * dim_);
+                for (size_t i = 0; i < n * dim_; ++i) half[i] = to_half(x[i]);
+                rows = half.data();
+                dtype = SVSB200_F16;
+            }
+            if (svsb200_dynamic_add(index_, rows, dtype, n, ids, 0, nullptr)) return gpu_error();
+            return Status_Ok;
+        } catch (const std::exception& e) {
+            return Status(ErrorCode::RUNTIME_ERROR, e.what());
+        }
+    }
+
+    // DynamicVamanaIndexImpl::remove (:325-346): soft deletion, then consolidate and compact once the soft deletions
+    // exceed half of the ids left, or none is left.  An index emptied this way is released: the next add builds anew.
+    Status remove(size_t n, const size_t* labels) noexcept override {
+        if (!index_) return not_initialized();
+        if (n && !labels) return Status(ErrorCode::INVALID_ARGUMENT, "null input");
+        if (svsb200_dynamic_delete(index_, reinterpret_cast<const uint64_t*>(labels), n)) return gpu_error();
+        soft_deleted_ += n;
+        size_t left = 0;
+        if (svsb200_dynamic_ids(index_, nullptr, &left)) return gpu_error();
+        if (left == 0) return reset();   // (nothing is left to consolidate towards)
+        if (float(soft_deleted_) / float(left) > 0.5f) {
+            if (svsb200_dynamic_consolidate(index_) || svsb200_dynamic_compact(index_)) return gpu_error();
+            soft_deleted_ = 0;
+        }
+        return Status_Ok;
+    }
+    // remove_selected (:348-363): the Valid ids the selector accepts, in slot order, through remove
+    Status remove_selected(size_t* num_removed, const IDFilter& selector) noexcept override {
+        if (!index_) return not_initialized();
+        try {
+            size_t count = svsb200_index_size(index_);
+            std::vector<uint64_t> ids(count);
+            std::vector<size_t> gone;
+            if (svsb200_dynamic_ids(index_, ids.data(), &count)) return gpu_error();
+            for (size_t i = 0; i < count; ++i)
+                if (selector(size_t(ids[i]))) gone.push_back(size_t(ids[i]));
+            if (Status st = remove(gone.size(), gone.data()); !st.ok()) return st;
+            if (num_removed) *num_removed = gone.size();
+            return Status_Ok;
+        } catch (const std::exception& e) {
+            return Status(ErrorCode::RUNTIME_ERROR, e.what());
+        }
+    }
+
+    Status reset() noexcept override {
+        svsb200_index_destroy(index_);
+        index_ = nullptr;
+        soft_deleted_ = 0;
+        return Status_Ok;
+    }
+
+    Status search(size_t n, const float* x, size_t k, float* distances, size_t* labels, const SearchParams* params,
+                  IDFilter* filter) const noexcept override {
+        if (!index_) {
+            pad_rows(0, n, k, distances, labels);
+            return not_initialized();
+        }
+        if (n == 0) return Status_Ok;
+        if (k == 0) return Status(ErrorCode::INVALID_ARGUMENT, "k must be greater than 0");
+        size_t window = 0, capacity = 0;
+        window_of(sp_, params, k, window, capacity);
+        if (!filter) {
+            if (svsb200_search(index_, x, SVSB200_F32, n, k, window, capacity, 0, labels, 8, distances, nullptr))
+                return gpu_error();
+            return Status_Ok;
+        }
+        const FilterStop fs = filter_stop_of(sp_, params);
+        size_t size = 0;
+        if (svsb200_dynamic_ids(index_, nullptr, &size)) return gpu_error();
+        auto held = [this](size_t id) {
+            int out = 0;
+            return svsb200_dynamic_has_id(index_, id, &out) == 0 && out != 0;
+        };
+        if (fs.estimate && sample_says_stop(*filter, size, fs.stop, held)) {
+            pad_rows(0, n, k, distances, labels);
+            return Status_Ok;
+        }
+        try {   // IDFilter -> bitmap over the slots: bit s when slot s is Valid and its external id a member
+            const size_t slots = svsb200_index_size(index_);
+            std::vector<uint8_t> status(slots);
+            std::vector<uint64_t> ext(slots);
+            if (svsb200_dynamic_export(index_, nullptr, status.data(), ext.data(), nullptr)) return gpu_error();
+            std::vector<uint32_t> bitmap((slots + 31) / 32, 0u);
+            for (size_t s = 0; s < slots; ++s)
+                if (status[s] == 1 && filter->is_member(size_t(ext[s]))) bitmap[s >> 5] |= 1u << (s & 31);
+            if (svsb200_search_filtered(index_, x, SVSB200_F32, n, k, window, bitmap.data(), reinterpret_cast<uint64_t*>(labels),
+                                        distances, nullptr))
+                return gpu_error();
+        } catch (const std::exception& e) {
+            return Status(ErrorCode::RUNTIME_ERROR, e.what());
+        }
+        return Status_Ok;
+    }
+
+    // range_search (:222-323): the search's results inside the radius, then the filter, as the static class applies it
+    Status range_search(size_t n, const float* x, float radius, const ResultsAllocator& results, const SearchParams* params,
+                        IDFilter* filter) const noexcept override {
+        if (!index_) return not_initialized();
+        if (radius <= 0) return Status(ErrorCode::INVALID_ARGUMENT, "radius must be greater than 0");
+        if (n == 0) return Status_Ok;
+        size_t window = 0, capacity = 0;
+        window_of(sp_, params, 10, window, capacity);
+        try {
+            std::vector<uint32_t> counts(n);
+            uint64_t* ids = nullptr;
+            float* dd = nullptr;
+            if (svsb200_range_search(index_, x, SVSB200_F32, n, radius, window, counts.data(), &ids, &dd)) return gpu_error();
+            std::unique_ptr<uint64_t, void (*)(void*)> ids_guard(ids, svsb200_free);
+            std::unique_ptr<float, void (*)(void*)> dd_guard(dd, svsb200_free);
+            std::vector<size_t> kept(n, 0), offs(n + 1, 0);
+            for (size_t q = 0; q < n; ++q) offs[q + 1] = offs[q] + counts[q];
+            for (size_t q = 0; q < n; ++q)
+                for (size_t j = offs[q]; j < offs[q + 1]; ++j)
+                    if (!filter || filter->is_member(ids[j])) ++kept[q];
+            SearchResultsStorage out = results.allocate(std::span<size_t>(kept.data(), kept.size()));
+            size_t o = 0;
+            for (size_t q = 0; q < n; ++q)
+                for (size_t j = offs[q]; j < offs[q + 1]; ++j)
+                    if (!filter || filter->is_member(ids[j])) {
+                        out.labels[o] = ids[j];
+                        out.distances[o] = dd[j];
+                        ++o;
+                    }
+        } catch (const std::exception& e) {
+            return Status(ErrorCode::RUNTIME_ERROR, e.what());
+        }
+        return Status_Ok;
+    }
+
+    // MutableVamanaIndex::get_distance / reconstruct_at on the device; an id the index does not hold is the reference's
+    // ANNEXCEPTION, a RUNTIME_ERROR through runtime_error_wrapper
+    Status get_distance(size_t id, const float* query, float* distance) const noexcept override {
+        if (!index_) return not_initialized();
+        const uint64_t ext = id;
+        if (svsb200_index_distances(index_, query, SVSB200_F32, 1, &ext, distance)) return gpu_error();
+        return Status_Ok;
+    }
+    Status reconstruct_at(size_t n, const size_t* ids, float* output) noexcept override {
+        if (!index_) return not_initialized();
+        if (svsb200_index_reconstruct(index_, reinterpret_cast<const uint64_t*>(ids), n, output)) return gpu_error();
+        return Status_Ok;
+    }
+
+    size_t get_memory_usage() const noexcept override { return index_ ? svsb200_index_device_bytes(index_) : 0; }
+    // The device bytes per slot: the row (16-byte aligned), the adjacency row (padded to whole 32-word groups) and its
+    // 16-bit length, and the status byte and 64-bit external id.  The slots counted are the capacity the arrays hold.
+    Status get_memory_breakdown(MemoryBreakdown* out) const noexcept override {
+        if (!out) return Status(ErrorCode::INVALID_ARGUMENT, "memory breakdown output must not be null");
+        *out = MemoryBreakdown{};
+        if (!index_) return Status_Ok;
+        const size_t total = svsb200_index_device_bytes(index_);
+        const size_t elem = kind_ == StorageKind::FP32 ? 4 : kind_ == StorageKind::FP16 ? 2 : 1;
+        const size_t row = (dim_ * elem + 15) / 16 * 16;
+        const size_t R = svsb200_index_max_degree(index_);
+        const size_t adjacency = (R + 31) / 32 * 32 * 4 + 2, meta = 1 + 8;
+        const size_t cap = total / (row + adjacency + meta);
+        out->data_bytes = cap * row;
+        out->metadata_bytes = cap * meta;
+        out->graph_bytes = total - out->data_bytes - out->metadata_bytes;
+        return Status_Ok;
+    }
+    size_t blocksize_bytes() const noexcept override { return 1u << dp_.blocksize_exp; }
+
+    Status save(std::ostream&) const noexcept override {
+        return Status(ErrorCode::NOT_IMPLEMENTED, "save stays on the reference's CPU index (index/vamana/dynamic_index.h)");
+    }
+
+  private:
+    static Status not_initialized() { return Status(ErrorCode::NOT_INITIALIZED, "Index not initialized"); }
+
+    // The first add: the graph over its rows (svsb200_dynamic_build / _build_sq).  The builder needs two rows, so a
+    // one-row index is assembled with an adjacency row of degree 0 and the build parameters as mutation parameters.
+    Status init(size_t n, const uint64_t* ids, const float* x) {
+        const GraphParams g = graph_params(bp_);
+        const int metric = metric_ == MetricType::L2 ? SVSB200_L2 : SVSB200_IP;
+        std::vector<uint32_t> graph(g.R + 1, 0u);   // (one row: degree 0)
+        svsb200_index* h = nullptr;
+        int rc = 0;
+        if (kind_ == StorageKind::SQI8) {   // int8 codes with one global scale and bias, as the static class compresses
+            std::vector<int8_t> codes(n * dim_);
+            float sq[2] = {0.f, 0.f};
+            if (svsb200_sq_compress(x, n, dim_, SVSB200_I8, 0, codes.data(), &sq[0], &sq[1])) return gpu_error();
+            rc = n == 1 ? svsb200_dynamic_create_sq(codes.data(), SVSB200_I8, 1, dim_, sq[0], sq[1], graph.data(), g.R + 1, 0,
+                                                    metric, ids, 0, &h)
+                        : svsb200_dynamic_build_sq(codes.data(), SVSB200_I8, n, dim_, metric, sq[0], sq[1], g.alpha, g.R,
+                                                   g.window, g.pool, g.prune_to, ids, 0, &h);
+        } else {
+            const void* rows = x;
+            int dtype = SVSB200_F32;
+            std::vector<uint16_t> half;
+            if (kind_ == StorageKind::FP16) {
+                half.resize(n * dim_);
+                for (size_t i = 0; i < n * dim_; ++i) half[i] = to_half(x[i]);
+                rows = half.data();
+                dtype = SVSB200_F16;
+            }
+            rc = n == 1 ? svsb200_dynamic_create(rows, dtype, 1, dim_, graph.data(), g.R + 1, 0, metric, ids, 0, &h)
+                        : svsb200_dynamic_build(rows, dtype, n, dim_, metric, g.alpha, g.R, g.window, g.pool, g.prune_to, ids,
+                                                0, &h);
+        }
+        if (rc == 0 && n == 1) rc = svsb200_dynamic_set_build_parameters(h, g.alpha, g.window, g.pool, g.prune_to);
+        if (rc) {
+            const Status st = gpu_error();
+            svsb200_index_destroy(h);
+            return st;
+        }
+        index_ = h;
+        soft_deleted_ = 0;
+        return Status_Ok;
+    }
+
+    size_t dim_;
+    MetricType metric_;
+    StorageKind kind_;
+    BuildParams bp_;
+    SearchParams sp_;
+    DynamicIndexParams dp_;
+    svsb200_index* index_ = nullptr;
+    size_t soft_deleted_ = 0;   // ntotal_soft_deleted
+};
+
+}  // namespace
+
+Status DynamicVamanaIndex::check_storage_kind(StorageKind kind) noexcept {
+    return kind == StorageKind::FP32 || kind == StorageKind::FP16 || kind == StorageKind::SQI8
+               ? Status_Ok
+               : Status(ErrorCode::NOT_IMPLEMENTED, "DynamicVamanaIndex on the GPU supports FP32, FP16 and SQI8 storage only");
+}
+
+// dynamic_vamana_index.cpp: the block size of the reference's blocked storage, 2^12 to 2^30 bytes
+Status DynamicVamanaIndex::check_params(const VamanaIndex::DynamicIndexParams& dynamic_index_params) noexcept {
+    if (dynamic_index_params.blocksize_exp > 30) return Status(ErrorCode::INVALID_ARGUMENT, "Blocksize is too large");
+    if (dynamic_index_params.blocksize_exp < 12) return Status(ErrorCode::INVALID_ARGUMENT, "Blocksize is too small");
+    return Status_Ok;
+}
+
+Status DynamicVamanaIndex::build(DynamicVamanaIndex** index, size_t dim, MetricType metric, StorageKind storage_kind,
+                                 const VamanaIndex::BuildParams& params,
+                                 const VamanaIndex::SearchParams& default_search_params) noexcept {
+    return build(index, dim, metric, storage_kind, params, default_search_params, VamanaIndex::DynamicIndexParams{});
+}
+
+Status DynamicVamanaIndex::build(DynamicVamanaIndex** index, size_t dim, MetricType metric, StorageKind storage_kind,
+                                 const VamanaIndex::BuildParams& params, const VamanaIndex::SearchParams& default_search_params,
+                                 const VamanaIndex::DynamicIndexParams& dynamic_index_params) noexcept {
+    if (!index) return Status(ErrorCode::INVALID_ARGUMENT, "null output");
+    *index = nullptr;
+    if (Status st = check_storage_kind(storage_kind); !st.ok()) return st;
+    if (Status st = check_params(dynamic_index_params); !st.ok()) return st;
+    if (dim == 0) return Status(ErrorCode::INVALID_ARGUMENT, "dim must be positive");
+    *index = new (std::nothrow) GpuDynamicVamanaIndex(dim, metric, storage_kind, params, default_search_params,
+                                                      dynamic_index_params);
+    return *index ? Status_Ok : Status(ErrorCode::RUNTIME_ERROR, "out of memory");
+}
+
+Status DynamicVamanaIndex::destroy(DynamicVamanaIndex* index) noexcept {
+    delete index;
+    return Status_Ok;
+}
+
+Status DynamicVamanaIndex::load(DynamicVamanaIndex** index, std::istream&, MetricType, StorageKind) noexcept {
+    if (index) *index = nullptr;
+    return Status(ErrorCode::NOT_IMPLEMENTED, "load stays on the reference's CPU library");
+}
+
+Status DynamicVamanaIndexLeanVec::build(DynamicVamanaIndex** index, size_t, MetricType, StorageKind, size_t,
+                                        const VamanaIndex::BuildParams&, const VamanaIndex::SearchParams&) noexcept {
+    if (index) *index = nullptr;
+    return Status(ErrorCode::NOT_IMPLEMENTED, "LeanVec storage is not available on the GPU");
+}
+Status DynamicVamanaIndexLeanVec::build(DynamicVamanaIndex** index, size_t, MetricType, StorageKind, size_t,
+                                        const VamanaIndex::BuildParams&, const VamanaIndex::SearchParams&,
+                                        const VamanaIndex::DynamicIndexParams&) noexcept {
+    if (index) *index = nullptr;
+    return Status(ErrorCode::NOT_IMPLEMENTED, "LeanVec storage is not available on the GPU");
+}
+Status DynamicVamanaIndexLeanVec::build(DynamicVamanaIndex** index, size_t, MetricType, StorageKind, const LeanVecTrainingData*,
+                                        const VamanaIndex::BuildParams&, const VamanaIndex::SearchParams&) noexcept {
+    if (index) *index = nullptr;
+    return Status(ErrorCode::NOT_IMPLEMENTED, "LeanVec storage is not available on the GPU");
+}
+Status DynamicVamanaIndexLeanVec::build(DynamicVamanaIndex** index, size_t, MetricType, StorageKind, const LeanVecTrainingData*,
+                                        const VamanaIndex::BuildParams&, const VamanaIndex::SearchParams&,
+                                        const VamanaIndex::DynamicIndexParams&) noexcept {
     if (index) *index = nullptr;
     return Status(ErrorCode::NOT_IMPLEMENTED, "LeanVec storage is not available on the GPU");
 }

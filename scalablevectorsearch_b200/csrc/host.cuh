@@ -138,6 +138,7 @@ struct Scratch {
     DeviceBuffer<uint64_t> stage_ids;
     DeviceBuffer<float> stage_dists;
     DeviceBuffer<uint32_t> dyn_ovf, dyn_qlist;        // dynamic search: overflowed queries, the list being re-run
+    DeviceBuffer<uint32_t> point_rows;                 // svsb200_index_distances / _reconstruct: the rows named
     bool dyn_slot_ids = false;                         // dynamic search: write slots, not external ids (filtered / range)
     int (*cancel_fn)(void*) = nullptr;                 // the caller's cancellation predicate while a search runs
     void* cancel_arg = nullptr;
@@ -416,6 +417,9 @@ enum PrepMode : int {
 // (query_stride(dim) apart) and sc->q_aux, enqueued on `stream`.
 int prepare_queries(const svsb200_index* ix, const Replica* rep, Scratch* sc, const void* d_queries, int qdtype, size_t nq,
                     int mode, cudaStream_t stream);
+// The search's distance operator (Op) and query preparation (PrepMode) for `qdtype` queries on this index; fails for a
+// query type its search refuses (search.cu).
+int choose_op(const svsb200_index* ix, int qdtype, int* op, int* mode);
 
 // Shared body of every graph-search entry point: everything on one device, enqueued on `stream`.  `exhaustive`
 // scans every base row instead of walking the graph; with `row_status` (one byte per row, the filtered flat search's)

@@ -265,7 +265,7 @@ static void balance(size_t n, size_t parts, size_t i, size_t* lo, size_t* hi) {
 
 // Which (query, data) pairs exist, mirroring the SIMD specialisations (euclidean.h:293-358) and the SQ CPOs
 // (extensions/vamana/scalar.h:32-43): the distance operator and the query preparation for them.
-static int choose_op(const svsb200_index* ix, int qdtype, int* op, int* mode) {
+int choose_op(const svsb200_index* ix, int qdtype, int* op, int* mode) {
     const int metric = ix->metric;
     if (ix->storage == SVSB200_LVQ8) {
         if (qdtype != SVSB200_F32 && qdtype != SVSB200_F16) return fail("LVQ-8 datasets take float32/float16 queries");

@@ -374,6 +374,32 @@ class Vamana(_lib._Handle):
         offs = np.concatenate([[0], np.cumsum(counts.astype(np.int64))])
         return [(ids[offs[i]:offs[i + 1]], dd[offs[i]:offs[i + 1]]) for i in range(nq)]
 
+    # ---- stored rows (bindings/python/include/svs/python/vamana.h:217, manager.h:141) --------------------------
+    def get_distance(self, external_id: int, query_vector: np.ndarray) -> float:
+        """``svs.Vamana.get_distance(external_id, query_vector)``: the distance the search computes between the query
+        (a 1-D array of the index's dimension; float32 unless it already has a query type the search takes) and the
+        stored row that a search returns as ``external_id``."""
+        q = np.asarray(query_vector)
+        if q.dtype not in _DTYPE_CODE:
+            q = q.astype(np.float32)
+        q = np.ascontiguousarray(q.reshape(-1))
+        if q.shape[0] != self.dimensions:
+            raise ValueError(f"Incompatible dimensions. Query has {q.shape[0]} while the index expects {self.dimensions}.")
+        ids = np.array([int(external_id)], dtype=np.uint64)
+        out = np.empty(1, dtype=np.float32)
+        _lib.check(self._lib.svsb200_index_distances(self._h, q.ctypes.data, _DTYPE_CODE[q.dtype], 1, ids.ctypes.data,
+                                                     out.ctypes.data))
+        return float(out[0])
+
+    def reconstruct(self, ids) -> np.ndarray:
+        """``svs.Vamana.reconstruct(ids)``: the stored rows named by ``ids`` (any shape) as float32, shaped
+        ``ids.shape + (dimensions,)``; SQ codes come back decompressed (scale * c + bias)."""
+        ids = np.asarray(ids, dtype=np.uint64)
+        flat = np.ascontiguousarray(ids.reshape(-1))
+        out = np.empty((flat.shape[0], self.dimensions), dtype=np.float32)
+        _lib.check(self._lib.svsb200_index_reconstruct(self._h, flat.ctypes.data, flat.shape[0], out.ctypes.data))
+        return out.reshape(ids.shape + (self.dimensions,))
+
     def flat_search(self, queries: np.ndarray, n_neighbors: int):
         """Exact top-k of every query over ALL base vectors -- what ``svs.Flat(...).search`` computes
         (index/flat/flat.h:421-465) -- on the tensor cores, with the graph search's bit-exact distances
